@@ -2,6 +2,7 @@
 """bench.py — train-step ray-samples/s of the NoPe-NeRF hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--engine tc|simt] [--scaling weak|strong]
+                    [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1], SURVEY.md 8(d) "C2"): Ignatius-shape scene, 1080x1920 frames,
 V=200 poses, 1024 rays x 128 samples per step, uniform sampling + stratified jitter, softplus
@@ -11,19 +12,24 @@ Trainer.train_step: pose exp-map, ray generation, sampling, encoding, 8x256 MLP,
 full backward (MLP + pose + depth-distortion gradients), [all-reduce], optimizer steps.
 
   value : whole-job ray-samples/s over EXACTLY K timed steps with the frame + DPT map already resident in HBM (after W warm-up
-          steps and ~1 s of untimed steps that let clocks and power settle).  `sustained` repeats the measurement over 1000 steps.
+          steps and SETTLE_STEPS untimed steps that let clocks and power settle).  Every other timed window is K steps too.
   e2e   : same step through the reference-facing API with HOST (page-locked) frame tensors, as train.py's DataLoader
           (pin_memory=True) hands them over: host->device traffic (DPT map copy + in-place gather of the sampled
           pixels over PCIe) and the D2H read of the loss every step (train.py:212) are inside the timed region.
   full_loss / c3 / fwd_only / reference_cuda (N = 1): the full default loss set (point-cloud chamfer + warped RGB, training.py:280-365),
           the LLFF-shape NDC + dist_alpha configuration, one 1/8 row block of a 1080p novel view (config 4), and the UNMODIFIED
-          reference's Trainer.train_step on the same GPU (oracle/_ref, tools/vendor_ref.py).
+          reference's Trainer.train_step on the same GPU (oracle/_ref, made by build() where the reference tree exists).
   N > 1 : weak scaling — every GPU keeps the C2 per-GPU work (1024 rays x 128 samples): the step draws a global batch of
           1024*N rays, sharded rank::N (Trainer dp_mode='rays'), ONE NCCL all-reduce of the flat [gradients | loss]
           buffer per step; value = all ranks' ray-samples / max-over-ranks time.  A `strong` record (the fixed 1024-ray batch
           split over the GPUs) is added to the same line.
   --impl reference : the UNMODIFIED reference's Trainer.train_step (oracle/_ref) on the host cores, full 1024 x 128 batch on the
           same synthetic C2 data, all host threads (rank 0 only under torchrun).
+  --dump-outputs DIR : after the headline window, a second trainer built from the same seeds runs the same timed path (W warm-up
+          + K steps on the same frames); the outputs of its last step go to DIR/<name>.npy (float32 / float64): the loss terms the
+          step returned and every parameter it updated (MLP, poses, distortions).  Inputs, seeds and step counts are fixed by the
+          arguments, and every reduction of the step runs in a fixed order (no float atomics), so two runs of one build write the
+          same bits and two builds can be compared output for output.
 """
 import argparse
 import json
@@ -41,23 +47,9 @@ H, W, HD, WD, V, NRAYS, S = 1080, 1920, 384, 672, 200, 1024, 128
 N_FRAMES = 8                      # distinct synthetic frames cycled through (each 24.9 MB + 1 MB DPT map)
 FLOP_PER_SAMPLE_STEP = 3560448    # fwd + dgrad + wgrad (BASELINE.md section 2)
 FLOP_PER_SAMPLE_FWD = 1186816
-# dram__bytes_read.sum + dram__bytes_write.sum per launch at 1024 x 128 samples, from the committed `ncu --set full` capture
-NCU_DRAM_FILE = os.path.join(ROOT, "profiles", "ncu_dram_bytes.json")
-NCU_DRAM_BYTES_R1 = {"field_fwd": 1.451e9, "dgrad": 1.335e9, "wgrad": 2.686e9, "source": "profiles/ncu_r1_final_tc_kernels_summary.txt"}
-
-
-def ncu_dram_bytes():
-    if os.path.exists(NCU_DRAM_FILE):
-        return json.load(open(NCU_DRAM_FILE))
-    return dict(NCU_DRAM_BYTES_R1)
-
-
-def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(tflops=d["bf16_tflops"], tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), hbm=d.get("hbm_gbs"), source="measured")
-    return dict(tflops=1590.0, tflops_sustained=1400.0, hbm=6500.0, source="fallback")
+SETTLE_STEPS = 300                # untimed steps before the headline window (about 2 s at 8 ms per step: clocks and power settle)
+# H100 SXM data sheet, dense FP16 / BF16 tensor rate and HBM3 bandwidth at the 700 W limit: a ceiling, not a measured rate
+PEAK = dict(tflops=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet (dense fp16, 700 W); see clocks for this card's limit")
 
 
 class ClockSampler:
@@ -165,14 +157,8 @@ def run_ours(args):
     dev = torch.device("cuda", local)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    import __graft_entry__ as ge
-    if rank == 0:
-        ge.build()
-    if world > 1:
-        dist.barrier()
-    from nope_nerf_b200 import ops, _lib as L
+    from nope_nerf_b200 import ops, _lib as L         # the library build() made; this script writes nothing into the tree
     ops.set_default_engine(args.engine)
-    WG_DEFAULT = ops.wgrad_precision()
     weak = args.scaling == "weak"
     n_local = NRAYS if weak else NRAYS // world
     trainer = build_trainer(make_cfg(n_local * world), dev, V)
@@ -186,16 +172,10 @@ def run_ours(args):
             dist.barrier()
         torch.cuda.synchronize()
 
-    def timed(tr, datas, K, Wm, sync_loss, settle_s=0.0):
-        for i in range(Wm):
+    def timed(tr, datas, K, Wm, sync_loss, settle=0):
+        for i in range(Wm + settle):                        # warm-up, then untimed steps while clocks / power settle
             ld = step(tr, datas[i % len(datas)], i)
-            if sync_loss: ld["loss"].item()
-        if settle_s > 0:                                    # untimed steps until clocks / power have settled
-            torch.cuda.synchronize(); t0 = time.perf_counter(); i = Wm
-            while time.perf_counter() - t0 < settle_s:
-                for _ in range(50):
-                    step(tr, datas[i % len(datas)], i); i += 1
-                torch.cuda.synchronize()
+            if sync_loss and i < Wm: ld["loss"].item()
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -239,22 +219,30 @@ def run_ours(args):
     # ---- headline: device-resident inputs, EXACTLY K timed steps after warm-up + settling ----
     cs = ClockSampler(local) if rank == 0 else None
     ms_burst, _ = timed(trainer, devd, K, Wm, sync_loss=False)               # right after warm-up: boost clocks (round-1 methodology)
-    ms, ld = timed(trainer, devd, K, 0, sync_loss=False, settle_s=1.0)        # headline: after ~1 s of untimed steps (power-capped regime)
-    ms_sus, _ = timed(trainer, devd, 1000, 0, sync_loss=False)
+    ms, ld = timed(trainer, devd, K, 0, sync_loss=False, settle=SETTLE_STEPS)  # headline: after the untimed settling steps
+    if args.dump_outputs:
+        # a second trainer from the same seeds runs the same timed path (W warm-up + K steps on the same frames): the dumped step
+        # is W + K steps from a fixed start, so rounding differences between builds have had few Adam steps to grow
+        tr_d = build_trainer(make_cfg(n_local * world), dev, V)
+        _, ld_d = timed(tr_d, devd, K, Wm, sync_loss=False)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, tr_d, ld_d)
+        del tr_d
+    ms_sus, _ = timed(trainer, devd, K, 0, sync_loss=False)
     clocks = cs.stop() if cs else {}
     launches = trainer.graph_kernel_nodes()
     # ---- e2e: host (pinned) frames, H2D inside the step, loss read back every step ----
     ms_e2e, _ = timed(trainer, host, K, max(Wm, N_FRAMES), sync_loss=True)   # warm-up touches every page-locked frame once (first-touch mapping)
-    ms_e2e_sus, _ = timed(trainer, host, 300, 0, sync_loss=True)
-    ms_dev_item, _ = timed(trainer, devd, 300, 0, sync_loss=True)           # breakdown: loss read-back alone
-    ms_host_noitem, _ = timed(trainer, host, 300, 0, sync_loss=False)       # breakdown: host frames alone
+    ms_e2e_sus, _ = timed(trainer, host, K, 0, sync_loss=True)
+    ms_dev_item, _ = timed(trainer, devd, K, 0, sync_loss=True)             # breakdown: loss read-back alone
+    ms_host_noitem, _ = timed(trainer, host, K, 0, sync_loss=False)         # breakdown: host frames alone
     extra = {}
     if world > 1 and weak:
         # strong scaling of the SAME 1024-ray batch (north_star): second trainer, rays split rank::world
         tr_s = build_trainer(make_cfg(NRAYS), dev, V)
-        ms_s, _ = timed(tr_s, devd, 300, 5, sync_loss=False)
-        extra["strong"] = {"value": round(NRAYS * S * 300 / (ms_s / 1e3), 1), "unit": "ray-samples/s", "ms_per_step": round(ms_s / 300, 4),
-                           "global_rays": NRAYS, "rays_per_gpu": NRAYS // world, "steps": 300}
+        ms_s, _ = timed(tr_s, devd, K, 5, sync_loss=False)
+        extra["strong"] = {"value": round(NRAYS * S * K / (ms_s / 1e3), 1), "unit": "ray-samples/s", "ms_per_step": round(ms_s / K, 4),
+                           "global_rays": NRAYS, "rays_per_gpu": NRAYS // world, "steps": K}
         del tr_s
     if world > 1 and weak:
         # C5 (BASELINE.json configs[4]): 4096 rays x 128 samples over the GPUs, one view per rank, full default loss set, one exchange
@@ -262,23 +250,15 @@ def run_ours(args):
         tr_c = build_trainer(ops_c5, dev, V, dp_mode="views")
         hostf, devf = synth_frames(H, W, HD, WD, 2 * world, V, dev, with_ref=True)
         mine = [devf[(2 * k + rank) % len(devf)] for k in range(2)]
-        ms_c, ldc = timed(tr_c, mine, 200, 5, sync_loss=False)
-        extra["c5"] = {"value": round(4096 * S * 200 / (ms_c / 1e3), 1), "unit": "ray-samples/s", "ms_per_step": round(ms_c / 200, 4), "global_rays": 4096,
-                       "rays_per_gpu": 4096 // world, "steps": 200,
+        ms_c, ldc = timed(tr_c, mine, K, 5, sync_loss=False)
+        extra["c5"] = {"value": round(4096 * S * K / (ms_c / 1e3), 1), "unit": "ray-samples/s", "ms_per_step": round(ms_c / K, 4), "global_rays": 4096,
+                       "rays_per_gpu": 4096 // world, "steps": K,
                        "workload": "C5: 4096 rays x 128 samples, dp_mode='views' (one view per rank), rgb + depth + point-cloud + warped-RGB losses"}
         del tr_c, hostf, devf
     if world == 1:
         extra.update(single_gpu_records(dev, step, timed, args))
-        # the same step with the exact (bf16 hi|lo, three MMAs per product) weight-gradient planes
-        ops.set_wgrad_precision("exact")
-        tr_x = build_trainer(make_cfg(NRAYS), dev, V)
-        ms_x, _ = timed(tr_x, devd, 300, 5, sync_loss=False)
-        ops.set_wgrad_precision(WG_DEFAULT)
-        extra["exact_wgrad_planes"] = {"ms_per_step": round(ms_x / 300, 4), "value": round(NRAYS * S * 300 / (ms_x / 1e3), 1), "steps": 300,
-                                       "note": "NNB_WGRAD=exact: MLP weight gradients to fp32 round-off (bf16 hi|lo planes) instead of fp16 operand rounding"}
-        del tr_x
     if rank == 0:
-        pk = peaks()
+        pk = PEAK
         samples_per_step = n_local * world * S
         value = samples_per_step * K / (ms / 1e3)
         e2e = samples_per_step * K / (ms_e2e / 1e3)
@@ -286,36 +266,32 @@ def run_ours(args):
         flops = {"field_fwd": FLOP_PER_SAMPLE_FWD, "dgrad": FLOP_PER_SAMPLE_FWD, "wgrad": FLOP_PER_SAMPLE_FWD}
         dom = max((k for k in prof if k in flops), key=lambda k: prof[k]) if prof else None
         roof = None
-        dram = ncu_dram_bytes()
         if dom:
             ach = flops[dom] * (n_local * S) / (prof[dom] / 1e3) / 1e12
             roof = {"bound": "tensor", "kernel": dom, "achieved": round(ach, 2), "peak": pk["tflops"], "unit": "TFLOP/s",
-                    "frac": round(ach / pk["tflops"], 4), "frac_of_sustained_peak": round(ach / pk["tflops_sustained"], 4),
-                    "traffic": dram.get(dom) if (n_local == NRAYS and args.engine == "tc") else None,
-                    "traffic_source": dram.get("source"), "peak_source": pk["source"] + " (burst bf16 cuBLAS: the profiled kernels run at "
-                    "the boost clock, see clocks)", "algorithmic_flop_per_launch": flops[dom] * n_local * S,
+                    "frac": round(ach / pk["tflops"], 4), "peak_source": pk["source"], "algorithmic_flop_per_launch": flops[dom] * n_local * S,
                     "kernel_ms": {k: round(v, 4) for k, v in prof.items()},
-                    "step_algorithmic_tflops": round(FLOP_PER_SAMPLE_STEP * n_local * S / (ms_sus / 1000 / 1e3) / 1e12, 1),
-                    "note": "algorithmic fp32-equivalent FLOPs; the tcgen05 engine issues split 16-bit MMAs per logical product"}
+                    "step_algorithmic_tflops": round(FLOP_PER_SAMPLE_STEP * n_local * S / (ms_sus / K / 1e3) / 1e12, 1),
+                    "note": "algorithmic fp32-equivalent FLOPs; the tensor-core forward issues three split-fp16 wgmma per logical product"}
         line = {"metric": "train-step ray-samples/sec", "value": round(value, 1), "unit": "ray-samples/s", "n_gpus": world, "steps": K,
                 "warmup": Wm, "ms_per_step": round(ms / K, 4), "higher_is_better": True, "scaling": "weak" if weak else "strong", "vs_baseline": None,
-                "dtype": ("fp32 (forward / data gradients: split fp16|bf16 hi+lo tcgen05 MMAs, fp32 accumulate; weight gradients: %s)" %
-                          ("one fp16 plane per operand, NNB_WG16" if ops.wgrad_precision() == "fp16" else "bf16 hi+lo planes")) if args.engine == "tc" else "fp32",
+                "dtype": "fp32 (split fp16 hi+lo wgmma forward, split bf16 hi+lo wgmma backward, fp32 accumulate)" if args.engine == "tc" else "fp32",
                 "data": "synthetic",
                 "config": {"workload": "C2 Ignatius-shape 1080x1920, V=200, 1024 rays x 128 samples, uniform+jitter, rgb L1 + depth L1, Adam x3",
                            "global_rays": n_local * world, "rays_per_gpu": n_local, "samples_per_ray": S,
                            "parallelism": "dp%d (ray shards, 1 all-reduce)" % world,
-                           "engine": args.engine, "wgrad_planes": ops.wgrad_precision(), "frames_resident": N_FRAMES, "cuda_graph": bool(trainer.use_cuda_graph),
-                           "l2_policy": "no flush: each step streams a >1 GB activation stash, far larger than the 126 MB L2",
-                           "settle": "W warm-up steps + ~1 s of untimed steps before the K timed steps"},
-                "sustained": {"steps": 1000, "ms_per_step": round(ms_sus / 1000, 4), "value": round(samples_per_step * 1000 / (ms_sus / 1e3), 1)},
+                           "engine": args.engine, "frames_resident": N_FRAMES, "cuda_graph": bool(trainer.use_cuda_graph),
+                           "l2_policy": "no flush: each step streams a >1 GB activation stash, far larger than the 50 MB L2",
+                           "settle": "W warm-up steps + %d untimed steps before the K timed steps" % SETTLE_STEPS},
+                "sustained": {"steps": K, "ms_per_step": round(ms_sus / K, 4), "value": round(samples_per_step * K / (ms_sus / 1e3), 1),
+                              "note": "the next K steps, right after the headline window"},
                 "burst": {"steps": K, "ms_per_step": round(ms_burst / K, 4), "value": round(samples_per_step * K / (ms_burst / 1e3), 1),
                           "note": "K steps timed right after the W warm-up steps, before clocks / power settle (how round 1 measured)"},
                 "e2e": {"value": round(e2e, 1), "unit": "ray-samples/s", "ms_per_step": round(ms_e2e / K, 4),
                         "h2d_bytes_per_step": int(n_local * 3 * 32 + HD * WD * 4 + 64 + 16) * world, "d2h_bytes_per_step": 4 * world,
-                        "sustained_ms_per_step": round(ms_e2e_sus / 300, 4),
-                        "breakdown_ms_per_step": {"device_frames_no_readback": round(ms_sus / 1000, 4), "device_frames_loss_item": round(ms_dev_item / 300, 4),
-                                                  "host_frames_no_readback": round(ms_host_noitem / 300, 4), "host_frames_loss_item": round(ms_e2e_sus / 300, 4)},
+                        "sustained_ms_per_step": round(ms_e2e_sus / K, 4),
+                        "breakdown_ms_per_step": {"device_frames_no_readback": round(ms_sus / K, 4), "device_frames_loss_item": round(ms_dev_item / K, 4),
+                                                  "host_frames_no_readback": round(ms_host_noitem / K, 4), "host_frames_loss_item": round(ms_e2e_sus / K, 4)},
                         "h2d_note": "host frames are page-locked: the loss kernel gathers the 1024x3 sampled pixels in place over PCIe "
                                     "(one 32-B sector each) instead of copying the 24.9 MB frame; the 1 MB DPT map, camera_mat and idx are copied"},
                 "gpu_launches": (launches["kernels"] if launches else 22) * K * world,
@@ -339,7 +315,8 @@ def single_gpu_records(dev, step, timed, args):
     # ---- full loss set: point-cloud chamfer (P = 96 x 168 = 16 128) + warped-RGB terms, training.py:280-365 ----
     tr_f = build_trainer(make_cfg(NRAYS, full_loss=True), dev, V)
     hostf, devf = synth_frames(H, W, HD, WD, 4, V, dev, with_ref=True)
-    ms_f, ld = timed(tr_f, devf, 300, 5, sync_loss=False)
+    K = args.steps
+    ms_f, ld = timed(tr_f, devf, K, 5, sync_loss=False)
     P = (HD // 4) * (WD // 4)
     X = torch.randn(P, 3, device=dev); Y = torch.randn(P, 3, device=dev) + 0.05
     keys = torch.empty(2 * P, dtype=torch.int64, device=dev); loss = torch.zeros(1, device=dev)
@@ -352,18 +329,18 @@ def single_gpu_records(dev, step, timed, args):
     for _ in range(20): L.lib.nnb_chamfer(L.ptr(X), P, L.ptr(Y), P, L.ptr(keys), None, None, L.ptr(loss), 1.0, None, None, st)
     e1.record(); torch.cuda.synchronize()
     ch_ms = e0.elapsed_time(e1) / 20
-    out["full_loss"] = {"ms_per_step": round(ms_f / 300, 4), "value": round(NRAYS * S * 300 / (ms_f / 1e3), 1), "steps": 300,
+    out["full_loss"] = {"ms_per_step": round(ms_f / K, 4), "value": round(NRAYS * S * K / (ms_f / 1e3), 1), "steps": K,
                         "loss_pc": float(ld["loss_pc"]), "loss_rgb_s": float(ld["loss_rgb_s"]), "points_per_cloud": P,
                         "chamfer_ms": round(ch_ms, 4), "chamfer_pairs_per_s": round(2.0 * P * P / (ch_ms / 1e3), 1),
-                        "chamfer_note": "brute force, both directions in one launch: 2*P*P fp32 pair distances (SIMT, packed fp32x2)",
+                        "chamfer_note": "brute force, both directions in one launch: 2*P*P fp32 pair distances (SIMT)",
                         "workload": "C2 + pc_weight = rgb_s_weight = 1 (configs/default.yaml:95-101 before annealing), captured in the same CUDA graph"}
     del tr_f, hostf, devf
     torch.cuda.empty_cache()
     # ---- C3: LLFF fern shape, NDC + dist_alpha, depth loss on 1 - 1/d ----
     tr_c = build_trainer(make_cfg(NRAYS, c3=True), dev, 20)
     _, devc = synth_frames(756, 1008, 384, 512, 4, 20, dev, with_ref=False)
-    ms_c, _ = timed(tr_c, devc, 300, 5, sync_loss=False)
-    out["c3"] = {"ms_per_step": round(ms_c / 300, 4), "value": round(NRAYS * S * 300 / (ms_c / 1e3), 1), "steps": 300,
+    ms_c, _ = timed(tr_c, devc, K, 5, sync_loss=False)
+    out["c3"] = {"ms_per_step": round(ms_c / K, 4), "value": round(NRAYS * S * K / (ms_c / 1e3), 1), "steps": K,
                  "workload": "C3 fern shape 756x1008, V=20, 1024 rays x 128 samples, NDC + dist_alpha (single 128-sample pass: the reference has no hierarchical sampling)"}
     del tr_c, devc
     # ---- config 4: one 1/8 row block of a 1080x1920 novel view, forward only ----
@@ -389,13 +366,30 @@ def single_gpu_records(dev, step, timed, args):
     return out
 
 
+def dump_outputs(out_dir, trainer, ld):
+    """the last step's loss terms and the parameters it updated, as float32 (parameters) / float64 (losses) .npy files"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for k, v in ld.items():
+        if torch.is_tensor(v) or isinstance(v, (int, float)):
+            np.save(os.path.join(out_dir, "loss_%s.npy" % k), np.asarray(torch.as_tensor(v).detach().double().cpu().numpy()))
+    mods = {"mlp": trainer.model, "pose": trainer.pose_param_net, "distortion": trainer.distortion_net}
+    for mn, mod in mods.items():
+        if mod is None:
+            continue
+        for pn, p in mod.named_parameters():
+            np.save(os.path.join(out_dir, "%s.%s.npy" % (mn, pn)), p.detach().float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------------------------
 def reference_on_device(device, steps, warm, budget_s):
     """Trainer.train_step of the UNMODIFIED reference (oracle/_ref) on the C2 workload at the full 1024 x 128 batch"""
     import torch
     from oracle import ref_harness as RH
     if not RH.available():
-        return {"unavailable": "oracle/_ref missing (tools/vendor_ref.py copies the reference there in the build container)"}
+        return {"unavailable": "oracle/_ref missing (oracle/vendor_ref.py copies a reference checkout there)"}
     cfg = RH.load_default_cfg()
     RH.set_cfg(cfg, {"training.pc_weight": [0.0, 0.0], "training.rgb_s_weight": [0.0, 0.0], "training.n_training_points": NRAYS,
                      "rendering.num_points": S, "training.vis_reprojection_every": 10 ** 9})
@@ -484,6 +478,8 @@ if __name__ == "__main__":
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--engine", default="tc", choices=["tc", "simt"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last step of the timed path (W warm-up + K steps from the seeded start) to DIR/<name>.npy")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="N > 1: weak = 1024 rays per GPU (global batch 1024*N), strong = the 1024-ray batch split over the GPUs")
     a = ap.parse_args()

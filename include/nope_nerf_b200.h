@@ -1,4 +1,4 @@
-/* nope_nerf_b200 — C ABI of the B200-native NoPe-NeRF render / pose-optimisation hot path.
+/* nope_nerf_b200 — C ABI of the H100-native (sm_90a) NoPe-NeRF render / pose-optimisation hot path.
  *
  * The reference (ActiveVisionLab/nope-nerf @ 47c861f6) is pure Python/PyTorch and has no
  * FFI layer (SURVEY.md 8(b)); the drop-in boundary is its Python class surface.  The host
@@ -32,21 +32,16 @@ extern "C" {
 #define NNB_SOFTPLUS 64u    /* model.occ_activation == 'softplus' (official_nerf.py:77-80)        */
 #define NNB_SHIFT_FIRST 128u /* training.shift_first    (training.py:241-245)                     */
 #define NNB_STASH 256u      /* keep activations in the workspace for nnb_render_bwd               */
-#define NNB_TCBWD 512u      /* NNB_ENGINE_TC only: tcgen05 backward (operand-image stash) instead of the fp32 one */
+#define NNB_TCBWD 512u      /* operand-plane backward of the TC engine: not available in the sm_90a library (rc < 0) */
 #define NNB_RAW_DENSITY 2048u /* nnb_field_fwd/bwd only: out_rgba[3] = the density LOGIT (fc_density output, official_nerf.py:66-67
                                 * infer_occ) instead of alpha / sigma; used for OfficialStaticNerf.gradient() (normals)            */
-#define NNB_FWD_DROP_WLO 4096u /* tcgen05 forward, precision experiment (DESIGN.md section 4; only in a library built with
-                                  -DNNB_FWD_SPLIT_EXPERIMENT, else rc -7): skip the a_hi*b_lo MMAs (weights = one fp16) */
-#define NNB_FWD_DROP_ALO 8192u /* tcgen05 forward, precision experiment: skip the a_lo*b_hi MMAs (activations = one fp16) */
-#define NNB_WG16 1024u      /* with NNB_TCBWD: the weight-gradient GEMMs dW = dY^T X read ONE fp16 plane per operand (X = the hi
-                             * half of the forward's fp16 hi|lo operand, dY = fp16 of dY * 2^k with a per-layer power-of-two scale
-                             * taken from the previous step's max |dY|, "delayed scaling") instead of bf16 hi|lo planes: half the
-                             * stash traffic, a third of the MMAs; MLP weight gradients then carry fp16 operand rounding
-                             * (~3e-4 relative, unbiased), everything else (outputs, pose / distortion / bias gradients) is unchanged */
+#define NNB_FWD_DROP_WLO 4096u /* forward precision experiment: rejected (rc -7) by this library */
+#define NNB_FWD_DROP_ALO 8192u /* forward precision experiment: rejected (rc -7) by this library */
+#define NNB_WG16 1024u      /* with NNB_TCBWD only (fp16 weight-gradient operand planes); without it the flag has no effect */
 
 /* engines */
 #define NNB_ENGINE_SIMT 0 /* exact fp32 FMA path                                        */
-#define NNB_ENGINE_TC 1   /* tcgen05 tensor cores, split-fp16 (hi/lo) operands, fp32 acc */
+#define NNB_ENGINE_TC 1   /* wgmma tensor cores, split 16-bit (hi/lo) operands, fp32 acc */
 
 /* One ray batch of one camera.  Mirrors the arguments of nope_nerf.forward
  * (model/network.py:19-20) + Renderer.nope_nerf (model/rendering.py:36-37) after the host
@@ -91,14 +86,10 @@ typedef struct nnb_render_bwd_args {
   float* g_cam;     /* [16] ([0],[5] written) or NULL */
   float* g_depth;   /* [N] d/d prior depth (overwritten) or NULL */
   float* g_scale_shift; /* [2] d/d scale, d/d shift when depth_map is used, or NULL */
-  /* 0 = whole backward.  The tcgen05 backward can be issued in two calls so that the caller may fork independent work (the
-   * reference-image stage) beside the HBM-bound weight-gradient kernel: 1 = compositing adjoint + data-gradient chain,
-   * 2 = weight gradients + ray adjoint.  Other engines do everything in phase 1 (or 0) and nothing in phase 2. */
+  /* 0 = whole backward.  A caller may issue it in two calls (1, then 2) to fork independent work beside it; this library does
+   * everything in phase 1 (or 0) and nothing in phase 2. */
   uint32_t phase;
-  /* NNB_WG16 only.  wg_state: 32 persistent device floats owned by the caller (zeroed once): [0..9] per-layer dY scales,
-   * [16..25] running max |dY| of the current step (uint bits).  wg_seed != 0 (the first step with this state): the data-gradient
-   * chain runs once more up front just to measure max |dY| (later steps reuse the previous step's maxima).  wg_state NULL:
-   * scratch state in the workspace, seeded on every call (stateless one-off calls, 2x the data-gradient time). */
+  /* state of the fp16 weight-gradient planes (NNB_WG16 with NNB_TCBWD); unused by this library, may be NULL */
   float* wg_state;
   uint32_t wg_seed;
 } nnb_render_bwd_args;
@@ -194,7 +185,7 @@ size_t nnb_refstage_workspace_bytes(int32_t h_d, int32_t w_d, int32_t pc_ratio);
 int nnb_refstage(const nnb_refstage_args* args, void* stream);
 
 /* ---- data-parallel exchange over NVLink peer memory (new component, SURVEY.md 8(e)) --------------------------------------
- * The reference has no distributed code; the B200 design shards a step's rays (or views) over the GPUs of one box and needs ONE
+ * The reference has no distributed code; the design shards a step's rays (or views) over the GPUs of one box and needs ONE
  * sum of the flat gradient buffer per step.  nnb_allreduce_adam does that sum with P2P loads from every rank's buffer and applies
  * the three torch.optim.Adam updates (train.py:58,99,117) in the same kernel; it is captured in the step's CUDA graph.
  * Buffers come from nnb_ipc_alloc (cudaMalloc + CUDA IPC handle); peers map them with nnb_ipc_open. */

@@ -59,7 +59,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             "nope_nerf_b200: CUDA library %s is missing. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     lib.nnb_last_error.restype = C.c_char_p
     lib.nnb_version.restype = C.c_int

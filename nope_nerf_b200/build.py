@@ -1,12 +1,12 @@
-"""Builds the in-tree CUDA library  nope_nerf_b200/libnope_nerf_b200.so  for sm_100a with nvcc.
+"""Builds the in-tree CUDA library  nope_nerf_b200/libnope_nerf_b200.so  for sm_90a (H100) with nvcc.
 No torch dependency: the library is a plain C-ABI shared object (include/nope_nerf_b200.h)."""
 import os, subprocess, sys, shutil
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libnope_nerf_b200.so")
-SOURCES = ["nnb_api.cu", "nnb_simt.cu", "nnb_misc.cu", "nnb_tc.cu", "nnb_tc_bwd.cu", "nnb_refstage.cu", "nnb_collective.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+SOURCES = ["nnb_api.cu", "nnb_simt.cu", "nnb_misc.cu", "nnb_tc.cu", "nnb_refstage.cu", "nnb_collective.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-DNNB_WITH_TC"]
 
 

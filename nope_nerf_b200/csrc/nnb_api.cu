@@ -89,10 +89,10 @@ static int check_args(const nnb_render_args* a) {
   if (!a->rgb || !a->depth_pred || !a->depth_gt || !a->mask) return fail(-3, "output pointers must be non-null");
   if (a->engine != NNB_ENGINE_SIMT && a->engine != NNB_ENGINE_TC) return fail(-4, "unknown engine %d", a->engine);
 #ifndef NNB_WITH_TC
-  if (a->engine == NNB_ENGINE_TC) return fail(-4, "library built without the tcgen05 engine");
+  if (a->engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
 #else
   if (a->engine == NNB_ENGINE_TC && !tc_supports(a->S))
-    return fail(-4, "tcgen05 engine needs S in {32,64,128,256} (got %d); use NNB_ENGINE_SIMT", a->S);
+    return fail(-4, "tensor-core engine needs S in {32,64,128,256} (got %d); use NNB_ENGINE_SIMT", a->S);
 #endif
   size_t need = nnb_workspace_bytes(a->N, a->S, a->flags, a->engine);
   if (!a->workspace || a->workspace_bytes < need)
@@ -105,7 +105,7 @@ int nnb_render_fwd(const nnb_render_args* a, void* stream) {
   int rc = check_args(a); if (rc) return rc;
 #ifndef NNB_FWD_SPLIT_EXPERIMENT
   if (a->flags & (NNB_FWD_DROP_WLO | NNB_FWD_DROP_ALO))
-    return fail(-7, "NNB_FWD_DROP_* needs a library built with -DNNB_FWD_SPLIT_EXPERIMENT (tools/fwd_split_check.py)");
+    return fail(-7, "NNB_FWD_DROP_* (forward precision experiment) is not built into this library");
 #endif
   WsLayout L = make_layout(a->N, a->S, a->flags, a->engine);
   cudaError_t e;

@@ -127,20 +127,16 @@ __global__ void loss_rgb_depth_k(const float* rgb, const float* rgb_gt, const fl
 //   * SIMT fp32, 2 * P * Q pairs (P = Q = 16 128 at the 384x672 DPT map / pc_ratio 4: 520 M pairs, ~6 instructions each).
 //   * squared distances in the difference form (a-b)^2 (no cancellation, no sqrt per pair: the MUFU pipe is 1/4 rate); ordering
 //     by d^2 equals ordering by |a-b| and exact duplicates keep the first index.
-//   * packed fp32x2 arithmetic (FADD2 / FMUL2 / FFMA2): one thread owns 4 queries = 2 register pairs, the target comes from shared
-//     memory already duplicated (bx,bx | by,by | bz,bz) so every LDS feeds both pairs.
-//   * 2-D decomposition queries x target splits so that ~4 blocks per SM are resident; the per-split winners meet in a 64-bit
-//     atomicMin on (d^2 bits << 32 | index): smallest distance first, smallest index among equal distances.
+//   * one thread owns 4 queries, the target comes from shared memory already duplicated (bx,bx | by,by | bz,bz) so every
+//     LDS feeds two queries.
 constexpr int NS_THREADS = 128, NS_QPT = 4, NS_CHUNK = 256;
 
-__device__ __forceinline__ unsigned long long pk2(float a, float b) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(unsigned long long v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) {
-  unsigned long long r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) {
-  unsigned long long r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+// two fp32 lanes, each rounded like a scalar sub / mul / fma (the (a-b)^2 ordering and tie-breaking stay those of scalar code)
+__device__ __forceinline__ float2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk2(float2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 __global__ void __launch_bounds__(NS_THREADS) nn_search_k(const float* __restrict__ X, int P, const float* __restrict__ Y, int Q,
                                                           unsigned long long* kxy, unsigned long long* kyx, int per_split) {
@@ -151,16 +147,16 @@ __global__ void __launch_bounds__(NS_THREADS) nn_search_k(const float* __restric
   if (blockIdx.x * (NS_THREADS * NS_QPT) >= na) return;
   const int t0 = blockIdx.y * per_split, t1 = min(nb, t0 + per_split);
   if (t0 >= t1) return;
-  __shared__ ulonglong2 sxy[NS_CHUNK];            // {(bx,bx), (by,by)}
-  __shared__ unsigned long long sz[NS_CHUNK];     // (bz,bz)
+  __shared__ float4 sxy[NS_CHUNK];                // {(bx,bx), (by,by)}
+  __shared__ float2 sz[NS_CHUNK];                 // (bz,bz)
   const int q0 = (blockIdx.x * NS_THREADS + threadIdx.x) * NS_QPT;
   float a[NS_QPT][3];
 #pragma unroll
   for (int j = 0; j < NS_QPT; ++j)
 #pragma unroll
     for (int c = 0; c < 3; ++c) a[j][c] = (q0 + j < na) ? A[3 * (size_t)(q0 + j) + c] : 0.f;
-  const unsigned long long ax0 = pk2(a[0][0], a[1][0]), ay0 = pk2(a[0][1], a[1][1]), az0 = pk2(a[0][2], a[1][2]);
-  const unsigned long long ax1 = pk2(a[2][0], a[3][0]), ay1 = pk2(a[2][1], a[3][1]), az1 = pk2(a[2][2], a[3][2]);
+  const float2 ax0 = pk2(a[0][0], a[1][0]), ay0 = pk2(a[0][1], a[1][1]), az0 = pk2(a[0][2], a[1][2]);
+  const float2 ax1 = pk2(a[2][0], a[3][0]), ay1 = pk2(a[2][1], a[3][1]), az1 = pk2(a[2][2], a[3][2]);
   float best[NS_QPT]; int bi[NS_QPT];
 #pragma unroll
   for (int j = 0; j < NS_QPT; ++j) { best[j] = INFINITY; bi[j] = 0; }
@@ -169,16 +165,16 @@ __global__ void __launch_bounds__(NS_THREADS) nn_search_k(const float* __restric
     __syncthreads();
     for (int k = threadIdx.x; k < n; k += NS_THREADS) {
       const float bx = B[3 * (size_t)(c0 + k)], by = B[3 * (size_t)(c0 + k) + 1], bz = B[3 * (size_t)(c0 + k) + 2];
-      sxy[k] = make_ulonglong2(pk2(bx, bx), pk2(by, by)); sz[k] = pk2(bz, bz);
+      sxy[k] = make_float4(bx, bx, by, by); sz[k] = pk2(bz, bz);
     }
     __syncthreads();
 #pragma unroll 4
     for (int k = 0; k < n; ++k) {
-      const ulonglong2 u = sxy[k]; const unsigned long long w = sz[k];
-      unsigned long long dx = sub2(ax0, u.x), dy = sub2(ay0, u.y), dz = sub2(az0, w);
-      const unsigned long long e0 = fma2(dz, dz, fma2(dy, dy, mul2(dx, dx)));
-      dx = sub2(ax1, u.x); dy = sub2(ay1, u.y); dz = sub2(az1, w);
-      const unsigned long long e1 = fma2(dz, dz, fma2(dy, dy, mul2(dx, dx)));
+      const float4 u4 = sxy[k]; const float2 ux = make_float2(u4.x, u4.y), uy = make_float2(u4.z, u4.w), w = sz[k];
+      float2 dx = sub2(ax0, ux), dy = sub2(ay0, uy), dz = sub2(az0, w);
+      const float2 e0 = fma2(dz, dz, fma2(dy, dy, mul2(dx, dx)));
+      dx = sub2(ax1, ux); dy = sub2(ay1, uy); dz = sub2(az1, w);
+      const float2 e1 = fma2(dz, dz, fma2(dy, dy, mul2(dx, dx)));
       float d[NS_QPT];
       upk2(e0, d[0], d[1]); upk2(e1, d[2], d[3]);
 #pragma unroll

@@ -1,11 +1,11 @@
 // Exact-fp32 SIMT engine (NNB_ENGINE_SIMT): the reference arithmetic (nn.Linear = fp32 FMA)
 // with the whole field evaluated tile-by-tile out of shared memory.  It is the bit-faithful
-// engine used for small batches and as the on-device cross-check of the tcgen05 engine.
+// engine used for small batches and as the on-device cross-check of the tensor-core engine.
 //   F1 simt_mlp_fwd     : ray-gen + sampling + encoding + 8x256 MLP + heads  (64 samples / CTA)
 //   F2 composite_fwd    : alpha compositing, one warp per ray (shared with the TC engine)
 //   B1 composite_bwd    : compositing adjoint -> per-sample (g_rgb, g_a)
 //   B2 simt_mlp_dgrad   : data-gradient chain through the MLP, emits dY per layer
-//   B3 simt_wgrad       : dW = dY^T X as split-M tiles with atomic accumulation
+//   B3 simt_wgrad       : dW = dY^T X as split-M tiles, one partial per split, summed in order by wgrad_reduce
 //   B4 ray_bwd          : per-ray geometry adjoint -> d c2w, d K, d depth, d scale/shift
 #include "nnb_workspace.cuh"
 
@@ -127,6 +127,7 @@ struct SimtPtrs {
   float *h[8], *feat, *hr, *enc, *denc;
   float *dy[8], *dfeat, *dyr;
   float4 *dyc, *gs, *gp, *gv;
+  float *rayred, *wpart;
 };
 
 __device__ __forceinline__ void row_geometry(const nnb_render_args& a, size_t m, size_t M, Ray& ray, int& n, int& i, float& z,
@@ -286,7 +287,7 @@ __global__ void composite_fwd(nnb_render_args a, const SampleRec* recs) {
 }
 
 // gmax (optional): running max |g| over all samples, as uint bits of a non-negative float
-// (feeds the power-of-two gradient scaling of the split-fp16 tcgen05 backward)
+// (feeds the power-of-two gradient scaling of an operand-plane backward)
 __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, float4* gs, unsigned int* gmax) {
   const nnb_render_args& a = b.fwd;
   const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -437,10 +438,12 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, Simt
 struct WJob {
   const float* dY; const float* X; float* dW; float* db;
   int ldy, Nn, ldx, Kk, ldw, tiles_k, tile_start, ntiles;
+  size_t part_off;   // this job's partials in the split buffer
 };
 struct WJobs { WJob j[16]; int njobs; };
 
-__global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int msplit) {
+// split blockIdx.y of job j writes its partial dW / db to part (layout of RedJob; wgrad_reduce sums the splits in order)
+__global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int msplit, float* part) {
   __shared__ __align__(16) float Ys[16][64];
   __shared__ __align__(16) float Xs[16][64];
   int ji = 0;
@@ -474,6 +477,7 @@ __global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int mspl
     }
     __syncthreads();
   }
+  float* pp = part + J.part_off + (size_t)blockIdx.y * ((size_t)J.Nn * J.Kk + J.Nn);
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
     int n = n0 + ni * 4 + r;
@@ -481,20 +485,38 @@ __global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int mspl
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       int k = k0 + ki * 4 + c;
-      if (k < J.Kk) atomicAdd(J.dW + (size_t)n * J.ldw + k, acc[r][c]);
+      if (k < J.Kk) pp[(size_t)n * J.Kk + k] = acc[r][c];
     }
-    if (J.db && tk == 0 && ki == 0) atomicAdd(J.db + n, bs[r]);
+    if (tk == 0 && ki == 0) pp[(size_t)J.Nn * J.Kk + n] = bs[r];
+  }
+}
+
+// dW[n][k] += sum over splits (fixed order); one thread per element of all jobs
+struct RedJobs { RedJob j[16]; int e0[17]; int njobs; };
+__global__ void wgrad_reduce(RedJobs J, const float* __restrict__ part) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= J.e0[J.njobs]) return;
+  int ji = 0;
+  while (ji + 1 < J.njobs && e >= J.e0[ji + 1]) ++ji;
+  const RedJob r = J.j[ji];
+  const int le = e - J.e0[ji], nk = r.Nn * r.Kk;
+  float s = 0.f;
+  if (le < nk) {
+    for (int y = 0; y < r.nsplit; ++y) s += part[r.off + (size_t)y * r.stride + le];
+    r.dW[(size_t)(le / r.Kk) * r.ldw + le % r.Kk] += s;
+  } else {
+    for (int y = 0; y < r.nsplit; ++y)
+      for (int q = 0; q < r.dbslots; ++q) s += part[r.off + (size_t)y * r.stride + nk + (size_t)q * r.Nn + (le - nk)];
+    r.db[le - nk] += s;
   }
 }
 
 // ---------------------------------------------------------------------------------------
 // B4: per-ray geometry adjoint (SURVEY.md A.6)
 // ---------------------------------------------------------------------------------------
-__global__ void ray_bwd(nnb_render_bwd_args b, const SampleRec* recs, const float4* gp, const float4* gv) {
+// per ray: red[0..8] d R, [9..11] d t, [12,13] d kx, ky, [14,15] d scale, shift -> rayred[n][16]; ray_reduce sums over the rays
+__global__ void ray_bwd(nnb_render_bwd_args b, const SampleRec* recs, const float4* gp, const float4* gv, float* rayred) {
   const nnb_render_args& a = b.fwd;
-  __shared__ float red[16];
-  if (threadIdx.x < 16) red[threadIdx.x] = 0.f;
-  __syncthreads();
   const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (n < a.N) {
     Ray r; setup_ray(a, n, r);
@@ -509,6 +531,9 @@ __global__ void ray_bwd(nnb_render_bwd_args b, const SampleRec* recs, const floa
 #pragma unroll
     for (int c = 0; c < 3; ++c) { so[c] = warp_sum(so[c]); sd[c] = warp_sum(sd[c]); sv[c] = warp_sum(sv[c]); }
     if (lane == 0) {
+      float red[16];
+#pragma unroll
+      for (int k = 0; k < 16; ++k) red[k] = 0.f;
       const bool normalise = a.flags & NNB_NORMALISE, ev = (a.flags & NNB_EVAL) && normalise;
       float g_nrm = 0.f;
       float gDo = b.g_depth_pred ? __ldg(b.g_depth_pred + n) : 0.f;
@@ -568,30 +593,40 @@ __global__ void ray_bwd(nnb_render_bwd_args b, const SampleRec* recs, const floa
 #pragma unroll
       for (int i = 0; i < 3; ++i) {
 #pragma unroll
-        for (int j = 0; j < 3; ++j) atomicAdd(&red[3 * i + j], g_dt[i] * r.dc[j]);
-        atomicAdd(&red[9 + i], g_o[i]);
+        for (int j = 0; j < 3; ++j) red[3 * i + j] = g_dt[i] * r.dc[j];
+        red[9 + i] = g_o[i];
       }
       float g_dc0 = g_dt[0] * r.R[0] + g_dt[1] * r.R[3] + g_dt[2] * r.R[6];
       float g_dc1 = g_dt[0] * r.R[1] + g_dt[1] * r.R[4] + g_dt[2] * r.R[7];
       g_kx += g_dc0 * (-r.x / (r.kx * r.kx));
       g_ky += g_dc1 * (-r.y / (r.ky * r.ky));
-      atomicAdd(&red[12], g_kx); atomicAdd(&red[13], g_ky);
+      red[12] = g_kx; red[13] = g_ky;
       if (b.g_depth) b.g_depth[n] = g_depth;
       if (!a.depth) {  // depth = raw*scale + shift  |  (raw + shift)*scale
         float sc = ld_scalar(a.scale, 1.f), sf = ld_scalar(a.shift, 0.f);
-        if (a.flags & NNB_SHIFT_FIRST) { atomicAdd(&red[14], g_depth * (r.depth_raw + sf)); atomicAdd(&red[15], g_depth * sc); }
-        else { atomicAdd(&red[14], g_depth * r.depth_raw); atomicAdd(&red[15], g_depth); }
+        if (a.flags & NNB_SHIFT_FIRST) { red[14] = g_depth * (r.depth_raw + sf); red[15] = g_depth * sc; }
+        else { red[14] = g_depth * r.depth_raw; red[15] = g_depth; }
       }
+#pragma unroll
+      for (int k = 0; k < 16; ++k) rayred[(size_t)n * 16 + k] = red[k];
     }
   }
-  __syncthreads();
-  if (threadIdx.x < 16) {
-    int k = threadIdx.x; float v = red[k];
-    if (k < 9) atomicAdd(b.g_c2w + 4 * (k / 3) + (k % 3), v);
-    else if (k < 12) atomicAdd(b.g_c2w + 4 * (k - 9) + 3, v);
-    else if (k == 12) { if (b.g_cam) atomicAdd(b.g_cam + 0, v); }
-    else if (k == 13) { if (b.g_cam) atomicAdd(b.g_cam + 5, v); }
-    else if (b.g_scale_shift && !a.depth) atomicAdd(b.g_scale_shift + (k - 14), v);
+}
+
+// warp k sums rayred[.][k] over the rays in a fixed order and adds the total to its gradient (one add per output and call; an
+// atomic one because the reference-image stage may add to g_c2w from a forked stream)
+__global__ void ray_reduce(nnb_render_bwd_args b, const float* __restrict__ rayred) {
+  const nnb_render_args& a = b.fwd;
+  const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float s = 0.f;
+  for (int n = lane; n < a.N; n += 32) s += rayred[(size_t)n * 16 + k];
+  s = warp_sum(s);
+  if (lane == 0) {
+    if (k < 9) atomicAdd(b.g_c2w + 4 * (k / 3) + (k % 3), s);
+    else if (k < 12) atomicAdd(b.g_c2w + 4 * (k - 9) + 3, s);
+    else if (k == 12) { if (b.g_cam) atomicAdd(b.g_cam + 0, s); }
+    else if (k == 13) { if (b.g_cam) atomicAdd(b.g_cam + 5, s); }
+    else if (b.g_scale_shift && !a.depth) atomicAdd(b.g_scale_shift + (k - 14), s);
   }
 }
 
@@ -605,6 +640,7 @@ SimtPtrs make_ptrs(const WsLayout& L, void* ws) {
   P.enc = reinterpret_cast<float*>(base + L.enc); P.denc = reinterpret_cast<float*>(base + L.denc);
   P.dfeat = reinterpret_cast<float*>(base + L.dfeat); P.dyr = reinterpret_cast<float*>(base + L.dyr);
   P.dyc = reinterpret_cast<float4*>(base + L.dyc);
+  P.rayred = reinterpret_cast<float*>(base + L.rayred); P.wpart = reinterpret_cast<float*>(base + L.wpart);
   return P;
 }
 
@@ -671,40 +707,47 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
   return cudaGetLastError();
 }
 
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, cudaStream_t st) {
-  WJobs J{}; int tile = 0;
+// jobs -> simt_wgrad into the partial buffer, then wgrad_reduce into dW / db
+cudaError_t run_simt_wgrad(WJobs& J, size_t M, int msplit, float* part, cudaStream_t st) {
+  RedJob R[16];
+  size_t off = 0; int tiles = 0;
+  for (int i = 0; i < J.njobs; ++i) {
+    WJob& j = J.j[i];
+    j.tiles_k = (j.Kk + 63) / 64; j.ntiles = ((j.Nn + 63) / 64) * j.tiles_k; j.tile_start = tiles; tiles += j.ntiles;
+    const size_t stride = (size_t)j.Nn * j.Kk + j.Nn;
+    R[i] = RedJob{j.dW, j.db, j.Nn, j.Kk, j.ldw, msplit, j.db ? 1 : 0, off, stride};
+    j.part_off = off;
+    off += stride * msplit;
+  }
+  if (off > wpart_floats(M)) return cudaErrorInvalidValue;
+  simt_wgrad<<<dim3(tiles, msplit), 256, 0, st>>>(J, M, msplit, part);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return launch_wgrad_reduce(R, J.njobs, part, st);
+}
+
+cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, float* part, cudaStream_t st) {
+  WJobs J{};
   for (int i = 0; i < njobs && i < 16; ++i) {
     WJob& j = J.j[i];
     j.dY = jobs[i].dY; j.ldy = jobs[i].ldy; j.Nn = jobs[i].Nn; j.X = jobs[i].X; j.ldx = jobs[i].ldx; j.Kk = jobs[i].Kk;
     j.dW = jobs[i].dW; j.ldw = jobs[i].ldw; j.db = jobs[i].db;
-    j.tiles_k = (j.Kk + 63) / 64; j.ntiles = ((j.Nn + 63) / 64) * j.tiles_k; j.tile_start = tile; tile += j.ntiles;
   }
-  J.njobs = njobs;
-  int msplit = (int)((M + 2047) / 2048); if (msplit < 1) msplit = 1; if (msplit > 64) msplit = 64;
-  simt_wgrad<<<dim3(tile, msplit), 256, 0, st>>>(J, M, msplit);
-  return cudaGetLastError();
+  J.njobs = njobs < 16 ? njobs : 16;
+  return run_simt_wgrad(J, M, jobs_wgrad_msplit(M), part, st);
 }
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st) {
   composite_fwd<<<(a.N + 7) / 8, 256, 0, st>>>(a, recs);
   return cudaGetLastError();
 }
-cudaError_t launch_composite_bwd(const nnb_render_bwd_args& b, const SampleRec* recs, float4* gs, unsigned int* gmax, cudaStream_t st) {
-  composite_bwd<<<(b.fwd.N + 7) / 8, 256, 0, st>>>(b, recs, gs, gmax);
-  return cudaGetLastError();
-}
-cudaError_t launch_ray_bwd(const nnb_render_bwd_args& b, const SampleRec* recs, const float4* gp, const float4* gv, cudaStream_t st) {
-  ray_bwd<<<(b.fwd.N + 7) / 8, 256, 0, st>>>(b, recs, gp, gv);
-  return cudaGetLastError();
-}
 
 cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cudaStream_t st) {
   {
-    WJobs J{}; int nj = 0, tile = 0;
+    WJobs J{}; int nj = 0;
     auto add = [&](const float* dY, int ldy, int Nn, const float* X, int ldx, int Kk, float* dW, int ldw, float* db) {
       WJob& j = J.j[nj++];
       j.dY = dY; j.ldy = ldy; j.Nn = Nn; j.X = X; j.ldx = ldx; j.Kk = Kk; j.dW = dW; j.ldw = ldw; j.db = db;
-      j.tiles_k = (Kk + 63) / 64; j.ntiles = ((Nn + 63) / 64) * j.tiles_k; j.tile_start = tile; tile += j.ntiles;
     };
     add(P.dy[0], 256, 256, P.enc, 64, 63, gw + nnb::w_off(0), 63, gw + nnb::b_off(0));
     for (int l = 1; l < 8; ++l) {
@@ -717,13 +760,24 @@ cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cuda
     add(P.dyr, 128, 128, P.denc, 32, 27, gw + nnb::W_RGBH + 256, 283, nullptr);
     add(reinterpret_cast<const float*>(P.dyc), 4, 3, P.hr, 128, 128, gw + nnb::W_RGB, 128, gw + nnb::B_RGB);
     J.njobs = nj;
-    int msplit = (int)((L.M + 4095) / 4096); if (msplit < 1) msplit = 1; if (msplit > 16) msplit = 16;
-    simt_wgrad<<<dim3(tile, msplit), 256, 0, st>>>(J, L.M, msplit);
+    return run_simt_wgrad(J, L.M, simt_wgrad_msplit(L.M), P.wpart, st);
   }
+}
+
+cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st) {
+  RedJobs J{};
+  J.njobs = njobs < 16 ? njobs : 16;
+  J.e0[0] = 0;
+  for (int i = 0; i < J.njobs; ++i) { J.j[i] = jobs[i]; J.e0[i + 1] = J.e0[i] + jobs[i].Nn * jobs[i].Kk + (jobs[i].db ? jobs[i].Nn : 0); }
+  wgrad_reduce<<<(J.e0[J.njobs] + 255) / 256, 256, 0, st>>>(J, part);
   return cudaGetLastError();
 }
 
-cudaError_t simt_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st) {
+cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
+cudaError_t simt_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st) { return simt_render_bwd_with(b, L, st, nullptr, nullptr); }
+
+// dgrad / wgrad: the data- / weight-gradient stages (nullptr: the fp32 SIMT kernels)
+cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad) {
   const nnb_render_args& a = b.fwd;
   SimtPtrs P = make_ptrs(L, a.workspace);
   cudaError_t e0 = simt_init();
@@ -733,11 +787,16 @@ cudaError_t simt_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cud
   composite_bwd<<<(a.N + 7) / 8, 256, 0, st>>>(b, P.rec, P.gs, nullptr);
   nnb_prof_mark(st);
   const int write_dy = b.g_weights ? 1 : 0;
-  simt_mlp_dgrad<<<tiles, 256, BWD_SMEM, st>>>(a, P, L.M, write_dy);
+  if (dgrad) { cudaError_t ed = dgrad(b, L, write_dy, st); if (ed != cudaSuccess) return ed; }
+  else simt_mlp_dgrad<<<tiles, 256, BWD_SMEM, st>>>(a, P, L.M, write_dy);
   nnb_prof_mark(st);
-  if (b.g_weights) { cudaError_t ew = simt_wgrad_all(P, L, b.g_weights, st); if (ew != cudaSuccess) return ew; }
+  if (b.g_weights) {
+    cudaError_t ew = wgrad ? wgrad(a, L, b.g_weights, st) : simt_wgrad_all(P, L, b.g_weights, st);
+    if (ew != cudaSuccess) return ew;
+  }
   nnb_prof_mark(st);
-  ray_bwd<<<(a.N + 7) / 8, 256, 0, st>>>(b, P.rec, P.gp, P.gv);
+  ray_bwd<<<(a.N + 7) / 8, 256, 0, st>>>(b, P.rec, P.gp, P.gv, P.rayred);
+  ray_reduce<<<1, 512, 0, st>>>(b, P.rayred);
   nnb_prof_mark(st);
   return cudaGetLastError();
 }

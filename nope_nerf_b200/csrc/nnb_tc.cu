@@ -1,38 +1,29 @@
-// tcgen05 engine (NNB_ENGINE_TC): the whole field of a 128-sample tile evaluated by one
-// persistent, warp-specialised CTA per SM.
+// Tensor-core engine (NNB_ENGINE_TC), Hopper (sm_90a): the whole field of a 128-sample tile evaluated by one persistent CTA
+// per SM.
 //
-//   warp 0      : weight producer  - cp.async.bulk (UBLKCP) of pre-imaged fp16 hi/lo weight
-//                 k-slices (16 KB) from L2 into a 3-deep shared-memory ring, mbarrier tx-count
-//   warp 1      : MMA issuer       - one elected thread issues tcgen05.mma.kind::f16
-//                 (M=128, N=256|128, K=16) with BOTH operands from shared memory; every logical
-//                 product runs as three MMAs a_hi*b_hi + a_hi*b_lo + a_lo*b_hi (split-fp16, 22-bit
-//                 operands, fp32 accumulation in TMEM) so results match the fp32 reference
-//   warps 10..13: prologue         - thread = sample row of the NEXT tile: ray generation, prior gather, sampling, the 63-column
-//                 positional encoding -> E operand (+ its plane / stash), direction encoding -> per-ray bias of rgb_layers.0;
-//                 runs one tile ahead of the epilogue (the E operand is free once layer 4's MMAs have completed), so the
-//                 30 sincosf per sample never sit between two tiles of the tensor pipe
-//   warps 2..9  : epilogue         - two warps per TMEM lane quarter (thread = sample row, the two warps take
-//                 alternate 32-column chunks): tcgen05.ld of the accumulator, bias + ReLU, re-split into
-//                 hi/lo halves written IN PLACE as the next layer's A operand (canonical no-swizzle
-//                 K-major core-matrix layout); then, from the same registers, density / colour heads and
-//                 the training stash (bf16 operand planes, ReLU bitmasks, fp32 side stash).
+//   warps 0..7: two consumer warpgroups, each owning 64 sample rows of the tile.  Prologue: ray generation, sampling, the
+//               63-column positional encoding -> E operand, direction encoding -> per-ray bias of rgb_layers.0.  Per layer the
+//               warpgroup issues wgmma.m64n256k16 (m64n128k16 for the rgb hidden layer) with both operands in shared memory;
+//               every logical product runs as three MMAs a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (split-fp16, 22-bit operands, fp32
+//               accumulation in registers) so results match the fp32 reference.  The epilogue (bias, ReLU, re-split into
+//               hi | lo halves) writes the next layer's A operand IN PLACE: a warpgroup's MMAs read only its own 64 rows, and
+//               they have completed (wgmma.wait_group 0) before the epilogue starts.  Density / colour heads, the per-sample
+//               record and the fp32 training stash come out of the same registers.
+//   warp 8   : weight producer (in the third warpgroup, whose registers go to the consumers) - cp.async.bulk of pre-imaged
+//               fp16 hi | lo weight stages (all output rows x 16 k) from L2 into a 3-deep shared-memory ring, mbarrier tx-count;
+//               a stage is released once both warpgroups' MMAs have read it.
 //
-// N-half pipeline: every 256-wide GEMM runs as two 128-column halves with one 128-column TMEM accumulator each, and the A operand
-// ALTERNATES between shared memory (odd layers, tcgen05.mma "ss" form) and tensor memory (even layers, "ts" form: lane = sample row,
-// two k per 32-bit column).  The epilogue of layer g therefore writes the next A operand into the medium the running MMAs of layer
-// g do NOT read: it converts half 0 (A blocks 0,1 of layer g+1) while the tensor core is still busy with half 1, and layer g+1
-// starts its first K-steps the moment half 1 is issued -- per layer the tensor pipe only waits for the epilogue of the LAST half
-// (blocks 2,3) instead of for the first chunk of a 256-column accumulator plus the pacing of all four blocks.
+// The backward of this engine (tc_render_bwd) runs tc_dgrad (the same skeleton through the transposed weights) and tc_wgrad (the
+// MLP weight-gradient GEMMs) on the fp32 stash, between the compositing and ray adjoints of nnb_simt.cu.
 //
-// Shared memory operand layout (no swizzle, "interleaved"): element (row, k) of a [rows x K] fp16
-// operand lives at byte  (k/8) * rows*16 + row*16 + (k%8)*2 : 8x8 core matrices of 128 contiguous
-// bytes, SBO = 128 B between row-groups, LBO = rows*16 B between the two k-halves of one MMA.
-// Tensor memory map (512 columns): [0,256) the two half accumulators, [256,384) A hi, [384,512) A lo (even layers).
+// Shared-memory operand layout (no swizzle, "interleave"): element (row, k) of a [rows x K] fp16 operand lives at byte
+// (k / 8) * rows * 16 + row * 16 + (k % 8) * 2: 8 x 8 core matrices of 128 contiguous bytes, SBO = 128 B between row groups,
+// LBO = rows * 16 B between the two k-halves of one MMA.
 #include "nnb_tc_common.cuh"
-#include <cstdlib>
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st);
-cudaError_t simt_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
+cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
+cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, float* part, cudaStream_t st);
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -40,105 +31,78 @@ namespace {
 
 constexpr int TILE = 128;
 constexpr int NST = 3;                      // weight ring depth
-constexpr int STAGE_BYTES = 16384;          // 128 rows x 32 k x (hi + lo) fp16 = two K-steps of one 128-column half
+constexpr int STAGE_BYTES = 16384;          // 256 output rows x 16 k x (hi + lo) fp16 = one K-step of a 256-wide layer
 constexpr int N_GEMM = 10;                  // L0..L7, feature, rgb-hidden
-// ---- stage table: the order in which weight stages are consumed for one tile: layer, half, k-group -----------------
-struct StageDesc { int w_off, ldw, kcol0, kvalid, row0, img_off; };
-constexpr int N_STAGES = 2 * 2 + 3 * 16 + 2 * (2 + 8) + 3 * 16 + 16 + 8;   // 144
+// ---- stage table: the order in which weight stages are consumed for one tile --------------------------------------------
+struct StageDesc { int w_off, ldw, kcol0, kvalid, nrows, img_off; };
+constexpr int N_STAGES = 4 + 3 * 16 + (4 + 16) + 3 * 16 + 16 + 16;   // 152
 __constant__ StageDesc c_stages[N_STAGES];
-constexpr size_t IMG_BYTES = (size_t)N_STAGES * STAGE_BYTES;
+constexpr size_t IMG_BYTES = (size_t)(N_STAGES - 16) * STAGE_BYTES + 16 * (STAGE_BYTES / 2);   // rgb hidden layer: 128 rows
 
 // shared memory map (bytes)
 constexpr int SM_AHI = 0, SM_ALO = 65536, SM_EHI = 131072, SM_ELO = 147456, SM_W = 163840;
 constexpr int SM_BIAS = SM_W + NST * STAGE_BYTES;             // 212992
 constexpr int BIAS_FLOATS = 8 * 256 + 256 + 256 + 384 + 4;    // trunk, feat, w_sigma, W_rgb, (b_sigma, b_rgb[3])
 constexpr int SM_RAYB = SM_BIAS + ((BIAS_FLOATS * 4 + 127) / 128) * 128;
-constexpr int RAYB_FLOATS = 4 * 128 + 4 * 32;                 // per-ray bias [4][128] + direction-encoding staging [4][32]
-constexpr int SM_PART = SM_RAYB + 2 * RAYB_FLOATS * 4;      // two buffers: the prologue warps run one tile ahead of the epilogue
-constexpr int SM_BAR = SM_PART + 128 * 4 * 4;                // head partial sums / exchange buffer
-constexpr int SM_TOTAL = SM_BAR + 32 * 8 + 16;
+constexpr int RAYB_FLOATS = 2 * 128 + 2 * 32;                 // per warpgroup: per-ray bias [2 rays][128] + direction encodings [2][32]
+constexpr int SM_BAR = SM_RAYB + 2 * RAYB_FLOATS * 4;
+constexpr int SM_TOTAL = SM_BAR + 2 * NST * 8;
 static_assert(SM_TOTAL <= 232448, "shared memory budget");
-enum { B_FULL = 0, B_EMPTY = NST, B_AREADY = 2 * NST, B_EREADY = 2 * NST + 4, B_ACCFULL = 2 * NST + 5, B_ACCEMPTY = 2 * NST + 7, B_EFREE = 2 * NST + 9, B_COUNT = 2 * NST + 10 };
-constexpr uint32_t TM_AHI = 256, TM_ALO = 384;   // tensor-memory columns of the even layers' A operand
+constexpr int N_THREADS = 384;              // two consumer warpgroups + the producer warpgroup (one thread of it issues the copies)
 
 using namespace tcu;
 
 // ---- weight imaging: fp32 (out,in) matrices -> per-stage shared-memory images (hi | lo) --------
 __global__ void tc_prep_weights(const float* __restrict__ w, unsigned char* __restrict__ img) {
-  const int s = blockIdx.x;
-  const StageDesc sd = c_stages[s];
-  unsigned char* hi = img + sd.img_off;       // [k-octet 0..3][128 rows][8] fp16
-  unsigned char* lo = hi + 8192;
-  for (int idx = threadIdx.x; idx < 128 * 4; idx += blockDim.x) {
-    const int n = idx & 127, ko = idx >> 7;
+  const StageDesc sd = c_stages[blockIdx.x];
+  unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] fp16
+  unsigned char* lo = hi + sd.nrows * 32;
+  for (int idx = threadIdx.x; idx < sd.nrows * 2; idx += blockDim.x) {
+    const int n = idx % sd.nrows, ko = idx / sd.nrows;
     float v[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int k = sd.kcol0 + ko * 8 + j;
-      v[j] = (k < sd.kvalid) ? __ldg(w + sd.w_off + (size_t)(sd.row0 + n) * sd.ldw + k) : 0.f;
+      v[j] = (k < sd.kvalid) ? __ldg(w + sd.w_off + (size_t)n * sd.ldw + k) : 0.f;
     }
-    split_store8(v, hi + ko * 2048 + n * 16, lo + ko * 2048 + n * 16);
+    split_store8(v, hi + ko * sd.nrows * 16 + n * 16, lo + ko * sd.nrows * 16 + n * 16);
   }
 }
 
-#ifdef NNB_TC_PROFILE
-__device__ unsigned long long g_tcprof[148][8];
-__device__ unsigned long long g_tcprof2[148][8];
-// timeline of ONE tile (CTA 0, its 4th tile): [0..63] MMA thread, [64..255] epilogue thread (warp 2 lane 0); raw clock64 values
-__device__ unsigned long long g_tctrace[256];
-#define TRACE(cond, idx) do { if ((cond) && blockIdx.x == 0 && (threadIdx.x & 31) == 0) g_tctrace[idx] = clock64(); } while (0)
-#define PROF_T0() unsigned long long _t0 = clock64()
-#define PROF_ADD(slot) do { unsigned long long _t1 = clock64(); _pacc[slot] += _t1 - _t0; _t0 = _t1; } while (0)
-#else
-#define PROF_T0()
-#define PROF_ADD(slot)
-#define TRACE(cond, idx)
-#endif
+struct TcStash { float *h[8], *feat, *hr, *enc, *denc; };   // fp32 [sample][feature] stash, layout of nnb_simt.cu
 
-struct TcStash {   // fp32 [sample][feature] stash (layout of nnb_simt.cu) and, with NNB_TCBWD, operand planes + ReLU bitmasks
-  float *h[8], *feat, *hr, *enc, *denc;
-  unsigned char* xp[10]; uint32_t* mask; size_t Mpad; int tcb;
-  int wg16;   // NNB_WG16: X planes are ONE fp16 plane per tile (the hi words of the forward's own A / E operands)
-};
-
-__device__ __forceinline__ void row_geometry_tc(const nnb_render_args& a, size_t m, size_t M, Ray& ray, int& n, int& i, float& z, float p[3]) {
-  size_t mm = m < M ? m : M - 1;
-  n = (int)(mm / a.S); i = (int)(mm % a.S);
+__device__ __forceinline__ void row_geometry_tc(const nnb_render_args& a, size_t m, size_t M, Ray& ray, float& z, float p[3]) {
+  const size_t mm = m < M ? m : M - 1;
+  const int n = (int)(mm / a.S), i = (int)(mm % a.S);
   setup_ray(a, n, ray);
   z = sample_z(a, n, i);
   sample_point(a, ray, z, p);
 }
 
-template <int CL>   // CL = thread-block cluster size (1 | 2 | 4): CTAs of a cluster share every weight stage via multicast
-__global__ void __launch_bounds__(448, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
-                                                        TcStash st, size_t M, int n_tiles, int stash) {
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+__global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                              SampleRec* __restrict__ recs, TcStash st, size_t M, int n_tiles, int stash) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* s_bias = reinterpret_cast<float*>(smem + SM_BIAS);
-  float* s_rayb = reinterpret_cast<float*>(smem + SM_RAYB);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM_BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 32 * 8);
-  const uint32_t bar0 = smem_u32(bars);
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
+  const uint32_t bar0 = smem_u32(smem + SM_BAR);
+  auto FULL = [&](uint32_t i) { return bar0 + 8u * i; };
+  auto EMPTY = [&](uint32_t i) { return bar0 + 8u * (NST + i); };
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NST; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), CL); }
-    for (int i = 0; i < 4; ++i) mbar_init(BAR(B_AREADY + i), 256);
-    mbar_init(BAR(B_EREADY), 128);
-    mbar_init(BAR(B_EFREE), 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(BAR(B_ACCFULL + i), 1); mbar_init(BAR(B_ACCEMPTY + i), 256); }
+    for (int i = 0; i < NST; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 2); }   // EMPTY: one arrival per warpgroup
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {  // TMEM: all 512 columns (two 128-column half accumulators + the even layers' A operand hi | lo)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   {  // biases / small heads -> shared (weights are constant for the launch)
     const float* w = a.weights;
     for (int i = threadIdx.x; i < BIAS_FLOATS; i += blockDim.x) {
       float v;
-      if (i < 2048) v = -__ldg(w + nnb::b_off(i >> 8) + (i & 255));       // trunk / feature biases are stored NEGATED (epi_chunk32)
-      else if (i < 2304) v = -__ldg(w + nnb::B_FEAT + (i - 2048));
+      if (i < 2048) v = __ldg(w + nnb::b_off(i >> 8) + (i & 255));
+      else if (i < 2304) v = __ldg(w + nnb::B_FEAT + (i - 2048));
       else if (i < 2560) v = __ldg(w + nnb::W_SIG + (i - 2304));
       else if (i < 2944) v = __ldg(w + nnb::W_RGB + (i - 2560));
       else if (i == 2944) v = __ldg(w + nnb::B_SIG);
@@ -146,141 +110,51 @@ __global__ void __launch_bounds__(448, 1) tc_field_fwd(nnb_render_args a, const 
       s_bias[i] = v;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();    // every CTA's barriers are initialised before any remote arrive / multicast lands
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // all CTAs run the same number of tile iterations (the weight stream is shared inside a cluster);
-  // iterations whose tile index is past the end only keep the stream flowing
-  const int my_tiles = (n_tiles + (int)gridDim.x - 1) / (int)gridDim.x;
-  const uint16_t cmask = (uint16_t)((1u << CL) - 1u);
-  const uint32_t crank = CL > 1 ? cluster_ctarank() : 0u;
+  const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles blockIdx.x, + gridDim.x, ...
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // =============================== weight producer ===============================
-    if (lane == 0) {
+    // registers move from the producer warpgroup to the consumers: 40 + 2 x 232 per SM sub-partition fits the register file
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0;
-      for (int t = 0; t < my_tiles; ++t) {
+      for (int t = 0; t < my_tiles; ++t)
         for (int s = 0; s < N_STAGES; ++s) {
-          const int bytes = STAGE_BYTES;
-          mbar_wait(BAR(B_EMPTY + slot), phase ^ 1);          // all CL consumers released this slot
-          mbar_expect_tx(BAR(B_FULL + slot), bytes);
-          if (CL == 1) bulk_g2s(smem_u32(smem + SM_W + slot * STAGE_BYTES), wimg + c_stages[s].img_off, bytes, BAR(B_FULL + slot));
-          else {   // this CTA fetches slice `crank` of the stage and multicasts it into every CTA of the cluster
-            const int sl = bytes / CL;
-            bulk_g2s_mc(smem_u32(smem + SM_W + slot * STAGE_BYTES + crank * sl), wimg + c_stages[s].img_off + crank * sl, sl,
-                        BAR(B_FULL + slot), cmask);
-          }
-          if (++slot == NST) { slot = 0; phase ^= 1; }
+          const uint32_t bytes = (uint32_t)c_stages[s].nrows * 64u;
+          mbar_wait(EMPTY(slot), phase ^ 1u);                 // both warpgroups released this slot
+          mbar_expect_tx(FULL(slot), bytes);
+          bulk_g2s(smem_u32(smem + SM_W + slot * STAGE_BYTES), wimg + c_stages[s].img_off, bytes, FULL(slot));
+          if (++slot == NST) { slot = 0; phase ^= 1u; }
         }
-      }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ====================================
-    // The WHOLE warp runs this loop converged (every lane polls the barriers, all values are warp-uniform); the tcgen05.mma /
-    // tcgen05.commit instructions are issued by the one lane elect.sync picks, so ptxas emits them under a uniform predicate
-    // instead of wrapping each in a divergence-election loop (6 extra instructions per MMA when the code sat under `lane == 0`).
+    return;
+  }
+  // =============================== consumer warpgroups ===============================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int wg = warp >> 2, tl = threadIdx.x & 127;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // tile rows r0 and r0 + 8 hold this thread's accumulator fragment
+  const int c0 = (lane & 3) * 2;                               // its column pair inside every 8-column block
+  float* rayb = reinterpret_cast<float*>(smem + SM_RAYB) + wg * RAYB_FLOATS;
+  const uint32_t a_hi = smem_u32(smem + SM_AHI) + wg * 1024, a_lo = smem_u32(smem + SM_ALO) + wg * 1024;
+  const uint32_t e_hi = smem_u32(smem + SM_EHI) + wg * 1024, e_lo = smem_u32(smem + SM_ELO) + wg * 1024;
+  const uint32_t w_base = smem_u32(smem + SM_W);
+  const uint32_t bar_id = 1u + (uint32_t)wg;
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
+  const int rays_per_wg = (a.S >= 64) ? 1 : 64 / a.S;
+  uint32_t slot = 0, phase = 0;
+  float acc[128];
+
+  for (int t = 0; t < my_tiles; ++t) {
+    const int tile = blockIdx.x + t * gridDim.x;
+    const size_t mt = (size_t)tile * TILE;
+    wg_sync();   // the previous tile's epilogue is done with the per-ray bias buffer
     {
-      uint32_t slot = 0, phase = 0;
-      // descriptor low words of the operand buffers (tc_stage6: everything else is an addition)
-      const uint32_t a_hi0 = desc_lo(smem_u32(smem + SM_AHI)), a_lo0 = desc_lo(smem_u32(smem + SM_ALO));
-      const uint32_t e_hi0 = desc_lo(smem_u32(smem + SM_EHI)), e_lo0 = desc_lo(smem_u32(smem + SM_ELO));
-      const uint32_t w_lo0 = desc_lo(smem_u32(smem + SM_W));
-      const uint32_t bar_full0 = BAR(B_FULL), bar_empty0 = BAR(B_EMPTY), bar_aready0 = BAR(B_AREADY);
-#ifdef NNB_FWD_SPLIT_EXPERIMENT
-      const uint32_t fmode = (a.flags >> 12) & 3u;   // NNB_FWD_DROP_WLO | NNB_FWD_DROP_ALO (instrumented build: the extra code costs 3.8 % of the kernel)
-#else
-      const uint32_t fmode = 0u;                     // product build: the experiment's code paths fold away
-#endif
-      int tv = 0;   // number of VALID tiles processed so far (phase bookkeeping of the per-tile barriers)
-#ifdef NNB_TC_PROFILE
-      unsigned long long _pacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      const unsigned long long _tstart = clock64();
-#endif
-      for (int t = 0; t < my_tiles; ++t) {
-        if (blockIdx.x + t * gridDim.x >= n_tiles) {   // past the end: consume + release the stages only
-          for (int s = 0; s < N_STAGES; ++s) {
-            mbar_wait(BAR(B_FULL + slot), phase);
-            tc_fence_after();
-            if (CL == 1) tc_commit_elect(BAR(B_EMPTY + slot)); else tc_commit_mc_elect(BAR(B_EMPTY + slot), cmask);
-            if (++slot == NST) { slot = 0; phase ^= 1; }
-          }
-          continue;
-        }
-        const uint32_t idesc = make_idesc(128, 128);
-        for (int g = 0; g < N_GEMM; ++g) {
-          const int e_stages = (g == 0 || g == 4) ? 2 : 0;        // weight stages (two K-steps each) fed by the encoding operand E
-          const bool has_a = (g != 0);                            // 8 stages fed by the previous layer's output
-          const bool a_tmem = (g & 1) == 0;                       // even layers read A from tensor memory (written by the odd layer before)
-          const int nhalf = (g == 9) ? 1 : 2;
-          for (int h = 0; h < nhalf; ++h) {
-            const uint32_t use = h ? (uint32_t)tv * 9u + (uint32_t)g : (uint32_t)tv * 10u + (uint32_t)g;
-            PROF_T0();
-            mbar_wait(BAR(B_ACCEMPTY + h), (use & 1u) ^ 1u);      // the epilogue of the previous layer has drained this half accumulator
-            tc_fence_after();
-            PROF_ADD(0);
-            TRACE(tv == 3, (g * 2 + h) * 3);
-            const uint32_t d_tmem = tmem_base + h * 128;
-            if (g == 0 && h == 0) { mbar_wait(BAR(B_EREADY), (uint32_t)tv & 1u); tc_fence_after(); }
-            PROF_ADD(1);
-            uint32_t acc = 0;
-            uint32_t full_ok = mbar_probe(BAR(B_FULL + slot), phase);    // probe early: its latency hides under the other waits
-            // one weight stage: wait (rarely) for its bytes, six MMAs, release; descriptors are additions to precomputed low words
-            auto stage = [&](bool ts, uint32_t aL, uint32_t aH) {
-              if (!full_ok) mbar_wait(bar_full0 + 8u * slot, phase);
-              tc_fence_after();
-              const uint32_t wb = w_lo0 + slot * (STAGE_BYTES >> 4);
-              const uint32_t nslot = (slot + 1 == NST) ? 0u : slot + 1, nphase = (slot + 1 == NST) ? phase ^ 1u : phase;
-              if (fmode == 0u) {
-                if (ts) full_ok = tc_stage6<CL, true>(d_tmem, aL, aH, wb, 256u, idesc, acc, bar_empty0 + 8u * slot, cmask, bar_full0 + 8u * nslot, nphase);
-                else full_ok = tc_stage6<CL, false>(d_tmem, aL, aH, wb, 256u, idesc, acc, bar_empty0 + 8u * slot, cmask, bar_full0 + 8u * nslot, nphase);
-              } else {   // NNB_FWD_DROP_*: fewer terms of the split (precision experiment)
-                if (ts) full_ok = tc_stage6_sel<CL, true>(fmode, d_tmem, aL, aH, wb, 256u, idesc, acc, bar_empty0 + 8u * slot, cmask, bar_full0 + 8u * nslot, nphase);
-                else full_ok = tc_stage6_sel<CL, false>(fmode, d_tmem, aL, aH, wb, 256u, idesc, acc, bar_empty0 + 8u * slot, cmask, bar_full0 + 8u * nslot, nphase);
-              }
-              acc = 1u; slot = nslot; phase = nphase;
-            };
-            for (int st = 0; st < e_stages; ++st) stage(false, e_lo0 + st * 512, e_hi0 + st * 512);
-            if (has_a) {
-              const uint32_t au = ((uint32_t)tv * 9u + (uint32_t)(g - 1)) & 1u;
-              const uint32_t aL = a_tmem ? tmem_base + TM_ALO : a_lo0, aH = a_tmem ? tmem_base + TM_AHI : a_hi0;
-              const uint32_t a_st = a_tmem ? 16u : 512u;         // two K-steps: 16 tensor-memory columns | 8192 B of shared memory
-#pragma unroll
-              for (int st = 0; st < 8; ++st) {
-                if ((st & 1) == 0 && h == 0) {   // first K-step of a 64-column block of A: wait for the previous layer's epilogue (half 1 re-reads)
-                  mbar_wait(bar_aready0 + 8u * (st >> 1), au);
-                  tc_fence_after();
-                  TRACE(tv == 3 && st == 6, (g * 2 + h) * 3 + 1);      // last A block of the layer has arrived
-                }
-                stage(a_tmem, aL + st * a_st, aH + st * a_st);
-              }
-            }
-            PROF_ADD(4);
-            tc_commit_elect(BAR(B_ACCFULL + h));
-            if (g == 4 && h == 1) tc_commit_elect(BAR(B_EFREE));   // every MMA that reads this tile's E operand has been issued
-            TRACE(tv == 3, (g * 2 + h) * 3 + 2);
-          }
-        }
-        ++tv;
-      }
-#ifdef NNB_TC_PROFILE
-      if (lane == 0 && blockIdx.x < 148) { for (int i = 0; i < 5; ++i) g_tcprof[blockIdx.x][i] = _pacc[i]; g_tcprof[blockIdx.x][5] = clock64() - _tstart; g_tcprof[blockIdx.x][6] = tv; }
-#endif
-    }
-  } else if (warp >= 10) {
-    // =============================== prologue warps ================================
-    // thread = sample row; one tile ahead of the epilogue warps (E operand double use: released by B_EFREE after layer 4's MMAs)
-    const int row = (warp - 10) * 32 + lane;
-    int tv = -1;
-    for (int tt = 0; tt < my_tiles; ++tt) {
-      const int tile = blockIdx.x + tt * gridDim.x;
-      if (tile >= n_tiles) continue;
-      const int t = ++tv;
-      const size_t m = (size_t)tile * TILE + row;
-      float* rayb = s_rayb + (t & 1) * RAYB_FLOATS;
-      Ray ray; int n, i; float z, p[3];
-      row_geometry_tc(a, m, M, ray, n, i, z, p);
+      // ---- prologue: thread (row rl, part) writes encoding columns [32 part, 32 part + 32) of its row ----
+      const int rl = tl & 63, part = tl >> 6, row = wg * 64 + rl;
+      const size_t m = mt + row;
+      Ray ray; float z, p[3];
+      row_geometry_tc(a, m, M, ray, z, p);
       float ee[64];
 #pragma unroll
       for (int c = 0; c < 3; ++c) ee[c] = p[c];
@@ -291,206 +165,562 @@ __global__ void __launch_bounds__(448, 1) tc_field_fwd(nnb_render_args a, const 
         for (int c = 0; c < 3; ++c) { float sn, cs; sincosf(__fmul_rn(f, p[c]), &sn, &cs); ee[3 + 6 * l + c] = sn; ee[6 + 6 * l + c] = cs; }
       }
       ee[63] = 0.f;
-      // direction-encoding term of rgb_layers.0 is constant per ray: fold it into a per-ray bias
-      float v[3], de[32];
-      view_dir(a, ray, v);
-      encode<4>(v, [&](int k, float val) { de[k] = val; });
-#pragma unroll
-      for (int k = 27; k < 32; ++k) de[k] = 0.f;
-      if (stash) {
-#pragma unroll
-        for (int k4 = 0; k4 < 8; ++k4)
-          *reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4) = make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]);
-      }
-      // the E operand / this per-ray bias buffer were last read by the tile before the previous one's ... -> wait for B_EFREE
-      mbar_wait(BAR(B_EFREE), ((uint32_t)t & 1u) ^ 1u);
 #pragma unroll
       for (int kb = 0; kb < 8; ++kb) {
-        const uint4 eh = split_store8_hi(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
-        if (stash && !(st.tcb & 1)) {
+        if ((kb >> 2) != part) continue;   // static register indices: ee[] stays in registers
+        split_store8(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
+        if (stash) {
           *reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8) = make_float4(ee[kb * 8], ee[kb * 8 + 1], ee[kb * 8 + 2], ee[kb * 8 + 3]);
           *reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8 + 4) = make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]);
         }
-        if (stash && (st.tcb & 1)) {   // X plane 0 (encoding) of the weight-gradient pass: bf16 hi|lo, [k/8][row][8]
-          if (st.wg16) {                 // ... or the fp16 hi half of the E operand itself: [half][kb][64][8], one plane
-            st_stream16(st.xp[0] + (size_t)tile * (PLANE_TILE_64 / 2) + (row >> 6) * 8192 + (row & 63) * 16 + kb * 1024, eh);
-          } else {
-            unsigned char* dst = st.xp[0] + (size_t)tile * PLANE_TILE_64 + (row >> 6) * 8192 + (row & 63) * 16;   // [hi|lo][half][kb][64][8]
-            split_stream8_bf16(ee + kb * 8, dst + kb * 1024, dst + 16384 + kb * 1024);
-          }
+      }
+      if (part == 0) {   // direction-encoding term of rgb_layers.0 is constant per ray: folded into a per-ray bias below
+        float v[3], de[32];
+        view_dir(a, ray, v);
+        encode<4>(v, [&](int k, float val) { de[k] = val; });
+#pragma unroll
+        for (int k = 27; k < 32; ++k) de[k] = 0.f;
+        if (stash) {
+#pragma unroll
+          for (int k4 = 0; k4 < 8; ++k4)
+            *reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4) = make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]);
         }
-      }
-      const int ray_local = (a.S >= TILE) ? 0 : row / a.S;
-      const bool first_of_ray = (a.S >= TILE) ? (row == 0) : (row % a.S == 0);
-      if (first_of_ray) {   // rows that start a ray publish their direction encoding
+        if (rl % (rays_per_wg == 1 ? 64 : a.S) == 0) {   // the row that starts a ray publishes its direction encoding
+          const int r = rays_per_wg == 1 ? 0 : rl / a.S;
 #pragma unroll
-        for (int k = 0; k < 32; ++k) rayb[512 + ray_local * 32 + k] = de[k];
-      }
-      asm volatile("bar.sync 2, 128;" ::: "memory");
-      {
-        const int nrays = (a.S >= TILE) ? 1 : TILE / a.S;
-        const float* w = a.weights;
-        for (int r = 0; r < nrays; ++r) {
-          float acc = __ldg(w + nnb::B_RGBH + row);
-#pragma unroll
-          for (int k = 0; k < 27; ++k) acc = fmaf(__ldg(w + nnb::W_RGBH + (size_t)row * 283 + 256 + k), rayb[512 + r * 32 + k], acc);
-          rayb[r * 128 + row] = -acc;            // negated like the other biases
+          for (int k = 0; k < 32; ++k) rayb[256 + r * 32 + k] = de[k];
         }
       }
       fence_async_smem();
-      mbar_arrive(BAR(B_EREADY));
+      wg_sync();
+      const float* w = a.weights;
+      for (int r = 0; r < rays_per_wg; ++r) {   // thread tl = output column of the rgb hidden layer
+        float b = __ldg(w + nnb::B_RGBH + tl);
+#pragma unroll
+        for (int k = 0; k < 27; ++k) b = fmaf(__ldg(w + nnb::W_RGBH + (size_t)tl * 283 + 256 + k), rayb[256 + r * 32 + k], b);
+        rayb[r * 128 + tl] = b;   // read after layer 0's epilogue barrier
+      }
     }
-  } else {
-    // =============================== epilogue warps ================================
-    // 8 warps: two per TMEM lane quarter.  Thread = sample row; `half` selects which column chunks of the
-    // accumulator this thread converts (two warps per scheduler hide the tcgen05.ld / convert latencies).
-    const int q = warp & 3;                    // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;          // 0: warps 2-5, 1: warps 6-9
-    const int row = q * 32 + lane;             // sample row of this thread
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    unsigned char* A_hi = smem + SM_AHI; unsigned char* A_lo = smem + SM_ALO;
-    float* s_part = reinterpret_cast<float*>(smem + SM_PART);   // [128][4] head partial sums of half 1
-#ifdef NNB_TC_PROFILE
-    unsigned long long _pacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#endif
-    int tv = -1;
-    for (int tt = 0; tt < my_tiles; ++tt) {
-      const int tile = blockIdx.x + tt * gridDim.x;
-      if (tile >= n_tiles) continue;
-      const int t = ++tv;        // index among this CTA's valid tiles (barrier phase bookkeeping)
-      const size_t m = (size_t)tile * TILE + row;
-      PROF_T0();
-      epi_bar();   // previous tile's epilogues are done with s_part
-      const size_t mm_ = m < M ? m : M - 1;
-      const float z = sample_z(a, (int)(mm_ / a.S), (int)(mm_ % a.S));
-      const int ray_local = (a.S >= TILE) ? 0 : row / a.S;
-      const float* rayb = s_rayb + (t & 1) * RAYB_FLOATS;
-      mbar_wait(BAR(B_EREADY), (uint32_t)t & 1u);     // this tile's per-ray bias (written by the prologue warps) is visible
-      float s_logit = 0.f, c_acc[3] = {0.f, 0.f, 0.f};
-      PROF_ADD(0);
-      // ---- per-GEMM epilogues ----
-      for (int g = 0; g < N_GEMM; ++g) {
-        const float* bias = (g < 8) ? s_bias + g * 256 : (g == 8 ? s_bias + 2048 : rayb + ray_local * 128);
-        const bool planes = stash && (st.tcb & 1);
-        const int dbg = st.tcb >> 1;
-        const bool wg16 = st.wg16 != 0;
-        unsigned char* xplane = (planes && g < 9 && !(dbg & 1)) ? st.xp[1 + g] + (size_t)tile * (wg16 ? PLANE_TILE_256 / 2 : PLANE_TILE_256) + (row >> 6) * 32768 + (row & 63) * 16 : nullptr;
-        // Per 32-column chunk: (1) critical path of the MMA warp: accumulator -> bias/ReLU -> fp16 hi|lo -> next A operand (shared
-        // memory for an odd next layer, tensor memory for an even one), block by block: the two thread halves convert adjacent
-        // chunks of the SAME 64-column block, so a block is complete after one chunk time; (2) after the block is signalled, from the
-        // same registers, everything the next MMA does not need: density / colour heads, fp32 side stash, operand planes, ReLU
-        // bitmasks.  The A operand of layer g+1 lives in the medium layer g's MMAs do not read, so half 0 is converted while the
-        // tensor core still works on half 1.
-        const bool need2 = (g == 7) || (g == 9) || stash;
-        const bool x_lo = !(dbg & 4);            // X planes carry the bf16 lo half too (NNB_DBG_FWD bit 2: hi only, experiment)
-        const bool next_tmem = (g & 1) == 1;     // layer g+1 is even -> its A operand goes to tensor memory
-        auto side_work = [&](int cb, const float* v, uint32_t mw, const uint32_t* hw) {
-          if (g == 7) {
+    float s_logit[2] = {0.f, 0.f};
+    for (int g = 0; g < N_GEMM; ++g) {
+      // ---- MMAs: K-steps from the encoding operand E (layers 0 and 4) first, then from the previous layer's output ----
+      const int n_e = (g == 0 || g == 4) ? 4 : 0, ns = n_e + (g == 0 ? 0 : 16);
+      const uint32_t nrows = (g == 9) ? 128u : 256u;
+      for (int s = 0; s < ns; ++s) {
+        const bool from_e = s < n_e;
+        const uint32_t ko = (uint32_t)(from_e ? s : s - n_e) * 4096u;   // two k-octets of 2048 B per K-step
+        const uint64_t dah = gdesc((from_e ? e_hi : a_hi) + ko, 2048, 128), dal = gdesc((from_e ? e_lo : a_lo) + ko, 2048, 128);
+        const uint32_t wb = w_base + slot * STAGE_BYTES;
+        const uint64_t dbh = gdesc(wb, nrows * 16u, 128), dbl = gdesc(wb + nrows * 32u, nrows * 16u, 128);
+        mbar_wait(FULL(slot), phase);
+        wgmma_fence();
+        if (g < 9) {
+          wgmma_f16<256>(acc, dal, dbh, s > 0 ? 1u : 0u);
+          wgmma_f16<256>(acc, dah, dbl, 1u);
+          wgmma_f16<256>(acc, dah, dbh, 1u);
+        } else {
+          wgmma_f16<128>(acc, dal, dbh, s > 0 ? 1u : 0u);
+          wgmma_f16<128>(acc, dah, dbl, 1u);
+          wgmma_f16<128>(acc, dah, dbh, 1u);
+        }
+        wgmma_commit();
+        if (s > 0) {   // the previous K-step's MMAs have completed: release its weight stage
+          wgmma_wait<1>();
+          if (tl == 0) mbar_arrive(EMPTY(slot == 0 ? NST - 1 : slot - 1));
+        }
+        if (++slot == NST) { slot = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      if (tl == 0) mbar_arrive(EMPTY(slot == 0 ? NST - 1 : slot - 1));
+      // ---- epilogue ----
+      if (g < 9) {
+        const float* bias = (g < 8) ? s_bias + g * 256 : s_bias + 2048;
+        float* sp = stash ? (g < 8 ? st.h[g] : st.feat) : nullptr;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) s_logit = fmaf(v[j], s_bias[2304 + cb * 32 + j], s_logit);
-          }
-          if (g == 9) {
+        for (int j = 0; j < 32; ++j) {
+          const int col = j * 8 + c0;
+          const float2 b = *reinterpret_cast<const float2*>(bias + col);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              c_acc[0] = fmaf(v[j], s_bias[2560 + cb * 32 + j], c_acc[0]);
-              c_acc[1] = fmaf(v[j], s_bias[2560 + 128 + cb * 32 + j], c_acc[1]);
-              c_acc[2] = fmaf(v[j], s_bias[2560 + 256 + cb * 32 + j], c_acc[2]);
-            }
+          for (int r = 0; r < 2; ++r) {
+            const int row = r0 + 8 * r;
+            float v0 = acc[4 * j + 2 * r] + b.x, v1 = acc[4 * j + 2 * r + 1] + b.y;
+            if (g != 8) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            uint32_t hw, lw;
+            split2(v0, v1, hw, lw);
+            const int off = j * 2048 + row * 16 + c0 * 2;
+            *reinterpret_cast<uint32_t*>(smem + SM_AHI + off) = hw;
+            *reinterpret_cast<uint32_t*>(smem + SM_ALO + off) = lw;
+            if (g == 7) s_logit[r] = fmaf(v1, s_bias[2304 + col + 1], fmaf(v0, s_bias[2304 + col], s_logit[r]));
+            if (sp) __stcs(reinterpret_cast<float2*>(sp + (mt + row) * 256 + col), make_float2(v0, v1));
           }
-          if (stash && !(planes && wg16) && (!planes || g == 7 || g == 9)) {     // fp32 side stashes of the heads (exact planes / fp32 backward)
-            float* dst = (g < 8) ? st.h[g] + m * 256 : (g == 8 ? st.feat + m * 256 : st.hr + m * 128);
+        }
+        fence_async_smem();
+        wg_sync();   // the whole A operand (and, after layer 0, the per-ray bias) is written before the next layer's MMAs
+      } else {
+        // rgb hidden layer (128 columns) -> colour head + per-sample record
+        float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4)
-              __stcs(reinterpret_cast<float4*>(dst + cb * 32 + j4 * 4), make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]));
-          }
-          if (planes && wg16 && g == 9) {   // NNB_WG16: the rgb hidden layer goes out as an fp16 plane too (fc_rgb's weight gradient reads it);
-            unsigned char* hp = reinterpret_cast<unsigned char*>(st.hr) + (size_t)tile * (PLANE_TILE_128 / 2) + (row >> 6) * 16384 + (row & 63) * 16;
-#pragma unroll                                // h7 needs nothing extra: fc_density's weight gradient reads the X plane of fc_feature
-            for (int kb = 0; kb < 4; ++kb)
-              st_stream16(hp + (cb * 4 + kb) * 1024, make_uint4(hw[kb * 4], hw[kb * 4 + 1], hw[kb * 4 + 2], hw[kb * 4 + 3]));
-          }
-          if (xplane && wg16) {   // the fp16 hi words just written as the next A operand ARE the X plane: 4 x 16 B, no conversion
+        for (int j = 0; j < 16; ++j) {
+          const int col = j * 8 + c0;
 #pragma unroll
-            for (int kb = 0; kb < 4; ++kb)
-              st_stream16(xplane + (cb * 4 + kb) * 1024, make_uint4(hw[kb * 4], hw[kb * 4 + 1], hw[kb * 4 + 2], hw[kb * 4 + 3]));
-          } else if (xplane) {   // X operand plane of the weight-gradient pass (h_g, or feat for g = 8): bf16 hi[|lo], coalesced 512 B per warp
+          for (int r = 0; r < 2; ++r) {
+            const int row = r0 + 8 * r;
+            const float* rb = rayb + (rays_per_wg == 1 ? 0 : (row - wg * 64) / a.S) * 128;
+            const float v0 = fmaxf(acc[4 * j + 2 * r] + rb[col], 0.f), v1 = fmaxf(acc[4 * j + 2 * r + 1] + rb[col + 1], 0.f);
 #pragma unroll
-            for (int kb = 0; kb < 4; ++kb)
-              plane_stream8_bf16(v + kb * 8, xplane + (cb * 4 + kb) * 1024, xplane + 65536 + (cb * 4 + kb) * 1024, x_lo);
+            for (int c = 0; c < 3; ++c)
+              c_acc[r][c] = fmaf(v1, s_bias[2560 + c * 128 + col + 1], fmaf(v0, s_bias[2560 + c * 128 + col], c_acc[r][c]));
+            if (stash) __stcs(reinterpret_cast<float2*>(st.hr + (mt + row) * 128 + col), make_float2(v0, v1));
           }
-          if (planes && (g < 8 || g == 9) && !(dbg & 2))     // ReLU gate bits of this 32-column chunk (g = 9: rgb hidden layer, slot 8);
-            __stcs(st.mask + ((size_t)(g < 8 ? g : 8) * st.Mpad + m) * 8 + cb, mw);   // column j at bit 31 - j (epi_chunk32)
-        };
-        const int nhalf = (g == 9) ? 1 : 2;
-#pragma unroll 1
-        for (int h = 0; h < nhalf; ++h) {
-          const uint32_t use = h ? (uint32_t)t * 9u + (uint32_t)g : (uint32_t)t * 10u + (uint32_t)g;
-          mbar_wait(BAR(B_ACCFULL + h), use & 1u);
-          tc_fence_after();
-          PROF_ADD(1);
-          TRACE(t == 3 && warp == 2 && lane == 0, 64 + (g * 2 + h) * 8);
-#pragma unroll 1
-          for (int ci = 0; ci < 2; ++ci) {
-            const int cb = 4 * h + 2 * ci + half;          // 32-column chunk of the layer output; A block of the next layer = cb >> 1
-            uint32_t r[32];
-            tc_ld32(lane_addr + cb * 32, r);
-            PROF_ADD(2);
-            float v[32];
-            uint32_t hw[16], lw[16];
-            const uint32_t mw = (g == 8) ? epi_chunk32<false>(r, bias + cb * 32, v, hw, lw, true)
-                                         : epi_chunk32<true>(r, bias + cb * 32, v, hw, lw, g < 9 || (planes && wg16), g < 9);
-            if (g < 9) {
-              PROF_ADD(3);
-              if (next_tmem) {
-                tc_st16(lane_addr + TM_AHI + cb * 16, hw); tc_st16(lane_addr + TM_ALO + cb * 16, lw);
-                tc_wait_st();
-                tc_fence_before();
-              } else {
-                store_words_smem(hw, lw, A_hi + cb * 4 * 2048 + row * 16, A_lo + cb * 4 * 2048 + row * 16);
-                fence_async_smem();
-              }
-              PROF_ADD(4);
-              mbar_arrive(BAR(B_AREADY + (cb >> 1)));     // 256 arrivals (both thread halves) complete the block
-              PROF_ADD(5);
-            }
-            TRACE(t == 3 && warp == 2 && lane == 0, 64 + (g * 2 + h) * 8 + 1 + ci * 2);
-            if (need2) side_work(cb, v, mw, hw);
-            TRACE(t == 3 && warp == 2 && lane == 0, 64 + (g * 2 + h) * 8 + 2 + ci * 2);
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const float sl = quad_sum(s_logit[r]);
+          const float cr = quad_sum(c_acc[r][0]), cg = quad_sum(c_acc[r][1]), cb = quad_sum(c_acc[r][2]);
+          if ((lane & 3) == 0) {
+            const size_t m = mt + r0 + 8 * r, mm = m < M ? m : M - 1;
+            const float s = sl + s_bias[2944];
+            float sigma;
+            SampleRec rec;
+            rec.r = sigmoid_f(cr + s_bias[2945]); rec.g = sigmoid_f(cg + s_bias[2946]); rec.b = sigmoid_f(cb + s_bias[2947]);
+            rec.a = density_act(s, a.flags, &sigma); rec.s = s; rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
+            rec.pad0 = 0.f; rec.pad1 = 0.f;
+            recs[m] = rec;
           }
-          tc_fence_before();
-          mbar_arrive(BAR(B_ACCEMPTY + h));
-          PROF_ADD(6);
-          TRACE(t == 3 && warp == 2 && lane == 0, 64 + (g * 2 + h) * 8 + 5);
         }
       }
-      // ---- heads + per-sample record (half 1 hands its partial dot products to half 0) ----
-      if (half == 1) {
-        *reinterpret_cast<float4*>(s_part + row * 4) = make_float4(s_logit, c_acc[0], c_acc[1], c_acc[2]);
-      }
-      epi_bar();
-      if (half == 0) {
-        const float4 o = *reinterpret_cast<const float4*>(s_part + row * 4);
-        const float s = s_logit + o.x + s_bias[2944];
-        float sigma;
-        SampleRec rec;
-        rec.r = sigmoid_f(c_acc[0] + o.y + s_bias[2945]); rec.g = sigmoid_f(c_acc[1] + o.z + s_bias[2946]);
-        rec.b = sigmoid_f(c_acc[2] + o.w + s_bias[2947]);
-        rec.a = density_act(s, a.flags, &sigma); rec.s = s; rec.z = z; rec.pad0 = 0.f; rec.pad1 = 0.f;
-        recs[m] = rec;
+    }
+  }
+}
+
+// ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
+// CTA = one 128-row slice of dW (two warpgroups x 64 rows, all KN columns in registers) over a contiguous share of the samples.
+// Per 64-sample block every thread converts its share of dY^T / X^T to bf16 hi | lo K-major operands in shared memory (double
+// buffered: the conversion of block c overlaps the MMAs of block c - 1), then each warpgroup issues 4 K-steps x three MMAs
+// (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi).  Each sample split stores its partial dW (and two bias partials per row, one per thread
+// half) to the split buffer; wgrad_reduce adds the splits to the gradient in a fixed order, so the result is the same every run.
+struct WgJobT { const float* dY; const float* X; float* dW; float* db; int ldy, Nn, ldx, Kk, ldw, cta0; size_t part_off; };
+constexpr int MAX_WG_JOBS = 10, WG_CHUNK = 64;
+struct WgJobsT { WgJobT j[MAX_WG_JOBS]; int njobs, msplit, per_cta; };
+template <int KN> constexpr int wg_smem() { return 2 * (2 * 128 * 128 + 2 * KN * 128); }
+
+template <int KN>   // 256 | 64: columns of dW (features of X) held by one CTA
+__global__ void __launch_bounds__(256, 1) tc_wgrad(WgJobsT J, size_t M, float* __restrict__ part) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  constexpr int A_BYTES = 128 * 128, B_BYTES = KN * 128, BUF = 2 * A_BYTES + 2 * B_BYTES;
+  int ji = 0;
+  while (ji + 1 < J.njobs && (int)blockIdx.x >= J.j[ji + 1].cta0) ++ji;
+  const WgJobT jb = J.j[ji];
+  const int local = blockIdx.x - jb.cta0, n0 = (local / J.msplit) * 128;
+  const size_t s_begin = (size_t)(local % J.msplit) * J.per_cta;
+  const size_t s_end = (s_begin + J.per_cta < M) ? s_begin + J.per_cta : M;   // an empty split stores zeros
+  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  float acc[KN / 2];
+#pragma unroll
+  for (int i = 0; i < KN / 2; ++i) acc[i] = 0.f;
+  float dbsum = 0.f;
+  int c = 0;
+  for (size_t s0 = s_begin; s0 < s_end; s0 += WG_CHUNK, ++c) {
+    unsigned char* buf = smem + (c & 1) * BUF;
+    __syncthreads();   // both warpgroups' MMAs of block c - 2 (the last readers of buf) have completed
+    {   // A = dY^T: row n (128), reduction index = sample; thread = one row x four 8-sample groups
+      const int n = tid & 127;
+      const bool nv = n0 + n < jb.Nn;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int so = (tid >> 7) * 4 + i;
+        float v[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const size_t s = s0 + so * 8 + q;
+          v[q] = (nv && s < s_end) ? __ldg(jb.dY + s * jb.ldy + n0 + n) : 0.f;
+          dbsum += v[q];
+        }
+        split_store8_bf16(v, buf + so * 2048 + n * 16, buf + A_BYTES + so * 2048 + n * 16);
       }
     }
-#ifdef NNB_TC_PROFILE
-    if (warp == 2 && lane == 0 && blockIdx.x < 148) for (int i = 0; i < 7; ++i) g_tcprof2[blockIdx.x][i] = _pacc[i];
-#endif
+#pragma unroll
+    for (int i = 0; i < KN * 8 / 256; ++i) {   // B = X^T: row k (KN), reduction index = sample
+      const int item = tid + i * 256, k = item % KN, so = item / KN;
+      float v[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const size_t s = s0 + so * 8 + q;
+        v[q] = (k < jb.Kk && s < s_end) ? __ldg(jb.X + s * jb.ldx + k) : 0.f;
+      }
+      split_store8_bf16(v, buf + 2 * A_BYTES + so * KN * 16 + k * 16, buf + 2 * A_BYTES + B_BYTES + so * KN * 16 + k * 16);
+    }
+    fence_async_smem();
+    __syncthreads();
+    const uint32_t a = smem_u32(buf) + wg * 1024, b = smem_u32(buf + 2 * A_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t dah = gdesc(a + ks * 4096, 2048, 128), dal = gdesc(a + A_BYTES + ks * 4096, 2048, 128);
+      const uint64_t dbh = gdesc(b + ks * 2 * KN * 16, KN * 16, 128), dbl = gdesc(b + B_BYTES + ks * 2 * KN * 16, KN * 16, 128);
+      wgmma_bf16<KN>(acc, dal, dbh, (c > 0 || ks > 0) ? 1u : 0u);
+      wgmma_bf16<KN>(acc, dah, dbl, 1u);
+      wgmma_bf16<KN>(acc, dah, dbh, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
   }
-  tc_fence_before();
+  wgmma_wait<0>();
+  float* pp = part + jb.part_off + (size_t)(local % J.msplit) * ((size_t)jb.Nn * jb.Kk + 2 * jb.Nn);
+  const int r0 = n0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
+#pragma unroll
+  for (int j = 0; j < KN / 8; ++j)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int n = r0 + 8 * r;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int k = j * 8 + c0 + e;
+        if (n < jb.Nn && k < jb.Kk) pp[(size_t)n * jb.Kk + k] = acc[4 * j + 2 * r + e];
+      }
+    }
+  if (n0 + (tid & 127) < jb.Nn) pp[(size_t)jb.Nn * jb.Kk + (tid >> 7) * jb.Nn + n0 + (tid & 127)] = dbsum;
+}
+
+template <int KN>
+cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int msplit, float* part, cudaStream_t st) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem<KN>());
+    if (e != cudaSuccess) return e;
+    attr = true;
+  }
+  WgJobsT J{};
+  RedJob R[MAX_WG_JOBS];
+  int ctas = 0;
+  size_t off = 0;
+  for (int i = 0; i < njobs; ++i) {
+    J.j[i] = jobs[i]; J.j[i].cta0 = ctas; ctas += (jobs[i].Nn + 127) / 128 * msplit;
+    const size_t stride = (size_t)jobs[i].Nn * jobs[i].Kk + 2 * jobs[i].Nn;
+    J.j[i].part_off = off;
+    R[i] = RedJob{jobs[i].dW, jobs[i].db, jobs[i].Nn, jobs[i].Kk, jobs[i].ldw, msplit, 2, off, stride};
+    off += stride * msplit;
+  }
+  if (off > wpart_floats(M)) return cudaErrorInvalidValue;
+  J.njobs = njobs; J.msplit = msplit;
+  J.per_cta = (int)(((M + msplit - 1) / msplit + WG_CHUNK - 1) / WG_CHUNK * WG_CHUNK);
+  tc_wgrad<KN><<<ctas, 256, wg_smem<KN>(), st>>>(J, M, part);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return launch_wgrad_reduce(R, njobs, part, st);
+}
+
+// the weight-gradient stage of the TC engine's backward: the MLP GEMMs on tensor cores, the small heads on the fp32 SIMT kernel
+cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) {
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  WgJobT big[9], enc[2];
+  int nb = 0;
+  for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(l), gw + nnb::b_off(l), 256, 256, 256, 256, nnb::w_ld(l), 0, 0};
+  big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT, gw + nnb::B_FEAT, 256, 256, 256, 256, 256, 0, 0};
+  big[nb++] = WgJobT{F(L.dyr), F(L.feat), gw + nnb::W_RGBH, gw + nnb::B_RGBH, 128, 128, 256, 256, 283, 0, 0};
+  enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(0), gw + nnb::b_off(0), 256, 256, 64, 63, 63, 0, 0};
+  enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(4) + 256, nullptr, 256, 256, 64, 63, 319, 0, 0};
+  float* part = F(L.wpart);   // reused by each launch: its reduction runs before the next launch on the same stream
+  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (17 | 4 row slices)
+  const int ms_big = L.M >= 8 * 128 ? 8 : 1, ms_enc = L.M >= 32 * 64 ? 32 : 1;
+  cudaError_t e = launch_wgrad<256>(big, nb, L.M, ms_big, part, st);
+  if (e != cudaSuccess) return e;
+  e = launch_wgrad<64>(enc, 2, L.M, ms_enc, part, st);
+  if (e != cudaSuccess) return e;
+  const float* dyc = F(L.dyc);
+  SmallJob sm[3] = {
+      {dyc + 3, F(L.h[7]), gw + nnb::W_SIG, gw + nnb::B_SIG, 4, 1, 256, 256, 256},
+      {F(L.dyr), F(L.denc), gw + nnb::W_RGBH + 256, nullptr, 128, 128, 32, 27, 283},
+      {dyc, F(L.hr), gw + nnb::W_RGB, gw + nnb::B_RGB, 4, 3, 128, 128, 128}};
+  return launch_simt_wgrad_jobs(sm, 3, L.M, part, st);
+}
+
+// ---- data-gradient chain (the forward's skeleton run backwards) ---------------------------------------------------------------------
+// Per 128-sample tile, two consumer warpgroups (64 rows each) and a producer warpgroup streaming TRANSPOSED weight stages: stage =
+// `nrows` input features n x 16 output features k of one layer, element (n, k) = W[k * ldw + coloff + n], bf16 hi | lo (gradients
+// span five decades).  A operand = the output gradient g_y of the current layer (bf16 hi | lo, K-major, rewritten in place by each
+// epilogue); the epilogue applies the ReLU gate of the layer below (its fp32 stash > 0) and writes that layer's dY stash for the
+// weight-gradient pass.  Order (matches the stage table): g_de = g_yr W_rgbh[:, 256:283] (N = 32), g_feat = g_yr W_rgbh[:, :256],
+// g_h7 = g_feat W_feat + g_s w_sigma, then layers 7..1 (layer 4 first adds its encoding slice, N = 64) and layer 0 (encoding, N = 64).
+struct StageDescT { int w_off, ldw, coloff, nvalid, k0, kvalid, nrows, img_off; };
+constexpr int N_STAGES_T = 8 + 8 + 16 + 7 * 16 + 16 + 16;   // 176
+__constant__ StageDescT c_stages_t[N_STAGES_T];
+constexpr size_t IMG_T_BYTES = (size_t)136 * STAGE_BYTES + 8 * 2048 + 32 * 4096;
+constexpr int DG_AHI = 0, DG_ALO = 65536, DG_W = 131072, DG_GENC = DG_W + NST * STAGE_BYTES;   // 180224
+constexpr int DG_SMALL = DG_GENC + 2 * 64 * 64 * 4;     // W_rgb [3][128] | w_sigma [256]
+constexpr int DG_GYC = DG_SMALL + 640 * 4;              // per row: d/d(rgb logits), d/d density logit
+constexpr int DG_BAR = DG_GYC + 128 * 4 * 4;
+constexpr int DG_TOTAL = DG_BAR + 2 * NST * 8;
+static_assert(DG_TOTAL <= 232448, "shared memory budget");
+
+__global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __restrict__ img) {
+  const StageDescT sd = c_stages_t[blockIdx.x];
+  unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] bf16
+  unsigned char* lo = hi + sd.nrows * 32;
+  for (int idx = threadIdx.x; idx < sd.nrows * 2; idx += blockDim.x) {
+    const int n = idx % sd.nrows, ko = idx / sd.nrows;
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = sd.k0 + ko * 8 + j;
+      v[j] = (n < sd.nvalid && k < sd.kvalid) ? __ldg(w + sd.w_off + (size_t)k * sd.ldw + sd.coloff + n) : 0.f;
+    }
+    split_store8_bf16(v, hi + ko * sd.nrows * 16 + n * 16, lo + ko * sd.nrows * 16 + n * 16);
+  }
+}
+
+struct DgPtrs {
+  const SampleRec* rec; const float4* gs; float4* gp; float4* gv; float4* dyc;
+  const float* h[8]; const float* hr; float* dy[8]; float* dfeat; float* dyr;
+};
+
+// K-steps of one GEMM: D[64 x N] = A[64 x 16 ksteps] B^T, weight stages from the ring (released as their MMAs complete)
+template <int N>
+__device__ __forceinline__ void dg_gemm(float* acc, uint32_t a_hi, uint32_t a_lo, int ksteps, uint32_t w_base, uint32_t bar0,
+                                        uint32_t& slot, uint32_t& phase, int tl) {
+  for (int s = 0; s < ksteps; ++s) {
+    const uint32_t ko = (uint32_t)s * 4096u;
+    const uint64_t dah = gdesc(a_hi + ko, 2048, 128), dal = gdesc(a_lo + ko, 2048, 128);
+    const uint32_t wb = w_base + slot * STAGE_BYTES;
+    const uint64_t dbh = gdesc(wb, N * 16, 128), dbl = gdesc(wb + N * 32, N * 16, 128);
+    mbar_wait(bar0 + 8u * slot, phase);
+    wgmma_fence();
+    wgmma_bf16<N>(acc, dal, dbh, s > 0 ? 1u : 0u);
+    wgmma_bf16<N>(acc, dah, dbl, 1u);
+    wgmma_bf16<N>(acc, dah, dbh, 1u);
+    wgmma_commit();
+    if (s > 0) {
+      wgmma_wait<1>();
+      if (tl == 0) mbar_arrive(bar0 + 8u * (NST + (slot == 0 ? NST - 1 : slot - 1)));
+    }
+    if (++slot == NST) { slot = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  if (tl == 0) mbar_arrive(bar0 + 8u * (NST + (slot == 0 ? NST - 1 : slot - 1)));
+}
+
+__device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 hh = __floats2bfloat162_rn(a, b);
+  hi = *reinterpret_cast<uint32_t*>(&hh);
+  __nv_bfloat162 ll = __floats2bfloat162_rn(a - __uint_as_float(hi << 16), b - __uint_as_float(hi & 0xffff0000u));
+  lo = *reinterpret_cast<uint32_t*>(&ll);
+}
+
+__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, const unsigned char* __restrict__ wimg, DgPtrs P, size_t M,
+                                                         int n_tiles, int write_dy) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* s_small = reinterpret_cast<float*>(smem + DG_SMALL);
+  const uint32_t bar0 = smem_u32(smem + DG_BAR);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < NST; ++i) { mbar_init(bar0 + 8u * i, 1); mbar_init(bar0 + 8u * (NST + i), 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = threadIdx.x; i < 640; i += blockDim.x) s_small[i] = (i < 384) ? __ldg(a.weights + nnb::W_RGB + i) : __ldg(a.weights + nnb::W_SIG + (i - 384));
   __syncthreads();
-  if (CL > 1) cluster_sync_all();    // no CTA leaves while a peer may still multicast into it / arrive on its barriers
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+  const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  if (warp >= 8) {   // weight producer (see tc_field_fwd)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
+      uint32_t slot = 0, phase = 0;
+      for (int t = 0; t < my_tiles; ++t)
+        for (int s = 0; s < N_STAGES_T; ++s) {
+          const uint32_t bytes = (uint32_t)c_stages_t[s].nrows * 64u;
+          mbar_wait(bar0 + 8u * (NST + slot), phase ^ 1u);
+          mbar_expect_tx(bar0 + 8u * slot, bytes);
+          bulk_g2s(smem_u32(smem + DG_W + slot * STAGE_BYTES), wimg + c_stages_t[s].img_off, bytes, bar0 + 8u * slot);
+          if (++slot == NST) { slot = 0; phase ^= 1u; }
+        }
+    }
+    return;
   }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int wg = warp >> 2, tl = threadIdx.x & 127;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
+  float* genc = reinterpret_cast<float*>(smem + DG_GENC) + wg * 64 * 64;   // [64 rows][64] encoding gradient; [64][32] g_de before
+  float* gyc = reinterpret_cast<float*>(smem + DG_GYC) + wg * 64 * 4;
+  const uint32_t a_hi = smem_u32(smem + DG_AHI) + wg * 1024, a_lo = smem_u32(smem + DG_ALO) + wg * 1024;
+  const uint32_t w_base = smem_u32(smem + DG_W);
+  const uint32_t bar_id = 1u + (uint32_t)wg;
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
+  uint32_t slot = 0, phase = 0;
+  float acc[128];   // the 32- / 64-wide GEMMs use its first registers (every result is consumed before the next GEMM)
+  // epilogue of a 256-wide layer: x (+ g_s w_sigma) -> ReLU gate of `hmask` -> dY stash -> next A operand (in place)
+  auto epi256 = [&](size_t mt, const float* hmask, float* dst, bool add_sigma) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = r0 + 8 * r;
+      const size_t rowoff = (mt + row) * 256 + c0;
+      const float g_s = add_sigma ? gyc[(row - wg * 64) * 4 + 3] : 0.f;
+      unsigned char* ahi = smem + DG_AHI + row * 16 + c0 * 2;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        float v0 = acc[4 * j + 2 * r], v1 = acc[4 * j + 2 * r + 1];
+        if (add_sigma) { v0 += g_s * s_small[384 + j * 8 + c0]; v1 += g_s * s_small[384 + j * 8 + c0 + 1]; }
+        if (hmask) {
+          const float2 h = __ldg(reinterpret_cast<const float2*>(hmask + rowoff + j * 8));
+          v0 = h.x > 0.f ? v0 : 0.f; v1 = h.y > 0.f ? v1 : 0.f;
+        }
+        if (dst) __stcs(reinterpret_cast<float2*>(dst + rowoff + j * 8), make_float2(v0, v1));
+        uint32_t hw, lw;
+        split2_bf16(v0, v1, hw, lw);
+        *reinterpret_cast<uint32_t*>(ahi + j * 2048) = hw;
+        *reinterpret_cast<uint32_t*>(ahi + DG_ALO + j * 2048) = lw;
+      }
+    }
+    fence_async_smem();
+    wg_sync();
+  };
+  auto epi_enc = [&](bool add) {   // 64-wide encoding gradient -> genc
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float* g = genc + (r0 + 8 * r - wg * 64) * 64 + j * 8 + c0;
+        if (add) { g[0] += acc[4 * j + 2 * r]; g[1] += acc[4 * j + 2 * r + 1]; }
+        else { g[0] = acc[4 * j + 2 * r]; g[1] = acc[4 * j + 2 * r + 1]; }
+      }
+  };
+
+  for (int t = 0; t < my_tiles; ++t) {
+    const int tile = blockIdx.x + t * gridDim.x;
+    const size_t mt = (size_t)tile * TILE;
+    wg_sync();   // the previous tile's encoding adjoint is done with genc
+    if (tl < 64) {   // head adjoints (one thread per row)
+      const size_t m = mt + wg * 64 + tl;
+      const float4 g = (m < M) ? P.gs[m] : make_float4(0.f, 0.f, 0.f, 0.f);
+      const SampleRec rec = P.rec[m];
+      const float g0 = g.x * rec.r * (1.f - rec.r), g1 = g.y * rec.g * (1.f - rec.g), g2 = g.z * rec.b * (1.f - rec.b);
+      const float g3 = g.w * density_act_grad(rec.s, a.flags);
+      if (write_dy) P.dyc[m] = make_float4(g0, g1, g2, g3);
+      gyc[tl * 4] = g0; gyc[tl * 4 + 1] = g1; gyc[tl * 4 + 2] = g2; gyc[tl * 4 + 3] = g3;
+    }
+    wg_sync();
+    {   // g_yr = (g_yc W_rgb) * (hr > 0): thread = row x 64 columns -> A operand (K = 128) + dY stash
+      const int rl = tl & 63, half = tl >> 6, row = wg * 64 + rl;
+      const size_t m = mt + row;
+      const float* g4 = gyc + rl * 4;
+#pragma unroll
+      for (int oc = 0; oc < 8; ++oc) {
+        const int j0 = half * 64 + oc * 8;
+        const float4 ha = __ldg(reinterpret_cast<const float4*>(P.hr + m * 128 + j0));
+        const float4 hb = __ldg(reinterpret_cast<const float4*>(P.hr + m * 128 + j0 + 4));
+        const float hv[8] = {ha.x, ha.y, ha.z, ha.w, hb.x, hb.y, hb.z, hb.w};
+        float v[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float x = g4[0] * s_small[j0 + q] + g4[1] * s_small[128 + j0 + q] + g4[2] * s_small[256 + j0 + q];
+          v[q] = hv[q] > 0.f ? x : 0.f;
+        }
+        if (write_dy) {
+          *reinterpret_cast<float4*>(P.dyr + m * 128 + j0) = make_float4(v[0], v[1], v[2], v[3]);
+          *reinterpret_cast<float4*>(P.dyr + m * 128 + j0 + 4) = make_float4(v[4], v[5], v[6], v[7]);
+        }
+        split_store8_bf16(v, smem + DG_AHI + (j0 >> 3) * 2048 + row * 16, smem + DG_ALO + (j0 >> 3) * 2048 + row * 16);
+      }
+    }
+    fence_async_smem();
+    wg_sync();
+    // g_de (direction-encoding slice of rgb_layers.0) -> view-direction adjoint
+    dg_gemm<32>(acc, a_hi, a_lo, 8, w_base, bar0, slot, phase, tl);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float* g = genc + (r0 + 8 * r - wg * 64) * 32 + j * 8 + c0;
+        g[0] = acc[4 * j + 2 * r]; g[1] = acc[4 * j + 2 * r + 1];
+      }
+    wg_sync();
+    if (tl < 64) {
+      const size_t m = mt + wg * 64 + tl, mm = m < M ? m : M - 1;
+      Ray ray; float z, p[3], v[3], gvd[3];
+      row_geometry_tc(a, m, M, ray, z, p);
+      if (a.pts) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
+      } else {
+        view_dir(a, ray, v);
+      }
+      const float* ge = genc + tl * 32;
+      encode_bwd<4>(v, [&](int k) { return ge[k]; }, gvd);
+      P.gv[m] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
+    }
+    dg_gemm<256>(acc, a_hi, a_lo, 8, w_base, bar0, slot, phase, tl);    // g_feat
+    epi256(mt, nullptr, write_dy ? P.dfeat : nullptr, false);
+    dg_gemm<256>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl);   // g_h7 = g_feat W_feat + g_s w_sigma
+    epi256(mt, P.h[7], write_dy ? P.dy[7] : nullptr, true);
+    for (int l = 7; l >= 1; --l) {
+      if (l == 4) { dg_gemm<64>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl); epi_enc(false); }
+      dg_gemm<256>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl);  // g_h(l-1) = dY_l W_l
+      epi256(mt, P.h[l - 1], write_dy ? P.dy[l - 1] : nullptr, false);
+    }
+    dg_gemm<64>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl);    // encoding gradient of layer 0
+    epi_enc(true);
+    wg_sync();
+    if (tl < 64) {   // encoding adjoint -> d p
+      const size_t m = mt + wg * 64 + tl;
+      Ray ray; float z, p[3], gp[3];
+      row_geometry_tc(a, m, M, ray, z, p);
+      const float* ge = genc + tl * 64;
+      encode_bwd<10>(p, [&](int k) { return ge[k]; }, gp);
+      P.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
+    }
+  }
+}
+
+bool g_stage_table_t_ready = false;
+
+cudaError_t upload_stage_table_t() {
+  if (g_stage_table_t_ready) return cudaSuccess;
+  StageDescT h[N_STAGES_T];
+  int s = 0, off = 0;
+  auto add = [&](int w_off, int ldw, int coloff, int nvalid, int k0, int kvalid, int nrows) {
+    h[s] = StageDescT{w_off, ldw, coloff, nvalid, k0, kvalid, nrows, off};
+    off += nrows * 64; ++s;
+  };
+  for (int i = 0; i < 8; ++i) add(nnb::W_RGBH, 283, 256, 27, 16 * i, 128, 32);
+  for (int i = 0; i < 8; ++i) add(nnb::W_RGBH, 283, 0, 256, 16 * i, 128, 256);
+  for (int i = 0; i < 16; ++i) add(nnb::W_FEAT, 256, 0, 256, 16 * i, 256, 256);
+  for (int l = 7; l >= 1; --l) {
+    if (l == 4) for (int i = 0; i < 16; ++i) add(nnb::w_off(4), 319, 256, 63, 16 * i, 256, 64);
+    for (int i = 0; i < 16; ++i) add(nnb::w_off(l), nnb::w_ld(l), 0, 256, 16 * i, 256, 256);
+  }
+  for (int i = 0; i < 16; ++i) add(nnb::w_off(0), 63, 0, 63, 16 * i, 256, 64);
+  if (s != N_STAGES_T || (size_t)off != IMG_T_BYTES) return cudaErrorInvalidValue;
+  cudaError_t e = cudaMemcpyToSymbol(c_stages_t, h, sizeof(h));
+  if (e == cudaSuccess) g_stage_table_t_ready = true;
+  return e;
+}
+
+// the data-gradient stage of the TC engine's backward (stash layout of nnb_simt.cu)
+cudaError_t tc_dgrad_launch(const nnb_render_bwd_args& b, const WsLayout& L, int write_dy, cudaStream_t st) {
+  const nnb_render_args& a = b.fwd;
+  cudaError_t e = upload_stage_table_t();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_dgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  unsigned char* img = reinterpret_cast<unsigned char*>(base + L.total + align_up(IMG_BYTES, 256));
+  DgPtrs P{};
+  P.rec = reinterpret_cast<const SampleRec*>(base + L.rec);
+  P.gs = reinterpret_cast<const float4*>(base + L.gs); P.gp = reinterpret_cast<float4*>(base + L.gp); P.gv = reinterpret_cast<float4*>(base + L.gv);
+  P.dyc = reinterpret_cast<float4*>(base + L.dyc);
+  for (int l = 0; l < 8; ++l) { P.h[l] = F(L.h[l]); P.dy[l] = F(L.dy[l]); }
+  P.hr = F(L.hr); P.dfeat = F(L.dfeat); P.dyr = F(L.dyr);
+  tc_prep_weights_t<<<N_STAGES_T, 256, 0, st>>>(a.weights, img);
+  const int n_tiles = (int)((L.M + TILE - 1) / TILE);
+  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  tc_dgrad<<<grid, N_THREADS, DG_TOTAL, st>>>(a, (const unsigned char*)img, P, L.M, n_tiles, write_dy);
+  return cudaGetLastError();
 }
 
 bool g_stage_table_ready = false;
@@ -499,19 +729,18 @@ cudaError_t upload_stage_table() {
   if (g_stage_table_ready) return cudaSuccess;
   StageDesc h[N_STAGES];
   int s = 0, off = 0;
-  auto add = [&](int w_off, int ldw, int kcol0, int kvalid, int row0) {
-    h[s].w_off = w_off; h[s].ldw = ldw; h[s].kcol0 = kcol0; h[s].kvalid = kvalid; h[s].row0 = row0; h[s].img_off = off;
-    off += STAGE_BYTES; ++s;
+  auto add = [&](int w_off, int ldw, int kcol0, int kvalid, int nrows) {
+    h[s].w_off = w_off; h[s].ldw = ldw; h[s].kcol0 = kcol0; h[s].kvalid = kvalid; h[s].nrows = nrows; h[s].img_off = off;
+    off += nrows * 64; ++s;
   };
-  // per layer: half 0 (rows 0..127) then half 1 (rows 128..255); inside a half the encoding K-steps (layers 0 and 4) come first
-  for (int hf = 0; hf < 2; ++hf) for (int i = 0; i < 2; ++i) add(nnb::w_off(0), 63, 32 * i, 63, 128 * hf);
-  for (int l = 1; l < 8; ++l)
-    for (int hf = 0; hf < 2; ++hf) {
-      if (l == 4) for (int i = 0; i < 2; ++i) add(nnb::w_off(4), 319, 256 + 32 * i, 319, 128 * hf);
-      for (int i = 0; i < 8; ++i) add(nnb::w_off(l), nnb::w_ld(l), 32 * i, 256, 128 * hf);
-    }
-  for (int hf = 0; hf < 2; ++hf) for (int i = 0; i < 8; ++i) add(nnb::W_FEAT, 256, 32 * i, 256, 128 * hf);
-  for (int i = 0; i < 8; ++i) add(nnb::W_RGBH, 283, 32 * i, 256, 0);
+  // per layer, one stage per K-step of 16; the encoding K-steps (layers 0 and 4) come first
+  for (int i = 0; i < 4; ++i) add(nnb::w_off(0), 63, 16 * i, 63, 256);
+  for (int l = 1; l < 8; ++l) {
+    if (l == 4) for (int i = 0; i < 4; ++i) add(nnb::w_off(4), 319, 256 + 16 * i, 319, 256);
+    for (int i = 0; i < 16; ++i) add(nnb::w_off(l), nnb::w_ld(l), 16 * i, 256, 256);
+  }
+  for (int i = 0; i < 16; ++i) add(nnb::W_FEAT, 256, 16 * i, 256, 256);
+  for (int i = 0; i < 16; ++i) add(nnb::W_RGBH, 283, 16 * i, 256, 128);
   if (s != N_STAGES || (size_t)off != IMG_BYTES) return cudaErrorInvalidValue;
   cudaError_t e = cudaMemcpyToSymbol(c_stages, h, sizeof(h));
   if (e == cudaSuccess) g_stage_table_ready = true;
@@ -520,36 +749,19 @@ cudaError_t upload_stage_table() {
 
 }  // namespace
 
-#ifdef NNB_TC_PROFILE
-extern "C" int nnb_debug_tcprof(unsigned long long* host148x8) {
-  return (int)cudaMemcpyFromSymbol(host148x8, g_tcprof, sizeof(unsigned long long) * 148 * 8);
-}
-extern "C" int nnb_debug_tctrace(unsigned long long* host256) {
-  return (int)cudaMemcpyFromSymbol(host256, g_tctrace, sizeof(unsigned long long) * 256);
-}
-extern "C" int nnb_debug_tcprof2(unsigned long long* host148x8) {
-  return (int)cudaMemcpyFromSymbol(host148x8, g_tcprof2, sizeof(unsigned long long) * 148 * 8);
-}
-#endif
-size_t tc_bwd_workspace_extra();
-cudaError_t tc_render_bwd_planes(const nnb_render_bwd_args& b, const WsLayout& L, size_t img_t_offset, cudaStream_t st);
-
-size_t tc_workspace_extra(int N, int S, uint32_t flags) { return align_up(IMG_BYTES, 256) + tc_bwd_workspace_extra(); }
+size_t tc_workspace_extra(int N, int S, uint32_t flags) { return align_up(IMG_BYTES, 256) + align_up(IMG_T_BYTES, 256); }
 
 bool tc_supports(int S) { return S == 32 || S == 64 || S == 128 || S == 256; }
 
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
   if (!tc_supports(a.S)) return cudaErrorNotSupported;
+  if (a.flags & NNB_TCBWD) return cudaErrorNotSupported;   // the operand-plane stash is not implemented for sm_90a
   cudaError_t e = upload_stage_table();
   if (e != cudaSuccess) return e;
   static bool attr = false;
   static int n_sm = 0;
   if (!attr) {
-    e = cudaFuncSetAttribute(tc_field_fwd<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(tc_field_fwd<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(tc_field_fwd<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    e = cudaFuncSetAttribute(tc_field_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
     if (e != cudaSuccess) return e;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -561,37 +773,27 @@ cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStrea
   TcStash ts{};
   const int stash = (a.flags & NNB_STASH) ? 1 : 0;
   if (stash) {
-    ts.tcb = (a.flags & NNB_TCBWD) ? 1 : 0;
-    ts.wg16 = (ts.tcb && (a.flags & NNB_WG16)) ? 1 : 0;
-    if (ts.tcb) { const char* e = getenv("NNB_DBG_FWD"); if (e) ts.tcb |= atoi(e) << 1; }   // experiment knob (default off)
-    for (int l = 0; l < 8; ++l) ts.h[l] = reinterpret_cast<float*>(base + L.h[l]);   // TCBWD: only h[7] is carved (others unused)
+    for (int l = 0; l < 8; ++l) ts.h[l] = reinterpret_cast<float*>(base + L.h[l]);
     ts.feat = reinterpret_cast<float*>(base + L.feat); ts.hr = reinterpret_cast<float*>(base + L.hr);
     ts.enc = reinterpret_cast<float*>(base + L.enc); ts.denc = reinterpret_cast<float*>(base + L.denc);
-    if (ts.tcb) {
-      for (int i = 0; i < 10; ++i) ts.xp[i] = reinterpret_cast<unsigned char*>(base + L.xp[i]);
-      ts.mask = reinterpret_cast<uint32_t*>(base + L.mask); ts.Mpad = L.Mpad;
-    }
   }
   nnb_prof_mark(st);
-  tc_prep_weights<<<N_STAGES, 256, 0, st>>>(a.weights, img);   // 144 x 16 KB stage images (fp16 hi | lo)
+  tc_prep_weights<<<N_STAGES, 256, 0, st>>>(a.weights, img);   // 152 stage images (fp16 hi | lo)
   nnb_prof_mark(st);
   const int n_tiles = (int)((L.M + TILE - 1) / TILE);
-  const int CL = cluster_size_option();
-  int grid = n_tiles < n_sm ? n_tiles : n_sm;
-  grid = (grid + CL - 1) / CL * CL; if (grid > n_sm) grid = n_sm / CL * CL;
-  if (CL == 4) e = launch_clustered(tc_field_fwd<4>, grid, 448, SM_TOTAL, 4, st, a, (const unsigned char*)img, recs, ts, L.M, n_tiles, stash);
-  else if (CL == 2) e = launch_clustered(tc_field_fwd<2>, grid, 448, SM_TOTAL, 2, st, a, (const unsigned char*)img, recs, ts, L.M, n_tiles, stash);
-  else e = launch_clustered(tc_field_fwd<1>, grid, 448, SM_TOTAL, 1, st, a, (const unsigned char*)img, recs, ts, L.M, n_tiles, stash);
+  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  tc_field_fwd<<<grid, N_THREADS, SM_TOTAL, st>>>(a, (const unsigned char*)img, recs, ts, L.M, n_tiles, stash);
   nnb_prof_mark(st);
+  e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   e = launch_composite_fwd(a, recs, st);
   nnb_prof_mark(st);
   return e;
 }
 
-// Backward of the TC engine: the forward stash has the SIMT engine's layout, so the exact-fp32
-// data/weight-gradient kernels consume it directly (a tcgen05 backward replaces this next).
+// Backward of the TC engine: compositing / ray adjoints of nnb_simt.cu around tc_dgrad and tc_wgrad, which read and write the SIMT
+// engine's fp32 stash layout.  The second phase of a split backward has nothing left to do.
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st) {
-  if (b.fwd.flags & NNB_TCBWD) return tc_render_bwd_planes(b, L, L.total + align_up(IMG_BYTES, 256), st);
-  return b.phase == 2 ? cudaSuccess : simt_render_bwd(b, L, st);
+  if (b.fwd.flags & NNB_TCBWD) return cudaErrorNotSupported;
+  return b.phase == 2 ? cudaSuccess : simt_render_bwd_with(b, L, st, tc_dgrad_launch, tc_wgrad_all);
 }

@@ -1,12 +1,12 @@
-// tcgen05 / mbarrier / bulk-copy PTX wrappers and shared-memory operand helpers shared by the
-// forward (nnb_tc.cu) and backward (nnb_tc_bwd.cu) tensor-core kernels.
+// Hopper (sm_90a) building blocks of the tensor-core engine (nnb_tc.cu): mbarrier / bulk-copy PTX wrappers, the
+// shared-memory matrix descriptor and the asynchronous warpgroup MMA (wgmma) with fp32 accumulators in registers.
 #pragma once
 #include "nnb_workspace.cuh"
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
 
 namespace tcu {
-// ---- PTX wrappers ------------------------------------------------------------------------------
+// ---- mbarrier / bulk copy ---------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
@@ -18,7 +18,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-#ifdef NNB_NO_WAIT_HINT
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
       "WAIT_%=:\n\t"
@@ -27,216 +26,83 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "bra WAIT_%=;\n\t"
       "DONE_%=:\n\t}"
       ::"r"(bar), "r"(parity) : "memory");
-#else
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}"
-      ::"r"(bar), "r"(parity), "r"(0x989680u) : "memory");   // suspend-time hint: sleep in hardware instead of spinning
-#endif
 }
-// non-blocking probe: lets the caller overlap the ~110-cycle barrier round trip with other work
-__device__ __forceinline__ uint32_t mbar_probe(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-               : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok;
-}
-// streaming (evict-first) 16-byte global store: stash / plane traffic must not push the weight images out of L2
-__device__ __forceinline__ void st_stream16(void* p, uint4 v) { __stcs(reinterpret_cast<uint4*>(p), v); }
+// global -> shared bulk copy (no tensor map: the weight images are pre-laid-out contiguous stages), completion on `bar`
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+// ---- wgmma ------------------------------------------------------------------------------------
+// shared-memory matrix descriptor, K-major, no swizzle ("interleave"): 8 x 16 B core matrices; lbo = byte stride between the
+// two core matrices of one K-step (along K), sbo = byte stride between 8-row groups (along M / N)
+__device__ __forceinline__ uint64_t gdesc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32);
 }
-// commit issued by ONE elected lane of a converged warp (the whole MMA warp runs the issue loop, see tc_stage6)
-__device__ __forceinline__ void tc_commit_elect(uint32_t bar) {
-  asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc_elect(uint32_t bar, uint16_t mask) {
-  asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands from shared memory, fp32 accumulators in registers (acc = 0: D = A B^T).
+// Fragment of thread t of the warpgroup: d[4j + 2r + c] = D[16 (t / 32) + (t % 32) / 4 + 8r][8j + 2 (t % 4) + c]
+template <int N> __device__ __forceinline__ void wgmma_f16(float* d, uint64_t da, uint64_t db, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_f16<256>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(acc));
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// issue only: the caller overlaps the load with other work and calls tc_wait_ld() before touching r[]
-__device__ __forceinline__ void tc_ld32_issue(uint32_t taddr, uint32_t* r) {
+template <> __device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// shared-memory matrix descriptor: K-major, no swizzle, version 1 (cute::UMMA::SmemDescriptor)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;   // version = 1 (Blackwell)
-  return d;                 // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
-}
-// instruction descriptor, kind::f16: D fp32, A/B fp16, both K-major (cute::UMMA::InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
 }
 
-// ---- packed fp32x2 arithmetic (Blackwell FADD2 / FMUL2 / FFMA2: two fp32 lanes per issue slot) ----
-__device__ __forceinline__ unsigned long long f2_pack(float a, float b) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ unsigned long long u2_pack(uint32_t a, uint32_t b) { unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(a), "r"(b)); return r; }
-__device__ __forceinline__ void f2_unpack(unsigned long long v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ unsigned long long f2_sub(unsigned long long a, unsigned long long b) {
-  unsigned long long r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-
-// Epilogue of one 32-column accumulator chunk of the forward chain, in ONE pass over the registers:
-//   nx = (-bias) - acc            (packed; `nbias` holds the NEGATED biases, so nx = -(acc + bias) bit for bit)
-//   v  = relu ? max(-nx, 0) : -nx (negation is a free operand modifier)
-//   gate bit = sign(nx)           (x > 0  <=>  nx < 0), shifted into `mw` MSB-first: column j ends up at bit 31 - j
-//   fp16 hi | lo split of v       (x = hi + lo to ~2^-22) as 16 + 16 packed words (column pairs in order, even column in the low
-//                                 half): the next layer's A operand -- the caller stores them to shared memory (core-matrix layout) or
-//                                 to tensor memory (row = lane, two k per column) -- and, with NNB_WG16, hw[] IS the X plane of the
-//                                 weight-gradient pass
-template <bool RELU>
-__device__ __forceinline__ uint32_t epi_chunk32(const uint32_t* r, const float* nbias, float* v, uint32_t* hw, uint32_t* lw, bool want_words,
-                                                bool want_lo = true) {
-  uint32_t mw = 0;
-  const ulonglong2* nb = reinterpret_cast<const ulonglong2*>(nbias);
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {          // 4 columns per step
-    const ulonglong2 b4 = nb[q];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int j = q * 4 + h * 2;
-      const unsigned long long nx2 = f2_sub(h ? b4.y : b4.x, u2_pack(r[j], r[j + 1]));
-      float n0, n1; f2_unpack(nx2, n0, n1);
-      if (RELU) {
-        mw = __funnelshift_l(__float_as_uint(n0), mw, 1); mw = __funnelshift_l(__float_as_uint(n1), mw, 1);
-        v[j] = fmaxf(-n0, 0.f); v[j + 1] = fmaxf(-n1, 0.f);
-      } else { v[j] = -n0; v[j + 1] = -n1; }
-      if (want_words) {
-        __half2 hh = __floats2half2_rn(v[j], v[j + 1]);
-        hw[j >> 1] = *reinterpret_cast<uint32_t*>(&hh);
-        if (want_lo) {
-          const float2 hf = __half22float2(hh);
-          float l0, l1; f2_unpack(f2_sub(f2_pack(v[j], v[j + 1]), f2_pack(hf.x, hf.y)), l0, l1);
-          __half2 ll = __floats2half2_rn(l0, l1);
-          lw[j >> 1] = *reinterpret_cast<uint32_t*>(&ll);
-        }
-      }
-    }
-  }
-  return mw;
-}
-// the 16 + 16 operand words of a chunk -> shared memory, canonical no-swizzle K-major core matrices (8 x 16 B per half)
-__device__ __forceinline__ void store_words_smem(const uint32_t* hw, const uint32_t* lw, unsigned char* hi_dst, unsigned char* lo_dst) {
-#pragma unroll
-  for (int kb = 0; kb < 4; ++kb) {
-    *reinterpret_cast<uint4*>(hi_dst + kb * 2048) = make_uint4(hw[kb * 4], hw[kb * 4 + 1], hw[kb * 4 + 2], hw[kb * 4 + 3]);
-    *reinterpret_cast<uint4*>(lo_dst + kb * 2048) = make_uint4(lw[kb * 4], lw[kb * 4 + 1], lw[kb * 4 + 2], lw[kb * 4 + 3]);
-  }
-}
-// ... or -> tensor memory (A operand of the .ts MMA form): lane = sample row, column c holds k = 2c, 2c + 1
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t* r) {
+// the same with bf16 operands (gradients: full fp32 exponent range)
+template <int N> __device__ __forceinline__ void wgmma_bf16(float* d, uint64_t da, uint64_t db, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_bf16<256>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(acc));
 }
-__device__ __forceinline__ void tc_st4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
 }
-// bf16 hi | lo split of 8 values as 4 + 4 packed words (even element in the low half)
-__device__ __forceinline__ void split8_bf16_words(const float* v, uint32_t* hw, uint32_t* lw) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-    const uint32_t hb = *reinterpret_cast<uint32_t*>(&hh);
-    float l0, l1;
-    f2_unpack(f2_sub(f2_pack(v[2 * i], v[2 * i + 1]), u2_pack(hb << 16, hb & 0xffff0000u)), l0, l1);   // bf16 -> f32 is a shift
-    __nv_bfloat162 ll = __floats2bfloat162_rn(l0, l1);
-    hw[i] = hb; lw[i] = *reinterpret_cast<uint32_t*>(&ll);
-  }
+
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(acc));
 }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// fp16 (saturating) of 8 values times a power-of-two scale, streamed to global memory: one plane of a NNB_WG16 dY operand
-__device__ __forceinline__ uint32_t pack_half2_sat(float lo, float hi) {
-  uint32_t d; asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo)); return d;
-}
-__device__ __forceinline__ unsigned long long f2_mul(unsigned long long a, unsigned long long b) {
-  unsigned long long r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ void stream8_f16_scaled(const float* v, float scale, unsigned char* dst) {
-  const unsigned long long s2 = f2_pack(scale, scale);
-  uint32_t w[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { float a, b; f2_unpack(f2_mul(f2_pack(v[2 * i], v[2 * i + 1]), s2), a, b); w[i] = pack_half2_sat(a, b); }   // packed FMUL2
-  st_stream16(dst, make_uint4(w[0], w[1], w[2], w[3]));
-}
-// bf16 hi (and optionally lo) operand plane of 8 values, streamed to global memory
-__device__ __forceinline__ void plane_stream8_bf16(const float* v, unsigned char* hi_dst, unsigned char* lo_dst, bool with_lo) {
+// split 8 fp32 values into hi / lo bf16 halves (x = hi + lo to ~2^-17, full fp32 exponent range) and store 16 B each
+__device__ __forceinline__ void split_store8_bf16(const float* v, unsigned char* hi_dst, unsigned char* lo_dst) {
   uint32_t hi[4], lo[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
     const uint32_t hb = *reinterpret_cast<uint32_t*>(&hh);
-    hi[i] = hb;
-    if (with_lo) {
-      float l0, l1;
-      f2_unpack(f2_sub(f2_pack(v[2 * i], v[2 * i + 1]), u2_pack(hb << 16, hb & 0xffff0000u)), l0, l1);   // bf16 -> f32 is a shift
-      __nv_bfloat162 ll = __floats2bfloat162_rn(l0, l1);
-      lo[i] = *reinterpret_cast<uint32_t*>(&ll);
-    }
-  }
-  st_stream16(hi_dst, make_uint4(hi[0], hi[1], hi[2], hi[3]));
-  if (with_lo) st_stream16(lo_dst, make_uint4(lo[0], lo[1], lo[2], lo[3]));
-}
-
-// split 8 fp32 values into hi / lo fp16 halves (x = hi + lo to ~2^-22) and store 16 B each
-__device__ __forceinline__ void split_store8(const float* v, unsigned char* hi_dst, unsigned char* lo_dst) {
-  uint32_t hi[4], lo[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    __half2 hh = __floats2half2_rn(v[2 * i], v[2 * i + 1]);        // one F2FP per pair
-    float2 hf = __half22float2(hh);
-    __half2 ll = __floats2half2_rn(v[2 * i] - hf.x, v[2 * i + 1] - hf.y);
-    hi[i] = *reinterpret_cast<uint32_t*>(&hh);
-    lo[i] = *reinterpret_cast<uint32_t*>(&ll);
+    const float h0 = __uint_as_float(hb << 16), h1 = __uint_as_float(hb & 0xffff0000u);   // bf16 -> f32 is a shift
+    __nv_bfloat162 ll = __floats2bfloat162_rn(v[2 * i] - h0, v[2 * i + 1] - h1);
+    hi[i] = hb; lo[i] = *reinterpret_cast<uint32_t*>(&ll);
   }
   *reinterpret_cast<uint4*>(hi_dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   *reinterpret_cast<uint4*>(lo_dst) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
-
-// same, and hands back the four packed hi words (NNB_WG16: the encoding's X plane is the hi half of the E operand)
-__device__ __forceinline__ uint4 split_store8_hi(const float* v, unsigned char* hi_dst, unsigned char* lo_dst) {
+// split 8 fp32 values into hi / lo fp16 halves (x = hi + lo to ~2^-22) and store 16 B each
+__device__ __forceinline__ void split_store8(const float* v, unsigned char* hi_dst, unsigned char* lo_dst) {
   uint32_t hi[4], lo[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -246,181 +112,14 @@ __device__ __forceinline__ uint4 split_store8_hi(const float* v, unsigned char* 
     hi[i] = *reinterpret_cast<uint32_t*>(&hh);
     lo[i] = *reinterpret_cast<uint32_t*>(&ll);
   }
-  const uint4 H = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-  *reinterpret_cast<uint4*>(hi_dst) = H;
-  *reinterpret_cast<uint4*>(lo_dst) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-  return H;
-}
-
-// bf16 hi/lo split (x = hi + lo to ~2^-17, full fp32 exponent range): used for GRADIENT operands, whose
-// magnitudes decay by orders of magnitude along the backward chain (fp16 would run into subnormals)
-__device__ __forceinline__ void split_store8_bf16(const float* v, unsigned char* hi_dst, unsigned char* lo_dst) {
-  uint32_t hi[4], lo[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-    const uint32_t hb = *reinterpret_cast<uint32_t*>(&hh);
-    const float h0 = __uint_as_float(hb << 16), h1 = __uint_as_float(hb & 0xffff0000u);   // bf16 -> f32 is a shift
-    __nv_bfloat162 ll = __floats2bfloat162_rn(v[2 * i] - h0, v[2 * i + 1] - h1);
-    hi[i] = hb;
-    lo[i] = *reinterpret_cast<uint32_t*>(&ll);
-  }
   *reinterpret_cast<uint4*>(hi_dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   *reinterpret_cast<uint4*>(lo_dst) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
-__device__ __forceinline__ void split_stream8_bf16(const float* v, unsigned char* hi_dst, unsigned char* lo_dst) {
-  uint32_t hi[4], lo[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-    const uint32_t hb = *reinterpret_cast<uint32_t*>(&hh);
-    const float h0 = __uint_as_float(hb << 16), h1 = __uint_as_float(hb & 0xffff0000u);
-    __nv_bfloat162 ll = __floats2bfloat162_rn(v[2 * i] - h0, v[2 * i + 1] - h1);
-    hi[i] = hb;
-    lo[i] = *reinterpret_cast<uint32_t*>(&ll);
-  }
-  st_stream16(hi_dst, make_uint4(hi[0], hi[1], hi[2], hi[3]));
-  st_stream16(lo_dst, make_uint4(lo[0], lo[1], lo[2], lo[3]));
+// same for one pair: the two packed words (even element in the low half)
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  __half2 hh = __floats2half2_rn(a, b);
+  const float2 hf = __half22float2(hh);
+  __half2 ll = __floats2half2_rn(a - hf.x, b - hf.y);
+  hi = *reinterpret_cast<uint32_t*>(&hh); lo = *reinterpret_cast<uint32_t*>(&ll);
 }
-// instruction descriptor with explicit operand formats (0 = fp16, 1 = bf16) and major-ness (0 = K, 1 = MN)
-__host__ __device__ constexpr uint32_t make_idesc_ex(int M, int N, int afmt, int bfmt, int amaj, int bmaj) {
-  return (1u << 4) | ((uint32_t)afmt << 7) | ((uint32_t)bfmt << 10) | ((uint32_t)amaj << 15) | ((uint32_t)bmaj << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// MN-major, no swizzle (cute::UMMA canonical "INTERLEAVE" MN layout): lbo = byte stride between core
-// matrices along K (the reduction), sbo = byte stride between 8-element groups along M/N.
-__host__ __device__ constexpr uint32_t make_idesc_mn(int M, int N) {   // both operands MN-major
-  return (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// ---- thread-block clusters: weight stages are fetched from L2 once per cluster and multicast to every CTA ----
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_g2s_mc(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"(mask) : "memory");
-}
-// ---- lean issue path -------------------------------------------------------------------------------------------------
-// One thread issues every MMA of a CTA; measured (tools/micro/mma_commit.cu) it sustains one tcgen05.mma per ~64 cycles only if
-// almost nothing else runs between them: building eight 64-bit descriptors per stage with shifts and masks made the issue loop,
-// not the tensor pipe, the bottleneck (130-190 cycles per MMA).  All operands here use LBO = 2048 B, SBO = 128 B, version 1, so
-// a descriptor is {low word = (addr >> 4) | (128 << 16), high word = DESC_HI}: the thread only ADDS to precomputed low words.
-constexpr uint32_t DESC_HI = 8u | (1u << 14);
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (128u << 16); }
-// Two K-steps of one 128-column half against one 16 KB weight stage ([hi: K-step 0 | K-step 1][lo: K-step 0 | K-step 1], 4096 B each):
-// probe of the next stage's barrier, six MMAs, release of the stage; the second K-step's operands are +256 descriptor units (A in
-// shared memory) or +8 tensor-memory columns (A in tensor memory, TS = true).
-// MODE (forward-precision experiment, NNB_FWD_DROP_*): 0 = the three-term split; 1 = without a_hi*b_lo (weights rounded to one fp16);
-// 2 = without a_lo*b_hi (activations rounded to one fp16); 3 = a_hi*b_hi only.  PA / PB are the predicates of the a_lo*b_hi /
-// a_hi*b_lo MMAs ("e" = the elected lane, "n" = never), ACCB / ACCC the accumulate predicates of the first a_hi*b_lo / a_hi*b_hi MMA.
-#define NNB_STAGE6_SS(PA, PB, ACCB, ACCC)                                                                                        \
-        "{\n\t.reg .pred p, q, t, e, n, ct, cm;\n\t.reg .b32 x;\n\t.reg .b64 al0, ah0, al1, ah1, bh0, bl0, bh1, bl1;\n\t"           \
-        "mbarrier.try_wait.parity.shared::cta.b64 q, [%8], %9;\n\t"                                                             \
-        "setp.ne.b32 p, %6, 0;\n\t"                                                                                             \
-        "setp.eq.u32 t, 0, 0;\n\t"                                                                                              \
-        "setp.ne.u32 n, 0, 0;\n\t"                                                                                              \
-        "elect.sync _|e, 0xffffffff;\n\t"                                                                                       \
-        "mov.b64 al0, {%2, %11};\n\t mov.b64 ah0, {%3, %11};\n\t"                                                               \
-        "add.u32 x, %2, 256;\n\t mov.b64 al1, {x, %11};\n\t add.u32 x, %3, 256;\n\t mov.b64 ah1, {x, %11};\n\t"                 \
-        "mov.b64 bh0, {%4, %11};\n\t add.u32 x, %4, %13;\n\t mov.b64 bh1, {x, %11};\n\t"                                        \
-        "add.u32 x, x, %13;\n\t mov.b64 bl0, {x, %11};\n\t add.u32 x, x, %13;\n\t mov.b64 bl1, {x, %11};\n\t"                   \
-        "@" PA " tcgen05.mma.cta_group::1.kind::f16 [%1], al0, bh0, %5, p;\n\t"                                                 \
-        "@" PB " tcgen05.mma.cta_group::1.kind::f16 [%1], ah0, bl0, %5, " ACCB ";\n\t"                                          \
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%1], ah0, bh0, %5, " ACCC ";\n\t"                                               \
-        "@" PA " tcgen05.mma.cta_group::1.kind::f16 [%1], al1, bh1, %5, t;\n\t"                                                 \
-        "@" PB " tcgen05.mma.cta_group::1.kind::f16 [%1], ah1, bl1, %5, t;\n\t"                                                 \
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%1], ah1, bh1, %5, t;\n\t"                                                      \
-        "setp.eq.u32 t, %12, 1;\n\t"                                                                                            \
-        "and.pred ct, e, t;\n\t"                                                                                                \
-        "not.pred t, t;\n\t"                                                                                                    \
-        "and.pred cm, e, t;\n\t"                                                                                                \
-        "@ct tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%7];\n\t"                                   \
-        "@cm tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%7], %10;\n\t"           \
-        "selp.u32 %0, 1, 0, q;\n\t}"
-#define NNB_STAGE6_TS(PA, PB, ACCB, ACCC)                                                                                        \
-        "{\n\t.reg .pred p, q, t, e, n, ct, cm;\n\t.reg .b32 x, al1, ah1;\n\t.reg .b64 bh0, bl0, bh1, bl1;\n\t"                   \
-        "mbarrier.try_wait.parity.shared::cta.b64 q, [%8], %9;\n\t"                                                             \
-        "setp.ne.b32 p, %6, 0;\n\t"                                                                                             \
-        "setp.eq.u32 t, 0, 0;\n\t"                                                                                              \
-        "setp.ne.u32 n, 0, 0;\n\t"                                                                                              \
-        "elect.sync _|e, 0xffffffff;\n\t"                                                                                       \
-        "add.u32 al1, %2, 8;\n\t add.u32 ah1, %3, 8;\n\t"                                                                       \
-        "mov.b64 bh0, {%4, %11};\n\t add.u32 x, %4, %13;\n\t mov.b64 bh1, {x, %11};\n\t"                                        \
-        "add.u32 x, x, %13;\n\t mov.b64 bl0, {x, %11};\n\t add.u32 x, x, %13;\n\t mov.b64 bl1, {x, %11};\n\t"                   \
-        "@" PA " tcgen05.mma.cta_group::1.kind::f16 [%1], [%2], bh0, %5, p;\n\t"                                                \
-        "@" PB " tcgen05.mma.cta_group::1.kind::f16 [%1], [%3], bl0, %5, " ACCB ";\n\t"                                         \
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%1], [%3], bh0, %5, " ACCC ";\n\t"                                              \
-        "@" PA " tcgen05.mma.cta_group::1.kind::f16 [%1], [al1], bh1, %5, t;\n\t"                                               \
-        "@" PB " tcgen05.mma.cta_group::1.kind::f16 [%1], [ah1], bl1, %5, t;\n\t"                                               \
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%1], [ah1], bh1, %5, t;\n\t"                                                    \
-        "setp.eq.u32 t, %12, 1;\n\t"                                                                                            \
-        "and.pred ct, e, t;\n\t"                                                                                                \
-        "not.pred t, t;\n\t"                                                                                                    \
-        "and.pred cm, e, t;\n\t"                                                                                                \
-        "@ct tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%7];\n\t"                                   \
-        "@cm tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%7], %10;\n\t"           \
-        "selp.u32 %0, 1, 0, q;\n\t}"
-#define NNB_STAGE6_OPERANDS                                                                                                      \
-        : "=r"(ok)                                                                                                              \
-        : "r"(d_tmem), "r"(aL), "r"(aH), "r"(wb), "r"(idesc), "r"(acc), "r"(empty_bar), "r"(next_full_bar), "r"(next_parity), "h"(cmask), \
-          "r"(DESC_HI), "r"((uint32_t)CL), "r"(b_ks)                                                                            \
-        : "memory"
-template <int CL, bool TS, int MODE = 0>
-__device__ __forceinline__ uint32_t tc_stage6(uint32_t d_tmem, uint32_t aL, uint32_t aH, uint32_t wb, uint32_t b_ks, uint32_t idesc, uint32_t acc, uint32_t empty_bar,
-                                              uint16_t cmask, uint32_t next_full_bar, uint32_t next_parity) {
-  uint32_t ok;
-  if (!TS) {
-    if (MODE == 0) asm volatile(NNB_STAGE6_SS("e", "e", "t", "t") NNB_STAGE6_OPERANDS);
-    else if (MODE == 1) asm volatile(NNB_STAGE6_SS("e", "n", "t", "t") NNB_STAGE6_OPERANDS);
-    else if (MODE == 2) asm volatile(NNB_STAGE6_SS("n", "e", "p", "t") NNB_STAGE6_OPERANDS);
-    else asm volatile(NNB_STAGE6_SS("n", "n", "t", "p") NNB_STAGE6_OPERANDS);
-  } else {
-    if (MODE == 0) asm volatile(NNB_STAGE6_TS("e", "e", "t", "t") NNB_STAGE6_OPERANDS);
-    else if (MODE == 1) asm volatile(NNB_STAGE6_TS("e", "n", "t", "t") NNB_STAGE6_OPERANDS);
-    else if (MODE == 2) asm volatile(NNB_STAGE6_TS("n", "e", "p", "t") NNB_STAGE6_OPERANDS);
-    else asm volatile(NNB_STAGE6_TS("n", "n", "t", "p") NNB_STAGE6_OPERANDS);
-  }
-  return ok;
-}
-// runtime selection of the split (warp-uniform mode): the default mode keeps its own straight-line copy
-template <int CL, bool TS>
-__device__ __forceinline__ uint32_t tc_stage6_sel(uint32_t mode, uint32_t d_tmem, uint32_t aL, uint32_t aH, uint32_t wb, uint32_t b_ks, uint32_t idesc, uint32_t acc,
-                                                  uint32_t empty_bar, uint16_t cmask, uint32_t next_full_bar, uint32_t next_parity) {
-  if (mode == 1u) return tc_stage6<CL, TS, 1>(d_tmem, aL, aH, wb, b_ks, idesc, acc, empty_bar, cmask, next_full_bar, next_parity);
-  if (mode == 2u) return tc_stage6<CL, TS, 2>(d_tmem, aL, aH, wb, b_ks, idesc, acc, empty_bar, cmask, next_full_bar, next_parity);
-  return tc_stage6<CL, TS, 3>(d_tmem, aL, aH, wb, b_ks, idesc, acc, empty_bar, cmask, next_full_bar, next_parity);
-}
-// single MMA from descriptor LOW words (high word shared), issued by the elect.sync lane of a converged warp
-__device__ __forceinline__ void tc_mma_lo_elect(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\t.reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "mov.b64 da, {%1, %3};\n\t mov.b64 db, {%2, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the 8 epilogue warps
-}  // namespace tcu
-
-#include <cstdlib>
-namespace tcu {
-template <typename K, typename... Args>
-cudaError_t launch_clustered(K kernel, int grid, int block, size_t smem, int cluster, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = cluster > 1 ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, args...);
-}
-
-inline int cluster_size_option() {
-  static int c = -1;
-  if (c < 0) { const char* e = getenv("NNB_CLUSTER"); c = e ? atoi(e) : 2; if (c != 1 && c != 2 && c != 4) c = 2; }
-  return c;
-}
-
 }  // namespace tcu

@@ -9,12 +9,14 @@ struct WsLayout {
   size_t gs;    // float4[Mpad]  d/d(rgb_i, a_i) from compositing adjoint
   size_t gp;    // float4[Mpad]  d/d p_i
   size_t gv;    // float4[Mpad]  d/d viewdir_i
+  // fixed-order reductions (no float atomics: a step's gradients are the same bits on every run)
+  size_t rayred;   // float[N][16]  per-ray pose / intrinsics / scale-shift adjoints, summed over rays by ray_reduce
+  size_t wpart;    // float[]       per-sample-split partial weight gradients, summed over the splits by wgrad_reduce
   // SIMT engine activation stash (fp32, [sample][feature])
   size_t h[8], feat, hr, enc, denc;
   size_t dy[8], dfeat, dyr, dyc;
-  // tcgen05 backward (NNB_TCBWD): activations / output-gradients as per-tile bf16 hi|lo operand planes
-  // ([tile][hi|lo][sample half][feature/8][64 samples][8 features]: every 64-sample half of a plane is one contiguous
-  // bulk copy for tc_wgrad and an MN-major tcgen05 operand as it lands) + ReLU bitmasks
+  // operand-plane backward (NNB_TCBWD; rejected by the sm_90a library): activations / output-gradients as per-tile bf16 hi|lo
+  // operand planes ([tile][hi|lo][sample half][feature/8][64 samples][8 features]) + ReLU bitmasks
   size_t n_tiles;
   size_t xp[10];    // X planes: 0 = enc (64 feat), 1..8 = h0..h7, 9 = feat
   size_t dyp[10];   // dY planes: 0..7 = dy0..dy7, 8 = dfeat, 9 = dyr (128 feat)
@@ -25,10 +27,31 @@ struct WsLayout {
 };
 constexpr size_t PLANE_TILE_256 = 131072, PLANE_TILE_128 = 65536, PLANE_TILE_64 = 32768;
 
+// weight-gradient stage of a backward that consumes the fp32 stash: accumulates every MLP parameter gradient into gw
+typedef cudaError_t (*WgradFn)(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
+// data-gradient stage of such a backward: head adjoints, the chain through the MLP (dY stash when write_dy), d p and d viewdir
+typedef cudaError_t (*DgradFn)(const nnb_render_bwd_args& b, const WsLayout& L, int write_dy, cudaStream_t st);
+
 // job of the fp32 SIMT weight-gradient kernel: dW[n][k] += sum_m dY[m*ldy+n] X[m*ldx+k]
 struct SmallJob { const float* dY; const float* X; float* dW; float* db; int ldy, Nn, ldx, Kk, ldw; };
 
 __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// sample splits of the weight-gradient kernels (each split writes its own partial dW, see wgrad_reduce)
+inline int simt_wgrad_msplit(size_t M) { int m = (int)((M + 4095) / 4096); return m < 1 ? 1 : (m > 16 ? 16 : m); }
+inline int jobs_wgrad_msplit(size_t M) { int m = (int)((M + 2047) / 2048); return m < 1 ? 1 : (m > 64 ? 64 : m); }
+constexpr size_t WPART_PAD = 16 * 512;   // bias slots of every job (up to two per output row)
+inline size_t wpart_floats(size_t M) {
+  const size_t a = (size_t)simt_wgrad_msplit(M) * (NNB_NUM_PARAMS + WPART_PAD);
+  const size_t b = (size_t)8 * (NNB_NUM_PARAMS + WPART_PAD);    // tc_wgrad: <= 8 splits of the 256-wide jobs, 32 of the encoding jobs
+  const size_t c = (size_t)jobs_wgrad_msplit(M) * 8192;         // small SIMT jobs
+  return a > b ? (a > c ? a : c) : (b > c ? b : c);
+}
+
+// one weight-gradient job's partials: split y writes part[off + y * stride + e], e < Nn * Kk the dW element (n * Kk + k),
+// then `dbslots` x Nn bias partials; wgrad_reduce adds sum_y (and sum over the slots) to dW[n * ldw + k] / db[n] in a fixed order
+struct RedJob { float* dW; float* db; int Nn, Kk, ldw, nsplit, dbslots; size_t off, stride; };
+cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st);
 
 inline WsLayout make_layout(int N, int S, uint32_t flags, int engine) {
   WsLayout L{};
@@ -39,6 +62,7 @@ inline WsLayout make_layout(int N, int S, uint32_t flags, int engine) {
   L.rec = take(L.Mpad * sizeof(SampleRec));
   if (flags & NNB_STASH) {
     L.gs = take(L.Mpad * 16); L.gp = take(L.Mpad * 16); L.gv = take(L.Mpad * 16);
+    L.rayred = take((size_t)N * 16 * 4); L.wpart = take(wpart_floats(L.M) * 4);
     L.n_tiles = L.Mpad / 128;
     if (engine == NNB_ENGINE_TC && (flags & NNB_TCBWD)) {
       // small fp32 side stashes (heads) + operand planes

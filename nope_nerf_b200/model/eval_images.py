@@ -1,6 +1,6 @@
 """Eval_Images (reference: model/eval_images.py:16-137): novel-view evaluation of one test frame — render, PSNR / SSIM / LPIPS,
 depth statistics inputs, image dumps.  The reference walks the frame in `points_batch_size` chunks through Renderer.forward
-(eval_images.py:73-84); here the frame is ONE library call (Extract_Images.render_frame -> the persistent tcgen05 forward) and MSE,
+(eval_images.py:73-84); here the frame is ONE library call (Extract_Images.render_frame -> the persistent tensor-core forward) and MSE,
 PSNR and SSIM are computed on the device from the rendered frame (the reference's third_party/pytorch_ssim formula: 11x11
 Gaussian window, sigma 1.5, zero padding, mean over the map).  LPIPS stays the caller's network (`lpips_vgg_fn`, eval_nvs.py)."""
 import os

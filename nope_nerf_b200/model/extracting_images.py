@@ -1,7 +1,7 @@
 """Extract_Images (reference: model/extracting_images.py:13-124): full-frame novel-view rendering, the caller of
 BASELINE config 4.  The reference splits a frame into 100 000-ray chunks x 64 000-sample MLP chunks (~4 200 Python-loop
 iterations per 1080p frame); here one frame (or one row block of it, for ray-sharded multi-GPU rendering) is ONE library
-call — the persistent tcgen05 kernel walks all 128-sample tiles itself.  File output is plain numpy / PIL."""
+call — the persistent tensor-core kernel walks all 128-sample tiles itself.  File output is plain numpy / PIL."""
 import os
 import numpy as np
 import torch

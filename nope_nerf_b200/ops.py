@@ -6,13 +6,15 @@ import torch
 from . import _lib as L
 
 _DEFAULT_ENGINE = [L.ENGINE_TC]
-_TC_BACKWARD = [True]     # tcgen05 backward (operand-plane stash); False -> fp32 SIMT backward after a TC forward
-# weight-gradient operand planes of the tcgen05 backward: 'fp16' = one fp16 plane per operand, per-layer power-of-two dY scales
+# operand-plane backward of the tensor-core engine (NNB_TCBWD): not implemented for sm_90a (the library rejects the flag); a TC
+# forward stashes fp32 activations, which the TC backward's wgmma data- / weight-gradient kernels read
+_TC_BACKWARD = [False]
+# weight-gradient operand planes of the operand-plane backward: 'fp16' = one fp16 plane per operand, per-layer power-of-two dY scales
 # from the previous step (NNB_WG16: half the stash traffic, a third of the MMAs, MLP weight gradients to ~3e-4);
 # 'exact' = bf16 hi|lo planes, three MMAs per product (MLP weight gradients to fp32 round-off).  NNB_WGRAD overrides.
 import os as _os
 _WGRAD = [_os.environ.get("NNB_WGRAD", "fp16")]
-# forward-precision EXPERIMENT of the tcgen05 engine (DESIGN.md section 4; never the default): 0 = three-term split, 1 = without
+# forward-precision EXPERIMENT of the tensor-core engine (DESIGN.md section 4; never the default): 0 = three-term split, 1 = without
 # a_hi*b_lo (NNB_FWD_DROP_WLO), 2 = without a_lo*b_hi (NNB_FWD_DROP_ALO), 3 = a_hi*b_hi only
 _FWD_DROP = [int(_os.environ.get("NNB_FWD_DROP", "0"))]
 
@@ -47,7 +49,7 @@ def default_engine():
 
 
 def pick_engine(engine, S):
-    """the tcgen05 engine tiles 128 samples per CTA and needs S in {32,64,128,256}; other sample counts
+    """the tensor-core engine tiles 128 samples per CTA and needs S in {32,64,128,256}; other sample counts
     run on the exact-fp32 SIMT engine (still CUDA; there is no CPU path)."""
     if engine is None:
         engine = _DEFAULT_ENGINE[0]
@@ -166,7 +168,7 @@ class RenderCall:
     def backward(self, g_rgb, g_depth_pred, g_depth_gt, g_weights, g_c2w, g_cam=None, g_depth=None, g_scale_shift=None, phase=0,
                  wg_state=None, wg_seed=False):
         """all outputs are accumulated into (caller-zeroed) buffers; g_weights may be None (pose only).  phase 1 / 2: the two halves
-        of the tcgen05 backward (data gradients | weight gradients + ray adjoint), see include/nope_nerf_b200.h.  wg_state: the
+        of the backward (data gradients | weight gradients + ray adjoint), see include/nope_nerf_b200.h.  wg_state: the
         caller's persistent 32-float dY-scale state of the fp16 weight-gradient planes (None: stateless, seeded per call)."""
         if self.ws is None:
             raise RuntimeError("backward called without a stashed forward")

@@ -9,7 +9,7 @@ and fails loudly when its CUDA library is missing.
 Parity status: PINNED.  The reference ships no tests or golden vectors
 (SURVEY.md section 4), so the oracle is pinned against outputs of the reference
 itself: ``tools/make_golden.py`` imports the unmodified reference from
-``/root/reference`` in the build container, runs it (torch CPU, fp32, autograd)
+a reference checkout, runs it (torch CPU, fp32, autograd)
 on seeded inputs and commits inputs/outputs/gradients under ``tests/golden/``;
 ``tests/test_oracle_golden.py`` checks this restatement against those fixtures.
 

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE — imports the UNMODIFIED reference from oracle/_ref/ (tools/vendor_ref.py) and builds its own
+"""TEST INFRASTRUCTURE — imports the UNMODIFIED reference from oracle/_ref/ (oracle/vendor_ref.py) and builds its own
 Trainer so that tests/, bench.py's reference arm and tools/psnr_parity.py can run the reference itself (CPU or cuda)
 beside the CUDA path.  Nothing under nope_nerf_b200/ imports this module.
 
@@ -58,7 +58,7 @@ def import_reference(device="cpu"):
     """returns the reference's `model` package (imported from oracle/_ref)"""
     import torch
     if not available():
-        raise RuntimeError("oracle/_ref is missing: run `python tools/vendor_ref.py` in the build container")
+        raise RuntimeError("oracle/_ref is missing: run `python oracle/vendor_ref.py` beside a reference checkout")
     install_stubs()
     if REF not in sys.path:
         sys.path.insert(0, REF)

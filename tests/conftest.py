@@ -7,7 +7,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     # the CUDA library is a build artefact (git-ignored): compile it when the tree is fresh, so the host-side tests that load
     # it (symbol exports, module mirrors) and the GPU tests never depend on an earlier manual build
     lib = os.path.join(ROOT, "nope_nerf_b200", "libnope_nerf_b200.so")

@@ -1,32 +1,35 @@
-"""Full-size parity against the LIVE reference on cuda (oracle/_ref = an unmodified copy of the reference tree, made by
-tools/vendor_ref.py; it ships to the GPU box like the built .so).  BASELINE.json's configs at their REAL sizes:
+"""Full-size parity against the reference on cuda, through its stored results (tests/golden/fullsize_*.npz, written by
+tools/make_golden_fullsize.py from the UNMODIFIED reference run on cuda).  BASELINE.json's configs at their REAL sizes:
 
   C2  1080x1920, DPT 384x672, V=200, 1024 rays x 128 samples, uniform + jitter, rgb L1 + depth L1            (+ full loss set)
   C3  756x1008,  DPT 384x512, V=20,  1024 rays x 128 samples, NDC + dist_alpha, depth loss on 1 - 1/d
   C5  1080x1920, 4096 rays x 128 samples (one rank's view of the 8-view batch), full loss set
 
-Both sides start from the same parameters (the reference's own torch init under a fixed seed), see the same frame pair, the
-same `ray_idx` (torch.randperm is patched to return a stored draw) and the same jitter (torch.rand likewise), and run ONE
-Trainer.train_step.  Compared: every loss scalar, the pose / distortion / MLP gradients the step leaves in .grad, and the rendered
-rgb / depth of a forward-only call.  The gradient gate is max(1e-4, 3 x envelope), envelope = |reference fp32 - reference fp64|
-(the reference itself re-run in float64 on the same inputs = its own rounding, dominated by ReLU-gate switches, see
-tests/test_oracle_golden.py::test_render_gate_matched_and_kxy)."""
+Both sides start from the same parameters (the reference's own torch init under a fixed seed, tests/_fullsize_cases.py), see the
+same frame pair, the same `ray_idx` (torch.randperm is patched to return a stored draw) and the same jitter (torch.rand likewise),
+and run ONE Trainer.train_step.  Compared: every loss scalar, the pose / distortion gradients the step leaves in .grad, a fixed
+seeded sample of the MLP gradient, and the rendered rgb / depth of a forward-only call.  The gradient gate is max(1e-4, 3 x
+envelope), envelope = |reference fp32 - reference fp64| (the reference itself re-run in float64 on the same inputs = its own
+rounding, dominated by ReLU-gate switches, see tests/test_oracle_golden.py::test_render_gate_matched_and_kxy)."""
 import os
-import sys
+
 import numpy as np
 import pytest
 import torch
 
 from _util import ROOT
+import _fullsize_cases as FC
 
 pytestmark = pytest.mark.gpu
-sys.path.insert(0, ROOT)
-from oracle import ref_harness as RH  # noqa: E402
-
-if not RH.available():
-    pytest.skip("oracle/_ref missing (run tools/vendor_ref.py in the build container)", allow_module_level=True)
-
+GOLDEN = os.path.join(ROOT, "tests", "golden")
 REPORT = {}
+
+
+def _golden(name, state=None):
+    g = dict(np.load(os.path.join(GOLDEN, "fullsize_%s.npz" % name)))
+    if state is not None:   # the stored results belong to this starting state
+        assert abs(FC.state_digest(state) - float(g["digest"])) <= 1e-9 * max(1.0, abs(float(g["digest"]))), name
+    return g
 
 
 def _report(key, **vals):
@@ -38,50 +41,13 @@ def _report(key, **vals):
 
 
 def rel(a, b):
-    a = a.detach().double().reshape(-1); b = b.detach().double().reshape(-1)
+    a = torch.as_tensor(a).detach().double().reshape(-1).cpu(); b = torch.as_tensor(b).detach().double().reshape(-1).cpu()
     return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
 
 
 def cosine(a, b):
-    a = a.detach().double().reshape(-1); b = b.detach().double().reshape(-1)
+    a = torch.as_tensor(a).detach().double().reshape(-1).cpu(); b = torch.as_tensor(b).detach().double().reshape(-1).cpu()
     return float((a @ b) / (a.norm() * b.norm()).clamp_min(1e-300))
-
-
-CASES = {
-    "C2_render": dict(H=1080, W=1920, hd=384, wd=672, V=200, N=1024, S=128, over={"training.pc_weight": [0.0, 0.0], "training.rgb_s_weight": [0.0, 0.0]}),
-    "C2_full": dict(H=1080, W=1920, hd=384, wd=672, V=200, N=1024, S=128, over={}),
-    "C3_ndc": dict(H=756, W=1008, hd=384, wd=512, V=20, N=1024, S=128,
-                   over={"rendering.sample_option": "ndc", "rendering.dist_alpha": True, "rendering.depth_range": [0.0, 1.0],
-                         "training.pc_weight": [0.0, 0.0], "training.rgb_s_weight": [0.0, 0.0]}),
-    "C5_full": dict(H=1080, W=1920, hd=384, wd=672, V=200, N=4096, S=128, over={}),
-    # the same C2 step with the high-frequency columns of the two encoding-fed layers damped by 2^-l (oracle.init_params(hf_damp)):
-    # no ReLU-gate switches and no 2^9-amplified rounding in the encoding adjoint -> the strict 1e-4 gate on every pose gradient
-    "C2_render_damped": dict(H=1080, W=1920, hd=384, wd=672, V=200, N=1024, S=128, damp=True,
-                             over={"training.pc_weight": [0.0, 0.0], "training.rgb_s_weight": [0.0, 0.0]}),
-}
-
-
-def _cfg(c):
-    cfg = RH.load_default_cfg()
-    RH.set_cfg(cfg, c["over"])
-    cfg["training"]["n_training_points"] = c["N"]; cfg["rendering"]["num_points"] = c["S"]
-    cfg["training"]["vis_reprojection_every"] = 10 ** 9
-    return cfg
-
-
-def _data(c, idx, seed):
-    g = torch.Generator().manual_seed(seed)
-    H, W, hd, wd = c["H"], c["W"], c["hd"], c["wd"]
-    fx = 0.6 * W
-    cam = torch.tensor([[2 * fx / W, 0, 0, 0], [0, -2 * fx / H, 0, 0], [0, 0, -1, 0], [0, 0, 0, 1]], dtype=torch.float32)[None]
-    # smooth frames / depth maps (low-res noise, bilinearly upsampled) so that the warped-RGB term sees image structure
-    up = lambda t, size: torch.nn.functional.interpolate(t, size, mode="bilinear", align_corners=False)
-    img = up(torch.rand(1, 3, 27, 48, generator=g), (H, W)).contiguous()
-    ref = up(torch.rand(1, 3, 27, 48, generator=g), (H, W)).contiguous()
-    dpt = (up(torch.rand(1, 1, 12, 21, generator=g), (hd, wd))[0] * 3.0 + 2.0).contiguous()
-    rdpt = (dpt * (1 + 0.05 * up(torch.rand(1, 1, 6, 8, generator=g), (hd, wd))[0])).contiguous()
-    return {"img": img, "img.idx": torch.tensor([idx]), "img.dpt": dpt, "img.camera_mat": cam, "img.scale_mat": torch.eye(4)[None],
-            "img.ref_imgs": ref, "img.ref_dpts": rdpt, "img.ref_idxs": torch.tensor([idx + 1])}
 
 
 def _ours(cfg, V, state, use_cuda_graph=False):
@@ -102,68 +68,44 @@ def _ours(cfg, V, state, use_cuda_graph=False):
     return trainer, net, pose, dist, model
 
 
-def _init_state(rig, V, seed):
-    g = torch.Generator().manual_seed(seed)
-    with torch.no_grad():
-        rig.pose.r.copy_((torch.randn(V, 3, generator=g) * 0.05).cuda()); rig.pose.t.copy_((torch.randn(V, 3, generator=g) * 0.05).cuda())
-        rig.dist.global_scales.copy_((1 + 0.1 * (torch.rand(V, 1, generator=g) - 0.5)).cuda())
-        rig.dist.global_shifts.copy_((0.1 * (torch.rand(V, 1, generator=g) - 0.5)).cuda())
-    return rig.state()
+def _patch_draws(monkeypatch, HW, N, S, ray_idx, noise):
+    real_randperm, real_rand = torch.randperm, torch.rand
+    monkeypatch.setattr(torch, "randperm", lambda n, *a, **k: ray_idx if n == HW else real_randperm(n, *a, **k))
+    monkeypatch.setattr(torch, "rand", lambda *a, **k: noise.to(torch.get_default_dtype()) if tuple(a) == (1, N, S) else real_rand(*a, **k))
 
 
-@pytest.mark.parametrize("name,eng", [(n, "tc") for n in CASES] + [("C2_render", "simt")])   # exact-fp32 engine: one full-size case (6 ms kernels)
+@pytest.mark.parametrize("name,eng", [(n, "tc") for n in FC.CASES] + [("C2_render", "simt")])   # exact-fp32 engine: one full-size case
 def test_train_step_vs_live_reference(name, eng, monkeypatch):
     from nope_nerf_b200 import ops
     ops.set_default_engine(eng)
-    c = CASES[name]; cfg = _cfg(c); V = c["V"]; idx = 7
-    torch.manual_seed(1234)
-    rig = RH.RefRig(cfg, V, "cuda")
-    if c.get("damp"):
-        with torch.no_grad():
-            damp = torch.ones(63, device="cuda")
-            for l in range(10):
-                damp[3 + 6 * l:9 + 6 * l] = 2.0 ** (-l)
-            rig.net.layers0[0].weight.mul_(damp[None, :]); rig.net.layers1[0].weight[:, 256:].mul_(damp[None, :])
-    state = _init_state(rig, V, 99)
-    data = _data(c, idx, 5)
+    c = FC.CASES[name]; cfg = FC.case_cfg(c); V = c["V"]
+    state = FC.start_state(cfg, V, 1234, 99, damp=c.get("damp", False))
+    gold = _golden("train_" + name, state)
+    data = FC.frames(c, 7, 5)
     H, W, N, S = c["H"], c["W"], c["N"], c["S"]
     g = torch.Generator().manual_seed(77)
     ray_idx = torch.randperm(H * W, generator=g)[:N].cuda(); noise = torch.rand(1, N, S, generator=g).cuda()
-    real_randperm, real_rand = torch.randperm, torch.rand
-    monkeypatch.setattr(torch, "randperm", lambda n, *a, **k: ray_idx if n == H * W else real_randperm(n, *a, **k))
-    monkeypatch.setattr(torch, "rand", lambda *a, **k: noise.to(torch.get_default_dtype()) if tuple(a) == (1, N, S) else real_rand(*a, **k))
-    # ---- reference fp32 (live, cuda) ----
-    ld_ref = rig.train_step(data)
-    gref = dict(r=rig.pose.r.grad.clone(), t=rig.pose.t.grad.clone(), scales=rig.dist.global_scales.grad.clone() if rig.dist.global_scales.grad is not None else torch.zeros(V, 1).cuda(),
-                shifts=rig.dist.global_shifts.grad.clone(), params=torch.cat([p.grad.reshape(-1) for p in rig.net.parameters()]))
-    # ---- reference fp64 (its own rounding envelope): the same unmodified code under float64 defaults ----
-    with RH.fp64_mode():
-        rig64 = RH.RefRig(cfg, V, "cuda", state=state)
-        data64 = {k: (v.double() if v.is_floating_point() else v) for k, v in data.items()}
-        rig64.train_step(data64)
-        g64 = dict(r=rig64.pose.r.grad, t=rig64.pose.t.grad, shifts=rig64.dist.global_shifts.grad,
-                   scales=rig64.dist.global_scales.grad if rig64.dist.global_scales.grad is not None else torch.zeros(V, 1).cuda(),
-                   params=torch.cat([p.grad.reshape(-1) for p in rig64.net.parameters()]))
-        env = {k: rel(gref[k], g64[k]) for k in gref}
-        del rig64
-    # ---- ours ----
+    _patch_draws(monkeypatch, H * W, N, S, ray_idx, noise)
     trainer, net, pose, dist, _ = _ours(cfg, V, state)
     ld = trainer.train_step(data, it=1, epoch=0, scheduling_start=10000, render_path="/tmp")
     torch.cuda.synchronize()
-    gours = dict(r=pose.r.grad, t=pose.t.grad, scales=dist.global_scales.grad, shifts=dist.global_shifts.grad,
-                 params=torch.cat([p.grad.reshape(-1) for p in net.parameters()]))
+    gours = dict(r=pose.r.grad, t=pose.t.grad, scales=dist.global_scales.grad, shifts=dist.global_shifts.grad)
+    params = torch.cat([p.grad.reshape(-1) for p in net.parameters()])
+    p_sample = params[FC.param_sample_idx(params.numel()).cuda()].double().cpu()
     e = {}
     for k in ("loss", "loss_rgb", "loss_depth", "l2_mean", "loss_pc", "loss_rgb_s"):
-        ref = float(ld_ref[k]); got = float(ld[k])
+        ref = float(gold["loss_" + k]); got = float(ld[k])
         e["loss_" + k] = abs(got - ref) / max(abs(ref), 1e-6) if ref != 0 else abs(got)
-    for k in gref:
-        e["g_" + k] = rel(gours[k], gref[k]); e["env_" + k] = env[k]
-    e["cos_params"] = 1.0 - cosine(gours["params"], gref["params"])
+    for k in gours:
+        e["g_" + k] = rel(gours[k], gold["g_" + k]); e["env_" + k] = float(gold["env_" + k])
+    ref_sample = torch.as_tensor(gold["params_sample"]).double()
+    e["g_params"] = float((p_sample - ref_sample).abs().max()) / float(gold["params_absmax"]); e["env_params"] = float(gold["env_params"])
+    e["cos_params"] = 1.0 - cosine(p_sample, ref_sample)
     _report("%s/%s" % (name, eng), **e)
     for k in ("loss", "loss_rgb", "loss_depth", "l2_mean", "loss_pc", "loss_rgb_s"):
         assert e["loss_" + k] < 1e-5, (k, e)
     # d t = sum of d p over all 131 072 samples, each carrying the 2^9-amplified fp32 rounding of the encoding adjoint: the exact-fp32
-    # engine sits at 9e-5, the tcgen05 engine at 1.2e-4, the reference's own fp32 at 3e-5 of its fp64 twin -> 2e-4 floor for d t only
+    # engine sits at 9e-5, the reference's own fp32 at 3e-5 of its fp64 twin -> 2e-4 floor for d t only
     for k in ("r", "t", "scales", "shifts"):
         floor = 1e-4 if (k != "t" or c.get("damp")) else 2e-4
         assert e["g_" + k] < max(floor, 3 * e["env_" + k]), (k, e)
@@ -173,45 +115,30 @@ def test_train_step_vs_live_reference(name, eng, monkeypatch):
 
 @pytest.mark.parametrize("name", ["C2_render", "C3_ndc"])
 def test_render_outputs_vs_live_reference(name):
-    """nope_nerf.forward at full size: rgb, depth_pred, depth_gt <= 1e-4 of the live reference (same ray_idx, no jitter so that the two
+    """nope_nerf.forward at full size: rgb, depth_pred, depth_gt <= 1e-4 of the reference (same ray_idx, no jitter so that the two
     sides need no RNG coupling; eval_mode False keeps the training-path arithmetic)."""
     from nope_nerf_b200 import ops
+    from nope_nerf_b200.model import common as mc
     ops.set_default_engine("tc")
-    c = CASES[name]; cfg = _cfg(c); V = c["V"]; idx = 3
-    torch.manual_seed(4321)
-    rig = RH.RefRig(cfg, V, "cuda")
-    state = _init_state(rig, V, 98)
-    data = _data(c, idx, 6)
+    c = FC.CASES[name]; cfg = FC.case_cfg(c); V = c["V"]; idx = 3
+    state = FC.start_state(cfg, V, 4321, 98)
+    gold = _golden("render_" + name, state)
+    data = FC.frames(c, idx, 6)
     H, W, N = c["H"], c["W"], c["N"]
     ray_idx = torch.randperm(H * W, generator=torch.Generator().manual_seed(3))[:N].cuda()
     trainer, net, pose, dist, model = _ours(cfg, V, state)
-    import model.common as mc                                          # the REFERENCE's helpers (oracle/_ref on sys.path)
-    p_full = mc.arange_pixels((H, W), 1)[1].cuda()
-    pix = p_full[:, ray_idx]
+    pix = mc.arange_pixels((H, W), 1)[1].cuda()[:, ray_idx]
+    assert rel(pix, gold["pixels"]) == 0.0
     cam = data["img.camera_mat"].cuda(); smat = data["img.scale_mat"].cuda()
     dpt = data["img.dpt"].cuda().unsqueeze(1)
-    outs = []
-    for (mod, ps, ds) in ((rig.model, rig.pose, rig.dist), (model, pose, dist)):
-        with torch.no_grad():
-            c2w = ps(idx); sc, sh = ds(idx)
-            out = mod(pix, ray_idx, cam, torch.inverse(c2w).unsqueeze(0), smat, "nope_nerf", it=0, eval_mode=False, depth_img=dpt * sc + sh,
-                      add_noise=False, img_size=(H, W))
-        outs.append(out)
-    e = dict(rgb=rel(outs[1]["rgb"], outs[0]["rgb"]), depth_pred=rel(outs[1]["depth_pred"], outs[0]["depth_pred"]),
-             depth_gt=rel(outs[1]["depth_gt"], outs[0]["depth_gt"]))
+    with torch.no_grad():
+        c2w = pose(idx); sc, sh = dist(idx)
+        out = model(pix, ray_idx, cam, torch.inverse(c2w).unsqueeze(0), smat, "nope_nerf", it=0, eval_mode=False, depth_img=dpt * sc + sh,
+                    add_noise=False, img_size=(H, W))
+    e = dict(rgb=rel(out["rgb"], gold["rgb"]), depth_pred=rel(out["depth_pred"], gold["depth_pred"]),
+             depth_gt=rel(out["depth_gt"], gold["depth_gt"]))
     _report("render/%s" % name, **e)
     assert max(e.values()) < 1e-4, e
-
-
-def _small_scene(H=48, W=64, hd=24, wd=32, V=4, seed=11):
-    g = torch.Generator().manual_seed(seed)
-    up = lambda t, size: torch.nn.functional.interpolate(t, size, mode="bilinear", align_corners=False)
-    fx = 0.6 * W
-    cam = torch.tensor([[2 * fx / W, 0, 0, 0], [0, -2 * fx / H, 0, 0], [0, 0, -1, 0], [0, 0, 0, 1]], dtype=torch.float32)[None]
-    img = up(torch.rand(1, 3, 6, 8, generator=g), (H, W)).contiguous()
-    dpt = (up(torch.rand(1, 1, 6, 8, generator=g), (hd, wd))[0] * 3.0 + 2.0).contiguous()
-    return {"img": img, "img.idx": torch.tensor([1]), "img.dpt": dpt, "img.camera_mat": cam, "img.scale_mat": torch.eye(4)[None],
-            "img.depth": torch.rand(1, H, W, generator=g) * 5 + 0.5}
 
 
 def test_eval_images_vs_live_reference(tmp_path):
@@ -221,75 +148,57 @@ def test_eval_images_vs_live_reference(tmp_path):
     from nope_nerf_b200 import ops
     ops.set_default_engine("tc")
     H, W, V = 48, 64, 4
-    cfg = RH.load_default_cfg()
+    cfg = FC.default_cfg()
     cfg["extract_images"] = {"resolution": [H, W]}
-    torch.manual_seed(21)
-    rig = RH.RefRig(cfg, V, "cuda")
-    state = _init_state(rig, V, 97)
-    data = _small_scene(H, W, V=V)
-    c2ws = torch.stack([rig.pose(i) for i in range(V)]).detach()
-    import model.eval_images as rei                                   # the REFERENCE's module (oracle/_ref on sys.path)
+    state = FC.start_state(cfg, V, 21, 97)
+    gold = _golden("eval_images", state)
+    data = FC.small_scene(H, W, V=V)
     lp = lambda a, b, normalize=True: (a - b).abs().mean()             # stand-in for the LPIPS network (same callable on both sides)
-    ref_ev = rei.Eval_Images(rig.rend, cfg, use_learnt_poses=True, use_learnt_focal=False, device=torch.device("cuda"), render_type="nope_nerf", c2ws=c2ws)
-    d_ref = ref_ev.eval_images(data, str(tmp_path / "ref"), None, lp, None)
     trainer, net, pose, dist, model = _ours(cfg, V, state)
+    c2ws = torch.stack([pose(i) for i in range(V)]).detach()
     ev = mdl.Eval_Images(model.renderer, cfg, use_learnt_poses=True, use_learnt_focal=False, device=torch.device("cuda"), render_type="nope_nerf", c2ws=c2ws)
     d = ev.eval_images(data, str(tmp_path / "ours"), None, lp, None)
-    e = dict(mse=abs(d["mse"] - d_ref["mse"]) / d_ref["mse"], psnr=abs(d["psnr"] - d_ref["psnr"]), ssim=abs(d["ssim"] - d_ref["ssim"]),
-             lpips=abs(d["lpips"] - d_ref["lpips"]) / d_ref["lpips"],
-             img=float(np.abs(d["img"].astype(np.int32) - d_ref["img"].astype(np.int32)).max()),
-             depth=float(np.abs(d["depth"].astype(np.int32) - d_ref["depth"].astype(np.int32)).max()))
+    e = dict(mse=abs(d["mse"] - float(gold["mse"])) / float(gold["mse"]), psnr=abs(d["psnr"] - float(gold["psnr"])),
+             ssim=abs(d["ssim"] - float(gold["ssim"])), lpips=abs(d["lpips"] - float(gold["lpips"])) / float(gold["lpips"]),
+             img=float(np.abs(d["img"].astype(np.int32) - gold["img"].astype(np.int32)).max()),
+             depth=float(np.abs(d["depth"].astype(np.int32) - gold["depth"].astype(np.int32)).max()))
     _report("eval_images", **e)
     assert e["mse"] < 1e-4 and e["psnr"] < 1e-3 and e["ssim"] < 1e-5 and e["lpips"] < 1e-4 and e["img"] <= 1 and e["depth"] <= 1, e
-    assert d["depth_gt"].shape == d_ref["depth_gt"].shape and os.path.exists(str(tmp_path / "ours" / "img_out" / "0001.png"))
+    assert tuple(d["depth_gt"].shape) == tuple(gold["depth_gt_shape"]) and os.path.exists(str(tmp_path / "ours" / "img_out" / "0001.png"))
 
 
 def test_render_visdata_vs_live_reference(tmp_path):
     """Trainer.render_visdata (model/training.py:100-163, nope_nerf view): uint8 frame of the reference's 1024-pixel chunk loop against
     the single-call drop-in; files written with the reference's names"""
-    import nope_nerf_b200.model as mdl
     from nope_nerf_b200 import ops
     ops.set_default_engine("tc")
     H, W, V = 48, 64, 4
-    cfg = RH.load_default_cfg()
-    cfg["training"]["vis_geo"] = False                                 # the phong geometry view is SURVEY 8(f) rank 4
-    torch.manual_seed(22)
-    rig = RH.RefRig(cfg, V, "cuda")
-    state = _init_state(rig, V, 96)
-    data = _small_scene(H, W, V=V)
-    (tmp_path / "ref").mkdir(); (tmp_path / "ours").mkdir()
-    img_ref = rig.trainer.render_visdata(data, (H, W), 0, str(tmp_path / "ref"))
+    cfg = FC.default_cfg()
+    cfg["training"]["vis_geo"] = False                                 # the phong geometry view is checked below
+    state = FC.start_state(cfg, V, 22, 96)
+    gold = _golden("render_visdata", state)
+    data = FC.small_scene(H, W, V=V)
+    (tmp_path / "ours").mkdir()
     trainer, net, pose, dist, model = _ours(cfg, V, state)
     img = trainer.render_visdata(data, (H, W), 0, str(tmp_path / "ours"))
-    diff = int(np.abs(img.astype(np.int32) - img_ref.astype(np.int32)).max())
+    diff = int(np.abs(img.astype(np.int32) - gold["img"].astype(np.int32)).max())
     _report("render_visdata", max_uint8_diff=diff)
-    assert img.shape == img_ref.shape == (H, W, 3) and diff <= 1, diff
+    assert img.shape == gold["img"].shape == (H, W, 3) and diff <= 1, diff
     for f in ("0001_img.png", "0001_depth.png"):
-        assert os.path.exists(str(tmp_path / "ours" / f)) and os.path.exists(str(tmp_path / "ref" / f)), f
-
-
-def _geo_rig(V=4, seed=31):
-    """a field whose occupancy crosses the ray-marching threshold (alpha = 0.5 <=> density logit = 0) inside the sphere"""
-    cfg = RH.load_default_cfg()
-    torch.manual_seed(seed)
-    rig = RH.RefRig(cfg, V, "cuda")
-    with torch.no_grad():
-        rig.net.fc_density.weight.mul_(10.0); rig.net.fc_density.bias.fill_(0.0)     # logit = -0.03 +- 0.04: 22 % of space occupied
-    return cfg, rig, _init_state(rig, V, 95)
+        assert os.path.exists(str(tmp_path / "ours" / f)), f
 
 
 def test_infer_occ_and_gradient_vs_live_reference():
     """OfficialStaticNerf.infer_occ / gradient (official_nerf.py:46-67: normals of the geometry view = -d logit / d p by autograd in the
     reference, the data-gradient chain of nnb_field_bwd here)"""
-    cfg, rig, state = _geo_rig()
+    cfg = FC.default_cfg()
+    state = FC.start_state(cfg, 4, 31, 95, geo=True)
+    gold = _golden("infer_occ", state)
     trainer, net, pose, dist, model = _ours(cfg, 4, state)
-    g = torch.Generator().manual_seed(8)
-    p = ((torch.rand(4096, 3, generator=g) - 0.5) * 6.0).cuda()
-    _, s_ref = rig.net.infer_occ(p)
+    p = ((torch.rand(4096, 3, generator=torch.Generator().manual_seed(8)) - 0.5) * 6.0).cuda()
     _, s = net.infer_occ(p)
-    g_ref = rig.net.gradient(p.clone(), 0).detach()
     g_our = net.gradient(p.clone(), 0).detach()
-    e = dict(logit=rel(s, s_ref), grad=rel(g_our, g_ref), shape=float(g_our.shape == g_ref.shape))
+    e = dict(logit=rel(s, gold["logit"]), grad=rel(g_our, gold["grad"]), shape=float(tuple(g_our.shape) == tuple(gold["grad_shape"])))
     _report("infer_occ_gradient", **e)
     assert e["shape"] == 1.0 and e["logit"] < 1e-5 and e["grad"] < 1e-4, e
 
@@ -298,65 +207,56 @@ def test_phong_renderer_vs_live_reference(tmp_path):
     """Renderer.phong_renderer (rendering.py:198-271: 512-step ray marching + 8 secant steps + normals + shading) and the geometry view
     of Trainer.render_visdata (training.py:146-161).  A pixel whose occupancy sits at the threshold may resolve to another march step on
     the other implementation: at most 1 % of the pixels may differ by more than 2 / 255."""
-    cfg, rig, state = _geo_rig()
+    from nope_nerf_b200.model import common as mc
+    cfg = FC.default_cfg(); assert cfg["training"]["vis_geo"] is True
     H, W, V = 24, 32, 4
+    state = FC.start_state(cfg, V, 31, 95, geo=True)
+    gold = _golden("phong", state)
     trainer, net, pose, dist, model = _ours(cfg, V, state)
-    data = _small_scene(H, W, V=V)
-    import model.common as mc
+    data = FC.small_scene(H, W, V=V)
     pixels = mc.arange_pixels((H, W), 1)[1].cuda()
     cam = data["img.camera_mat"].cuda(); smat = data["img.scale_mat"].cuda()
-    def shade(mod, ps, view):
-        with torch.no_grad():
-            c2w = ps(view)
-        o = mod(pixels, None, cam, torch.inverse(c2w).unsqueeze(0), smat, "phong_renderer", it=0, eval_mode=True, depth_img=None, add_noise=False,
-                img_size=(H, W))
-        return (o["rgb"].detach().reshape(-1, 3), o["rgb_surf"].detach().reshape(-1, 3))
-    view = 1
-    for v in range(V):          # a view whose camera sits in free space and sees a surface (random field: not every pose does)
-        if float((shade(rig.model, rig.pose, v)[1].abs().sum(1) > 0).float().mean()) > 0.02:
-            view = v; break
-    outs = [shade(rig.model, rig.pose, view), shade(model, pose, view)]
+    view = int(gold["view"])   # the reference's first view whose camera sits in free space and sees a surface
+    with torch.no_grad():
+        c2w = pose(view)
+    o = model(pixels, None, cam, torch.inverse(c2w).unsqueeze(0), smat, "phong_renderer", it=0, eval_mode=True, depth_img=None, add_noise=False,
+              img_size=(H, W))
+    rgb, surf = o["rgb"].detach().reshape(-1, 3).cpu(), o["rgb_surf"].detach().reshape(-1, 3).cpu()
+    rgb_ref, surf_ref = torch.as_tensor(gold["rgb"]), torch.as_tensor(gold["rgb_surf"])
     data["img.idx"] = torch.tensor([view])
-    hit_ref = (outs[0][1].abs().sum(1) > 0)
-    bad = ((outs[0][0] - outs[1][0]).abs().max(1).values > 2.0 / 255) | ((outs[0][1] - outs[1][1]).abs().max(1).values > 2.0 / 255)
+    hit_ref = (surf_ref.abs().sum(1) > 0)
+    bad = ((rgb_ref - rgb).abs().max(1).values > 2.0 / 255) | ((surf_ref - surf).abs().max(1).values > 2.0 / 255)
     e = dict(frac_bad=float(bad.float().mean()), frac_surface=float(hit_ref.float().mean()),
-             med_rgb=float((outs[0][0] - outs[1][0]).abs().median()), med_surf=float((outs[0][1] - outs[1][1]).abs().median()))
+             med_rgb=float((rgb_ref - rgb).abs().median()), med_surf=float((surf_ref - surf).abs().median()))
     _report("phong_renderer", **e)
     assert 0.02 < e["frac_surface"] <= 1.0, e                  # the scene has a visible surface
     assert e["frac_bad"] <= 0.01 and e["med_rgb"] < 1e-4 and e["med_surf"] < 1e-4, e
     # render_visdata with vis_geo (configs/default.yaml:106): returns the shaded view and writes %04d_geo.png
-    cfg2 = RH.load_default_cfg(); assert cfg2["training"]["vis_geo"] is True
-    (tmp_path / "ref").mkdir(); (tmp_path / "ours").mkdir()
-    img_ref = rig.trainer.render_visdata(data, (H, W), 0, str(tmp_path / "ref"))
+    (tmp_path / "ours").mkdir()
     img = trainer.render_visdata(data, (H, W), 0, str(tmp_path / "ours"))
-    far = (np.abs(img.astype(np.int32) - img_ref.astype(np.int32)).max(-1) > 2).mean()
-    assert img.shape == img_ref.shape and far <= 0.01, far
+    far = (np.abs(img.astype(np.int32) - gold["img"].astype(np.int32)).max(-1) > 2).mean()
+    assert img.shape == gold["img"].shape and far <= 0.01, far
     assert os.path.exists(str(tmp_path / "ours" / ("%04d_geo.png" % view)))
 
 
 def test_invariant_depth_loss_vs_live_reference(monkeypatch):
-    """training.depth_loss_type = 'invariant' (losses.py:34-57): one Trainer.train_step against the live reference, small scene"""
+    """training.depth_loss_type = 'invariant' (losses.py:34-57): one Trainer.train_step against the reference, small scene"""
     from nope_nerf_b200 import ops
     ops.set_default_engine("tc")
     H, W, V, N, S = 48, 64, 4, 256, 64
-    cfg = RH.load_default_cfg()
-    RH.set_cfg(cfg, {"training.depth_loss_type": "invariant", "training.pc_weight": [0.0, 0.0], "training.rgb_s_weight": [0.0, 0.0],
+    cfg = FC.default_cfg()
+    FC.set_cfg(cfg, {"training.depth_loss_type": "invariant", "training.pc_weight": [0.0, 0.0], "training.rgb_s_weight": [0.0, 0.0],
                      "training.n_training_points": N, "rendering.num_points": S, "training.vis_reprojection_every": 10 ** 9})
-    torch.manual_seed(77)
-    rig = RH.RefRig(cfg, V, "cuda")
-    state = _init_state(rig, V, 94)
-    data = _small_scene(H, W, V=V)
+    state = FC.start_state(cfg, V, 77, 94)
+    gold = _golden("invariant_depth", state)
+    data = FC.small_scene(H, W, V=V)
     g = torch.Generator().manual_seed(78)
     ray_idx = torch.randperm(H * W, generator=g)[:N].cuda(); noise = torch.rand(1, N, S, generator=g).cuda()
-    real_randperm, real_rand = torch.randperm, torch.rand
-    monkeypatch.setattr(torch, "randperm", lambda n, *a, **k: ray_idx if n == H * W else real_randperm(n, *a, **k))
-    monkeypatch.setattr(torch, "rand", lambda *a, **k: noise if tuple(a) == (1, N, S) else real_rand(*a, **k))
-    ld_ref = rig.train_step(data)
-    gref = dict(r=rig.pose.r.grad.clone(), t=rig.pose.t.grad.clone(), shifts=rig.dist.global_shifts.grad.clone())
+    _patch_draws(monkeypatch, H * W, N, S, ray_idx, noise)
     trainer, net, pose, dist, _ = _ours(cfg, V, state)
     ld = trainer.train_step(data, it=1, epoch=0, scheduling_start=10000, render_path="/tmp")
-    e = dict(loss=abs(float(ld["loss"]) - float(ld_ref["loss"])) / abs(float(ld_ref["loss"])),
-             loss_depth=abs(float(ld["loss_depth"]) - float(ld_ref["loss_depth"])) / abs(float(ld_ref["loss_depth"])),
-             g_r=rel(pose.r.grad, gref["r"]), g_t=rel(pose.t.grad, gref["t"]), g_shifts=rel(dist.global_shifts.grad, gref["shifts"]))
+    e = dict(loss=abs(float(ld["loss"]) - float(gold["loss"])) / abs(float(gold["loss"])),
+             loss_depth=abs(float(ld["loss_depth"]) - float(gold["loss_depth"])) / abs(float(gold["loss_depth"])),
+             g_r=rel(pose.r.grad, gold["g_r"]), g_t=rel(pose.t.grad, gold["g_t"]), g_shifts=rel(dist.global_shifts.grad, gold["g_shifts"]))
     _report("invariant_depth", **e)
     assert e["loss"] < 1e-5 and e["loss_depth"] < 1e-5 and e["g_r"] < 2e-3 and e["g_t"] < 2e-3 and e["g_shifts"] < 2e-3, e

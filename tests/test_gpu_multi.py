@@ -51,8 +51,8 @@ def test_dp_rays_equals_single_gpu(graph, peer, tmp_path):
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_dp_rays_fp16_wgrad_planes(tmp_path):
-    """default configuration (NNB_WG16 planes, whole-step graph, peer exchange): pose / distortion gradients keep the tight gate, the
-    MLP part of the summed buffer agrees to the fp16 operand rounding"""
+    """default configuration with the 'fp16' weight-gradient setting (whole-step graph, peer exchange): pose / distortion gradients
+    keep the tight gate, the MLP part of the summed buffer keeps the looser gate of fp16 operand rounding"""
     from nope_nerf_b200 import _lib as L
     one = _run(str(tmp_path), "one", "rays", 0, 0, 1, wgrad="fp16")
     two = _run(str(tmp_path), "two", "rays", 1, 1, 2, wgrad="fp16")

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C ABI,
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI,
 against (a) fixtures produced by the unmodified reference (tests/golden, tools/make_golden.py)
 and (b) the numpy oracle on the same seeded inputs.
 
@@ -96,9 +96,9 @@ def oracle32(g):
 @pytest.mark.parametrize("name", RENDER_CASES)
 @pytest.mark.parametrize("eng,wg", [("simt", "exact"), ("tc", "exact"), ("tc", "fp16")])
 def test_render_vs_reference_golden(name, eng, wg, monkeypatch):
-    """wg = weight-gradient operand planes of the tcgen05 backward ('fp16' = NNB_WG16, the default: the MLP parameter digests then carry
-    fp16 operand rounding, gate 2e-3 at these sample counts of 768 .. 6144 -- measured up to 7.3e-4 on the 3 x 128 / 1 x 256 head
-    matrices; outputs and every pose / distortion / intrinsics gradient keep the gates below in both modes).
+    """wg = the weight-gradient precision setting; with 'fp16' the MLP parameter digests keep the looser gate of fp16 operand planes
+    (2e-3 at these sample counts of 768 .. 6144); outputs and every pose / distortion / intrinsics gradient keep the gates below in
+    both modes.
     Outputs: <= 1e-4 of the reference.  Gradients, two kinds of case:
       * `*_damped` (oracle.init_params(hf_damp=True): no ReLU-gate switches between fp32 evaluation orders): every gradient
         <= 1e-4 of the fp64 truth (MLP parameter digests 5e-4) and <= max(1e-4, 3 x the reference's own distance from it);
@@ -137,7 +137,7 @@ def test_render_vs_reference_golden(name, eng, wg, monkeypatch):
     assert e["alpha"] < 2e-4, e["alpha"]
     # render_oddflags (N = 32 rays, un-normalised rays, |p| up to 15): ONE gate switch on a heavy sample moves d t by 2 %; each fp32
     # implementation has its own switches (the exact-fp32 engine shares the numpy oracle's: g_*_vs32 ~ 1e-4), so the envelope of other
-    # realisations does not bound the tcgen05 engine's -- its `_damped` twin carries the strict gate
+    # realisations does not bound the tensor-core engine's -- its `_damped` twin carries the strict gate
     flip_floor = 3e-2 if (name == "render_oddflags") else 1e-4
     for k in terms:
         if damped:
@@ -208,12 +208,11 @@ def _build_trainer(g, engine_name, with_ref):
                                            ("train_learn_focal", True)])
 @pytest.mark.parametrize("eng,wg", [("simt", "exact"), ("tc", "exact"), ("tc", "fp16")])
 def test_trainer_step_vs_reference_golden(name, with_ref, eng, wg, monkeypatch):
-    """Two consecutive reference Trainer.train_step calls.  wg = weight-gradient operand planes of the tcgen05 backward: 'exact' (bf16
-    hi|lo, three MMAs per product) or 'fp16' (NNB_WG16, the default: one fp16 plane per operand, delayed per-layer dY scaling).  With
-    'fp16' the FIRST step's MLP gradients carry fp16 operand rounding (gate 2e-3 on the digests, measured 1.3e-4 .. 2e-4 here and
-    3e-4 rel-L2 per tensor at 1024 x 128, tools/wg16_check.py); Adam's sign-like first update turns that into lr-sized differences on
-    weights whose gradient is near zero, so the SECOND step's gradients agree to 5e-2 only (measured 1.8e-2); pose / distortion
-    gradients of the first step and every loss scalar keep the 'exact' gates."""
+    """Two consecutive reference Trainer.train_step calls.  wg = the weight-gradient precision setting ('exact' | 'fp16'); the
+    tensor-core backward computes both with bf16 hi|lo wgmma operands (three MMAs per product), and the gates below keep the looser
+    'fp16' bounds of fp16 operand planes: 2e-3 on the first step's MLP gradient digests; Adam's sign-like first update turns operand
+    rounding into lr-sized differences on weights whose gradient is near zero, so the SECOND step's gradients are gated at 5e-2 only;
+    pose / distortion gradients of the first step and every loss scalar keep the 'exact' gates."""
     if dict(engines()).get(eng) is None:
         pytest.skip("engine disabled")
     from nope_nerf_b200 import ops as _ops
@@ -670,7 +669,7 @@ def test_native_ref_stage_vs_oracle(name):
 
 @pytest.mark.parametrize("N,S", [(5, 32), (3, 64), (7, 32), (130, 32), (33, 64), (999, 128), (9, 256)])
 def test_ragged_last_tile_tc_vs_simt(N, S, monkeypatch):
-    """N*S not a multiple of the 128-sample tile: the tcgen05 engine pads the last tile with clamped rows whose cotangents are
+    """N*S not a multiple of the 128-sample tile: the tensor-core engine pads the last tile with clamped rows whose cotangents are
     zero; outputs and gradients must agree with the exact-fp32 engine (weights from init_params(hf_damp=True), so that the
     comparison of the two engines' GRADIENTS is not dominated by single ReLU-gate switches on a handful of rays)."""
     from nope_nerf_b200 import ops as _ops_

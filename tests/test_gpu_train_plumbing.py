@@ -17,7 +17,7 @@ sys.path.insert(0, ROOT)
 from oracle import ref_harness as RH  # noqa: E402
 
 if not RH.available():
-    pytest.skip("oracle/_ref missing (run tools/vendor_ref.py in the build container)", allow_module_level=True)
+    pytest.skip("oracle/_ref missing (oracle/vendor_ref.py needs a reference checkout)", allow_module_level=True)
 
 
 def _run(tmp, impl):

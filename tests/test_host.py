@@ -234,69 +234,60 @@ def test_refstage_device_math_on_host(name, detach, scale_pcs, shift_first, tmp_
     assert relmax(o[20:22], gr["kxy"]) < 5e-5, (o[20:22], gr["kxy"])          # d/d(kx, ky): what LearnFocal receives from this stage
 
 
-def test_resident_dataset_equals_reference_dataloader_items(tmp_path):
-    """SURVEY.md 8(f) rank 1 against the real thing: the UNMODIFIED reference loader (oracle/_ref: dataloading.get_dataloader -> OurDataset
-    -> DataLoader(batch_size=1), dataloading/dataloading.py:13-45,105-139) reads a fixture scene in the on-disk layout of SURVEY.md
-    appendix B; ResidentDataset.from_reference_field(fields['img']) must hand out the same items (keys, shapes, dtypes, values, reference-frame
-    choice under the same `random` state)."""
+def test_resident_dataset_equals_reference_dataloader_items():
+    """SURVEY.md 8(f) rank 1 against the real thing: the UNMODIFIED reference loader (dataloading.get_dataloader -> OurDataset ->
+    DataLoader(batch_size=1), dataloading/dataloading.py:13-45,105-139) read a fixture scene in the on-disk layout of SURVEY.md
+    appendix B; its loaded DataField and every item it yielded are stored in tests/golden/dataloader_items.npz
+    (tools/make_golden_dataloader.py).  ResidentDataset.from_reference_field(that field) must hand out the same items (keys,
+    shapes, dtypes, values, reference-frame choice under the same `random` state)."""
     import random
-    import sys
-    import warnings
-    from oracle import ref_harness as RH
-    if not RH.available():
-        pytest.skip("oracle/_ref missing (tools/vendor_ref.py needs /root/reference)")
-    sys.path.insert(0, os.path.join(ROOT, "tools"))
-    from run_ref_train import write_scene
+    import types
     from nope_nerf_b200.dataloading import ResidentDataset
-    write_scene(str(tmp_path / "data" / "Test" / "images"), V=10)
-    RH.install_stubs()
-    if RH.REF not in sys.path:
-        sys.path.insert(0, RH.REF)
-    import dataloading as dl                                      # the reference's package, unchanged
-    cfg = dl.load_config(os.path.join(RH.REF, "configs", "Test", "images.yaml"), os.path.join(RH.REF, "configs", "default.yaml"))
-    cfg["dataloading"].update(path=str(tmp_path / "data" / "Test"), n_workers=0, resize_factor=None, random_ref=2)
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")                           # pin_memory=True without a GPU
-        loader, fields = dl.get_dataloader(cfg, mode="train", shuffle=False)
-        random.seed(11)
-        ref_items = list(loader)
-    ds = ResidentDataset.from_reference_field(fields["img"], device="cpu", pin_host=False)
-    assert len(ds) == len(ref_items) == fields["img"].N_imgs
+    g = np.load(os.path.join(ROOT, "tests", "golden", "dataloader_items.npz"))
+    imgs = (g["imgs_u8"] / 255.0).astype(np.float32)                # exactly the reference's frames (checked when stored)
+    field = types.SimpleNamespace(imgs=imgs, dpt_depth=g["dpt_depth"], K=g["K"], ref_img=bool(g["ref_img"]), random_ref=int(g["random_ref"]),
+                                  N_imgs=int(g["N_imgs"]))
+    frames = {"imgs": torch.from_numpy(imgs), "dpt_depth": torch.from_numpy(g["dpt_depth"])}
+    ds = ResidentDataset.from_reference_field(field, device="cpu", pin_host=False)
+    n = int(g["n_items"])
+    assert len(ds) == n == field.N_imgs
     random.seed(11)
-    for i, ref in enumerate(ref_items):
+    for i in range(n):
         ours = ds[i]
-        assert set(ours) == set(ref), (sorted(ours), sorted(ref))
-        for k, v in ref.items():
+        keys = [str(k) for k in g["item%d_keys" % i]]
+        assert sorted(ours) == keys, (sorted(ours), keys)
+        for k in keys:
+            pre = "item%d_%s" % (i, k)
             o = ours[k]
-            assert tuple(o.shape) == tuple(v.shape) and o.dtype == v.dtype, (k, o.shape, v.shape, o.dtype, v.dtype)
-            assert torch.equal(o, v), k
+            assert tuple(o.shape) == tuple(g[pre + "_shape"]) and str(o.dtype) == str(g[pre + "_dtype"]), (k, o.shape, o.dtype)
+            ref = torch.from_numpy(g[pre + "_value"]) if pre + "_value" in g else frames[str(g[pre + "_src"])][int(g[pre + "_frame"])][None]
+            assert torch.equal(o, ref.to(o.dtype)), k
+
+
+def rgb_s_inputs():
+    g = torch.Generator().manual_seed(3)
+    a = torch.rand(1, 3, 24, 32, generator=g); b = (a + 0.1 * torch.randn(1, 3, 24, 32, generator=g)).clamp(0, 1)
+    valid = torch.rand(1, 1, 24, 32, generator=g) > 0.3
+    return a, b, valid
 
 
 @pytest.mark.parametrize("with_ssim", [False, True])
 def test_rgb_s_loss_with_ssim_vs_live_reference(with_ssim):
     """Loss.get_rgb_s_loss (losses.py:150-157) incl. the SSIM term (class SSIM, losses.py:222-252; configs/default.yaml:109 `with_ssim`)
-    against the UNMODIFIED reference class on the CPU: value and gradient with respect to both images."""
-    from oracle import ref_harness as RH
-    if not RH.available():
-        pytest.skip("oracle/_ref missing (tools/vendor_ref.py needs /root/reference)")
-    rmdl = RH.import_reference("cpu")
-    import model.losses as ref_losses                              # the reference's module (oracle/_ref on sys.path)
-    assert os.path.abspath(ref_losses.__file__).startswith(RH.REF)
+    against the UNMODIFIED reference class on the CPU (its stored results, tests/golden/rgb_s_loss.npz from tools/make_golden_host.py):
+    value and gradient with respect to both images."""
     from nope_nerf_b200.model.losses import Loss
+    gold = np.load(os.path.join(ROOT, "tests", "golden", "rgb_s_loss.npz"))
     cfg = {"depth_loss_type": "l1", "with_ssim": with_ssim, "with_auto_mask": False, "match_method": "dense"}
-    g = torch.Generator().manual_seed(3)
-    a = torch.rand(1, 3, 24, 32, generator=g); b = (a + 0.1 * torch.randn(1, 3, 24, 32, generator=g)).clamp(0, 1)
-    valid = torch.rand(1, 1, 24, 32, generator=g) > 0.3
-    outs = []
-    for L_ in (ref_losses.Loss(cfg), Loss(cfg)):
-        x, y = a.clone().requires_grad_(True), b.clone().requires_grad_(True)
-        v = L_.get_rgb_s_loss(x, y, valid)
-        v.backward()
-        outs.append((float(v.detach()), x.grad.clone(), y.grad.clone()))
-    (v0, gx0, gy0), (v1, gx1, gy1) = outs
+    a, b, valid = rgb_s_inputs()
+    x, y = a.clone().requires_grad_(True), b.clone().requires_grad_(True)
+    v = Loss(cfg).get_rgb_s_loss(x, y, valid)
+    v.backward()
+    v0, gx0, gy0 = float(gold["value_%d" % with_ssim]), torch.from_numpy(gold["gx_%d" % with_ssim]), torch.from_numpy(gold["gy_%d" % with_ssim])
+    v1, gx1, gy1 = float(v.detach()), x.grad, y.grad
     assert abs(v0 - v1) <= 1e-6 * abs(v0), (v0, v1)
     # fp32: the variances are differences of nearly equal means, the two implementations order the operations differently
     assert (gx0 - gx1).abs().max() <= 2e-5 * gx0.abs().max() and (gy0 - gy1).abs().max() <= 2e-5 * gy0.abs().max()
     if with_ssim:
-        m0 = ref_losses.compute_ssim_loss(a, b); m1 = Loss.ssim_loss_map(a, b)
+        m0 = torch.from_numpy(gold["ssim_map"]); m1 = Loss.ssim_loss_map(a, b)
         assert m0.shape == m1.shape and (m0 - m1).abs().max() < 1e-6

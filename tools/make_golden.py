@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by running the UNMODIFIED reference (torch CPU, fp32).
 
-Run in the build container only (needs /root/reference):  python tools/make_golden.py
+Needs a reference checkout ($NOPE_NERF_REFERENCE, default ../reference beside this repository):  python tools/make_golden.py
 The GPU box never runs this; it only reads the committed .npz fixtures.
 
 Harness-side shims (reference files untouched, SURVEY.md section 8(c)):
@@ -15,8 +15,8 @@ outputs and gradient digests are stored.
 import os, sys, types
 import numpy as np
 
-REF = os.environ.get("NOPE_NERF_REFERENCE", "/root/reference")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF = os.environ.get("NOPE_NERF_REFERENCE", os.path.join(os.path.dirname(ROOT), "reference"))
 sys.path.insert(0, ROOT)
 
 

@@ -64,7 +64,7 @@ def main():
             "graph_exact": dict(_wgrad="exact"),
             "eager_torchadam": dict(use_cuda_graph=False, pixel_sampler="randperm", fused_adam=False)}
     arms = [(n, dict(ARMS[n])) for n in a.arms.split(",")]
-    assert RH.available(), "oracle/_ref missing (tools/vendor_ref.py)"
+    assert RH.available(), "oracle/_ref missing (oracle/vendor_ref.py)"
     dev = torch.device("cuda")
     H, W, hd, wd, V, N, S = 60, 80, 60, 80, 6, 512, 64
     kx, ky = 1.2, -1.6

@@ -70,7 +70,7 @@ def main():
     a = ap.parse_args()
     import torch
     from oracle import ref_harness as RH
-    assert RH.available(), "oracle/_ref missing (tools/vendor_ref.py)"
+    assert RH.available(), "oracle/_ref missing (oracle/vendor_ref.py)"
     work = os.path.abspath(a.workdir)
     scene = os.path.join(work, "data", "Test", "images")
     write_scene(scene)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Eager-PyTorch statement of the same C2 training step (autograd, torch.optim.Adam x3), timed on the device it is run on.
 
-/root/reference cannot travel to the GPU box, so this is the stand-in for "the reference's single-GPU PyTorch path" that
+Where no reference checkout is available, this is the stand-in for "the reference's single-GPU PyTorch path" that
 BASELINE.md section 3 asks to time next to the product: the SAME op structure as the reference's step (SURVEY.md 8a: whole-map
 nearest interpolation + gather, randperm(H*W), pixel grid rebuilt per step, exp-map pose, per-level sin/cos + cat encoding,
 nn.Linear MLP, cumprod compositing, L1 losses, loss.backward(), three Adam optimizers), written from the equations of
