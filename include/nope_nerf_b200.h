@@ -160,10 +160,11 @@ int nnb_chamfer(const float* X, int32_t P, const float* Y, int32_t Q, uint64_t* 
                 float* loss, float weight, float* gX, float* gY, void* stream);
 
 /* Reference-image stage of Trainer.compute_loss (model/training.py:280-365): point-cloud (dense chamfer) + warped-RGB terms
- * between the current view and one detached reference view (training.detach_ref_img = True, the default), forward AND adjoint
- * in one call.
+ * between the current view and one reference view, forward AND adjoint in one call.
  *   img_* (3,H,W) planar fp32; dpt_* (h_d,w_d) raw DPT maps; c2w_* (4,4) row-major; dist_* = {effective scale, shift}
- *   (Learn_Distortion.forward) -- all device pointers.  flags: 1 = scale_pcs, 2 = detach_rgbs_scale, 4 = shift_first.
+ *   (Learn_Distortion.forward) -- all device pointers.  flags: 1 = scale_pcs, 2 = detach_rgbs_scale, 4 = shift_first,
+ *   8 = with_ssim (warped-RGB loss 0.15 L1 + 0.85 SSIM, losses.py:150-157; needs nnb_refstage_workspace_bytes_flags),
+ *   16 = gradients into the reference view too (training.detach_ref_img = False; needs g_c2w_ref and g_dist_ref).
  *   losses[2] = {loss_pc, loss_rgb_s}; g_c2w[16] / g_dist[2] / g_kxy[2] ACCUMULATE grad_scale * d(w_pc*loss_pc + w_rgb_s*loss_rgb_s) /
  *   d(c2w_cur, dist_cur, (kx, ky)); loss_total (optional) += the weighted sum.
  * CUDA-graph replay: per-step values may come from device memory instead of the host fields -- img_pp (device array of the two
@@ -180,8 +181,11 @@ typedef struct nnb_refstage_args {
   /* optional (NULL / 0 = unused) */
   const float* const* img_pp; const float* cam; const int32_t* cam_idx_dev; int32_t num_cams; const float* weights_dev;
   float* g_kxy; float* loss_total; float grad_scale;   /* grad_scale 0 is read as 1 */
+  /* flag 16: ACCUMULATE grad_scale * d(...) / d(c2w_ref) (rows 0-2 of the 4x4) and d / d(dist_ref) */
+  float* g_c2w_ref; float* g_dist_ref;
 } nnb_refstage_args;
-size_t nnb_refstage_workspace_bytes(int32_t h_d, int32_t w_d, int32_t pc_ratio);
+size_t nnb_refstage_workspace_bytes(int32_t h_d, int32_t w_d, int32_t pc_ratio);          /* flags 1 | 2 | 4 */
+size_t nnb_refstage_workspace_bytes_flags(int32_t h_d, int32_t w_d, int32_t pc_ratio, uint32_t flags);
 int nnb_refstage(const nnb_refstage_args* args, void* stream);
 
 /* ---- data-parallel exchange over NVLink peer memory (new component, SURVEY.md 8(e)) --------------------------------------

@@ -13,6 +13,7 @@ NUM_PARAMS = 595844
 DIST_ALPHA, NDC, NORMALISE, USE_DIR, WHITE_BG, EVAL, SOFTPLUS, SHIFT_FIRST, STASH, TCBWD, WG16, RAW_DENSITY = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048
 FWD_DROP_WLO, FWD_DROP_ALO = 4096, 8192
 ENGINE_SIMT, ENGINE_TC = 0, 1
+RS_SCALE_PCS, RS_DETACH_RGBS_SCALE, RS_SHIFT_FIRST, RS_WITH_SSIM, RS_GRAD_REF = 1, 2, 4, 8, 16   # nnb_refstage_args.flags
 
 _f = C.c_void_p  # device pointers travel as integers
 
@@ -38,7 +39,7 @@ class RefStageArgs(C.Structure):
                 ("flags", C.c_uint32), ("kx", C.c_float), ("ky", C.c_float), ("nearest_limit", C.c_float), ("w_pc", C.c_float), ("w_rgb_s", C.c_float),
                 ("losses", _f), ("g_c2w", _f), ("g_dist", _f), ("workspace", _f), ("workspace_bytes", C.c_size_t),
                 ("img_pp", _f), ("cam", _f), ("cam_idx_dev", _f), ("num_cams", C.c_int32), ("weights_dev", _f),
-                ("g_kxy", _f), ("loss_total", _f), ("grad_scale", C.c_float)]
+                ("g_kxy", _f), ("loss_total", _f), ("grad_scale", C.c_float), ("g_c2w_ref", _f), ("g_dist_ref", _f)]
 
 
 MAX_RANKS = 8
@@ -87,6 +88,8 @@ def _load():
                                                 _f, _f, _f, C.c_void_p]
     lib.nnb_refstage_workspace_bytes.restype = C.c_size_t
     lib.nnb_refstage_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    lib.nnb_refstage_workspace_bytes_flags.restype = C.c_size_t
+    lib.nnb_refstage_workspace_bytes_flags.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_uint32]
     lib.nnb_refstage.argtypes = [C.POINTER(RefStageArgs), C.c_void_p]
     lib.nnb_ipc_alloc.argtypes = [C.c_size_t, C.POINTER(C.c_void_p), C.POINTER(C.c_ubyte)]
     lib.nnb_ipc_open.argtypes = [C.POINTER(C.c_ubyte), C.POINTER(C.c_void_p)]

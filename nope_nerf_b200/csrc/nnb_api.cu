@@ -29,6 +29,7 @@ cudaError_t launch_chamfer_full(const float*, int, const float*, int, unsigned l
                                 int*, int*, cudaStream_t);
 cudaError_t launch_adam(float*, const float*, float*, float*, int64_t, int, float, float, float, float, cudaStream_t);
 size_t refstage_workspace_bytes(int hd, int wd, int ratio);
+size_t refstage_workspace_bytes_flags(int hd, int wd, int ratio, unsigned flags);
 cudaError_t launch_refstage(const nnb_refstage_args& a, cudaStream_t st);
 cudaError_t launch_allreduce_adam(const nnb_allreduce_adam_args& a, cudaStream_t st);
 
@@ -233,6 +234,11 @@ size_t nnb_refstage_workspace_bytes(int32_t h_d, int32_t w_d, int32_t pc_ratio) 
   return refstage_workspace_bytes(h_d, w_d, pc_ratio);
 }
 
+size_t nnb_refstage_workspace_bytes_flags(int32_t h_d, int32_t w_d, int32_t pc_ratio, uint32_t flags) {
+  if (h_d <= 0 || w_d <= 0 || pc_ratio <= 0 || h_d / pc_ratio < 2 || w_d / pc_ratio < 2) return 0;
+  return refstage_workspace_bytes_flags(h_d, w_d, pc_ratio, flags);
+}
+
 int nnb_refstage(const nnb_refstage_args* a, void* stream) {
   if (!a) return fail(-1, "null args");
   if ((!a->img_pp && (!a->img_cur || !a->img_ref)) || !a->dpt_cur || !a->dpt_ref || !a->c2w_cur || !a->c2w_ref || !a->dist_cur || !a->dist_ref ||
@@ -241,7 +247,10 @@ int nnb_refstage(const nnb_refstage_args* a, void* stream) {
   if (a->cam_idx_dev && a->num_cams <= 0) return fail(-3, "nnb_refstage: cam_idx_dev needs num_cams");
   if (a->H < 2 || a->W < 2 || a->pc_ratio <= 0 || a->h_d / a->pc_ratio < 2 || a->w_d / a->pc_ratio < 2)
     return fail(-2, "nnb_refstage: bad sizes");
-  if (!a->workspace || a->workspace_bytes < refstage_workspace_bytes(a->h_d, a->w_d, a->pc_ratio)) return fail(-4, "nnb_refstage: workspace too small");
+  if ((a->flags & 16u) && (!a->g_c2w_ref || !a->g_dist_ref))
+    return fail(-3, "nnb_refstage: flag 16 (gradients into the reference view) needs g_c2w_ref and g_dist_ref");
+  if (!a->workspace || a->workspace_bytes < refstage_workspace_bytes_flags(a->h_d, a->w_d, a->pc_ratio, a->flags))
+    return fail(-4, "nnb_refstage: workspace too small");
   cudaError_t e = launch_refstage(*a, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_refstage");
 }

@@ -1,6 +1,9 @@
 // Reference-image stage of Trainer.compute_loss (model/training.py:280-365) as four small kernels around the dense chamfer:
 //   prep (relative pose, scale2)  ->  points forward (clouds, warped-RGB residual)  ->  nnb chamfer (nearest neighbours, d/dX, d/dY)
 //   ->  points backward (block-reduced sums)  ->  finish (gradients of the current view's pose matrix and distortion).
+// With SSIM (flag 8) the points forward also stores both colours of every point and one more kernel (rs_ssim_k) evaluates the SSIM
+// windows before the chamfer; the points backward gathers the windows' adjoint per point.  With flag 16 the same reduction carries
+// two more sums and finish also writes the reference view's gradients.  With both flags clear the launches are those of before.
 // The per-point arithmetic lives in nnb_refstage.cuh and is checked on the CPU against oracle.ref_stage; the kernels are
 // checked on hardware by tests/test_gpu_parity.py (test_native_ref_stage_vs_oracle, full-loss trainer goldens).
 #include "nnb_common.cuh"
@@ -14,12 +17,14 @@ namespace {
 using refstage::Geom;
 using refstage::Point;
 using refstage::kAcc;
+using refstage::kAccRef;
 
 struct Scratch {       // device-resident state of one call (512 B at the start of the workspace)
   Geom G;
   const float* img1; const float* img2;    // the two frames in the order of the warp (training.py:296-313)
   float sum_abs, nvalid, loss_pc, w_pc;    // w_pc sits next to loss_pc: the chamfer reads its weight from device memory
-  float acc[kAcc];
+  float acc[kAcc + kAccRef];
+  float sum_ssim;                          // SSIM map summed over valid points and channels (flag 8)
 };
 static_assert(sizeof(Scratch) <= 512, "scratch layout");
 
@@ -37,7 +42,8 @@ __global__ void rs_prep_k(Scratch* S, Geom G0, nnb_refstage_args a) {
   const float* ref = a.img_pp ? a.img_pp[1] : a.img_ref;
   S->G = G; S->img1 = G.is_last ? ref : cur; S->img2 = G.is_last ? cur : ref;
   S->sum_abs = 0.f; S->nvalid = 0.f; S->loss_pc = 0.f; S->w_pc = G.w_pc;
-  for (int i = 0; i < kAcc; ++i) S->acc[i] = 0.f;
+  for (int i = 0; i < kAcc + kAccRef; ++i) S->acc[i] = 0.f;
+  S->sum_ssim = 0.f;
 }
 
 template <int K>
@@ -53,7 +59,9 @@ __device__ void block_reduce_add(float (&v)[K], float* dst) {   // sum v[k] over
   }
 }
 
-__global__ void rs_points_fwd_k(Scratch* S, const float* dpt_cur, const float* dpt_ref, float* Xs, float* Ys) {
+// rgb1 / rgb2 / vmask: with SSIM, both colours and the validity of EVERY point (the SSIM windows also read invalid points)
+__global__ void rs_points_fwd_k(Scratch* S, const float* dpt_cur, const float* dpt_ref, float* Xs, float* Ys, float* rgb1, float* rgb2,
+                                float* vmask) {
   const Geom& G = S->G;
   const int P = G.rh * G.rw, i = blockIdx.x * blockDim.x + threadIdx.x;
   float part[2] = {0.f, 0.f};
@@ -63,7 +71,18 @@ __global__ void rs_points_fwd_k(Scratch* S, const float* dpt_cur, const float* d
     const float s2 = G.scale_pcs ? G.s2 : 1.f;
 #pragma unroll
     for (int r = 0; r < 3; ++r) { Xs[3 * i + r] = p.X[r] / s2; Ys[3 * i + r] = p.pc2[r] / s2; }
-    if (G.w_rgb_s != 0.f && p.valid) {
+    if (G.with_ssim) {
+      float a[3], b[3];
+      refstage::point_rgb(G, S->img1, S->img2, p, a, b);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { rgb1[3 * i + c] = a[c]; rgb2[3 * i + c] = b[c]; }
+      vmask[i] = p.valid ? 1.f : 0.f;
+      if (G.w_rgb_s != 0.f && p.valid) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) part[0] += fminf(fabsf(a[c] - b[c]), 1.f);
+        part[1] = 1.f;
+      }
+    } else if (G.w_rgb_s != 0.f && p.valid) {
       float diff[3];
       refstage::point_rgb_diff(G, S->img1, S->img2, p, diff);
 #pragma unroll
@@ -74,19 +93,49 @@ __global__ void rs_points_fwd_k(Scratch* S, const float* dpt_cur, const float* d
   block_reduce_add<2>(part, &S->sum_abs);     // sum_abs, nvalid are adjacent
 }
 
-__global__ void rs_points_bwd_k(Scratch* S, const float* dpt_cur, const float* dpt_ref, const float* gXs, const float* gYs) {
+// SSIM map of every valid point's three windows (summed into sum_ssim) and the adjoint coefficients of every window (coef [P][3][3]);
+// a window centred on an invalid point has no loss and zero coefficients
+__global__ void rs_ssim_k(Scratch* S, const float* rgb1, const float* rgb2, const float* vmask, float* coef) {
   const Geom& G = S->G;
   const int P = G.rh * G.rw, i = blockIdx.x * blockDim.x + threadIdx.x;
-  float acc[kAcc];
+  float part[1] = {0.f};
+  if (i < P) {
+    const int row = i / G.rw, col = i - row * G.rw;
+    const size_t ro = (size_t)row * 3 * G.rw;
+    const bool valid = vmask[i] != 0.f;
+    const float g = (valid && G.w_rgb_s != 0.f && S->nvalid > 0.f) ? 0.85f * (G.w_rgb_s / (3.f * S->nvalid)) : 0.f;
 #pragma unroll
-  for (int k = 0; k < kAcc; ++k) acc[k] = 0.f;
+    for (int c = 0; c < 3; ++c) {
+      const float m = refstage::ssim_window(rgb1 + ro, rgb2 + ro, G.rw, col, c, g, coef + 9 * (size_t)i + 3 * c);
+      if (valid) part[0] += m;
+    }
+  }
+  block_reduce_add<1>(part, &S->sum_ssim);
+}
+
+// NA = kAcc, or kAcc + kAccRef with gradients into the reference view.  With SSIM, each point first gathers d loss / d rgb_pc1_proj
+// from the windows that read it (rgb1 / rgb2 / coef non-null).
+template <int NA>
+__global__ void rs_points_bwd_k(Scratch* S, const float* dpt_cur, const float* dpt_ref, const float* gXs, const float* gYs, const float* rgb1,
+                                const float* rgb2, const float* coef) {
+  const Geom& G = S->G;
+  const int P = G.rh * G.rw, i = blockIdx.x * blockDim.x + threadIdx.x;
+  float acc[NA];
+#pragma unroll
+  for (int k = 0; k < NA; ++k) acc[k] = 0.f;
   if (i < P) {
     Point p;
     refstage::point_forward(G, dpt_cur, dpt_ref, i, p);
     const float inv_nv = (G.w_rgb_s != 0.f && S->nvalid > 0.f) ? G.w_rgb_s / (3.f * S->nvalid) : 0.f;
-    refstage::point_backward(G, S->img1, S->img2, p, gXs + 3 * i, gYs + 3 * i, inv_nv, acc);
+    float g2[3] = {0.f, 0.f, 0.f};
+    if (G.with_ssim) {
+      const int row = i / G.rw, col = i - row * G.rw;
+      const size_t ro = (size_t)row * 3 * G.rw;
+      refstage::ssim_gather(rgb1 + ro, rgb2 + ro, coef + 3 * ro, G.rw, col, g2);
+    }
+    refstage::point_backward(G, S->img1, S->img2, p, gXs + 3 * i, gYs + 3 * i, inv_nv, g2, acc);
   }
-  block_reduce_add<kAcc>(acc, S->acc);
+  block_reduce_add<NA>(acc, S->acc);
 }
 
 __global__ void rs_finish_k(const Scratch* S, nnb_refstage_args a) {
@@ -94,7 +143,7 @@ __global__ void rs_finish_k(const Scratch* S, nnb_refstage_args a) {
   float g[16], gs, gh;
   refstage::finish(S->G, a.c2w_cur, a.c2w_ref, S->acc, g, &gs, &gh);
   const float l_pc = S->G.w_pc != 0.f ? S->loss_pc : 0.f;
-  const float l_rgbs = S->nvalid > 0.f ? S->sum_abs / (3.f * S->nvalid) : 0.f;
+  const float l_rgbs = S->nvalid > 0.f ? (S->G.with_ssim ? 0.15f * S->sum_abs + 0.85f * S->sum_ssim : S->sum_abs) / (3.f * S->nvalid) : 0.f;
   a.losses[0] = l_pc; a.losses[1] = l_rgbs;
   if (a.loss_total) atomicAdd(a.loss_total, S->G.w_pc * l_pc + S->G.w_rgb_s * l_rgbs);
   const float gsc = a.grad_scale == 0.f ? 1.f : a.grad_scale;
@@ -102,6 +151,12 @@ __global__ void rs_finish_k(const Scratch* S, nnb_refstage_args a) {
   if (a.g_c2w) for (int i = 0; i < 12; ++i) atomicAdd(a.g_c2w + i, gsc * g[i]);
   if (a.g_dist) { atomicAdd(a.g_dist, gsc * gs); atomicAdd(a.g_dist + 1, gsc * gh); }
   if (a.g_kxy) { atomicAdd(a.g_kxy, gsc * S->acc[15]); atomicAdd(a.g_kxy + 1, gsc * S->acc[16]); }
+  if (S->G.grad_ref) {
+    float gr[16], grs, grh;
+    refstage::finish_ref(S->G, a.c2w_cur, a.c2w_ref, S->acc, gr, &grs, &grh);
+    for (int i = 0; i < 12; ++i) atomicAdd(a.g_c2w_ref + i, gsc * gr[i]);
+    atomicAdd(a.g_dist_ref, gsc * grs); atomicAdd(a.g_dist_ref + 1, gsc * grh);
+  }
 }
 
 }  // namespace
@@ -111,28 +166,40 @@ size_t refstage_workspace_bytes(int hd, int wd, int ratio) {
   return 512 + P * (4 * 3 * sizeof(float) + 2 * sizeof(unsigned long long));
 }
 
+// flag 8 (SSIM) appends rgb1 [P][3], rgb2 [P][3], vmask [P] and the window coefficients [P][3][3]
+size_t refstage_workspace_bytes_flags(int hd, int wd, int ratio, unsigned flags) {
+  const size_t P = (size_t)(hd / ratio) * (size_t)(wd / ratio);
+  return refstage_workspace_bytes(hd, wd, ratio) + ((flags & 8u) ? P * (3 + 3 + 1 + 9) * sizeof(float) : 0);
+}
+
 cudaError_t launch_refstage(const nnb_refstage_args& a, cudaStream_t st) {
   Geom G0{};
   G0.H = a.H; G0.W = a.W; G0.hd = a.h_d; G0.wd = a.w_d; G0.rh = a.h_d / a.pc_ratio; G0.rw = a.w_d / a.pc_ratio;
   G0.kx = a.kx; G0.ky = a.ky; G0.nl = a.nearest_limit; G0.w_pc = a.w_pc; G0.w_rgb_s = a.w_rgb_s;
   G0.is_last = a.is_last ? 1 : 0; G0.scale_pcs = (a.flags & 1u) ? 1 : 0; G0.detach_rgbs_scale = (a.flags & 2u) ? 1 : 0;
-  G0.shift_first = (a.flags & 4u) ? 1 : 0;
+  G0.shift_first = (a.flags & 4u) ? 1 : 0; G0.with_ssim = (a.flags & 8u) ? 1 : 0; G0.grad_ref = (a.flags & 16u) ? 1 : 0;
   const int P = G0.rh * G0.rw;
   char* base = static_cast<char*>(a.workspace);
   Scratch* S = reinterpret_cast<Scratch*>(base);
   float* Xs = reinterpret_cast<float*>(base + 512); float* Ys = Xs + 3 * (size_t)P;
   float* gXs = Ys + 3 * (size_t)P; float* gYs = gXs + 3 * (size_t)P;
   unsigned long long* kxy = reinterpret_cast<unsigned long long*>(gYs + 3 * (size_t)P); unsigned long long* kyx = kxy + P;
+  float* rgb1 = nullptr; float* rgb2 = nullptr; float* vmask = nullptr; float* coef = nullptr;
+  if (G0.with_ssim) {
+    rgb1 = reinterpret_cast<float*>(kyx + P); rgb2 = rgb1 + 3 * (size_t)P; vmask = rgb2 + 3 * (size_t)P; coef = vmask + P;
+  }
   rs_prep_k<<<1, 32, 0, st>>>(S, G0, a);
   const int nb = (P + 127) / 128;
-  rs_points_fwd_k<<<nb, 128, 0, st>>>(S, a.dpt_cur, a.dpt_ref, Xs, Ys);
+  rs_points_fwd_k<<<nb, 128, 0, st>>>(S, a.dpt_cur, a.dpt_ref, Xs, Ys, rgb1, rgb2, vmask);
+  if (G0.with_ssim) rs_ssim_k<<<nb, 128, 0, st>>>(S, rgb1, rgb2, vmask, coef);
   cudaError_t e = cudaMemsetAsync(gXs, 0, sizeof(float) * 6 * (size_t)P, st);
   if (e != cudaSuccess) return e;
   if (a.w_pc != 0.f || a.weights_dev) {      // device-resident weights: the term is always evaluated (a weight of 0 zeroes its gradients)
     e = launch_chamfer_dev(Xs, P, Ys, P, kxy, kyx, &S->loss_pc, &S->w_pc, gXs, gYs, st);
     if (e != cudaSuccess) return e;
   }
-  rs_points_bwd_k<<<nb, 128, 0, st>>>(S, a.dpt_cur, a.dpt_ref, gXs, gYs);
+  if (G0.grad_ref) rs_points_bwd_k<kAcc + kAccRef><<<nb, 128, 0, st>>>(S, a.dpt_cur, a.dpt_ref, gXs, gYs, rgb1, rgb2, coef);
+  else rs_points_bwd_k<kAcc><<<nb, 128, 0, st>>>(S, a.dpt_cur, a.dpt_ref, gXs, gYs, rgb1, rgb2, coef);
   rs_finish_k<<<1, 32, 0, st>>>(S, a);
   return cudaGetLastError();
 }

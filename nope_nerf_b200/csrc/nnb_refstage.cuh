@@ -22,8 +22,11 @@ struct Geom {            // everything a point needs besides the image / depth p
   float s2;                      // scale both clouds are divided by (scale_pcs), training.py:357-359
   int is_last, scale_pcs, detach_rgbs_scale, shift_first;
   float w_pc, w_rgb_s;           // loss weights (annealed per epoch, training.py:208-217)
+  int with_ssim;                 // warped-RGB term 0.15 L1 + 0.85 SSIM (training.with_ssim, losses.py:150-157)
+  int grad_ref;                  // gradients into the reference view too (training.detach_ref_img = False, training.py:288-292)
 };
 constexpr int kAcc = 17;         // reduced sums: gR (9) | gt (3) | g_s2 | g_scale_cur | g_shift_cur | g_kx | g_ky
+constexpr int kAccRef = 2;       // with grad_ref, after those: g_scale_ref (through the reference depth) | g_shift_ref
 
 // F.interpolate(..., mode='nearest') source index: floor(dst * in/out), scale in float32 (training.py:318-319)
 NNB_HD int nearest_src(int dst, int n_in, int n_out) {
@@ -72,6 +75,8 @@ struct Point {           // forward state of one low-resolution pixel
   float px, py;          // arange_pixels coordinates in [-1,1] (model/common.py:13-39)
   float raw_cur;         // raw DPT depth of the current view at this pixel (d scale / d shift need it)
   int live_cur;          // current view's depth not clamped to nearest_limit
+  float raw_ref;         // the same for the reference view
+  int live_ref;
   float pc1[3], pc2[3];  // back-projected clouds (transform_to_world with the identity pose, model/common.py:112-160)
   float X[3];            // R pc1 + t
   int bad, valid;        // behind-camera fix-up (training.py:334-335), |xy| <= 1 (project_to_cam)
@@ -83,12 +88,13 @@ NNB_HD void point_forward(const Geom& G, const float* dpt_cur, const float* dpt_
   p.px = 2.f * (float)col / (float)(G.rw - 1) - 1.f; p.py = 2.f * (float)row / (float)(G.rh - 1) - 1.f;
   const int sr = nearest_src(row, G.hd, G.rh), sc = nearest_src(col, G.wd, G.rw);
   p.raw_cur = dpt_cur[(size_t)sr * G.wd + sc];
-  const float raw_ref = dpt_ref[(size_t)sr * G.wd + sc];
+  p.raw_ref = dpt_ref[(size_t)sr * G.wd + sc];
   float dc = G.shift_first ? (p.raw_cur + G.h_cur) * G.s_cur : p.raw_cur * G.s_cur + G.h_cur;           // training.py:241-245
-  float dr = G.shift_first ? (raw_ref + G.h_ref) * G.s_ref : raw_ref * G.s_ref + G.h_ref;               // training.py:283-287
+  float dr = G.shift_first ? (p.raw_ref + G.h_ref) * G.s_ref : p.raw_ref * G.s_ref + G.h_ref;           // training.py:283-287
   p.live_cur = dc >= G.nl;
   if (!p.live_cur) dc = G.nl;                                                                          // d[d < nl] = nl (training.py:320-321)
-  if (dr < G.nl) dr = G.nl;
+  p.live_ref = !(dr < G.nl);
+  if (!p.live_ref) dr = G.nl;
   const float d1 = G.is_last ? dr : dc, d2 = G.is_last ? dc : dr;
   p.pc1[0] = p.px * d1 / G.kx; p.pc1[1] = p.py * d1 / G.ky; p.pc1[2] = -d1;
   p.pc2[0] = p.px * d2 / G.kx; p.pc2[1] = p.py * d2 / G.ky; p.pc2[2] = -d2;
@@ -108,10 +114,74 @@ NNB_HD void point_rgb_diff(const Geom& G, const float* img1, const float* img2, 
   for (int c = 0; c < 3; ++c) diff[c] = a[c] - b[c];
 }
 
+// the two colours of a point: rgb_pc1 (img1 on the fixed grid) and rgb_pc1_proj (img2 at the projection), training.py:326-333
+NNB_HD void point_rgb(const Geom& G, const float* img1, const float* img2, const Point& p, float a[3], float b[3]) {
+  sample_lowres(img1, G, p.px, p.py, a, nullptr, nullptr);
+  sample_lowres(img2, G, p.xy[0], p.xy[1], b, nullptr, nullptr);
+}
+
+// ---- SSIM of the warped-RGB term (class SSIM, losses.py:222-253) ----
+// training.py:338-343 hands Loss channel-last (1, rh, rw, 3) maps, so SSIM sees rh channels of (rw x 3) images: its 3x3 windows slide
+// over (column, colour channel) inside ONE low-resolution row, with reflection padding of both axes.  x, y: one row, element
+// (col, ch) at [3 col + ch]; x = rgb_pc1 (data), y = rgb_pc1_proj (the only input with a gradient).
+constexpr float kSsimC1 = 0.01f * 0.01f, kSsimC2 = 0.03f * 0.03f;
+NNB_HD int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
+
+// map value clamp((1 - SSIM) / 2, 0, 1) of the window centred at (col, ch).  With coef: the window's adjoint for a cotangent g on the
+// map value, as coefficients of (E[y], E[y^2], E[xy]) divided by 9, so that d map / d y_tap = coef0 + 2 coef1 y_tap + coef2 x_tap
+NNB_HD float ssim_window(const float* x, const float* y, int rw, int col, int ch, float g, float* coef) {
+  float sx = 0.f, sy = 0.f, sxx = 0.f, syy = 0.f, sxy = 0.f;
+  for (int i = -1; i <= 1; ++i) {
+    const int cc = reflect_idx(col + i, rw);
+    for (int j = -1; j <= 1; ++j) {
+      const int k = 3 * cc + reflect_idx(ch + j, 3);
+      const float a = x[k], b = y[k];
+      sx += a; sy += b; sxx += a * a; syy += b * b; sxy += a * b;
+    }
+  }
+  const float mx = sx / 9.f, my = sy / 9.f;
+  const float vx = sxx / 9.f - mx * mx, vy = syy / 9.f - my * my, cxy = sxy / 9.f - mx * my;
+  const float a1 = 2.f * mx * my + kSsimC1, a2 = 2.f * cxy + kSsimC2;
+  const float b1 = mx * mx + my * my + kSsimC1, b2 = vx + vy + kSsimC2;
+  const float S = a1 * a2 / (b1 * b2);
+  const float raw = (1.f - S) * 0.5f;
+  if (coef) {
+    coef[0] = coef[1] = coef[2] = 0.f;
+    if (g != 0.f && raw >= 0.f && raw <= 1.f) {               // torch.clamp passes the gradient on [0, 1]
+      const float gs = -0.5f * g;
+      const float d_my = gs * (2.f * mx * a2 / (b1 * b2) - S * 2.f * my / b1);
+      const float d_vy = gs * (-S / b2);
+      const float d_cxy = gs * (2.f * a1 / (b1 * b2));
+      coef[0] = (d_my - 2.f * my * d_vy - mx * d_cxy) / 9.f; coef[1] = d_vy / 9.f; coef[2] = d_cxy / 9.f;
+    }
+  }
+  return raw < 0.f ? 0.f : (raw > 1.f ? 1.f : raw);
+}
+
+// gather form of the SSIM adjoint: d loss / d y at the three channels of column `col`, summed over every window that reads them
+// (a reflected tap reads an element twice and counts twice).  coef: one row, 3 coefficients per window centre at [9 col + 3 ch].
+NNB_HD void ssim_gather(const float* x, const float* y, const float* coef, int rw, int col, float g[3]) {
+  g[0] = g[1] = g[2] = 0.f;
+  for (int xc = col - 1; xc <= col + 1; ++xc) {
+    if (xc < 0 || xc >= rw) continue;
+    const int ncol = (reflect_idx(xc - 1, rw) == col) + (xc == col) + (reflect_idx(xc + 1, rw) == col);
+    if (!ncol) continue;
+    for (int cc = 0; cc < 3; ++cc) {
+      const float* k = coef + 9 * xc + 3 * cc;
+      for (int ch = 0; ch < 3; ++ch) {
+        const int nch = (reflect_idx(cc - 1, 3) == ch) + (cc == ch) + (reflect_idx(cc + 1, 3) == ch);
+        if (nch) g[ch] += (float)(ncol * nch) * (k[0] + 2.f * k[1] * y[3 * col + ch] + k[2] * x[3 * col + ch]);
+      }
+    }
+  }
+}
+
 // Adjoint of one point.  gXs, gYs: d(w_pc * chamfer) / d(scaled clouds) of this point (already weighted); inv_nv: w_rgb_s /
-// (3 * #valid) or 0.  Accumulates into acc[kAcc] = { gR (9, row-major), gt (3), g_s2, g_scale_cur, g_shift_cur, g_kx, g_ky }.
+// (3 * #valid) or 0; g_rgb2: with G.with_ssim, d(SSIM part) / d rgb_pc1_proj of this point (ssim_gather), else unused.
+// Accumulates into acc = { gR (9, row-major), gt (3), g_s2, g_scale_cur, g_shift_cur, g_kx, g_ky } and, with G.grad_ref,
+// { g_scale_ref, g_shift_ref } after them (kAcc + kAccRef entries).
 NNB_HD void point_backward(const Geom& G, const float* img1, const float* img2, const Point& p, const float gXs[3], const float gYs[3],
-                           float inv_nv, float acc[kAcc]) {
+                           float inv_nv, const float* g_rgb2, float* acc) {
   float gX[3] = {0.f, 0.f, 0.f}, gXr[3] = {0.f, 0.f, 0.f}, gY[3];
   const float s2 = G.scale_pcs ? G.s2 : 1.f;
   float gs2 = 0.f;
@@ -119,10 +189,11 @@ NNB_HD void point_backward(const Geom& G, const float* img1, const float* img2, 
     gX[r] = gXs[r] / s2; gY[r] = gYs[r] / s2;
     if (G.scale_pcs) gs2 -= (gXs[r] * (p.X[r] / s2) + gYs[r] * (p.pc2[r] / s2)) / s2;
   }
-  if (inv_nv != 0.f && p.valid) {
+  if (inv_nv != 0.f && (p.valid || G.with_ssim)) {       // SSIM windows also read the warped colour of invalid points
     float diff[3], gp[3], dummy[3], gxy[2];
     point_rgb_diff(G, img1, img2, p, diff);
-    for (int c = 0; c < 3; ++c) gp[c] = (fabsf(diff[c]) < 1.f) ? -(diff[c] > 0.f ? 1.f : (diff[c] < 0.f ? -1.f : 0.f)) * inv_nv : 0.f;
+    for (int c = 0; c < 3; ++c) gp[c] = (p.valid && fabsf(diff[c]) < 1.f) ? -(diff[c] > 0.f ? 1.f : (diff[c] < 0.f ? -1.f : 0.f)) * inv_nv : 0.f;
+    if (G.with_ssim) for (int c = 0; c < 3; ++c) gp[c] = 0.15f * gp[c] + g_rgb2[c];
     sample_lowres(img2, G, p.xy[0], p.xy[1], dummy, gp, gxy);
     {                                                      // xy = (kx Xc_x, ky Xc_y) / z: the projection's own d/dK (also for fixed-up points)
       const float z = -p.Xc[2];
@@ -148,6 +219,13 @@ NNB_HD void point_backward(const Geom& G, const float* img1, const float* img2, 
   if (!p.live_cur) gd = 0.f;
   if (G.shift_first) { acc[13] += gd * (p.raw_cur + G.h_cur); acc[14] += gd * G.s_cur; }
   else { acc[13] += gd * p.raw_cur; acc[14] += gd; }
+  if (G.grad_ref) {                                     // the other cloud was built from the reference view's depth
+    const float* gr_src = G.is_last ? gpc1 : gY;
+    float gdr = gr_src[0] * p.px / G.kx + gr_src[1] * p.py / G.ky - gr_src[2];
+    if (!p.live_ref) gdr = 0.f;
+    if (G.shift_first) { acc[kAcc] += gdr * (p.raw_ref + G.h_ref); acc[kAcc + 1] += gdr * G.s_ref; }
+    else { acc[kAcc] += gdr * p.raw_ref; acc[kAcc + 1] += gdr; }
+  }
   // back-projection (x d / kx, y d / ky, -d): d pc_x / d kx = -pc_x / kx, for both clouds
   acc[15] -= (gpc1[0] * p.pc1[0] + gY[0] * p.pc2[0]) / G.kx;
   acc[16] -= (gpc1[1] * p.pc1[1] + gY[1] * p.pc2[1]) / G.ky;
@@ -196,6 +274,28 @@ NNB_HD void finish(const Geom& G, const float* c2w_cur, const float* c2w_ref, co
     *g_scale = acc[13] + acc[12];                                  // scale2 is the current view's own scale
   }
   *g_shift = acc[14];
+}
+
+// with G.grad_ref: reduced sums -> gradients w.r.t. the reference view's c2w (16, row-major), effective scale and shift
+NNB_HD void finish_ref(const Geom& G, const float* c2w_cur, const float* c2w_ref, const float* acc, float g_c2w_ref[16], float* g_scale,
+                       float* g_shift) {
+  float gM[16], inv[16], invT[16], tmp[16], tmp2[16];
+  for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) gM[4 * r + c] = acc[3 * r + c]; gM[4 * r + 3] = acc[9 + r]; }
+  gM[12] = gM[13] = gM[14] = gM[15] = 0.f;
+  if (!G.is_last) {
+    rigid_inverse(c2w_ref, inv);
+    for (int r = 0; r < 4; ++r) for (int c = 0; c < 4; ++c) { invT[4 * r + c] = inv[4 * c + r]; tmp[4 * r + c] = c2w_cur[4 * c + r]; }
+    mat4_mul(gM, tmp, tmp2);                                       // d loss / d inv(c2w_ref) = gM c2w^T
+    mat4_mul(invT, tmp2, tmp); mat4_mul(tmp, invT, g_c2w_ref);     // d inv(A) = -A^-1 dA A^-1
+    for (int i = 0; i < 16; ++i) g_c2w_ref[i] = -g_c2w_ref[i];
+    *g_scale = acc[kAcc] + acc[12];                                // scale2 is the reference view's scale
+  } else {
+    rigid_inverse(c2w_cur, inv);
+    for (int r = 0; r < 4; ++r) for (int c = 0; c < 4; ++c) invT[4 * r + c] = inv[4 * c + r];
+    mat4_mul(invT, gM, g_c2w_ref);                                 // M = inv(c2w) c2w_ref
+    *g_scale = acc[kAcc];
+  }
+  *g_shift = acc[kAcc + 1];
 }
 
 }  // namespace refstage

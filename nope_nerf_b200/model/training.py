@@ -204,11 +204,16 @@ class _GraphStep:
         if self.use_ref:
             self.dpt_ref = torch.zeros(hd, wd, device=dev)
             self.c2w_ref = torch.zeros(4, 4, device=dev); self.ss_ref = torch.zeros(2, device=dev)
-            nbytes = L.lib.nnb_refstage_workspace_bytes(hd, wd, int(tr.pc_ratio))
+            self.with_ssim = bool(tr.loss.cfg.get('with_ssim', False))
+            self.grad_ref = not tr.detach_ref_img
+            flags = ops.refstage_flags(tr.scale_pcs, tr.detach_rgbs_scale, tr.shift_first, self.with_ssim, self.grad_ref)
+            nbytes = L.lib.nnb_refstage_workspace_bytes_flags(hd, wd, int(tr.pc_ratio), flags)
             if nbytes == 0:
                 raise ValueError("reference-image stage: DPT map %dx%d too small for pc_ratio %d" % (hd, wd, tr.pc_ratio))
             self.rs_ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             self.side = torch.cuda.Stream(device=dev)
+            # training.detach_ref_img = False: [g_c2w_ref | g_scale_shift_ref] of the reference view, chained after the current view's
+            self.small_ref = torch.zeros(16 + 2, device=dev) if self.grad_ref else None
             self.stage = None                              # device staging of host frames (2,3,h,w), allocated on first use
         self.fadams = None
 
@@ -254,6 +259,9 @@ class _GraphStep:
         gbuf, gv = tr._grad_buffer(peer_step=True)
         self.small.zero_()
         g_c2w = self.small[:16].view(4, 4); g_ss = self.small[16:18]
+        grad_ref = self.use_ref and self.grad_ref
+        if grad_ref:
+            self.small_ref.zero_()
         ops.distortion_fwd_dev(dnet.global_scales.detach(), dnet.global_shifts.detach(), self.idx, dnet.fix_scaleN, self.ss)
         init = None if pose.init_c2w is None else pose.init_c2w.detach()
         ops.pose_fwd_dev(pose.r.detach(), pose.t.detach(), init, self.idx, self.c2w)
@@ -301,7 +309,9 @@ class _GraphStep:
                 ops.refstage_raw(self.c2w, self.ss, self.c2w_ref, self.ss_ref, self.dpt, self.dpt_ref, H=h, W=w, img_pp=self.imgpp, cam=self.cam,
                                  cam_idx_dev=self.idx, num_cams=pose.num_cams, weights_dev=self.wts[2:4], nearest_limit=tr.nearest_limit,
                                  pc_ratio=tr.pc_ratio, scale_pcs=tr.scale_pcs, detach_rgbs_scale=tr.detach_rgbs_scale, shift_first=tr.shift_first,
-                                 losses=self.rs_losses, g_c2w=g_c2w, g_dist=g_ss, loss_total=self.rs_total, grad_scale=gs, workspace=self.rs_ws)
+                                 losses=self.rs_losses, g_c2w=g_c2w, g_dist=g_ss, loss_total=self.rs_total, grad_scale=gs, workspace=self.rs_ws,
+                                 with_ssim=self.with_ssim, g_c2w_ref=self.small_ref[:16].view(4, 4) if grad_ref else None,
+                                 g_dist_ref=self.small_ref[16:18] if grad_ref else None)
             cur.wait_stream(self.side)
         self.keep.append((call, ws, ray_idx, noise))        # graph-owned memory stays referenced (and out of the workspace pool)
         ops.pose_bwd_dev(pose.r.detach(), pose.t.detach(), init, self.idx, g_c2w,
@@ -309,6 +319,12 @@ class _GraphStep:
         ops.distortion_bwd_dev(dnet.global_scales.detach(), self.idx, dnet.fix_scaleN, g_ss,
                                gv['scales'] if dnet.global_scales.requires_grad else None,
                                gv['shifts'] if dnet.global_shifts.requires_grad else None)
+        if grad_ref:                                        # the reference view's rows, after the current view's (fixed order)
+            ops.pose_bwd_dev(pose.r.detach(), pose.t.detach(), init, self.idx_ref, self.small_ref[:16].view(4, 4),
+                             gv['r'] if pose.r.requires_grad else None, gv['t'] if pose.t.requires_grad else None)
+            ops.distortion_bwd_dev(dnet.global_scales.detach(), self.idx_ref, dnet.fix_scaleN, self.small_ref[16:18],
+                                   gv['scales'] if dnet.global_scales.requires_grad else None,
+                                   gv['shifts'] if dnet.global_shifts.requires_grad else None)
         gv['losses'].copy_(self.out4 * gs if tr.world > 1 else self.out4)
         if self.use_ref:
             gv['losses'][0:1].add_(self.rs_total, alpha=gs)
@@ -656,15 +672,10 @@ class Trainer(object):
         return tot if found else None
 
     def _check_ref_stage_cfg(self):
-        """the fused reference-image stage (nnb_refstage) covers the reference's defaults"""
-        if not self.detach_ref_img:
-            raise NotImplementedError("training.detach_ref_img=False (gradients into the reference view) is not fused; the default is True "
-                                      "(configs/default.yaml:117)")
+        """the fused reference-image stage (nnb_refstage) covers every option the reference's own Trainer accepts (detach_ref_img and
+        with_ssim included); only 'dense' matching exists in the reference"""
         if self.match_method != 'dense':
             raise NotImplementedError("training.match_method=%r: only 'dense' (configs/default.yaml) is fused" % (self.match_method,))
-        if self.loss.cfg.get('with_ssim', False):
-            raise NotImplementedError("training.with_ssim=True: the SSIM term of the warped-RGB loss is available in Loss.get_rgb_s_loss for "
-                                      "direct callers but not in the fused reference-image stage (configs/default.yaml:109 is False)")
 
     # ------------------------------------------------------------------------------------
     def process_data_dict(self, data, keep_pinned=False):
@@ -818,7 +829,8 @@ class Trainer(object):
             init = None if pose.init_c2w is None else pose.init_c2w.detach()
             c2w_cur = torch.empty(4, 4, device=device); c2w_ref = torch.empty(4, 4, device=device)
             ops.pose_fwd_raw(pose.r.detach(), pose.t.detach(), init, img_idx, c2w_cur)
-            ops.pose_fwd_raw(pose.r.detach(), pose.t.detach(), init, ref_idx, c2w_ref)                  # detached (training.py:288-292)
+            ops.pose_fwd_raw(pose.r.detach(), pose.t.detach(), init, ref_idx, c2w_ref)
+            grad_ref = backward and not self.detach_ref_img       # training.py:288-292: gradients into the reference view too
             if self.distortion_net is not None:
                 s_ref, h_ref = self.distortion_net(ref_idx)
             else:
@@ -828,12 +840,15 @@ class Trainer(object):
             g_c2w_rs = torch.zeros(4, 4, device=device) if backward else None
             g_ss_rs = torch.zeros(2, device=device) if backward else None
             g_kxy_rs = torch.zeros(2, device=device) if (backward and fxfy is not None) else None
+            g_c2w_ref_rs = torch.zeros(4, 4, device=device) if grad_ref else None
+            g_ss_ref_rs = torch.zeros(2, device=device) if grad_ref else None
             ops.refstage_raw(c2w_cur, dist_cur, c2w_ref, dist_ref, depth_input.detach().reshape(h_depth, w_depth).contiguous(),
                              depth_ref.detach().reshape(h_depth, w_depth).contiguous(), H=h, W=w, img_cur=ops._f32c(img[0]), img_ref=ops._f32c(ref_img[0]),
                              is_last=(img_idx == V - 1), cam=cam_dev, nearest_limit=self.nearest_limit, pc_ratio=self.pc_ratio,
                              scale_pcs=self.scale_pcs, detach_rgbs_scale=self.detach_rgbs_scale, shift_first=self.shift_first,
                              w_pc=weights['pc_weight'], w_rgb_s=weights['rgb_s_weight'], losses=rs_losses, g_c2w=g_c2w_rs, g_dist=g_ss_rs,
-                             g_kxy=g_kxy_rs, loss_total=rs_total, grad_scale=grad_scale)
+                             g_kxy=g_kxy_rs, loss_total=rs_total, grad_scale=grad_scale, with_ssim=bool(self.loss.cfg.get('with_ssim', False)),
+                             g_c2w_ref=g_c2w_ref_rs, g_dist_ref=g_ss_ref_rs)
             if weights['pc_weight'] != 0.0: ref_terms['loss_pc'] = rs_losses[0]
             if weights['rgb_s_weight'] != 0.0: ref_terms['loss_rgb_s'] = rs_losses[1]
             loss_total = loss_total + rs_total[0]
@@ -849,6 +864,17 @@ class Trainer(object):
                     torch.autograd.backward(outs, gouts)
                 if g_kxy_rs is not None and fxfy.requires_grad:
                     fxfy.backward(torch.stack([g_kxy_rs[0], -g_kxy_rs[1]]))          # camera_mat = diag(fx, -fy, -1, 1)
+                if grad_ref:
+                    ops.pose_bwd_raw(pose.r.detach(), pose.t.detach(), init, ref_idx, g_c2w_ref_rs,
+                                     gv['r'] if pose.r.requires_grad else None, gv['t'] if pose.t.requires_grad else None)
+                    # through Learn_Distortion(ref_idx): its clamp and the fixed scale of the last view leave constants without a gradient
+                    outs, gouts = [], []
+                    if s_ref.requires_grad:
+                        outs.append(s_ref); gouts.append(g_ss_ref_rs[0:1].reshape(s_ref.shape))
+                    if h_ref.requires_grad:
+                        outs.append(h_ref); gouts.append(g_ss_ref_rs[1:2].reshape(h_ref.shape))
+                    if outs:
+                        torch.autograd.backward(outs, gouts)
 
         # pose-smoothness terms (losses.py:103-112, weight 0 by default): every rank holds the same t, so each contributes
         # 1/world of the gradient BEFORE the all-reduce sums the ranks

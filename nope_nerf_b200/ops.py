@@ -305,18 +305,27 @@ def chamfer(X, Y):
 _rs_ws = {}
 
 
+def refstage_flags(scale_pcs=True, detach_rgbs_scale=False, shift_first=False, with_ssim=False, grad_ref=False):
+    """nnb_refstage_args.flags"""
+    return ((L.RS_SCALE_PCS if scale_pcs else 0) | (L.RS_DETACH_RGBS_SCALE if detach_rgbs_scale else 0) | (L.RS_SHIFT_FIRST if shift_first else 0) |
+            (L.RS_WITH_SSIM if with_ssim else 0) | (L.RS_GRAD_REF if grad_ref else 0))
+
+
 def refstage_raw(c2w_cur, dist_cur, c2w_ref, dist_ref, dpt_cur, dpt_ref, *, H, W, img_cur=None, img_ref=None, img_pp=None, is_last=False,
                  kx=0.0, ky=0.0, cam=None, cam_idx_dev=None, num_cams=0, weights_dev=None, nearest_limit=0.01, pc_ratio=4, scale_pcs=True,
                  detach_rgbs_scale=False, shift_first=False, w_pc=1.0, w_rgb_s=1.0, losses=None, g_c2w=None, g_dist=None, g_kxy=None,
-                 loss_total=None, grad_scale=1.0, workspace=None):
+                 loss_total=None, grad_scale=1.0, workspace=None, with_ssim=False, g_c2w_ref=None, g_dist_ref=None):
     """nnb_refstage: the reference-image stage of Trainer.compute_loss (model/training.py:280-365), forward + adjoint in one call.
-    All tensor arguments are device tensors (frames may be page-locked host tensors); g_* / loss_total ACCUMULATE."""
+    All tensor arguments are device tensors (frames may be page-locked host tensors); g_* / loss_total ACCUMULATE.
+    with_ssim: warped-RGB loss 0.15 L1 + 0.85 SSIM (training.with_ssim).  g_c2w_ref (4,4) / g_dist_ref (2): also the gradients w.r.t. the
+    reference view's pose matrix and effective distortion (training.detach_ref_img = False); both or neither."""
     _need_cuda(c2w_cur, "c2w_cur")
     for n_, t_ in (("img_cur", img_cur), ("img_ref", img_ref)):
         _need_cuda(t_, n_, allow_pinned=True)
     dev = c2w_cur.device
     hd, wd = int(dpt_cur.shape[-2]), int(dpt_cur.shape[-1])
-    nbytes = L.lib.nnb_refstage_workspace_bytes(hd, wd, int(pc_ratio))
+    flags = refstage_flags(scale_pcs, detach_rgbs_scale, shift_first, with_ssim, g_c2w_ref is not None or g_dist_ref is not None)
+    nbytes = L.lib.nnb_refstage_workspace_bytes_flags(hd, wd, int(pc_ratio), flags)
     if nbytes == 0:
         raise ValueError("reference-image stage: DPT map %dx%d too small for pc_ratio %d" % (hd, wd, pc_ratio))
     if workspace is None:
@@ -330,56 +339,70 @@ def refstage_raw(c2w_cur, dist_cur, c2w_ref, dist_ref, dpt_cur, dpt_ref, *, H, W
     a.img_cur, a.img_ref, a.dpt_cur, a.dpt_ref = L.ptr(img_cur), L.ptr(img_ref), L.ptr(dpt_cur), L.ptr(dpt_ref)
     a.c2w_cur, a.c2w_ref, a.dist_cur, a.dist_ref = L.ptr(c2w_cur), L.ptr(c2w_ref), L.ptr(dist_cur), L.ptr(dist_ref)
     a.H, a.W, a.h_d, a.w_d, a.pc_ratio, a.is_last = int(H), int(W), hd, wd, int(pc_ratio), int(bool(is_last))
-    a.flags = (1 if scale_pcs else 0) | (2 if detach_rgbs_scale else 0) | (4 if shift_first else 0)
+    a.flags = flags
     a.kx, a.ky, a.nearest_limit, a.w_pc, a.w_rgb_s = float(kx), float(ky), float(nearest_limit), float(w_pc), float(w_rgb_s)
     a.losses, a.g_c2w, a.g_dist = L.ptr(losses), L.ptr(g_c2w), L.ptr(g_dist)
     a.workspace, a.workspace_bytes = L.ptr(workspace), workspace.numel()
     a.img_pp, a.cam, a.cam_idx_dev, a.num_cams, a.weights_dev = L.ptr(img_pp), L.ptr(cam), L.ptr(cam_idx_dev), int(num_cams), L.ptr(weights_dev)
     a.g_kxy, a.loss_total, a.grad_scale = L.ptr(g_kxy), L.ptr(loss_total), float(grad_scale)
+    a.g_c2w_ref, a.g_dist_ref = L.ptr(g_c2w_ref), L.ptr(g_dist_ref)
     L.check(L.lib.nnb_refstage(C.byref(a), _stream()), "nnb_refstage")
     return losses
 
 
 class _RefStageFn(torch.autograd.Function):
     """w_pc * loss_pc + w_rgb_s * loss_rgb_s of the reference-image stage (model/training.py:280-365) as a function of the current
-    view's pose matrix, effective distortion {scale, shift} and (kx, ky); forward and adjoint come out of ONE library call."""
+    view's pose matrix, effective distortion {scale, shift} and (kx, ky) and, when they require grad, the reference view's pose matrix
+    and distortion (training.detach_ref_img = False); forward and adjoint come out of ONE library call."""
 
     @staticmethod
     def forward(ctx, c2w_cur, dist_cur, kxy, c2w_ref, dist_ref, img_cur, img_ref, dpt_cur, dpt_ref, is_last, nearest_limit, pc_ratio,
-                scale_pcs, detach_rgbs_scale, shift_first, w_pc, w_rgb_s):
+                scale_pcs, detach_rgbs_scale, shift_first, w_pc, w_rgb_s, with_ssim):
         dev = c2w_cur.device
         f = lambda t: _f32c(t.detach())
         H, W = img_cur.shape[-2:]
         g_c2w = torch.zeros(4, 4, device=dev); g_dist = torch.zeros(2, device=dev); g_kxy = torch.zeros(2, device=dev)
+        grad_ref = ctx.needs_input_grad[3] or ctx.needs_input_grad[4]
+        g_c2w_ref = torch.zeros(4, 4, device=dev) if grad_ref else None
+        g_dist_ref = torch.zeros(2, device=dev) if grad_ref else None
         kx, ky = (float(v) for v in kxy.detach().cpu())
+        flags = refstage_flags(scale_pcs, detach_rgbs_scale, shift_first, with_ssim, grad_ref)
         losses = refstage_raw(f(c2w_cur), f(dist_cur), f(c2w_ref), f(dist_ref), _f32c(dpt_cur), _f32c(dpt_ref), H=H, W=W, img_cur=_f32c(img_cur),
                               img_ref=_f32c(img_ref), is_last=is_last, kx=kx, ky=ky, nearest_limit=nearest_limit, pc_ratio=pc_ratio,
                               scale_pcs=scale_pcs, detach_rgbs_scale=detach_rgbs_scale, shift_first=shift_first, w_pc=w_pc, w_rgb_s=w_rgb_s,
-                              g_c2w=g_c2w, g_dist=g_dist, g_kxy=g_kxy, workspace=torch.empty(
-                                  L.lib.nnb_refstage_workspace_bytes(int(dpt_cur.shape[-2]), int(dpt_cur.shape[-1]), int(pc_ratio)) or 1,
-                                  dtype=torch.uint8, device=dev))
-        ctx.save_for_backward(g_c2w, g_dist, g_kxy)
+                              g_c2w=g_c2w, g_dist=g_dist, g_kxy=g_kxy, with_ssim=with_ssim, g_c2w_ref=g_c2w_ref, g_dist_ref=g_dist_ref,
+                              workspace=torch.empty(L.lib.nnb_refstage_workspace_bytes_flags(int(dpt_cur.shape[-2]), int(dpt_cur.shape[-1]),
+                                                                                              int(pc_ratio), flags) or 1, dtype=torch.uint8, device=dev))
+        if grad_ref:
+            ctx.save_for_backward(g_c2w, g_dist, g_kxy, g_c2w_ref, g_dist_ref)
+        else:
+            ctx.save_for_backward(g_c2w, g_dist, g_kxy)
         ctx.mark_non_differentiable(losses)
         return float(w_pc) * losses[0] + float(w_rgb_s) * losses[1], losses
 
     @staticmethod
     def backward(ctx, g, _g_losses):
-        g_c2w, g_dist, g_kxy = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        g_c2w, g_dist, g_kxy = saved[:3]
+        g_c2w_ref, g_dist_ref = saved[3:] if len(saved) == 5 else (None, None)
         return (g_c2w * g if ctx.needs_input_grad[0] else None, g_dist * g if ctx.needs_input_grad[1] else None,
-                g_kxy * g if ctx.needs_input_grad[2] else None) + (None,) * 14
+                g_kxy * g if ctx.needs_input_grad[2] else None, g_c2w_ref * g if ctx.needs_input_grad[3] else None,
+                g_dist_ref * g if ctx.needs_input_grad[4] else None) + (None,) * 13
 
 
 def refstage(c2w_cur, dist_cur, c2w_ref, dist_ref, img_cur, img_ref, dpt_cur, dpt_ref, is_last, kx, ky, nearest_limit=0.01, pc_ratio=4,
-             scale_pcs=True, detach_rgbs_scale=False, shift_first=False, w_pc=1.0, w_rgb_s=1.0):
-    """(total, losses[2] = {loss_pc, loss_rgb_s}); total is differentiable w.r.t. c2w_cur (4,4), dist_cur = [scale_eff, shift] and, when
-    kx / ky are tensors, the intrinsics (autograd wrapper over refstage_raw; the Trainer calls refstage_raw directly)."""
+             scale_pcs=True, detach_rgbs_scale=False, shift_first=False, w_pc=1.0, w_rgb_s=1.0, with_ssim=False):
+    """(total, losses[2] = {loss_pc, loss_rgb_s}); total is differentiable w.r.t. c2w_cur (4,4), dist_cur = [scale_eff, shift], when
+    kx / ky are tensors the intrinsics, and when c2w_ref / dist_ref require grad the reference view's pose matrix and distortion
+    (training.detach_ref_img = False).  with_ssim: warped-RGB loss 0.15 L1 + 0.85 SSIM (training.with_ssim).  Autograd wrapper over
+    refstage_raw; the Trainer calls refstage_raw directly."""
     _need_cuda(c2w_cur, "c2w_cur")
     if isinstance(kx, torch.Tensor) or isinstance(ky, torch.Tensor):
         kxy = torch.stack([torch.as_tensor(kx, device=c2w_cur.device).reshape(()), torch.as_tensor(ky, device=c2w_cur.device).reshape(())])
     else:
         kxy = torch.tensor([float(kx), float(ky)], device=c2w_cur.device)
     return _RefStageFn.apply(c2w_cur, dist_cur, kxy, c2w_ref, dist_ref, img_cur, img_ref, dpt_cur, dpt_ref, is_last, nearest_limit, pc_ratio,
-                             scale_pcs, detach_rgbs_scale, shift_first, w_pc, w_rgb_s)
+                             scale_pcs, detach_rgbs_scale, shift_first, w_pc, w_rgb_s, bool(with_ssim))
 
 
 def adam_step(p, g, m, v, step, lr, beta1=0.9, beta2=0.999, eps=1e-8):

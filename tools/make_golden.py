@@ -206,11 +206,13 @@ def case_pose(mdl, name):
     print("wrote", name)
 
 
-def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_view=False, learn_focal=False):
-    """Trainer.train_step (model/training.py:67-97) for `steps` iterations on one synthetic pair."""
+def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_view=False, learn_focal=False, training=None):
+    """Trainer.train_step (model/training.py:67-97) for `steps` iterations on one synthetic pair; `training` overrides keys of
+    cfg['training'] (stored as cfg.training.<key>)."""
     import torch
     from oracle import nerf_oracle as O
     cfg = base_cfg()
+    cfg["training"].update(training or {})
     cfg["rendering"]["num_points"] = S; cfg["training"]["n_training_points"] = N
     if not with_ref:
         cfg["training"]["pc_weight"] = [0.0, 0.0]; cfg["training"]["rgb_s_weight"] = [0.0, 0.0]
@@ -251,6 +253,8 @@ def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_v
             "img.ref_idxs": torch.tensor([ref_idx])}
     rec = dict(N=N, S=S, H=H, W=W, V=V, seed=seed, idx=idx, ref_idx=ref_idx, kx=kx, ky=ky, img=img[0], ref=ref[0],
                dpt=dpt[0], rdpt=rdpt[0], r0=r0, t0=t0, scales0=sc0, shifts0=sh0, steps=steps, with_ref=with_ref)
+    for k, v in (training or {}).items():
+        rec["cfg.training." + k] = np.array(v)
     if learn_focal:
         rec["focal0"] = np.array([focal.fx.item(), focal.fy.item()], np.float32)
     for it in range(steps):
@@ -343,6 +347,15 @@ def main():
                         last_view=True)
     if "focal" in which or "train" in which:
         case_train_step(mdl, "train_learn_focal", True, steps=2, N=48, S=32, H=24, W=32, hd=16, wd=24, seed=34, learn_focal=True)
+    if "refopts" in which:
+        # training.with_ssim / training.detach_ref_img: False; a 32x48 DPT map gives an 8x12 low-resolution grid with interior columns
+        case_train_step(mdl, "train_full_ssim", True, steps=2, N=48, S=32, H=24, W=32, hd=32, wd=48, seed=35, training={"with_ssim": True})
+        case_train_step(mdl, "train_full_undetached", True, steps=2, N=48, S=32, H=24, W=32, hd=32, wd=48, seed=36,
+                        training={"detach_ref_img": False})
+        case_train_step(mdl, "train_full_undetached_lastview", True, steps=1, N=48, S=32, H=24, W=32, hd=32, wd=48, seed=37, last_view=True,
+                        training={"detach_ref_img": False})
+        case_train_step(mdl, "train_full_ssim_undetached_shiftfirst", True, steps=1, N=48, S=32, H=24, W=32, hd=32, wd=48, seed=38,
+                        training={"with_ssim": True, "detach_ref_img": False, "shift_first": True})
 
 
 if __name__ == "__main__":
