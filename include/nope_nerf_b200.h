@@ -47,7 +47,7 @@ extern "C" {
  * (model/network.py:19-20) + Renderer.nope_nerf (model/rendering.py:36-37) after the host
  * mirror has resolved world_mat -> c2w (training.py:238 / common.py:139-141). */
 typedef struct nnb_render_args {
-  const float* weights;   /* [NNB_NUM_PARAMS] flat, OfficialStaticNerf.parameters() order           */
+  const float* weights;   /* [nnb_num_params(hidden_dim)] flat, OfficialStaticNerf.parameters() order */
   const float* c2w;       /* [16] row-major camera-to-world (LearnPose.forward, poses.py:23-31)     */
   const float* cam;       /* [16] camera_mat diag(kx,ky,-1,1) (dataset.py:101-104); [0],[5] are read */
   const int64_t* ray_idx; /* [N] row-major pixel ids (training.py:257) or NULL                      */
@@ -73,6 +73,9 @@ typedef struct nnb_render_args {
   /* explicit-point field queries (nnb_field_fwd/bwd only; NULL for rendering): OfficialStaticNerf.forward(p, ray_d) */
   const float* pts;  /* [N,3] */
   const float* dirs; /* [N,3] or NULL (-> ones, like use_ray_dir = False) */
+  /* model.hidden_dim (official_nerf.py:11): 64, 128 or 256; 0 means 256.  `weights` / g_weights then hold nnb_num_params(hidden_dim)
+   * floats and the workspace is sized by nnb_workspace_bytes_dim(..., hidden_dim).  Other widths are rejected (rc < 0). */
+  int32_t hidden_dim;
 } nnb_render_args;
 
 typedef struct nnb_render_bwd_args {
@@ -81,7 +84,7 @@ typedef struct nnb_render_bwd_args {
   const float* g_depth_pred; /* [N] dense (0 where masked out) or NULL */
   const float* g_depth_gt;   /* [N] dense or NULL                      */
   /* outputs, all ACCUMULATED (+=): caller zeroes them */
-  float* g_weights; /* [NNB_NUM_PARAMS] or NULL (pose-only: Trainer_pose, eval_pose_one_epoch.py:25-41) */
+  float* g_weights; /* [nnb_num_params(fwd.hidden_dim)] or NULL (pose-only: Trainer_pose, eval_pose_one_epoch.py:25-41) */
   float* g_c2w;     /* [16] (rows 0..2 written) */
   float* g_cam;     /* [16] ([0],[5] written) or NULL */
   float* g_depth;   /* [N] d/d prior depth (overwritten) or NULL */
@@ -104,8 +107,12 @@ int nnb_profile_events(void** events, int32_t count);
 int nnb_profile_cursor(void);
 /* test aid: byte offsets of the workspace sections {records, h0..h7, feat, hr, enc, denc, total} */
 int nnb_debug_layout(int32_t N, int32_t S, uint32_t flags, int32_t engine, size_t* out14);
-/* bytes of workspace needed by nnb_render_fwd (+bwd when NNB_STASH) */
+/* bytes of workspace needed by nnb_render_fwd (+bwd when NNB_STASH) at hidden_dim 256 */
 size_t nnb_workspace_bytes(int32_t N, int32_t S, uint32_t flags, int32_t engine);
+/* the same for the field of width hidden_dim (0 = 256); 0 for an unsupported width */
+size_t nnb_workspace_bytes_dim(int32_t N, int32_t S, uint32_t flags, int32_t engine, int32_t hidden_dim);
+/* floats of the flat MLP parameter vector of width hidden_dim (0 = 256; NNB_NUM_PARAMS at 256); 0 for an unsupported width */
+size_t nnb_num_params(int32_t hidden_dim);
 int nnb_render_fwd(const nnb_render_args* a, void* stream);
 /* OfficialStaticNerf.forward(p, ray_d, return_addocc=True) on explicit points (model/official_nerf.py:69-96), exact-fp32
  * engine.  Uses a->pts/dirs, N points (S is ignored), weights, flags (NNB_DIST_ALPHA / NNB_SOFTPLUS / NNB_STASH) and the

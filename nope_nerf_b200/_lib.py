@@ -9,7 +9,8 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NNB_LIB_PATH") or os.path.join(HERE, "libnope_nerf_b200.so")   # NNB_LIB_PATH: instrumented debug builds
 
-NUM_PARAMS = 595844
+NUM_PARAMS = 595844              # hidden_dim 256; num_params(D) for the other widths
+HIDDEN_DIMS = (64, 128, 256)     # model.hidden_dim values with a kernel instantiation
 DIST_ALPHA, NDC, NORMALISE, USE_DIR, WHITE_BG, EVAL, SOFTPLUS, SHIFT_FIRST, STASH, TCBWD, WG16, RAW_DENSITY = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048
 FWD_DROP_WLO, FWD_DROP_ALO = 4096, 8192
 ENGINE_SIMT, ENGINE_TC = 0, 1
@@ -24,7 +25,7 @@ class RenderArgs(C.Structure):
                 ("N", C.c_int32), ("S", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("h_d", C.c_int32), ("w_d", C.c_int32),
                 ("near_", C.c_float), ("far_", C.c_float), ("flags", C.c_uint32), ("engine", C.c_int32),
                 ("rgb", _f), ("depth_pred", _f), ("depth_gt", _f), ("mask", _f), ("z_vals", _f), ("alpha", _f),
-                ("workspace", _f), ("workspace_bytes", C.c_size_t), ("pts", _f), ("dirs", _f)]
+                ("workspace", _f), ("workspace_bytes", C.c_size_t), ("pts", _f), ("dirs", _f), ("hidden_dim", C.c_int32)]
 
 
 class RenderBwdArgs(C.Structure):
@@ -66,6 +67,10 @@ def _load():
     lib.nnb_version.restype = C.c_int
     lib.nnb_workspace_bytes.restype = C.c_size_t
     lib.nnb_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_uint32, C.c_int32]
+    lib.nnb_workspace_bytes_dim.restype = C.c_size_t
+    lib.nnb_workspace_bytes_dim.argtypes = [C.c_int32, C.c_int32, C.c_uint32, C.c_int32, C.c_int32]
+    lib.nnb_num_params.restype = C.c_size_t
+    lib.nnb_num_params.argtypes = [C.c_int32]
     lib.nnb_render_fwd.argtypes = [C.POINTER(RenderArgs), C.c_void_p]
     lib.nnb_render_bwd.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
     lib.nnb_field_fwd.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]
@@ -108,6 +113,14 @@ EXPORTS = ["nnb_last_error", "nnb_version", "nnb_profile_events", "nnb_profile_c
 def check(rc, what):
     if rc != 0:
         raise RuntimeError("%s failed (%d): %s" % (what, rc, lib.nnb_last_error().decode()))
+
+
+def num_params(hidden_dim=256):
+    """floats in the flat MLP parameter vector of OfficialStaticNerf at width hidden_dim (ValueError for an unsupported width)"""
+    n = lib.nnb_num_params(int(hidden_dim))
+    if n == 0:
+        raise ValueError("hidden_dim %s is not supported (supported: %s)" % (hidden_dim, ", ".join(map(str, HIDDEN_DIMS))))
+    return int(n)
 
 
 def ptr(t):

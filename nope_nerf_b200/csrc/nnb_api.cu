@@ -13,7 +13,7 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
-size_t tc_workspace_extra(int N, int S, uint32_t flags);
+size_t tc_workspace_extra(int N, int S, uint32_t flags, int D);
 bool tc_supports(int S);
 #endif
 cudaError_t launch_pose_fwd(const float*, const float*, const float*, int, const int*, float*, cudaStream_t);
@@ -68,14 +68,31 @@ int nnb_debug_layout(int32_t N, int32_t S, uint32_t flags, int32_t engine, size_
   return 0;
 }
 
-size_t nnb_workspace_bytes(int32_t N, int32_t S, uint32_t flags, int32_t engine) {
-  if (N <= 0 || S <= 0) return 0;
-  WsLayout L = make_layout(N, S, flags, engine);
+// model.hidden_dim of a call: 0 means 256
+static int hidden_of(int32_t hidden_dim) { return hidden_dim == 0 ? 256 : hidden_dim; }
+
+size_t nnb_num_params(int32_t hidden_dim) {
+  const int D = hidden_of(hidden_dim);
+  return nnb::dim_supported(D) ? (size_t)nnb::num_params(D) : 0;
+}
+
+size_t nnb_workspace_bytes_dim(int32_t N, int32_t S, uint32_t flags, int32_t engine, int32_t hidden_dim) {
+  const int D = hidden_of(hidden_dim);
+  if (N <= 0 || S <= 0 || !nnb::dim_supported(D)) return 0;
+  WsLayout L = make_layout(N, S, flags, engine, D);
   size_t tot = L.total;
 #ifdef NNB_WITH_TC
-  if (engine == NNB_ENGINE_TC) tot += tc_workspace_extra(N, S, flags);
+  if (engine == NNB_ENGINE_TC) tot += tc_workspace_extra(N, S, flags, D);
 #endif
   return tot;
+}
+
+size_t nnb_workspace_bytes(int32_t N, int32_t S, uint32_t flags, int32_t engine) { return nnb_workspace_bytes_dim(N, S, flags, engine, 256); }
+
+static int check_dim(const nnb_render_args* a) {
+  if (!nnb::dim_supported(hidden_of(a->hidden_dim)))
+    return fail(-8, "hidden_dim %d is not supported (supported: 64, 128, 256; 0 means 256)", a->hidden_dim);
+  return 0;
 }
 
 static int check_args(const nnb_render_args* a) {
@@ -89,13 +106,14 @@ static int check_args(const nnb_render_args* a) {
     return fail(-3, "need depth[N] or (depth_map,h_d,w_d,H,W,ray_idx)");
   if (!a->rgb || !a->depth_pred || !a->depth_gt || !a->mask) return fail(-3, "output pointers must be non-null");
   if (a->engine != NNB_ENGINE_SIMT && a->engine != NNB_ENGINE_TC) return fail(-4, "unknown engine %d", a->engine);
+  if (int rc = check_dim(a)) return rc;
 #ifndef NNB_WITH_TC
   if (a->engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
 #else
   if (a->engine == NNB_ENGINE_TC && !tc_supports(a->S))
     return fail(-4, "tensor-core engine needs S in {32,64,128,256} (got %d); use NNB_ENGINE_SIMT", a->S);
 #endif
-  size_t need = nnb_workspace_bytes(a->N, a->S, a->flags, a->engine);
+  size_t need = nnb_workspace_bytes_dim(a->N, a->S, a->flags, a->engine, a->hidden_dim);
   if (!a->workspace || a->workspace_bytes < need)
     return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
@@ -108,7 +126,7 @@ int nnb_render_fwd(const nnb_render_args* a, void* stream) {
   if (a->flags & (NNB_FWD_DROP_WLO | NNB_FWD_DROP_ALO))
     return fail(-7, "NNB_FWD_DROP_* (forward precision experiment) is not built into this library");
 #endif
-  WsLayout L = make_layout(a->N, a->S, a->flags, a->engine);
+  WsLayout L = make_layout(a->N, a->S, a->flags, a->engine, hidden_of(a->hidden_dim));
   cudaError_t e;
 #ifdef NNB_WITH_TC
   if (a->engine == NNB_ENGINE_TC) e = tc_render_fwd(*a, L, (cudaStream_t)stream); else
@@ -123,7 +141,7 @@ int nnb_render_bwd(const nnb_render_bwd_args* b, void* stream) {
   if (!(b->fwd.flags & NNB_STASH)) return fail(-6, "nnb_render_bwd needs the forward call to have run with NNB_STASH");
   if (!b->g_rgb || !b->g_c2w) return fail(-3, "g_rgb and g_c2w must be non-null");
   if (b->phase > 2) return fail(-2, "nnb_render_bwd: phase must be 0, 1 or 2");
-  WsLayout L = make_layout(b->fwd.N, b->fwd.S, b->fwd.flags, b->fwd.engine);
+  WsLayout L = make_layout(b->fwd.N, b->fwd.S, b->fwd.flags, b->fwd.engine, hidden_of(b->fwd.hidden_dim));
   cudaError_t e;
 #ifdef NNB_WITH_TC
   if (b->fwd.engine == NNB_ENGINE_TC) e = tc_render_bwd(*b, L, (cudaStream_t)stream); else
@@ -134,7 +152,8 @@ int nnb_render_bwd(const nnb_render_bwd_args* b, void* stream) {
 
 static int check_field(const nnb_render_args* a) {
   if (!a || !a->pts || !a->weights || a->N <= 0) return fail(-3, "nnb_field_*: need pts, weights, N > 0");
-  size_t need = make_layout(a->N, 1, a->flags, NNB_ENGINE_SIMT).total;
+  if (int rc = check_dim(a)) return rc;
+  size_t need = make_layout(a->N, 1, a->flags, NNB_ENGINE_SIMT, hidden_of(a->hidden_dim)).total;
   if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
   return 0;
 }
@@ -142,14 +161,15 @@ int nnb_field_fwd(const nnb_render_args* a, float* out_rgba, void* stream) {
   int rc = check_field(a); if (rc) return rc;
   if (!out_rgba) return fail(-3, "nnb_field_fwd: out_rgba is null");
   nnb_render_args b = *a; b.S = 1; b.engine = NNB_ENGINE_SIMT;
-  cudaError_t e = simt_field_fwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT), out_rgba, (cudaStream_t)stream);
+  cudaError_t e = simt_field_fwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT, hidden_of(b.hidden_dim)), out_rgba, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_fwd");
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {
   int rc = check_field(a); if (rc) return rc;
   if (!g_rgba || !(a->flags & NNB_STASH)) return fail(-3, "nnb_field_bwd: need g_rgba and a forward run with NNB_STASH");
   nnb_render_args b = *a; b.S = 1; b.engine = NNB_ENGINE_SIMT;
-  cudaError_t e = simt_field_bwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT), g_rgba, g_pts, g_dirs, g_weights, (cudaStream_t)stream);
+  cudaError_t e = simt_field_bwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT, hidden_of(b.hidden_dim)), g_rgba, g_pts, g_dirs, g_weights,
+                                 (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_bwd");
 }
 

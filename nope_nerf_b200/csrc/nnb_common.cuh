@@ -10,23 +10,35 @@
 
 #define NNB_EPS 1e-6f  // model/rendering.py:9
 
-// ---- flat parameter layout (floats), OfficialStaticNerf.parameters() order -------------
+// ---- flat parameter layout (floats), OfficialStaticNerf.parameters() order, for hidden width D -------------
 namespace nnb {
-constexpr int D = 256;
 constexpr int PE = 63;   // (2*10+1)*3
 constexpr int DE = 27;   // (2*4+1)*3
-constexpr int W_SIG = 493056, B_SIG = 493312;               // fc_density
-constexpr int W_FEAT = 493313, B_FEAT = 558849;             // fc_feature
-constexpr int W_RGBH = 559105, B_RGBH = 595329;             // rgb_layers.0 (128 x 283)
-constexpr int W_RGB = 595457, B_RGB = 595841;               // fc_rgb (3 x 128)
-static_assert(B_RGB + 3 == NNB_NUM_PARAMS, "layout");
-// trunk layer l = 0..7 (layers0.{0,2,4,6}, layers1.{0,2,4,6}): weight (256 x w_ld) then bias (256)
-__host__ __device__ constexpr int w_ld(int l) { return l == 0 ? PE : (l == 4 ? D + PE : D); }
-__host__ __device__ constexpr int w_off(int l) {
-  return l == 0 ? 0 : (l < 4 ? 16384 + (l - 1) * 65792 : (l == 4 ? 213760 : 295680 + (l - 5) * 65792));
+// widths with a kernel instantiation (model.hidden_dim); nnb_render_args.hidden_dim == 0 means 256
+__host__ __device__ constexpr bool dim_supported(int D) { return D == 64 || D == 128 || D == 256; }
+// trunk layer l = 0..7 (layers0.{0,2,4,6}, layers1.{0,2,4,6}): weight (D x w_ld) then bias (D)
+__host__ __device__ constexpr int w_ld(int D, int l) { return l == 0 ? PE : (l == 4 ? D + PE : D); }
+__host__ __device__ constexpr int w_off(int D, int l) {
+  return l == 0 ? 0
+       : (l < 4 ? D * PE + D + (l - 1) * (D * D + D)
+       : (l == 4 ? D * PE + D + 3 * (D * D + D)
+       : D * PE + D + 3 * (D * D + D) + D * (D + PE) + D + (l - 5) * (D * D + D)));
 }
-__host__ __device__ constexpr int b_off(int l) { return w_off(l) + 256 * w_ld(l); }
-static_assert(w_off(3) == 147968 && b_off(3) == 213504 && w_off(7) == 427264 && b_off(7) == 492800 && b_off(4) == 295424, "layout");
+__host__ __device__ constexpr int b_off(int D, int l) { return w_off(D, l) + D * w_ld(D, l); }
+__host__ __device__ constexpr int W_SIG(int D) { return b_off(D, 7) + D; }               // fc_density (1 x D)
+__host__ __device__ constexpr int B_SIG(int D) { return W_SIG(D) + D; }
+__host__ __device__ constexpr int W_FEAT(int D) { return B_SIG(D) + 1; }                 // fc_feature (D x D)
+__host__ __device__ constexpr int B_FEAT(int D) { return W_FEAT(D) + D * D; }
+__host__ __device__ constexpr int W_RGBH(int D) { return B_FEAT(D) + D; }                // rgb_layers.0 (D/2 x (D + 27))
+__host__ __device__ constexpr int B_RGBH(int D) { return W_RGBH(D) + (D / 2) * (D + DE); }
+__host__ __device__ constexpr int W_RGB(int D) { return B_RGBH(D) + D / 2; }             // fc_rgb (3 x D/2)
+__host__ __device__ constexpr int B_RGB(int D) { return W_RGB(D) + 3 * (D / 2); }
+__host__ __device__ constexpr int num_params(int D) { return B_RGB(D) + 3; }
+static_assert(W_SIG(256) == 493056 && B_SIG(256) == 493312 && W_FEAT(256) == 493313 && B_FEAT(256) == 558849 && W_RGBH(256) == 559105 &&
+              B_RGBH(256) == 595329 && W_RGB(256) == 595457 && B_RGB(256) == 595841, "layout");
+static_assert(w_off(256, 3) == 147968 && b_off(256, 3) == 213504 && w_off(256, 7) == 427264 && b_off(256, 7) == 492800 &&
+              b_off(256, 4) == 295424, "layout");
+static_assert(num_params(256) == NNB_NUM_PARAMS && num_params(128) == 158660 && num_params(64) == 44516, "layout");
 }  // namespace nnb
 
 struct Ray {

@@ -1,7 +1,8 @@
 // Exact-fp32 SIMT engine (NNB_ENGINE_SIMT): the reference arithmetic (nn.Linear = fp32 FMA)
 // with the whole field evaluated tile-by-tile out of shared memory.  It is the bit-faithful
 // engine used for small batches and as the on-device cross-check of the tensor-core engine.
-//   F1 simt_mlp_fwd     : ray-gen + sampling + encoding + 8x256 MLP + heads  (64 samples / CTA)
+// Every MLP kernel is instantiated once per supported hidden width D (64 | 128 | 256) and dispatched on nnb_render_args.hidden_dim.
+//   F1 simt_mlp_fwd     : ray-gen + sampling + encoding + 8xD MLP + heads  (64 samples / CTA)
 //   F2 composite_fwd    : alpha compositing, one warp per ray (shared with the TC engine)
 //   B1 composite_bwd    : compositing adjoint -> per-sample (g_rgb, g_a)
 //   B2 simt_mlp_dgrad   : data-gradient chain through the MLP, emits dY per layer
@@ -14,7 +15,7 @@ void nnb_prof_mark(cudaStream_t st);
 namespace {
 
 constexpr int TM = 64;         // samples per CTA tile
-constexpr int LDB = 324;       // activation buffer row stride (256 hidden + 64 enc + 4 pad)
+template <int D> constexpr int ldb() { return D + 68; }   // activation buffer row stride (D hidden + 64 enc + 4 pad)
 constexpr int WS_LD = 260;     // staged weight row stride
 constexpr int KC = 16;         // reduction chunk
 
@@ -144,17 +145,19 @@ __device__ __forceinline__ void row_geometry(const nnb_render_args& a, size_t m,
   sample_point(a, ray, z, p);
 }
 
+template <int D>
 __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPtrs P, size_t M, int stash) {
+  constexpr int LDB = ldb<D>(), NJ = D / 64, NJR = D >= 128 ? D / 128 : 1;   // output column blocks of the trunk / rgb hidden layers
   extern __shared__ __align__(16) float smem[];
   float* buf0 = smem; float* buf1 = buf0 + TM * LDB; float* Ws = buf1 + TM * LDB;
   const int tid = threadIdx.x;
   const size_t m0 = (size_t)blockIdx.x * TM;
   const float* w = a.weights;
-  {  // prologue: encode positions into columns 256..319 of both buffers
+  {  // prologue: encode positions into columns D..D+63 of both buffers
     int row = tid & 63, part = tid >> 6;
     Ray ray; int n, i; float z, p[3];
     row_geometry(a, m0 + row, M, ray, n, i, z, p);
-    float* e0 = buf0 + row * LDB + 256; float* e1 = buf1 + row * LDB + 256;
+    float* e0 = buf0 + row * LDB + D; float* e1 = buf1 + row * LDB + D;
     if (part == 0) {
 #pragma unroll
       for (int c = 0; c < 3; ++c) { e0[c] = p[c]; e1[c] = p[c]; }
@@ -173,17 +176,17 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
   if (stash) {
     for (int idx = tid; idx < TM * 16; idx += 256) {
       int row = idx >> 4, c4 = idx & 15;
-      *reinterpret_cast<float4*>(P.enc + (m0 + row) * 64 + c4 * 4) = *reinterpret_cast<const float4*>(buf0 + row * LDB + 256 + c4 * 4);
+      *reinterpret_cast<float4*>(P.enc + (m0 + row) * 64 + c4 * 4) = *reinterpret_cast<const float4*>(buf0 + row * LDB + D + c4 * 4);
     }
   }
   float* cur = buf0; float* oth = buf1;
   for (int l = 0; l < 8; ++l) {
-    const float* in = (l == 0) ? cur + 256 : cur;
-    int K = (l == 0) ? 64 : (l == 4 ? 320 : 256);
-    int kvalid = (l == 0) ? 63 : (l == 4 ? 319 : 256);
-    tile_gemm<4, false, 1, false>(in, LDB, K, w + nnb::w_off(l), nnb::w_ld(l), 256, kvalid, w + nnb::b_off(l), oth, LDB, Ws);
+    const float* in = (l == 0) ? cur + D : cur;
+    int K = (l == 0) ? 64 : (l == 4 ? D + 64 : D);
+    int kvalid = (l == 0) ? 63 : (l == 4 ? D + 63 : D);
+    tile_gemm<NJ, false, 1, false>(in, LDB, K, w + nnb::w_off(D, l), nnb::w_ld(D, l), D, kvalid, w + nnb::b_off(D, l), oth, LDB, Ws);
     __syncthreads();
-    if (stash) tile_to_global(oth, LDB, P.h[l], m0, 256);
+    if (stash) tile_to_global(oth, LDB, P.h[l], m0, D);
     float* t_ = cur; cur = oth; oth = t_;
   }
   // cur = h8.  density head: 4 threads per row
@@ -191,44 +194,45 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
   float s_logit;
   {
     float acc = 0.f;
-    const float* hr_ = cur + hrow * LDB + hc * 64;
-    const float* ws_ = w + nnb::W_SIG + hc * 64;
+    const float* hr_ = cur + hrow * LDB + hc * (D / 4);
+    const float* ws_ = w + nnb::W_SIG(D) + hc * (D / 4);
 #pragma unroll 8
-    for (int k = 0; k < 64; ++k) acc = fmaf(hr_[k], __ldg(ws_ + k), acc);
+    for (int k = 0; k < D / 4; ++k) acc = fmaf(hr_[k], __ldg(ws_ + k), acc);
     acc += __shfl_xor_sync(0xffffffffu, acc, 1);
     acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-    s_logit = acc + __ldg(w + nnb::B_SIG);
+    s_logit = acc + __ldg(w + nnb::B_SIG(D));
   }
-  // feature layer (no activation) -> oth, then dir encoding into cols 256..287
-  tile_gemm<4, false, 0, false>(cur, LDB, 256, w + nnb::W_FEAT, 256, 256, 256, w + nnb::B_FEAT, oth, LDB, Ws);
+  // feature layer (no activation) -> oth, then dir encoding into cols D..D+31
+  tile_gemm<NJ, false, 0, false>(cur, LDB, D, w + nnb::W_FEAT(D), D, D, D, w + nnb::B_FEAT(D), oth, LDB, Ws);
   if (tid < TM) {
     Ray ray; int n, i; float z, p[3], v[3];
     row_geometry(a, m0 + tid, M, ray, n, i, z, p);
     row_view_dir(a, m0 + tid, M, ray, v);
-    float* de = oth + tid * LDB + 256;
+    float* de = oth + tid * LDB + D;
     encode<4>(v, [&](int k, float val) { de[k] = val; });
 #pragma unroll
     for (int k = 27; k < 32; ++k) de[k] = 0.f;
   }
   __syncthreads();
   if (stash) {
-    tile_to_global(oth, LDB, P.feat, m0, 256);
+    tile_to_global(oth, LDB, P.feat, m0, D);
     for (int idx = tid; idx < TM * 8; idx += 256) {
       int row = idx >> 3, c4 = idx & 7;
-      *reinterpret_cast<float4*>(P.denc + (m0 + row) * 32 + c4 * 4) = *reinterpret_cast<const float4*>(oth + row * LDB + 256 + c4 * 4);
+      *reinterpret_cast<float4*>(P.denc + (m0 + row) * 32 + c4 * 4) = *reinterpret_cast<const float4*>(oth + row * LDB + D + c4 * 4);
     }
   }
-  tile_gemm<2, false, 1, false>(oth, LDB, 288, w + nnb::W_RGBH, 283, 128, 283, w + nnb::B_RGBH, cur, LDB, Ws);
+  // rgb hidden layer: D / 2 columns (at D = 64 one 64-column block with the upper 32 columns zero)
+  tile_gemm<NJR, false, 1, false>(oth, LDB, D + 32, w + nnb::W_RGBH(D), D + 27, D / 2, D + 27, w + nnb::B_RGBH(D), cur, LDB, Ws);
   __syncthreads();
-  if (stash) tile_to_global(cur, LDB, P.hr, m0, 128);
+  if (stash) tile_to_global(cur, LDB, P.hr, m0, D / 2);
   {  // colour head + record
     float val = 0.f;
     if (hc < 3) {
-      const float* hr_ = cur + hrow * LDB; const float* wc = w + nnb::W_RGB + hc * 128;
+      const float* hr_ = cur + hrow * LDB; const float* wc = w + nnb::W_RGB(D) + hc * (D / 2);
       float acc = 0.f;
 #pragma unroll 8
-      for (int k = 0; k < 128; ++k) acc = fmaf(hr_[k], __ldg(wc + k), acc);
-      val = sigmoid_f(acc + __ldg(w + nnb::B_RGB + hc));
+      for (int k = 0; k < D / 2; ++k) acc = fmaf(hr_[k], __ldg(wc + k), acc);
+      val = sigmoid_f(acc + __ldg(w + nnb::B_RGB(D) + hc));
     }
     float* rec = reinterpret_cast<float*>(P.rec + m0 + hrow);
     if (hc < 3) rec[hc] = val;
@@ -350,7 +354,9 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
 // ---------------------------------------------------------------------------------------
 // B2: data-gradient chain
 // ---------------------------------------------------------------------------------------
+template <int D>
 __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, SimtPtrs P, size_t M, int write_dy) {
+  constexpr int LDB = ldb<D>(), NJ = D / 64, DR = D / 2;
   extern __shared__ __align__(16) float smem[];
   float* bufA = smem; float* bufB = bufA + TM * LDB; float* Ws = bufB + TM * LDB;
   float* genc = Ws + 2 * KC * WS_LD;          // [64][64]
@@ -370,54 +376,54 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, Simt
   }
   __syncthreads();
   // 2. g_yr = (g_yc @ Wc) * (hr > 0)
-  for (int idx = tid; idx < TM * 128; idx += 256) {
-    int row = idx >> 7, j = idx & 127; size_t m = m0 + row;
-    float v = gyc[row * 4] * __ldg(w + nnb::W_RGB + j) + gyc[row * 4 + 1] * __ldg(w + nnb::W_RGB + 128 + j) +
-              gyc[row * 4 + 2] * __ldg(w + nnb::W_RGB + 256 + j);
-    v = (P.hr[m * 128 + j] > 0.f) ? v : 0.f;
+  for (int idx = tid; idx < TM * DR; idx += 256) {
+    int row = idx / DR, j = idx % DR; size_t m = m0 + row;
+    float v = gyc[row * 4] * __ldg(w + nnb::W_RGB(D) + j) + gyc[row * 4 + 1] * __ldg(w + nnb::W_RGB(D) + DR + j) +
+              gyc[row * 4 + 2] * __ldg(w + nnb::W_RGB(D) + 2 * DR + j);
+    v = (P.hr[m * DR + j] > 0.f) ? v : 0.f;
     bufA[row * LDB + j] = v;
-    if (write_dy) P.dyr[m * 128 + j] = v;
+    if (write_dy) P.dyr[m * DR + j] = v;
   }
   __syncthreads();
-  // 3. g_xr = g_yr @ Wr : feature part -> bufB[:, :256], dir-encoding part -> bufB[:, 256:320]
-  tile_gemm<4, true, 0, false>(bufA, LDB, 128, w + nnb::W_RGBH, 283, 256, 128, nullptr, bufB, LDB, Ws);
-  tile_gemm<1, true, 0, false>(bufA, LDB, 128, w + nnb::W_RGBH + 256, 283, 27, 128, nullptr, bufB + 256, LDB, Ws);
+  // 3. g_xr = g_yr @ Wr : feature part -> bufB[:, :D], dir-encoding part -> bufB[:, D:D+64]
+  tile_gemm<NJ, true, 0, false>(bufA, LDB, DR, w + nnb::W_RGBH(D), D + 27, D, DR, nullptr, bufB, LDB, Ws);
+  tile_gemm<1, true, 0, false>(bufA, LDB, DR, w + nnb::W_RGBH(D) + D, D + 27, 27, DR, nullptr, bufB + D, LDB, Ws);
   __syncthreads();
-  if (write_dy) tile_to_global(bufB, LDB, P.dfeat, m0, 256);
+  if (write_dy) tile_to_global(bufB, LDB, P.dfeat, m0, D);
   if (tid < TM) {
     Ray ray; int n, i; float z, p[3], v[3], gvd[3];
     row_geometry(a, m0 + tid, M, ray, n, i, z, p);
     row_view_dir(a, m0 + tid, M, ray, v);
-    const float* ge = bufB + tid * LDB + 256;
+    const float* ge = bufB + tid * LDB + D;
     encode_bwd<4>(v, [&](int k) { return ge[k]; }, gvd);
     P.gv[m0 + tid] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
   }
   // 4. g_h8 = g_feat @ Wf + g_s * w_sigma
-  tile_gemm<4, true, 0, false>(bufB, LDB, 256, w + nnb::W_FEAT, 256, 256, 256, nullptr, bufA, LDB, Ws);
+  tile_gemm<NJ, true, 0, false>(bufB, LDB, D, w + nnb::W_FEAT(D), D, D, D, nullptr, bufA, LDB, Ws);
   __syncthreads();
-  for (int idx = tid; idx < TM * 256; idx += 256) {
-    int row = idx >> 8, k = idx & 255;
-    bufA[row * LDB + k] += gyc[row * 4 + 3] * __ldg(w + nnb::W_SIG + k);
+  for (int idx = tid; idx < TM * D; idx += 256) {
+    int row = idx / D, k = idx % D;
+    bufA[row * LDB + k] += gyc[row * 4 + 3] * __ldg(w + nnb::W_SIG(D) + k);
   }
   __syncthreads();
   // 5. trunk
   float* X = bufA; float* Y = bufB;
   for (int l = 7; l >= 0; --l) {
-    for (int idx = tid; idx < TM * 64; idx += 256) {
-      int row = idx >> 6, c4 = idx & 63; size_t m = m0 + row;
-      float4 hv = *reinterpret_cast<const float4*>(P.h[l] + m * 256 + c4 * 4);
+    for (int idx = tid; idx < TM * (D / 4); idx += 256) {
+      int row = idx / (D / 4), c4 = idx % (D / 4); size_t m = m0 + row;
+      float4 hv = *reinterpret_cast<const float4*>(P.h[l] + m * D + c4 * 4);
       float4* xp = reinterpret_cast<float4*>(X + row * LDB + c4 * 4);
       float4 g = *xp;
       g.x = hv.x > 0.f ? g.x : 0.f; g.y = hv.y > 0.f ? g.y : 0.f; g.z = hv.z > 0.f ? g.z : 0.f; g.w = hv.w > 0.f ? g.w : 0.f;
       *xp = g;
-      if (write_dy) *reinterpret_cast<float4*>(P.dy[l] + m * 256 + c4 * 4) = g;
+      if (write_dy) *reinterpret_cast<float4*>(P.dy[l] + m * D + c4 * 4) = g;
     }
     __syncthreads();
     if (l == 0) {
-      tile_gemm<1, true, 0, true>(X, LDB, 256, w + nnb::w_off(0), 63, 63, 256, nullptr, genc, 64, Ws);
+      tile_gemm<1, true, 0, true>(X, LDB, D, w + nnb::w_off(D, 0), 63, 63, D, nullptr, genc, 64, Ws);
     } else {
-      tile_gemm<4, true, 0, false>(X, LDB, 256, w + nnb::w_off(l), nnb::w_ld(l), 256, 256, nullptr, Y, LDB, Ws);
-      if (l == 4) tile_gemm<1, true, 0, false>(X, LDB, 256, w + nnb::w_off(4) + 256, 319, 63, 256, nullptr, genc, 64, Ws);
+      tile_gemm<NJ, true, 0, false>(X, LDB, D, w + nnb::w_off(D, l), nnb::w_ld(D, l), D, D, nullptr, Y, LDB, Ws);
+      if (l == 4) tile_gemm<1, true, 0, false>(X, LDB, D, w + nnb::w_off(D, 4) + D, D + 63, 63, D, nullptr, genc, 64, Ws);
       float* t_ = X; X = Y; Y = t_;
     }
     __syncthreads();
@@ -644,31 +650,50 @@ SimtPtrs make_ptrs(const WsLayout& L, void* ws) {
   return P;
 }
 
-constexpr size_t FWD_SMEM = (2 * TM * LDB + 2 * KC * WS_LD) * sizeof(float);
-constexpr size_t BWD_SMEM = FWD_SMEM + (TM * 64 + TM * 4) * sizeof(float);
+template <int D> constexpr size_t fwd_smem() { return (2 * TM * ldb<D>() + 2 * KC * WS_LD) * sizeof(float); }
+template <int D> constexpr size_t bwd_smem() { return fwd_smem<D>() + (TM * 64 + TM * 4) * sizeof(float); }
 
 }  // namespace
 
 // entry points used by nnb_api.cu ------------------------------------------------------
-static cudaError_t simt_init() {
+template <int D>
+static cudaError_t simt_init_dim() {
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(simt_mlp_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FWD_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(simt_mlp_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(simt_mlp_dgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM);
+    e = cudaFuncSetAttribute(simt_mlp_dgrad<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
     if (e != cudaSuccess) return e;
     attr = true;
   }
   return cudaSuccess;
+}
+static cudaError_t simt_init() {
+  cudaError_t e = simt_init_dim<256>();
+  if (e == cudaSuccess) e = simt_init_dim<128>();
+  if (e == cudaSuccess) e = simt_init_dim<64>();
+  return e;
+}
+// the MLP kernels of width L.D (the width was validated by nnb_api.cu)
+static void launch_mlp_fwd(const nnb_render_args& a, const SimtPtrs& P, const WsLayout& L, int stash, cudaStream_t st) {
+  const int tiles = (int)((L.M + TM - 1) / TM);
+  if (L.D == 128) simt_mlp_fwd<128><<<tiles, 256, fwd_smem<128>(), st>>>(a, P, L.M, stash);
+  else if (L.D == 64) simt_mlp_fwd<64><<<tiles, 256, fwd_smem<64>(), st>>>(a, P, L.M, stash);
+  else simt_mlp_fwd<256><<<tiles, 256, fwd_smem<256>(), st>>>(a, P, L.M, stash);
+}
+static void launch_mlp_dgrad(const nnb_render_args& a, const SimtPtrs& P, const WsLayout& L, int write_dy, cudaStream_t st) {
+  const int tiles = (int)((L.M + TM - 1) / TM);
+  if (L.D == 128) simt_mlp_dgrad<128><<<tiles, 256, bwd_smem<128>(), st>>>(a, P, L.M, write_dy);
+  else if (L.D == 64) simt_mlp_dgrad<64><<<tiles, 256, bwd_smem<64>(), st>>>(a, P, L.M, write_dy);
+  else simt_mlp_dgrad<256><<<tiles, 256, bwd_smem<256>(), st>>>(a, P, L.M, write_dy);
 }
 
 cudaError_t simt_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
   SimtPtrs P = make_ptrs(L, a.workspace);
   cudaError_t e0 = simt_init();
   if (e0 != cudaSuccess) return e0;
-  int tiles = (int)((L.M + TM - 1) / TM);
   nnb_prof_mark(st); nnb_prof_mark(st);
-  simt_mlp_fwd<<<tiles, 256, FWD_SMEM, st>>>(a, P, L.M, (a.flags & NNB_STASH) ? 1 : 0);
+  launch_mlp_fwd(a, P, L, (a.flags & NNB_STASH) ? 1 : 0, st);
   nnb_prof_mark(st);
   composite_fwd<<<(a.N + 7) / 8, 256, 0, st>>>(a, P.rec);
   nnb_prof_mark(st);
@@ -684,8 +709,7 @@ cudaError_t simt_field_fwd(const nnb_render_args& a, const WsLayout& L, float* o
   SimtPtrs P = make_ptrs(L, a.workspace);
   cudaError_t e0 = simt_init();
   if (e0 != cudaSuccess) return e0;
-  int tiles = (int)((L.M + TM - 1) / TM);
-  simt_mlp_fwd<<<tiles, 256, FWD_SMEM, st>>>(a, P, L.M, (a.flags & NNB_STASH) ? 1 : 0);
+  launch_mlp_fwd(a, P, L, (a.flags & NNB_STASH) ? 1 : 0, st);
   rec_to_rgba<<<(unsigned)((L.M + 255) / 256), 256, 0, st>>>(P.rec, reinterpret_cast<float4*>(out_rgba), L.M);
   return cudaGetLastError();
 }
@@ -699,8 +723,7 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
   if (e != cudaSuccess) return e;
   e = cudaMemcpyAsync(P.gs, g_rgba, L.M * 16, cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return e;
-  int tiles = (int)((L.M + TM - 1) / TM);
-  simt_mlp_dgrad<<<tiles, 256, BWD_SMEM, st>>>(a, P, L.M, g_weights ? 1 : 0);
+  launch_mlp_dgrad(a, P, L, g_weights ? 1 : 0, st);
   if (g_weights) { e = simt_wgrad_all(P, L, g_weights, st); if (e != cudaSuccess) return e; }
   if (g_pts) { e = cudaMemcpyAsync(g_pts, P.gp, L.M * 16, cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) return e; }
   if (g_dirs) { e = cudaMemcpyAsync(g_dirs, P.gv, L.M * 16, cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) return e; }
@@ -708,7 +731,7 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
 }
 
 // jobs -> simt_wgrad into the partial buffer, then wgrad_reduce into dW / db
-cudaError_t run_simt_wgrad(WJobs& J, size_t M, int msplit, float* part, cudaStream_t st) {
+cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st) {
   RedJob R[16];
   size_t off = 0; int tiles = 0;
   for (int i = 0; i < J.njobs; ++i) {
@@ -719,14 +742,14 @@ cudaError_t run_simt_wgrad(WJobs& J, size_t M, int msplit, float* part, cudaStre
     j.part_off = off;
     off += stride * msplit;
   }
-  if (off > wpart_floats(M)) return cudaErrorInvalidValue;
+  if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
   simt_wgrad<<<dim3(tiles, msplit), 256, 0, st>>>(J, M, msplit, part);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, J.njobs, part, st);
 }
 
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, float* part, cudaStream_t st) {
+cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, cudaStream_t st) {
   WJobs J{};
   for (int i = 0; i < njobs && i < 16; ++i) {
     WJob& j = J.j[i];
@@ -734,7 +757,7 @@ cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, fl
     j.dW = jobs[i].dW; j.ldw = jobs[i].ldw; j.db = jobs[i].db;
   }
   J.njobs = njobs < 16 ? njobs : 16;
-  return run_simt_wgrad(J, M, jobs_wgrad_msplit(M), part, st);
+  return run_simt_wgrad(J, M, D, jobs_wgrad_msplit(M), part, st);
 }
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st) {
@@ -749,18 +772,19 @@ cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cuda
       WJob& j = J.j[nj++];
       j.dY = dY; j.ldy = ldy; j.Nn = Nn; j.X = X; j.ldx = ldx; j.Kk = Kk; j.dW = dW; j.ldw = ldw; j.db = db;
     };
-    add(P.dy[0], 256, 256, P.enc, 64, 63, gw + nnb::w_off(0), 63, gw + nnb::b_off(0));
+    const int D = L.D, DR = D / 2;
+    add(P.dy[0], D, D, P.enc, 64, 63, gw + nnb::w_off(D, 0), 63, gw + nnb::b_off(D, 0));
     for (int l = 1; l < 8; ++l) {
-      add(P.dy[l], 256, 256, P.h[l - 1], 256, 256, gw + nnb::w_off(l), nnb::w_ld(l), gw + nnb::b_off(l));
-      if (l == 4) add(P.dy[4], 256, 256, P.enc, 64, 63, gw + nnb::w_off(4) + 256, 319, nullptr);
+      add(P.dy[l], D, D, P.h[l - 1], D, D, gw + nnb::w_off(D, l), nnb::w_ld(D, l), gw + nnb::b_off(D, l));
+      if (l == 4) add(P.dy[4], D, D, P.enc, 64, 63, gw + nnb::w_off(D, 4) + D, D + 63, nullptr);
     }
-    add(reinterpret_cast<const float*>(P.dyc) + 3, 4, 1, P.h[7], 256, 256, gw + nnb::W_SIG, 256, gw + nnb::B_SIG);
-    add(P.dfeat, 256, 256, P.h[7], 256, 256, gw + nnb::W_FEAT, 256, gw + nnb::B_FEAT);
-    add(P.dyr, 128, 128, P.feat, 256, 256, gw + nnb::W_RGBH, 283, gw + nnb::B_RGBH);
-    add(P.dyr, 128, 128, P.denc, 32, 27, gw + nnb::W_RGBH + 256, 283, nullptr);
-    add(reinterpret_cast<const float*>(P.dyc), 4, 3, P.hr, 128, 128, gw + nnb::W_RGB, 128, gw + nnb::B_RGB);
+    add(reinterpret_cast<const float*>(P.dyc) + 3, 4, 1, P.h[7], D, D, gw + nnb::W_SIG(D), D, gw + nnb::B_SIG(D));
+    add(P.dfeat, D, D, P.h[7], D, D, gw + nnb::W_FEAT(D), D, gw + nnb::B_FEAT(D));
+    add(P.dyr, DR, DR, P.feat, D, D, gw + nnb::W_RGBH(D), D + 27, gw + nnb::B_RGBH(D));
+    add(P.dyr, DR, DR, P.denc, 32, 27, gw + nnb::W_RGBH(D) + D, D + 27, nullptr);
+    add(reinterpret_cast<const float*>(P.dyc), 4, 3, P.hr, DR, DR, gw + nnb::W_RGB(D), DR, gw + nnb::B_RGB(D));
     J.njobs = nj;
-    return run_simt_wgrad(J, L.M, simt_wgrad_msplit(L.M), P.wpart, st);
+    return run_simt_wgrad(J, L.M, D, simt_wgrad_msplit(L.M), P.wpart, st);
   }
 }
 
@@ -782,13 +806,12 @@ cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L
   SimtPtrs P = make_ptrs(L, a.workspace);
   cudaError_t e0 = simt_init();
   if (e0 != cudaSuccess) return e0;
-  int tiles = (int)((L.M + TM - 1) / TM);
   nnb_prof_mark(st);
   composite_bwd<<<(a.N + 7) / 8, 256, 0, st>>>(b, P.rec, P.gs, nullptr);
   nnb_prof_mark(st);
   const int write_dy = b.g_weights ? 1 : 0;
   if (dgrad) { cudaError_t ed = dgrad(b, L, write_dy, st); if (ed != cudaSuccess) return ed; }
-  else simt_mlp_dgrad<<<tiles, 256, BWD_SMEM, st>>>(a, P, L.M, write_dy);
+  else launch_mlp_dgrad(a, P, L, write_dy, st);
   nnb_prof_mark(st);
   if (b.g_weights) {
     cudaError_t ew = wgrad ? wgrad(a, L, b.g_weights, st) : simt_wgrad_all(P, L, b.g_weights, st);

@@ -1,9 +1,11 @@
 // Tensor-core engine (NNB_ENGINE_TC), Hopper (sm_90a): the whole field of a 128-sample tile evaluated by one persistent CTA
 // per SM.
 //
+// Every kernel is a template on the hidden width D (64 | 128 | 256), one instantiation per width, dispatched on WsLayout::D.
+//
 //   warps 0..7: two consumer warpgroups, each owning 64 sample rows of the tile.  Prologue: ray generation, sampling, the
 //               63-column positional encoding -> E operand, direction encoding -> per-ray bias of rgb_layers.0.  Per layer the
-//               warpgroup issues wgmma.m64n256k16 (m64n128k16 for the rgb hidden layer) with both operands in shared memory;
+//               warpgroup issues wgmma.m64n{D}k16 (m64n{D/2}k16 for the rgb hidden layer) with both operands in shared memory;
 //               every logical product runs as three MMAs a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (split-fp16, 22-bit operands, fp32
 //               accumulation in registers) so results match the fp32 reference.  The epilogue (bias, ReLU, re-split into
 //               hi | lo halves) writes the next layer's A operand IN PLACE: a warpgroup's MMAs read only its own 64 rows, and
@@ -23,7 +25,7 @@
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st);
 cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, float* part, cudaStream_t st);
+cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, cudaStream_t st);
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -31,30 +33,55 @@ namespace {
 
 constexpr int TILE = 128;
 constexpr int NST = 3;                      // weight ring depth
-constexpr int STAGE_BYTES = 16384;          // 256 output rows x 16 k x (hi + lo) fp16 = one K-step of a 256-wide layer
 constexpr int N_GEMM = 10;                  // L0..L7, feature, rgb-hidden
-// ---- stage table: the order in which weight stages are consumed for one tile --------------------------------------------
 struct StageDesc { int w_off, ldw, kcol0, kvalid, nrows, img_off; };
-constexpr int N_STAGES = 4 + 3 * 16 + (4 + 16) + 3 * 16 + 16 + 16;   // 152
-__constant__ StageDesc c_stages[N_STAGES];
-constexpr size_t IMG_BYTES = (size_t)(N_STAGES - 16) * STAGE_BYTES + 16 * (STAGE_BYTES / 2);   // rgb hidden layer: 128 rows
-
-// shared memory map (bytes)
-constexpr int SM_AHI = 0, SM_ALO = 65536, SM_EHI = 131072, SM_ELO = 147456, SM_W = 163840;
-constexpr int SM_BIAS = SM_W + NST * STAGE_BYTES;             // 212992
-constexpr int BIAS_FLOATS = 8 * 256 + 256 + 256 + 384 + 4;    // trunk, feat, w_sigma, W_rgb, (b_sigma, b_rgb[3])
-constexpr int SM_RAYB = SM_BIAS + ((BIAS_FLOATS * 4 + 127) / 128) * 128;
-constexpr int RAYB_FLOATS = 2 * 128 + 2 * 32;                 // per warpgroup: per-ray bias [2 rays][128] + direction encodings [2][32]
-constexpr int SM_BAR = SM_RAYB + 2 * RAYB_FLOATS * 4;
-constexpr int SM_TOTAL = SM_BAR + 2 * NST * 8;
-static_assert(SM_TOTAL <= 232448, "shared memory budget");
+struct StageDescT { int w_off, ldw, coloff, nvalid, k0, kvalid, nrows, img_off; };
 constexpr int N_THREADS = 384;              // two consumer warpgroups + the producer warpgroup (one thread of it issues the copies)
+
+// sizes and shared-memory maps (bytes) of the field kernels at hidden width D
+template <int D> struct Tc {
+  static constexpr int LOG_D = D == 256 ? 8 : (D == 128 ? 7 : 6);
+  static constexpr int KS = D / 16;                       // K-steps of a D-wide input
+  static constexpr int STAGE_BYTES = D * 64;              // D output rows x 16 k x (hi + lo) 16-bit = one K-step of a D-wide layer
+  // ---- forward stage table: the order in which weight stages are consumed for one tile (152 stages at D = 256) ----
+  static constexpr int N_STAGES = 4 + 3 * KS + (4 + KS) + 3 * KS + KS + KS;
+  static constexpr size_t IMG_BYTES = (size_t)(N_STAGES - KS) * STAGE_BYTES + KS * (STAGE_BYTES / 2);   // rgb hidden layer: D/2 rows
+  static constexpr int SM_AHI = 0, SM_ALO = D * 256, SM_EHI = 2 * D * 256, SM_ELO = SM_EHI + 16384, SM_W = SM_ELO + 16384;
+  static constexpr int SM_BIAS = SM_W + NST * STAGE_BYTES;
+  static constexpr int BIAS_FLOATS = 8 * D + D + D + 3 * (D / 2) + 4;   // trunk, feat, w_sigma, W_rgb, (b_sigma, b_rgb[3])
+  static constexpr int SM_RAYB = SM_BIAS + ((BIAS_FLOATS * 4 + 127) / 128) * 128;
+  static constexpr int RAYB_FLOATS = 2 * (D / 2) + 2 * 32;   // per warpgroup: per-ray bias [2 rays][D/2] + direction encodings [2][32]
+  static constexpr int SM_BAR = SM_RAYB + 2 * RAYB_FLOATS * 4;
+  static constexpr int SM_TOTAL = SM_BAR + 2 * NST * 8;
+  // ---- data-gradient chain (176 transposed stages at D = 256) ----
+  static constexpr int N_STAGES_T = D / 32 + D / 32 + KS + 7 * KS + KS + KS;
+  static constexpr size_t IMG_T_BYTES = (size_t)34 * D * D + (size_t)576 * D;
+  static constexpr int DG_AHI = 0, DG_ALO = D * 256, DG_W = 2 * D * 256, DG_GENC = DG_W + NST * STAGE_BYTES;
+  static constexpr int DG_SMALL = DG_GENC + 2 * 64 * 64 * 4;     // W_rgb [3][D/2] | w_sigma [D]
+  static constexpr int DG_GYC = DG_SMALL + (5 * D / 2) * 4;      // per row: d/d(rgb logits), d/d density logit
+  static constexpr int DG_BAR = DG_GYC + 128 * 4 * 4;
+  static constexpr int DG_TOTAL = DG_BAR + 2 * NST * 8;
+  static_assert(SM_TOTAL <= 232448 && DG_TOTAL <= 232448, "shared memory budget");
+};
+static_assert(Tc<256>::N_STAGES == 152 && Tc<256>::SM_BIAS == 212992 && Tc<256>::BIAS_FLOATS == 2948 && Tc<256>::N_STAGES_T == 176 &&
+              Tc<256>::IMG_T_BYTES == (size_t)136 * 16384 + 8 * 2048 + 32 * 4096 && Tc<256>::DG_GENC == 180224, "D = 256 layout");
+
+// stage tables, one per width
+__constant__ StageDesc c_stages_256[Tc<256>::N_STAGES], c_stages_128[Tc<128>::N_STAGES], c_stages_64[Tc<64>::N_STAGES];
+__constant__ StageDescT c_stages_t_256[Tc<256>::N_STAGES_T], c_stages_t_128[Tc<128>::N_STAGES_T], c_stages_t_64[Tc<64>::N_STAGES_T];
+template <int D> __device__ __forceinline__ const StageDesc& stage(int s) {
+  if constexpr (D == 256) return c_stages_256[s]; else if constexpr (D == 128) return c_stages_128[s]; else return c_stages_64[s];
+}
+template <int D> __device__ __forceinline__ const StageDescT& stage_t(int s) {
+  if constexpr (D == 256) return c_stages_t_256[s]; else if constexpr (D == 128) return c_stages_t_128[s]; else return c_stages_t_64[s];
+}
 
 using namespace tcu;
 
 // ---- weight imaging: fp32 (out,in) matrices -> per-stage shared-memory images (hi | lo) --------
+template <int D>
 __global__ void tc_prep_weights(const float* __restrict__ w, unsigned char* __restrict__ img) {
-  const StageDesc sd = c_stages[blockIdx.x];
+  const StageDesc sd = stage<D>(blockIdx.x);
   unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] fp16
   unsigned char* lo = hi + sd.nrows * 32;
   for (int idx = threadIdx.x; idx < sd.nrows * 2; idx += blockDim.x) {
@@ -84,8 +111,14 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                               SampleRec* __restrict__ recs, TcStash st, size_t M, int n_tiles, int stash) {
+  using T = Tc<D>;
+  constexpr int SM_AHI = T::SM_AHI, SM_ALO = T::SM_ALO, SM_EHI = T::SM_EHI, SM_ELO = T::SM_ELO, SM_W = T::SM_W, SM_BIAS = T::SM_BIAS;
+  constexpr int SM_RAYB = T::SM_RAYB, SM_BAR = T::SM_BAR, BIAS_FLOATS = T::BIAS_FLOATS, RAYB_FLOATS = T::RAYB_FLOATS;
+  constexpr int STAGE_BYTES = T::STAGE_BYTES, N_STAGES = T::N_STAGES, DR = D / 2;
+  constexpr int B_FEAT0 = 8 * D, W_SIG0 = 9 * D, W_RGB0 = 10 * D, B_SIG0 = 10 * D + 3 * DR;   // s_bias sections
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* s_bias = reinterpret_cast<float*>(smem + SM_BIAS);
@@ -101,12 +134,12 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
     const float* w = a.weights;
     for (int i = threadIdx.x; i < BIAS_FLOATS; i += blockDim.x) {
       float v;
-      if (i < 2048) v = __ldg(w + nnb::b_off(i >> 8) + (i & 255));
-      else if (i < 2304) v = __ldg(w + nnb::B_FEAT + (i - 2048));
-      else if (i < 2560) v = __ldg(w + nnb::W_SIG + (i - 2304));
-      else if (i < 2944) v = __ldg(w + nnb::W_RGB + (i - 2560));
-      else if (i == 2944) v = __ldg(w + nnb::B_SIG);
-      else v = __ldg(w + nnb::B_RGB + (i - 2945));
+      if (i < B_FEAT0) v = __ldg(w + nnb::b_off(D, i >> T::LOG_D) + (i & (D - 1)));
+      else if (i < W_SIG0) v = __ldg(w + nnb::B_FEAT(D) + (i - B_FEAT0));
+      else if (i < W_RGB0) v = __ldg(w + nnb::W_SIG(D) + (i - W_SIG0));
+      else if (i < B_SIG0) v = __ldg(w + nnb::W_RGB(D) + (i - W_RGB0));
+      else if (i == B_SIG0) v = __ldg(w + nnb::B_SIG(D));
+      else v = __ldg(w + nnb::B_RGB(D) + (i - (B_SIG0 + 1)));
       s_bias[i] = v;
     }
   }
@@ -121,10 +154,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
       uint32_t slot = 0, phase = 0;
       for (int t = 0; t < my_tiles; ++t)
         for (int s = 0; s < N_STAGES; ++s) {
-          const uint32_t bytes = (uint32_t)c_stages[s].nrows * 64u;
+          const uint32_t bytes = (uint32_t)stage<D>(s).nrows * 64u;
           mbar_wait(EMPTY(slot), phase ^ 1u);                 // both warpgroups released this slot
           mbar_expect_tx(FULL(slot), bytes);
-          bulk_g2s(smem_u32(smem + SM_W + slot * STAGE_BYTES), wimg + c_stages[s].img_off, bytes, FULL(slot));
+          bulk_g2s(smem_u32(smem + SM_W + slot * STAGE_BYTES), wimg + stage<D>(s).img_off, bytes, FULL(slot));
           if (++slot == NST) { slot = 0; phase ^= 1u; }
         }
     }
@@ -143,7 +176,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
   const int rays_per_wg = (a.S >= 64) ? 1 : 64 / a.S;
   uint32_t slot = 0, phase = 0;
-  float acc[128];
+  float acc[D / 2];
 
   for (int t = 0; t < my_tiles; ++t) {
     const int tile = blockIdx.x + t * gridDim.x;
@@ -188,24 +221,25 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
         if (rl % (rays_per_wg == 1 ? 64 : a.S) == 0) {   // the row that starts a ray publishes its direction encoding
           const int r = rays_per_wg == 1 ? 0 : rl / a.S;
 #pragma unroll
-          for (int k = 0; k < 32; ++k) rayb[256 + r * 32 + k] = de[k];
+          for (int k = 0; k < 32; ++k) rayb[D + r * 32 + k] = de[k];
         }
       }
       fence_async_smem();
       wg_sync();
       const float* w = a.weights;
       for (int r = 0; r < rays_per_wg; ++r) {   // thread tl = output column of the rgb hidden layer
-        float b = __ldg(w + nnb::B_RGBH + tl);
+        if (DR < 128 && tl >= DR) break;
+        float b = __ldg(w + nnb::B_RGBH(D) + tl);
 #pragma unroll
-        for (int k = 0; k < 27; ++k) b = fmaf(__ldg(w + nnb::W_RGBH + (size_t)tl * 283 + 256 + k), rayb[256 + r * 32 + k], b);
-        rayb[r * 128 + tl] = b;   // read after layer 0's epilogue barrier
+        for (int k = 0; k < 27; ++k) b = fmaf(__ldg(w + nnb::W_RGBH(D) + (size_t)tl * (D + 27) + D + k), rayb[D + r * 32 + k], b);
+        rayb[r * DR + tl] = b;   // read after layer 0's epilogue barrier
       }
     }
     float s_logit[2] = {0.f, 0.f};
     for (int g = 0; g < N_GEMM; ++g) {
       // ---- MMAs: K-steps from the encoding operand E (layers 0 and 4) first, then from the previous layer's output ----
-      const int n_e = (g == 0 || g == 4) ? 4 : 0, ns = n_e + (g == 0 ? 0 : 16);
-      const uint32_t nrows = (g == 9) ? 128u : 256u;
+      const int n_e = (g == 0 || g == 4) ? 4 : 0, ns = n_e + (g == 0 ? 0 : T::KS);
+      const uint32_t nrows = (g == 9) ? (uint32_t)DR : (uint32_t)D;
       for (int s = 0; s < ns; ++s) {
         const bool from_e = s < n_e;
         const uint32_t ko = (uint32_t)(from_e ? s : s - n_e) * 4096u;   // two k-octets of 2048 B per K-step
@@ -215,13 +249,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
         mbar_wait(FULL(slot), phase);
         wgmma_fence();
         if (g < 9) {
-          wgmma_f16<256>(acc, dal, dbh, s > 0 ? 1u : 0u);
-          wgmma_f16<256>(acc, dah, dbl, 1u);
-          wgmma_f16<256>(acc, dah, dbh, 1u);
+          wgmma_f16<D>(acc, dal, dbh, s > 0 ? 1u : 0u);
+          wgmma_f16<D>(acc, dah, dbl, 1u);
+          wgmma_f16<D>(acc, dah, dbh, 1u);
         } else {
-          wgmma_f16<128>(acc, dal, dbh, s > 0 ? 1u : 0u);
-          wgmma_f16<128>(acc, dah, dbl, 1u);
-          wgmma_f16<128>(acc, dah, dbh, 1u);
+          wgmma_f16<DR>(acc, dal, dbh, s > 0 ? 1u : 0u);
+          wgmma_f16<DR>(acc, dah, dbl, 1u);
+          wgmma_f16<DR>(acc, dah, dbh, 1u);
         }
         wgmma_commit();
         if (s > 0) {   // the previous K-step's MMAs have completed: release its weight stage
@@ -234,10 +268,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
       if (tl == 0) mbar_arrive(EMPTY(slot == 0 ? NST - 1 : slot - 1));
       // ---- epilogue ----
       if (g < 9) {
-        const float* bias = (g < 8) ? s_bias + g * 256 : s_bias + 2048;
+        const float* bias = (g < 8) ? s_bias + g * D : s_bias + B_FEAT0;
         float* sp = stash ? (g < 8 ? st.h[g] : st.feat) : nullptr;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
+        for (int j = 0; j < D / 8; ++j) {
           const int col = j * 8 + c0;
           const float2 b = *reinterpret_cast<const float2*>(bias + col);
 #pragma unroll
@@ -250,27 +284,27 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
             const int off = j * 2048 + row * 16 + c0 * 2;
             *reinterpret_cast<uint32_t*>(smem + SM_AHI + off) = hw;
             *reinterpret_cast<uint32_t*>(smem + SM_ALO + off) = lw;
-            if (g == 7) s_logit[r] = fmaf(v1, s_bias[2304 + col + 1], fmaf(v0, s_bias[2304 + col], s_logit[r]));
-            if (sp) __stcs(reinterpret_cast<float2*>(sp + (mt + row) * 256 + col), make_float2(v0, v1));
+            if (g == 7) s_logit[r] = fmaf(v1, s_bias[W_SIG0 + col + 1], fmaf(v0, s_bias[W_SIG0 + col], s_logit[r]));
+            if (sp) __stcs(reinterpret_cast<float2*>(sp + (mt + row) * D + col), make_float2(v0, v1));
           }
         }
         fence_async_smem();
         wg_sync();   // the whole A operand (and, after layer 0, the per-ray bias) is written before the next layer's MMAs
       } else {
-        // rgb hidden layer (128 columns) -> colour head + per-sample record
+        // rgb hidden layer (D/2 columns) -> colour head + per-sample record
         float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+        for (int j = 0; j < DR / 8; ++j) {
           const int col = j * 8 + c0;
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
             const int row = r0 + 8 * r;
-            const float* rb = rayb + (rays_per_wg == 1 ? 0 : (row - wg * 64) / a.S) * 128;
+            const float* rb = rayb + (rays_per_wg == 1 ? 0 : (row - wg * 64) / a.S) * DR;
             const float v0 = fmaxf(acc[4 * j + 2 * r] + rb[col], 0.f), v1 = fmaxf(acc[4 * j + 2 * r + 1] + rb[col + 1], 0.f);
 #pragma unroll
             for (int c = 0; c < 3; ++c)
-              c_acc[r][c] = fmaf(v1, s_bias[2560 + c * 128 + col + 1], fmaf(v0, s_bias[2560 + c * 128 + col], c_acc[r][c]));
-            if (stash) __stcs(reinterpret_cast<float2*>(st.hr + (mt + row) * 128 + col), make_float2(v0, v1));
+              c_acc[r][c] = fmaf(v1, s_bias[W_RGB0 + c * DR + col + 1], fmaf(v0, s_bias[W_RGB0 + c * DR + col], c_acc[r][c]));
+            if (stash) __stcs(reinterpret_cast<float2*>(st.hr + (mt + row) * DR + col), make_float2(v0, v1));
           }
         }
 #pragma unroll
@@ -279,10 +313,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
           const float cr = quad_sum(c_acc[r][0]), cg = quad_sum(c_acc[r][1]), cb = quad_sum(c_acc[r][2]);
           if ((lane & 3) == 0) {
             const size_t m = mt + r0 + 8 * r, mm = m < M ? m : M - 1;
-            const float s = sl + s_bias[2944];
+            const float s = sl + s_bias[B_SIG0];
             float sigma;
             SampleRec rec;
-            rec.r = sigmoid_f(cr + s_bias[2945]); rec.g = sigmoid_f(cg + s_bias[2946]); rec.b = sigmoid_f(cb + s_bias[2947]);
+            rec.r = sigmoid_f(cr + s_bias[B_SIG0 + 1]); rec.g = sigmoid_f(cg + s_bias[B_SIG0 + 2]); rec.b = sigmoid_f(cb + s_bias[B_SIG0 + 3]);
             rec.a = density_act(s, a.flags, &sigma); rec.s = s; rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
             rec.pad0 = 0.f; rec.pad1 = 0.f;
             recs[m] = rec;
@@ -304,7 +338,7 @@ constexpr int MAX_WG_JOBS = 10, WG_CHUNK = 64;
 struct WgJobsT { WgJobT j[MAX_WG_JOBS]; int njobs, msplit, per_cta; };
 template <int KN> constexpr int wg_smem() { return 2 * (2 * 128 * 128 + 2 * KN * 128); }
 
-template <int KN>   // 256 | 64: columns of dW (features of X) held by one CTA
+template <int KN>   // 256 | 128 | 64: columns of dW (features of X) held by one CTA
 __global__ void __launch_bounds__(256, 1) tc_wgrad(WgJobsT J, size_t M, float* __restrict__ part) {
   extern __shared__ __align__(1024) unsigned char smem[];
   constexpr int A_BYTES = 128 * 128, B_BYTES = KN * 128, BUF = 2 * A_BYTES + 2 * B_BYTES;
@@ -383,7 +417,7 @@ __global__ void __launch_bounds__(256, 1) tc_wgrad(WgJobsT J, size_t M, float* _
 }
 
 template <int KN>
-cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int msplit, float* part, cudaStream_t st) {
+cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msplit, float* part, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem<KN>());
@@ -401,7 +435,7 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int msplit, fl
     R[i] = RedJob{jobs[i].dW, jobs[i].db, jobs[i].Nn, jobs[i].Kk, jobs[i].ldw, msplit, 2, off, stride};
     off += stride * msplit;
   }
-  if (off > wpart_floats(M)) return cudaErrorInvalidValue;
+  if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
   J.njobs = njobs; J.msplit = msplit;
   J.per_cta = (int)(((M + msplit - 1) / msplit + WG_CHUNK - 1) / WG_CHUNK * WG_CHUNK);
   tc_wgrad<KN><<<ctas, 256, wg_smem<KN>(), st>>>(J, M, part);
@@ -414,26 +448,28 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int msplit, fl
 cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) {
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  const int D = L.D, DR = D / 2;
   WgJobT big[9], enc[2];
   int nb = 0;
-  for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(l), gw + nnb::b_off(l), 256, 256, 256, 256, nnb::w_ld(l), 0, 0};
-  big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT, gw + nnb::B_FEAT, 256, 256, 256, 256, 256, 0, 0};
-  big[nb++] = WgJobT{F(L.dyr), F(L.feat), gw + nnb::W_RGBH, gw + nnb::B_RGBH, 128, 128, 256, 256, 283, 0, 0};
-  enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(0), gw + nnb::b_off(0), 256, 256, 64, 63, 63, 0, 0};
-  enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(4) + 256, nullptr, 256, 256, 64, 63, 319, 0, 0};
+  for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(D, l), gw + nnb::b_off(D, l), D, D, D, D, nnb::w_ld(D, l), 0, 0};
+  big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT(D), gw + nnb::B_FEAT(D), D, D, D, D, D, 0, 0};
+  big[nb++] = WgJobT{F(L.dyr), F(L.feat), gw + nnb::W_RGBH(D), gw + nnb::B_RGBH(D), DR, DR, D, D, D + 27, 0, 0};
+  enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(D, 0), gw + nnb::b_off(D, 0), D, D, 64, 63, 63, 0, 0};
+  enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(D, 4) + D, nullptr, D, D, 64, 63, D + 63, 0, 0};
   float* part = F(L.wpart);   // reused by each launch: its reduction runs before the next launch on the same stream
-  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (17 | 4 row slices)
-  const int ms_big = L.M >= 8 * 128 ? 8 : 1, ms_enc = L.M >= 32 * 64 ? 32 : 1;
-  cudaError_t e = launch_wgrad<256>(big, nb, L.M, ms_big, part, st);
+  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (17 | 4 row slices at D = 256)
+  const int ms_big = L.M >= 8 * 128 ? tc_wgrad_msplit_big(D) : 1, ms_enc = L.M >= 32 * 64 ? 32 : 1;
+  cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, st)
+                : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, st) : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, st);
   if (e != cudaSuccess) return e;
-  e = launch_wgrad<64>(enc, 2, L.M, ms_enc, part, st);
+  e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, st);
   if (e != cudaSuccess) return e;
   const float* dyc = F(L.dyc);
   SmallJob sm[3] = {
-      {dyc + 3, F(L.h[7]), gw + nnb::W_SIG, gw + nnb::B_SIG, 4, 1, 256, 256, 256},
-      {F(L.dyr), F(L.denc), gw + nnb::W_RGBH + 256, nullptr, 128, 128, 32, 27, 283},
-      {dyc, F(L.hr), gw + nnb::W_RGB, gw + nnb::B_RGB, 4, 3, 128, 128, 128}};
-  return launch_simt_wgrad_jobs(sm, 3, L.M, part, st);
+      {dyc + 3, F(L.h[7]), gw + nnb::W_SIG(D), gw + nnb::B_SIG(D), 4, 1, D, D, D},
+      {F(L.dyr), F(L.denc), gw + nnb::W_RGBH(D) + D, nullptr, DR, DR, 32, 27, D + 27},
+      {dyc, F(L.hr), gw + nnb::W_RGB(D), gw + nnb::B_RGB(D), 4, 3, DR, DR, DR}};
+  return launch_simt_wgrad_jobs(sm, 3, L.M, D, part, st);
 }
 
 // ---- data-gradient chain (the forward's skeleton run backwards) ---------------------------------------------------------------------
@@ -443,19 +479,9 @@ cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw,
 // epilogue); the epilogue applies the ReLU gate of the layer below (its fp32 stash > 0) and writes that layer's dY stash for the
 // weight-gradient pass.  Order (matches the stage table): g_de = g_yr W_rgbh[:, 256:283] (N = 32), g_feat = g_yr W_rgbh[:, :256],
 // g_h7 = g_feat W_feat + g_s w_sigma, then layers 7..1 (layer 4 first adds its encoding slice, N = 64) and layer 0 (encoding, N = 64).
-struct StageDescT { int w_off, ldw, coloff, nvalid, k0, kvalid, nrows, img_off; };
-constexpr int N_STAGES_T = 8 + 8 + 16 + 7 * 16 + 16 + 16;   // 176
-__constant__ StageDescT c_stages_t[N_STAGES_T];
-constexpr size_t IMG_T_BYTES = (size_t)136 * STAGE_BYTES + 8 * 2048 + 32 * 4096;
-constexpr int DG_AHI = 0, DG_ALO = 65536, DG_W = 131072, DG_GENC = DG_W + NST * STAGE_BYTES;   // 180224
-constexpr int DG_SMALL = DG_GENC + 2 * 64 * 64 * 4;     // W_rgb [3][128] | w_sigma [256]
-constexpr int DG_GYC = DG_SMALL + 640 * 4;              // per row: d/d(rgb logits), d/d density logit
-constexpr int DG_BAR = DG_GYC + 128 * 4 * 4;
-constexpr int DG_TOTAL = DG_BAR + 2 * NST * 8;
-static_assert(DG_TOTAL <= 232448, "shared memory budget");
-
+template <int D>
 __global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __restrict__ img) {
-  const StageDescT sd = c_stages_t[blockIdx.x];
+  const StageDescT sd = stage_t<D>(blockIdx.x);
   unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] bf16
   unsigned char* lo = hi + sd.nrows * 32;
   for (int idx = threadIdx.x; idx < sd.nrows * 2; idx += blockDim.x) {
@@ -476,9 +502,10 @@ struct DgPtrs {
 };
 
 // K-steps of one GEMM: D[64 x N] = A[64 x 16 ksteps] B^T, weight stages from the ring (released as their MMAs complete)
-template <int N>
+template <int D, int N>
 __device__ __forceinline__ void dg_gemm(float* acc, uint32_t a_hi, uint32_t a_lo, int ksteps, uint32_t w_base, uint32_t bar0,
                                         uint32_t& slot, uint32_t& phase, int tl) {
+  constexpr int STAGE_BYTES = Tc<D>::STAGE_BYTES;
   for (int s = 0; s < ksteps; ++s) {
     const uint32_t ko = (uint32_t)s * 4096u;
     const uint64_t dah = gdesc(a_hi + ko, 2048, 128), dal = gdesc(a_lo + ko, 2048, 128);
@@ -507,8 +534,12 @@ __device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint
   lo = *reinterpret_cast<uint32_t*>(&ll);
 }
 
+template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, const unsigned char* __restrict__ wimg, DgPtrs P, size_t M,
                                                          int n_tiles, int write_dy) {
+  using T = Tc<D>;
+  constexpr int DG_AHI = T::DG_AHI, DG_ALO = T::DG_ALO, DG_W = T::DG_W, DG_GENC = T::DG_GENC, DG_SMALL = T::DG_SMALL, DG_GYC = T::DG_GYC;
+  constexpr int DG_BAR = T::DG_BAR, STAGE_BYTES = T::STAGE_BYTES, N_STAGES_T = T::N_STAGES_T, DR = D / 2, KS = T::KS;
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* s_small = reinterpret_cast<float*>(smem + DG_SMALL);
@@ -517,7 +548,8 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
     for (int i = 0; i < NST; ++i) { mbar_init(bar0 + 8u * i, 1); mbar_init(bar0 + 8u * (NST + i), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = threadIdx.x; i < 640; i += blockDim.x) s_small[i] = (i < 384) ? __ldg(a.weights + nnb::W_RGB + i) : __ldg(a.weights + nnb::W_SIG + (i - 384));
+  for (int i = threadIdx.x; i < 5 * DR; i += blockDim.x)
+    s_small[i] = (i < 3 * DR) ? __ldg(a.weights + nnb::W_RGB(D) + i) : __ldg(a.weights + nnb::W_SIG(D) + (i - 3 * DR));
   __syncthreads();
   const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
   if (warp >= 8) {   // weight producer (see tc_field_fwd)
@@ -526,10 +558,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
       uint32_t slot = 0, phase = 0;
       for (int t = 0; t < my_tiles; ++t)
         for (int s = 0; s < N_STAGES_T; ++s) {
-          const uint32_t bytes = (uint32_t)c_stages_t[s].nrows * 64u;
+          const uint32_t bytes = (uint32_t)stage_t<D>(s).nrows * 64u;
           mbar_wait(bar0 + 8u * (NST + slot), phase ^ 1u);
           mbar_expect_tx(bar0 + 8u * slot, bytes);
-          bulk_g2s(smem_u32(smem + DG_W + slot * STAGE_BYTES), wimg + c_stages_t[s].img_off, bytes, bar0 + 8u * slot);
+          bulk_g2s(smem_u32(smem + DG_W + slot * STAGE_BYTES), wimg + stage_t<D>(s).img_off, bytes, bar0 + 8u * slot);
           if (++slot == NST) { slot = 0; phase ^= 1u; }
         }
     }
@@ -545,19 +577,19 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
   const uint32_t bar_id = 1u + (uint32_t)wg;
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
   uint32_t slot = 0, phase = 0;
-  float acc[128];   // the 32- / 64-wide GEMMs use its first registers (every result is consumed before the next GEMM)
-  // epilogue of a 256-wide layer: x (+ g_s w_sigma) -> ReLU gate of `hmask` -> dY stash -> next A operand (in place)
-  auto epi256 = [&](size_t mt, const float* hmask, float* dst, bool add_sigma) {
+  float acc[D / 2];   // the 32- / 64-wide GEMMs use its first registers (every result is consumed before the next GEMM)
+  // epilogue of a D-wide layer: x (+ g_s w_sigma) -> ReLU gate of `hmask` -> dY stash -> next A operand (in place)
+  auto epiD = [&](size_t mt, const float* hmask, float* dst, bool add_sigma) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int row = r0 + 8 * r;
-      const size_t rowoff = (mt + row) * 256 + c0;
+      const size_t rowoff = (mt + row) * D + c0;
       const float g_s = add_sigma ? gyc[(row - wg * 64) * 4 + 3] : 0.f;
       unsigned char* ahi = smem + DG_AHI + row * 16 + c0 * 2;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
+      for (int j = 0; j < D / 8; ++j) {
         float v0 = acc[4 * j + 2 * r], v1 = acc[4 * j + 2 * r + 1];
-        if (add_sigma) { v0 += g_s * s_small[384 + j * 8 + c0]; v1 += g_s * s_small[384 + j * 8 + c0 + 1]; }
+        if (add_sigma) { v0 += g_s * s_small[3 * DR + j * 8 + c0]; v1 += g_s * s_small[3 * DR + j * 8 + c0 + 1]; }
         if (hmask) {
           const float2 h = __ldg(reinterpret_cast<const float2*>(hmask + rowoff + j * 8));
           v0 = h.x > 0.f ? v0 : 0.f; v1 = h.y > 0.f ? v1 : 0.f;
@@ -597,25 +629,25 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
       gyc[tl * 4] = g0; gyc[tl * 4 + 1] = g1; gyc[tl * 4 + 2] = g2; gyc[tl * 4 + 3] = g3;
     }
     wg_sync();
-    {   // g_yr = (g_yc W_rgb) * (hr > 0): thread = row x 64 columns -> A operand (K = 128) + dY stash
+    {   // g_yr = (g_yc W_rgb) * (hr > 0): thread = row x D/4 columns -> A operand (K = D/2) + dY stash
       const int rl = tl & 63, half = tl >> 6, row = wg * 64 + rl;
       const size_t m = mt + row;
       const float* g4 = gyc + rl * 4;
 #pragma unroll
-      for (int oc = 0; oc < 8; ++oc) {
-        const int j0 = half * 64 + oc * 8;
-        const float4 ha = __ldg(reinterpret_cast<const float4*>(P.hr + m * 128 + j0));
-        const float4 hb = __ldg(reinterpret_cast<const float4*>(P.hr + m * 128 + j0 + 4));
+      for (int oc = 0; oc < D / 32; ++oc) {
+        const int j0 = half * (D / 4) + oc * 8;
+        const float4 ha = __ldg(reinterpret_cast<const float4*>(P.hr + m * DR + j0));
+        const float4 hb = __ldg(reinterpret_cast<const float4*>(P.hr + m * DR + j0 + 4));
         const float hv[8] = {ha.x, ha.y, ha.z, ha.w, hb.x, hb.y, hb.z, hb.w};
         float v[8];
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
-          const float x = g4[0] * s_small[j0 + q] + g4[1] * s_small[128 + j0 + q] + g4[2] * s_small[256 + j0 + q];
+          const float x = g4[0] * s_small[j0 + q] + g4[1] * s_small[DR + j0 + q] + g4[2] * s_small[2 * DR + j0 + q];
           v[q] = hv[q] > 0.f ? x : 0.f;
         }
         if (write_dy) {
-          *reinterpret_cast<float4*>(P.dyr + m * 128 + j0) = make_float4(v[0], v[1], v[2], v[3]);
-          *reinterpret_cast<float4*>(P.dyr + m * 128 + j0 + 4) = make_float4(v[4], v[5], v[6], v[7]);
+          *reinterpret_cast<float4*>(P.dyr + m * DR + j0) = make_float4(v[0], v[1], v[2], v[3]);
+          *reinterpret_cast<float4*>(P.dyr + m * DR + j0 + 4) = make_float4(v[4], v[5], v[6], v[7]);
         }
         split_store8_bf16(v, smem + DG_AHI + (j0 >> 3) * 2048 + row * 16, smem + DG_ALO + (j0 >> 3) * 2048 + row * 16);
       }
@@ -623,7 +655,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
     fence_async_smem();
     wg_sync();
     // g_de (direction-encoding slice of rgb_layers.0) -> view-direction adjoint
-    dg_gemm<32>(acc, a_hi, a_lo, 8, w_base, bar0, slot, phase, tl);
+    dg_gemm<D, 32>(acc, a_hi, a_lo, D / 32, w_base, bar0, slot, phase, tl);
 #pragma unroll
     for (int j = 0; j < 4; ++j)
 #pragma unroll
@@ -646,16 +678,16 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
       encode_bwd<4>(v, [&](int k) { return ge[k]; }, gvd);
       P.gv[m] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
     }
-    dg_gemm<256>(acc, a_hi, a_lo, 8, w_base, bar0, slot, phase, tl);    // g_feat
-    epi256(mt, nullptr, write_dy ? P.dfeat : nullptr, false);
-    dg_gemm<256>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl);   // g_h7 = g_feat W_feat + g_s w_sigma
-    epi256(mt, P.h[7], write_dy ? P.dy[7] : nullptr, true);
+    dg_gemm<D, D>(acc, a_hi, a_lo, D / 32, w_base, bar0, slot, phase, tl);   // g_feat
+    epiD(mt, nullptr, write_dy ? P.dfeat : nullptr, false);
+    dg_gemm<D, D>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);       // g_h7 = g_feat W_feat + g_s w_sigma
+    epiD(mt, P.h[7], write_dy ? P.dy[7] : nullptr, true);
     for (int l = 7; l >= 1; --l) {
-      if (l == 4) { dg_gemm<64>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl); epi_enc(false); }
-      dg_gemm<256>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl);  // g_h(l-1) = dY_l W_l
-      epi256(mt, P.h[l - 1], write_dy ? P.dy[l - 1] : nullptr, false);
+      if (l == 4) { dg_gemm<D, 64>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl); epi_enc(false); }
+      dg_gemm<D, D>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);     // g_h(l-1) = dY_l W_l
+      epiD(mt, P.h[l - 1], write_dy ? P.dy[l - 1] : nullptr, false);
     }
-    dg_gemm<64>(acc, a_hi, a_lo, 16, w_base, bar0, slot, phase, tl);    // encoding gradient of layer 0
+    dg_gemm<D, 64>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);      // encoding gradient of layer 0
     epi_enc(true);
     wg_sync();
     if (tl < 64) {   // encoding adjoint -> d p
@@ -669,39 +701,46 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
   }
 }
 
-bool g_stage_table_t_ready = false;
-
+template <int D>
 cudaError_t upload_stage_table_t() {
-  if (g_stage_table_t_ready) return cudaSuccess;
-  StageDescT h[N_STAGES_T];
+  using T = Tc<D>;
+  static bool ready = false;
+  if (ready) return cudaSuccess;
+  StageDescT h[T::N_STAGES_T];
   int s = 0, off = 0;
   auto add = [&](int w_off, int ldw, int coloff, int nvalid, int k0, int kvalid, int nrows) {
     h[s] = StageDescT{w_off, ldw, coloff, nvalid, k0, kvalid, nrows, off};
     off += nrows * 64; ++s;
   };
-  for (int i = 0; i < 8; ++i) add(nnb::W_RGBH, 283, 256, 27, 16 * i, 128, 32);
-  for (int i = 0; i < 8; ++i) add(nnb::W_RGBH, 283, 0, 256, 16 * i, 128, 256);
-  for (int i = 0; i < 16; ++i) add(nnb::W_FEAT, 256, 0, 256, 16 * i, 256, 256);
+  constexpr int DR = D / 2, KS = T::KS;
+  for (int i = 0; i < DR / 16; ++i) add(nnb::W_RGBH(D), D + 27, D, 27, 16 * i, DR, 32);
+  for (int i = 0; i < DR / 16; ++i) add(nnb::W_RGBH(D), D + 27, 0, D, 16 * i, DR, D);
+  for (int i = 0; i < KS; ++i) add(nnb::W_FEAT(D), D, 0, D, 16 * i, D, D);
   for (int l = 7; l >= 1; --l) {
-    if (l == 4) for (int i = 0; i < 16; ++i) add(nnb::w_off(4), 319, 256, 63, 16 * i, 256, 64);
-    for (int i = 0; i < 16; ++i) add(nnb::w_off(l), nnb::w_ld(l), 0, 256, 16 * i, 256, 256);
+    if (l == 4) for (int i = 0; i < KS; ++i) add(nnb::w_off(D, 4), D + 63, D, 63, 16 * i, D, 64);
+    for (int i = 0; i < KS; ++i) add(nnb::w_off(D, l), nnb::w_ld(D, l), 0, D, 16 * i, D, D);
   }
-  for (int i = 0; i < 16; ++i) add(nnb::w_off(0), 63, 0, 63, 16 * i, 256, 64);
-  if (s != N_STAGES_T || (size_t)off != IMG_T_BYTES) return cudaErrorInvalidValue;
-  cudaError_t e = cudaMemcpyToSymbol(c_stages_t, h, sizeof(h));
-  if (e == cudaSuccess) g_stage_table_t_ready = true;
+  for (int i = 0; i < KS; ++i) add(nnb::w_off(D, 0), 63, 0, 63, 16 * i, D, 64);
+  if (s != T::N_STAGES_T || (size_t)off != T::IMG_T_BYTES) return cudaErrorInvalidValue;
+  cudaError_t e;
+  if constexpr (D == 256) e = cudaMemcpyToSymbol(c_stages_t_256, h, sizeof(h));
+  else if constexpr (D == 128) e = cudaMemcpyToSymbol(c_stages_t_128, h, sizeof(h));
+  else e = cudaMemcpyToSymbol(c_stages_t_64, h, sizeof(h));
+  if (e == cudaSuccess) ready = true;
   return e;
 }
 
 // the data-gradient stage of the TC engine's backward (stash layout of nnb_simt.cu)
-cudaError_t tc_dgrad_launch(const nnb_render_bwd_args& b, const WsLayout& L, int write_dy, cudaStream_t st) {
+template <int D>
+cudaError_t tc_dgrad_launch_dim(const nnb_render_bwd_args& b, const WsLayout& L, int write_dy, cudaStream_t st) {
+  using T = Tc<D>;
   const nnb_render_args& a = b.fwd;
-  cudaError_t e = upload_stage_table_t();
+  cudaError_t e = upload_stage_table_t<D>();
   if (e != cudaSuccess) return e;
   static bool attr = false;
   static int n_sm = 0;
   if (!attr) {
-    e = cudaFuncSetAttribute(tc_dgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_TOTAL);
+    e = cudaFuncSetAttribute(tc_dgrad<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
     if (e != cudaSuccess) return e;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -709,59 +748,63 @@ cudaError_t tc_dgrad_launch(const nnb_render_bwd_args& b, const WsLayout& L, int
   }
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
-  unsigned char* img = reinterpret_cast<unsigned char*>(base + L.total + align_up(IMG_BYTES, 256));
+  unsigned char* img = reinterpret_cast<unsigned char*>(base + L.total + align_up(T::IMG_BYTES, 256));
   DgPtrs P{};
   P.rec = reinterpret_cast<const SampleRec*>(base + L.rec);
   P.gs = reinterpret_cast<const float4*>(base + L.gs); P.gp = reinterpret_cast<float4*>(base + L.gp); P.gv = reinterpret_cast<float4*>(base + L.gv);
   P.dyc = reinterpret_cast<float4*>(base + L.dyc);
   for (int l = 0; l < 8; ++l) { P.h[l] = F(L.h[l]); P.dy[l] = F(L.dy[l]); }
   P.hr = F(L.hr); P.dfeat = F(L.dfeat); P.dyr = F(L.dyr);
-  tc_prep_weights_t<<<N_STAGES_T, 256, 0, st>>>(a.weights, img);
+  tc_prep_weights_t<D><<<T::N_STAGES_T, 256, 0, st>>>(a.weights, img);
   const int n_tiles = (int)((L.M + TILE - 1) / TILE);
   const int grid = n_tiles < n_sm ? n_tiles : n_sm;
-  tc_dgrad<<<grid, N_THREADS, DG_TOTAL, st>>>(a, (const unsigned char*)img, P, L.M, n_tiles, write_dy);
+  tc_dgrad<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, (const unsigned char*)img, P, L.M, n_tiles, write_dy);
   return cudaGetLastError();
 }
 
-bool g_stage_table_ready = false;
+cudaError_t tc_dgrad_launch(const nnb_render_bwd_args& b, const WsLayout& L, int write_dy, cudaStream_t st) {
+  return L.D == 128 ? tc_dgrad_launch_dim<128>(b, L, write_dy, st)
+       : L.D == 64  ? tc_dgrad_launch_dim<64>(b, L, write_dy, st) : tc_dgrad_launch_dim<256>(b, L, write_dy, st);
+}
 
+template <int D>
 cudaError_t upload_stage_table() {
-  if (g_stage_table_ready) return cudaSuccess;
-  StageDesc h[N_STAGES];
+  using T = Tc<D>;
+  static bool ready = false;
+  if (ready) return cudaSuccess;
+  StageDesc h[T::N_STAGES];
   int s = 0, off = 0;
   auto add = [&](int w_off, int ldw, int kcol0, int kvalid, int nrows) {
     h[s].w_off = w_off; h[s].ldw = ldw; h[s].kcol0 = kcol0; h[s].kvalid = kvalid; h[s].nrows = nrows; h[s].img_off = off;
     off += nrows * 64; ++s;
   };
   // per layer, one stage per K-step of 16; the encoding K-steps (layers 0 and 4) come first
-  for (int i = 0; i < 4; ++i) add(nnb::w_off(0), 63, 16 * i, 63, 256);
+  constexpr int KS = Tc<D>::KS;
+  for (int i = 0; i < 4; ++i) add(nnb::w_off(D, 0), 63, 16 * i, 63, D);
   for (int l = 1; l < 8; ++l) {
-    if (l == 4) for (int i = 0; i < 4; ++i) add(nnb::w_off(4), 319, 256 + 16 * i, 319, 256);
-    for (int i = 0; i < 16; ++i) add(nnb::w_off(l), nnb::w_ld(l), 16 * i, 256, 256);
+    if (l == 4) for (int i = 0; i < 4; ++i) add(nnb::w_off(D, 4), D + 63, D + 16 * i, D + 63, D);
+    for (int i = 0; i < KS; ++i) add(nnb::w_off(D, l), nnb::w_ld(D, l), 16 * i, D, D);
   }
-  for (int i = 0; i < 16; ++i) add(nnb::W_FEAT, 256, 16 * i, 256, 256);
-  for (int i = 0; i < 16; ++i) add(nnb::W_RGBH, 283, 16 * i, 256, 128);
-  if (s != N_STAGES || (size_t)off != IMG_BYTES) return cudaErrorInvalidValue;
-  cudaError_t e = cudaMemcpyToSymbol(c_stages, h, sizeof(h));
-  if (e == cudaSuccess) g_stage_table_ready = true;
+  for (int i = 0; i < KS; ++i) add(nnb::W_FEAT(D), D, 16 * i, D, D);
+  for (int i = 0; i < KS; ++i) add(nnb::W_RGBH(D), D + 27, 16 * i, D, D / 2);
+  if (s != T::N_STAGES || (size_t)off != T::IMG_BYTES) return cudaErrorInvalidValue;
+  cudaError_t e;
+  if constexpr (D == 256) e = cudaMemcpyToSymbol(c_stages_256, h, sizeof(h));
+  else if constexpr (D == 128) e = cudaMemcpyToSymbol(c_stages_128, h, sizeof(h));
+  else e = cudaMemcpyToSymbol(c_stages_64, h, sizeof(h));
+  if (e == cudaSuccess) ready = true;
   return e;
 }
 
-}  // namespace
-
-size_t tc_workspace_extra(int N, int S, uint32_t flags) { return align_up(IMG_BYTES, 256) + align_up(IMG_T_BYTES, 256); }
-
-bool tc_supports(int S) { return S == 32 || S == 64 || S == 128 || S == 256; }
-
-cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
-  if (!tc_supports(a.S)) return cudaErrorNotSupported;
-  if (a.flags & NNB_TCBWD) return cudaErrorNotSupported;   // the operand-plane stash is not implemented for sm_90a
-  cudaError_t e = upload_stage_table();
+template <int D>
+cudaError_t tc_render_fwd_dim(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
+  using T = Tc<D>;
+  cudaError_t e = upload_stage_table<D>();
   if (e != cudaSuccess) return e;
   static bool attr = false;
   static int n_sm = 0;
   if (!attr) {
-    e = cudaFuncSetAttribute(tc_field_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    e = cudaFuncSetAttribute(tc_field_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
     if (e != cudaSuccess) return e;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -778,17 +821,33 @@ cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStrea
     ts.enc = reinterpret_cast<float*>(base + L.enc); ts.denc = reinterpret_cast<float*>(base + L.denc);
   }
   nnb_prof_mark(st);
-  tc_prep_weights<<<N_STAGES, 256, 0, st>>>(a.weights, img);   // 152 stage images (fp16 hi | lo)
+  tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);   // 152 stage images (fp16 hi | lo) at D = 256
   nnb_prof_mark(st);
   const int n_tiles = (int)((L.M + TILE - 1) / TILE);
   const int grid = n_tiles < n_sm ? n_tiles : n_sm;
-  tc_field_fwd<<<grid, N_THREADS, SM_TOTAL, st>>>(a, (const unsigned char*)img, recs, ts, L.M, n_tiles, stash);
+  tc_field_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, (const unsigned char*)img, recs, ts, L.M, n_tiles, stash);
   nnb_prof_mark(st);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   e = launch_composite_fwd(a, recs, st);
   nnb_prof_mark(st);
   return e;
+}
+
+template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
+
+}  // namespace
+
+size_t tc_workspace_extra(int N, int S, uint32_t flags, int D) {
+  return D == 128 ? tc_extra_dim<128>() : (D == 64 ? tc_extra_dim<64>() : tc_extra_dim<256>());
+}
+
+bool tc_supports(int S) { return S == 32 || S == 64 || S == 128 || S == 256; }
+
+cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
+  if (!tc_supports(a.S)) return cudaErrorNotSupported;
+  if (a.flags & NNB_TCBWD) return cudaErrorNotSupported;   // the operand-plane stash is not implemented for sm_90a
+  return L.D == 128 ? tc_render_fwd_dim<128>(a, L, st) : (L.D == 64 ? tc_render_fwd_dim<64>(a, L, st) : tc_render_fwd_dim<256>(a, L, st));
 }
 
 // Backward of the TC engine: compositing / ray adjoints of nnb_simt.cu around tc_dgrad and tc_wgrad, which read and write the SIMT

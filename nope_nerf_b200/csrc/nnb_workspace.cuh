@@ -4,6 +4,7 @@
 
 struct WsLayout {
   size_t M, Mpad;
+  int D;        // hidden width of the field (64 | 128 | 256)
   // per-sample records
   size_t rec;   // SampleRec[Mpad]            (forward -> compositing / backward)
   size_t gs;    // float4[Mpad]  d/d(rgb_i, a_i) from compositing adjoint
@@ -12,7 +13,7 @@ struct WsLayout {
   // fixed-order reductions (no float atomics: a step's gradients are the same bits on every run)
   size_t rayred;   // float[N][16]  per-ray pose / intrinsics / scale-shift adjoints, summed over rays by ray_reduce
   size_t wpart;    // float[]       per-sample-split partial weight gradients, summed over the splits by wgrad_reduce
-  // SIMT engine activation stash (fp32, [sample][feature])
+  // SIMT engine activation stash (fp32, [sample][feature]; D features per trunk layer, D / 2 of the rgb hidden layer)
   size_t h[8], feat, hr, enc, denc;
   size_t dy[8], dfeat, dyr, dyc;
   // operand-plane backward (NNB_TCBWD; rejected by the sm_90a library): activations / output-gradients as per-tile bf16 hi|lo
@@ -40,11 +41,14 @@ __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a -
 // sample splits of the weight-gradient kernels (each split writes its own partial dW, see wgrad_reduce)
 inline int simt_wgrad_msplit(size_t M) { int m = (int)((M + 4095) / 4096); return m < 1 ? 1 : (m > 16 ? 16 : m); }
 inline int jobs_wgrad_msplit(size_t M) { int m = (int)((M + 2047) / 2048); return m < 1 ? 1 : (m > 64 ? 64 : m); }
+// sample splits of tc_wgrad's D-wide jobs: 8 at D = 256, more at smaller widths (fewer row slices per job) to fill the SMs
+inline int tc_wgrad_msplit_big(int D) { return 2048 / D; }
 constexpr size_t WPART_PAD = 16 * 512;   // bias slots of every job (up to two per output row)
-inline size_t wpart_floats(size_t M) {
-  const size_t a = (size_t)simt_wgrad_msplit(M) * (NNB_NUM_PARAMS + WPART_PAD);
-  const size_t b = (size_t)8 * (NNB_NUM_PARAMS + WPART_PAD);    // tc_wgrad: <= 8 splits of the 256-wide jobs, 32 of the encoding jobs
-  const size_t c = (size_t)jobs_wgrad_msplit(M) * 8192;         // small SIMT jobs
+inline size_t wpart_floats(size_t M, int D) {
+  const size_t np = (size_t)nnb::num_params(D);
+  const size_t a = (size_t)simt_wgrad_msplit(M) * (np + WPART_PAD);
+  const size_t b = (size_t)tc_wgrad_msplit_big(D) * (np + WPART_PAD);   // tc_wgrad: <= 2048 / D splits of the D-wide jobs, 32 of the encoding jobs
+  const size_t c = (size_t)jobs_wgrad_msplit(M) * 8192;                 // small SIMT jobs
   return a > b ? (a > c ? a : c) : (b > c ? b : c);
 }
 
@@ -53,8 +57,9 @@ inline size_t wpart_floats(size_t M) {
 struct RedJob { float* dW; float* db; int Nn, Kk, ldw, nsplit, dbslots; size_t off, stride; };
 cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st);
 
-inline WsLayout make_layout(int N, int S, uint32_t flags, int engine) {
+inline WsLayout make_layout(int N, int S, uint32_t flags, int engine, int D = 256) {
   WsLayout L{};
+  L.D = D;
   L.M = (size_t)N * S;
   L.Mpad = align_up(L.M, 128);
   size_t o = 0;
@@ -62,7 +67,7 @@ inline WsLayout make_layout(int N, int S, uint32_t flags, int engine) {
   L.rec = take(L.Mpad * sizeof(SampleRec));
   if (flags & NNB_STASH) {
     L.gs = take(L.Mpad * 16); L.gp = take(L.Mpad * 16); L.gv = take(L.Mpad * 16);
-    L.rayred = take((size_t)N * 16 * 4); L.wpart = take(wpart_floats(L.M) * 4);
+    L.rayred = take((size_t)N * 16 * 4); L.wpart = take(wpart_floats(L.M, D) * 4);
     L.n_tiles = L.Mpad / 128;
     if (engine == NNB_ENGINE_TC && (flags & NNB_TCBWD)) {
       // small fp32 side stashes (heads) + operand planes
@@ -76,11 +81,12 @@ inline WsLayout make_layout(int N, int S, uint32_t flags, int engine) {
       L.gmax = take(256);
       L.wgstate = take(256);
     } else {  // fp32 [sample][feature] stash (SIMT backward; also consumed after a TC forward)
-      for (int l = 0; l < 8; ++l) L.h[l] = take(L.Mpad * 256 * 4);
-      L.feat = take(L.Mpad * 256 * 4); L.hr = take(L.Mpad * 128 * 4);
+      const size_t d = (size_t)D, dr = (size_t)(D / 2);
+      for (int l = 0; l < 8; ++l) L.h[l] = take(L.Mpad * d * 4);
+      L.feat = take(L.Mpad * d * 4); L.hr = take(L.Mpad * dr * 4);
       L.enc = take(L.Mpad * 64 * 4); L.denc = take(L.Mpad * 32 * 4);
-      for (int l = 0; l < 8; ++l) L.dy[l] = take(L.Mpad * 256 * 4);
-      L.dfeat = take(L.Mpad * 256 * 4); L.dyr = take(L.Mpad * 128 * 4); L.dyc = take(L.Mpad * 16);
+      for (int l = 0; l < 8; ++l) L.dy[l] = take(L.Mpad * d * 4);
+      L.dfeat = take(L.Mpad * d * 4); L.dyr = take(L.Mpad * dr * 4); L.dyc = take(L.Mpad * 16);
     }
   }
   L.total = o;

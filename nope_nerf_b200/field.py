@@ -8,20 +8,21 @@ from . import ops
 
 class _FieldFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, flags, flat, p, d, *params):
+    def forward(ctx, flags, net, flat, p, d, *params):
         M = p.shape[0]
         need = any(ctx.needs_input_grad)
         if need: flags |= L.STASH
         a = L.RenderArgs()
         p_c = ops._f32c(p.detach()); d_c = None if d is None else ops._f32c(d.detach())
         a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = L.ptr(d_c)
-        a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_SIMT
-        nbytes = L.lib.nnb_workspace_bytes(M, 1, flags, L.ENGINE_SIMT)
+        a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_SIMT; a.hidden_dim = net.hidden_dim
+        nbytes = L.lib.nnb_workspace_bytes_dim(M, 1, flags, L.ENGINE_SIMT, net.hidden_dim)
         ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=p.device)
         a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
         out = torch.empty(M, 4, device=p.device)
         L.check(L.lib.nnb_field_fwd(C.byref(a), L.ptr(out), ops._stream()), "nnb_field_fwd")
         ctx.args = a; ctx.keep = (ws, p_c, d_c, flat); ctx.M = M; ctx.nparams = len(params); ctx.has_d = d is not None
+        ctx.slices = net.param_slices
         return out[:, :3], out[:, 3]
 
     @staticmethod
@@ -31,14 +32,13 @@ class _FieldFn(torch.autograd.Function):
         if g_rgb is not None: g[:, :3] = g_rgb
         if g_a is not None: g[:, 3] = g_a
         g_p = torch.empty(M, 4, device=dev); g_d = torch.empty(M, 4, device=dev)
-        need_w = any(ctx.needs_input_grad[4:])
-        g_w = torch.zeros(L.NUM_PARAMS, device=dev) if need_w else None
+        need_w = any(ctx.needs_input_grad[5:])
+        g_w = torch.zeros(ctx.keep[3].numel(), device=dev) if need_w else None
         L.check(L.lib.nnb_field_bwd(C.byref(ctx.args), L.ptr(g), L.ptr(g_p), L.ptr(g_d), L.ptr(g_w), ops._stream()), "nnb_field_bwd")
         gp = [None] * ctx.nparams
         if g_w is not None:
-            from .model.official_nerf import PARAM_SLICES
-            gp = [g_w[o:o + n].view(s) for (o, n, s) in PARAM_SLICES]
-        return (None, None, g_p[:, :3], g_d[:, :3] if ctx.has_d else None) + tuple(gp)
+            gp = [g_w[o:o + n].view(s) for (o, n, s) in ctx.slices]
+        return (None, None, None, g_p[:, :3], g_d[:, :3] if ctx.has_d else None) + tuple(gp)
 
 
 def field_query(net, p, ray_d, raw_density=False):
@@ -48,5 +48,5 @@ def field_query(net, p, ray_d, raw_density=False):
     shp = p.shape[:-1]
     flags = (L.DIST_ALPHA if net.dist_alpha else 0) | (L.SOFTPLUS if net.occ_activation == 'softplus' else 0) | (L.RAW_DENSITY if raw_density else 0)
     d = None if ray_d is None else ray_d.reshape(-1, 3)
-    rgb, a = _FieldFn.apply(flags, net.flat_weights(), p.reshape(-1, 3), d, *list(net.parameters()))
+    rgb, a = _FieldFn.apply(flags, net, net.flat_weights(), p.reshape(-1, 3), d, *list(net.parameters()))
     return rgb.reshape(*shp, 3), a.reshape(*shp, 1)

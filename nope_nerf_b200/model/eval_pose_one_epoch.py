@@ -50,7 +50,7 @@ class Trainer_pose(object):
                               flags=ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=True),
                               engine=rend.engine if rend.engine is not None else ops.default_engine(),
                               near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
-                              ray_idx=ray_idx, depth=ones, H=h, W=w, stash=backward)
+                              ray_idx=ray_idx, depth=ones, H=h, W=w, stash=backward, hidden_dim=net.hidden_dim)
         # F.mse_loss(rgb, rgb_gt) == l2_mean; seeds: d/d rgb = 2 diff / (3 N)  -> w_rgb = 1/3 with the l2 form
         out4, g_rgb, g_dp, g_dg = ops.loss_rgb_depth(call.rgb, call.depth_pred, call.depth_gt, call.mask, 1.0 / 3.0, 0.0, True,
                                                      img=img.reshape(3, h * w), ray_idx=ray_idx)

@@ -33,7 +33,7 @@ class Extract_Images(object):
                               flags=ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=True),
                               engine=rend.engine if rend.engine is not None else ops.default_engine(),
                               near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
-                              ray_idx=ray_idx, depth_map=torch.ones(1, 1, device=dev), H=h, W=w, stash=False)
+                              ray_idx=ray_idx, depth_map=torch.ones(1, 1, device=dev), H=h, W=w, stash=False, hidden_dim=net.hidden_dim)
         return call.rgb.view(r1 - r0, w, 3), call.depth_pred.view(r1 - r0, w)
 
     def render_geometry(self, c2w, camera_mat, scale_mat, h, w, it=0):

@@ -7,29 +7,47 @@ import torch
 import torch.nn as nn
 from .. import _lib as L
 
-_D, _PIN, _DIN = 256, 63, 27
-_SHAPES = []
-for _blk, _ins in (("layers0", [_PIN, _D, _D, _D]), ("layers1", [_D + _PIN, _D, _D, _D])):
-    for _j, _i in enumerate((0, 2, 4, 6)):
-        _SHAPES += [("%s.%d.weight" % (_blk, _i), (_D, _ins[_j])), ("%s.%d.bias" % (_blk, _i), (_D,))]
-_SHAPES += [("fc_density.weight", (1, _D)), ("fc_density.bias", (1,)), ("fc_feature.weight", (_D, _D)),
-            ("fc_feature.bias", (_D,)), ("rgb_layers.0.weight", (_D // 2, _D + _DIN)), ("rgb_layers.0.bias", (_D // 2,)),
-            ("fc_rgb.weight", (3, _D // 2)), ("fc_rgb.bias", (3,))]
-PARAM_NAMES = [n for n, _ in _SHAPES]
-PARAM_SLICES = []  # (offset, numel, shape) in flat order == parameters() order
-_o = 0
-for _n, _s in _SHAPES:
-    _k = int(math.prod(_s)); PARAM_SLICES.append((_o, _k, _s)); _o += _k
-assert _o == L.NUM_PARAMS
+_PIN, _DIN = 63, 27
+
+
+def param_shapes(D=256):
+    """(state_dict key, shape) of every parameter of a width-D field, in parameters() order (official_nerf.py:20-37)"""
+    shapes = []
+    for blk, ins in (("layers0", [_PIN, D, D, D]), ("layers1", [D + _PIN, D, D, D])):
+        for j, i in enumerate((0, 2, 4, 6)):
+            shapes += [("%s.%d.weight" % (blk, i), (D, ins[j])), ("%s.%d.bias" % (blk, i), (D,))]
+    shapes += [("fc_density.weight", (1, D)), ("fc_density.bias", (1,)), ("fc_feature.weight", (D, D)),
+               ("fc_feature.bias", (D,)), ("rgb_layers.0.weight", (D // 2, D + _DIN)), ("rgb_layers.0.bias", (D // 2,)),
+               ("fc_rgb.weight", (3, D // 2)), ("fc_rgb.bias", (3,))]
+    return shapes
+
+
+def param_slices(D=256):
+    """(offset, numel, shape) of every parameter in the flat vector of a width-D field (flat order == parameters() order)"""
+    out, o = [], 0
+    for _, s in param_shapes(D):
+        k = int(math.prod(s)); out.append((o, k, s)); o += k
+    assert o == L.num_params(D)
+    return out
+
+
+PARAM_NAMES = [n for n, _ in param_shapes()]
+PARAM_SLICES = param_slices(256)  # the default width; a module's own layout is OfficialStaticNerf.param_slices
+assert PARAM_SLICES[-1][0] + 3 == L.NUM_PARAMS
 
 
 class OfficialStaticNerf(nn.Module):
     def __init__(self, cfg):
         super().__init__()
         D = cfg['model']['hidden_dim']
-        if D != 256 or cfg['model']['pos_enc_levels'] != 10 or cfg['model']['dir_enc_levels'] != 4:
-            raise NotImplementedError("the CUDA field is specialised for hidden_dim=256, pos/dir levels 10/4 "
+        if D not in L.HIDDEN_DIMS:
+            raise NotImplementedError("the CUDA field supports model.hidden_dim in {%s} (got %r)" % (", ".join(map(str, L.HIDDEN_DIMS)), D))
+        if cfg['model']['pos_enc_levels'] != 10 or cfg['model']['dir_enc_levels'] != 4:
+            raise NotImplementedError("the CUDA field is specialised for pos/dir encoding levels 10/4 "
                                       "(the reference hard-codes the levels, official_nerf.py:61,87)")
+        self.hidden_dim = D
+        self.num_params = L.num_params(D)
+        self.param_slices = param_slices(D)
         pos_in, dir_in = 63, 27
         self.white_bkgd = cfg['rendering']['white_background']
         self.dist_alpha = cfg['rendering']['dist_alpha']
@@ -51,7 +69,7 @@ class OfficialStaticNerf(nn.Module):
     # ---- flat parameter view -------------------------------------------------------------
     def _plist(self):
         ps = list(self.parameters())
-        assert len(ps) == len(PARAM_SLICES)
+        assert len(ps) == len(self.param_slices)
         return ps
 
     def flat_weights(self):
@@ -61,13 +79,13 @@ class OfficialStaticNerf(nn.Module):
         ok = f is not None and f.device == ps[0].device
         if ok:
             base = f.data_ptr()
-            for p, (o, n, s) in zip(ps, PARAM_SLICES):
+            for p, (o, n, s) in zip(ps, self.param_slices):
                 if p.data_ptr() != base + 4 * o:
                     ok = False; break
         if not ok:
-            f = torch.empty(L.NUM_PARAMS, dtype=torch.float32, device=ps[0].device)
+            f = torch.empty(self.num_params, dtype=torch.float32, device=ps[0].device)
             with torch.no_grad():
-                for p, (o, n, s) in zip(ps, PARAM_SLICES):
+                for p, (o, n, s) in zip(ps, self.param_slices):
                     f[o:o + n].copy_(p.detach().reshape(-1).float())
                     p.data = f[o:o + n].view(s)
             self._flat = f
@@ -79,12 +97,12 @@ class OfficialStaticNerf(nn.Module):
         ps = self._plist()
         g = alias if alias is not None else self._flat_grad
         if g is None or g.device != ps[0].device:
-            g = torch.zeros(L.NUM_PARAMS, dtype=torch.float32, device=ps[0].device)
+            g = torch.zeros(self.num_params, dtype=torch.float32, device=ps[0].device)
             zero = False
         self._flat_grad = g
         if zero:
             g.zero_()
-        for p, (o, n, s) in zip(ps, PARAM_SLICES):
+        for p, (o, n, s) in zip(ps, self.param_slices):
             if p.requires_grad:
                 p.grad = g[o:o + n].view(s)
         return g

@@ -36,7 +36,8 @@ class Renderer(nn.Module):
         meta = dict(N=N, S=int(cfg['num_points']), near=0.0 if ndc else float(self.depth_range[0]),
                     far=1.0 if ndc else float(self.depth_range[1]),
                     flags=ops.flags_from_cfg(cfg, self.model.occ_activation, eval_=eval_),
-                    engine=self.engine if self.engine is not None else ops.default_engine())
+                    engine=self.engine if self.engine is not None else ops.default_engine(),
+                    hidden_dim=getattr(self.model, 'hidden_dim', 256))
         if extra: meta.update(extra)
         return meta
 
@@ -58,7 +59,7 @@ class Renderer(nn.Module):
         if add_noise and self.cfg['sample_option'] == 'uniform':
             noise = torch.rand(batch_size, n_points, S, device=pixels.device)[0]     # rendering.py:189
         meta = self.render_meta(n_points, eval_, dict(pixels=pixels.reshape(n_points, 2).contiguous().float(), noise=noise,
-                                                      want_z_alpha=True))
+                                                      want_z_alpha=True, param_slices=getattr(self.model, 'param_slices', None)))
         flat = self.model.flat_weights()
         d = depth.reshape(n_points)
         rgb, dp, dg, mask, z, alpha = ops.render_autograd(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))

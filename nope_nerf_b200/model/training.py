@@ -238,7 +238,7 @@ class _GraphStep:
         """data parallel: all-reduce of the flat gradient buffer over NVLink peer memory fused with the three Adam updates"""
         tr = self.tr
         net = tr.model.renderer.model; pose, dnet = tr.pose_param_net, tr.distortion_net
-        V = pose.num_cams; o = L.NUM_PARAMS
+        V = pose.num_cams; o = net.num_params
         ops.counter_incr(self.steps)
         fa_m, fa_p, fa_d = self._adams()
         gm = tr.optimizer.param_groups[0]; b1, b2 = gm['betas']
@@ -284,12 +284,13 @@ class _GraphStep:
         call = ops.RenderCall(net.flat_weights(), self.c2w, self.cam, N=n_local, S=S, flags=flags,
                               engine=rend.engine if rend.engine is not None else ops.default_engine(),
                               near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
-                              ray_idx=ray_idx, depth_map=self.dpt, scale=self.ss[0:1], shift=self.ss[1:2], noise=noise, H=h, W=w, stash=True)
+                              ray_idx=ray_idx, depth_map=self.dpt, scale=self.ss[0:1], shift=self.ss[1:2], noise=noise, H=h, W=w, stash=True,
+                              hidden_dim=net.hidden_dim)
         ops.loss_rgb_depth_indirect(call.rgb, call.depth_pred, call.depth_gt, call.mask, 0.0, 0.0, self.rgb_l2, self.imgpp,
                                     ray_idx, h * w, self.out4, self.g_rgb, self.g_dp, self.g_dg, grad_scale=gs, w_dev=self.wts)
         ws = call.ws
         call.pooled = False                                 # memory referenced by a captured graph never returns to the pool
-        bw = (self.g_rgb, self.g_dp, None if tr.detach_gt_depth else self.g_dg, gbuf[:L.NUM_PARAMS], g_c2w, None, None, g_ss)
+        bw = (self.g_rgb, self.g_dp, None if tr.detach_gt_depth else self.g_dg, gbuf[:net.num_params], g_c2w, None, None, g_ss)
         wgk = tr._wg_kwargs()
         if not self.use_ref:
             call.backward(*bw, **wgk)
@@ -343,7 +344,7 @@ class _GraphStep:
         fa_m, fa_p, fa_d = self._adams()
         gm = tr.optimizer.param_groups[0]; b1, b2 = gm['betas']
         flat = net.flat_weights()
-        ops.adam_step_dev(flat, gbuf[:L.NUM_PARAMS], fa_m.m, fa_m.v, self.steps[0:1], self.lrs[0:1], b1, b2, gm['eps'])
+        ops.adam_step_dev(flat, gbuf[:net.num_params], fa_m.m, fa_m.v, self.steps[0:1], self.lrs[0:1], b1, b2, gm['eps'])
         for fa, opt, k in ((fa_p, tr.optimizer_pose, 1), (fa_d, tr.optimizer_distortion, 2)):
             g = opt.param_groups[0]; b1, b2 = g['betas']
             for p in g['params']:
@@ -531,11 +532,12 @@ class Trainer(object):
         return kw
 
     def _grad_buffer(self, peer_step=False):
-        """[MLP 595844 | r 3V | t 3V | scales V | shifts V | loss scalars 4], zeroed; the kernels accumulate into it.
+        """[MLP (595844 floats at hidden_dim 256) | r 3V | t 3V | scales V | shifts V | loss scalars 4], zeroed; the kernels accumulate into it.
         Installed as every parameter's .grad -- except in a peer-exchange step (data parallel, nnb_allreduce_adam), where .grad
         shows the buffer that receives the SUM over the ranks while the local contributions go to the IPC-shared buffer."""
         V = self.pose_param_net.num_cams if self.pose_param_net is not None else 0
-        n = L.NUM_PARAMS + 8 * V + 4
+        n_mlp = self.model.renderer.model.num_params
+        n = n_mlp + 8 * V + 4
         dev = self.device
         if self._gbuf is None or self._gbuf.numel() != n:
             if self.peer_exchange and torch.device(dev).type == 'cuda' and (self.world > 1 or self.fused_adam):
@@ -548,7 +550,7 @@ class Trainer(object):
                 self._gbuf = torch.zeros(n, device=dev)
         g = self._gbuf
         g.zero_()
-        o = L.NUM_PARAMS
+        o = n_mlp
         net = self.model.renderer.model
         shown = self._peer.reduced if (peer_step and self._peer is not None) else g
 
@@ -594,9 +596,8 @@ class Trainer(object):
         fa = self._fadam.get(id(opt))
         if fa is None:
             if mlp:
-                from .official_nerf import PARAM_SLICES
                 net = self.model.renderer.model
-                fa = _FlatAdam(opt, flat_param=net.flat_weights, flat_slices=PARAM_SLICES)
+                fa = _FlatAdam(opt, flat_param=net.flat_weights, flat_slices=net.param_slices)
             else:
                 fa = _FlatAdam(opt)
             self._fadam[id(opt)] = fa
@@ -787,7 +788,7 @@ class Trainer(object):
                                   engine=rend.engine if rend.engine is not None else ops.default_engine(),
                                   near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
                                   ray_idx=ray_idx, depth_map=depth_input.detach().reshape(h_depth, w_depth).contiguous(),
-                                  scale=scale_dev, shift=shift_dev, noise=noise, H=h, W=w, stash=backward)
+                                  scale=scale_dev, shift=shift_dev, noise=noise, H=h, W=w, stash=backward, hidden_dim=net.hidden_dim)
             inv = self.depth_loss_type == 'invariant' and weights['depth_weight'] != 0.0
             out4, g_rgb, g_dp, g_dg = ops.loss_rgb_depth(call.rgb, call.depth_pred, call.depth_gt, call.mask,
                                                          weights['rgb_weight'], 0.0 if inv else weights['depth_weight'], rgb_loss_type == 'l2',
@@ -807,7 +808,7 @@ class Trainer(object):
                 g_c2w = torch.zeros(4, 4, device=device)
                 g_ss = torch.zeros(2, device=device)
                 g_cam = torch.zeros(4, 4, device=device) if fxfy is not None else None
-                call.backward(g_rgb, g_dp, None if self.detach_gt_depth else g_dg, gbuf[:L.NUM_PARAMS], g_c2w, g_cam, None, g_ss, **self._wg_kwargs())
+                call.backward(g_rgb, g_dp, None if self.detach_gt_depth else g_dg, gbuf[:net.num_params], g_c2w, g_cam, None, g_ss, **self._wg_kwargs())
                 ops.pose_bwd_raw(pose.r.detach(), pose.t.detach(), init, img_idx, g_c2w,
                                  gv['r'] if pose.r.requires_grad else None, gv['t'] if pose.t.requires_grad else None)
                 # chain d/d(scale_eff, shift) into global_scales / global_shifts (clamp / fixed-last-view aware)

@@ -122,7 +122,7 @@ class RenderCall:
     """One forward launch + the state its backward needs (workspace with the stash)."""
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
-                 depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, wgrad=None):
+                 depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, wgrad=None, hidden_dim=256):
         for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels),
                        ("depth", depth), ("noise", noise)):
             _need_cuda(t_, n_)
@@ -145,14 +145,17 @@ class RenderCall:
                 if (wgrad or _WGRAD[0]) == "fp16": flags |= L.WG16
         if engine == L.ENGINE_TC and _FWD_DROP[0]:
             flags |= (_FWD_DROP[0] & 1) * L.FWD_DROP_WLO | ((_FWD_DROP[0] >> 1) & 1) * L.FWD_DROP_ALO
-        a.flags = flags; a.engine = engine
+        a.flags = flags; a.engine = engine; a.hidden_dim = int(hidden_dim)
+        self.hidden_dim = int(hidden_dim)
         self.rgb = torch.empty(N, 3, device=dev); self.depth_pred = torch.empty(N, device=dev)
         self.depth_gt = torch.empty(N, device=dev); self.mask = torch.empty(N, dtype=torch.uint8, device=dev)
         self.z_vals = torch.empty(N, S, device=dev) if want_z_alpha else None
         self.alpha = torch.empty(N, S, device=dev) if want_z_alpha else None
         a.rgb = L.ptr(self.rgb); a.depth_pred = L.ptr(self.depth_pred); a.depth_gt = L.ptr(self.depth_gt)
         a.mask = L.ptr(self.mask); a.z_vals = L.ptr(self.z_vals); a.alpha = L.ptr(self.alpha)
-        nbytes = L.lib.nnb_workspace_bytes(N, S, flags, engine)
+        nbytes = L.lib.nnb_workspace_bytes_dim(N, S, flags, engine, int(hidden_dim))
+        if nbytes == 0:
+            raise ValueError("nope_nerf_b200: hidden_dim %s is not supported (supported: %s)" % (hidden_dim, L.HIDDEN_DIMS))
         self.ws = _pool.take(nbytes, dev)
         a.workspace = L.ptr(self.ws); a.workspace_bytes = self.ws.numel()
         self.args = a; self.N = N; self.S = S; self.stash = stash; self.pooled = True
@@ -187,12 +190,16 @@ class RenderCall:
 
 class _RenderFn(torch.autograd.Function):
     """autograd glue for the drop-in Renderer / nope_nerf modules.
-    differentiable inputs: c2w (4,4), cam (4,4), depth (N,) | (scale, shift) and the 24 MLP parameters."""
+    differentiable inputs: c2w (4,4), cam (4,4), depth (N,) | (scale, shift) and the 24 MLP parameters.
+    meta['param_slices'] (optional): the model's (offset, numel, shape) list (OfficialStaticNerf.param_slices); meta['hidden_dim']
+    its width (default 256)."""
 
     @staticmethod
     def forward(ctx, meta, flat, c2w, cam, depth, scale, shift, *params):
         # (grad mode is always off inside Function.forward: decide from the inputs' requires_grad)
         need_grad = any(ctx.needs_input_grad)
+        meta = dict(meta)
+        ctx.param_slices = meta.pop("param_slices", None)
         call = RenderCall(flat, _f32c(c2w.detach()), _f32c(cam.detach()), stash=need_grad,
                           depth=None if depth is None else _f32c(depth.detach()),
                           scale=None if scale is None else _f32c(scale.detach()),
@@ -213,15 +220,17 @@ class _RenderFn(torch.autograd.Function):
         dev = call.rgb.device
         if g_rgb is None: g_rgb = torch.zeros(call.N, 3, device=dev)
         g_c2w = torch.zeros(4, 4, device=dev); g_cam = torch.zeros(4, 4, device=dev)
-        g_w = torch.zeros(L.NUM_PARAMS, device=dev) if ctx.params_need else None
+        g_w = torch.zeros(L.num_params(call.hidden_dim), device=dev) if ctx.params_need else None
         has_depth, has_scale, has_shift = ctx.has
         g_depth = torch.empty(call.N, device=dev) if has_depth else None
         g_ss = torch.zeros(2, device=dev) if (has_scale or has_shift) else None
         call.backward(g_rgb, g_dp, g_dg, g_w, g_c2w, g_cam, g_depth, g_ss)
         gp = [None] * ctx.nparams
         if g_w is not None:
-            from .model.official_nerf import PARAM_SLICES
-            gp = [g_w[o:o + n].view(shape) for (o, n, shape) in PARAM_SLICES]
+            slices = ctx.param_slices
+            if slices is None:
+                from .model.official_nerf import PARAM_SLICES as slices
+            gp = [g_w[o:o + n].view(shape) for (o, n, shape) in slices]
         return (None, None, g_c2w, g_cam, g_depth, g_ss[0] if has_scale else None, g_ss[1] if has_shift else None) + tuple(gp)
 
 

@@ -70,8 +70,8 @@ def build_model(mdl, cfg, P):
     return net, rend, model
 
 
-def case_render(mdl, name, overrides, N, S, H, W, hd, wd, eval_mode, add_noise, seed, pose_mode, prior="dpt", hf_damp=False):
-    """nope_nerf.forward (model/network.py:19-33 -> model/rendering.py:36-167) + autograd grads."""
+def case_render(mdl, name, overrides, N, S, H, W, hd, wd, eval_mode, add_noise, seed, pose_mode, prior="dpt", hf_damp=False, hidden_dim=256):
+    """nope_nerf.forward (model/network.py:19-33 -> model/rendering.py:36-167) + autograd grads; hidden_dim = model.hidden_dim."""
     import torch
     from oracle import nerf_oracle as O
     cfg = base_cfg()
@@ -79,7 +79,8 @@ def case_render(mdl, name, overrides, N, S, H, W, hd, wd, eval_mode, add_noise, 
         sec, key = k.split(".")
         cfg[sec][key] = v
     cfg["rendering"]["num_points"] = S
-    P = O.init_params(seed=seed, white_bkgd=cfg["rendering"]["white_background"], hf_damp=hf_damp)
+    cfg["model"]["hidden_dim"] = hidden_dim
+    P = O.init_params(seed=seed, D=hidden_dim, white_bkgd=cfg["rendering"]["white_background"], hf_damp=hf_damp)
     net, rend, model = build_model(mdl, cfg, P)
     rng = np.random.default_rng(seed + 1)
     V = 5
@@ -131,7 +132,7 @@ def case_render(mdl, name, overrides, N, S, H, W, hd, wd, eval_mode, add_noise, 
     scalar = (out["rgb"] * torch.from_numpy(g_rgb)).sum() + (out["depth_pred"] * torch.from_numpy(g_dp)).sum() \
         + (out["depth_gt"] * torch.from_numpy(g_dg)).sum()
     scalar.backward()
-    rec = dict(N=N, S=S, H=H, W=W, seed=seed, cam_id=cam_id, kx=kx, ky=ky, eval_mode=eval_mode, hf_damp=hf_damp,
+    rec = dict(N=N, S=S, H=H, W=W, seed=seed, cam_id=cam_id, kx=kx, ky=ky, eval_mode=eval_mode, hf_damp=hf_damp, hidden_dim=hidden_dim,
                add_noise=add_noise, r=r, t=t, dpt=dpt, ray_idx=ray_idx, scale=1.07, shift=-0.03,
                pixels=p[0].detach().numpy(), c2w=c2w.detach().numpy(),
                g_rgb=g_rgb[0], g_dp=g_dp, g_dg=g_dg,
@@ -154,12 +155,13 @@ def case_render(mdl, name, overrides, N, S, H, W, hd, wd, eval_mode, add_noise, 
     print("wrote", name, "rgb[0]", rec["rgb"][0], "grad_r", rec["grad_r"][cam_id])
 
 
-def case_mlp(mdl, name, M, dist_alpha, occ, seed):
+def case_mlp(mdl, name, M, dist_alpha, occ, seed, hidden_dim=256):
     """OfficialStaticNerf.forward (model/official_nerf.py:69-96) + grads wrt inputs/params."""
     import torch
     from oracle import nerf_oracle as O
     cfg = base_cfg(); cfg["rendering"]["dist_alpha"] = dist_alpha; cfg["model"]["occ_activation"] = occ
-    P = O.init_params(seed=seed)
+    cfg["model"]["hidden_dim"] = hidden_dim
+    P = O.init_params(seed=seed, D=hidden_dim)
     net = mdl.OfficialStaticNerf(cfg)
     net.load_state_dict({k: torch.from_numpy(np.array(v)) for k, v in P.items()})
     rng = np.random.default_rng(seed + 7)
@@ -169,7 +171,7 @@ def case_mlp(mdl, name, M, dist_alpha, occ, seed):
     rgb, a = net(tp, td, return_addocc=True)
     g_rgb = rng.normal(0, 1, (M, 3)).astype(np.float32); g_a = rng.normal(0, 1, (M, 1)).astype(np.float32)
     ((rgb * torch.from_numpy(g_rgb)).sum() + (a * torch.from_numpy(g_a)).sum()).backward()
-    rec = dict(M=M, seed=seed, dist_alpha=dist_alpha, occ=occ, pts=pts, dirs=dirs, g_rgb=g_rgb, g_a=g_a[:, 0],
+    rec = dict(M=M, seed=seed, dist_alpha=dist_alpha, occ=occ, hidden_dim=hidden_dim, pts=pts, dirs=dirs, g_rgb=g_rgb, g_a=g_a[:, 0],
                rgb=rgb.detach().numpy(), a=a.detach().numpy()[:, 0], g_pts=tp.grad.numpy(), g_dirs=td.grad.numpy(),
                enc=__import__("model.official_nerf", fromlist=["x"]).encode_position(torch.from_numpy(pts), 10, True).numpy())
     for n, prm in net.named_parameters():
@@ -206,9 +208,10 @@ def case_pose(mdl, name):
     print("wrote", name)
 
 
-def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_view=False, learn_focal=False, training=None):
+def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_view=False, learn_focal=False, training=None,
+                    hidden_dim=256):
     """Trainer.train_step (model/training.py:67-97) for `steps` iterations on one synthetic pair; `training` overrides keys of
-    cfg['training'] (stored as cfg.training.<key>)."""
+    cfg['training'] (stored as cfg.training.<key>); hidden_dim = model.hidden_dim (stored as hidden_dim)."""
     import torch
     from oracle import nerf_oracle as O
     cfg = base_cfg()
@@ -217,7 +220,8 @@ def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_v
     if not with_ref:
         cfg["training"]["pc_weight"] = [0.0, 0.0]; cfg["training"]["rgb_s_weight"] = [0.0, 0.0]
     cfg["training"]["vis_reprojection_every"] = 10 ** 9
-    P = O.init_params(seed=seed)
+    cfg["model"]["hidden_dim"] = hidden_dim
+    P = O.init_params(seed=seed, D=hidden_dim)
     net, rend, model = build_model(mdl, cfg, P)
     V = 4
     rng = np.random.default_rng(seed + 3)
@@ -252,7 +256,7 @@ def case_train_step(mdl, name, with_ref, steps, N, S, H, W, hd, wd, seed, last_v
             "img.ref_imgs": torch.from_numpy(ref), "img.ref_dpts": torch.from_numpy(rdpt),
             "img.ref_idxs": torch.tensor([ref_idx])}
     rec = dict(N=N, S=S, H=H, W=W, V=V, seed=seed, idx=idx, ref_idx=ref_idx, kx=kx, ky=ky, img=img[0], ref=ref[0],
-               dpt=dpt[0], rdpt=rdpt[0], r0=r0, t0=t0, scales0=sc0, shifts0=sh0, steps=steps, with_ref=with_ref)
+               dpt=dpt[0], rdpt=rdpt[0], r0=r0, t0=t0, scales0=sc0, shifts0=sh0, steps=steps, with_ref=with_ref, hidden_dim=hidden_dim)
     for k, v in (training or {}).items():
         rec["cfg.training." + k] = np.array(v)
     if learn_focal:
@@ -356,6 +360,20 @@ def main():
                         training={"detach_ref_img": False})
         case_train_step(mdl, "train_full_ssim_undetached_shiftfirst", True, steps=1, N=48, S=32, H=24, W=32, hd=32, wd=48, seed=38,
                         training={"with_ssim": True, "detach_ref_img": False, "shift_first": True})
+
+    if "hidden" in which:
+        # model.hidden_dim 128 and 64: the field's trunk / rgb hidden layers D and D/2 wide (official_nerf.py:11-37)
+        for D in (128, 64):
+            case_mlp(mdl, "mlp_alpha_softplus_d%d" % D, 96, False, "softplus", 11, hidden_dim=D)
+            for damp in (False, True):
+                sfx = "_d%d%s" % (D, "_damped" if damp else "")
+                case_render(mdl, "render_tanks_noise" + sfx, {}, N=24, S=128, H=30, W=40, hd=12, wd=21, eval_mode=False,
+                            add_noise=True, seed=21, pose_mode="rand", hf_damp=damp, hidden_dim=D)
+                case_render(mdl, "render_ndc_distalpha" + sfx, {"rendering.sample_option": "ndc", "rendering.dist_alpha": True,
+                                                                "rendering.depth_range": [0.0, 1.0]},
+                            N=24, S=128, H=30, W=40, hd=16, wd=20, eval_mode=False, add_noise=True, seed=24, pose_mode="rand", hf_damp=damp,
+                            hidden_dim=D)
+            case_train_step(mdl, "train_full_losses_d%d" % D, True, steps=2, N=48, S=32, H=24, W=32, hd=16, wd=24, seed=32, hidden_dim=D)
 
 
 if __name__ == "__main__":
