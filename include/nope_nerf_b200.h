@@ -57,6 +57,8 @@ typedef struct nnb_render_args {
   const float* scale;     /* [1] depth distortion scale or NULL (=1)  (distortions.py:19-27)        */
   const float* shift;     /* [1] depth distortion shift or NULL (=0)                                */
   const float* noise;     /* [N,S] stratified jitter U[0,1) (rendering.py:189) or NULL              */
+  /* S = rendering.num_points, samples per ray: 2..1024 on NNB_ENGINE_SIMT, 16..1024 on NNB_ENGINE_TC; other values are rejected
+   * (rc < 0).  The Python package runs S < 16 on the SIMT engine and every other S on the tensor-core engine by default. */
   int32_t N, S, H, W, h_d, w_d;
   float near_, far_;      /* rendering.depth_range                                                  */
   uint32_t flags;

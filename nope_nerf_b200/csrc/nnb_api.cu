@@ -98,7 +98,7 @@ static int check_dim(const nnb_render_args* a) {
 static int check_args(const nnb_render_args* a) {
   if (!a) return fail(-1, "null args");
   if (a->N <= 0) return fail(-2, "N must be positive (got %d)", a->N);
-  if (a->S < 2 || a->S > 256) return fail(-2, "S must be in [2,256] (got %d)", a->S);
+  if (a->S < 2 || a->S > 1024) return fail(-2, "S must be in [2,1024] (got %d)", a->S);
   if (!a->weights || !a->c2w || !a->cam) return fail(-3, "weights / c2w / cam must be non-null");
   if (!a->ray_idx && !a->pixels) return fail(-3, "need ray_idx or pixels");
   if (!a->pixels && (a->H < 2 || a->W < 2)) return fail(-3, "H,W needed to derive pixels from ray_idx");
@@ -111,7 +111,7 @@ static int check_args(const nnb_render_args* a) {
   if (a->engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
 #else
   if (a->engine == NNB_ENGINE_TC && !tc_supports(a->S))
-    return fail(-4, "tensor-core engine needs S in {32,64,128,256} (got %d); use NNB_ENGINE_SIMT", a->S);
+    return fail(-4, "tensor-core engine needs S in [16,1024] (got %d); use NNB_ENGINE_SIMT", a->S);
 #endif
   size_t need = nnb_workspace_bytes_dim(a->N, a->S, a->flags, a->engine, a->hidden_dim);
   if (!a->workspace || a->workspace_bytes < need)

@@ -248,8 +248,6 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
 // ---------------------------------------------------------------------------------------
 // compositing (rendering.py:122-158), one warp per ray; shared by both engines
 // ---------------------------------------------------------------------------------------
-constexpr int MAXC = 8;  // S <= 256
-
 __device__ __forceinline__ float sample_alpha(const nnb_render_args& a, const SampleRec* rr, int i, const SampleRec& me) {
   if (!(a.flags & NNB_DIST_ALPHA)) return me.a;
   if (i == a.S - 1) return 1.f;  // alpha[:, -1] = 1 (rendering.py:128)
@@ -302,46 +300,53 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
   if ((a.flags & NNB_EVAL) && (a.flags & NNB_NORMALISE)) gD = gD / ray.nrm;
   const float gC0 = __ldg(b.g_rgb + 3 * n), gC1 = __ldg(b.g_rgb + 3 * n + 1), gC2 = __ldg(b.g_rgb + 3 * n + 2);
   const float gsum = (a.flags & NNB_WHITE_BG) ? (gC0 + gC1 + gC2) : 0.f;
-  float Tm[MAXC], wm[MAXC], gwm[MAXC], omm[MAXC], dfac[MAXC];
-  float carry = 1.f;
+  // chunk c's terms from its records: alpha, om = 1 - alpha + eps, the inclusive product of om over the chunk, and the transmittance
+  // T given the carry into the chunk
+  auto chunk = [&](int c, float carry, float& alpha, float& om, float& incl, float& T) {
+    const int i = c * 32 + lane; const bool valid = i < a.S;
+    const SampleRec me = valid ? rr[i] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
+    alpha = valid ? sample_alpha(a, rr, i, me) : 0.f;
+    om = valid ? __fadd_rn(__fsub_rn(1.f, alpha), NNB_EPS) : 1.f;
+    incl = warp_incl_prod(om, lane);
+    float excl = __shfl_up_sync(0xffffffffu, incl, 1); if (lane == 0) excl = 1.f;
+    T = carry * excl;
+    return me;
+  };
+  // forward sweep: only the transmittance carried into each chunk of 32 samples; lane c keeps chunk c's, hence S <= 32 * 32 = 1024
+  float carry = 1.f, carry_c = 1.f;
   const int C = (a.S + 31) / 32;
-#pragma unroll
-  for (int c = 0; c < MAXC; ++c) {
-    if (c < C) {
-      int i = c * 32 + lane; bool valid = i < a.S;
-      SampleRec me = valid ? rr[i] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
-      float alpha = valid ? sample_alpha(a, rr, i, me) : 0.f;
-      float om = valid ? __fadd_rn(__fsub_rn(1.f, alpha), NNB_EPS) : 1.f;
-      float incl = warp_incl_prod(om, lane);
-      float excl = __shfl_up_sync(0xffffffffu, incl, 1); if (lane == 0) excl = 1.f;
-      float T = carry * excl;
-      carry *= __shfl_sync(0xffffffffu, incl, 31);
-      Tm[c] = T; wm[c] = alpha * T; omm[c] = om;
-      gwm[c] = gC0 * me.r + gC1 * me.g + gC2 * me.b + gD * me.z - gsum;
-      float df = 1.f;  // d alpha / d a
-      if (a.flags & NNB_DIST_ALPHA) {
-        if (i >= a.S - 1) df = 0.f;
-        else { float delta = __fsub_rn(rr[i + 1].z, me.z); df = delta * expf(-me.a * delta); }
-      }
-      dfac[c] = df;
-    }
+  for (int c = 0; c < C; ++c) {
+    if (lane == c) carry_c = carry;
+    float alpha, om, incl, T;
+    chunk(c, carry, alpha, om, incl, T);
+    carry *= __shfl_sync(0xffffffffu, incl, 31);
   }
+  // reverse sweep: each chunk's terms recomputed from the records with the same operations, then the in-chunk suffix scan with the
+  // suffix of the later chunks carried in
   float carry_s = 0.f, vmax = 0.f;
-#pragma unroll
-  for (int c = MAXC - 1; c >= 0; --c) {
-    if (c < C) {
-      int i = c * 32 + lane; bool valid = i < a.S;
-      float wg = valid ? wm[c] * gwm[c] : 0.f;
-      float incl = warp_incl_sum_rev(wg, lane);
-      float excl = __shfl_down_sync(0xffffffffu, incl, 1); if (lane == 31) excl = 0.f;
-      float suffix = excl + carry_s;
-      carry_s += __shfl_sync(0xffffffffu, incl, 0);
-      float g_alpha = Tm[c] * gwm[c] - suffix / omm[c];
-      if (valid) {
-        float4 o = make_float4(wm[c] * gC0, wm[c] * gC1, wm[c] * gC2, g_alpha * dfac[c]);
-        gs[(size_t)n * a.S + i] = o;
-        vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
-      }
+  for (int c = C - 1; c >= 0; --c) {
+    const int i = c * 32 + lane; const bool valid = i < a.S;
+    float alpha, om, incl_p, T;
+    const SampleRec me = chunk(c, __shfl_sync(0xffffffffu, carry_c, c), alpha, om, incl_p, T);
+    const float w = alpha * T;
+    // d L / d w with its multiply-adds spelled out: a contracted a*b + c*d may fuse either product, and the choice would otherwise
+    // depend on how the compiler schedules this loop
+    const float gw = fmaf(gD, me.z, fmaf(gC2, me.b, fmaf(gC1, me.g, gC0 * me.r))) - gsum;
+    float df = 1.f;  // d alpha / d a
+    if (a.flags & NNB_DIST_ALPHA) {
+      if (i >= a.S - 1) df = 0.f;
+      else { float delta = __fsub_rn(rr[i + 1].z, me.z); df = delta * expf(-me.a * delta); }
+    }
+    float wg = valid ? w * gw : 0.f;
+    float incl = warp_incl_sum_rev(wg, lane);
+    float excl = __shfl_down_sync(0xffffffffu, incl, 1); if (lane == 31) excl = 0.f;
+    float suffix = excl + carry_s;
+    carry_s += __shfl_sync(0xffffffffu, incl, 0);
+    float g_alpha = T * gw - suffix / om;
+    if (valid) {
+      float4 o = make_float4(w * gC0, w * gC1, w * gC2, g_alpha * df);
+      gs[(size_t)n * a.S + i] = o;
+      vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
     }
   }
   if (gmax) {

@@ -50,7 +50,10 @@ template <int D> struct Tc {
   static constexpr int SM_BIAS = SM_W + NST * STAGE_BYTES;
   static constexpr int BIAS_FLOATS = 8 * D + D + D + 3 * (D / 2) + 4;   // trunk, feat, w_sigma, W_rgb, (b_sigma, b_rgb[3])
   static constexpr int SM_RAYB = SM_BIAS + ((BIAS_FLOATS * 4 + 127) / 128) * 128;
-  static constexpr int RAYB_FLOATS = 2 * (D / 2) + 2 * 32;   // per warpgroup: per-ray bias [2 rays][D/2] + direction encodings [2][32]
+  // per warpgroup: per-ray bias [RAYB_RAYS][D/2] + direction encodings [RAYB_RAYS][32].  A 64-row block that starts at a multiple of 64
+  // overlaps at most ceil(63 / S) + 1 rays: 5 at the smallest S of this engine (16), 2 for S >= 64
+  static constexpr int RAYB_RAYS = 5;
+  static constexpr int RAYB_FLOATS = RAYB_RAYS * (D / 2) + RAYB_RAYS * 32;
   static constexpr int SM_BAR = SM_RAYB + 2 * RAYB_FLOATS * 4;
   static constexpr int SM_TOTAL = SM_BAR + 2 * NST * 8;
   // ---- data-gradient chain (176 transposed stages at D = 256) ----
@@ -174,15 +177,19 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
   const uint32_t w_base = smem_u32(smem + SM_W);
   const uint32_t bar_id = 1u + (uint32_t)wg;
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
-  const int rays_per_wg = (a.S >= 64) ? 1 : 64 / a.S;
+  constexpr int RAYB_DE = T::RAYB_RAYS * DR;   // direction encodings after the per-ray biases
   uint32_t slot = 0, phase = 0;
   float acc[D / 2];
 
   for (int t = 0; t < my_tiles; ++t) {
     const int tile = blockIdx.x + t * gridDim.x;
     const size_t mt = (size_t)tile * TILE;
+    // sample index of this warpgroup's first row inside its ray: row rl reads the bias of the block's ray (ray_off() + rl) / S.  Computed
+    // where it is used, not held across the MMAs.
+    auto ray_off = [&]() { return (int)((mt + (size_t)wg * 64) % (size_t)a.S); };
     wg_sync();   // the previous tile's epilogue is done with the per-ray bias buffer
     {
+      const int off0 = ray_off();
       // ---- prologue: thread (row rl, part) writes encoding columns [32 part, 32 part + 32) of its row ----
       const int rl = tl & 63, part = tl >> 6, row = wg * 64 + rl;
       const size_t m = mt + row;
@@ -218,20 +225,21 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
           for (int k4 = 0; k4 < 8; ++k4)
             *reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4) = make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]);
         }
-        if (rl % (rays_per_wg == 1 ? 64 : a.S) == 0) {   // the row that starts a ray publishes its direction encoding
-          const int r = rays_per_wg == 1 ? 0 : rl / a.S;
+        if (rl == 0 || (off0 + rl) % a.S == 0) {   // the block's first row and every row that starts a ray publish its direction encoding
+          const int r = (off0 + rl) / a.S;
 #pragma unroll
-          for (int k = 0; k < 32; ++k) rayb[D + r * 32 + k] = de[k];
+          for (int k = 0; k < 32; ++k) rayb[RAYB_DE + r * 32 + k] = de[k];
         }
       }
       fence_async_smem();
       wg_sync();
       const float* w = a.weights;
-      for (int r = 0; r < rays_per_wg; ++r) {   // thread tl = output column of the rgb hidden layer
+      const int n_rays = (off0 + 63) / a.S + 1;
+      for (int r = 0; r < n_rays; ++r) {   // thread tl = output column of the rgb hidden layer
         if (DR < 128 && tl >= DR) break;
         float b = __ldg(w + nnb::B_RGBH(D) + tl);
 #pragma unroll
-        for (int k = 0; k < 27; ++k) b = fmaf(__ldg(w + nnb::W_RGBH(D) + (size_t)tl * (D + 27) + D + k), rayb[D + r * 32 + k], b);
+        for (int k = 0; k < 27; ++k) b = fmaf(__ldg(w + nnb::W_RGBH(D) + (size_t)tl * (D + 27) + D + k), rayb[RAYB_DE + r * 32 + k], b);
         rayb[r * DR + tl] = b;   // read after layer 0's epilogue barrier
       }
     }
@@ -293,13 +301,14 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
       } else {
         // rgb hidden layer (D/2 columns) -> colour head + per-sample record
         float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+        const int off0 = ray_off();
 #pragma unroll
         for (int j = 0; j < DR / 8; ++j) {
           const int col = j * 8 + c0;
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
             const int row = r0 + 8 * r;
-            const float* rb = rayb + (rays_per_wg == 1 ? 0 : (row - wg * 64) / a.S) * DR;
+            const float* rb = rayb + ((off0 + row - wg * 64) / a.S) * DR;
             const float v0 = fmaxf(acc[4 * j + 2 * r] + rb[col], 0.f), v1 = fmaxf(acc[4 * j + 2 * r + 1] + rb[col + 1], 0.f);
 #pragma unroll
             for (int c = 0; c < 3; ++c)
@@ -842,7 +851,8 @@ size_t tc_workspace_extra(int N, int S, uint32_t flags, int D) {
   return D == 128 ? tc_extra_dim<128>() : (D == 64 ? tc_extra_dim<64>() : tc_extra_dim<256>());
 }
 
-bool tc_supports(int S) { return S == 32 || S == 64 || S == 128 || S == 256; }
+// S >= 16 bounds the rays one 64-row block overlaps (Tc<D>::RAYB_RAYS); S <= 1024 is the compositing adjoint's limit
+bool tc_supports(int S) { return S >= 16 && S <= 1024; }
 
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
   if (!tc_supports(a.S)) return cudaErrorNotSupported;

@@ -48,12 +48,15 @@ def default_engine():
     return _DEFAULT_ENGINE[0]
 
 
+TC_MIN_S = 16   # samples per ray: the tensor-core engine's lower limit; both engines go up to 1024
+
+
 def pick_engine(engine, S):
-    """the tensor-core engine tiles 128 samples per CTA and needs S in {32,64,128,256}; other sample counts
-    run on the exact-fp32 SIMT engine (still CUDA; there is no CPU path)."""
+    """the tensor-core engine serves 16 <= S <= 1024 samples per ray; fewer samples run on the exact-fp32 SIMT engine (still CUDA;
+    there is no CPU path), which serves 2 <= S <= 1024.  An explicit ENGINE_SIMT is kept at every S."""
     if engine is None:
         engine = _DEFAULT_ENGINE[0]
-    if engine == L.ENGINE_TC and S not in (32, 64, 128, 256):
+    if engine == L.ENGINE_TC and S < TC_MIN_S:
         return L.ENGINE_SIMT
     return engine
 

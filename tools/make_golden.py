@@ -375,6 +375,22 @@ def main():
                             hidden_dim=D)
             case_train_step(mdl, "train_full_losses_d%d" % D, True, steps=2, N=48, S=32, H=24, W=32, hd=16, wd=24, seed=32, hidden_dim=D)
 
+    if "samples" in which:
+        # rendering.num_points outside {32, 64, 128, 256}: rays that straddle the 64-row blocks of the tensor-core engine, and S > 256
+        for damp in (False, True):
+            sfx = "_damped" if damp else ""
+            case_render(mdl, "render_tanks_noise_s48" + sfx, {}, N=32, S=48, H=30, W=40, hd=12, wd=21, eval_mode=False,
+                        add_noise=True, seed=51, pose_mode="rand", hf_damp=damp)
+            case_render(mdl, "render_ndc_distalpha_s96" + sfx, {"rendering.sample_option": "ndc", "rendering.dist_alpha": True,
+                                                                "rendering.depth_range": [0.0, 1.0]},
+                        N=24, S=96, H=30, W=40, hd=16, wd=20, eval_mode=False, add_noise=True, seed=52, pose_mode="rand", hf_damp=damp)
+            case_render(mdl, "render_eval_ones_s200" + sfx, {}, N=24, S=200, H=27, W=48, hd=27, wd=48, eval_mode=True,
+                        add_noise=False, seed=53, pose_mode="init", prior="ones", hf_damp=damp)
+            case_render(mdl, "render_tanks_noise_s300" + sfx, {}, N=24, S=300, H=30, W=40, hd=12, wd=21, eval_mode=False,
+                        add_noise=True, seed=54, pose_mode="rand", hf_damp=damp)
+        case_train_step(mdl, "train_full_losses_s48", True, steps=2, N=48, S=48, H=24, W=32, hd=16, wd=24, seed=55)
+        case_train_step(mdl, "train_render_only_s300", False, steps=2, N=24, S=300, H=24, W=32, hd=16, wd=24, seed=56)
+
 
 if __name__ == "__main__":
     main()
