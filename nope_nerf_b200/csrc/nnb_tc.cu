@@ -10,13 +10,14 @@
 //               accumulation in registers) so results match the fp32 reference.  The epilogue (bias, ReLU, re-split into
 //               hi | lo halves) writes the next layer's A operand IN PLACE: a warpgroup's MMAs read only its own 64 rows, and
 //               they have completed (wgmma.wait_group 0) before the epilogue starts.  Density / colour heads, the per-sample
-//               record and the fp32 training stash come out of the same registers.
+//               record, the fp32 training stash and the ReLU gate bits of the backward come out of the same registers.
 //   warp 8   : weight producer (in the third warpgroup, whose registers go to the consumers) - cp.async.bulk of pre-imaged
 //               fp16 hi | lo weight stages (all output rows x 16 k) from L2 into a 3-deep shared-memory ring, mbarrier tx-count;
 //               a stage is released once both warpgroups' MMAs have read it.
 //
-// The backward of this engine (tc_render_bwd) runs tc_dgrad (the same skeleton through the transposed weights) and tc_wgrad (the
-// MLP weight-gradient GEMMs) on the fp32 stash, between the compositing and ray adjoints of nnb_simt.cu.
+// The backward of this engine (tc_render_bwd) runs tc_dgrad (the same skeleton through the transposed weights, gated by the
+// forward's ReLU bits) and tc_wgrad (the MLP weight-gradient GEMMs on the fp32 stash), between the compositing and ray adjoints of
+// nnb_simt.cu.
 //
 // Shared-memory operand layout (no swizzle, "interleave"): element (row, k) of a [rows x K] fp16 operand lives at byte
 // (k / 8) * rows * 16 + row * 16 + (k % 8) * 2: 8 x 8 core matrices of 128 contiguous bytes, SBO = 128 B between row groups,
@@ -99,7 +100,29 @@ __global__ void tc_prep_weights(const float* __restrict__ w, unsigned char* __re
   }
 }
 
-struct TcStash { float *h[8], *feat, *hr, *enc, *denc; };   // fp32 [sample][feature] stash, layout of nnb_simt.cu
+// fp32 [sample][feature] stash, layout of nnb_simt.cu, and the ReLU gate bits of h0..h7 and hr (gate_bits_off).  This and DgPtrs are
+// __grid_constant__ kernel parameters: indexed by layer in parameter space, not copied to local memory (which would also leave the
+// pointers generic instead of global)
+struct TcStash { float *h[8], *feat, *hr, *enc, *denc; unsigned char* gates; };
+
+// this thread's NB ReLU gate bits of one tile and layer (NB = 16 | 32 | 64 | 128, see gate_bits_off): one vector access.  In
+// registers, bit b of the set is bit 31 - b % 32 of word b / 32 (a 16-bit set is loaded into the upper half of its word).  Stored
+// like the stash (st.global.cs, evict-first).
+template <int NB> __device__ __forceinline__ void store_gates(unsigned char* p, const uint32_t* w) {
+  if constexpr (NB == 128) __stcs(reinterpret_cast<uint4*>(p), make_uint4(w[0], w[1], w[2], w[3]));
+  else if constexpr (NB == 64) __stcs(reinterpret_cast<uint2*>(p), make_uint2(w[0], w[1]));
+  else if constexpr (NB == 32) __stcs(reinterpret_cast<unsigned int*>(p), w[0]);
+  else __stcs(reinterpret_cast<unsigned short*>(p), (unsigned short)w[0]);
+}
+template <int NB> __device__ __forceinline__ void load_gates(const unsigned char* p, uint32_t* w) {
+  if constexpr (NB == 128) { const uint4 v = __ldg(reinterpret_cast<const uint4*>(p)); w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w; }
+  else if constexpr (NB == 64) { const uint2 v = __ldg(reinterpret_cast<const uint2*>(p)); w[0] = v.x; w[1] = v.y; }
+  else if constexpr (NB == 32) w[0] = __ldg(reinterpret_cast<const unsigned int*>(p));
+  else w[0] = (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(p)) << 16;
+}
+// shifts the gate bit of v (a ReLU output, so v >= 0 or -0) in at the bottom of w: w = (w << 1) | (v > 0).  0 - v is negative exactly
+// when v > 0 (0 - (-0) = +0), so the bit is its sign: one FADD and one funnel shift per bit.
+__device__ __forceinline__ uint32_t push_gate(uint32_t w, float v) { return __funnelshift_l(__float_as_uint(0.f - v), w, 1); }
 
 __device__ __forceinline__ void row_geometry_tc(const nnb_render_args& a, size_t m, size_t M, Ray& ray, float& z, float p[3]) {
   const size_t mm = m < M ? m : M - 1;
@@ -116,7 +139,8 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
-                                              SampleRec* __restrict__ recs, TcStash st, size_t M, int n_tiles, int stash) {
+                                              SampleRec* __restrict__ recs, const __grid_constant__ TcStash st, size_t M, int n_tiles,
+                                              int stash) {
   using T = Tc<D>;
   constexpr int SM_AHI = T::SM_AHI, SM_ALO = T::SM_ALO, SM_EHI = T::SM_EHI, SM_ELO = T::SM_ELO, SM_W = T::SM_W, SM_BIAS = T::SM_BIAS;
   constexpr int SM_RAYB = T::SM_RAYB, SM_BAR = T::SM_BAR, BIAS_FLOATS = T::BIAS_FLOATS, RAYB_FLOATS = T::RAYB_FLOATS;
@@ -278,6 +302,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
       if (g < 9) {
         const float* bias = (g < 8) ? s_bias + g * D : s_bias + B_FEAT0;
         float* sp = stash ? (g < 8 ? st.h[g] : st.feat) : nullptr;
+        uint32_t gw[D / 64] = {};   // ReLU gate bits of this thread's fragment, shifted in in the order b = 4j + 2r + e
 #pragma unroll
         for (int j = 0; j < D / 8; ++j) {
           const int col = j * 8 + c0;
@@ -294,13 +319,16 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
             *reinterpret_cast<uint32_t*>(smem + SM_ALO + off) = lw;
             if (g == 7) s_logit[r] = fmaf(v1, s_bias[W_SIG0 + col + 1], fmaf(v0, s_bias[W_SIG0 + col], s_logit[r]));
             if (sp) __stcs(reinterpret_cast<float2*>(sp + (mt + row) * D + col), make_float2(v0, v1));
+            gw[j / 8] = push_gate(push_gate(gw[j / 8], v0), v1);
           }
         }
+        if (stash && g < 8) store_gates<D / 2>(st.gates + gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
         fence_async_smem();
         wg_sync();   // the whole A operand (and, after layer 0, the per-ray bias) is written before the next layer's MMAs
       } else {
         // rgb hidden layer (D/2 columns) -> colour head + per-sample record
         float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+        uint32_t gw[D / 128 > 0 ? D / 128 : 1] = {};
         const int off0 = ray_off();
 #pragma unroll
         for (int j = 0; j < DR / 8; ++j) {
@@ -314,8 +342,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
             for (int c = 0; c < 3; ++c)
               c_acc[r][c] = fmaf(v1, s_bias[W_RGB0 + c * DR + col + 1], fmaf(v0, s_bias[W_RGB0 + c * DR + col], c_acc[r][c]));
             if (stash) __stcs(reinterpret_cast<float2*>(st.hr + (mt + row) * DR + col), make_float2(v0, v1));
+            gw[j / 8] = push_gate(push_gate(gw[j / 8], v0), v1);
           }
         }
+        if (stash) store_gates<D / 4>(st.gates + gate_bits_off(8, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const float sl = quad_sum(s_logit[r]);
@@ -485,9 +515,10 @@ cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw,
 // Per 128-sample tile, two consumer warpgroups (64 rows each) and a producer warpgroup streaming TRANSPOSED weight stages: stage =
 // `nrows` input features n x 16 output features k of one layer, element (n, k) = W[k * ldw + coloff + n], bf16 hi | lo (gradients
 // span five decades).  A operand = the output gradient g_y of the current layer (bf16 hi | lo, K-major, rewritten in place by each
-// epilogue); the epilogue applies the ReLU gate of the layer below (its fp32 stash > 0) and writes that layer's dY stash for the
-// weight-gradient pass.  Order (matches the stage table): g_de = g_yr W_rgbh[:, 256:283] (N = 32), g_feat = g_yr W_rgbh[:, :256],
-// g_h7 = g_feat W_feat + g_s w_sigma, then layers 7..1 (layer 4 first adds its encoding slice, N = 64) and layer 0 (encoding, N = 64).
+// epilogue); the epilogue applies the ReLU gate of the layer below (its gate bits from the forward, h > 0) and writes that layer's dY
+// stash for the weight-gradient pass.  Order (matches the stage table): g_de = g_yr W_rgbh[:, 256:283] (N = 32),
+// g_feat = g_yr W_rgbh[:, :256], g_h7 = g_feat W_feat + g_s w_sigma, then layers 7..1 (layer 4 first adds its encoding slice, N = 64)
+// and layer 0 (encoding, N = 64).
 template <int D>
 __global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __restrict__ img) {
   const StageDescT sd = stage_t<D>(blockIdx.x);
@@ -507,7 +538,7 @@ __global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __
 
 struct DgPtrs {
   const SampleRec* rec; const float4* gs; float4* gp; float4* gv; float4* dyc;
-  const float* h[8]; const float* hr; float* dy[8]; float* dfeat; float* dyr;
+  const unsigned char* gates; float* dy[8]; float* dfeat; float* dyr;
 };
 
 // K-steps of one GEMM: D[64 x N] = A[64 x 16 ksteps] B^T, weight stages from the ring (released as their MMAs complete)
@@ -544,7 +575,8 @@ __device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint
 }
 
 template <int D>
-__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, const unsigned char* __restrict__ wimg, DgPtrs P, size_t M,
+__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                         const __grid_constant__ DgPtrs P, size_t M,
                                                          int n_tiles, int write_dy) {
   using T = Tc<D>;
   constexpr int DG_AHI = T::DG_AHI, DG_ALO = T::DG_ALO, DG_W = T::DG_W, DG_GENC = T::DG_GENC, DG_SMALL = T::DG_SMALL, DG_GYC = T::DG_GYC;
@@ -587,8 +619,12 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
   auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
   uint32_t slot = 0, phase = 0;
   float acc[D / 2];   // the 32- / 64-wide GEMMs use its first registers (every result is consumed before the next GEMM)
-  // epilogue of a D-wide layer: x (+ g_s w_sigma) -> ReLU gate of `hmask` -> dY stash -> next A operand (in place)
-  auto epiD = [&](size_t mt, const float* hmask, float* dst, bool add_sigma) {
+  // ReLU gate bits of the layer below the next epilogue (the rgb hidden layer's for the head prologue), loaded before the GEMM that
+  // precedes that epilogue so the load completes behind its MMAs
+  uint32_t gm[D / 64];
+  const size_t Mpad = (size_t)n_tiles * TILE;
+  // epilogue of a D-wide layer: x (+ g_s w_sigma) -> ReLU gate gm (when `gated`) -> dY stash -> next A operand (in place)
+  auto epiD = [&](size_t mt, bool gated, float* dst, bool add_sigma) {
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int row = r0 + 8 * r;
@@ -599,9 +635,9 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
       for (int j = 0; j < D / 8; ++j) {
         float v0 = acc[4 * j + 2 * r], v1 = acc[4 * j + 2 * r + 1];
         if (add_sigma) { v0 += g_s * s_small[3 * DR + j * 8 + c0]; v1 += g_s * s_small[3 * DR + j * 8 + c0 + 1]; }
-        if (hmask) {
-          const float2 h = __ldg(reinterpret_cast<const float2*>(hmask + rowoff + j * 8));
-          v0 = h.x > 0.f ? v0 : 0.f; v1 = h.y > 0.f ? v1 : 0.f;
+        if (gated) {
+          const uint32_t b = gm[j / 8] << (4 * (j & 7) + 2 * r);   // gate bits of columns c0 and c0 + 1 at bits 31 and 30
+          v0 = (b & 0x80000000u) ? v0 : 0.f; v1 = (b & 0x40000000u) ? v1 : 0.f;
         }
         if (dst) __stcs(reinterpret_cast<float2*>(dst + rowoff + j * 8), make_float2(v0, v1));
         uint32_t hw, lw;
@@ -627,6 +663,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
   for (int t = 0; t < my_tiles; ++t) {
     const int tile = blockIdx.x + t * gridDim.x;
     const size_t mt = (size_t)tile * TILE;
+    load_gates<D / 4>(P.gates + gate_bits_off(8, tile, threadIdx.x, Mpad, D), gm);
     wg_sync();   // the previous tile's encoding adjoint is done with genc
     if (tl < 64) {   // head adjoints (one thread per row)
       const size_t m = mt + wg * 64 + tl;
@@ -638,27 +675,25 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
       gyc[tl * 4] = g0; gyc[tl * 4 + 1] = g1; gyc[tl * 4 + 2] = g2; gyc[tl * 4 + 3] = g3;
     }
     wg_sync();
-    {   // g_yr = (g_yc W_rgb) * (hr > 0): thread = row x D/4 columns -> A operand (K = D/2) + dY stash
-      const int rl = tl & 63, half = tl >> 6, row = wg * 64 + rl;
-      const size_t m = mt + row;
-      const float* g4 = gyc + rl * 4;
+    {   // g_yr = (g_yc W_rgb) * (hr > 0), in the accumulator-fragment mapping of the gate bits -> A operand (K = D/2) + dY stash
 #pragma unroll
-      for (int oc = 0; oc < D / 32; ++oc) {
-        const int j0 = half * (D / 4) + oc * 8;
-        const float4 ha = __ldg(reinterpret_cast<const float4*>(P.hr + m * DR + j0));
-        const float4 hb = __ldg(reinterpret_cast<const float4*>(P.hr + m * DR + j0 + 4));
-        const float hv[8] = {ha.x, ha.y, ha.z, ha.w, hb.x, hb.y, hb.z, hb.w};
-        float v[8];
+      for (int r = 0; r < 2; ++r) {
+        const int row = r0 + 8 * r;
+        const float* g4 = gyc + (row - wg * 64) * 4;
+        unsigned char* ahi = smem + DG_AHI + row * 16 + c0 * 2;
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float x = g4[0] * s_small[j0 + q] + g4[1] * s_small[DR + j0 + q] + g4[2] * s_small[2 * DR + j0 + q];
-          v[q] = hv[q] > 0.f ? x : 0.f;
+        for (int j = 0; j < DR / 8; ++j) {
+          const int col = j * 8 + c0;
+          const float x0 = g4[0] * s_small[col] + g4[1] * s_small[DR + col] + g4[2] * s_small[2 * DR + col];
+          const float x1 = g4[0] * s_small[col + 1] + g4[1] * s_small[DR + col + 1] + g4[2] * s_small[2 * DR + col + 1];
+          const uint32_t b = gm[j / 8] << (4 * (j & 7) + 2 * r);
+          const float v0 = (b & 0x80000000u) ? x0 : 0.f, v1 = (b & 0x40000000u) ? x1 : 0.f;
+          if (write_dy) *reinterpret_cast<float2*>(P.dyr + (mt + row) * DR + col) = make_float2(v0, v1);
+          uint32_t hw, lw;
+          split2_bf16(v0, v1, hw, lw);
+          *reinterpret_cast<uint32_t*>(ahi + j * 2048) = hw;
+          *reinterpret_cast<uint32_t*>(ahi + DG_ALO + j * 2048) = lw;
         }
-        if (write_dy) {
-          *reinterpret_cast<float4*>(P.dyr + m * DR + j0) = make_float4(v[0], v[1], v[2], v[3]);
-          *reinterpret_cast<float4*>(P.dyr + m * DR + j0 + 4) = make_float4(v[4], v[5], v[6], v[7]);
-        }
-        split_store8_bf16(v, smem + DG_AHI + (j0 >> 3) * 2048 + row * 16, smem + DG_ALO + (j0 >> 3) * 2048 + row * 16);
       }
     }
     fence_async_smem();
@@ -688,13 +723,15 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
       P.gv[m] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
     }
     dg_gemm<D, D>(acc, a_hi, a_lo, D / 32, w_base, bar0, slot, phase, tl);   // g_feat
-    epiD(mt, nullptr, write_dy ? P.dfeat : nullptr, false);
+    epiD(mt, false, write_dy ? P.dfeat : nullptr, false);
+    load_gates<D / 2>(P.gates + gate_bits_off(7, tile, threadIdx.x, Mpad, D), gm);
     dg_gemm<D, D>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);       // g_h7 = g_feat W_feat + g_s w_sigma
-    epiD(mt, P.h[7], write_dy ? P.dy[7] : nullptr, true);
+    epiD(mt, true, write_dy ? P.dy[7] : nullptr, true);
     for (int l = 7; l >= 1; --l) {
+      load_gates<D / 2>(P.gates + gate_bits_off(l - 1, tile, threadIdx.x, Mpad, D), gm);
       if (l == 4) { dg_gemm<D, 64>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl); epi_enc(false); }
       dg_gemm<D, D>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);     // g_h(l-1) = dY_l W_l
-      epiD(mt, P.h[l - 1], write_dy ? P.dy[l - 1] : nullptr, false);
+      epiD(mt, true, write_dy ? P.dy[l - 1] : nullptr, false);
     }
     dg_gemm<D, 64>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);      // encoding gradient of layer 0
     epi_enc(true);
@@ -762,8 +799,8 @@ cudaError_t tc_dgrad_launch_dim(const nnb_render_bwd_args& b, const WsLayout& L,
   P.rec = reinterpret_cast<const SampleRec*>(base + L.rec);
   P.gs = reinterpret_cast<const float4*>(base + L.gs); P.gp = reinterpret_cast<float4*>(base + L.gp); P.gv = reinterpret_cast<float4*>(base + L.gv);
   P.dyc = reinterpret_cast<float4*>(base + L.dyc);
-  for (int l = 0; l < 8; ++l) { P.h[l] = F(L.h[l]); P.dy[l] = F(L.dy[l]); }
-  P.hr = F(L.hr); P.dfeat = F(L.dfeat); P.dyr = F(L.dyr);
+  for (int l = 0; l < 8; ++l) P.dy[l] = F(L.dy[l]);
+  P.gates = reinterpret_cast<const unsigned char*>(base + L.gates); P.dfeat = F(L.dfeat); P.dyr = F(L.dyr);
   tc_prep_weights_t<D><<<T::N_STAGES_T, 256, 0, st>>>(a.weights, img);
   const int n_tiles = (int)((L.M + TILE - 1) / TILE);
   const int grid = n_tiles < n_sm ? n_tiles : n_sm;
@@ -828,6 +865,7 @@ cudaError_t tc_render_fwd_dim(const nnb_render_args& a, const WsLayout& L, cudaS
     for (int l = 0; l < 8; ++l) ts.h[l] = reinterpret_cast<float*>(base + L.h[l]);
     ts.feat = reinterpret_cast<float*>(base + L.feat); ts.hr = reinterpret_cast<float*>(base + L.hr);
     ts.enc = reinterpret_cast<float*>(base + L.enc); ts.denc = reinterpret_cast<float*>(base + L.denc);
+    ts.gates = reinterpret_cast<unsigned char*>(base + L.gates);
   }
   nnb_prof_mark(st);
   tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);   // 152 stage images (fp16 hi | lo) at D = 256

@@ -16,6 +16,8 @@ struct WsLayout {
   // SIMT engine activation stash (fp32, [sample][feature]; D features per trunk layer, D / 2 of the rgb hidden layer)
   size_t h[8], feat, hr, enc, denc;
   size_t dy[8], dfeat, dyr, dyc;
+  // TC engine: ReLU gate bits (h > 0) of h0..h7 and the rgb hidden layer, written by tc_field_fwd, read by tc_dgrad (see gate_bits_off)
+  size_t gates;
   // operand-plane backward (NNB_TCBWD; rejected by the sm_90a library): activations / output-gradients as per-tile bf16 hi|lo
   // operand planes ([tile][hi|lo][sample half][feature/8][64 samples][8 features]) + ReLU bitmasks
   size_t n_tiles;
@@ -57,6 +59,18 @@ inline size_t wpart_floats(size_t M, int D) {
 struct RedJob { float* dW; float* db; int Nn, Kk, ldw, nsplit, dbslots; size_t off, stride; };
 cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st);
 
+// ReLU gate bits of the TC engine, in the order of the wgmma accumulator fragment, so that each consumer thread (0..255) of a
+// 128-sample tile writes its bits with one vector store in tc_field_fwd and reads them with one vector load in tc_dgrad.
+// Region `gates`: [layer 0..8][tile][thread][D/2 bits of a trunk layer (layers 0..7 = h0..h7) | D/4 bits of the rgb hidden layer
+// (layer 8)].  Thread t (warp w = t / 32, lane) holds tile rows r0 = 64 (w / 4) + 16 (w % 4) + lane / 4 and r0 + 8, columns
+// 8j + c0 + {0, 1} with c0 = 2 (lane % 4); its bit b = 4j + 2r + e is (h[row r0 + 8r][column 8j + c0 + e] > 0), stored most significant
+// first: bit W - 1 - b % W of its little-endian W-bit word b / W, W = 32 (W = 16 for the 16 bits of the rgb hidden layer at D = 64).
+__host__ __device__ inline size_t gate_bits_bytes(size_t Mpad, int D) { return Mpad * (size_t)D + Mpad * (size_t)D / 16; }
+__host__ __device__ inline size_t gate_bits_off(int layer, size_t tile, int thread, size_t Mpad, int D) {
+  return layer < 8 ? ((size_t)layer * (Mpad / 128) + tile) * (16 * (size_t)D) + (size_t)thread * (D / 16)
+                   : Mpad * (size_t)D + tile * (8 * (size_t)D) + (size_t)thread * (D / 32);
+}
+
 inline WsLayout make_layout(int N, int S, uint32_t flags, int engine, int D = 256) {
   WsLayout L{};
   L.D = D;
@@ -87,6 +101,7 @@ inline WsLayout make_layout(int N, int S, uint32_t flags, int engine, int D = 25
       L.enc = take(L.Mpad * 64 * 4); L.denc = take(L.Mpad * 32 * 4);
       for (int l = 0; l < 8; ++l) L.dy[l] = take(L.Mpad * d * 4);
       L.dfeat = take(L.Mpad * d * 4); L.dyr = take(L.Mpad * dr * 4); L.dyc = take(L.Mpad * 16);
+      if (engine == NNB_ENGINE_TC) L.gates = take(gate_bits_bytes(L.Mpad, D));
     }
   }
   L.total = o;
