@@ -367,68 +367,135 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
 }
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
-// CTA = one 128-row slice of dW (two warpgroups x 64 rows, all KN columns in registers) over a contiguous share of the samples.
-// Per 64-sample block every thread converts its share of dY^T / X^T to bf16 hi | lo K-major operands in shared memory (double
-// buffered: the conversion of block c overlaps the MMAs of block c - 1), then each warpgroup issues 4 K-steps x three MMAs
-// (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi).  Each sample split stores its partial dW (and two bias partials per row, one per thread
-// half) to the split buffer; wgrad_reduce adds the splits to the gradient in a fixed order, so the result is the same every run.
+// CTA = one 128-row slice of dW (all KN columns) over a contiguous share of the samples, warp-specialized in 32-sample chunks:
+//   warpgroup 2 (converter): one thread streams each chunk's fp32 rows into a staging ring with cp.async.bulk, completion on an
+//     mbarrier tx-count: two copies per chunk, 32 contiguous rows of X and of dY (whole rows: the row slices of a job read the same
+//     dY and X rows, and the second read of each comes from L2; 1D copies need no tensor map).  All 128 threads
+//     then convert the staged chunk to bf16 hi | lo K-major operands dY^T / X^T (zeroing samples >= s_end, rows >= Nn, columns >= Kk,
+//     and summing the bias partials), publish them to the MMA warpgroups through an mbarrier and refill the staging slot.
+//   warpgroups 0, 1 (MMA): 64 rows of dW each, 128 fp32 accumulators in registers; per chunk 2 K-steps x three MMAs
+//     (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi), an operand buffer released once wgmma.wait_group shows its MMAs complete.
+// A split covers whole 64-sample blocks (two chunks each; samples past s_end are zeros), so every output element sees the same MMA
+// sequence for any chunking.  Bias slot h of a row sums samples 32h .. 32h + 31 of each 64-sample block in sample order.  Each split
+// stores its partial dW and bias slots to the split buffer; wgrad_reduce adds the splits in a fixed order, so the result is the same
+// every run.
 struct WgJobT { const float* dY; const float* X; float* dW; float* db; int ldy, Nn, ldx, Kk, ldw, cta0; size_t part_off; };
-constexpr int MAX_WG_JOBS = 10, WG_CHUNK = 64;
+constexpr int MAX_WG_JOBS = 10, WG_BLOCK = 64;
 struct WgJobsT { WgJobT j[MAX_WG_JOBS]; int njobs, msplit, per_cta; };
-template <int KN> constexpr int wg_smem() { return 2 * (2 * 128 * 128 + 2 * KN * 128); }
+constexpr int WG_MAX_LDY = 256;
+template <int KN> struct Wg {   // shared-memory map (bytes) of tc_wgrad<KN>; X rows are KN floats (ldx == KN)
+  static constexpr int CH = 32, NOP = 2;                                   // samples per chunk, operand buffers
+  static constexpr int SY = CH * WG_MAX_LDY * 4, STG = SY + CH * KN * 4;   // fp32 staging: dY [CH][ldy] | X [CH][KN]
+  static constexpr int A_BYTES = 128 * CH * 2, B_BYTES = KN * CH * 2; // one bf16 plane of dY^T / X^T
+  static constexpr int OPB = 2 * A_BYTES + 2 * B_BYTES;
+  static constexpr int NSTG = (232448 - 128 - NOP * OPB) / STG;      // staging ring: all the rest of shared memory (loads in flight)
+  static constexpr int SM_OP = NSTG * STG, SM_BAR = SM_OP + NOP * OPB;
+  static constexpr int SMEM = SM_BAR + (NSTG + 2 * NOP) * 8;
+  static_assert(NSTG >= 2 && SMEM <= 232448, "shared memory budget");
+};
 
 template <int KN>   // 256 | 128 | 64: columns of dW (features of X) held by one CTA
-__global__ void __launch_bounds__(256, 1) tc_wgrad(WgJobsT J, size_t M, float* __restrict__ part) {
+__global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJobsT J, size_t M, float* __restrict__ part) {
+  using W = Wg<KN>;
+  constexpr int CH = W::CH, NSTG = W::NSTG, NOP = W::NOP, A_BYTES = W::A_BYTES, B_BYTES = W::B_BYTES;
   extern __shared__ __align__(1024) unsigned char smem[];
-  constexpr int A_BYTES = 128 * 128, B_BYTES = KN * 128, BUF = 2 * A_BYTES + 2 * B_BYTES;
   int ji = 0;
   while (ji + 1 < J.njobs && (int)blockIdx.x >= J.j[ji + 1].cta0) ++ji;
-  const WgJobT jb = J.j[ji];
+  const WgJobT& jb = J.j[ji];
   const int local = blockIdx.x - jb.cta0, n0 = (local / J.msplit) * 128;
   const size_t s_begin = (size_t)(local % J.msplit) * J.per_cta;
   const size_t s_end = (s_begin + J.per_cta < M) ? s_begin + J.per_cta : M;   // an empty split stores zeros
-  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  const int nch = s_begin < s_end ? (int)((s_end - s_begin + WG_BLOCK - 1) / WG_BLOCK) * (WG_BLOCK / CH) : 0;
+  float* pp = part + jb.part_off + (size_t)(local % J.msplit) * ((size_t)jb.Nn * jb.Kk + 2 * jb.Nn);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t bar0 = smem_u32(smem + W::SM_BAR);
+  auto SFULL = [&](int i) { return bar0 + 8u * i; };                    // staging slot filled (tx-count)
+  auto OPFULL = [&](int i) { return bar0 + 8u * (NSTG + i); };          // operand buffer written by the converter
+  auto OPEMPTY = [&](int i) { return bar0 + 8u * (NSTG + NOP + i); };   // operand buffer read by both MMA warpgroups
+  if (tid == 0) {
+    for (int i = 0; i < NSTG; ++i) mbar_init(SFULL(i), 1);
+    for (int i = 0; i < NOP; ++i) { mbar_init(OPFULL(i), 1); mbar_init(OPEMPTY(i), 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // =============================== converter warpgroup ===============================
+    // 104 + 2 x 200 = 3 x 168 registers per thread: the MMA warpgroups get what the converter gives up
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 104;" ::: "memory");
+    const int ct = tid - 256;
+    const int ny = jb.Nn - n0 < 128 ? jb.Nn - n0 : 128;   // dY columns of this row slice
+    auto issue = [&](int c) {   // thread 0 of the warpgroup: chunk c -> staging slot c % NSTG (a chunk past s_end copies nothing)
+      const int sl = c % NSTG;
+      const size_t s0 = s_begin + (size_t)c * CH;
+      if (s0 < s_end) {   // then rows s0 .. s0 + 31 < Mpad: in bounds of the stash
+        mbar_expect_tx(SFULL(sl), (uint32_t)(CH * (jb.ldy + KN) * 4));
+        bulk_g2s(smem_u32(smem + sl * W::STG), jb.dY + s0 * jb.ldy, (uint32_t)(CH * jb.ldy * 4), SFULL(sl));
+        bulk_g2s(smem_u32(smem + sl * W::STG + W::SY), jb.X + s0 * KN, CH * KN * 4, SFULL(sl));
+      } else {
+        mbar_arrive(SFULL(sl));
+      }
+    };
+    if (ct == 0)
+      for (int c = 0; c < NSTG && c < nch; ++c) issue(c);
+    float db0 = 0.f, db1 = 0.f;   // bias slots 0 and 1
+    for (int c = 0; c < nch; ++c) {
+      const int sl = c % NSTG, ob = c % NOP;
+      const size_t s0 = s_begin + (size_t)c * CH;
+      const int nvalid = s0 < s_end ? (s_end - s0 < (size_t)CH ? (int)(s_end - s0) : CH) : 0;
+      const float* sy = reinterpret_cast<const float*>(smem + sl * W::STG);
+      const float* sx = reinterpret_cast<const float*>(smem + sl * W::STG + W::SY);
+      unsigned char* op = smem + W::SM_OP + ob * W::OPB;
+      mbar_wait(SFULL(sl), (uint32_t)(c / NSTG) & 1u);
+      mbar_wait(OPEMPTY(ob), ((uint32_t)(c / NOP) & 1u) ^ 1u);
+      const bool half1 = (c * CH) & 32;   // the chunk lies in the second half of its 64-sample block: bias slot 1
+      {   // A = dY^T: thread = row n, CH / 8 8-sample octets
+        const bool nv = ct < ny;
+        float db = half1 ? db1 : db0;
+#pragma unroll
+        for (int so = 0; so < CH / 8; ++so) {
+          float v[8];
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            v[q] = (nv && so * 8 + q < nvalid) ? sy[(so * 8 + q) * jb.ldy + n0 + ct] : 0.f;
+            db += v[q];
+          }
+          split_store8_bf16(v, op + so * 2048 + ct * 16, op + A_BYTES + so * 2048 + ct * 16);
+        }
+        if (half1) db1 = db; else db0 = db;
+      }
+#pragma unroll 4
+      for (int i = 0; i < KN * (CH / 8) / 128; ++i) {   // B = X^T: row k (KN), reduction index = sample
+        const int item = ct + i * 128, k = item % KN, so = item / KN;
+        float v[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) v[q] = (k < jb.Kk && so * 8 + q < nvalid) ? sx[(so * 8 + q) * KN + k] : 0.f;
+        split_store8_bf16(v, op + 2 * A_BYTES + so * KN * 16 + k * 16, op + 2 * A_BYTES + B_BYTES + so * KN * 16 + k * 16);
+      }
+      fence_async_smem();
+      asm volatile("bar.sync 1, 128;" ::: "memory");   // the operands are written and the staging slot is read
+      if (ct == 0) mbar_arrive(OPFULL(ob));
+      if (ct == 0 && c + NSTG < nch) issue(c + NSTG);
+    }
+    if (ct < ny) {
+      pp[(size_t)jb.Nn * jb.Kk + n0 + ct] = db0;
+      pp[(size_t)jb.Nn * jb.Kk + jb.Nn + n0 + ct] = db1;
+    }
+    return;
+  }
+  // =============================== MMA warpgroups ===============================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 200;" ::: "memory");
+  const int wg = warp >> 2;
   float acc[KN / 2];
 #pragma unroll
   for (int i = 0; i < KN / 2; ++i) acc[i] = 0.f;
-  float dbsum = 0.f;
-  int c = 0;
-  for (size_t s0 = s_begin; s0 < s_end; s0 += WG_CHUNK, ++c) {
-    unsigned char* buf = smem + (c & 1) * BUF;
-    __syncthreads();   // both warpgroups' MMAs of block c - 2 (the last readers of buf) have completed
-    {   // A = dY^T: row n (128), reduction index = sample; thread = one row x four 8-sample groups
-      const int n = tid & 127;
-      const bool nv = n0 + n < jb.Nn;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int so = (tid >> 7) * 4 + i;
-        float v[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const size_t s = s0 + so * 8 + q;
-          v[q] = (nv && s < s_end) ? __ldg(jb.dY + s * jb.ldy + n0 + n) : 0.f;
-          dbsum += v[q];
-        }
-        split_store8_bf16(v, buf + so * 2048 + n * 16, buf + A_BYTES + so * 2048 + n * 16);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < KN * 8 / 256; ++i) {   // B = X^T: row k (KN), reduction index = sample
-      const int item = tid + i * 256, k = item % KN, so = item / KN;
-      float v[8];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const size_t s = s0 + so * 8 + q;
-        v[q] = (k < jb.Kk && s < s_end) ? __ldg(jb.X + s * jb.ldx + k) : 0.f;
-      }
-      split_store8_bf16(v, buf + 2 * A_BYTES + so * KN * 16 + k * 16, buf + 2 * A_BYTES + B_BYTES + so * KN * 16 + k * 16);
-    }
-    fence_async_smem();
-    __syncthreads();
-    const uint32_t a = smem_u32(buf) + wg * 1024, b = smem_u32(buf + 2 * A_BYTES);
+  for (int c = 0; c < nch; ++c) {
+    const int ob = c % NOP;
+    const uint32_t a = smem_u32(smem + W::SM_OP + ob * W::OPB) + wg * 1024, b = smem_u32(smem + W::SM_OP + ob * W::OPB + 2 * A_BYTES);
+    mbar_wait(OPFULL(ob), (uint32_t)(c / NOP) & 1u);
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
+    for (int ks = 0; ks < CH / 16; ++ks) {
       const uint64_t dah = gdesc(a + ks * 4096, 2048, 128), dal = gdesc(a + A_BYTES + ks * 4096, 2048, 128);
       const uint64_t dbh = gdesc(b + ks * 2 * KN * 16, KN * 16, 128), dbl = gdesc(b + B_BYTES + ks * 2 * KN * 16, KN * 16, 128);
       wgmma_bf16<KN>(acc, dal, dbh, (c > 0 || ks > 0) ? 1u : 0u);
@@ -436,10 +503,12 @@ __global__ void __launch_bounds__(256, 1) tc_wgrad(WgJobsT J, size_t M, float* _
       wgmma_bf16<KN>(acc, dah, dbh, 1u);
     }
     wgmma_commit();
-    wgmma_wait<1>();
+    if (c > 0) {   // the previous chunk's MMAs have completed: release its operand buffer
+      wgmma_wait<1>();
+      if ((tid & 127) == 0) mbar_arrive(OPEMPTY((c - 1) % NOP));
+    }
   }
   wgmma_wait<0>();
-  float* pp = part + jb.part_off + (size_t)(local % J.msplit) * ((size_t)jb.Nn * jb.Kk + 2 * jb.Nn);
   const int r0 = n0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
 #pragma unroll
   for (int j = 0; j < KN / 8; ++j)
@@ -452,14 +521,13 @@ __global__ void __launch_bounds__(256, 1) tc_wgrad(WgJobsT J, size_t M, float* _
         if (n < jb.Nn && k < jb.Kk) pp[(size_t)n * jb.Kk + k] = acc[4 * j + 2 * r + e];
       }
     }
-  if (n0 + (tid & 127) < jb.Nn) pp[(size_t)jb.Nn * jb.Kk + (tid >> 7) * jb.Nn + n0 + (tid & 127)] = dbsum;
 }
 
 template <int KN>
 cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msplit, float* part, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem<KN>());
+    cudaError_t e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -468,6 +536,8 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
   int ctas = 0;
   size_t off = 0;
   for (int i = 0; i < njobs; ++i) {
+    // X and dY chunks are staged as whole rows (16-byte multiples)
+    if (jobs[i].ldx != KN || jobs[i].ldy > WG_MAX_LDY || jobs[i].ldy % 4) return cudaErrorInvalidValue;
     J.j[i] = jobs[i]; J.j[i].cta0 = ctas; ctas += (jobs[i].Nn + 127) / 128 * msplit;
     const size_t stride = (size_t)jobs[i].Nn * jobs[i].Kk + 2 * jobs[i].Nn;
     J.j[i].part_off = off;
@@ -476,8 +546,8 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
   }
   if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
   J.njobs = njobs; J.msplit = msplit;
-  J.per_cta = (int)(((M + msplit - 1) / msplit + WG_CHUNK - 1) / WG_CHUNK * WG_CHUNK);
-  tc_wgrad<KN><<<ctas, 256, wg_smem<KN>(), st>>>(J, M, part);
+  J.per_cta = (int)(((M + msplit - 1) / msplit + WG_BLOCK - 1) / WG_BLOCK * WG_BLOCK);
+  tc_wgrad<KN><<<ctas, 384, Wg<KN>::SMEM, st>>>(J, M, part);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, njobs, part, st);

@@ -1,0 +1,67 @@
+#!/usr/bin/env python
+"""Per-kernel cost of the weight-gradient stage in the eager C2 train step (1024 rays x 128 samples, D = 256): torch.profiler with CUDA
+activities over PK steps, device time per step of tc_wgrad<KN>, simt_wgrad and wgrad_reduce, and for tc_wgrad the achieved bytes/s
+and tensor FLOP/s from the job shapes.  bench.py and tools/step_time.py time the whole stage as one interval.  NNB_LIB_PATH selects a
+library variant (alternate the runs of two builds to compare them).   python tools/wgrad_cost.py [tag]"""
+import json, os, re, subprocess, sys
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
+import torch
+import bench
+from nope_nerf_b200 import _lib as L
+
+PK = 10
+
+
+def tc_shapes(M, D):
+    """per tc_wgrad launch of tc_wgrad_all: (bytes of dY and X if each is read once, bytes as issued (every 128-row slice of a job reads
+    its X), tensor FLOP: three bf16 MMAs per logical multiply-add)"""
+    launches = {"tc_wgrad<%d>" % D: ([D] * 8 + [D // 2], D, D, False),   # dY widths (layers 1..7, fc_feature, rgb_layers.0), X width, Kk
+                "tc_wgrad<64>": ([D, D], 64, 63, True)}                  # layers 0 and 4: one shared X (the encoding stash)
+    out = {}
+    for name, (nns, ldx, kk, shared_x) in launches.items():
+        once = sum(M * nn * 4 for nn in nns) + M * ldx * 4 * (1 if shared_x else len(nns))
+        issued = sum(M * (nn + (nn + 127) // 128 * ldx) * 4 for nn in nns)
+        out[name] = (once, issued, sum(3 * 2 * M * nn * kk for nn in nns))
+    return out
+
+
+def main():
+    dev = torch.device("cuda", 0); torch.cuda.set_device(0)
+    tr = bench.build_trainer(bench.make_cfg(bench.NRAYS), dev, bench.V)
+    _, frames = bench.synth_frames(bench.H, bench.W, bench.HD, bench.WD, 4, bench.V, dev, with_ref=False)
+    step = lambda i: tr.train_step(frames[i % 4], it=i, epoch=0, scheduling_start=10000, render_path=None)
+    tr.use_cuda_graph = False
+    for i in range(5): step(i)
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for i in range(PK): step(i)
+        torch.cuda.synchronize()
+    pat = re.compile(r"(tc_wgrad<\d+>|simt_wgrad|wgrad_reduce)")
+    agg = {}
+    for ev in prof.key_averages():
+        m = pat.search(ev.key)
+        if not m:
+            continue
+        t = getattr(ev, "device_time_total", None)
+        if t is None: t = ev.cuda_time_total
+        a = agg.setdefault(m.group(1), [0.0, 0])
+        a[0] += t; a[1] += ev.count
+    M, D = bench.NRAYS * bench.S, 256
+    shapes = tc_shapes(M, D)
+    kernels = {}
+    for name, (us, n) in sorted(agg.items()):
+        ms = us / 1e3 / PK
+        k = {"ms_per_step": round(ms, 4), "launches_per_step": n / PK}
+        if name in shapes:
+            once, issued, flop = shapes[name]
+            k.update(gb_read_once=round(once / 1e9, 3), gb_issued=round(issued / 1e9, 3), tb_per_s_once=round(once / ms / 1e9, 3),
+                     tensor_tflop=round(flop / 1e12, 4), tensor_tflop_per_s=round(flop / ms / 1e9, 1))
+        kernels[name] = k
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"tag": sys.argv[1] if len(sys.argv) > 1 else "", "lib": os.path.basename(L.LIB_PATH), "gpu": q.splitlines()[0] if q else "",
+                      "steps": PK, "wgrad_ms_per_step": round(sum(v["ms_per_step"] for v in kernels.values()), 4), "kernels": kernels}))
+
+
+if __name__ == "__main__":
+    main()
