@@ -500,6 +500,7 @@ __global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int mspl
     }
     if (tk == 0 && ki == 0) pp[(size_t)J.Nn * J.Kk + n] = bs[r];
   }
+  if (blockIdx.x == gridDim.x - 1 && blockIdx.y == gridDim.y - 1) pdl_wait();   // chained launch: see tc_wgrad_all
 }
 
 // dW[n][k] += sum over splits (fixed order); one thread per element of all jobs
@@ -735,10 +736,10 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
   return cudaGetLastError();
 }
 
-// jobs -> simt_wgrad into the partial buffer, then wgrad_reduce into dW / db
-cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st) {
-  RedJob R[16];
-  size_t off = 0; int tiles = 0;
+// jobs -> simt_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent
+// launch behind the previous grid on the stream (see tc_wgrad_all)
+cudaError_t launch_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, size_t off, RedJob* R, bool chained, cudaStream_t st) {
+  int tiles = 0;
   for (int i = 0; i < J.njobs; ++i) {
     WJob& j = J.j[i];
     j.tiles_k = (j.Kk + 63) / 64; j.ntiles = ((j.Nn + 63) / 64) * j.tiles_k; j.tile_start = tiles; tiles += j.ntiles;
@@ -748,21 +749,35 @@ cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, c
     off += stride * msplit;
   }
   if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
-  simt_wgrad<<<dim3(tiles, msplit), 256, 0, st>>>(J, M, msplit, part);
-  cudaError_t e = cudaGetLastError();
+  cudaLaunchAttribute at{};
+  at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(tiles, msplit); cfg.blockDim = dim3(256); cfg.stream = st;
+  cfg.attrs = &at; cfg.numAttrs = chained ? 1 : 0;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, simt_wgrad, J, M, msplit, part);
+  return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+// jobs -> simt_wgrad into the partial buffer, then wgrad_reduce into dW / db
+cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st) {
+  RedJob R[16];
+  cudaError_t e = launch_simt_wgrad(J, M, D, msplit, part, 0, R, false, st);
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, J.njobs, part, st);
 }
 
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, cudaStream_t st) {
+// the small jobs of tc_wgrad_all, launched chained into part[off ..] (njobs <= 16); the caller reduces them through R
+cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st) {
+  if (njobs > 16) return cudaErrorInvalidValue;
   WJobs J{};
-  for (int i = 0; i < njobs && i < 16; ++i) {
+  for (int i = 0; i < njobs; ++i) {
     WJob& j = J.j[i];
     j.dY = jobs[i].dY; j.ldy = jobs[i].ldy; j.Nn = jobs[i].Nn; j.X = jobs[i].X; j.ldx = jobs[i].ldx; j.Kk = jobs[i].Kk;
     j.dW = jobs[i].dW; j.ldw = jobs[i].ldw; j.db = jobs[i].db;
   }
-  J.njobs = njobs < 16 ? njobs : 16;
-  return run_simt_wgrad(J, M, D, jobs_wgrad_msplit(M), part, st);
+  J.njobs = njobs;
+  return launch_simt_wgrad(J, M, D, jobs_wgrad_msplit(M), part, off, R, true, st);
 }
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st) {

@@ -26,7 +26,7 @@
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st);
 cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, cudaStream_t st);
+cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st);
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -418,6 +418,8 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  pdl_launch_dependents();   // the next grid of the stage starts only once every CTA of this one is resident (see tc_wgrad_all)
+  const bool last_cta = blockIdx.x == gridDim.x - 1;
 
   if (warp >= 8) {
     // =============================== converter warpgroup ===============================
@@ -481,6 +483,7 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
       pp[(size_t)jb.Nn * jb.Kk + n0 + ct] = db0;
       pp[(size_t)jb.Nn * jb.Kk + jb.Nn + n0 + ct] = db1;
     }
+    if (last_cta) pdl_wait();
     return;
   }
   // =============================== MMA warpgroups ===============================
@@ -521,10 +524,21 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
         if (n < jb.Nn && k < jb.Kk) pp[(size_t)n * jb.Kk + k] = acc[4 * j + 2 * r + e];
       }
     }
+  if (last_cta) pdl_wait();
 }
 
+// floats of the partial buffer that tc_wgrad uses for these jobs at msplit sample splits (two bias slots per row)
+size_t wg_part_floats(const WgJobT* jobs, int njobs, int msplit) {
+  size_t f = 0;
+  for (int i = 0; i < njobs; ++i) f += (size_t)jobs[i].Nn * jobs[i].Kk + 2 * jobs[i].Nn;
+  return f * msplit;
+}
+
+// jobs -> tc_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent
+// launch behind the previous grid on the stream (see tc_wgrad_all)
 template <int KN>
-cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msplit, float* part, cudaStream_t st) {
+cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msplit, float* part, size_t off, RedJob* R, bool chained,
+                         cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
@@ -532,9 +546,7 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
     attr = true;
   }
   WgJobsT J{};
-  RedJob R[MAX_WG_JOBS];
   int ctas = 0;
-  size_t off = 0;
   for (int i = 0; i < njobs; ++i) {
     // X and dY chunks are staged as whole rows (16-byte multiples)
     if (jobs[i].ldx != KN || jobs[i].ldy > WG_MAX_LDY || jobs[i].ldy % 4) return cudaErrorInvalidValue;
@@ -547,13 +559,25 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
   if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
   J.njobs = njobs; J.msplit = msplit;
   J.per_cta = (int)(((M + msplit - 1) / msplit + WG_BLOCK - 1) / WG_BLOCK * WG_BLOCK);
-  tc_wgrad<KN><<<ctas, 384, Wg<KN>::SMEM, st>>>(J, M, part);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return launch_wgrad_reduce(R, njobs, part, st);
+  cudaLaunchAttribute at{};
+  at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(ctas); cfg.blockDim = dim3(384); cfg.dynamicSmemBytes = Wg<KN>::SMEM; cfg.stream = st;
+  cfg.attrs = &at; cfg.numAttrs = chained ? 1 : 0;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, tc_wgrad<KN>, J, M, part);
+  return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-// the weight-gradient stage of the TC engine's backward: the MLP GEMMs on tensor cores, the small heads on the fp32 SIMT kernel
+// The weight-gradient stage of the TC engine's backward: the MLP GEMMs on tensor cores, the small heads on the fp32 SIMT kernel.
+// The D-wide jobs run as (Nn / 128) x ms_big CTAs, one per SM: 136 at D = 256, one full wave on 132 SMs and a second wave of 4 CTAs.
+// The encoding jobs (tc_wgrad<64>) and the head jobs (simt_wgrad) read only the dgrad stash, so they are launched behind it with
+// programmatic dependent launch: each grid starts once every CTA of the grid before it is resident, so they fill the SMs that the
+// second wave leaves idle.  The last CTA of each chained grid waits (griddepcontrol.wait) for the grid before it after storing its
+// partials, so the heads complete only after the encoding jobs and the D-wide jobs have; one plain-launched wgrad_reduce then adds
+// the splits of all 14 jobs.  Each job has its own region of the partial buffer, so the grids never write the same floats, and no
+// two jobs write the same dW / db element (the encoding slice of layer 4 and the direction slice of rgb_layers.0 are at column
+// offset D, enc[1] has no bias), so one reduce gives the same bits as one per grid.
 cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) {
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
@@ -565,20 +589,40 @@ cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw,
   big[nb++] = WgJobT{F(L.dyr), F(L.feat), gw + nnb::W_RGBH(D), gw + nnb::B_RGBH(D), DR, DR, D, D, D + 27, 0, 0};
   enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(D, 0), gw + nnb::b_off(D, 0), D, D, 64, 63, 63, 0, 0};
   enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(D, 4) + D, nullptr, D, D, 64, 63, D + 63, 0, 0};
-  float* part = F(L.wpart);   // reused by each launch: its reduction runs before the next launch on the same stream
-  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (17 | 4 row slices at D = 256)
-  const int ms_big = L.M >= 8 * 128 ? tc_wgrad_msplit_big(D) : 1, ms_enc = L.M >= 32 * 64 ? 32 : 1;
-  cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, st)
-                : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, st) : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, st);
-  if (e != cudaSuccess) return e;
-  e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, st);
-  if (e != cudaSuccess) return e;
   const float* dyc = F(L.dyc);
   SmallJob sm[3] = {
       {dyc + 3, F(L.h[7]), gw + nnb::W_SIG(D), gw + nnb::B_SIG(D), 4, 1, D, D, D},
       {F(L.dyr), F(L.denc), gw + nnb::W_RGBH(D) + D, nullptr, DR, DR, 32, 27, D + 27},
       {dyc, F(L.hr), gw + nnb::W_RGB(D), gw + nnb::B_RGB(D), 4, 3, DR, DR, DR}};
-  return launch_simt_wgrad_jobs(sm, 3, L.M, D, part, st);
+  float* part = F(L.wpart);
+  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (17 | 4 row slices at D = 256)
+  const int ms_big = L.M >= 8 * 128 ? tc_wgrad_msplit_big(D) : 1, ms_enc = L.M >= 32 * 64 ? 32 : 1;
+  // Partial regions: D-wide jobs, then heads, then encoding jobs.  In floats, np = num_params(D), at most 64 head splits and
+  // 32 encoding splits: at D = 256 big + heads = 4 491 264 + 270 592 <= 8 (np + 8192) = 4 832 288 <= wpart_floats, and likewise at
+  // D = 128 (2 398 464 <= 2 669 632) and D = 64 (1 216 768 <= 1 686 656).  The encoding region (1 064 960 floats at D = 256) fits
+  // as well only where wpart_floats is larger: at D = 256 when M > 36 864 (16 (np + 8192) at the C2 size), at D = 64 always, at
+  // D = 128 never.  Where it does not fit, the encoding jobs run after the chained reduce, with their own reduce, from offset 0.
+  const size_t big_f = wg_part_floats(big, nb, ms_big), head_f = small_jobs_part_floats(sm, 3, L.M);
+  const bool enc_chained = big_f + head_f + wg_part_floats(enc, 2, ms_enc) <= wpart_floats(L.M, D);
+  RedJob R[9 + 2 + 3];
+  int nr = nb;
+  cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
+                : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
+                           : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, 0, R, false, st);
+  if (e != cudaSuccess) return e;
+  if (enc_chained) {   // encoding before heads: its CTAs need a whole SM each, and the small head CTAs would fragment the free SMs
+    e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, big_f + head_f, R + nr, true, st);
+    if (e != cudaSuccess) return e;
+    nr += 2;
+  }
+  e = launch_simt_wgrad_jobs(sm, 3, L.M, D, part, big_f, R + nr, st);
+  if (e != cudaSuccess) return e;
+  nr += 3;
+  e = launch_wgrad_reduce(R, nr, part, st);
+  if (e != cudaSuccess || enc_chained) return e;
+  e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, 0, R, false, st);   // the chained reduce has read the whole buffer
+  if (e != cudaSuccess) return e;
+  return launch_wgrad_reduce(R, 2, part, st);
 }
 
 // ---- data-gradient chain (the forward's skeleton run backwards) ---------------------------------------------------------------------

@@ -43,6 +43,12 @@ __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a -
 // sample splits of the weight-gradient kernels (each split writes its own partial dW, see wgrad_reduce)
 inline int simt_wgrad_msplit(size_t M) { int m = (int)((M + 4095) / 4096); return m < 1 ? 1 : (m > 16 ? 16 : m); }
 inline int jobs_wgrad_msplit(size_t M) { int m = (int)((M + 2047) / 2048); return m < 1 ? 1 : (m > 64 ? 64 : m); }
+// floats of the partial buffer that the small SIMT jobs use (one bias slot per row, jobs_wgrad_msplit splits)
+inline size_t small_jobs_part_floats(const SmallJob* jobs, int njobs, size_t M) {
+  size_t f = 0;
+  for (int i = 0; i < njobs; ++i) f += (size_t)jobs[i].Nn * jobs[i].Kk + jobs[i].Nn;
+  return f * jobs_wgrad_msplit(M);
+}
 // sample splits of tc_wgrad's D-wide jobs: 8 at D = 256, more at smaller widths (fewer row slices per job) to fill the SMs
 inline int tc_wgrad_msplit_big(int D) { return 2048 / D; }
 constexpr size_t WPART_PAD = 16 * 512;   // bias slots of every job (up to two per output row)
@@ -58,6 +64,15 @@ inline size_t wpart_floats(size_t M, int D) {
 // then `dbslots` x Nn bias partials; wgrad_reduce adds sum_y (and sum over the slots) to dW[n * ldw + k] / db[n] in a fixed order
 struct RedJob { float* dW; float* db; int Nn, Kk, ldw, nsplit, dbslots; size_t off, stride; };
 cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st);
+
+// Programmatic dependent launch (PDL) of the TC engine's weight-gradient stage (see tc_wgrad_all).
+// launch_dependents: once every CTA of this grid has issued it (or exited), the next grid on the stream may start, if that grid is
+// launched with cudaLaunchAttributeProgrammaticStreamSerialization; otherwise it has no effect.
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+// wait: blocks until the grid this one was launched behind has completed and its stores are visible; a no-op in a grid launched
+// without that attribute.  A CTA blocked here keeps its SM, so the weight-gradient kernels let only their last CTA wait, after its
+// partials are stored: that is enough to make the grid complete only after its predecessor has.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ReLU gate bits of the TC engine, in the order of the wgmma accumulator fragment, so that each consumer thread (0..255) of a
 // 128-sample tile writes its bits with one vector store in tc_field_fwd and reads them with one vector load in tc_dgrad.

@@ -2,8 +2,14 @@
 """Per-kernel cost of the weight-gradient stage in the eager C2 train step (1024 rays x 128 samples, D = 256): torch.profiler with CUDA
 activities over PK steps, device time per step of tc_wgrad<KN>, simt_wgrad and wgrad_reduce, and for tc_wgrad the achieved bytes/s
 and tensor FLOP/s from the job shapes.  bench.py and tools/step_time.py time the whole stage as one interval.  NNB_LIB_PATH selects a
-library variant (alternate the runs of two builds to compare them).   python tools/wgrad_cost.py [tag]"""
-import json, os, re, subprocess, sys
+library variant (alternate the runs of two builds to compare them).   python tools/wgrad_cost.py [tag]
+
+The encoding and head jobs run beside the second wave of tc_wgrad<256>, so the kernel times overlap and "wgrad_ms_per_step", their
+sum, is not the stage time.  "timeline" gives, from the kernels' device timestamps, per step: the stage's wall interval (start of the
+first weight-gradient kernel to the end of the last wgrad_reduce) and the start and end of tc_wgrad<64> and simt_wgrad relative to the
+end of tc_wgrad<256> (negative: before it ends), as medians over the PK steps and per step.  A chained grid cannot end before the grid
+it was launched behind (its last CTA waits for it), so an end at about 0 means its work was done inside tc_wgrad<256>."""
+import json, os, re, statistics, subprocess, sys, tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
@@ -26,6 +32,33 @@ def tc_shapes(M, D):
     return out
 
 
+def timeline(trace_path, D):
+    """per-step intervals of the stage from a chrome trace of the profiled steps (see the module docstring)"""
+    with open(trace_path) as f:
+        evs = json.load(f)["traceEvents"]
+    ks = sorted((e["ts"], e["ts"] + e["dur"], e["name"]) for e in evs if e.get("ph") == "X" and e.get("cat") == "kernel")
+    pat = re.compile(r"(tc_wgrad<\d+>|simt_wgrad|wgrad_reduce)")
+    big = "tc_wgrad<%d>" % D
+    steps = []
+    for i, (t0, t1, name) in enumerate(ks):
+        if pat.search(name) is None or pat.search(name).group(1) != big:
+            continue
+        stage = {}
+        for s0, s1, n in ks[i:]:   # the stage: the weight-gradient kernels from this tc_wgrad<D> up to the next other kernel
+            m = pat.search(n)
+            if m is None or (s0 > t0 and m.group(1) == big):
+                break
+            stage.setdefault(m.group(1), []).append((s0, s1))
+        step = {"wall_ms": (max(e for v in stage.values() for _, e in v) - t0) / 1e3, "big_ms": (t1 - t0) / 1e3}
+        for k in ("tc_wgrad<64>", "simt_wgrad"):
+            if k in stage and k != big:
+                step[k + "_start_ms"] = (stage[k][0][0] - t1) / 1e3
+                step[k + "_end_ms"] = (stage[k][-1][1] - t1) / 1e3
+        steps.append(step)
+    med = {k: round(statistics.median(s[k] for s in steps), 4) for k in steps[0]} if steps else {}
+    return {"median": med, "per_step": [{k: round(v, 4) for k, v in s.items()} for s in steps]}
+
+
 def main():
     dev = torch.device("cuda", 0); torch.cuda.set_device(0)
     tr = bench.build_trainer(bench.make_cfg(bench.NRAYS), dev, bench.V)
@@ -37,6 +70,10 @@ def main():
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         for i in range(PK): step(i)
         torch.cuda.synchronize()
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "trace.json")
+        prof.export_chrome_trace(path)
+        tl = timeline(path, 256)
     pat = re.compile(r"(tc_wgrad<\d+>|simt_wgrad|wgrad_reduce)")
     agg = {}
     for ev in prof.key_averages():
@@ -60,7 +97,8 @@ def main():
         kernels[name] = k
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     print(json.dumps({"tag": sys.argv[1] if len(sys.argv) > 1 else "", "lib": os.path.basename(L.LIB_PATH), "gpu": q.splitlines()[0] if q else "",
-                      "steps": PK, "wgrad_ms_per_step": round(sum(v["ms_per_step"] for v in kernels.values()), 4), "kernels": kernels}))
+                      "steps": PK, "wgrad_ms_per_step": round(sum(v["ms_per_step"] for v in kernels.values()), 4), "kernels": kernels,
+                      "timeline": tl}))
 
 
 if __name__ == "__main__":
