@@ -7,8 +7,9 @@
 //   B1 composite_bwd    : compositing adjoint -> per-sample (g_rgb, g_a)
 //   B2 simt_mlp_dgrad   : data-gradient chain through the MLP, emits dY per layer
 //   B3 simt_wgrad       : dW = dY^T X as split-M tiles, one partial per split, summed in order by wgrad_reduce
+//      head_wgrad       : the same arithmetic for the TC engine's narrow head jobs, streamed at memory speed
 //   B4 ray_bwd          : per-ray geometry adjoint -> d c2w, d K, d depth, d scale/shift
-#include "nnb_workspace.cuh"
+#include "nnb_tc_common.cuh"   // mbarrier / bulk-copy wrappers (head_wgrad)
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -503,6 +504,108 @@ __global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int mspl
   if (blockIdx.x == gridDim.x - 1 && blockIdx.y == gridDim.y - 1) pdl_wait();   // chained launch: see tc_wgrad_all
 }
 
+// The head jobs of the TC engine's weight-gradient stage (fc_density, fc_rgb: 1 and 3 rows of dW; the direction slice of
+// rgb_layers.0: 27 columns), at the arithmetic of simt_wgrad: per element acc = fmaf(y, x, acc) from 0 over its split's samples in
+// increasing order, the bias in the same order, the same splits and partial layout.  They are narrow, so they read 0.29 GB at C2 size
+// for 0.6 GFLOP, and simt_wgrad's 64 x 64 tiles would stage and discard 63 of 64 dY columns (or most X columns).  Here a CTA is one
+// split of one job with all of its Nn x Kk outputs: one thread streams the split's rows, which are contiguous, into a HW_NSTG-deep
+// shared-memory ring with cp.async.bulk (whole dY and X rows, completion on an mbarrier), and thread t owns column k = t % KW
+// (KW = Kk rounded up to a power of two >= 32) and RN rows starting at RN (t / KW).  Warps release a slot through a second mbarrier.
+struct HJob { const float* dY; const float* X; int ldy, yoff, Nn, ldx, Kk, kw, rn; size_t part_off; };
+struct HJobs { HJob j[4]; int njobs; };
+constexpr int HW_CH = 16, HW_NSTG = 4, HW_MAX_LDX = 256, HW_MAX_LDY = 128;        // samples per chunk, ring depth, row limits
+constexpr int HW_SY = HW_CH * HW_MAX_LDX * 4, HW_STG = HW_SY + HW_CH * HW_MAX_LDY * 4;   // slot: X [CH][ldx] | dY [CH][ldy]
+constexpr int HW_SMEM = HW_NSTG * HW_STG + 2 * HW_NSTG * 8;
+
+template <int RN>
+__device__ __forceinline__ void head_wgrad_split(const HJob& J, size_t mb, size_t me, float* pp, unsigned char* smem) {
+  using namespace tcu;
+  const int tid = threadIdx.x, k = tid % J.kw, n0 = (tid / J.kw) * RN;
+  const int nv = J.Nn - n0 < RN ? J.Nn - n0 : RN;   // rows of this thread (<= 0: none)
+  const bool kv = k < J.Kk, bias = k < nv;   // column k valid; this thread sums the bias of row n0 + k
+  const int nch = mb < me ? (int)((me - mb + HW_CH - 1) / HW_CH) : 0;
+  const uint32_t bar0 = smem_u32(smem + HW_NSTG * HW_STG);
+  auto FULL = [&](int i) { return bar0 + 8u * i; };
+  auto EMPTY = [&](int i) { return bar0 + 8u * (HW_NSTG + i); };
+  const float* ybase = J.dY - J.yoff;   // 16-byte aligned rows
+  auto issue = [&](int c) {
+    const size_t s0 = mb + (size_t)c * HW_CH;
+    const uint32_t rows = (uint32_t)(me - s0 < (size_t)HW_CH ? me - s0 : HW_CH);
+    const uint32_t bx = rows * J.ldx * 4, by = rows * J.ldy * 4, sl = c % HW_NSTG;
+    mbar_expect_tx(FULL(sl), bx + by);
+    bulk_g2s(smem_u32(smem + sl * HW_STG), J.X + s0 * J.ldx, bx, FULL(sl));
+    bulk_g2s(smem_u32(smem + sl * HW_STG + HW_SY), ybase + s0 * J.ldy, by, FULL(sl));
+  };
+  if (tid == 0) {
+    for (int i = 0; i < HW_NSTG; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), blockDim.x / 32); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int c = 0; c < HW_NSTG && c < nch; ++c) issue(c);
+  }
+  __syncthreads();
+  float acc[RN], bsum = 0.f;
+#pragma unroll
+  for (int r = 0; r < RN; ++r) acc[r] = 0.f;
+  for (int c = 0; c < nch; ++c) {
+    const int sl = c % HW_NSTG;
+    if (tid == 0 && c > 0 && c - 1 + HW_NSTG < nch) {   // refill the slot of chunk c - 1 once every warp has released it
+      mbar_wait(EMPTY((c - 1) % HW_NSTG), (uint32_t)((c - 1) / HW_NSTG) & 1u);
+      issue(c - 1 + HW_NSTG);
+    }
+    mbar_wait(FULL(sl), (uint32_t)(c / HW_NSTG) & 1u);
+    const size_t s0 = mb + (size_t)c * HW_CH;
+    const int rows = me - s0 < (size_t)HW_CH ? (int)(me - s0) : HW_CH;
+    const float* sx = reinterpret_cast<const float*>(smem + sl * HW_STG) + k;
+    const float* sy = reinterpret_cast<const float*>(smem + sl * HW_STG + HW_SY) + J.yoff + n0;
+    if (nv > 0) {
+#pragma unroll 2
+      for (int i = 0; i < rows; ++i) {
+        const float* yr = sy + i * J.ldy;
+        if (kv) {
+          const float x = sx[i * J.ldx];
+          float y[RN];
+          if constexpr (RN >= 4) {   // 16-byte aligned: yoff = 0 and n0 a multiple of RN (launch_head_wgrad)
+#pragma unroll
+            for (int q = 0; q < RN / 4; ++q) {
+              const float4 v = reinterpret_cast<const float4*>(yr)[q];
+              y[4 * q] = v.x; y[4 * q + 1] = v.y; y[4 * q + 2] = v.z; y[4 * q + 3] = v.w;
+            }
+          } else {
+#pragma unroll
+            for (int r = 0; r < RN; ++r) y[r] = r < nv ? yr[r] : 0.f;
+          }
+#pragma unroll
+          for (int r = 0; r < RN; ++r)
+            if (r < nv) acc[r] = fmaf(y[r], x, acc[r]);
+        }
+        bsum += yr[bias ? k : 0];   // lane k < nv: the bias of row n0 + k
+      }
+    }
+    __syncwarp();
+    if ((tid & 31) == 0) mbar_arrive(EMPTY(sl));
+  }
+#pragma unroll
+  for (int r = 0; r < RN; ++r)
+    if (r < nv && kv) pp[(size_t)(n0 + r) * J.Kk + k] = acc[r];
+  if (bias) pp[(size_t)J.Nn * J.Kk + n0 + k] = bsum;
+}
+
+// grid (msplit, jobs): split blockIdx.x of job blockIdx.y; chained launch as simt_wgrad
+__global__ void __launch_bounds__(256) head_wgrad(const __grid_constant__ HJobs jobs, size_t M, int msplit, float* part) {
+  extern __shared__ __align__(128) unsigned char hsmem[];
+  const HJob& J = jobs.j[blockIdx.y];
+  size_t chunk = (M + msplit - 1) / msplit; chunk = (chunk + 15) / 16 * 16;
+  const size_t mb = (size_t)blockIdx.x * chunk, me = mb + chunk < M ? mb + chunk : M;
+  float* pp = part + J.part_off + (size_t)blockIdx.x * ((size_t)J.Nn * J.Kk + J.Nn);
+  switch (J.rn) {
+    case 1: head_wgrad_split<1>(J, mb, me, pp, hsmem); break;
+    case 2: head_wgrad_split<2>(J, mb, me, pp, hsmem); break;
+    case 4: head_wgrad_split<4>(J, mb, me, pp, hsmem); break;
+    case 8: head_wgrad_split<8>(J, mb, me, pp, hsmem); break;
+    default: head_wgrad_split<16>(J, mb, me, pp, hsmem); break;
+  }
+  if (blockIdx.x == gridDim.x - 1 && blockIdx.y == gridDim.y - 1) pdl_wait();   // chained launch: see tc_wgrad_all
+}
+
 // dW[n][k] += sum over splits (fixed order); one thread per element of all jobs
 struct RedJobs { RedJob j[16]; int e0[17]; int njobs; };
 __global__ void wgrad_reduce(RedJobs J, const float* __restrict__ part) {
@@ -767,17 +870,43 @@ cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, c
   return launch_wgrad_reduce(R, J.njobs, part, st);
 }
 
-// the small jobs of tc_wgrad_all, launched chained into part[off ..] (njobs <= 16); the caller reduces them through R
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st) {
-  if (njobs > 16) return cudaErrorInvalidValue;
-  WJobs J{};
-  for (int i = 0; i < njobs; ++i) {
-    WJob& j = J.j[i];
-    j.dY = jobs[i].dY; j.ldy = jobs[i].ldy; j.Nn = jobs[i].Nn; j.X = jobs[i].X; j.ldx = jobs[i].ldx; j.Kk = jobs[i].Kk;
-    j.dW = jobs[i].dW; j.ldw = jobs[i].ldw; j.db = jobs[i].db;
+// the head jobs of tc_wgrad_all -> head_wgrad at jobs_wgrad_msplit(M) splits, launched chained into part[off ..] (njobs <= 4); the
+// caller reduces them through R
+cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(head_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, HW_SMEM);
+    if (e != cudaSuccess) return e;
+    attr = true;
   }
+  if (njobs > 4) return cudaErrorInvalidValue;
+  const int msplit = jobs_wgrad_msplit(M);
+  HJobs J{};
+  for (int i = 0; i < njobs; ++i) {
+    const SmallJob& s = jobs[i];
+    // rows are staged whole by bulk copies: 16-byte aligned rows of 16-byte multiples (dY from its aligned row start)
+    const int yoff = (int)((reinterpret_cast<uintptr_t>(s.dY) % 16) / 4);
+    int kw = 32, rn = 1;
+    while (kw < s.Kk) kw *= 2;
+    while (rn * (256 / (kw < 256 ? kw : 256)) < s.Nn) rn *= 2;
+    if (kw > 256 || rn > 16 || s.ldx > HW_MAX_LDX || s.ldx % 4 || reinterpret_cast<uintptr_t>(s.X) % 16 || s.ldy > HW_MAX_LDY ||
+        s.ldy % 4 || yoff + s.Nn > s.ldy || (rn >= 4 && yoff != 0))
+      return cudaErrorInvalidValue;
+    J.j[i] = HJob{s.dY, s.X, s.ldy, yoff, s.Nn, s.ldx, s.Kk, kw, rn, off};
+    const size_t stride = (size_t)s.Nn * s.Kk + s.Nn;
+    R[i] = RedJob{s.dW, s.db, s.Nn, s.Kk, s.ldw, msplit, s.db ? 1 : 0, off, stride};
+    off += stride * msplit;
+  }
+  if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
   J.njobs = njobs;
-  return launch_simt_wgrad(J, M, D, jobs_wgrad_msplit(M), part, off, R, true, st);
+  cudaLaunchAttribute at{};
+  at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(msplit, njobs); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = HW_SMEM; cfg.stream = st;
+  cfg.attrs = &at; cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, head_wgrad, J, M, msplit, part);
+  return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st) {

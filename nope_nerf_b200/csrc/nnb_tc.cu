@@ -23,10 +23,12 @@
 // (k / 8) * rows * 16 + row * 16 + (k % 8) * 2: 8 x 8 core matrices of 128 contiguous bytes, SBO = 128 B between row groups,
 // LBO = rows * 16 B between the two k-halves of one MMA.
 #include "nnb_tc_common.cuh"
+#include <cuda.h>            // CUtensorMap (types only: the driver entry point is obtained at run time)
+#include <cudaTypedefs.h>    // PFN_cuTensorMapEncodeTiled
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st);
 cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
-cudaError_t launch_simt_wgrad_jobs(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st);
+cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st);
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -379,7 +381,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
 // sequence for any chunking.  Bias slot h of a row sums samples 32h .. 32h + 31 of each 64-sample block in sample order.  Each split
 // stores its partial dW and bias slots to the split buffer; wgrad_reduce adds the splits in a fixed order, so the result is the same
 // every run.
-struct WgJobT { const float* dY; const float* X; float* dW; float* db; int ldy, Nn, ldx, Kk, ldw, cta0; size_t part_off; };
+// tc_wgrad_piece<KN> runs one job as column pieces: the CTA holds columns k0 .. k0 + KN - 1 of the job's dW and stages that column
+// block of X through a 2-D tensor map (X rows are wider than KN).  An output element's K-steps, MMAs and operands are those of the
+// whole-job CTA, and the piece stores exactly that CTA's floats of its columns; only the piece at k0 = 0 stores the bias slots.
+struct WgJobT { const float* dY; const float* X; float* dW; float* db; int ldy, Nn, ldx, Kk, ldw, cta0; size_t part_off; int k0; };
 constexpr int MAX_WG_JOBS = 10, WG_BLOCK = 64;
 struct WgJobsT { WgJobT j[MAX_WG_JOBS]; int njobs, msplit, per_cta; };
 constexpr int WG_MAX_LDY = 256;
@@ -394,8 +399,15 @@ template <int KN> struct Wg {   // shared-memory map (bytes) of tc_wgrad<KN>; X 
   static_assert(NSTG >= 2 && SMEM <= 232448, "shared memory budget");
 };
 
-template <int KN>   // 256 | 128 | 64: columns of dW (features of X) held by one CTA
-__global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJobsT J, size_t M, float* __restrict__ part) {
+// 2-D bulk tensor copy of box (c0, c1) of the map (innermost coordinate first), completion on `bar`
+__device__ __forceinline__ void tma_g2s_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar) : "memory");
+}
+
+// KN = 256 | 128 | 64: columns of dW (features of X) held by one CTA.  XMAP: X column block k0 .. k0 + KN - 1 through xmap (box KN x CH)
+template <int KN, bool XMAP>
+__device__ __forceinline__ void wgrad_body(const WgJobsT& J, const CUtensorMap* xmap, size_t M, float* __restrict__ part) {
   using W = Wg<KN>;
   constexpr int CH = W::CH, NSTG = W::NSTG, NOP = W::NOP, A_BYTES = W::A_BYTES, B_BYTES = W::B_BYTES;
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -433,7 +445,8 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
       if (s0 < s_end) {   // then rows s0 .. s0 + 31 < Mpad: in bounds of the stash
         mbar_expect_tx(SFULL(sl), (uint32_t)(CH * (jb.ldy + KN) * 4));
         bulk_g2s(smem_u32(smem + sl * W::STG), jb.dY + s0 * jb.ldy, (uint32_t)(CH * jb.ldy * 4), SFULL(sl));
-        bulk_g2s(smem_u32(smem + sl * W::STG + W::SY), jb.X + s0 * KN, CH * KN * 4, SFULL(sl));
+        if constexpr (XMAP) tma_g2s_2d(smem_u32(smem + sl * W::STG + W::SY), xmap, jb.k0, (int)s0, SFULL(sl));
+        else bulk_g2s(smem_u32(smem + sl * W::STG + W::SY), jb.X + s0 * KN, CH * KN * 4, SFULL(sl));
       } else {
         mbar_arrive(SFULL(sl));
       }
@@ -471,7 +484,7 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
         const int item = ct + i * 128, k = item % KN, so = item / KN;
         float v[8];
 #pragma unroll
-        for (int q = 0; q < 8; ++q) v[q] = (k < jb.Kk && so * 8 + q < nvalid) ? sx[(so * 8 + q) * KN + k] : 0.f;
+        for (int q = 0; q < 8; ++q) v[q] = (jb.k0 + k < jb.Kk && so * 8 + q < nvalid) ? sx[(so * 8 + q) * KN + k] : 0.f;
         split_store8_bf16(v, op + 2 * A_BYTES + so * KN * 16 + k * 16, op + 2 * A_BYTES + B_BYTES + so * KN * 16 + k * 16);
       }
       fence_async_smem();
@@ -479,7 +492,7 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
       if (ct == 0) mbar_arrive(OPFULL(ob));
       if (ct == 0 && c + NSTG < nch) issue(c + NSTG);
     }
-    if (ct < ny) {
+    if (ct < ny && jb.k0 == 0) {
       pp[(size_t)jb.Nn * jb.Kk + n0 + ct] = db0;
       pp[(size_t)jb.Nn * jb.Kk + jb.Nn + n0 + ct] = db1;
     }
@@ -520,11 +533,21 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJob
       const int n = r0 + 8 * r;
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int k = j * 8 + c0 + e;
+        const int k = jb.k0 + j * 8 + c0 + e;
         if (n < jb.Nn && k < jb.Kk) pp[(size_t)n * jb.Kk + k] = acc[4 * j + 2 * r + e];
       }
     }
   if (last_cta) pdl_wait();
+}
+
+template <int KN>
+__global__ void __launch_bounds__(384, 1) tc_wgrad(const __grid_constant__ WgJobsT J, size_t M, float* __restrict__ part) {
+  wgrad_body<KN, false>(J, nullptr, M, part);
+}
+template <int KN>   // a separate name in profiles: the column pieces of one job, X through the tensor map
+__global__ void __launch_bounds__(384, 1) tc_wgrad_piece(const __grid_constant__ WgJobsT J, const __grid_constant__ CUtensorMap xmap,
+                                                         size_t M, float* __restrict__ part) {
+  wgrad_body<KN, true>(J, &xmap, M, part);
 }
 
 // floats of the partial buffer that tc_wgrad uses for these jobs at msplit sample splits (two bias slots per row)
@@ -534,30 +557,58 @@ size_t wg_part_floats(const WgJobT* jobs, int njobs, int msplit) {
   return f * msplit;
 }
 
-// jobs -> tc_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent
-// launch behind the previous grid on the stream (see tc_wgrad_all)
-template <int KN>
+// map of the fp32 [rows][ldx] matrix X with a box of box_cols x box_rows floats (rows past `rows` read as zeros).  The library links
+// cudart statically and not libcuda, so the driver's encoder is looked up through the runtime.
+cudaError_t encode_x_map(CUtensorMap* map, const float* X, int ldx, size_t rows, int box_cols, int box_rows) {
+  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+  if (!encode) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    cudaError_t e = cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q);
+    if (e != cudaSuccess) return e;
+    if (q != cudaDriverEntryPointSuccess || !fn) return cudaErrorSymbolNotFound;
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)ldx, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)ldx * 4};
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows}, elem_strides[2] = {1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(X), dims, strides, box, elem_strides,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
+}
+
+// jobs -> tc_wgrad<KN> into part[off ..], or with PIECES one job as ceil(Kk / KN) column pieces of tc_wgrad_piece<KN>; R[i] receives
+// job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent launch behind the previous grid on the stream (see
+// tc_wgrad_all)
+template <int KN, bool PIECES = false>
 cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msplit, float* part, size_t off, RedJob* R, bool chained,
                          cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+    cudaError_t e;
+    if constexpr (PIECES) e = cudaFuncSetAttribute(tc_wgrad_piece<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+    else e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
     if (e != cudaSuccess) return e;
     attr = true;
   }
+  if (PIECES && njobs != 1) return cudaErrorInvalidValue;   // one tensor map per launch
   WgJobsT J{};
-  int ctas = 0;
+  int ctas = 0, nj = 0;
   for (int i = 0; i < njobs; ++i) {
-    // X and dY chunks are staged as whole rows (16-byte multiples)
-    if (jobs[i].ldx != KN || jobs[i].ldy > WG_MAX_LDY || jobs[i].ldy % 4) return cudaErrorInvalidValue;
-    J.j[i] = jobs[i]; J.j[i].cta0 = ctas; ctas += (jobs[i].Nn + 127) / 128 * msplit;
+    // dY chunks are staged as whole rows, X chunks as whole rows or (pieces) KN-column boxes: 16-byte multiples
+    if ((PIECES ? jobs[i].ldx % 4 != 0 : jobs[i].ldx != KN) || jobs[i].ldy > WG_MAX_LDY || jobs[i].ldy % 4) return cudaErrorInvalidValue;
+    const int pieces = PIECES ? (jobs[i].Kk + KN - 1) / KN : 1;
+    if (nj + pieces > MAX_WG_JOBS) return cudaErrorInvalidValue;
+    for (int p = 0; p < pieces; ++p, ++nj) {
+      J.j[nj] = jobs[i]; J.j[nj].k0 = p * KN; J.j[nj].cta0 = ctas; J.j[nj].part_off = off;
+      ctas += (jobs[i].Nn + 127) / 128 * msplit;
+    }
     const size_t stride = (size_t)jobs[i].Nn * jobs[i].Kk + 2 * jobs[i].Nn;
-    J.j[i].part_off = off;
     R[i] = RedJob{jobs[i].dW, jobs[i].db, jobs[i].Nn, jobs[i].Kk, jobs[i].ldw, msplit, 2, off, stride};
     off += stride * msplit;
   }
   if (off > wpart_floats(M, D)) return cudaErrorInvalidValue;
-  J.njobs = njobs; J.msplit = msplit;
+  J.njobs = nj; J.msplit = msplit;
   J.per_cta = (int)(((M + msplit - 1) / msplit + WG_BLOCK - 1) / WG_BLOCK * WG_BLOCK);
   cudaLaunchAttribute at{};
   at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -565,28 +616,39 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(ctas); cfg.blockDim = dim3(384); cfg.dynamicSmemBytes = Wg<KN>::SMEM; cfg.stream = st;
   cfg.attrs = &at; cfg.numAttrs = chained ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, tc_wgrad<KN>, J, M, part);
+  cudaError_t e;
+  if constexpr (PIECES) {
+    CUtensorMap xmap;
+    e = encode_x_map(&xmap, jobs[0].X, jobs[0].ldx, M, KN, Wg<KN>::CH);
+    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, tc_wgrad_piece<KN>, J, xmap, M, part);
+  } else {
+    e = cudaLaunchKernelEx(&cfg, tc_wgrad<KN>, J, M, part);
+  }
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-// The weight-gradient stage of the TC engine's backward: the MLP GEMMs on tensor cores, the small heads on the fp32 SIMT kernel.
-// The D-wide jobs run as (Nn / 128) x ms_big CTAs, one per SM: 136 at D = 256, one full wave on 132 SMs and a second wave of 4 CTAs.
-// The encoding jobs (tc_wgrad<64>) and the head jobs (simt_wgrad) read only the dgrad stash, so they are launched behind it with
-// programmatic dependent launch: each grid starts once every CTA of the grid before it is resident, so they fill the SMs that the
-// second wave leaves idle.  The last CTA of each chained grid waits (griddepcontrol.wait) for the grid before it after storing its
-// partials, so the heads complete only after the encoding jobs and the D-wide jobs have; one plain-launched wgrad_reduce then adds
-// the splits of all 14 jobs.  Each job has its own region of the partial buffer, so the grids never write the same floats, and no
-// two jobs write the same dW / db element (the encoding slice of layer 4 and the direction slice of rgb_layers.0 are at column
-// offset D, enc[1] has no bias), so one reduce gives the same bits as one per grid.
+// The weight-gradient stage of the TC engine's backward: the MLP GEMMs on tensor cores, the small heads on the fp32 SIMT kernel
+// head_wgrad.  Four grids, each chained behind the one before with programmatic dependent launch:
+//   1. the D-wide jobs (layers 1..7, fc_feature): (Nn / 128) x ms_big CTAs of one SM each, 128 at D = 256 and at D = 128, so one
+//      wave on 132 SMs (256 at D = 64);
+//   2. rgb_layers.0 (D / 2 rows, X = feat) as 64-column pieces, tc_wgrad_piece<64>: 4 pieces x 8 splits at D = 256.  The first ones
+//      run on the SMs that grid 1 leaves free, the rest spread over all SMs when it ends.  Whole, this job made a second wave;
+//   3. the encoding jobs (tc_wgrad<64>), which read only the dgrad stash;
+//   4. the head jobs (head_wgrad).
+// A chained grid starts once every CTA of the grid before it is resident.  The last CTA of each chained grid waits
+// (griddepcontrol.wait) for the grid before it after storing its partials, so each grid completes only after every grid before it;
+// one plain-launched wgrad_reduce then adds the splits of all 14 jobs.  Each job has its own region of the partial buffer, so the
+// grids never write the same floats, and no two jobs write the same dW / db element (the encoding slice of layer 4 and the
+// direction slice of rgb_layers.0 are at column offset D, enc[1] has no bias), so one reduce gives the same bits as one per grid.
 cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) {
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
   const int D = L.D, DR = D / 2;
-  WgJobT big[9], enc[2];
+  WgJobT big[8], enc[2];
   int nb = 0;
   for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(D, l), gw + nnb::b_off(D, l), D, D, D, D, nnb::w_ld(D, l), 0, 0};
   big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT(D), gw + nnb::B_FEAT(D), D, D, D, D, D, 0, 0};
-  big[nb++] = WgJobT{F(L.dyr), F(L.feat), gw + nnb::W_RGBH(D), gw + nnb::B_RGBH(D), DR, DR, D, D, D + 27, 0, 0};
+  const WgJobT rgb{F(L.dyr), F(L.feat), gw + nnb::W_RGBH(D), gw + nnb::B_RGBH(D), DR, DR, D, D, D + 27, 0, 0};
   enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(D, 0), gw + nnb::b_off(D, 0), D, D, 64, 63, 63, 0, 0};
   enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(D, 4) + D, nullptr, D, D, 64, 63, D + 63, 0, 0};
   const float* dyc = F(L.dyc);
@@ -595,27 +657,31 @@ cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw,
       {F(L.dyr), F(L.denc), gw + nnb::W_RGBH(D) + D, nullptr, DR, DR, 32, 27, D + 27},
       {dyc, F(L.hr), gw + nnb::W_RGB(D), gw + nnb::B_RGB(D), 4, 3, DR, DR, DR}};
   float* part = F(L.wpart);
-  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (17 | 4 row slices at D = 256)
+  // sample splits: about one wave of 1-CTA-per-SM blocks per launch (16 | 4 row slices at D = 256)
   const int ms_big = L.M >= 8 * 128 ? tc_wgrad_msplit_big(D) : 1, ms_enc = L.M >= 32 * 64 ? 32 : 1;
-  // Partial regions: D-wide jobs, then heads, then encoding jobs.  In floats, np = num_params(D), at most 64 head splits and
-  // 32 encoding splits: at D = 256 big + heads = 4 491 264 + 270 592 <= 8 (np + 8192) = 4 832 288 <= wpart_floats, and likewise at
-  // D = 128 (2 398 464 <= 2 669 632) and D = 64 (1 216 768 <= 1 686 656).  The encoding region (1 064 960 floats at D = 256) fits
-  // as well only where wpart_floats is larger: at D = 256 when M > 36 864 (16 (np + 8192) at the C2 size), at D = 64 always, at
-  // D = 128 never.  Where it does not fit, the encoding jobs run after the chained reduce, with their own reduce, from offset 0.
-  const size_t big_f = wg_part_floats(big, nb, ms_big), head_f = small_jobs_part_floats(sm, 3, L.M);
+  // Partial regions: D-wide jobs, rgb_layers.0, then heads, then encoding jobs.  In floats, np = num_params(D), at most 64 head
+  // splits and 32 encoding splits: at D = 256 (D-wide + rgb) + heads = 4 491 264 + 270 592 <= 8 (np + 8192) = 4 832 288 <= wpart_floats,
+  // and likewise at D = 128 (2 398 464 <= 2 669 632) and D = 64 (1 216 768 <= 1 686 656).  The encoding region (1 064 960 floats at
+  // D = 256) fits as well only where wpart_floats is larger: at D = 256 when M > 36 864 (16 (np + 8192) at the C2 size), at D = 64
+  // always, at D = 128 never.  Where it does not fit, the encoding jobs run after the chained reduce, with their own reduce, from
+  // offset 0.
+  const size_t trunk_f = wg_part_floats(big, nb, ms_big), big_f = trunk_f + wg_part_floats(&rgb, 1, ms_big);
+  const size_t head_f = small_jobs_part_floats(sm, 3, L.M);
   const bool enc_chained = big_f + head_f + wg_part_floats(enc, 2, ms_enc) <= wpart_floats(L.M, D);
   RedJob R[9 + 2 + 3];
-  int nr = nb;
   cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
                 : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
                            : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, 0, R, false, st);
   if (e != cudaSuccess) return e;
+  e = launch_wgrad<64, true>(&rgb, 1, L.M, D, ms_big, part, trunk_f, R + nb, true, st);
+  if (e != cudaSuccess) return e;
+  int nr = nb + 1;
   if (enc_chained) {   // encoding before heads: its CTAs need a whole SM each, and the small head CTAs would fragment the free SMs
     e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, big_f + head_f, R + nr, true, st);
     if (e != cudaSuccess) return e;
     nr += 2;
   }
-  e = launch_simt_wgrad_jobs(sm, 3, L.M, D, part, big_f, R + nr, st);
+  e = launch_head_wgrad(sm, 3, L.M, D, part, big_f, R + nr, st);
   if (e != cudaSuccess) return e;
   nr += 3;
   e = launch_wgrad_reduce(R, nr, part, st);

@@ -1,14 +1,15 @@
 #!/usr/bin/env python
 """Per-kernel cost of the weight-gradient stage in the eager C2 train step (1024 rays x 128 samples, D = 256): torch.profiler with CUDA
-activities over PK steps, device time per step of tc_wgrad<KN>, simt_wgrad and wgrad_reduce, and for tc_wgrad the achieved bytes/s
-and tensor FLOP/s from the job shapes.  bench.py and tools/step_time.py time the whole stage as one interval.  NNB_LIB_PATH selects a
+activities over PK steps, device time per step of tc_wgrad<KN>, tc_wgrad_piece<64>, head_wgrad (simt_wgrad in older builds) and
+wgrad_reduce, and for the tensor-core kernels the achieved bytes/s and tensor FLOP/s from the job shapes.  bench.py and tools/step_time.py time the whole stage as one interval.  NNB_LIB_PATH selects a
 library variant (alternate the runs of two builds to compare them).   python tools/wgrad_cost.py [tag]
 
-The encoding and head jobs run beside the second wave of tc_wgrad<256>, so the kernel times overlap and "wgrad_ms_per_step", their
-sum, is not the stage time.  "timeline" gives, from the kernels' device timestamps, per step: the stage's wall interval (start of the
-first weight-gradient kernel to the end of the last wgrad_reduce) and the start and end of tc_wgrad<64> and simt_wgrad relative to the
-end of tc_wgrad<256> (negative: before it ends), as medians over the PK steps and per step.  A chained grid cannot end before the grid
-it was launched behind (its last CTA waits for it), so an end at about 0 means its work was done inside tc_wgrad<256>."""
+The rgb_layers.0 pieces, the encoding jobs and the head jobs are chained behind tc_wgrad<256>, so the kernel times overlap and
+"wgrad_ms_per_step", their sum, is not the stage time.  "timeline" gives, from the kernels' device timestamps, per step: the stage's
+wall interval (start of the first weight-gradient kernel to the end of the last wgrad_reduce) and the start and end of
+tc_wgrad_piece<64>, tc_wgrad<64> and the head kernel relative to the end of tc_wgrad<256> (negative: before it ends), as medians over
+the PK steps and per step.  A chained grid cannot end before the grid it was launched behind (its last CTA waits for it), so an end at
+about 0 means its work was done inside tc_wgrad<256>."""
 import json, os, re, statistics, subprocess, sys, tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -20,14 +21,15 @@ PK = 10
 
 
 def tc_shapes(M, D):
-    """per tc_wgrad launch of tc_wgrad_all: (bytes of dY and X if each is read once, bytes as issued (every 128-row slice of a job reads
-    its X), tensor FLOP: three bf16 MMAs per logical multiply-add)"""
-    launches = {"tc_wgrad<%d>" % D: ([D] * 8 + [D // 2], D, D, False),   # dY widths (layers 1..7, fc_feature, rgb_layers.0), X width, Kk
-                "tc_wgrad<64>": ([D, D], 64, 63, True)}                  # layers 0 and 4: one shared X (the encoding stash)
+    """per tensor-core launch of tc_wgrad_all: (bytes of dY and X if each is read once, bytes as issued (every 128-row slice of a job
+    reads its X, every 64-column piece its whole dY rows and its X columns), tensor FLOP: three bf16 MMAs per logical multiply-add)"""
+    launches = {"tc_wgrad<%d>" % D: ([D] * 8, D, D, False, 1),   # dY widths (layers 1..7, fc_feature), X width, Kk, X shared, pieces
+                "tc_wgrad_piece<64>": ([D // 2], D, D, False, D // 64),   # rgb_layers.0 in 64-column pieces
+                "tc_wgrad<64>": ([D, D], 64, 63, True, 1)}                # layers 0 and 4: one shared X (the encoding stash)
     out = {}
-    for name, (nns, ldx, kk, shared_x) in launches.items():
+    for name, (nns, ldx, kk, shared_x, pieces) in launches.items():
         once = sum(M * nn * 4 for nn in nns) + M * ldx * 4 * (1 if shared_x else len(nns))
-        issued = sum(M * (nn + (nn + 127) // 128 * ldx) * 4 for nn in nns)
+        issued = sum(M * (nn * pieces + (nn + 127) // 128 * ldx) * 4 for nn in nns)
         out[name] = (once, issued, sum(3 * 2 * M * nn * kk for nn in nns))
     return out
 
@@ -37,7 +39,7 @@ def timeline(trace_path, D):
     with open(trace_path) as f:
         evs = json.load(f)["traceEvents"]
     ks = sorted((e["ts"], e["ts"] + e["dur"], e["name"]) for e in evs if e.get("ph") == "X" and e.get("cat") == "kernel")
-    pat = re.compile(r"(tc_wgrad<\d+>|simt_wgrad|wgrad_reduce)")
+    pat = re.compile(r"(tc_wgrad<\d+>|tc_wgrad_piece<\d+>|simt_wgrad|head_wgrad|wgrad_reduce)")
     big = "tc_wgrad<%d>" % D
     steps = []
     for i, (t0, t1, name) in enumerate(ks):
@@ -50,7 +52,7 @@ def timeline(trace_path, D):
                 break
             stage.setdefault(m.group(1), []).append((s0, s1))
         step = {"wall_ms": (max(e for v in stage.values() for _, e in v) - t0) / 1e3, "big_ms": (t1 - t0) / 1e3}
-        for k in ("tc_wgrad<64>", "simt_wgrad"):
+        for k in ("tc_wgrad_piece<64>", "tc_wgrad<64>", "head_wgrad", "simt_wgrad"):
             if k in stage and k != big:
                 step[k + "_start_ms"] = (stage[k][0][0] - t1) / 1e3
                 step[k + "_end_ms"] = (stage[k][-1][1] - t1) / 1e3
@@ -74,7 +76,7 @@ def main():
         path = os.path.join(tmp, "trace.json")
         prof.export_chrome_trace(path)
         tl = timeline(path, 256)
-    pat = re.compile(r"(tc_wgrad<\d+>|simt_wgrad|wgrad_reduce)")
+    pat = re.compile(r"(tc_wgrad<\d+>|tc_wgrad_piece<\d+>|simt_wgrad|head_wgrad|wgrad_reduce)")
     agg = {}
     for ev in prof.key_averages():
         m = pat.search(ev.key)
