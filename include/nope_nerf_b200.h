@@ -109,6 +109,11 @@ int nnb_profile_events(void** events, int32_t count);
 int nnb_profile_cursor(void);
 /* test aid: byte offsets of the workspace sections {records, h0..h7, feat, hr, enc, denc, total} */
 int nnb_debug_layout(int32_t N, int32_t S, uint32_t flags, int32_t engine, size_t* out14);
+/* test aid: the weight-gradient stage that nnb_render_bwd runs for a->engine, alone, on whatever the workspace's activation / output-
+ * gradient stash holds (layout of nnb_debug_layout); g_weights [nnb_num_params(a->hidden_dim)] is ACCUMULATED (+=).  Reads a->N, S,
+ * flags (NNB_STASH required; NNB_TCBWD, which no engine of this library runs, is rejected on both), engine, hidden_dim, workspace and
+ * workspace_bytes only. */
+int nnb_debug_wgrad(const nnb_render_args* a, float* g_weights, void* stream);
 /* bytes of workspace needed by nnb_render_fwd (+bwd when NNB_STASH) at hidden_dim 256 */
 size_t nnb_workspace_bytes(int32_t N, int32_t S, uint32_t flags, int32_t engine);
 /* the same for the field of width hidden_dim (0 = 256); 0 for an unsupported width */

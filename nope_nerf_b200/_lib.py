@@ -73,6 +73,7 @@ def _load():
     lib.nnb_num_params.argtypes = [C.c_int32]
     lib.nnb_render_fwd.argtypes = [C.POINTER(RenderArgs), C.c_void_p]
     lib.nnb_render_bwd.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
+    lib.nnb_debug_wgrad.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]   # test aid
     lib.nnb_field_fwd.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]
     lib.nnb_field_bwd.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, C.c_void_p]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]

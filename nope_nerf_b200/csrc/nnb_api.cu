@@ -10,9 +10,11 @@ cudaError_t simt_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cud
 cudaError_t simt_field_fwd(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st);
 cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights,
                            cudaStream_t st);
+cudaError_t simt_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
+cudaError_t tc_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
 size_t tc_workspace_extra(int N, int S, uint32_t flags, int D);
 bool tc_supports(int S);
 #endif
@@ -95,6 +97,7 @@ static int check_dim(const nnb_render_args* a) {
   return 0;
 }
 
+static int check_engine_ws(const nnb_render_args* a);
 static int check_args(const nnb_render_args* a) {
   if (!a) return fail(-1, "null args");
   if (a->N <= 0) return fail(-2, "N must be positive (got %d)", a->N);
@@ -105,6 +108,11 @@ static int check_args(const nnb_render_args* a) {
   if (!a->depth && !(a->depth_map && a->ray_idx && a->h_d > 0 && a->w_d > 0 && a->H > 0 && a->W > 0))
     return fail(-3, "need depth[N] or (depth_map,h_d,w_d,H,W,ray_idx)");
   if (!a->rgb || !a->depth_pred || !a->depth_gt || !a->mask) return fail(-3, "output pointers must be non-null");
+  return check_engine_ws(a);
+}
+
+// engine, width, the engine's S range, and the workspace's size and alignment
+static int check_engine_ws(const nnb_render_args* a) {
   if (a->engine != NNB_ENGINE_SIMT && a->engine != NNB_ENGINE_TC) return fail(-4, "unknown engine %d", a->engine);
   if (int rc = check_dim(a)) return rc;
 #ifndef NNB_WITH_TC
@@ -148,6 +156,22 @@ int nnb_render_bwd(const nnb_render_bwd_args* b, void* stream) {
 #endif
   e = (b->phase == 2) ? cudaSuccess : simt_render_bwd(*b, L, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_bwd");
+}
+
+// test aid: the weight-gradient stage of nnb_render_bwd for a->engine alone, on whatever the workspace's stash holds
+int nnb_debug_wgrad(const nnb_render_args* a, float* g_weights, void* stream) {
+  if (!a || !g_weights) return fail(-3, "nnb_debug_wgrad: need args and g_weights");
+  if (a->N <= 0) return fail(-2, "N must be positive (got %d)", a->N);
+  if (a->S < 2 || a->S > 1024) return fail(-2, "S must be in [2,1024] (got %d)", a->S);
+  if (!(a->flags & NNB_STASH) || (a->flags & NNB_TCBWD)) return fail(-6, "nnb_debug_wgrad needs the fp32 stash layout (NNB_STASH without NNB_TCBWD)");
+  if (int rc = check_engine_ws(a)) return rc;
+  WsLayout L = make_layout(a->N, a->S, a->flags, a->engine, hidden_of(a->hidden_dim));
+  cudaError_t e;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) e = tc_wgrad_stage(*a, L, g_weights, (cudaStream_t)stream); else
+#endif
+  e = simt_wgrad_stage(*a, L, g_weights, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_debug_wgrad");
 }
 
 static int check_field(const nnb_render_args* a) {

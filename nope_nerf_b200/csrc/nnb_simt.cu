@@ -937,6 +937,11 @@ cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cuda
   }
 }
 
+// the weight-gradient stage of simt_render_bwd alone, on whatever the stash holds (nnb_debug_wgrad)
+cudaError_t simt_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) {
+  return simt_wgrad_all(make_ptrs(L, a.workspace), L, gw, st);
+}
+
 cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st) {
   RedJobs J{};
   J.njobs = njobs < 16 ? njobs : 16;

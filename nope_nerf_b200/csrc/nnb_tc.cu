@@ -1084,3 +1084,6 @@ cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaS
   if (b.fwd.flags & NNB_TCBWD) return cudaErrorNotSupported;
   return b.phase == 2 ? cudaSuccess : simt_render_bwd_with(b, L, st, tc_dgrad_launch, tc_wgrad_all);
 }
+
+// the weight-gradient stage of tc_render_bwd alone, on whatever the stash holds (nnb_debug_wgrad)
+cudaError_t tc_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) { return tc_wgrad_all(a, L, gw, st); }

@@ -109,8 +109,8 @@ def _cuda(x):
     return torch.from_numpy(np.ascontiguousarray(x)).cuda()
 
 
-def _render(P, D, N, S, seed):
-    """TC render forward with NNB_STASH on seeded inputs; returns the call (its workspace holds the stash)"""
+def _render(P, D, N, S, seed, engine=None):
+    """TC (or `engine`) render forward with NNB_STASH on seeded inputs; returns the call (its workspace holds the stash)"""
     from nope_nerf_b200 import ops, _lib as L
     rng = np.random.default_rng(seed)
     H, W = 48, 64
@@ -119,7 +119,8 @@ def _render(P, D, N, S, seed):
     c2w = torch.empty(4, 4, device="cuda"); ops.pose_fwd_raw(r, t, None, 1, c2w)
     cam = torch.diag(torch.tensor([1.2, -1.6, -1.0, 1.0])).cuda()
     ray_idx = rng.permutation(H * W)[:N]
-    return ops.RenderCall(_cuda(O.flatten_params(P)), c2w, cam, N=N, S=S, flags=ops.flags_from_cfg(cfg, "softplus"), engine=L.ENGINE_TC,
+    return ops.RenderCall(_cuda(O.flatten_params(P)), c2w, cam, N=N, S=S, flags=ops.flags_from_cfg(cfg, "softplus"),
+                          engine=L.ENGINE_TC if engine is None else engine,
                           near=0.01, far=10.0, ray_idx=_cuda(ray_idx), depth_map=_cuda(rng.uniform(.6, 7.2, (24, 32)).astype(np.float32)),
                           scale=torch.tensor([1.05]).cuda(), shift=torch.tensor([0.02]).cuda(),
                           noise=_cuda(rng.uniform(0, 1, (N, S)).astype(np.float32)), H=H, W=W, stash=True, hidden_dim=D)
