@@ -85,7 +85,10 @@ typedef struct nnb_render_bwd_args {
   const float* g_rgb;        /* [N,3] */
   const float* g_depth_pred; /* [N] dense (0 where masked out) or NULL */
   const float* g_depth_gt;   /* [N] dense or NULL                      */
-  /* outputs, all ACCUMULATED (+=): caller zeroes them */
+  /* outputs, all ACCUMULATED (+=): caller zeroes them.  Reproducible: every reduction runs in a fixed order, so the same inputs give
+   * the same bits on every run.  g_weights gets plain adds (and g_depth is overwritten): no other work may write them during the call.  g_c2w, g_cam
+   * and g_scale_shift get one atomic add per element: other work may add into them concurrently (the sums stay correct), but the bits
+   * are reproducible only when that work is ordered before or after the call. */
   float* g_weights; /* [nnb_num_params(fwd.hidden_dim)] or NULL (pose-only: Trainer_pose, eval_pose_one_epoch.py:25-41) */
   float* g_c2w;     /* [16] (rows 0..2 written) */
   float* g_cam;     /* [16] ([0],[5] written) or NULL */
@@ -100,7 +103,7 @@ typedef struct nnb_render_bwd_args {
 } nnb_render_bwd_args;
 
 const char* nnb_last_error(void);
-int nnb_version(void);
+int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys */
 /* Profiling hook used by bench.py: `events` is a HOST array of cudaEvent_t handles that stays alive until
  * nnb_profile_events(NULL,0).  Every nnb_render_fwd records 4 marks (start, weights imaged, field done,
  * composited) and every nnb_render_bwd 5 marks (start, compositing adjoint, data-gradient chain,
@@ -168,10 +171,20 @@ int nnb_loss_rgb_depth(const float* rgb, const float* rgb_gt, const float* img, 
                        float* g_rgb, float* g_depth_pred, float* g_depth_gt, void* stream);
 
 /* Loss.get_pc_loss 'dense' (model/losses.py:114-148): symmetric mean nearest-neighbour distance (brute force, argmin ties ->
- * first index like torch.argmin).  X [P,3], Y [Q,3]; keys [P+Q] 64-bit scratch; idx_xy [P], idx_yx [Q] optional int32
- * nearest-neighbour outputs (both or neither); loss [1] (+=); optional adjoints gX, gY (+=, both or neither). */
+ * first index like torch.argmin).  X [P,3], Y [Q,3]; keys: scratch of nnb_chamfer_workspace_bytes(P, Q) bytes when the adjoints
+ * are requested, [P+Q] 64-bit otherwise; idx_xy [P], idx_yx [Q] optional int32 nearest-neighbour outputs (both or neither);
+ * loss [1] (+=); optional adjoints gX, gY (+=, both or neither).
+ * Reproducible: the same inputs give the same bits on every run.  The loss is summed from block partials in block order; each
+ * adjoint element collects the terms of the pairs whose nearest neighbour it is in 64-bit fixed point (integer adds, so their order
+ * does not matter) and rounds that sum to float once.  Each term is first rounded to a quantum of 2^-F |weight| / n, n the size of
+ * its cloud and F = 62 - bits(n) (2^-48 at n = 16 128): far below float resolution for the large terms, coarser than a float sum
+ * for components many orders of magnitude below |weight| / n.  A component that receives a non-finite term comes out NaN.
+ * loss, gX and gY get plain (non-atomic) adds: no other work may write them while the call runs. */
 int nnb_chamfer(const float* X, int32_t P, const float* Y, int32_t Q, uint64_t* keys, int32_t* idx_xy, int32_t* idx_yx,
                 float* loss, float weight, float* gX, float* gY, void* stream);
+/* bytes of `keys` scratch nnb_chamfer needs with adjoints (search keys, fixed-point group sums); 0 on bad sizes.  The call cannot
+ * check the size it is given: a smaller buffer is written out of bounds. */
+size_t nnb_chamfer_workspace_bytes(int32_t P, int32_t Q);
 
 /* Reference-image stage of Trainer.compute_loss (model/training.py:280-365): point-cloud (dense chamfer) + warped-RGB terms
  * between the current view and one reference view, forward AND adjoint in one call.
@@ -183,7 +196,11 @@ int nnb_chamfer(const float* X, int32_t P, const float* Y, int32_t Q, uint64_t* 
  *   d(c2w_cur, dist_cur, (kx, ky)); loss_total (optional) += the weighted sum.
  * CUDA-graph replay: per-step values may come from device memory instead of the host fields -- img_pp (device array of the two
  * frame pointers {cur, ref}, replaces img_cur / img_ref), cam (device camera_mat [16]: kx = cam[0], ky = cam[5]), cam_idx_dev +
- * num_cams (is_last = *cam_idx_dev == num_cams - 1), weights_dev ({w_pc, w_rgb_s}). */
+ * num_cams (is_last = *cam_idx_dev == num_cams - 1), weights_dev ({w_pc, w_rgb_s}).
+ * Reproducible: every sum over the points runs in a fixed order (per-block partials in the workspace, added in block order), so the
+ * same inputs give the same bits on every run.  losses is overwritten.  g_c2w, g_dist, g_kxy, loss_total, g_c2w_ref and g_dist_ref
+ * each get one atomic add per element from one thread: other work may add into the same buffers concurrently (the sums stay
+ * correct), but the bits are reproducible only when that work is ordered before or after the call (same stream, or an event). */
 typedef struct nnb_refstage_args {
   const float* img_cur; const float* img_ref; const float* dpt_cur; const float* dpt_ref;
   const float* c2w_cur; const float* c2w_ref; const float* dist_cur; const float* dist_ref;

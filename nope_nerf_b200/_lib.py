@@ -81,6 +81,8 @@ def _load():
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,
                                        C.c_float, _f, _f, _f, _f, C.c_void_p]
     lib.nnb_chamfer.argtypes = [_f, C.c_int32, _f, C.c_int32, _f, _f, _f, _f, C.c_float, _f, _f, C.c_void_p]
+    lib.nnb_chamfer_workspace_bytes.restype = C.c_size_t
+    lib.nnb_chamfer_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
     lib.nnb_adam_step.argtypes = [_f, _f, _f, _f, C.c_int64, C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p]
     lib.nnb_profile_events.argtypes = [C.c_void_p, C.c_int32]
     lib.nnb_pose_fwd_dev.argtypes = [_f, _f, _f, _f, _f, C.c_void_p]
@@ -108,7 +110,7 @@ def _load():
 lib = _load()
 
 EXPORTS = ["nnb_last_error", "nnb_version", "nnb_profile_events", "nnb_profile_cursor", "nnb_workspace_bytes", "nnb_render_fwd", "nnb_render_bwd", "nnb_pose_fwd",
-           "nnb_pose_bwd", "nnb_loss_rgb_depth", "nnb_chamfer", "nnb_adam_step"]
+           "nnb_pose_bwd", "nnb_loss_rgb_depth", "nnb_chamfer", "nnb_chamfer_workspace_bytes", "nnb_adam_step"]
 
 
 def check(rc, what):

@@ -27,8 +27,8 @@ cudaError_t launch_incr(int*, int, cudaStream_t);
 cudaError_t launch_sample_pixels(const float*, int, int, long long*, cudaStream_t);
 cudaError_t launch_loss(const float*, const float*, const float*, const float* const*, const int64_t*, int, const float*, const float*, const uint8_t*,
                         int, float, float, int, float, float*, float*, float*, float*, const float*, cudaStream_t);
-cudaError_t launch_chamfer_full(const float*, int, const float*, int, unsigned long long*, unsigned long long*, float*, float, const float*, float*, float*,
-                                int*, int*, cudaStream_t);
+cudaError_t launch_chamfer_full(const float*, int, const float*, int, void*, float*, float, const float*, float*, float*, int*, int*, cudaStream_t);
+size_t chamfer_workspace_bytes(int P, int Q);
 cudaError_t launch_adam(float*, const float*, float*, float*, int64_t, int, float, float, float, float, cudaStream_t);
 size_t refstage_workspace_bytes(int hd, int wd, int ratio);
 size_t refstage_workspace_bytes_flags(int hd, int wd, int ratio, unsigned flags);
@@ -54,7 +54,7 @@ static int cuda_fail(cudaError_t e, const char* where) {
 extern "C" {
 
 const char* nnb_last_error(void) { return g_err; }
-int nnb_version(void) { return 100; }
+int nnb_version(void) { return 101; }   // 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys
 int nnb_profile_events(void** events, int32_t count) {
   g_prof_events = reinterpret_cast<cudaEvent_t*>(events); g_prof_n = events ? count : 0; g_prof_i = 0;
   return 0;
@@ -268,9 +268,13 @@ int nnb_chamfer(const float* X, int32_t P, const float* Y, int32_t Q, uint64_t* 
                 float* gX, float* gY, void* stream) {
   if (!X || !Y || !keys || !loss || P <= 0 || Q <= 0 || ((gX == nullptr) != (gY == nullptr)) || ((ixy == nullptr) != (iyx == nullptr)))
     return fail(-3, "nnb_chamfer: bad arguments");
-  cudaError_t e = launch_chamfer_full(X, P, Y, Q, reinterpret_cast<unsigned long long*>(keys), reinterpret_cast<unsigned long long*>(keys) + P, loss,
-                                      weight, nullptr, gX, gY, ixy, iyx, (cudaStream_t)stream);
+  cudaError_t e = launch_chamfer_full(X, P, Y, Q, keys, loss, weight, nullptr, gX, gY, ixy, iyx, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_chamfer");
+}
+
+size_t nnb_chamfer_workspace_bytes(int32_t P, int32_t Q) {
+  if (P <= 0 || Q <= 0 || (int64_t)P + Q > INT32_MAX) return 0;
+  return chamfer_workspace_bytes(P, Q);
 }
 
 size_t nnb_refstage_workspace_bytes(int32_t h_d, int32_t w_d, int32_t pc_ratio) {

@@ -185,31 +185,98 @@ __global__ void __launch_bounds__(NS_THREADS) nn_search_k(const float* __restric
   for (int j = 0; j < NS_QPT; ++j)
     if (q0 + j < na) atomicMin(keys + q0 + j, ((unsigned long long)__float_as_uint(best[j]) << 32) | (unsigned)bi[j]);
 }
-// loss += mean |a - b_nn| (+ the other direction), adjoints scattered with atomics; weight from device memory when weight_dev
-__global__ void chamfer_acc_k(const float* X, int P, const float* Y, int Q, const unsigned long long* kxy, const unsigned long long* kyx,
-                              float weight, const float* weight_dev, float* loss, float* gX, float* gY, int* ixy, int* iyx) {
+// Reduction after the search, with results fixed by the inputs alone (no float atomics).  Points are numbered in one space u in
+// [0, P + Q): X[u] for u < P, Y[u - P] after.  Every point is the source of one pair (itself -> its nearest neighbour, term
+// weight * v / (|v| * n) with v = a - b_nn) and the target of the pairs whose nearest neighbour it is; its adjoint is its own term
+// minus the sum of its group's terms.
+//   * chamfer_pairs_k: per point its own term (+= into its adjoint, one writer per element), the term in 64-bit fixed point added
+//     into its target's accumulator (integer atomics: the sum is exact, so the order of the adds cannot change a bit), and one loss
+//     partial per block (stored in the block's first key slot, which no other block reads);
+//   * chamfer_finish_k: per point, minus its accumulator rounded once to float; block 0's first warp adds up the loss partials.
+// A target that is everyone's nearest neighbour gets P same-address integer adds, as many as the float scatter had.
+constexpr int CH_THREADS = 256;
+
+// the pair term weight * v / (|v| * na) of a -> b (zero for a zero-length pair)
+__device__ __forceinline__ void pair_term(const float* A, const float* B, int i, int j, int na, float weight, float& dist, float t[3]) {
+  const float vx = __fsub_rn(A[3 * i], B[3 * j]), vy = __fsub_rn(A[3 * i + 1], B[3 * j + 1]), vz = __fsub_rn(A[3 * i + 2], B[3 * j + 2]);
+  dist = __fsqrt_rn(__fmaf_rn(vz, vz, __fmaf_rn(vy, vy, __fmul_rn(vx, vx))));
+  const float s = dist > 0.f ? __fdiv_rn(weight, __fmul_rn(dist, (float)na)) : 0.f;
+  t[0] = __fmul_rn(s, vx); t[1] = __fmul_rn(s, vy); t[2] = __fmul_rn(s, vz);
+}
+
+// Fixed point of the group sums: a finite term of a source in a cloud of na points has components of magnitude <= |weight| / na
+// (|v_c| <= |v|), and a group has at most na of them, so the terms scaled by 2^F na / |weight| with F = 62 - bits(na) and rounded to
+// integers add up in 64 bits without overflow.  Each term is rounded to a quantum of 2^-F |weight| / na (2^-48 |weight| / na at
+// na = 16 128) before the exact sum; the sum is rounded to float once.
+__device__ __forceinline__ double group_scale(int na, float weight) {
+  return weight != 0.f ? ldexp((double)na / fabs((double)weight), 62 - (32 - __clz(na))) : 0.0;
+}
+
+// keys [P + Q]: kxy then kyx.  With adjoints: acc [P + Q][3] fixed-point group sums and bad [P + Q] (bit c: a non-finite term in
+// component c), zeroed by the caller
+__global__ void __launch_bounds__(CH_THREADS) chamfer_pairs_k(const float* X, int P, const float* Y, int Q, unsigned long long* keys,
+                                                               float weight, const float* weight_dev, float* gX, float* gY, int* ixy, int* iyx,
+                                                               unsigned long long* acc, unsigned* bad) {
   __shared__ float sh[33];
-  const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool rev = i0 >= P; const int i = rev ? i0 - P : i0;
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool rev = u >= P; const int i = rev ? u - P : u;
   const float* A = rev ? Y : X; const float* B = rev ? X : Y; const int na = rev ? Q : P;
-  float* gA = rev ? gY : gX; float* gB = rev ? gX : gY;
+  float* gA = rev ? gY : gX;
   if (weight_dev) weight = *weight_dev;
   float dist = 0.f;
-  if (i0 < P + Q) {
-    const int j = (int)(unsigned)((rev ? kyx : kxy)[i] & 0xffffffffull);
+  if (u < P + Q) {
+    const int j = (int)(unsigned)(keys[u] & 0xffffffffull);
     if (ixy) (rev ? iyx : ixy)[i] = j;
-    float vx = A[3 * i] - B[3 * j], vy = A[3 * i + 1] - B[3 * j + 1], vz = A[3 * i + 2] - B[3 * j + 2];
-    dist = sqrtf(vx * vx + vy * vy + vz * vz);
-    if (gA && dist > 0.f) {
-      float s = weight / (dist * (float)na);
-      atomicAdd(gA + 3 * i, s * vx); atomicAdd(gA + 3 * i + 1, s * vy); atomicAdd(gA + 3 * i + 2, s * vz);
-      atomicAdd(gB + 3 * j, -s * vx); atomicAdd(gB + 3 * j + 1, -s * vy); atomicAdd(gB + 3 * j + 2, -s * vz);
+    float t[3];
+    pair_term(A, B, i, j, na, weight, dist, t);
+    if (gA) {
+      const int tu = rev ? j : P + j;
+      const double sc = group_scale(na, weight);
+      unsigned nf = 0;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        gA[3 * i + c] += t[c];
+        if (!isfinite(t[c])) { nf |= 1u << c; continue; }
+        const long long q = __double2ll_rn((double)t[c] * sc);
+        if (q != 0) atomicAdd(acc + 3 * (size_t)tu + c, (unsigned long long)q);
+      }
+      if (nf) atomicOr(bad + tu, nf);
     }
     dist /= (float)na;
   }
   // blocks never straddle the two directions' normalisation because dist is already divided by its own count
-  float tot = block_sum(dist, sh);
-  if (threadIdx.x == 0) atomicAdd(loss, tot);
+  const float tot = block_sum(dist, sh);        // its barriers order every read of this block's keys before the store below
+  if (threadIdx.x == 0) reinterpret_cast<float*>(keys + (size_t)blockIdx.x * CH_THREADS)[0] = tot;
+}
+
+// loss += the nb block partials, summed by one warp in a fixed order
+__device__ __forceinline__ void add_loss_partials(const unsigned long long* keys, int nb, float* loss) {
+  float s = 0.f;
+  for (int b = threadIdx.x; b < nb; b += 32) s += reinterpret_cast<const float*>(keys + (size_t)b * CH_THREADS)[0];
+  s = warp_sum(s);
+  if (threadIdx.x == 0) loss[0] += s;
+}
+__global__ void chamfer_loss_k(const unsigned long long* keys, int nb, float* loss) { add_loss_partials(keys, nb, loss); }
+
+// a component that received a non-finite term becomes NaN (the float scatter would have carried the NaN / Inf as well)
+__global__ void __launch_bounds__(CH_THREADS) chamfer_finish_k(int P, int Q, const unsigned long long* __restrict__ acc,
+                                                                const unsigned* __restrict__ bad, float weight, const float* weight_dev,
+                                                                float* gX, float* gY, const unsigned long long* keys, int nb, float* loss) {
+  if (blockIdx.x == 0 && threadIdx.x < 32) add_loss_partials(keys, nb, loss);
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= P + Q) return;
+  if (weight_dev) weight = *weight_dev;
+  const bool tx = u < P;                       // an X point's group are Y points (na = Q), and the other way round
+  const double sc = group_scale(tx ? Q : P, weight);
+  if (sc == 0.0) return;
+  float* g = tx ? gX + 3 * (size_t)u : gY + 3 * (size_t)(u - P);
+  const unsigned b = bad[u];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const long long v = (long long)acc[3 * (size_t)u + c];
+    if ((b >> c) & 1u) g[c] = __int_as_float(0x7fffffff);
+    else if (v != 0) g[c] -= (float)((double)v / sc);
+  }
 }
 
 // Learn_Distortion.forward (model/distortions.py:19-27) for a device-resident camera index:
@@ -352,13 +419,28 @@ cudaError_t launch_loss(const float* rgb, const float* rgb_gt, const float* img,
                                        w_dev);
   return cudaGetLastError();
 }
-// keys: caller scratch, 64-bit per point (P + Q entries); optional int32 index outputs for the C ABI
-cudaError_t launch_chamfer_full(const float* X, int P, const float* Y, int Q, unsigned long long* kxy, unsigned long long* kyx, float* loss,
-                                float weight, const float* weight_dev, float* gX, float* gY, int* ixy, int* iyx, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(kxy, 0xff, sizeof(unsigned long long) * (size_t)P, st);
+// Scratch of the chamfer: the search keys (64-bit, P + Q), then with adjoints acc [P + Q][3] (64-bit) and bad [P + Q] (32-bit)
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+size_t chamfer_workspace_bytes(int P, int Q) {
+  const size_t n = (size_t)P + (size_t)Q;
+  return align256(n * sizeof(unsigned long long)) + n * (3 * sizeof(unsigned long long) + sizeof(unsigned));
+}
+
+// ws: caller scratch of chamfer_workspace_bytes(P, Q) bytes, or (P + Q) 64-bit keys when gX / gY are null; optional int32 index
+// outputs for the C ABI
+cudaError_t launch_chamfer_full(const float* X, int P, const float* Y, int Q, void* ws, float* loss, float weight, const float* weight_dev,
+                                float* gX, float* gY, int* ixy, int* iyx, cudaStream_t st) {
+  const int n = P + Q;
+  unsigned long long* kxy = static_cast<unsigned long long*>(ws); unsigned long long* kyx = kxy + P;
+  cudaError_t e = cudaMemsetAsync(kxy, 0xff, sizeof(unsigned long long) * (size_t)n, st);
   if (e != cudaSuccess) return e;
-  e = cudaMemsetAsync(kyx, 0xff, sizeof(unsigned long long) * (size_t)Q, st);
-  if (e != cudaSuccess) return e;
+  unsigned long long* acc = nullptr; unsigned* bad = nullptr;
+  if (gX) {
+    acc = reinterpret_cast<unsigned long long*>(static_cast<char*>(ws) + align256((size_t)n * sizeof(unsigned long long)));
+    bad = reinterpret_cast<unsigned*>(acc + 3 * (size_t)n);
+    e = cudaMemsetAsync(acc, 0, (size_t)n * (3 * sizeof(unsigned long long) + sizeof(unsigned)), st);
+    if (e != cudaSuccess) return e;
+  }
   const int per_block = NS_THREADS * NS_QPT, mx = P > Q ? P : Q;
   const int bx = (mx + per_block - 1) / per_block;
   int splits = (2 * 148 + bx - 1) / bx;                       // ~4 resident blocks per SM over both directions
@@ -368,12 +450,15 @@ cudaError_t launch_chamfer_full(const float* X, int P, const float* Y, int Q, un
   int per_split = (mx + splits - 1) / splits;
   per_split = (per_split + 3) & ~3;
   nn_search_k<<<dim3(bx, splits, 2), NS_THREADS, 0, st>>>(X, P, Y, Q, kxy, kyx, per_split);
-  chamfer_acc_k<<<(P + Q + 255) / 256, 256, 0, st>>>(X, P, Y, Q, kxy, kyx, weight, weight_dev, loss, gX, gY, ixy, iyx);
+  const int nb = (n + CH_THREADS - 1) / CH_THREADS;
+  chamfer_pairs_k<<<nb, CH_THREADS, 0, st>>>(X, P, Y, Q, kxy, weight, weight_dev, gX, gY, ixy, iyx, acc, bad);
+  if (gX) chamfer_finish_k<<<nb, CH_THREADS, 0, st>>>(P, Q, acc, bad, weight, weight_dev, gX, gY, kxy, nb, loss);
+  else chamfer_loss_k<<<1, 32, 0, st>>>(kxy, nb, loss);
   return cudaGetLastError();
 }
-cudaError_t launch_chamfer_dev(const float* X, int P, const float* Y, int Q, unsigned long long* kxy, unsigned long long* kyx, float* loss,
-                               const float* weight_dev, float* gX, float* gY, cudaStream_t st) {
-  return launch_chamfer_full(X, P, Y, Q, kxy, kyx, loss, 1.f, weight_dev, gX, gY, nullptr, nullptr, st);
+cudaError_t launch_chamfer_dev(const float* X, int P, const float* Y, int Q, void* ws, float* loss, const float* weight_dev, float* gX, float* gY,
+                               cudaStream_t st) {
+  return launch_chamfer_full(X, P, Y, Q, ws, loss, 1.f, weight_dev, gX, gY, nullptr, nullptr, st);
 }
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int step, float lr, float b1, float b2, float eps, cudaStream_t st) {
   double bc1 = 1.0 - pow((double)b1, step), bc2 = 1.0 - pow((double)b2, step);

@@ -728,8 +728,10 @@ __global__ void ray_bwd(nnb_render_bwd_args b, const SampleRec* recs, const floa
   }
 }
 
-// warp k sums rayred[.][k] over the rays in a fixed order and adds the total to its gradient (one add per output and call; an
-// atomic one because the reference-image stage may add to g_c2w from a forked stream)
+// warp k sums rayred[.][k] over the rays in a fixed order and adds the total to its gradient: one add per output and call, so within
+// the call nothing can reorder.  The add is atomic so that other work (the reference-image stage on a forked stream) may add into the
+// same buffers at the same time and the sum stays correct; it is reproducible bit for bit when that work is ordered after this call,
+// as the Trainer does (model/training.py, _GraphStep.body_a: the stage's stream waits for the whole backward).
 __global__ void ray_reduce(nnb_render_bwd_args b, const float* __restrict__ rayred) {
   const nnb_render_args& a = b.fwd;
   const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;

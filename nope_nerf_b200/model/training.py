@@ -295,10 +295,11 @@ class _GraphStep:
         if not self.use_ref:
             call.backward(*bw, **wgk)
         else:
-            # The reference-image stage only needs the two poses / distortions / frames.  It is forked beside the weight-gradient
-            # kernel of the render backward: tc_wgrad sits on the HBM roofline with the SIMT pipes idle (192 threads, 108 registers per
-            # SM), so the brute-force chamfer's blocks run in its shadow; its pose / distortion gradients accumulate (atomics) into the
-            # buffers the render backward also accumulates into.
+            # The reference-image stage only needs the two poses / distortions / frames.  It runs on a side stream that starts after
+            # the whole render backward (this library does all of it in phase 1 and nothing in phase 2), so it sits on the step's
+            # critical path.  The stage sums in a fixed order (the chamfer's adjoint groups exactly, in integers) and adds its pose /
+            # distortion gradients once per element into the buffers the render backward also accumulates into; because the backward
+            # has finished by then, those adds always land in the same order and the step is reproducible bit for bit.
             call.backward(*bw, phase=1, **wgk)
             cur = torch.cuda.current_stream()
             self.side.wait_stream(cur)

@@ -293,9 +293,15 @@ class _ChamferFn(torch.autograd.Function):
     def forward(ctx, X, Y):
         X = _f32c(X); Y = _f32c(Y)
         P, Q = X.shape[0], Y.shape[0]
-        keys = torch.empty(P + Q, dtype=torch.int64, device=X.device)
-        loss = torch.zeros(1, device=X.device)
         need = X.requires_grad or Y.requires_grad
+        if need:                                           # the adjoints' fixed-point group sums need more scratch than the search keys
+            nbytes = L.lib.nnb_chamfer_workspace_bytes(P, Q)
+            if nbytes == 0:
+                raise RuntimeError("nnb_chamfer_workspace_bytes(%d, %d) failed" % (P, Q))
+            keys = torch.empty((nbytes + 7) // 8, dtype=torch.int64, device=X.device)
+        else:
+            keys = torch.empty(P + Q, dtype=torch.int64, device=X.device)
+        loss = torch.zeros(1, device=X.device)
         gX = torch.zeros_like(X) if need else None; gY = torch.zeros_like(Y) if need else None
         L.check(L.lib.nnb_chamfer(L.ptr(X), P, L.ptr(Y), Q, L.ptr(keys), None, None, L.ptr(loss), 1.0, L.ptr(gX), L.ptr(gY),
                                   _stream()), "nnb_chamfer")

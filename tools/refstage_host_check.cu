@@ -48,7 +48,7 @@ int main(int argc, char** argv) {
       ++nvalid;
     }
   }
-  // dense chamfer (model/losses.py:114-148), same arithmetic as nn_search_k / chamfer_acc_k
+  // dense chamfer (model/losses.py:114-148), the nearest neighbours and terms of nn_search_k / chamfer_pairs_k
   float loss_pc = 0.f;
   if (w_pc != 0.f) {
     for (int dir = 0; dir < 2; ++dir) {
