@@ -248,6 +248,39 @@ typedef struct nnb_allreduce_adam_args {
  * reduced_out and ZEROES the local gradient buffer for the next step.  Every rank must call it the same number of times. */
 int nnb_allreduce_adam(const nnb_allreduce_adam_args* args, void* stream);
 
+/* ---- training options of the whole-step CUDA graph ------------------------------------------------------------------------
+ * Each is one single-CTA launch.  Per-step values (loss weights, parameters) are read from device memory, nothing synchronises or
+ * allocates, and every sum runs in a fixed order without float atomics: the same inputs give the same bits on every run. */
+
+/* Scale / shift invariant depth term (training.depth_loss_type = invariant; Loss.depth_loss_dpt, model/losses.py:34-57) over the rays
+ * with mask[i] != 0 of the dense depth_pred / depth_gt / mask that nnb_render_fwd writes, forward and adjoint:
+ *   t = lower median (sorted position (n-1)/2 of the n masked values, as torch.median), s = mean |x - t|,
+ *   L = mean ((p - t_p) / s_p - (g - t_g) / s_g)^2.
+ * w = *w_dev (the annealed depth weight).  w == 0: nothing is read or written.  n == 0: nothing is written.  Otherwise
+ * out_losses[2] = L (overwritten) and out_losses[0] += w * L, and the seeds are ADDED (plain adds, one writer per element) on the masked
+ * rays: g_depth_pred += grad_scale * w * dL/dp, g_depth_gt (NULL = not wanted: training.detach_gt_depth) += grad_scale * w * dL/dg.
+ * The adjoint follows torch's autograd through every path: through the two mean absolute deviations (|x - t| has gradient
+ * sign(x - t), 0 at the median itself) and through the medians.  Ties at the median: like torch.median's backward, the median's
+ * gradient is split evenly over ALL masked rays whose value equals the median (+0 and -0 compare equal).  n == 1 or all masked values
+ * equal gives s = 0 and NaN, as in torch.  The masked count n lives on the device only.  One CTA: meant for the N <= 8192 rays of a
+ * training step; N <= NNB_INVARIANT_MAX_N. */
+#define NNB_INVARIANT_MAX_N 16777216
+int nnb_depth_invariant(const float* depth_pred, const float* depth_gt, const uint8_t* mask, int32_t N, const float* w_dev, float grad_scale,
+                        float* out_losses /*[4]*/, float* g_depth_pred, float* g_depth_gt, void* stream);
+/* LearnFocal.forward (model/intrinsics.py) as the camera matrix of the step (training.py:247-252): cam[16] = diag(fx', -fy', -1, 1)
+ * with (fx', fy') = (*fx, *fy) at order 1 and their squares at order 2; fy = NULL means fx_only (fy' = fx'). */
+int nnb_focal_fwd(const float* fx, const float* fy, int32_t order, float* cam, void* stream);
+/* its adjoint, ADDED into *g_fx / *g_fy: d/dfx' = g_cam[0] + g_kxy[0], d/dfy' = -(g_cam[5] + g_kxy[1]), chained through the square at
+ * order 2; with fy = g_fy = NULL (fx_only) both terms go to *g_fx.  g_cam[16] is nnb_render_bwd's camera-matrix gradient, g_kxy[2]
+ * nnb_refstage's (NULL when the reference-image stage does not run). */
+int nnb_focal_bwd(const float* fx, const float* fy, int32_t order, const float* g_cam, const float* g_kxy, float* g_fx, float* g_fy, void* stream);
+/* Pose-smoothness terms (Loss.get_weight_dist_loss, model/losses.py:103-112) of the translations t[V,3], V >= 2:
+ *   dist_i = |t_i - t_{i-1}| (i = 1..V-1), out2[0] = loss_dist_1st = mean dist, out2[1] = loss_dist_2nd = mean_{j=2..V-1} (dist_j - dist_{j-1})^2
+ * (NaN at V = 2, torch's mean over no element).  With {w1, w2} = w_dev[0..1]: loss_total (optional) += grad_scale (w1 1st + w2 2nd),
+ * g_t[V,3] (optional) += grad_scale d(w1 1st + w2 2nd)/dt (plain adds, one writer per row; a zero-length step has gradient 0, like
+ * the norm's autograd).  While w1 == w2 == 0 nothing is written. */
+int nnb_pose_smooth(const float* t, int32_t V, const float* w_dev, float grad_scale, float* out2, float* loss_total, float* g_t, void* stream);
+
 /* torch.optim.Adam step (train.py:58,99,117 defaults) over one flat buffer. step_count is the
  * 1-based step; lr/betas/eps as torch. */
 int nnb_adam_step(float* p, const float* g, float* m, float* v, int64_t n, int32_t step, float lr, float beta1,

@@ -104,6 +104,10 @@ def _load():
     lib.nnb_ipc_close.argtypes = [C.c_void_p]
     lib.nnb_ipc_free.argtypes = [C.c_void_p]
     lib.nnb_allreduce_adam.argtypes = [C.POINTER(AllreduceAdamArgs), C.c_void_p]
+    lib.nnb_depth_invariant.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_float, _f, _f, _f, C.c_void_p]
+    lib.nnb_focal_fwd.argtypes = [_f, _f, C.c_int32, _f, C.c_void_p]
+    lib.nnb_focal_bwd.argtypes = [_f, _f, C.c_int32, _f, _f, _f, _f, C.c_void_p]
+    lib.nnb_pose_smooth.argtypes = [_f, C.c_int32, _f, C.c_float, _f, _f, _f, C.c_void_p]
     return lib
 
 

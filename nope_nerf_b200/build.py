@@ -5,7 +5,7 @@ import os, subprocess, sys, shutil
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libnope_nerf_b200.so")
-SOURCES = ["nnb_api.cu", "nnb_simt.cu", "nnb_misc.cu", "nnb_tc.cu", "nnb_refstage.cu", "nnb_collective.cu"]
+SOURCES = ["nnb_api.cu", "nnb_simt.cu", "nnb_misc.cu", "nnb_tc.cu", "nnb_refstage.cu", "nnb_collective.cu", "nnb_options.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-DNNB_WITH_TC"]
 

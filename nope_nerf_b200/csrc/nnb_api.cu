@@ -34,6 +34,10 @@ size_t refstage_workspace_bytes(int hd, int wd, int ratio);
 size_t refstage_workspace_bytes_flags(int hd, int wd, int ratio, unsigned flags);
 cudaError_t launch_refstage(const nnb_refstage_args& a, cudaStream_t st);
 cudaError_t launch_allreduce_adam(const nnb_allreduce_adam_args& a, cudaStream_t st);
+cudaError_t launch_depth_invariant(const float*, const float*, const uint8_t*, int, const float*, float, float*, float*, float*, cudaStream_t);
+cudaError_t launch_focal_fwd(const float*, const float*, int, float*, cudaStream_t);
+cudaError_t launch_focal_bwd(const float*, const float*, int, const float*, const float*, float*, float*, cudaStream_t);
+cudaError_t launch_pose_smooth(const float*, int, const float*, float, float*, float*, float*, cudaStream_t);
 
 // optional profiling hook (bench.py): CUDA events recorded between the kernels of one call
 static cudaEvent_t* g_prof_events = nullptr;
@@ -343,6 +347,30 @@ int nnb_allreduce_adam(const nnb_allreduce_adam_args* a, void* stream) {
   }
   cudaError_t e = launch_allreduce_adam(*a, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_allreduce_adam");
+}
+
+int nnb_depth_invariant(const float* dp, const float* dg, const uint8_t* mask, int32_t N, const float* w_dev, float grad_scale, float* out_losses,
+                        float* g_dp, float* g_dg, void* stream) {
+  if (!dp || !dg || !mask || !w_dev || !out_losses || !g_dp || N <= 0 || N > NNB_INVARIANT_MAX_N)
+    return fail(-3, "nnb_depth_invariant: bad arguments (need 0 < N <= %d)", NNB_INVARIANT_MAX_N);
+  cudaError_t e = launch_depth_invariant(dp, dg, mask, N, w_dev, grad_scale, out_losses, g_dp, g_dg, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_depth_invariant");
+}
+int nnb_focal_fwd(const float* fx, const float* fy, int32_t order, float* cam, void* stream) {
+  if (!fx || !cam || (order != 1 && order != 2)) return fail(-3, "nnb_focal_fwd: bad arguments (order must be 1 or 2)");
+  cudaError_t e = launch_focal_fwd(fx, fy, order, cam, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_focal_fwd");
+}
+int nnb_focal_bwd(const float* fx, const float* fy, int32_t order, const float* g_cam, const float* g_kxy, float* g_fx, float* g_fy, void* stream) {
+  if (!fx || !g_cam || !g_fx || ((fy == nullptr) != (g_fy == nullptr)) || (order != 1 && order != 2))
+    return fail(-3, "nnb_focal_bwd: bad arguments (fy and g_fy both or neither; order 1 or 2)");
+  cudaError_t e = launch_focal_bwd(fx, fy, order, g_cam, g_kxy, g_fx, g_fy, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_focal_bwd");
+}
+int nnb_pose_smooth(const float* t, int32_t V, const float* w_dev, float grad_scale, float* out2, float* loss_total, float* g_t, void* stream) {
+  if (!t || !w_dev || !out2 || V < 2) return fail(-3, "nnb_pose_smooth: bad arguments (need V >= 2)");
+  cudaError_t e = launch_pose_smooth(t, V, w_dev, grad_scale, out2, loss_total, g_t, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_pose_smooth");
 }
 
 int nnb_adam_step(float* p, const float* g, float* m, float* v, int64_t n, int32_t step, float lr, float b1, float b2, float eps,

@@ -6,7 +6,7 @@ CUDA library (no autograd graph over the field):
 
     nnb_pose_fwd -> nnb_render_fwd(STASH) -> nnb_loss_rgb_depth -> nnb_render_bwd -> nnb_pose_bwd
 
-Gradients land in ONE flat fp32 buffer [MLP | r | t | scales | shifts | 4 loss scalars] whose
+Gradients land in ONE flat fp32 buffer [MLP | r | t | scales | shifts | (focal, when learned) | 4 loss scalars] whose
 slices are installed as every parameter's .grad, so (a) train.py's own torch.optim.Adam
 instances step unchanged and (b) data-parallel training is a single NCCL all-reduce of that
 buffer per step (SURVEY.md 8(e)).  The point-cloud / warped-RGB terms of the reference-image
@@ -171,13 +171,22 @@ class _GraphStep:
     to step is read from device memory: camera indices, frame pointers, DPT maps, camera matrix, loss weights (annealed per
     epoch), Adam step counters, learning rates.  The first call runs the same body eagerly (that IS that call's training step and
     warms every lazy initialisation), the second call captures, later calls replay.  With `use_ref` the reference-image stage
-    (point-cloud + warped-RGB terms, training.py:280-365) runs on a forked stream beside the render forward / backward."""
+    (point-cloud + warped-RGB terms, training.py:280-365) runs on a forked stream beside the render forward / backward.
+    Options of the trainer that add kernels to the step (each only when on, so the default step's graph is unchanged):
+      * learned focal (pose.learn_focal): the camera matrix is written from the focal parameters on the device (nnb_focal_fwd), their
+        gradient (render backward's g_cam + the reference-image stage's g_kxy) lands in the focal slot of the flat gradient buffer
+        (nnb_focal_bwd) and the focal optimizer is one more Adam segment of the exchange;
+      * invariant depth (training.depth_loss_type = invariant): nnb_depth_invariant replaces the L1 depth term and adds its seeds;
+      * pose smoothness (training.weight_dist_1st_loss / weight_dist_2nd_loss): nnb_pose_smooth adds its translation gradient."""
 
     def __init__(self, tr, h, w, hd, wd, rgb_l2, use_ref):
         self.tr = tr; self.key = (h, w, hd, wd, bool(rgb_l2), bool(use_ref))
         dev = tr.device
         self.h, self.w, self.hd, self.wd = h, w, hd, wd
         self.rgb_l2, self.use_ref = bool(rgb_l2), bool(use_ref)
+        self.focal = tr.optimizer_focal is not None
+        self.inv = tr.depth_loss_type == 'invariant'
+        self.smooth = tr._smoothness_on()
         # per-step host scalars travel as ONE 32-byte asynchronous copy from a ring of page-locked slots:
         # meta = int64 [camera index, reference camera index, frame pointer, reference frame pointer]
         self.meta = torch.zeros(4, dtype=torch.int64, device=dev)
@@ -192,9 +201,16 @@ class _GraphStep:
         self.ss = torch.zeros(2, device=dev)               # effective (scale, shift) of the current view
         self.c2w = torch.zeros(4, 4, device=dev)
         self.small = torch.zeros(16 + 2, device=dev)       # [g_c2w | g_scale_shift]
-        self.steps = torch.zeros(3, dtype=torch.int32, device=dev)   # Adam step counters: mlp, pose, distortion
-        self.lrs = torch.zeros(3, device=dev); self.lr_host = [None, None, None]
-        self.wts = torch.zeros(4, device=dev); self.wts_host = None  # {w_rgb, w_depth, w_pc, w_rgb_s}
+        n_opt = 4 if self.focal else 3
+        self.steps = torch.zeros(n_opt, dtype=torch.int32, device=dev)   # Adam step counters: mlp, pose, distortion[, focal]
+        self.lrs = torch.zeros(n_opt, device=dev); self.lr_host = [None] * n_opt
+        # {w_rgb, w_depth (L1), w_pc, w_rgb_s, w_dist_1st, w_dist_2nd, w_depth (invariant), 0}
+        self.wts = torch.zeros(8, device=dev); self.wts_host = None
+        if self.focal:
+            self.cam_gt = torch.zeros(4, 4, device=dev)          # the dataset's camera matrix (loss_dict['focalx'/'focaly'])
+            self.g_focal = torch.zeros(16 + 2, device=dev)       # [g_cam | g_kxy]
+        if self.smooth:
+            self.dist_losses = torch.zeros(2, device=dev)        # {loss_dist_1st, loss_dist_2nd}
         self.out4 = torch.zeros(4, device=dev)
         N = tr.n_training_points // tr.world if tr.dp_mode == 'rays' else tr.n_training_points
         self.g_rgb = torch.zeros(N, 3, device=dev); self.g_dp = torch.zeros(N, device=dev); self.g_dg = torch.zeros(N, device=dev)
@@ -222,7 +238,18 @@ class _GraphStep:
         if self.fadams is None:
             self.fadams = [tr._fadam_for(tr.optimizer, True), tr._fadam_for(tr.optimizer_pose, False),
                            tr._fadam_for(tr.optimizer_distortion, False)]
+            if self.focal:
+                self.fadams.append(tr._fadam_for(tr.optimizer_focal, False))
         return self.fadams
+
+    def _optimizers(self):
+        tr = self.tr
+        return (tr.optimizer, tr.optimizer_pose, tr.optimizer_distortion) + ((tr.optimizer_focal,) if self.focal else ())
+
+    def _focal_params(self):
+        """(fx, fy or None (fx_only), order) of the LearnFocal module"""
+        fn = self.tr.focal_net
+        return fn.fx, (None if fn.fx_only else fn.fy), int(fn.order)
 
     def eligible_optimizers(self):
         return all(fa.ok for fa in self._adams())
@@ -240,12 +267,16 @@ class _GraphStep:
         net = tr.model.renderer.model; pose, dnet = tr.pose_param_net, tr.distortion_net
         V = pose.num_cams; o = net.num_params
         ops.counter_incr(self.steps)
-        fa_m, fa_p, fa_d = self._adams()
+        fa_m, fa_p, fa_d = self._adams()[:3]
         gm = tr.optimizer.param_groups[0]; b1, b2 = gm['betas']
         segs = [(net.flat_weights(), fa_m.m, fa_m.v, 0, o, self.lrs[0:1], self.steps[0:1], b1, b2, gm['eps'])]
         gp = tr.optimizer_pose.param_groups[0]; gd = tr.optimizer_distortion.param_groups[0]
-        for prm, off, cnt, fa, g_, k in ((pose.r, o, 3 * V, fa_p, gp, 1), (pose.t, o + 3 * V, 3 * V, fa_p, gp, 1),
-                                         (dnet.global_scales, o + 6 * V, V, fa_d, gd, 2), (dnet.global_shifts, o + 7 * V, V, fa_d, gd, 2)):
+        groups = [(pose.r, o, 3 * V, fa_p, gp, 1), (pose.t, o + 3 * V, 3 * V, fa_p, gp, 1),
+                  (dnet.global_scales, o + 6 * V, V, fa_d, gd, 2), (dnet.global_shifts, o + 7 * V, V, fa_d, gd, 2)]
+        if self.focal:                                      # focal slot [fx, fy] after the shifts
+            fx, fy, _ = self._focal_params(); fa_f = self._adams()[3]; gf = tr.optimizer_focal.param_groups[0]
+            groups += [(fx, o + 8 * V, 1, fa_f, gf, 3)] + ([(fy, o + 8 * V + 1, 1, fa_f, gf, 3)] if fy is not None else [])
+        for prm, off, cnt, fa, g_, k in groups:
             if prm.requires_grad and id(prm) in fa.m:
                 segs.append((prm.data, fa.m[id(prm)], fa.v[id(prm)], off, cnt, self.lrs[k:k + 1], self.steps[k:k + 1], g_['betas'][0], g_['betas'][1], g_['eps']))
         tr._peer.allreduce_adam(segs)
@@ -262,6 +293,13 @@ class _GraphStep:
         grad_ref = self.use_ref and self.grad_ref
         if grad_ref:
             self.small_ref.zero_()
+        g_cam = g_kxy = None
+        if self.focal:                                      # camera matrix from the focal parameters (training.py:247-252)
+            fx, fy, order = self._focal_params()
+            ops.focal_fwd(fx.detach(), None if fy is None else fy.detach(), order, self.cam)
+            self.g_focal.zero_()
+            g_cam = self.g_focal[:16].view(4, 4)
+            g_kxy = self.g_focal[16:18] if self.use_ref else None
         ops.distortion_fwd_dev(dnet.global_scales.detach(), dnet.global_shifts.detach(), self.idx, dnet.fix_scaleN, self.ss)
         init = None if pose.init_c2w is None else pose.init_c2w.detach()
         ops.pose_fwd_dev(pose.r.detach(), pose.t.detach(), init, self.idx, self.c2w)
@@ -288,9 +326,12 @@ class _GraphStep:
                               hidden_dim=net.hidden_dim)
         ops.loss_rgb_depth_indirect(call.rgb, call.depth_pred, call.depth_gt, call.mask, 0.0, 0.0, self.rgb_l2, self.imgpp,
                                     ray_idx, h * w, self.out4, self.g_rgb, self.g_dp, self.g_dg, grad_scale=gs, w_dev=self.wts)
+        if self.inv:                                        # losses.py:34-57 (the L1 depth weight on the device is 0)
+            ops.depth_invariant(call.depth_pred, call.depth_gt, call.mask, self.wts[6:7], self.out4, self.g_dp,
+                                None if tr.detach_gt_depth else self.g_dg, grad_scale=gs)
         ws = call.ws
         call.pooled = False                                 # memory referenced by a captured graph never returns to the pool
-        bw = (self.g_rgb, self.g_dp, None if tr.detach_gt_depth else self.g_dg, gbuf[:net.num_params], g_c2w, None, None, g_ss)
+        bw = (self.g_rgb, self.g_dp, None if tr.detach_gt_depth else self.g_dg, gbuf[:net.num_params], g_c2w, g_cam, None, g_ss)
         wgk = tr._wg_kwargs()
         if not self.use_ref:
             call.backward(*bw, **wgk)
@@ -313,7 +354,7 @@ class _GraphStep:
                                  pc_ratio=tr.pc_ratio, scale_pcs=tr.scale_pcs, detach_rgbs_scale=tr.detach_rgbs_scale, shift_first=tr.shift_first,
                                  losses=self.rs_losses, g_c2w=g_c2w, g_dist=g_ss, loss_total=self.rs_total, grad_scale=gs, workspace=self.rs_ws,
                                  with_ssim=self.with_ssim, g_c2w_ref=self.small_ref[:16].view(4, 4) if grad_ref else None,
-                                 g_dist_ref=self.small_ref[16:18] if grad_ref else None)
+                                 g_dist_ref=self.small_ref[16:18] if grad_ref else None, g_kxy=g_kxy)
             cur.wait_stream(self.side)
         self.keep.append((call, ws, ray_idx, noise))        # graph-owned memory stays referenced (and out of the workspace pool)
         ops.pose_bwd_dev(pose.r.detach(), pose.t.detach(), init, self.idx, g_c2w,
@@ -327,9 +368,14 @@ class _GraphStep:
             ops.distortion_bwd_dev(dnet.global_scales.detach(), self.idx_ref, dnet.fix_scaleN, self.small_ref[16:18],
                                    gv['scales'] if dnet.global_scales.requires_grad else None,
                                    gv['shifts'] if dnet.global_shifts.requires_grad else None)
+        if self.focal:                                      # after the reference-image stage's g_kxy (fixed order)
+            ops.focal_bwd(fx.detach(), None if fy is None else fy.detach(), order, g_cam, g_kxy, gv['fx'], gv.get('fy'))
         gv['losses'].copy_(self.out4 * gs if tr.world > 1 else self.out4)
         if self.use_ref:
             gv['losses'][0:1].add_(self.rs_total, alpha=gs)
+        if self.smooth:                                     # losses.py:103-112; every rank holds the same t: 1/world of it each
+            ops.pose_smooth(pose.t.detach(), self.wts[4:6], self.dist_losses, loss_total=gv['losses'][0:1],
+                            g_t=gv['t'] if pose.t.requires_grad else None, grad_scale=gs)
 
     def reduce(self):
         tr = self.tr
@@ -342,11 +388,13 @@ class _GraphStep:
         gbuf = tr._gbuf
         net = tr.model.renderer.model
         ops.counter_incr(self.steps)
-        fa_m, fa_p, fa_d = self._adams()
+        fas = self._adams(); fa_m = fas[0]
         gm = tr.optimizer.param_groups[0]; b1, b2 = gm['betas']
         flat = net.flat_weights()
         ops.adam_step_dev(flat, gbuf[:net.num_params], fa_m.m, fa_m.v, self.steps[0:1], self.lrs[0:1], b1, b2, gm['eps'])
-        for fa, opt, k in ((fa_p, tr.optimizer_pose, 1), (fa_d, tr.optimizer_distortion, 2)):
+        for k, (fa, opt) in enumerate(zip(fas, self._optimizers())):
+            if k == 0:
+                continue
             g = opt.param_groups[0]; b1, b2 = g['betas']
             for p in g['params']:
                 if p.requires_grad and p.grad is not None:
@@ -388,20 +436,20 @@ class _GraphStep:
         self.dev_refs = keep
         cm = data.get('img.camera_mat')
         cm_key = (cm.data_ptr(), cm._version)
+        cam = self.cam_gt if self.focal else self.cam          # learned focal: the step's camera matrix comes from nnb_focal_fwd
         if cm.device.type == 'cpu' and self.cam_host is not None and getattr(self, 'cam_key', None) == cm_key:
             pass                                              # same host tensor as last step, unmodified
         elif self.cam_host is None or (cm.device.type == 'cpu' and not torch.equal(cm.reshape(4, 4), self.cam_host)):
             _host_diag_check(cm)
             self.cam_host = cm.reshape(4, 4).clone() if cm.device.type == 'cpu' else None
-            self.cam.copy_(cm.reshape(4, 4))
+            cam.copy_(cm.reshape(4, 4))
         elif cm.device.type != 'cpu':
-            self.cam.copy_(cm.reshape(4, 4))
+            cam.copy_(cm.reshape(4, 4))
         self.cam_key = cm_key
         if self.wts_host != wts:
             self.wts.copy_(torch.tensor(wts, dtype=torch.float32)); self.wts_host = list(wts)
         fas = self._adams()
-        opts = (tr.optimizer, tr.optimizer_pose, tr.optimizer_distortion)
-        for k, (fa, opt) in enumerate(zip(fas, opts)):
+        for k, (fa, opt) in enumerate(zip(fas, self._optimizers())):
             fa.ensure_state()
             lr = float(opt.param_groups[0]['lr'])
             if self.lr_host[k] != lr:
@@ -445,14 +493,25 @@ class _GraphStep:
                 self.ev_pool.append(self.host_refs.pop(0)[1])
         # per-call snapshot (ONE small kernel): later steps overwrite the persistent buffers the graph writes to, and train.py
         # keeps loss_dict['scale'/'shift'] per view (train.py:215-216)
-        snap = torch.cat([(tr._peer.reduced if tr._peer is not None else tr._gbuf)[-4:], self.ss, self.rs_losses])
+        parts = [(tr._peer.reduced if tr._peer is not None else tr._gbuf)[-4:], self.ss, self.rs_losses]
+        if self.smooth:
+            parts.append(self.dist_losses)
+        if self.focal:                                        # {fx', -fy'} of this step's camera matrix over the dataset's {kx, ky}
+            parts.append(self.cam.view(16)[0:6:5] / self.cam_gt.view(16)[0:6:5])
+        snap = torch.cat(parts)
         s_ = snap.unbind(0)
         if getattr(self, 'zero', None) is None:
             self.zero = snap.new_zeros(())
         zero = self.zero
-        return {'loss': s_[0], 'loss_rgb': s_[1], 'loss_depth': s_[2], 'l2_mean': s_[3],
-                'loss_dist_1st': zero, 'loss_dist_2nd': zero, 'loss_pc': s_[6] if wts[2] != 0.0 else zero,
-                'loss_rgb_s': s_[7] if wts[3] != 0.0 else zero, 'loss_depth_consistency': zero, 'scale': snap[4:5], 'shift': snap[5:6]}
+        ld = {'loss': s_[0], 'loss_rgb': s_[1], 'loss_depth': s_[2], 'l2_mean': s_[3],
+              'loss_dist_1st': zero, 'loss_dist_2nd': zero, 'loss_pc': s_[6] if wts[2] != 0.0 else zero,
+              'loss_rgb_s': s_[7] if wts[3] != 0.0 else zero, 'loss_depth_consistency': zero, 'scale': snap[4:5], 'shift': snap[5:6]}
+        if self.smooth and (wts[4] != 0.0 or wts[5] != 0.0):
+            ld['loss_dist_1st'], ld['loss_dist_2nd'] = s_[8], s_[9]
+        if self.focal:
+            j = 10 if self.smooth else 8
+            ld['focalx'], ld['focaly'] = s_[j], -s_[j + 1]
+        return ld
 
 
 class Trainer(object):
@@ -489,7 +548,7 @@ class Trainer(object):
         self.depth_consistency_weight = cfg['depth_consistency_weight']
         if cfg['depth_loss_type'] not in ('l1', 'invariant'):
             raise ValueError("training.depth_loss_type must be 'l1' or 'invariant' (losses.py:59-64)")
-        self.depth_loss_type = cfg['depth_loss_type']     # 'invariant' (median / mean-abs-deviation normalised, losses.py:34-57) takes the general path
+        self.depth_loss_type = cfg['depth_loss_type']     # 'invariant': median / mean-abs-deviation normalised (losses.py:34-57)
         self.loss = Loss(cfg)
         # ---- data parallel (new component, SURVEY.md 8(e)) ----
         self.dp_group = kwargs.get('process_group', None)
@@ -532,13 +591,31 @@ class Trainer(object):
         self._wg_seeded = True
         return kw
 
+    def _smoothness_on(self):
+        """the pose-smoothness terms have a non-zero weight somewhere on their annealing schedule"""
+        return any(float(v) != 0.0 for v in list(self.weight_dist_1st_loss) + list(self.weight_dist_2nd_loss))
+
+    def _focal_graphable(self):
+        """a LearnFocal module whose fx (and fy) are exactly the parameters of the focal optimizer"""
+        fn = self.focal_net
+        if fn is None or getattr(fn, 'order', None) not in (1, 2) or not isinstance(getattr(fn, 'fx', None), torch.nn.Parameter):
+            return False
+        prm = [fn.fx] if fn.fx_only else [fn.fx, getattr(fn, 'fy', None)]
+        if any(p is None or p.numel() != 1 or p.dtype != torch.float32 or not p.is_cuda for p in prm):
+            return False
+        groups = self.optimizer_focal.param_groups
+        return len(groups) == 1 and [id(p) for p in groups[0]['params']] == [id(p) for p in prm]
+
     def _grad_buffer(self, peer_step=False):
-        """[MLP (595844 floats at hidden_dim 256) | r 3V | t 3V | scales V | shifts V | loss scalars 4], zeroed; the kernels accumulate into it.
+        """[MLP (595844 floats at hidden_dim 256) | r 3V | t 3V | scales V | shifts V | [fx, fy, 0, 0] | loss scalars 4], zeroed; the kernels
+        accumulate into it.  The focal slot exists only with a learned focal (graph steps install it as the focal parameters' .grad; the
+        general path keeps their autograd .grad).
         Installed as every parameter's .grad -- except in a peer-exchange step (data parallel, nnb_allreduce_adam), where .grad
         shows the buffer that receives the SUM over the ranks while the local contributions go to the IPC-shared buffer."""
         V = self.pose_param_net.num_cams if self.pose_param_net is not None else 0
         n_mlp = self.model.renderer.model.num_params
-        n = n_mlp + 8 * V + 4
+        n_focal = 4 if self.optimizer_focal else 0
+        n = n_mlp + 8 * V + n_focal + 4
         dev = self.device
         if self._gbuf is None or self._gbuf.numel() != n:
             if self.peer_exchange and torch.device(dev).type == 'cuda' and (self.world > 1 or self.fused_adam):
@@ -561,10 +638,17 @@ class Trainer(object):
                 v['r'] = buf[o:o + 3 * V].view(V, 3); v['t'] = buf[o + 3 * V:o + 6 * V].view(V, 3)
             if self.distortion_net is not None:
                 v['scales'] = buf[o + 6 * V:o + 7 * V].view(V, 1); v['shifts'] = buf[o + 7 * V:o + 8 * V].view(V, 1)
+            if n_focal:
+                v['fx'] = buf[o + 8 * V]
+                if not getattr(self.focal_net, 'fx_only', True): v['fy'] = buf[o + 8 * V + 1]
             v['losses'] = buf[n - 4:]
             return v
         views = split(g)
         sv = views if shown is g else split(shown)
+        if n_focal and peer_step:
+            for k in ('fx', 'fy'):
+                prm = getattr(self.focal_net, k, None)
+                if k in sv and prm.requires_grad: prm.grad = sv[k]
         net.flat_grad(zero=False, alias=shown[:o])
         if self.pose_param_net is not None:
             if self.pose_param_net.r.requires_grad: self.pose_param_net.r.grad = sv['r']
@@ -579,12 +663,12 @@ class Trainer(object):
         # (nn.Module.train() walks every submodule: ~60 us of host time per step -- only when the mode actually changes)
         if not self.model.training: self.model.train()
         if self.pose_param_net and not self.pose_param_net.training: self.pose_param_net.train()
-        if self.focal_net:
-            self.focal_net.train(); self.optimizer_focal.zero_grad()
+        if self.focal_net: self.focal_net.train()
         if self.distortion_net and not self.distortion_net.training: self.distortion_net.train()
         gs = self._graph_step_or_none(data, epoch, scheduling_start)
         if gs is not None:
             return gs[0].run(data, gs[1])          # fixed kernel sequence; replayed as one CUDA graph when use_cuda_graph
+        if self.focal_net: self.optimizer_focal.zero_grad()     # (graph steps keep the focal slot of the gradient buffer as .grad)
         loss_dict = self.compute_loss(data, it=it, epoch=epoch, scheduling_start=scheduling_start,
                                       out_render_path=render_path, backward=True)
         self._opt_step(self.optimizer, mlp=True)
@@ -611,17 +695,22 @@ class Trainer(object):
 
     def _graph_step_or_none(self, data, epoch, scheduling_start):
         """fast path: the whole step as one fixed kernel sequence / CUDA graph.  Returns (graph step, device weights) or None for
-        configurations that take the general path (learnable focal, pose-smoothness terms, no render terms, foreign optimizers)."""
-        if not self.fused_adam or self.optimizer_focal or self.pose_param_net is None or self.distortion_net is None:
+        configurations that take the general path (no render terms, foreign optimizers or focal modules, invariant depth with the rays
+        of one view sharded over ranks -- its median is over the whole batch)."""
+        if not self.fused_adam or self.pose_param_net is None or self.distortion_net is None:
             return None
-        if self.depth_loss_type != 'l1':
+        if (self.optimizer_focal or self.depth_loss_type == 'invariant' or self._smoothness_on()) and not self.use_cuda_graph:
+            return None          # eager trainers keep these options on the general path (torch autograd / median / Adam)
+        if self.optimizer_focal and not self._focal_graphable():
+            return None
+        if self.depth_loss_type == 'invariant' and self.world > 1 and self.dp_mode == 'rays':
             return None
         if self.optimizer_pose is None or self.optimizer_distortion is None:
             return None
         names = ['rgb_weight', 'depth_weight', 'pc_weight', 'rgb_s_weight', 'depth_consistency_weight', 'weight_dist_2nd_loss',
                  'weight_dist_1st_loss']
         wts = {n: self.anneal(getattr(self, n)[0], getattr(self, n)[1], scheduling_start, self.annealing_epochs, epoch) for n in names}
-        if any(wts[n] != 0.0 for n in names[4:]) or (wts['rgb_weight'] == 0.0 and wts['depth_weight'] == 0.0):
+        if wts['depth_consistency_weight'] != 0.0 or (wts['rgb_weight'] == 0.0 and wts['depth_weight'] == 0.0):
             return None
         use_ref = wts['pc_weight'] != 0.0 or wts['rgb_s_weight'] != 0.0
         if use_ref:
@@ -642,7 +731,10 @@ class Trainer(object):
             self._gsteps[key] = gs
         if gs is False:
             return None
-        return gs, [float(wts['rgb_weight']), float(wts['depth_weight']), float(wts['pc_weight']), float(wts['rgb_s_weight'])]
+        inv = self.depth_loss_type == 'invariant'
+        w_depth = float(wts['depth_weight'])
+        return gs, [float(wts['rgb_weight']), 0.0 if inv else w_depth, float(wts['pc_weight']), float(wts['rgb_s_weight']),
+                    float(wts['weight_dist_1st_loss']), float(wts['weight_dist_2nd_loss']), w_depth if inv else 0.0, 0.0]
 
     def graph_kernel_nodes(self):
         """{kernels, memcpy, memset, other} node counts of the captured step graph(s) (needs Trainer(keep_graph=True)); None if no

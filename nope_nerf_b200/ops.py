@@ -464,6 +464,35 @@ def loss_rgb_depth_indirect(rgb, depth_pred, depth_gt, mask, w_rgb, w_depth, rgb
                                               L.ptr(g_rgb), L.ptr(g_dp), L.ptr(g_dg), L.ptr(w_dev), _stream()), "nnb_loss_rgb_depth_indirect")
 
 
+def depth_invariant(depth_pred, depth_gt, mask, w_dev, out, g_dp, g_dg=None, grad_scale=1.0):
+    """scale / shift invariant depth term (Loss.depth_loss_dpt over the masked rays) with weight w_dev[0]: out[2] = the term,
+    out[0] += w * term, g_dp / g_dg (None: detached ground truth) += grad_scale * w * its seeds"""
+    for n_, t_ in (("depth_pred", depth_pred), ("depth_gt", depth_gt), ("mask", mask), ("w_dev", w_dev), ("out", out), ("g_dp", g_dp)):
+        _need_cuda(t_, n_)
+    L.check(L.lib.nnb_depth_invariant(L.ptr(depth_pred), L.ptr(depth_gt), L.ptr(mask), int(depth_pred.shape[0]), L.ptr(w_dev), float(grad_scale),
+                                      L.ptr(out), L.ptr(g_dp), L.ptr(g_dg), _stream()), "nnb_depth_invariant")
+
+
+def focal_fwd(fx, fy, order, cam):
+    """cam (4,4) = diag(fx', -fy', -1, 1) of LearnFocal (fy None: fx_only)"""
+    _need_cuda(fx, "fx")
+    L.check(L.lib.nnb_focal_fwd(L.ptr(fx), L.ptr(fy), int(order), L.ptr(cam), _stream()), "nnb_focal_fwd")
+
+
+def focal_bwd(fx, fy, order, g_cam, g_kxy, g_fx, g_fy):
+    """g_fx / g_fy += the focal parameters' gradient from the camera-matrix gradient g_cam (4,4) and g_kxy (2,) (or None)"""
+    _need_cuda(fx, "fx")
+    L.check(L.lib.nnb_focal_bwd(L.ptr(fx), L.ptr(fy), int(order), L.ptr(g_cam), L.ptr(g_kxy), L.ptr(g_fx), L.ptr(g_fy), _stream()), "nnb_focal_bwd")
+
+
+def pose_smooth(t, w_dev, out2, loss_total=None, g_t=None, grad_scale=1.0):
+    """pose-smoothness terms of the translations t (V,3) with weights w_dev[0:2]: out2 = {loss_dist_1st, loss_dist_2nd},
+    loss_total += grad_scale * (w1 1st + w2 2nd), g_t += grad_scale * its gradient"""
+    _need_cuda(t, "t")
+    L.check(L.lib.nnb_pose_smooth(L.ptr(t), int(t.shape[0]), L.ptr(w_dev), float(grad_scale), L.ptr(out2), L.ptr(loss_total), L.ptr(g_t), _stream()),
+            "nnb_pose_smooth")
+
+
 def sample_pixels(hw, n, device):
     """n distinct pixel ids uniform in [0, hw) (distribution of torch.randperm(hw)[:n])"""
     u = torch.rand(2 * n, device=device)
