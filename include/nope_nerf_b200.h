@@ -38,6 +38,7 @@ extern "C" {
 #define NNB_FWD_DROP_WLO 4096u /* forward precision experiment: rejected (rc -7) by this library */
 #define NNB_FWD_DROP_ALO 8192u /* forward precision experiment: rejected (rc -7) by this library */
 #define NNB_WG16 1024u      /* with NNB_TCBWD only (fp16 weight-gradient operand planes); without it the flag has no effect */
+#define NNB_HVP 16384u      /* with NNB_STASH on NNB_ENGINE_SIMT: the workspace also holds the tangent stash of nnb_field_hvp; sizes only */
 
 /* engines */
 #define NNB_ENGINE_SIMT 0 /* exact fp32 FMA path                                        */
@@ -103,7 +104,7 @@ typedef struct nnb_render_bwd_args {
 } nnb_render_bwd_args;
 
 const char* nnb_last_error(void);
-int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys */
+int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys; >= 102: nnb_field_hvp */
 /* Profiling hook used by bench.py: `events` is a HOST array of cudaEvent_t handles that stays alive until
  * nnb_profile_events(NULL,0).  Every nnb_render_fwd records 4 marks (start, weights imaged, field done,
  * composited) and every nnb_render_bwd 5 marks (start, compositing adjoint, data-gradient chain,
@@ -130,6 +131,14 @@ int nnb_render_fwd(const nnb_render_args* a, void* stream);
  * g_weights (+=, may be NULL). */
 int nnb_field_fwd(const nnb_render_args* a, float* out_rgba, void* stream);
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream);
+/* Second-order backward of the surface normal n(p) = d s / d p, s the density logit (OfficialStaticNerf.gradient with
+ * create_graph=True, official_nerf.py:46-58): for a cotangent u [N,4] (xyz used) on n, with s' = u . n,
+ *   g_pts [N,4] = d s' / d p (xyz; overwritten; may be NULL),  g_weights += sum over the points of d s' / d weights (may be NULL).
+ * Recomputes everything from a->pts and a->weights (forward, data-gradient chain, tangent chain, weight gradients); reads a->pts, N,
+ * weights, hidden_dim, workspace.  a->flags must contain NNB_STASH | NNB_HVP and the workspace be sized by
+ * nnb_workspace_bytes_dim(N, 1, flags, NNB_ENGINE_SIMT, hidden_dim); dirs and the activation flags do not enter (the logit is raw).
+ * u and g_pts are 16-byte aligned.  Exact-fp32 engine; every sum runs in a fixed order, so the same inputs give the same bits. */
+int nnb_field_hvp(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream);
 int nnb_render_bwd(const nnb_render_bwd_args* a, void* stream);
 
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */

@@ -13,6 +13,7 @@ NUM_PARAMS = 595844              # hidden_dim 256; num_params(D) for the other w
 HIDDEN_DIMS = (64, 128, 256)     # model.hidden_dim values with a kernel instantiation
 DIST_ALPHA, NDC, NORMALISE, USE_DIR, WHITE_BG, EVAL, SOFTPLUS, SHIFT_FIRST, STASH, TCBWD, WG16, RAW_DENSITY = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048
 FWD_DROP_WLO, FWD_DROP_ALO = 4096, 8192
+HVP = 16384                      # with STASH: workspace of nnb_field_hvp (second-order field backward)
 ENGINE_SIMT, ENGINE_TC = 0, 1
 RS_SCALE_PCS, RS_DETACH_RGBS_SCALE, RS_SHIFT_FIRST, RS_WITH_SSIM, RS_GRAD_REF = 1, 2, 4, 8, 16   # nnb_refstage_args.flags
 
@@ -76,6 +77,7 @@ def _load():
     lib.nnb_debug_wgrad.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]   # test aid
     lib.nnb_field_fwd.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]
     lib.nnb_field_bwd.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, C.c_void_p]
+    lib.nnb_field_hvp.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, C.c_void_p]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]
     lib.nnb_pose_bwd.argtypes = [_f, _f, _f, C.c_int32, _f, _f, _f, C.c_void_p]
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,

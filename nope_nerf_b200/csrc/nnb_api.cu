@@ -10,6 +10,7 @@ cudaError_t simt_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cud
 cudaError_t simt_field_fwd(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st);
 cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights,
                            cudaStream_t st);
+cudaError_t simt_field_hvp(const nnb_render_args& a, const WsLayout& L, const float* u, float* g_pts, float* g_weights, cudaStream_t st);
 cudaError_t simt_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
@@ -58,7 +59,7 @@ static int cuda_fail(cudaError_t e, const char* where) {
 extern "C" {
 
 const char* nnb_last_error(void) { return g_err; }
-int nnb_version(void) { return 101; }   // 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys
+int nnb_version(void) { return 102; }   // 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys; 102: nnb_field_hvp
 int nnb_profile_events(void** events, int32_t count) {
   g_prof_events = reinterpret_cast<cudaEvent_t*>(events); g_prof_n = events ? count : 0; g_prof_i = 0;
   return 0;
@@ -199,6 +200,19 @@ int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, f
   cudaError_t e = simt_field_bwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT, hidden_of(b.hidden_dim)), g_rgba, g_pts, g_dirs, g_weights,
                                  (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_bwd");
+}
+int nnb_field_hvp(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream) {
+  int rc = check_field(a); if (rc) return rc;
+  if (!u || (!g_pts && !g_weights)) return fail(-3, "nnb_field_hvp: need u and at least one of g_pts, g_weights");
+  if (!(a->flags & NNB_STASH) || !(a->flags & NNB_HVP) || (a->flags & NNB_TCBWD))
+    return fail(-6, "nnb_field_hvp: flags must contain NNB_STASH | NNB_HVP (without NNB_TCBWD), and the workspace be sized with them");
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(u) & 15) != 0 || (reinterpret_cast<uintptr_t>(g_pts) & 15) != 0)
+    return fail(-3, "nnb_field_hvp: u and g_pts must be 16-byte aligned [N][4] arrays");
+  nnb_render_args b = *a; b.S = 1; b.engine = NNB_ENGINE_SIMT; b.flags |= NNB_RAW_DENSITY;
+  cudaError_t e = simt_field_hvp(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT, hidden_of(b.hidden_dim)), u, g_pts, g_weights,
+                                 (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_hvp");
 }
 
 int nnb_pose_fwd(const float* r, const float* t, const float* init, int32_t cam, float* c2w, void* stream) {

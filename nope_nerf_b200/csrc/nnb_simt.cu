@@ -445,6 +445,118 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, Simt
 }
 
 // ---------------------------------------------------------------------------------------
+// H: second-order field backward (nnb_field_hvp, DESIGN.md §4).  For a cotangent u on n = d s / d p, s' = u . n is the derivative
+// of the logit along u: the tangent chain e' = J_enc(p) u, z'_l = W_l x'_{l-1} (no bias; [h'3 | e'] into layer 4), h'_l = [h_l > 0] z'_l,
+// s' = w_sigma . h'7.  The ReLU masks are piecewise constant, so d s' / d W_l = dy_l (x) x'_{l-1} with dy_l the gated output gradient
+// of the data-gradient chain for a cotangent 1 on the logit, d s' / d w_sigma = h'7, no bias term, and d s' / d p only the encoding's
+// own second derivative.
+// ---------------------------------------------------------------------------------------
+struct TangentPtrs {
+  float* th[8]; float* tenc;   // tangent stash [Mpad][D] / [Mpad][64]
+  const float4* u;             // [M] cotangent on n (xyz)
+  float4* gp;                  // [M] d s' / d p, or nullptr
+};
+
+// cotangent (0, 0, 0, 1) on out_rgba: 1 on the logit (NNB_RAW_DENSITY)
+__global__ void logit_seed(float4* gs, size_t M) {
+  const size_t m = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (m < M) gs[m] = make_float4(0.f, 0.f, 0.f, 1.f);
+}
+
+// one 64-row tile: e' and h'0..h'7 into the tangent stash (whole tile, Mpad rows), then delta_enc = dy4 W4[:, D:] + dy0 W0 (the data-
+// gradient kernel's order) and the point term, written for rows m < M only.  Reads the stash of simt_mlp_fwd (h) and simt_mlp_dgrad (dy).
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_field_tangent(nnb_render_args a, SimtPtrs P, TangentPtrs T, size_t M) {
+  constexpr int LDB = ldb<D>(), NJ = D / 64;
+  extern __shared__ __align__(16) float smem[];
+  float* buf0 = smem; float* buf1 = buf0 + TM * LDB; float* Ws = buf1 + TM * LDB;
+  float* genc = Ws + 2 * KC * WS_LD;          // [64][64]
+  const int tid = threadIdx.x;
+  const size_t m0 = (size_t)blockIdx.x * TM;
+  const float* w = a.weights;
+  {  // 1. e' = J_enc(p) u into columns D..D+63 of both buffers (tail rows: u = 0)
+    const int row = tid & 63, part = tid >> 6;
+    const size_t m = m0 + row;
+    Ray ray; int n, i; float z, p[3];
+    row_geometry(a, m, M, ray, n, i, z, p);
+    const float4 uv = m < M ? T.u[m] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float u[3] = {uv.x, uv.y, uv.z};
+    float* e0 = buf0 + row * LDB + D; float* e1 = buf1 + row * LDB + D;
+    if (part == 0) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { e0[c] = u[c]; e1[c] = u[c]; }
+      e0[63] = 0.f; e1[63] = 0.f;
+    }
+    for (int l = part; l < 10; l += 4) {
+      const float f = (float)(1 << l);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        float s, co; sincosf(__fmul_rn(f, p[c]), &s, &co);
+        const float ds = __fmul_rn(__fmul_rn(f, co), u[c]), dc = -__fmul_rn(__fmul_rn(f, s), u[c]);   // d sin(f p) / d p, d cos(f p) / d p
+        e0[3 + 6 * l + c] = ds; e1[3 + 6 * l + c] = ds; e0[6 + 6 * l + c] = dc; e1[6 + 6 * l + c] = dc;
+      }
+    }
+  }
+  __syncthreads();
+  for (int idx = tid; idx < TM * 16; idx += 256) {
+    const int row = idx >> 4, c4 = idx & 15;
+    *reinterpret_cast<float4*>(T.tenc + (m0 + row) * 64 + c4 * 4) = *reinterpret_cast<const float4*>(buf0 + row * LDB + D + c4 * 4);
+  }
+  // 2. h'_l = [h_l > 0] (W_l x'_{l-1}), the forward's layer loop without bias
+  float* cur = buf0; float* oth = buf1;
+  for (int l = 0; l < 8; ++l) {
+    const float* in = (l == 0) ? cur + D : cur;
+    const int K = (l == 0) ? 64 : (l == 4 ? D + 64 : D);
+    const int kvalid = (l == 0) ? 63 : (l == 4 ? D + 63 : D);
+    tile_gemm<NJ, false, 0, false>(in, LDB, K, w + nnb::w_off(D, l), nnb::w_ld(D, l), D, kvalid, nullptr, oth, LDB, Ws);
+    __syncthreads();
+    for (int idx = tid; idx < TM * (D / 4); idx += 256) {
+      const int row = idx / (D / 4), c4 = idx % (D / 4); const size_t m = m0 + row;
+      const float4 hv = *reinterpret_cast<const float4*>(P.h[l] + m * D + c4 * 4);
+      float4* xp = reinterpret_cast<float4*>(oth + row * LDB + c4 * 4);
+      float4 g = *xp;
+      g.x = hv.x > 0.f ? g.x : 0.f; g.y = hv.y > 0.f ? g.y : 0.f; g.z = hv.z > 0.f ? g.z : 0.f; g.w = hv.w > 0.f ? g.w : 0.f;
+      *xp = g;
+      *reinterpret_cast<float4*>(T.th[l] + m * D + c4 * 4) = g;
+    }
+    __syncthreads();
+    float* t_ = cur; cur = oth; oth = t_;
+  }
+  if (!T.gp) return;
+  // 3. delta_enc = d s / d enc from the dy stash: dy4 into buf0, dy0 into buf1
+  for (int idx = tid; idx < TM * (D / 4); idx += 256) {
+    const int row = idx / (D / 4), c4 = idx % (D / 4); const size_t m = m0 + row;
+    *reinterpret_cast<float4*>(buf0 + row * LDB + c4 * 4) = *reinterpret_cast<const float4*>(P.dy[4] + m * D + c4 * 4);
+    *reinterpret_cast<float4*>(buf1 + row * LDB + c4 * 4) = *reinterpret_cast<const float4*>(P.dy[0] + m * D + c4 * 4);
+  }
+  __syncthreads();
+  tile_gemm<1, true, 0, false>(buf0, LDB, D, w + nnb::w_off(D, 4) + D, D + 63, 63, D, nullptr, genc, 64, Ws);
+  tile_gemm<1, true, 0, true>(buf1, LDB, D, w + nnb::w_off(D, 0), 63, 63, D, nullptr, genc, 64, Ws);
+  __syncthreads();
+  // 4. d s' / d p_c = -u_c sum_l f^2 (delta_sin sin(f p_c) + delta_cos cos(f p_c)), f = 2^l; the identity columns contribute nothing
+  if (tid < TM && m0 + tid < M) {
+    const size_t m = m0 + tid;
+    Ray ray; int n, i; float z, p[3];
+    row_geometry(a, m, M, ray, n, i, z, p);
+    const float4 uv = T.u[m];
+    const float u[3] = {uv.x, uv.y, uv.z};
+    const float* ge = genc + tid * 64;
+    float gp[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float acc = 0.f;
+      for (int l = 0; l < 10; ++l) {
+        const float f = (float)(1 << l);
+        float s, co; sincosf(__fmul_rn(f, p[c]), &s, &co);
+        acc = fmaf(__fmul_rn(f, f), fmaf(ge[3 + 6 * l + c], s, __fmul_rn(ge[6 + 6 * l + c], co)), acc);
+      }
+      gp[c] = -__fmul_rn(acc, u[c]);
+    }
+    T.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
+  }
+}
+
+// ---------------------------------------------------------------------------------------
 // B3: weight gradients.  dW[n][k] += sum_m dY[m][n] X[m][k]
 // ---------------------------------------------------------------------------------------
 struct WJob {
@@ -775,6 +887,8 @@ static cudaError_t simt_init_dim() {
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(simt_mlp_dgrad<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
     if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(simt_field_tangent<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
+    if (e != cudaSuccess) return e;
     attr = true;
   }
   return cudaSuccess;
@@ -826,6 +940,44 @@ cudaError_t simt_field_fwd(const nnb_render_args& a, const WsLayout& L, float* o
 }
 
 cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cudaStream_t st);
+cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st);
+
+// nnb_field_hvp: forward with stash, data-gradient chain for a cotangent 1 on the logit (dy stash), tangent chain + point term, then
+// the weight-gradient jobs d s' / d W_l = sum_m dy_l[m] (x) x'_{l-1}[m] and d s' / d w_sigma = sum_m h'7[m] (no bias jobs).
+// a.flags holds NNB_STASH | NNB_HVP | NNB_RAW_DENSITY (nnb_api.cu)
+cudaError_t simt_field_hvp(const nnb_render_args& a, const WsLayout& L, const float* u, float* g_pts, float* g_weights, cudaStream_t st) {
+  SimtPtrs P = make_ptrs(L, a.workspace);
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  char* base = static_cast<char*>(a.workspace);
+  TangentPtrs T{};
+  for (int l = 0; l < 8; ++l) T.th[l] = reinterpret_cast<float*>(base + L.th[l]);
+  T.tenc = reinterpret_cast<float*>(base + L.tenc);
+  T.u = reinterpret_cast<const float4*>(u); T.gp = reinterpret_cast<float4*>(g_pts);
+  launch_mlp_fwd(a, P, L, 1, st);
+  logit_seed<<<(unsigned)((L.M + 255) / 256), 256, 0, st>>>(P.gs, L.M);
+  launch_mlp_dgrad(a, P, L, 1, st);
+  const int tiles = (int)((L.M + TM - 1) / TM);
+  if (L.D == 128) simt_field_tangent<128><<<tiles, 256, bwd_smem<128>(), st>>>(a, P, T, L.M);
+  else if (L.D == 64) simt_field_tangent<64><<<tiles, 256, bwd_smem<64>(), st>>>(a, P, T, L.M);
+  else simt_field_tangent<256><<<tiles, 256, bwd_smem<256>(), st>>>(a, P, T, L.M);
+  e = cudaGetLastError();
+  if (e != cudaSuccess || !g_weights) return e;
+  WJobs J{}; int nj = 0;
+  auto add = [&](const float* dY, int ldy, int Nn, const float* X, int ldx, int Kk, float* dW, int ldw) {
+    WJob& j = J.j[nj++];
+    j.dY = dY; j.ldy = ldy; j.Nn = Nn; j.X = X; j.ldx = ldx; j.Kk = Kk; j.dW = dW; j.ldw = ldw; j.db = nullptr;
+  };
+  const int D = L.D;
+  add(P.dy[0], D, D, T.tenc, 64, 63, g_weights + nnb::w_off(D, 0), 63);
+  for (int l = 1; l < 8; ++l) {
+    add(P.dy[l], D, D, T.th[l - 1], D, D, g_weights + nnb::w_off(D, l), nnb::w_ld(D, l));
+    if (l == 4) add(P.dy[4], D, D, T.tenc, 64, 63, g_weights + nnb::w_off(D, 4) + D, D + 63);
+  }
+  add(reinterpret_cast<const float*>(P.dyc) + 3, 4, 1, T.th[7], D, D, g_weights + nnb::W_SIG(D), D);   // the logit's cotangent, 1
+  J.njobs = nj;
+  return run_simt_wgrad(J, L.M, D, simt_wgrad_msplit(L.M), P.wpart, st);
+}
 
 cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights,
                            cudaStream_t st) {

@@ -16,6 +16,8 @@ struct WsLayout {
   // SIMT engine activation stash (fp32, [sample][feature]; D features per trunk layer, D / 2 of the rgb hidden layer)
   size_t h[8], feat, hr, enc, denc;
   size_t dy[8], dfeat, dyr, dyc;
+  // second-order field backward (NNB_HVP, SIMT engine only): tangent stash of nnb_field_hvp, [sample][feature] like h / enc
+  size_t th[8], tenc;
   // TC engine: ReLU gate bits (h > 0) of h0..h7 and the rgb hidden layer, written by tc_field_fwd, read by tc_dgrad (see gate_bits_off)
   size_t gates;
   // operand-plane backward (NNB_TCBWD; rejected by the sm_90a library): activations / output-gradients as per-tile bf16 hi|lo
@@ -117,6 +119,10 @@ inline WsLayout make_layout(int N, int S, uint32_t flags, int engine, int D = 25
       for (int l = 0; l < 8; ++l) L.dy[l] = take(L.Mpad * d * 4);
       L.dfeat = take(L.Mpad * d * 4); L.dyr = take(L.Mpad * dr * 4); L.dyc = take(L.Mpad * 16);
       if (engine == NNB_ENGINE_TC) L.gates = take(gate_bits_bytes(L.Mpad, D));
+      if (engine == NNB_ENGINE_SIMT && (flags & NNB_HVP)) {   // Mpad rows: the SIMT kernels process whole 64-row tiles
+        for (int l = 0; l < 8; ++l) L.th[l] = take(L.Mpad * d * 4);
+        L.tenc = take(L.Mpad * 64 * 4);
+      }
     }
   }
   L.total = o;

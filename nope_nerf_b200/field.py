@@ -41,6 +41,71 @@ class _FieldFn(torch.autograd.Function):
         return (None, None, None, g_p[:, :3], g_d[:, :3] if ctx.has_d else None) + tuple(gp)
 
 
+def _field_flags(net):
+    return (L.DIST_ALPHA if net.dist_alpha else 0) | (L.SOFTPLUS if net.occ_activation == 'softplus' else 0)
+
+
+class _GradFn(torch.autograd.Function):
+    """n = d s / d p of the density logit s (OfficialStaticNerf.gradient, official_nerf.py:46-58), differentiable once more.
+    forward: nnb_field_fwd + nnb_field_bwd with cotangent 1 on the logit.  backward: nnb_field_hvp, which recomputes everything from the
+    points and weights, so only p is kept."""
+
+    @staticmethod
+    def forward(ctx, net, flat, p, *params):
+        M = p.shape[0]
+        dev = p.device
+        flags = _field_flags(net) | L.RAW_DENSITY | L.STASH
+        a = L.RenderArgs()
+        p_c = ops._f32c(p.detach())
+        a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = None
+        a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_SIMT; a.hidden_dim = net.hidden_dim
+        nbytes = L.lib.nnb_workspace_bytes_dim(M, 1, flags, L.ENGINE_SIMT, net.hidden_dim)
+        ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
+        a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+        out = torch.empty(M, 4, device=dev)
+        L.check(L.lib.nnb_field_fwd(C.byref(a), L.ptr(out), ops._stream()), "nnb_field_fwd")
+        g = torch.zeros(M, 4, device=dev); g[:, 3] = 1.0
+        g_p = torch.empty(M, 4, device=dev); g_d = torch.empty(M, 4, device=dev)
+        L.check(L.lib.nnb_field_bwd(C.byref(a), L.ptr(g), L.ptr(g_p), L.ptr(g_d), None, ops._stream()), "nnb_field_bwd")
+        ctx.net = net; ctx.flat = flat; ctx.nparams = len(params); ctx.slices = net.param_slices
+        ctx.save_for_backward(p_c)
+        return g_p[:, :3]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, u):
+        p_c, = ctx.saved_tensors
+        net, flat = ctx.net, ctx.flat
+        need_p = ctx.needs_input_grad[2]
+        need_w = any(ctx.needs_input_grad[3:])
+        M = p_c.shape[0]; dev = p_c.device
+        flags = _field_flags(net) | L.RAW_DENSITY | L.STASH | L.HVP
+        u4 = torch.zeros(M, 4, device=dev); u4[:, :3] = u
+        g_p = torch.empty(M, 4, device=dev) if need_p else None
+        g_w = torch.zeros(flat.numel(), device=dev) if need_w else None
+        if need_p or need_w:
+            a = L.RenderArgs()
+            a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = None
+            a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_SIMT; a.hidden_dim = net.hidden_dim
+            nbytes = L.lib.nnb_workspace_bytes_dim(M, 1, flags, L.ENGINE_SIMT, net.hidden_dim)
+            ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=dev)
+            a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+            L.check(L.lib.nnb_field_hvp(C.byref(a), L.ptr(u4), L.ptr(g_p), L.ptr(g_w), ops._stream()), "nnb_field_hvp")
+        gp = [None] * ctx.nparams
+        if g_w is not None:
+            gp = [g_w[o:o + n].view(s) for (o, n, s) in ctx.slices]
+        return (None, None, g_p[:, :3] if need_p else None) + tuple(gp)
+
+
+def field_normal(net, p):
+    """n = d(density logit)/d p, shape (M, 3), for p (M, 3).  Differentiable with respect to p and the MLP parameters (the second-order
+    backward is nnb_field_hvp); a third derivative raises.  M == 0 returns an empty tensor without a library call."""
+    ops._need_cuda(p, "p")
+    if p.shape[0] == 0:
+        return p * 0.0          # shape (0, 3), connected to p when p requires grad, so a backward over it gives zeros
+    return _GradFn.apply(net, net.flat_weights(), p, *list(net.parameters()))
+
+
 def field_query(net, p, ray_d, raw_density=False):
     """returns (rgb (..,3), a (..,1)) with a = alpha (or sigma when rendering.dist_alpha), like return_addocc=True;
     raw_density: a = the density logit (OfficialStaticNerf.infer_occ, official_nerf.py:60-67)"""

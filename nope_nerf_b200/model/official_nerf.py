@@ -117,13 +117,20 @@ class OfficialStaticNerf(nn.Module):
 
     def gradient(self, p, it):
         """official_nerf.py:46-58: -d(density logit)/d p, shape (N, 1, 3) (surface normals of the geometry view).  The reference
-        differentiates infer_occ with autograd; here it is the data-gradient chain of the field kernel with cotangent 1 on the logit."""
-        from ..field import field_query
-        with torch.enable_grad():
-            q = p.detach().clone().requires_grad_(True)
-            _, s = field_query(self, q, None, raw_density=True)
-            g, = torch.autograd.grad(s, q, torch.ones_like(s), create_graph=False, retain_graph=False, allow_unused=True)
-        return -g.unsqueeze(1)
+        differentiates infer_occ with autograd (create_graph=True); here it is the data-gradient chain of the field kernel with cotangent
+        1 on the logit.  With grad mode on and p requiring grad the result has a grad_fn: its backward is the second-order field kernel
+        (nnb_field_hvp) and reaches p and the MLP parameters, so normal regularisers train the field.  The reference sets requires_grad
+        on the caller's p itself; here the caller does (p.requires_grad_(True) for a regulariser on fixed points), and otherwise the
+        normals come back detached, as plain values that callers may read directly (.numpy()).  Renderer.nope_nerf's normal term sets
+        requires_grad on its own surface points, as the reference does, so it reaches the MLP with a fixed pose, camera and depth too."""
+        from ..field import field_normal
+        q = p.reshape(-1, 3)
+        if torch.is_grad_enabled() and p.requires_grad:
+            n = field_normal(self, q)
+        else:
+            with torch.no_grad():
+                n = field_normal(self, q)
+        return -n.reshape(p.shape).unsqueeze(1)
 
     def forward(self, p, ray_d=None, only_occupancy=False, return_logits=False, return_addocc=False,
                 noise=False, it=100000, **kwargs):

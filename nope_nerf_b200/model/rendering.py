@@ -42,9 +42,12 @@ class Renderer(nn.Module):
         return meta
 
     def nope_nerf(self, pixels, depth, camera_mat, world_mat, scale_mat, add_noise=False, it=100000, eval_=False,
-                  c2w=None):
+                  c2w=None, normal_noise=None):
         """rendering.py:36-167.  camera_mat must be diag(kx,ky,-1,1) and scale_mat identity (the only
-        forms the reference constructs: dataset.py:101-104,199; training.py:247-252)."""
+        forms the reference constructs: dataset.py:101-104,199; training.py:247-252).
+        With rendering.normal_loss and not eval_, out['normal'] is the reference's diff_norm (rendering.py:133-141): |n(x) - n(x')| of
+        the unit normals at each valid ray's surface point x and a jittered neighbour x' = x + 0.01 (U - 0.5), differentiable with
+        respect to the MLP, the pose, the camera matrix and the prior depth.  normal_noise (valid rays, 3) replaces the draw U."""
         batch_size, n_points, _ = pixels.shape
         if batch_size != 1:
             raise NotImplementedError("batch_size must be 1 (configs/default.yaml:14)")
@@ -64,8 +67,40 @@ class Renderer(nn.Module):
         d = depth.reshape(n_points)
         rgb, dp, dg, mask, z, alpha = ops.render_autograd(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))
         m = mask.bool()
-        return {'rgb': rgb.reshape(1, n_points, 3), 'z_vals': z, 'normal': None,
+        diff_norm = None
+        if self.cfg.get('normal_loss', False) and not eval_:
+            diff_norm = self._normal_diff(pixels.reshape(n_points, 2), d, c2w, cam, m, it, normal_noise)
+        return {'rgb': rgb.reshape(1, n_points, 3), 'z_vals': z, 'normal': diff_norm,
                 'depth_pred': dp[m], 'depth_gt': dg[m], 'alpha': alpha}
+
+    def _normal_diff(self, pix, depth, c2w, cam, m, it, noise=None):
+        """rendering.py:53-94,133-141 on the valid-prior rays m: surface point camera_world + ray_vector * dists, in torch from the same
+        c2w / camera matrix / depth as the render call so that gradients reach the pose, the focal and the distortion"""
+        kx, ky = cam[0, 0], cam[1, 1]
+        R, t = c2w[:3, :3], c2w[:3, 3]
+        x, y = pix[m, 0], pix[m, 1]
+        dc = torch.stack([x / kx, y / ky, -torch.ones_like(x)], dim=-1)        # K^-1 (x, y, 1): camera-space direction at depth 1
+        dt = dc @ R.t()                                                         # pixels_world - camera_world
+        d_i = (depth[m].unsqueeze(-1) * dt).norm(2, dim=-1)                     # |points_world - camera_world|
+        nrm = dt.norm(2, dim=-1)
+        if self.cfg['normalise_ray']:
+            points = t + (dt / nrm.unsqueeze(-1)) * d_i.unsqueeze(-1)
+        else:
+            points = t + dt * (d_i / nrm).unsqueeze(-1)
+        N = points.shape[0]
+        if N == 0:
+            return points.sum(-1) * 0.0          # shape (0,), still connected to whatever the points depend on; no library call
+        if noise is None:
+            noise = torch.rand_like(points)
+        neig = points + (noise - 0.5) * 0.01
+        pp = torch.cat([points, neig], dim=0)
+        if torch.is_grad_enabled() and not pp.requires_grad:
+            # fixed pose, camera and depth: like the reference (official_nerf.py:48, p.requires_grad_(True) inside gradient()), the
+            # points this renderer owns become a leaf that requires grad, so the normal term still reaches the MLP
+            pp.requires_grad_(True)
+        g = self.model.gradient(pp, it)[:, 0, :]
+        normals = g / (g.norm(2, dim=1).unsqueeze(-1) + 10 ** (-5))
+        return torch.norm(normals[:N] - normals[N:], dim=-1)
 
     # ---- geometry visualiser (SURVEY.md 8(f) rank 4; reference rendering.py:198-418): evaluation-time only (render_visdata every
     #      `visualize_every` iterations).  Host logic mirrors the reference; every field evaluation (occupancy along the rays, secant

@@ -324,6 +324,8 @@ class _GraphStep:
                               near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
                               ray_idx=ray_idx, depth_map=self.dpt, scale=self.ss[0:1], shift=self.ss[1:2], noise=noise, H=h, W=w, stash=True,
                               hidden_dim=net.hidden_dim)
+        if rend.cfg.get('normal_loss', False) and not tr.use_cuda_graph:
+            tr._normal_draw(call.mask)
         ops.loss_rgb_depth_indirect(call.rgb, call.depth_pred, call.depth_gt, call.mask, 0.0, 0.0, self.rgb_l2, self.imgpp,
                                     ray_idx, h * w, self.out4, self.g_rgb, self.g_dp, self.g_dg, grad_scale=gs, w_dev=self.wts)
         if self.inv:                                        # losses.py:34-57 (the L1 depth weight on the device is 0)
@@ -765,6 +767,15 @@ class Trainer(object):
                     return None
         return tot if found else None
 
+    def _normal_draw(self, mask):
+        """rendering.normal_loss: the reference's renderer draws the neighbour jitter of its surface normals, rand_like of the (valid rays,
+        3) surface points, right after the sample jitter (rendering.py:133-141).  Its Loss never reads the normals, so losses and gradients
+        are those of normal_loss False; an eager step only makes the same draw, to keep the reference's random stream.  One host read of
+        the valid-ray count; the CUDA-graph step does not draw."""
+        n_valid = int(mask.sum().item())
+        if n_valid > 0:
+            torch.rand(n_valid, 3, device=mask.device)
+
     def _check_ref_stage_cfg(self):
         """the fused reference-image stage (nnb_refstage) covers every option the reference's own Trainer accepts (detach_ref_img and
         with_ssim included); only 'dense' matching exists in the reference"""
@@ -882,6 +893,8 @@ class Trainer(object):
                                   near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
                                   ray_idx=ray_idx, depth_map=depth_input.detach().reshape(h_depth, w_depth).contiguous(),
                                   scale=scale_dev, shift=shift_dev, noise=noise, H=h, W=w, stash=backward, hidden_dim=net.hidden_dim)
+            if rend.cfg.get('normal_loss', False) and not eval_mode:
+                self._normal_draw(call.mask)
             inv = self.depth_loss_type == 'invariant' and weights['depth_weight'] != 0.0
             out4, g_rgb, g_dp, g_dg = ops.loss_rgb_depth(call.rgb, call.depth_pred, call.depth_gt, call.mask,
                                                          weights['rgb_weight'], 0.0 if inv else weights['depth_weight'], rgb_loss_type == 'l2',

@@ -96,8 +96,6 @@ def flags_from_cfg(cfg, occ_activation="softplus", eval_=False, shift_first=Fals
     if occ_activation == "softplus": f |= L.SOFTPLUS
     if eval_: f |= L.EVAL
     if shift_first: f |= L.SHIFT_FIRST
-    if cfg.get("normal_loss", False):
-        raise NotImplementedError("rendering.normal_loss=True is outside the hot path (SURVEY.md 8(f) rank 4)")
     if cfg.get("outside_steps", 0) != 0:
         raise NotImplementedError("rendering.outside_steps != 0 is not supported")
     return f

@@ -308,6 +308,97 @@ def case_chamfer(mdl, name, P, Q, seed):
     print("wrote", name, float(loss))
 
 
+def case_normals(mdl, name, overrides, D, N, S, H, W, hd, wd, seed):
+    """rendering.normal_loss: True (model/rendering.py:133-141, OfficialStaticNerf.gradient with create_graph): the reference's
+    nope_nerf forward in fp32 and again in fp64 on the same draws (the sample jitter and the neighbour offsets, recorded from the fp32
+    run), diff_norm and the gradients of a fixed random weighting of it with respect to the MLP (sampled entries), r, t, the camera
+    matrix's kx / ky, scale and shift."""
+    import torch
+    from oracle import nerf_oracle as O
+    cfg = base_cfg()
+    for k, v in overrides.items():
+        sec, key = k.split(".")
+        cfg[sec][key] = v
+    cfg["rendering"]["num_points"] = S
+    cfg["rendering"]["normal_loss"] = True
+    cfg["model"]["hidden_dim"] = D
+    P = O.init_params(seed=seed, D=D, white_bkgd=cfg["rendering"]["white_background"], hf_damp=True)
+    rng = np.random.default_rng(seed + 1)
+    V, cam_id = 4, 1
+    r = rng.normal(0, 0.05, (V, 3)).astype(np.float32); t = rng.normal(0, 0.05, (V, 3)).astype(np.float32)
+    fx = 0.6 * W
+    kx, ky = 2 * fx / W, -2 * fx / H
+    dpt = rng.uniform(0.6, 7.2, (hd, wd)).astype(np.float32)
+    ray_idx = rng.permutation(H * W)[:N].astype(np.int64)
+    import model.common as mc
+    pix = mc.arange_pixels((H, W), 1)[1][:, torch.from_numpy(ray_idx)]
+
+    draws = []
+
+    def run(dtype):
+        torch.set_default_dtype(dtype)
+        real_rand, real_rand_like = torch.rand, torch.rand_like
+        k = [0]
+
+        def replay(real):
+            def f(*a, **kw):
+                if dtype == torch.float32:
+                    v = real(*a, **kw); draws.append(v.detach().clone()); return v
+                v = draws[k[0]].to(dtype); k[0] += 1
+                return v
+            return f
+        torch.rand, torch.rand_like = replay(real_rand), replay(real_rand_like)
+        try:
+            net, rend, model = build_model(mdl, cfg, P)
+            net.to(dtype)
+            pose = mdl.LearnPose(V, True, True, cfg).to(dtype)
+            with torch.no_grad():
+                pose.r.copy_(torch.from_numpy(r)); pose.t.copy_(torch.from_numpy(t))
+            kxy = torch.tensor([kx, ky], dtype=dtype, requires_grad=True)
+            z4 = torch.zeros(4); one = torch.ones(1)
+            camera_mat = torch.cat([kxy[0:1], z4, kxy[1:2], z4, -one, z4, one]).view(1, 4, 4)
+            scale = torch.tensor(1.07, dtype=dtype, requires_grad=True); shift = torch.tensor(-0.03, dtype=dtype, requires_grad=True)
+            depth_img = torch.from_numpy(dpt).to(dtype)[None, None] * scale + shift
+            world_mat = torch.inverse(pose(cam_id)).unsqueeze(0)
+            out = model(pix.to(dtype), torch.from_numpy(ray_idx), camera_mat, world_mat, torch.eye(4).unsqueeze(0), "nope_nerf", it=0,
+                        eval_mode=False, depth_img=depth_img, add_noise=True, img_size=(H, W))
+        finally:
+            torch.rand, torch.rand_like = real_rand, real_rand_like
+        dn = out["normal"]
+        wts = torch.from_numpy(np.random.default_rng(seed + 2).normal(0, 1, dn.shape[0])).to(dtype)
+        (dn * wts).sum().backward()
+        res = dict(diff_norm=dn.detach().numpy().astype(np.float64), wts=wts.numpy().astype(np.float64),
+                   grad_r=pose.r.grad[cam_id].numpy().astype(np.float64), grad_t=pose.t.grad[cam_id].numpy().astype(np.float64),
+                   grad_kxy=kxy.grad.numpy().astype(np.float64), grad_scale=scale.grad.numpy().astype(np.float64),
+                   grad_shift=shift.grad.numpy().astype(np.float64))
+        for n_, prm in net.named_parameters():
+            g_ = torch.zeros_like(prm) if prm.grad is None else prm.grad          # biases and the rgb branch do not enter diff_norm
+            res["pg." + n_] = g_.numpy().reshape(-1).astype(np.float64)
+        torch.set_default_dtype(torch.float32)
+        return res
+
+    r32 = run(torch.float32)
+    r64 = run(torch.float64)
+    uniform = cfg["rendering"]["sample_option"] == "uniform"
+    rec = dict(N=N, S=S, H=H, W=W, hd=hd, wd=wd, seed=seed, hidden_dim=D, cam_id=cam_id, kx=kx, ky=ky, r=r, t=t, dpt=dpt, ray_idx=ray_idx,
+               scale=1.07, shift=-0.03, pixels=pix[0].numpy(), wts=r32["wts"].astype(np.float32),
+               noise=draws[0].numpy()[0] if uniform else np.zeros((N, S), np.float32), nbr=draws[1 if uniform else 0].numpy())
+    for k, v in overrides.items():
+        rec["cfg." + k] = np.array(v)
+    sel = np.random.default_rng(seed + 3)
+    for key in r32:
+        if key == "wts":
+            continue
+        a32, a64 = r32[key], r64[key]
+        if key.startswith("pg.") and a32.size > 256:
+            idx = np.sort(sel.choice(a32.size, 256, replace=False))
+            rec[key + ".idx"] = idx; a32, a64 = a32[idx], a64[idx]
+        rec[key + ".f32"] = a32.astype(np.float32); rec[key + ".f64"] = a64
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", name + ".npz"), **rec)
+    print("wrote", name, "valid", rec["diff_norm.f32"].shape[0], "|dn32-dn64|", np.abs(r32["diff_norm"] - r64["diff_norm"]).max(),
+          "grad_t", rec["grad_t.f32"], rec["grad_t.f64"])
+
+
 def main():
     mdl = import_reference()
     os.makedirs(os.path.join(ROOT, "tests", "golden"), exist_ok=True)
@@ -390,6 +481,14 @@ def main():
                         add_noise=True, seed=54, pose_mode="rand", hf_damp=damp)
         case_train_step(mdl, "train_full_losses_s48", True, steps=2, N=48, S=48, H=24, W=32, hd=16, wd=24, seed=55)
         case_train_step(mdl, "train_render_only_s300", False, steps=2, N=24, S=300, H=24, W=32, hd=16, wd=24, seed=56)
+
+    if "normals" in which:
+        # rendering.normal_loss: True -- diff_norm and its gradients through the second derivative of the field
+        for D in (64, 256):
+            case_normals(mdl, "normals_uniform_d%d" % D, {}, D=D, N=64, S=32, H=30, W=40, hd=12, wd=21, seed=61)
+            case_normals(mdl, "normals_ndc_d%d" % D, {"rendering.sample_option": "ndc", "rendering.dist_alpha": True,
+                                                      "rendering.depth_range": [0.0, 1.0]},
+                         D=D, N=64, S=32, H=30, W=40, hd=16, wd=20, seed=62)
 
 
 if __name__ == "__main__":

@@ -67,6 +67,7 @@ class _Writer:
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("workdir"); ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--normal-loss", action="store_true", help="rendering.normal_loss: True (the renderer computes the normal term)")
     a = ap.parse_args()
     import torch
     from oracle import ref_harness as RH
@@ -86,6 +87,7 @@ def main():
                            backup_every=-1, validate_every=-1, eval_pose_every=-1, eval_img_every=1, scheduling_start=1, scheduling_epoch=1,
                            scheduling_mode="reset", vis_resolution=[24, 32], vis_geo=False, log_scale_shift_per_view=True, length_smooth=1)
     cfg["rendering"]["num_points"] = 64
+    cfg["rendering"]["normal_loss"] = bool(a.normal_loss)
     os.makedirs(cfg["training"]["out_dir"], exist_ok=True)
     # ---- the INTEGRATION.md binding: reference `model` package, hot-path classes redirected ----
     mdl = RH.import_reference("cuda" if torch.cuda.is_available() else "cpu")
