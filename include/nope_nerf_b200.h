@@ -39,6 +39,8 @@ extern "C" {
 #define NNB_FWD_DROP_ALO 8192u /* forward precision experiment: rejected (rc -7) by this library */
 #define NNB_WG16 1024u      /* with NNB_TCBWD only (fp16 weight-gradient operand planes); without it the flag has no effect */
 #define NNB_HVP 16384u      /* with NNB_STASH on NNB_ENGINE_SIMT: the workspace also holds the tangent stash of nnb_field_hvp; sizes only */
+#define NNB_OCC_ONLY 32768u /* nnb_field_fwd on NNB_ENGINE_TC only: out_rgba = (0, 0, 0, a); the colour branch (fc_feature, rgb_layers.0,
+                             * fc_rgb) is not evaluated.  a is bit-identical to the full query's (OfficialStaticNerf.forward(only_occupancy=True)) */
 
 /* engines */
 #define NNB_ENGINE_SIMT 0 /* exact fp32 FMA path                                        */
@@ -104,7 +106,8 @@ typedef struct nnb_render_bwd_args {
 } nnb_render_bwd_args;
 
 const char* nnb_last_error(void);
-int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys; >= 102: nnb_field_hvp */
+int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys; >= 102: nnb_field_hvp;
+                          * >= 103: nnb_field_fwd honours NNB_ENGINE_TC, NNB_OCC_ONLY */
 /* Profiling hook used by bench.py: `events` is a HOST array of cudaEvent_t handles that stays alive until
  * nnb_profile_events(NULL,0).  Every nnb_render_fwd records 4 marks (start, weights imaged, field done,
  * composited) and every nnb_render_bwd 5 marks (start, compositing adjoint, data-gradient chain,
@@ -125,10 +128,21 @@ size_t nnb_workspace_bytes_dim(int32_t N, int32_t S, uint32_t flags, int32_t eng
 /* floats of the flat MLP parameter vector of width hidden_dim (0 = 256; NNB_NUM_PARAMS at 256); 0 for an unsupported width */
 size_t nnb_num_params(int32_t hidden_dim);
 int nnb_render_fwd(const nnb_render_args* a, void* stream);
-/* OfficialStaticNerf.forward(p, ray_d, return_addocc=True) on explicit points (model/official_nerf.py:69-96), exact-fp32
- * engine.  Uses a->pts/dirs, N points (S is ignored), weights, flags (NNB_DIST_ALPHA / NNB_SOFTPLUS / NNB_STASH) and the
- * workspace; out_rgba [N,4] = (r,g,b, alpha-or-sigma).  nnb_field_bwd: g_rgba [N,4] -> g_pts [N,4], g_dirs [N,4] (xyz used),
- * g_weights (+=, may be NULL). */
+/* OfficialStaticNerf.forward(p, ray_d, return_addocc=True) on explicit points (model/official_nerf.py:69-96).  Uses a->pts/dirs,
+ * N points (S is ignored), weights, flags (NNB_DIST_ALPHA / NNB_SOFTPLUS / NNB_RAW_DENSITY / NNB_STASH) and the workspace;
+ * out_rgba [N,4] = (r,g,b, alpha-or-sigma-or-logit).  nnb_field_bwd: g_rgba [N,4] -> g_pts [N,4], g_dirs [N,4] (xyz used),
+ * g_weights (+=, may be NULL).
+ * Engine of nnb_field_fwd: a->engine == NNB_ENGINE_TC runs the tensor-core kernel (inference only); every other value runs the
+ * exact-fp32 engine, as in versions < 103, which ignored the field.  nnb_field_bwd and nnb_field_hvp always run exact fp32.
+ *   NNB_ENGINE_TC: flags NNB_DIST_ALPHA / NNB_SOFTPLUS / NNB_RAW_DENSITY / NNB_OCC_ONLY.  NNB_STASH is rejected (rc -6): gradients
+ *   need the exact-fp32 engine.  The workspace holds nnb_workspace_bytes_dim(N, 1, flags, NNB_ENGINE_TC, hidden_dim) bytes, 256-byte
+ *   aligned; out_rgba is 16-byte aligned; c2w / cam / ray_idx are not read.  Rows of out_rgba past N are not written.
+ *   Precision: every layer is the split-fp16 product of the render path (three MMAs a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, 22-bit
+ *   operands, fp32 accumulation): outputs agree with float64 to about 1e-6 of the tensor's maximum.  fp16 halves have a limited
+ *   exponent range: the low half is a normal number only for |x| above about 2^-3, is subnormal (absolute quantum 2^-24) below
+ *   that, and an operand below about 6e-8 vanishes, so a field whose activations are very small is evaluated less accurately than
+ *   on the exact engine.
+ *   Every other engine value: NNB_OCC_ONLY is rejected (rc -6); the workspace rule is that of NNB_ENGINE_SIMT. */
 int nnb_field_fwd(const nnb_render_args* a, float* out_rgba, void* stream);
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream);
 /* Second-order backward of the surface normal n(p) = d s / d p, s the density logit (OfficialStaticNerf.gradient with

@@ -14,6 +14,7 @@ HIDDEN_DIMS = (64, 128, 256)     # model.hidden_dim values with a kernel instant
 DIST_ALPHA, NDC, NORMALISE, USE_DIR, WHITE_BG, EVAL, SOFTPLUS, SHIFT_FIRST, STASH, TCBWD, WG16, RAW_DENSITY = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048
 FWD_DROP_WLO, FWD_DROP_ALO = 4096, 8192
 HVP = 16384                      # with STASH: workspace of nnb_field_hvp (second-order field backward)
+OCC_ONLY = 32768                 # nnb_field_fwd on ENGINE_TC: density only, out = (0, 0, 0, a)
 ENGINE_SIMT, ENGINE_TC = 0, 1
 RS_SCALE_PCS, RS_DETACH_RGBS_SCALE, RS_SHIFT_FIRST, RS_WITH_SSIM, RS_GRAD_REF = 1, 2, 4, 8, 16   # nnb_refstage_args.flags
 

@@ -16,6 +16,7 @@ cudaError_t simt_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float*
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
+cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st);
 size_t tc_workspace_extra(int N, int S, uint32_t flags, int D);
 bool tc_supports(int S);
 #endif
@@ -59,7 +60,8 @@ static int cuda_fail(cudaError_t e, const char* where) {
 extern "C" {
 
 const char* nnb_last_error(void) { return g_err; }
-int nnb_version(void) { return 102; }   // 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys; 102: nnb_field_hvp
+// 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys; 102: nnb_field_hvp; 103: nnb_field_fwd on NNB_ENGINE_TC
+int nnb_version(void) { return 103; }
 int nnb_profile_events(void** events, int32_t count) {
   g_prof_events = reinterpret_cast<cudaEvent_t*>(events); g_prof_n = events ? count : 0; g_prof_i = 0;
   return 0;
@@ -189,6 +191,22 @@ static int check_field(const nnb_render_args* a) {
 int nnb_field_fwd(const nnb_render_args* a, float* out_rgba, void* stream) {
   int rc = check_field(a); if (rc) return rc;
   if (!out_rgba) return fail(-3, "nnb_field_fwd: out_rgba is null");
+  if (a->engine == NNB_ENGINE_TC) {
+#ifndef NNB_WITH_TC
+    return fail(-4, "library built without the tensor-core engine");
+#else
+    if (a->flags & NNB_STASH)
+      return fail(-6, "nnb_field_fwd: NNB_STASH needs NNB_ENGINE_SIMT (the tensor-core field query is inference only; gradients run on the exact-fp32 engine)");
+    const size_t need = nnb_workspace_bytes_dim(a->N, 1, a->flags, NNB_ENGINE_TC, a->hidden_dim);
+    if (a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+    if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(out_rgba) & 15) != 0) return fail(-3, "nnb_field_fwd: out_rgba must be 16-byte aligned");
+    nnb_render_args b = *a; b.S = 1;
+    cudaError_t e = tc_field_fwd_points(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_TC, hidden_of(b.hidden_dim)), out_rgba, (cudaStream_t)stream);
+    return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_fwd");
+#endif
+  }
+  if (a->flags & NNB_OCC_ONLY) return fail(-6, "nnb_field_fwd: NNB_OCC_ONLY needs NNB_ENGINE_TC");
   nnb_render_args b = *a; b.S = 1; b.engine = NNB_ENGINE_SIMT;
   cudaError_t e = simt_field_fwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT, hidden_of(b.hidden_dim)), out_rgba, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_fwd");

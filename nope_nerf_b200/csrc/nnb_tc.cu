@@ -15,6 +15,10 @@
 //               fp16 hi | lo weight stages (all output rows x 16 k) from L2 into a 3-deep shared-memory ring, mbarrier tx-count;
 //               a stage is released once both warpgroups' MMAs have read it.
 //
+// tc_points_fwd is the same kernel on explicit points (nnb_field_fwd with NNB_ENGINE_TC): the row's point and view direction are
+// read instead of generated, the direction term of rgb_layers.0 is two more K-steps of its GEMM (every row has its own direction),
+// the output is one float4 per point, and NNB_OCC_ONLY ends the tile after the density head.
+//
 // The backward of this engine (tc_render_bwd) runs tc_dgrad (the same skeleton through the transposed weights, gated by the
 // forward's ReLU bits) and tc_wgrad (the MLP weight-gradient GEMMs on the fp32 stash), between the compositing and ray adjoints of
 // nnb_simt.cu.
@@ -49,6 +53,21 @@ template <int D> struct Tc {
   // ---- forward stage table: the order in which weight stages are consumed for one tile (152 stages at D = 256) ----
   static constexpr int N_STAGES = 4 + 3 * KS + (4 + KS) + 3 * KS + KS + KS;
   static constexpr size_t IMG_BYTES = (size_t)(N_STAGES - KS) * STAGE_BYTES + KS * (STAGE_BYTES / 2);   // rgb hidden layer: D/2 rows
+  // The producer's and the consumers' loop bounds both come from gemm_steps: K-steps (= weight stages) of GEMM g.  Points mode (pts)
+  // appends the two direction K-steps of the rgb hidden layer; an occupancy-only tile (occ) ends after GEMM 7.
+  static constexpr int enc_steps(int g) { return (g == 0 || g == 4) ? 4 : 0; }   // of them, the leading K-steps from the encoding operand E
+  static constexpr int gemm_steps(int g, bool pts) { return enc_steps(g) + (g == 0 ? 0 : KS) + (pts && g == 9 ? 2 : 0); }
+  static constexpr int n_gemm(bool occ) { return occ ? 8 : N_GEMM; }
+  static constexpr int tile_stages(bool pts, bool occ) {
+    int n = 0;
+    for (int g = 0; g < n_gemm(occ); ++g) n += gemm_steps(g, pts);
+    return n;
+  }
+  static_assert(tile_stages(false, false) == N_STAGES, "ray-mode stage count");
+  // points mode: the direction stages (D/2 rows each) follow the ray-mode table and image
+  static constexpr int N_STAGES_PTS = tile_stages(true, false), N_STAGES_OCC = tile_stages(true, true);
+  static constexpr size_t IMG_PTS_BYTES = IMG_BYTES + 2 * (STAGE_BYTES / 2);
+  static_assert(N_STAGES_PTS == N_STAGES + 2 && N_STAGES_OCC == N_STAGES - 2 * KS && IMG_PTS_BYTES == IMG_BYTES + 64 * D, "points-mode stages");
   static constexpr int SM_AHI = 0, SM_ALO = D * 256, SM_EHI = 2 * D * 256, SM_ELO = SM_EHI + 16384, SM_W = SM_ELO + 16384;
   static constexpr int SM_BIAS = SM_W + NST * STAGE_BYTES;
   static constexpr int BIAS_FLOATS = 8 * D + D + D + 3 * (D / 2) + 4;   // trunk, feat, w_sigma, W_rgb, (b_sigma, b_rgb[3])
@@ -68,12 +87,16 @@ template <int D> struct Tc {
   static constexpr int DG_BAR = DG_GYC + 128 * 4 * 4;
   static constexpr int DG_TOTAL = DG_BAR + 2 * NST * 8;
   static_assert(SM_TOTAL <= 232448 && DG_TOTAL <= 232448, "shared memory budget");
+  // a field query's workspace is sized like a render's: the direction stages spill into the transposed-image region behind the
+  // forward image, which only the backward uses
+  static_assert(IMG_PTS_BYTES <= (IMG_BYTES + 255) / 256 * 256 + IMG_T_BYTES, "points-mode weight image fits the workspace");
+  static_assert(RAYB_FLOATS >= D / 2, "points mode keeps the bias of the rgb hidden layer in the per-ray bias area");
 };
 static_assert(Tc<256>::N_STAGES == 152 && Tc<256>::SM_BIAS == 212992 && Tc<256>::BIAS_FLOATS == 2948 && Tc<256>::N_STAGES_T == 176 &&
               Tc<256>::IMG_T_BYTES == (size_t)136 * 16384 + 8 * 2048 + 32 * 4096 && Tc<256>::DG_GENC == 180224, "D = 256 layout");
 
 // stage tables, one per width
-__constant__ StageDesc c_stages_256[Tc<256>::N_STAGES], c_stages_128[Tc<128>::N_STAGES], c_stages_64[Tc<64>::N_STAGES];
+__constant__ StageDesc c_stages_256[Tc<256>::N_STAGES_PTS], c_stages_128[Tc<128>::N_STAGES_PTS], c_stages_64[Tc<64>::N_STAGES_PTS];
 __constant__ StageDescT c_stages_t_256[Tc<256>::N_STAGES_T], c_stages_t_128[Tc<128>::N_STAGES_T], c_stages_t_64[Tc<64>::N_STAGES_T];
 template <int D> __device__ __forceinline__ const StageDesc& stage(int s) {
   if constexpr (D == 256) return c_stages_256[s]; else if constexpr (D == 128) return c_stages_128[s]; else return c_stages_64[s];
@@ -134,16 +157,22 @@ __device__ __forceinline__ void row_geometry_tc(const nnb_render_args& a, size_t
   sample_point(a, ray, z, p);
 }
 
+// x, opaque to the compiler: an address formed from it is computed where it is used, not once per tile and held (or spilled) across the MMAs
+__device__ __forceinline__ uint32_t computed_here(uint32_t x) { asm volatile("" : "+r"(x)); return x; }
+
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <int D>
-__global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
-                                              SampleRec* __restrict__ recs, const __grid_constant__ TcStash st, size_t M, int n_tiles,
-                                              int stash) {
+// PTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] -> out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is
+// stashed and recs is not written.  M = a.N there, so point indices are 32-bit.  Otherwise rays (tc_field_fwd): recs [Mpad], out unused.
+template <int D, bool PTS>
+__device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
+                                            float4* __restrict__ out, const TcStash& st, size_t M, int n_tiles, int stash) {
   using T = Tc<D>;
+  if constexpr (PTS) stash = 0;
+  const bool occ = PTS && (a.flags & NNB_OCC_ONLY);
   constexpr int SM_AHI = T::SM_AHI, SM_ALO = T::SM_ALO, SM_EHI = T::SM_EHI, SM_ELO = T::SM_ELO, SM_W = T::SM_W, SM_BIAS = T::SM_BIAS;
   constexpr int SM_RAYB = T::SM_RAYB, SM_BAR = T::SM_BAR, BIAS_FLOATS = T::BIAS_FLOATS, RAYB_FLOATS = T::RAYB_FLOATS;
   constexpr int STAGE_BYTES = T::STAGE_BYTES, N_STAGES = T::N_STAGES, DR = D / 2;
@@ -181,8 +210,9 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0;
+      const int n_st = PTS ? (occ ? T::N_STAGES_OCC : T::N_STAGES_PTS) : N_STAGES;
       for (int t = 0; t < my_tiles; ++t)
-        for (int s = 0; s < N_STAGES; ++s) {
+        for (int s = 0; s < n_st; ++s) {
           const uint32_t bytes = (uint32_t)stage<D>(s).nrows * 64u;
           mbar_wait(EMPTY(slot), phase ^ 1u);                 // both warpgroups released this slot
           mbar_expect_tx(FULL(slot), bytes);
@@ -206,6 +236,10 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
   constexpr int RAYB_DE = T::RAYB_RAYS * DR;   // direction encodings after the per-ray biases
   uint32_t slot = 0, phase = 0;
   float acc[D / 2];
+  if constexpr (PTS) {   // b_rgbh is a plain bias here; visible after the tile's first barrier
+    if (tl < DR) rayb[tl] = __ldg(a.weights + nnb::B_RGBH(D) + tl);
+  }
+  const int n_gemm = T::n_gemm(occ);
 
   for (int t = 0; t < my_tiles; ++t) {
     const int tile = blockIdx.x + t * gridDim.x;
@@ -215,12 +249,18 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
     auto ray_off = [&]() { return (int)((mt + (size_t)wg * 64) % (size_t)a.S); };
     wg_sync();   // the previous tile's epilogue is done with the per-ray bias buffer
     {
-      const int off0 = ray_off();
+      const int off0 = PTS ? 0 : ray_off();
       // ---- prologue: thread (row rl, part) writes encoding columns [32 part, 32 part + 32) of its row ----
       const int rl = tl & 63, part = tl >> 6, row = wg * 64 + rl;
       const size_t m = mt + row;
       Ray ray; float z, p[3];
-      row_geometry_tc(a, m, M, ray, z, p);
+      if constexpr (PTS) {
+        const uint32_t mm = min(tile * (uint32_t)TILE + row, (uint32_t)M - 1u);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + (size_t)mm * 3 + c);
+      } else {
+        row_geometry_tc(a, m, M, ray, z, p);
+      }
       float ee[64];
 #pragma unroll
       for (int c = 0; c < 3; ++c) ee[c] = p[c];
@@ -240,7 +280,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
           *reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8 + 4) = make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]);
         }
       }
-      if (part == 0) {   // direction-encoding term of rgb_layers.0 is constant per ray: folded into a per-ray bias below
+      if constexpr (!PTS) if (part == 0) {   // direction-encoding term of rgb_layers.0 is constant per ray: folded into a per-ray bias below
         float v[3], de[32];
         view_dir(a, ray, v);
         encode<4>(v, [&](int k, float val) { de[k] = val; });
@@ -260,7 +300,7 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
       fence_async_smem();
       wg_sync();
       const float* w = a.weights;
-      const int n_rays = (off0 + 63) / a.S + 1;
+      const int n_rays = PTS ? 0 : (off0 + 63) / a.S + 1;
       for (int r = 0; r < n_rays; ++r) {   // thread tl = output column of the rgb hidden layer
         if (DR < 128 && tl >= DR) break;
         float b = __ldg(w + nnb::B_RGBH(D) + tl);
@@ -270,13 +310,15 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
       }
     }
     float s_logit[2] = {0.f, 0.f};
-    for (int g = 0; g < N_GEMM; ++g) {
-      // ---- MMAs: K-steps from the encoding operand E (layers 0 and 4) first, then from the previous layer's output ----
-      const int n_e = (g == 0 || g == 4) ? 4 : 0, ns = n_e + (g == 0 ? 0 : T::KS);
+    for (int g = 0; g < n_gemm; ++g) {
+      // ---- MMAs: K-steps from the encoding operand E (layers 0 and 4) first, then from the previous layer's output; in points mode
+      //      the rgb hidden layer ends with the two K-steps of the direction operand, which took E's place after layer 4 ----
+      const int n_e = T::enc_steps(g), ns = T::gemm_steps(g, PTS);
       const uint32_t nrows = (g == 9) ? (uint32_t)DR : (uint32_t)D;
       for (int s = 0; s < ns; ++s) {
-        const bool from_e = s < n_e;
-        const uint32_t ko = (uint32_t)(from_e ? s : s - n_e) * 4096u;   // two k-octets of 2048 B per K-step
+        const bool from_dir = PTS && g == 9 && s >= T::KS;
+        const bool from_e = s < n_e || from_dir;
+        const uint32_t ko = (uint32_t)(from_dir ? s - T::KS : (from_e ? s : s - n_e)) * 4096u;   // two k-octets of 2048 B per K-step
         const uint64_t dah = gdesc((from_e ? e_hi : a_hi) + ko, 2048, 128), dal = gdesc((from_e ? e_lo : a_lo) + ko, 2048, 128);
         const uint32_t wb = w_base + slot * STAGE_BYTES;
         const uint64_t dbh = gdesc(wb, nrows * 16u, 128), dbl = gdesc(wb + nrows * 32u, nrows * 16u, 128);
@@ -325,20 +367,40 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
           }
         }
         if (stash && g < 8) store_gates<D / 2>(st.gates + gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
+        if constexpr (PTS) {
+          // Layer 4 was the last reader of E.  The direction operand of the rgb hidden layer takes its place: enc4(dirs[m]), 27 columns
+          // padded to 32 (two K-steps), as fp16 hi | lo in E's layout.  A warp writes the 16 rows its own MMAs read, like the A operand
+          // above, and the barrier below orders the writes before the rgb hidden layer's MMAs.
+          if (g == 4 && !occ) {
+            const int row = wg * 64 + (warp & 3) * 16 + (lane & 15), part = lane >> 4;
+            const uint32_t mm = computed_here(min(tile * (uint32_t)TILE + row, (uint32_t)M - 1u));
+            float v[3], de[32];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + (size_t)mm * 3 + c) : 1.f;
+            encode<4>(v, [&](int k, float val) { de[k] = val; });
+#pragma unroll
+            for (int k = 27; k < 32; ++k) de[k] = 0.f;
+#pragma unroll
+            for (int kb = 0; kb < 4; ++kb) {
+              if ((kb >> 1) != part) continue;   // static register indices
+              split_store8(de + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
+            }
+          }
+        }
         fence_async_smem();
         wg_sync();   // the whole A operand (and, after layer 0, the per-ray bias) is written before the next layer's MMAs
       } else {
         // rgb hidden layer (D/2 columns) -> colour head + per-sample record
         float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
         uint32_t gw[D / 128 > 0 ? D / 128 : 1] = {};
-        const int off0 = ray_off();
+        const int off0 = PTS ? 0 : ray_off();
 #pragma unroll
         for (int j = 0; j < DR / 8; ++j) {
           const int col = j * 8 + c0;
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
             const int row = r0 + 8 * r;
-            const float* rb = rayb + ((off0 + row - wg * 64) / a.S) * DR;
+            const float* rb = PTS ? rayb : rayb + ((off0 + row - wg * 64) / a.S) * DR;   // points mode: b_rgbh
             const float v0 = fmaxf(acc[4 * j + 2 * r] + rb[col], 0.f), v1 = fmaxf(acc[4 * j + 2 * r + 1] + rb[col + 1], 0.f);
 #pragma unroll
             for (int c = 0; c < 3; ++c)
@@ -358,14 +420,42 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, 
             float sigma;
             SampleRec rec;
             rec.r = sigmoid_f(cr + s_bias[B_SIG0 + 1]); rec.g = sigmoid_f(cg + s_bias[B_SIG0 + 2]); rec.b = sigmoid_f(cb + s_bias[B_SIG0 + 3]);
-            rec.a = density_act(s, a.flags, &sigma); rec.s = s; rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
-            rec.pad0 = 0.f; rec.pad1 = 0.f;
-            recs[m] = rec;
+            rec.a = density_act(s, a.flags, &sigma); rec.s = s;
+            if constexpr (PTS) {
+              const uint32_t mp = computed_here(tile * (uint32_t)TILE + r0 + 8 * r);
+              if (mp < (uint32_t)M) out[mp] = make_float4(rec.r, rec.g, rec.b, rec.a);
+            } else {
+              rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
+              rec.pad0 = 0.f; rec.pad1 = 0.f;
+              recs[m] = rec;
+            }
           }
         }
       }
     }
+    if (occ) {   // the tile ended after layer 7 and the density head
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float sl = quad_sum(s_logit[r]);
+        const uint32_t mp = computed_here(tile * (uint32_t)TILE + r0 + 8 * r);
+        float sigma;
+        if ((lane & 3) == 0 && mp < (uint32_t)M) out[mp] = make_float4(0.f, 0.f, 0.f, density_act(sl + s_bias[B_SIG0], a.flags, &sigma));
+      }
+    }
   }
+}
+
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                              SampleRec* __restrict__ recs, const __grid_constant__ TcStash st, size_t M, int n_tiles,
+                                              int stash) {
+  tc_fwd_body<D, false>(a, wimg, recs, nullptr, st, M, n_tiles, stash);
+}
+
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                              float4* __restrict__ out, size_t M, int n_tiles) {
+  tc_fwd_body<D, true>(a, wimg, nullptr, out, TcStash{}, M, n_tiles, 0);
 }
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
@@ -998,7 +1088,7 @@ cudaError_t upload_stage_table() {
   using T = Tc<D>;
   static bool ready = false;
   if (ready) return cudaSuccess;
-  StageDesc h[T::N_STAGES];
+  StageDesc h[T::N_STAGES_PTS];
   int s = 0, off = 0;
   auto add = [&](int w_off, int ldw, int kcol0, int kvalid, int nrows) {
     h[s].w_off = w_off; h[s].ldw = ldw; h[s].kcol0 = kcol0; h[s].kvalid = kvalid; h[s].nrows = nrows; h[s].img_off = off;
@@ -1011,9 +1101,14 @@ cudaError_t upload_stage_table() {
     if (l == 4) for (int i = 0; i < 4; ++i) add(nnb::w_off(D, 4), D + 63, D + 16 * i, D + 63, D);
     for (int i = 0; i < KS; ++i) add(nnb::w_off(D, l), nnb::w_ld(D, l), 16 * i, D, D);
   }
+  // A producer that waits for a stage no consumer takes never returns: the counts the kernels loop over (Tc::tile_stages) must be
+  // the table's, for rays, for points and for the occupancy-only prefix.
+  if (s != T::N_STAGES_OCC) return cudaErrorInvalidValue;
   for (int i = 0; i < KS; ++i) add(nnb::W_FEAT(D), D, 16 * i, D, D);
   for (int i = 0; i < KS; ++i) add(nnb::W_RGBH(D), D + 27, 16 * i, D, D / 2);
   if (s != T::N_STAGES || (size_t)off != T::IMG_BYTES) return cudaErrorInvalidValue;
+  for (int i = 0; i < 2; ++i) add(nnb::W_RGBH(D), D + 27, D + 16 * i, D + 27, D / 2);   // points mode: the direction columns
+  if (s != T::N_STAGES_PTS || (size_t)off != T::IMG_PTS_BYTES) return cudaErrorInvalidValue;
   cudaError_t e;
   if constexpr (D == 256) e = cudaMemcpyToSymbol(c_stages_256, h, sizeof(h));
   else if constexpr (D == 128) e = cudaMemcpyToSymbol(c_stages_128, h, sizeof(h));
@@ -1061,6 +1156,30 @@ cudaError_t tc_render_fwd_dim(const nnb_render_args& a, const WsLayout& L, cudaS
   return e;
 }
 
+// nnb_field_fwd on this engine: a.pts / a.dirs [L.M][3] -> out_rgba [L.M][4]
+template <int D>
+cudaError_t tc_points_fwd_dim(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st) {
+  using T = Tc<D>;
+  cudaError_t e = upload_stage_table<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_points_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  unsigned char* img = reinterpret_cast<unsigned char*>(static_cast<char*>(a.workspace) + L.total);
+  const int n_st = (a.flags & NNB_OCC_ONLY) ? T::N_STAGES_OCC : T::N_STAGES_PTS;   // the stages the kernel walks
+  tc_prep_weights<D><<<n_st, 256, 0, st>>>(a.weights, img);
+  const int n_tiles = (int)((L.M + TILE - 1) / TILE);
+  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  tc_points_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, (const unsigned char*)img, reinterpret_cast<float4*>(out_rgba), L.M, n_tiles);
+  return cudaGetLastError();
+}
+
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
 
 }  // namespace
@@ -1076,6 +1195,11 @@ cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStrea
   if (!tc_supports(a.S)) return cudaErrorNotSupported;
   if (a.flags & NNB_TCBWD) return cudaErrorNotSupported;   // the operand-plane stash is not implemented for sm_90a
   return L.D == 128 ? tc_render_fwd_dim<128>(a, L, st) : (L.D == 64 ? tc_render_fwd_dim<64>(a, L, st) : tc_render_fwd_dim<256>(a, L, st));
+}
+
+cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st) {
+  return L.D == 128 ? tc_points_fwd_dim<128>(a, L, out_rgba, st)
+       : L.D == 64  ? tc_points_fwd_dim<64>(a, L, out_rgba, st) : tc_points_fwd_dim<256>(a, L, out_rgba, st);
 }
 
 // Backward of the TC engine: compositing / ray adjoints of nnb_simt.cu around tc_dgrad and tc_wgrad, which read and write the SIMT

@@ -1,5 +1,6 @@
-"""OfficialStaticNerf.forward on explicit points (reference: model/official_nerf.py:69-96) through nnb_field_fwd/bwd
-(exact-fp32 engine): used by direct callers of the field module; the renderer path never materialises points."""
+"""OfficialStaticNerf.forward on explicit points (reference: model/official_nerf.py:69-96) through nnb_field_fwd/bwd: used by direct
+callers of the field module and the geometry view; the nope_nerf render path never materialises points.  The exact-fp32 engine
+serves every call; a call that needs no gradient can ask for the tensor-core engine (field_query(engine='tc'))."""
 import ctypes as C
 import torch
 from . import _lib as L
@@ -106,12 +107,51 @@ def field_normal(net, p):
     return _GradFn.apply(net, net.flat_weights(), p, *list(net.parameters()))
 
 
-def field_query(net, p, ray_d, raw_density=False):
+def _field_tc(net, flags, p, d):
+    """nnb_field_fwd on the tensor-core engine: p (M, 3), d (M, 3) or None -> out (M, 4).  No autograd."""
+    M = p.shape[0]
+    a = L.RenderArgs()
+    flat = net.flat_weights()
+    p_c = ops._f32c(p.detach()); d_c = None if d is None else ops._f32c(d.detach())
+    a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = L.ptr(d_c)
+    a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_TC; a.hidden_dim = net.hidden_dim
+    ws = torch.empty(L.lib.nnb_workspace_bytes_dim(M, 1, flags, L.ENGINE_TC, net.hidden_dim), dtype=torch.uint8, device=p.device)
+    a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+    out = torch.empty(M, 4, device=p.device)
+    L.check(L.lib.nnb_field_fwd(C.byref(a), L.ptr(out), ops._stream()), "nnb_field_fwd")
+    return out
+
+
+def _engine_id(engine):
+    if engine is None or engine in (L.ENGINE_SIMT, L.ENGINE_TC):
+        return engine
+    try:
+        return {"simt": L.ENGINE_SIMT, "tc": L.ENGINE_TC}[engine]
+    except (KeyError, TypeError):
+        raise ValueError("engine must be None, 'simt', 'tc', ENGINE_SIMT or ENGINE_TC (got %r)" % (engine,))
+
+
+def field_query(net, p, ray_d, raw_density=False, occ_only=False, engine=None):
     """returns (rgb (..,3), a (..,1)) with a = alpha (or sigma when rendering.dist_alpha), like return_addocc=True;
-    raw_density: a = the density logit (OfficialStaticNerf.infer_occ, official_nerf.py:60-67)"""
+    raw_density: a = the density logit (OfficialStaticNerf.infer_occ, official_nerf.py:60-67).
+    engine: None or 'simt' = the exact-fp32 engine.  'tc' (or ENGINE_TC) = the tensor-core engine when the call needs no gradient
+    (grad mode off, or neither p, ray_d nor a parameter of net requires grad); a call that needs one runs on the exact engine, which
+    has the backward.  The engines agree to about 1e-6 of the output's maximum, not bit for bit.
+    occ_only: the caller uses a only.  On the tensor-core engine the colour branch is then skipped and rgb is zeros (a is bit-identical
+    to the full query's); the exact engine evaluates everything regardless.
+    No point (M == 0) returns empty tensors without a library call."""
     ops._need_cuda(p, "p")
     shp = p.shape[:-1]
     flags = (L.DIST_ALPHA if net.dist_alpha else 0) | (L.SOFTPLUS if net.occ_activation == 'softplus' else 0) | (L.RAW_DENSITY if raw_density else 0)
     d = None if ray_d is None else ray_d.reshape(-1, 3)
+    if p.numel() == 0:
+        z = p.reshape(-1, 3)[:, :1] * 0.0      # stays connected to p, like an empty result of the library would
+        return z.expand(-1, 3).reshape(*shp, 3), z.reshape(*shp, 1)
+    if _engine_id(engine) == L.ENGINE_TC:
+        needs_grad = torch.is_grad_enabled() and (p.requires_grad or (d is not None and d.requires_grad)
+                                                  or any(q.requires_grad for q in net.parameters()))
+        if not needs_grad:
+            out = _field_tc(net, flags | (L.OCC_ONLY if occ_only else 0), p.reshape(-1, 3), d)
+            return out[:, :3].reshape(*shp, 3), out[:, 3].reshape(*shp, 1)
     rgb, a = _FieldFn.apply(flags, net, net.flat_weights(), p.reshape(-1, 3), d, *list(net.parameters()))
     return rgb.reshape(*shp, 3), a.reshape(*shp, 1)

@@ -16,6 +16,9 @@ class Renderer(nn.Module):
         self.cfg = cfg
         self.model = model.to(device)
         self.engine = kwargs.get("engine", None)
+        # engine of the geometry view's explicit-point queries (ray marching, secant steps, surface colour): None = exact fp32,
+        # 'tc' = tensor cores (OfficialStaticNerf.forward(engine=)).  The normals stay on gradient(), which is exact fp32.
+        self.field_engine = kwargs.get("field_engine", None)
 
     def to(self, device):
         model = super().to(device)
@@ -160,7 +163,7 @@ class Renderer(nn.Module):
             diffuse = torch.mm(surface_normals, light).clamp_min(0).repeat(1, 3) * diffuse_per.unsqueeze(0)
             rgb_values[network_object_mask] = (ambiant.unsqueeze(0) + diffuse).clamp_max(1.0)
             with torch.no_grad():
-                rgb_val[network_object_mask] = self.model(surface_points, surface_view_vol)
+                rgb_val[network_object_mask] = self.model(surface_points, surface_view_vol, engine=self.field_engine)
         return {'rgb': rgb_values.reshape(batch_size, -1, 3), 'normal': None, 'rgb_surf': rgb_val.reshape(batch_size, -1, 3)}
 
     def ray_marching(self, ray0, ray_direction, model, c=None, tau=0.5, n_steps=[128, 129], n_secant_steps=8, depth_range=[0., 2.4],
@@ -175,7 +178,7 @@ class Renderer(nn.Module):
         d_proposal = depth_range[0] * (1. - d_proposal) + d_intersect.view(1, -1, 1, 1) * d_proposal
         p_proposal = ray0.unsqueeze(2) + ray_direction.unsqueeze(2) * d_proposal
         with torch.no_grad():
-            val = torch.cat([model(p_split, only_occupancy=True) - tau
+            val = torch.cat([model(p_split, only_occupancy=True, engine=self.field_engine) - tau
                              for p_split in torch.split(p_proposal.reshape(batch_size, -1, 3), int(max_points / batch_size), dim=1)],
                             dim=1).view(batch_size, -1, n_steps)
         mask_0_not_occupied = val[:, :, 0] < 0
@@ -209,7 +212,7 @@ class Renderer(nn.Module):
         for _ in range(n_secant_steps):
             p_mid = ray0_masked + d_pred.unsqueeze(-1) * ray_direction_masked
             with torch.no_grad():
-                f_mid = self.model(p_mid, batchwise=False, only_occupancy=True, it=it)[..., 0] - tau
+                f_mid = self.model(p_mid, batchwise=False, only_occupancy=True, it=it, engine=self.field_engine)[..., 0] - tau
             ind_low = f_mid < 0
             d_low = torch.where(ind_low, d_pred, d_low); f_low = torch.where(ind_low, f_mid, f_low)
             d_high = torch.where(ind_low, d_high, d_pred); f_high = torch.where(ind_low, f_high, f_mid)
