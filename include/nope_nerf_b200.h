@@ -107,7 +107,7 @@ typedef struct nnb_render_bwd_args {
 
 const char* nnb_last_error(void);
 int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys; >= 102: nnb_field_hvp;
-                          * >= 103: nnb_field_fwd honours NNB_ENGINE_TC, NNB_OCC_ONLY */
+                          * >= 103: nnb_field_fwd honours NNB_ENGINE_TC, NNB_OCC_ONLY; >= 104: nnb_ray_march */
 /* Profiling hook used by bench.py: `events` is a HOST array of cudaEvent_t handles that stays alive until
  * nnb_profile_events(NULL,0).  Every nnb_render_fwd records 4 marks (start, weights imaged, field done,
  * composited) and every nnb_render_bwd 5 marks (start, compositing adjoint, data-gradient chain,
@@ -154,6 +154,46 @@ int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, f
  * u and g_pts are 16-byte aligned.  Exact-fp32 engine; every sum runs in a fixed order, so the same inputs give the same bits. */
 int nnb_field_hvp(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream);
 int nnb_render_bwd(const nnb_render_bwd_args* a, void* stream);
+
+/* Fused ray marching of the geometry view: what Renderer.ray_marching + Renderer.secant (model/rendering.py:274-418) do for N rays, in
+ * one stream-ordered call that never holds a point or an occupancy in global memory.  Ray n is sampled at the n_steps depths
+ *   t_i = near_ (1 - frac[i]) + far_[n] frac[i],   p_i = ray0[n] + ray_dir[n] t_i,   val_i = occupancy(p_i) - tau,
+ * the occupancy being OfficialStaticNerf.forward(only_occupancy=True) (alpha, or sigma with NNB_DIST_ALPHA; NNB_SOFTPLUS as in the
+ * render).  first = the smallest i with val_i val_{i+1} < 0 (the rounded fp32 product, so a product that underflows to 0 is no sign
+ * change).  The ray hits when first exists, val_first < 0 and val_0 < 0; its bracket (d_low, d_high, f_low, f_high) = (t_first,
+ * t_{first+1}, val_first, val_{first+1}) is then refined by n_secant secant steps d = -f_low (d_high - d_low) / (f_high - f_low) + d_low,
+ * f_mid = occupancy(ray0 + d ray_dir) - tau, f_mid < 0 ? (d_low, f_low) = (d, f_mid) : (d_high, f_high) = (d, f_mid).
+ *   depth [N]: the secant iterate of the final bracket on a hit; 0 where val_0 >= 0 (the first sample is occupied), whatever follows;
+ *     +inf otherwise.
+ *   first [N] (optional, NULL = not wanted): the index above; -1 where there is none or val_0 >= 0 (such a ray is not searched further).
+ *   bracket [N,4] (optional, 16-byte aligned): the bracket before the secant steps on a hit, zeros elsewhere.
+ * Engine: tensor cores only.  engine != NNB_ENGINE_TC is rejected (rc < 0); the exact-fp32 engine has no fused march.  Precision is
+ * that of nnb_field_fwd on NNB_ENGINE_TC.
+ * Bit-equality contract: on this engine a point's occupancy does not depend on the tile or row that evaluates it, and every product, sum
+ * and quotient above is rounded on its own in the order of the torch code.  depth, first and bracket are therefore bit-identical to
+ * Renderer.ray_marching / secant run on nnb_field_fwd(NNB_ENGINE_TC | NNB_OCC_ONLY) with frac = torch.linspace(0, 1, n_steps) (passed in,
+ * so the library does not reproduce linspace's rounding).
+ * Work: the rays advance in rounds of 128 steps; a ray whose first sign change (or occupied first sample) has been seen takes no part in
+ * later rounds, so a ray costs ceil((first + 2) / 128) tiles of 128 queries instead of n_steps queries.
+ * The workspace holds nnb_ray_march_workspace_bytes(N, n_steps, hidden_dim) bytes, 256-byte aligned.  After the call its first
+ * int32s are counters: [0] = rays that hit, [k] (1 <= k < ceil(n_steps / 128)) = rays that took part in round k.
+ * N == 0 returns 0 and does nothing.  Nothing synchronises or allocates; every launch after the first sizes itself from a counter in
+ * the workspace. */
+typedef struct nnb_ray_march_args {
+  const float* weights;  /* [nnb_num_params(hidden_dim)] */
+  const float* ray0;     /* [N,3] */
+  const float* ray_dir;  /* [N,3] */
+  const float* far_;     /* [N] per-ray far depth */
+  const float* frac;     /* [n_steps] */
+  int32_t N, n_steps /* >= 2 */, n_secant /* >= 0 */, hidden_dim /* 64, 128, 256; 0 = 256 */;
+  float near_, tau;
+  uint32_t flags;        /* NNB_DIST_ALPHA | NNB_SOFTPLUS */
+  int32_t engine;        /* NNB_ENGINE_TC */
+  float* depth; int32_t* first; float* bracket;
+  void* workspace; size_t workspace_bytes;
+} nnb_ray_march_args;
+size_t nnb_ray_march_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
+int nnb_ray_march(const nnb_ray_march_args* a, void* stream);
 
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,

@@ -30,6 +30,13 @@ class RenderArgs(C.Structure):
                 ("workspace", _f), ("workspace_bytes", C.c_size_t), ("pts", _f), ("dirs", _f), ("hidden_dim", C.c_int32)]
 
 
+class RayMarchArgs(C.Structure):   # nnb_ray_march_args
+    _fields_ = [("weights", _f), ("ray0", _f), ("ray_dir", _f), ("far_", _f), ("frac", _f),
+                ("N", C.c_int32), ("n_steps", C.c_int32), ("n_secant", C.c_int32), ("hidden_dim", C.c_int32),
+                ("near_", C.c_float), ("tau", C.c_float), ("flags", C.c_uint32), ("engine", C.c_int32),
+                ("depth", _f), ("first", _f), ("bracket", _f), ("workspace", _f), ("workspace_bytes", C.c_size_t)]
+
+
 class RenderBwdArgs(C.Structure):
     _fields_ = [("fwd", RenderArgs), ("g_rgb", _f), ("g_depth_pred", _f), ("g_depth_gt", _f),
                 ("g_weights", _f), ("g_c2w", _f), ("g_cam", _f), ("g_depth", _f), ("g_scale_shift", _f), ("phase", C.c_uint32),
@@ -77,6 +84,9 @@ def _load():
     lib.nnb_render_bwd.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
     lib.nnb_debug_wgrad.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]   # test aid
     lib.nnb_field_fwd.argtypes = [C.POINTER(RenderArgs), _f, C.c_void_p]
+    lib.nnb_ray_march.argtypes = [C.POINTER(RayMarchArgs), C.c_void_p]
+    lib.nnb_ray_march_workspace_bytes.restype = C.c_size_t
+    lib.nnb_ray_march_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     lib.nnb_field_bwd.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, C.c_void_p]
     lib.nnb_field_hvp.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, C.c_void_p]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]

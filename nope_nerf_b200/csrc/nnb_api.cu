@@ -18,6 +18,8 @@ cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaS
 cudaError_t tc_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
 cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st);
 size_t tc_workspace_extra(int N, int S, uint32_t flags, int D);
+size_t tc_ray_march_workspace(int N, int n_steps, int D);
+cudaError_t tc_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
 cudaError_t launch_pose_fwd(const float*, const float*, const float*, int, const int*, float*, cudaStream_t);
@@ -60,8 +62,9 @@ static int cuda_fail(cudaError_t e, const char* where) {
 extern "C" {
 
 const char* nnb_last_error(void) { return g_err; }
-// 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys; 102: nnb_field_hvp; 103: nnb_field_fwd on NNB_ENGINE_TC
-int nnb_version(void) { return 103; }
+// 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys; 102: nnb_field_hvp; 103: nnb_field_fwd on NNB_ENGINE_TC;
+// 104: nnb_ray_march
+int nnb_version(void) { return 104; }
 int nnb_profile_events(void** events, int32_t count) {
   g_prof_events = reinterpret_cast<cudaEvent_t*>(events); g_prof_n = events ? count : 0; g_prof_i = 0;
   return 0;
@@ -210,6 +213,35 @@ int nnb_field_fwd(const nnb_render_args* a, float* out_rgba, void* stream) {
   nnb_render_args b = *a; b.S = 1; b.engine = NNB_ENGINE_SIMT;
   cudaError_t e = simt_field_fwd(b, make_layout(b.N, 1, b.flags, NNB_ENGINE_SIMT, hidden_of(b.hidden_dim)), out_rgba, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_fwd");
+}
+size_t nnb_ray_march_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && n_steps >= 2 && nnb::dim_supported(D)) return tc_ray_march_workspace(N, n_steps, D);
+#endif
+  return 0;
+}
+int nnb_ray_march(const nnb_ray_march_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_ray_march: engine %d has no fused march (NNB_ENGINE_TC only; march on the exact-fp32 engine through nnb_field_fwd)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  const int D = hidden_of(a->hidden_dim);
+  if (!nnb::dim_supported(D)) return fail(-8, "hidden_dim %d is not supported (supported: 64, 128, 256; 0 means 256)", a->hidden_dim);
+  if (a->N < 0) return fail(-2, "nnb_ray_march: N must not be negative (got %d)", a->N);
+  if (a->n_steps < 2 || a->n_secant < 0) return fail(-2, "nnb_ray_march: need n_steps >= 2 and n_secant >= 0 (got %d, %d)", a->n_steps, a->n_secant);
+  if (a->N == 0) return 0;
+  if (!a->weights || !a->ray0 || !a->ray_dir || !a->far_ || !a->frac || !a->depth)
+    return fail(-3, "nnb_ray_march: weights, ray0, ray_dir, far_, frac and depth must be non-null");
+  const size_t need = tc_ray_march_workspace(a->N, a->n_steps, D);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(a->bracket) & 15) != 0) return fail(-3, "nnb_ray_march: bracket must be 16-byte aligned");
+  cudaError_t e = tc_ray_march(*a, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_ray_march");
+#endif
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {
   int rc = check_field(a); if (rc) return rc;

@@ -19,6 +19,10 @@
 // read instead of generated, the direction term of rgb_layers.0 is two more K-steps of its GEMM (every row has its own direction),
 // the output is one float4 per point, and NNB_OCC_ONLY ends the tile after the density head.
 //
+// tc_march / tc_secant (nnb_ray_march, the geometry view's fused ray march) are the occupancy-only kernel again with points made from
+// (ray origin, direction, depth) in the prologue and a reduction instead of an output: the first sign change of a ray's 128-step block,
+// or the update of a hit ray's secant bracket (see MarchPtrs).
+//
 // The backward of this engine (tc_render_bwd) runs tc_dgrad (the same skeleton through the transposed weights, gated by the
 // forward's ReLU bits) and tc_wgrad (the MLP weight-gradient GEMMs on the fp32 stash), between the compositing and ray adjoints of
 // nnb_simt.cu.
@@ -165,14 +169,90 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// PTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] -> out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is
-// stashed and recs is not written.  M = a.N there, so point indices are 32-bit.  Otherwise rays (tc_field_fwd): recs [Mpad], out unused.
-template <int D, bool PTS>
+// ---- fused ray marching (nnb_ray_march): tc_march / tc_secant are tc_fwd_body with a front end that makes each row's point from
+// (origin, direction, depth) and a back end that reduces the tile's occupancies instead of writing them ----
+// Every product and sum below is rounded on its own (no FMA contraction), in the order of Renderer.ray_marching / Renderer.secant, so
+// that depths, points and secant iterates carry the bits the torch code computes.
+__device__ __forceinline__ float march_depth(float near, float far, float frac) {   // near (1 - frac) + far frac
+  return __fadd_rn(__fmul_rn(near, __fsub_rn(1.f, frac)), __fmul_rn(far, frac));
+}
+__device__ __forceinline__ float secant_depth(const float4& b) {   // b = (d_low, d_high, f_low, f_high)
+  return __fadd_rn(__fdiv_rn(__fmul_rn(-b.z, __fsub_rn(b.y, b.x)), __fsub_rn(b.w, b.z)), b.x);
+}
+enum : int { RAY_SEARCHING = 0, RAY_HIT = 1, RAY_OCCUPIED = 2, RAY_NO_HIT = 3 };   // MarchPtrs::status
+struct MarchPtrs {
+  const float *ray0, *dir, *far, *frac;   // [N][3], [N][3], [N], [n_steps]
+  float near, tau;
+  int n_steps, n_secant;
+  int block;           // tc_march: this launch evaluates steps 128 block .. 128 block + 127 of its rays
+  const int* list;     // tc_march: the rays of this round (NULL: every ray, tile = ray); tc_secant: the hit rays
+  const int* count;    // device count of `list` (NULL: the launch's n_tiles)
+  int *next_list, *next_count;   // rays still searching after this block
+  int *hit_list, *hit_count;
+  float* carry;        // [N] val of the ray's last evaluated step
+  int *status, *first; // [N]
+  float4 *brk0, *brk1; // [N] bracket found by the march | bracket after the secant passes so far
+};
+
+// Back end of a march tile, one warp: the first pair (i, i + 1) of the tile's steps, including the pair formed with the previous
+// block's last value, whose rounded product val[i] val[i + 1] is negative.  A ray with that pair, or whose very first value is not
+// negative, is finished; any other ray with steps left is appended to the next round's list.
+__device__ __forceinline__ void march_scan(const MarchPtrs& q, int ray, const float* s_val, int lane) {
+  const int base = q.block * TILE;
+  const int nv = min(TILE, q.n_steps - base);   // steps of the ray in this tile; the rows past them were evaluated on a clamped index
+  const float prev = lane > 0 ? s_val[4 * lane - 1] : (q.block > 0 ? q.carry[ray] : 0.f);   // 0: step 0 has no predecessor
+  const float4 v = *reinterpret_cast<const float4*>(s_val + 4 * lane);
+  uint32_t m = 0;
+  if (4 * lane + 0 < nv && __fmul_rn(prev, v.x) < 0.f) m |= 1u;
+  if (4 * lane + 1 < nv && __fmul_rn(v.x, v.y) < 0.f) m |= 2u;
+  if (4 * lane + 2 < nv && __fmul_rn(v.y, v.z) < 0.f) m |= 4u;
+  if (4 * lane + 3 < nv && __fmul_rn(v.z, v.w) < 0.f) m |= 8u;
+  const uint32_t lanes = __ballot_sync(0xffffffffu, m != 0);
+  const int src = lanes ? __ffs(lanes) - 1 : 0;
+  const int r = __shfl_sync(0xffffffffu, 4 * lane + __ffs(m) - 1, src);   // tile row of the pair's second step
+  if (lane != 0) return;
+  if (q.block == 0 && !(s_val[0] < 0.f)) { q.status[ray] = RAY_OCCUPIED; return; }
+  if (lanes) {
+    const float f_low = r > 0 ? s_val[r - 1] : prev, f_high = s_val[r];
+    const int i = base + r - 1;
+    q.first[ray] = i;
+    q.status[ray] = f_low < 0.f ? RAY_HIT : RAY_NO_HIT;
+    if (f_low < 0.f) {
+      const float far = __ldg(q.far + ray);
+      q.brk0[ray] = make_float4(march_depth(q.near, far, __ldg(q.frac + i)), march_depth(q.near, far, __ldg(q.frac + i + 1)), f_low, f_high);
+      q.hit_list[atomicAdd(q.hit_count, 1)] = ray;
+    }
+  } else if (base + TILE < q.n_steps) {
+    q.carry[ray] = s_val[TILE - 1];
+    q.next_list[atomicAdd(q.next_count, 1)] = ray;
+  }
+}
+
+// MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
+// out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is stashed and recs is not written.  M = a.N there, so point indices
+// are 32-bit.  FWD_MARCH / FWD_SECANT (tc_march / tc_secant): occupancy-only tiles of points made from q; n_tiles (and M, the hit count
+// of tc_secant) are read from *q.count when the kernel starts and fixed from then on.
+//   FWD_MARCH: tile = 128 consecutive steps of one ray; march_scan reduces them.
+//   FWD_SECANT: tile = 128 hit rays, evaluated q.n_secant times in a row at the secant iterate of each ray's bracket, which the thread
+//   that owns the row's logit then updates in q.brk1 (pass 0 reads q.brk0).  A row's prologue threads and that thread sit in the same
+//   warpgroup, whose barrier at the top of the tile loop orders the update before the next pass reads it.
+enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3 };
+template <int D, int MODE>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
-                                            float4* __restrict__ out, const TcStash& st, size_t M, int n_tiles, int stash) {
+                                            float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
+                                            int stash) {
   using T = Tc<D>;
+  constexpr bool PTS = MODE != FWD_RAYS, MARCH = MODE >= FWD_MARCH;
   if constexpr (PTS) stash = 0;
-  const bool occ = PTS && (a.flags & NNB_OCC_ONLY);
+  if constexpr (MARCH) {
+    if (q.count) {
+      const int c = *q.count;
+      M = (size_t)c;
+      n_tiles = MODE == FWD_SECANT ? (c + TILE - 1) / TILE : c;
+    }
+    if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
+  }
+  const bool occ = MARCH || (PTS && (a.flags & NNB_OCC_ONLY));
   constexpr int SM_AHI = T::SM_AHI, SM_ALO = T::SM_ALO, SM_EHI = T::SM_EHI, SM_ELO = T::SM_ELO, SM_W = T::SM_W, SM_BIAS = T::SM_BIAS;
   constexpr int SM_RAYB = T::SM_RAYB, SM_BAR = T::SM_BAR, BIAS_FLOATS = T::BIAS_FLOATS, RAYB_FLOATS = T::RAYB_FLOATS;
   constexpr int STAGE_BYTES = T::STAGE_BYTES, N_STAGES = T::N_STAGES, DR = D / 2;
@@ -203,6 +283,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
   }
   __syncthreads();
   const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // tiles blockIdx.x, + gridDim.x, ...
+  // tile evaluations of this CTA: the producer's and the consumers' common bound.  tc_secant evaluates each tile n_secant times in a row.
+  const int my_evals = MODE == FWD_SECANT ? my_tiles * q.n_secant : my_tiles;
 
   if (warp >= 8) {
     // =============================== weight producer ===============================
@@ -211,7 +293,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
     if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0;
       const int n_st = PTS ? (occ ? T::N_STAGES_OCC : T::N_STAGES_PTS) : N_STAGES;
-      for (int t = 0; t < my_tiles; ++t)
+      for (int t = 0; t < my_evals; ++t)
         for (int s = 0; s < n_st; ++s) {
           const uint32_t bytes = (uint32_t)stage<D>(s).nrows * 64u;
           mbar_wait(EMPTY(slot), phase ^ 1u);                 // both warpgroups released this slot
@@ -236,13 +318,13 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
   constexpr int RAYB_DE = T::RAYB_RAYS * DR;   // direction encodings after the per-ray biases
   uint32_t slot = 0, phase = 0;
   float acc[D / 2];
-  if constexpr (PTS) {   // b_rgbh is a plain bias here; visible after the tile's first barrier
+  if constexpr (MODE == FWD_POINTS) {   // b_rgbh is a plain bias here; visible after the tile's first barrier
     if (tl < DR) rayb[tl] = __ldg(a.weights + nnb::B_RGBH(D) + tl);
   }
   const int n_gemm = T::n_gemm(occ);
 
-  for (int t = 0; t < my_tiles; ++t) {
-    const int tile = blockIdx.x + t * gridDim.x;
+  for (int t = 0; t < my_evals; ++t) {
+    const int tile = blockIdx.x + (MODE == FWD_SECANT ? t / q.n_secant : t) * gridDim.x;
     const size_t mt = (size_t)tile * TILE;
     // sample index of this warpgroup's first row inside its ray: row rl reads the bias of the block's ray (ray_off() + rl) / S.  Computed
     // where it is used, not held across the MMAs.
@@ -254,7 +336,21 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
       const int rl = tl & 63, part = tl >> 6, row = wg * 64 + rl;
       const size_t m = mt + row;
       Ray ray; float z, p[3];
-      if constexpr (PTS) {
+      if constexpr (MODE == FWD_MARCH) {
+        const int ray = q.list ? q.list[tile] : tile;
+        const float depth = march_depth(q.near, __ldg(q.far + ray), __ldg(q.frac + min(q.block * TILE + row, q.n_steps - 1)));
+#pragma unroll
+        for (int c = 0; c < 3; ++c) p[c] = __fadd_rn(__ldg(q.ray0 + (size_t)ray * 3 + c), __fmul_rn(__ldg(q.dir + (size_t)ray * 3 + c), depth));
+      } else if constexpr (MODE == FWD_SECANT) {
+        const uint32_t mp = tile * (uint32_t)TILE + row;
+        p[0] = p[1] = p[2] = 0.f;   // rows past the last hit ray are evaluated and ignored
+        if (mp < (uint32_t)M) {
+          const int ray = q.list[mp];
+          const float depth = secant_depth((t % q.n_secant == 0 ? q.brk0 : q.brk1)[ray]);
+#pragma unroll
+          for (int c = 0; c < 3; ++c) p[c] = __fadd_rn(__ldg(q.ray0 + (size_t)ray * 3 + c), __fmul_rn(depth, __ldg(q.dir + (size_t)ray * 3 + c)));
+        }
+      } else if constexpr (PTS) {
         const uint32_t mm = min(tile * (uint32_t)TILE + row, (uint32_t)M - 1u);
 #pragma unroll
         for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + (size_t)mm * 3 + c);
@@ -434,12 +530,33 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
       }
     }
     if (occ) {   // the tile ended after layer 7 and the density head
+      // an occupancy-only tile does not use the per-ray bias area: a march tile's 128 values (occupancy - tau) go there
+      float* s_val = reinterpret_cast<float*>(smem + SM_RAYB);
+      static_assert(2 * RAYB_FLOATS >= TILE, "a march tile's values fit the per-ray bias area");
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const float sl = quad_sum(s_logit[r]);
         const uint32_t mp = computed_here(tile * (uint32_t)TILE + r0 + 8 * r);
         float sigma;
-        if ((lane & 3) == 0 && mp < (uint32_t)M) out[mp] = make_float4(0.f, 0.f, 0.f, density_act(sl + s_bias[B_SIG0], a.flags, &sigma));
+        if constexpr (MODE == FWD_POINTS) {
+          if ((lane & 3) == 0 && mp < (uint32_t)M) out[mp] = make_float4(0.f, 0.f, 0.f, density_act(sl + s_bias[B_SIG0], a.flags, &sigma));
+        } else if constexpr (MODE == FWD_MARCH) {
+          if ((lane & 3) == 0) s_val[r0 + 8 * r] = __fsub_rn(density_act(sl + s_bias[B_SIG0], a.flags, &sigma), q.tau);
+        } else if constexpr (MODE == FWD_SECANT) {
+          if ((lane & 3) == 0 && mp < (uint32_t)M) {
+            const int ray = q.list[mp];
+            float4 b = (t % q.n_secant == 0 ? q.brk0 : q.brk1)[ray];
+            const float d_mid = secant_depth(b), f_mid = __fsub_rn(density_act(sl + s_bias[B_SIG0], a.flags, &sigma), q.tau);
+            if (f_mid < 0.f) { b.x = d_mid; b.z = f_mid; } else { b.y = d_mid; b.w = f_mid; }
+            q.brk1[ray] = b;
+          }
+        }
+      }
+      if constexpr (MODE == FWD_MARCH) {
+        // both warpgroups' values are written before the scan, and the scan has read them before either warpgroup's next tile writes
+        asm volatile("bar.sync 3, 256;" ::: "memory");
+        if (warp == 0) march_scan(q, q.list ? q.list[tile] : tile, s_val, lane);
+        asm volatile("bar.sync 3, 256;" ::: "memory");
       }
     }
   }
@@ -449,13 +566,37 @@ template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_field_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                               SampleRec* __restrict__ recs, const __grid_constant__ TcStash st, size_t M, int n_tiles,
                                               int stash) {
-  tc_fwd_body<D, false>(a, wimg, recs, nullptr, st, M, n_tiles, stash);
+  tc_fwd_body<D, FWD_RAYS>(a, wimg, recs, nullptr, st, MarchPtrs{}, M, n_tiles, stash);
 }
 
 template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_points_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                               float4* __restrict__ out, size_t M, int n_tiles) {
-  tc_fwd_body<D, true>(a, wimg, nullptr, out, TcStash{}, M, n_tiles, 0);
+  tc_fwd_body<D, FWD_POINTS>(a, wimg, nullptr, out, TcStash{}, MarchPtrs{}, M, n_tiles, 0);
+}
+
+// one round of nnb_ray_march: block q.block of every ray of q.list (n_rays rays when q.count is NULL)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_march(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                         const __grid_constant__ MarchPtrs q, int n_rays) {
+  tc_fwd_body<D, FWD_MARCH>(a, wimg, nullptr, nullptr, TcStash{}, q, 0, n_rays, 0);
+}
+// the q.n_secant secant passes of nnb_ray_march over the *q.count hit rays of q.list
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_secant(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                          const __grid_constant__ MarchPtrs q) {
+  tc_fwd_body<D, FWD_SECANT>(a, wimg, nullptr, nullptr, TcStash{}, q, 0, 0, 0);
+}
+
+// depth (and the optional first / bracket) of every ray from the state the march and the secant passes left
+__global__ void march_finish(const __grid_constant__ MarchPtrs q, int N, float* __restrict__ depth, int* __restrict__ first,
+                             float4* __restrict__ bracket) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int s = q.status[i];
+  depth[i] = s == RAY_HIT ? secant_depth((q.n_secant > 0 ? q.brk1 : q.brk0)[i]) : (s == RAY_OCCUPIED ? 0.f : __int_as_float(0x7f800000));
+  if (first) first[i] = (s == RAY_HIT || s == RAY_NO_HIT) ? q.first[i] : -1;
+  if (bracket) bracket[i] = s == RAY_HIT ? q.brk0[i] : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
@@ -1180,6 +1321,73 @@ cudaError_t tc_points_fwd_dim(const nnb_render_args& a, const WsLayout& L, float
   return cudaGetLastError();
 }
 
+// Workspace of nnb_ray_march, every section 256-byte aligned: counters [rounds + 1] (0: hit rays; k >= 1: rays of round k) | status,
+// first, carry [N] | the two ray lists that alternate between rounds, the hit list [N] | brk0, brk1 [N] float4 | the weight image of the
+// occupancy-only stages
+struct MarchWs { size_t status, first, carry, list[2], hits, brk0, brk1, img, total; int rounds; };
+template <int D> MarchWs march_layout(int N, int n_steps) {
+  MarchWs w{};
+  w.rounds = (n_steps + TILE - 1) / TILE;
+  size_t off = align_up((size_t)(w.rounds + 1) * 4, 256);
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  w.status = take((size_t)N * 4); w.first = take((size_t)N * 4); w.carry = take((size_t)N * 4);
+  w.list[0] = take((size_t)N * 4); w.list[1] = take((size_t)N * 4); w.hits = take((size_t)N * 4);
+  w.brk0 = take((size_t)N * 16); w.brk1 = take((size_t)N * 16);
+  w.img = take((size_t)Tc<D>::N_STAGES_OCC * Tc<D>::STAGE_BYTES);
+  w.total = off;
+  return w;
+}
+
+// nnb_ray_march: weight image once, then one tc_march launch per 128-step block (round k takes its rays from the list round k - 1
+// appended to), tc_secant over the hit rays, march_finish.  Every launch after the first sizes itself from a device counter; nothing is
+// read back.
+template <int D>
+cudaError_t tc_ray_march_dim(const nnb_ray_march_args& r, cudaStream_t st) {
+  using T = Tc<D>;
+  cudaError_t e = upload_stage_table<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_march<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_secant<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  const MarchWs w = march_layout<D>(r.N, r.n_steps);
+  char* base = static_cast<char*>(r.workspace);
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  int* counters = I(0);
+  e = cudaMemsetAsync(base, 0, w.status + (size_t)r.N * 4, st);   // counters and status (RAY_SEARCHING)
+  if (e != cudaSuccess) return e;
+  nnb_render_args a{};
+  a.weights = r.weights; a.flags = (r.flags & (NNB_DIST_ALPHA | NNB_SOFTPLUS)) | NNB_OCC_ONLY; a.hidden_dim = D;
+  MarchPtrs q{};
+  q.ray0 = r.ray0; q.dir = r.ray_dir; q.far = r.far_; q.frac = r.frac; q.near = r.near_; q.tau = r.tau;
+  q.n_steps = r.n_steps; q.n_secant = r.n_secant;
+  q.hit_list = I(w.hits); q.hit_count = counters;
+  q.carry = reinterpret_cast<float*>(base + w.carry); q.status = I(w.status); q.first = I(w.first);
+  q.brk0 = reinterpret_cast<float4*>(base + w.brk0); q.brk1 = reinterpret_cast<float4*>(base + w.brk1);
+  const unsigned char* img = reinterpret_cast<const unsigned char*>(base + w.img);
+  tc_prep_weights<D><<<T::N_STAGES_OCC, 256, 0, st>>>(r.weights, reinterpret_cast<unsigned char*>(base + w.img));
+  const int grid = r.N < n_sm ? r.N : n_sm;
+  for (int k = 0; k < w.rounds; ++k) {
+    q.block = k;
+    q.list = k > 0 ? I(w.list[k & 1]) : nullptr; q.count = k > 0 ? counters + k : nullptr;
+    q.next_list = I(w.list[(k + 1) & 1]); q.next_count = counters + k + 1;   // not written by the last round
+    tc_march<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, q, r.N);
+  }
+  if (r.n_secant > 0) {
+    q.list = q.hit_list; q.count = counters;
+    const int tiles = (r.N + TILE - 1) / TILE;
+    tc_secant<D><<<tiles < n_sm ? tiles : n_sm, N_THREADS, T::SM_TOTAL, st>>>(a, img, q);
+  }
+  march_finish<<<(r.N + 255) / 256, 256, 0, st>>>(q, r.N, r.depth, r.first, reinterpret_cast<float4*>(r.bracket));
+  return cudaGetLastError();
+}
+
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
 
 }  // namespace
@@ -1195,6 +1403,13 @@ cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStrea
   if (!tc_supports(a.S)) return cudaErrorNotSupported;
   if (a.flags & NNB_TCBWD) return cudaErrorNotSupported;   // the operand-plane stash is not implemented for sm_90a
   return L.D == 128 ? tc_render_fwd_dim<128>(a, L, st) : (L.D == 64 ? tc_render_fwd_dim<64>(a, L, st) : tc_render_fwd_dim<256>(a, L, st));
+}
+
+size_t tc_ray_march_workspace(int N, int n_steps, int D) {
+  return D == 128 ? march_layout<128>(N, n_steps).total : (D == 64 ? march_layout<64>(N, n_steps).total : march_layout<256>(N, n_steps).total);
+}
+cudaError_t tc_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st) {
+  return D == 128 ? tc_ray_march_dim<128>(r, st) : (D == 64 ? tc_ray_march_dim<64>(r, st) : tc_ray_march_dim<256>(r, st));
 }
 
 cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st) {

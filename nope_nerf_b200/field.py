@@ -122,6 +122,46 @@ def _field_tc(net, flags, p, d):
     return out
 
 
+MARCH_BLOCK = 128   # steps one round of nnb_ray_march advances every ray that is still searching
+
+
+def ray_march(net, ray0, dirs, far, frac, near, n_secant, tau, want_bracket=False):
+    """nnb_ray_march: Renderer.ray_marching + Renderer.secant for N rays in one call on the tensor-core engine, without points or
+    occupancies in global memory.  ray0, dirs (N, 3); far (N,) per-ray far depth; frac (n_steps,) = torch.linspace(0, 1, n_steps); near,
+    tau floats.  Returns depth (N,): the refined depth on a hit, 0 where the first sample is occupied, inf otherwise; bit-identical to
+    the torch march over field_query(engine='tc', occ_only=True).  No autograd.
+    want_bracket: returns (depth, first (N,) int32, bracket (N, 4), counts) with first / bracket as nnb_ray_march documents them and
+    counts (rounds + 1,) int32 = [rays that hit, rays that took part in round 1, 2, ...] (round 0 takes every ray)."""
+    ops._need_cuda(ray0, "ray0")
+    N, n_steps, dev = ray0.shape[0], frac.shape[0], ray0.device
+    depth = torch.empty(N, device=dev)
+    first = torch.empty(N, dtype=torch.int32, device=dev) if want_bracket else None
+    bracket = torch.empty(N, 4, device=dev) if want_bracket else None
+    rounds = (n_steps + MARCH_BLOCK - 1) // MARCH_BLOCK
+    if N == 0:
+        return (depth, first, bracket, torch.zeros(rounds + 1, dtype=torch.int32, device=dev)) if want_bracket else depth
+    a = L.RayMarchArgs()
+    keep = [net.flat_weights()] + [ops._f32c(t.detach()) for t in (ray0, dirs, far, frac)]
+    a.weights, a.ray0, a.ray_dir, a.far_, a.frac = [L.ptr(t) for t in keep]
+    a.N = N; a.n_steps = n_steps; a.n_secant = n_secant; a.hidden_dim = net.hidden_dim
+    a.near_ = near; a.tau = tau; a.flags = _field_flags(net); a.engine = L.ENGINE_TC
+    a.depth = L.ptr(depth); a.first = L.ptr(first); a.bracket = L.ptr(bracket)
+    ws = ops._pool.take(L.lib.nnb_ray_march_workspace_bytes(N, n_steps, net.hidden_dim), dev)
+    a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+    try:
+        L.check(L.lib.nnb_ray_march(C.byref(a), ops._stream()), "nnb_ray_march")
+        counts = ws[:4 * (rounds + 1)].view(torch.int32).clone() if want_bracket else None
+    finally:
+        ops._pool.give(ws)   # stream-ordered: the next call on this stream that takes it runs after this one
+    return (depth, first, bracket, counts) if want_bracket else depth
+
+
+def needs_grad(net, *tensors):
+    """whether a field call on these inputs has to be differentiable: grad mode is on and an input or a parameter of net requires grad"""
+    return torch.is_grad_enabled() and (any(t is not None and t.requires_grad for t in tensors)
+                                        or any(q.requires_grad for q in net.parameters()))
+
+
 def _engine_id(engine):
     if engine is None or engine in (L.ENGINE_SIMT, L.ENGINE_TC):
         return engine
@@ -148,9 +188,7 @@ def field_query(net, p, ray_d, raw_density=False, occ_only=False, engine=None):
         z = p.reshape(-1, 3)[:, :1] * 0.0      # stays connected to p, like an empty result of the library would
         return z.expand(-1, 3).reshape(*shp, 3), z.reshape(*shp, 1)
     if _engine_id(engine) == L.ENGINE_TC:
-        needs_grad = torch.is_grad_enabled() and (p.requires_grad or (d is not None and d.requires_grad)
-                                                  or any(q.requires_grad for q in net.parameters()))
-        if not needs_grad:
+        if not needs_grad(net, p, d):
             out = _field_tc(net, flags | (L.OCC_ONLY if occ_only else 0), p.reshape(-1, 3), d)
             return out[:, :3].reshape(*shp, 3), out[:, 3].reshape(*shp, 1)
     rgb, a = _FieldFn.apply(flags, net, net.flat_weights(), p.reshape(-1, 3), d, *list(net.parameters()))

@@ -4,6 +4,8 @@ MLP, compositing) is one call into the CUDA library with autograd glue."""
 import torch
 import torch.nn as nn
 from .. import ops
+from .. import _lib as L
+from ..field import ray_march, needs_grad, _engine_id
 
 
 class Renderer(nn.Module):
@@ -17,7 +19,8 @@ class Renderer(nn.Module):
         self.model = model.to(device)
         self.engine = kwargs.get("engine", None)
         # engine of the geometry view's explicit-point queries (ray marching, secant steps, surface colour): None = exact fp32,
-        # 'tc' = tensor cores (OfficialStaticNerf.forward(engine=)).  The normals stay on gradient(), which is exact fp32.
+        # 'tc' = tensor cores (OfficialStaticNerf.forward(engine=)); ray marching and the secant steps are then one fused call
+        # (field.ray_march).  The normals stay on gradient(), which is exact fp32.
         self.field_engine = kwargs.get("field_engine", None)
 
     def to(self, device):
@@ -168,17 +171,33 @@ class Renderer(nn.Module):
 
     def ray_marching(self, ray0, ray_direction, model, c=None, tau=0.5, n_steps=[128, 129], n_secant_steps=8, depth_range=[0., 2.4],
                      max_points=3500000, rad=1.0):
-        """rendering.py:274-384: first sign change of (occupancy - tau) along each ray, refined by the secant method"""
+        """rendering.py:274-384: first sign change of (occupancy - tau) along each ray, refined by the secant method.  With
+        field_engine='tc' and no gradient needed (the rule of field.field_query) the march and the secant steps are one fused call into
+        the library; it returns the bits the torch march below returns on that engine."""
         batch_size, n_pts, _ = ray0.shape
         dev = ray0.device
         tau = 0.5
         n_steps = int(torch.randint(n_steps[0], n_steps[1], (1,)).item())
+        if _engine_id(self.field_engine) == L.ENGINE_TC and not needs_grad(model, ray0, ray_direction) and ray0.is_cuda:
+            d_intersect = self._sphere_far(ray0[:, 0], ray_direction, rad)
+            frac = torch.linspace(0, 1, steps=n_steps, device=dev)
+            return ray_march(model, ray0.reshape(-1, 3), ray_direction.reshape(-1, 3), d_intersect.reshape(-1), frac,
+                             float(depth_range[0]), n_secant_steps, tau).view(batch_size, n_pts)
+        return self._ray_marching_torch(ray0, ray_direction, model, n_steps, n_secant_steps, depth_range, max_points, rad,
+                                        self.field_engine)
+
+    def _ray_marching_torch(self, ray0, ray_direction, model, n_steps, n_secant_steps, depth_range, max_points, rad, engine):
+        """the march in torch over explicit-point field queries on `engine`: the exact engine's path, and the reference the fused
+        march is checked against"""
+        batch_size, n_pts, _ = ray0.shape
+        dev = ray0.device
+        tau = 0.5
         d_intersect = self._sphere_far(ray0[:, 0], ray_direction, rad)
         d_proposal = torch.linspace(0, 1, steps=n_steps, device=dev).view(1, 1, n_steps, 1)
         d_proposal = depth_range[0] * (1. - d_proposal) + d_intersect.view(1, -1, 1, 1) * d_proposal
         p_proposal = ray0.unsqueeze(2) + ray_direction.unsqueeze(2) * d_proposal
         with torch.no_grad():
-            val = torch.cat([model(p_split, only_occupancy=True, engine=self.field_engine) - tau
+            val = torch.cat([model(p_split, only_occupancy=True, engine=engine) - tau
                              for p_split in torch.split(p_proposal.reshape(batch_size, -1, 3), int(max_points / batch_size), dim=1)],
                             dim=1).view(batch_size, -1, n_steps)
         mask_0_not_occupied = val[:, :, 0] < 0
@@ -201,18 +220,22 @@ class Renderer(nn.Module):
         ray0_masked = ray0[mask]; ray_direction_masked = ray_direction[mask]
         d_pred_out = torch.ones(batch_size, n_pts, device=dev)
         if ray0_masked.shape[0] != 0:
-            d_pred_out[mask] = self.secant(f_low, f_high, d_low, d_high, n_secant_steps, ray0_masked, ray_direction_masked, tau)
+            d_pred_out[mask] = self._secant(f_low, f_high, d_low, d_high, n_secant_steps, ray0_masked, ray_direction_masked, tau, 0,
+                                            engine)
         d_pred_out[mask == 0] = float('inf')
         d_pred_out[mask_0_not_occupied == 0] = 0
         return d_pred_out
 
     def secant(self, f_low, f_high, d_low, d_high, n_secant_steps, ray0_masked, ray_direction_masked, tau, it=0):
         """rendering.py:386-418"""
+        return self._secant(f_low, f_high, d_low, d_high, n_secant_steps, ray0_masked, ray_direction_masked, tau, it, self.field_engine)
+
+    def _secant(self, f_low, f_high, d_low, d_high, n_secant_steps, ray0_masked, ray_direction_masked, tau, it, engine):
         d_pred = -f_low * (d_high - d_low) / (f_high - f_low) + d_low
         for _ in range(n_secant_steps):
             p_mid = ray0_masked + d_pred.unsqueeze(-1) * ray_direction_masked
             with torch.no_grad():
-                f_mid = self.model(p_mid, batchwise=False, only_occupancy=True, it=it, engine=self.field_engine)[..., 0] - tau
+                f_mid = self.model(p_mid, batchwise=False, only_occupancy=True, it=it, engine=engine)[..., 0] - tau
             ind_low = f_mid < 0
             d_low = torch.where(ind_low, d_pred, d_low); f_low = torch.where(ind_low, f_mid, f_low)
             d_high = torch.where(ind_low, d_high, d_pred); f_high = torch.where(ind_low, f_high, f_mid)

@@ -1,7 +1,10 @@
 #!/usr/bin/env python
 """Cost of explicit-point field queries (nnb_field_fwd) on the exact-fp32 engine, the tensor-core engine, and the tensor-core engine
 with NNB_OCC_ONLY, for M points x model.hidden_dim D; and of one geometry frame (Renderer.phong_renderer: 512-step ray marching,
-8 secant steps, normals, surface colour) with Renderer(field_engine=None) against field_engine='tc'.
+8 secant steps, normals, surface colour) with Renderer(field_engine=None), with field_engine='tc' through the torch march over
+explicit-point queries (Renderer._ray_marching_torch), and with field_engine='tc' as it runs (the fused march, nnb_ray_march); for the
+fused march also the share of the frame's rays that take part in each 128-step round, and one ray_march call over the whole frame
+instead of 1024-pixel chunks.
 
 CUDA events around each call.  Every shape is warmed up first; then every configuration is timed in each of --rounds rounds, the
 configurations alternating within a round, and the JSON line gives the median and the range over the rounds.  FLOP per point come from
@@ -72,13 +75,17 @@ def field_fn(L, ops, flat, D, p, d, flags, engine):
     return call
 
 
-def geometry_frame(H, W, warmup, reps, rounds):
-    """one phong_renderer frame of H x W pixels in chunks of 1024 pixels (the chunk size of render_visdata / render_geometry)"""
+def geometry_frame(H, W, D, warmup, reps, rounds):
+    """one phong_renderer frame of H x W pixels in chunks of 1024 pixels (the chunk size of render_visdata / render_geometry).  The
+    field is the seeded geometry field of the tests at width D (tests/_fullsize_cases.start_state(geo=True), net seed 31): the share of
+    rays each round of the fused march still carries depends on it."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import _fullsize_cases as FC
     import nope_nerf_b200.model as mdl
+    from nope_nerf_b200 import field
     from nope_nerf_b200.model import common as mc
     cfg = FC.default_cfg()
+    cfg["model"]["hidden_dim"] = D
     state = FC.start_state(cfg, 4, 31, 95, geo=True)
     dev = torch.device("cuda")
     net = mdl.OfficialStaticNerf(cfg)
@@ -90,16 +97,39 @@ def geometry_frame(H, W, warmup, reps, rounds):
     with torch.no_grad():
         pose.r.copy_(state["r"]); pose.t.copy_(state["t"])
         wmat = torch.inverse(pose(1)).unsqueeze(0)
+    class TorchMarch(mdl.Renderer):   # field_engine's queries through the torch march, as before the fused march existed
+        def ray_marching(self, ray0, ray_direction, model, c=None, tau=0.5, n_steps=[128, 129], n_secant_steps=8, depth_range=[0., 2.4],
+                         max_points=3500000, rad=1.0):
+            n = int(torch.randint(n_steps[0], n_steps[1], (1,)).item())
+            return self._ray_marching_torch(ray0, ray_direction, model, n, n_secant_steps, depth_range, max_points, rad, self.field_engine)
+
     fns = {}
-    for name, fe in (("exact", None), ("tc", "tc")):
-        rend = mdl.Renderer(net, cfg["rendering"], device=dev, field_engine=fe)
+    for name, cls, fe in (("exact", mdl.Renderer, None), ("tc_torch_march", TorchMarch, "tc"), ("tc", mdl.Renderer, "tc")):
+        rend = cls(net, cfg["rendering"], device=dev, field_engine=fe)
 
         def frame(rend=rend):
             for px in torch.split(pixels, 1024, dim=1):
                 rend(px, None, cam, wmat, smat, "phong_renderer", it=0)
         fns[name] = frame
+    # the march of the whole frame as one nnb_ray_march call (no renderer around it), and what it reports about the rounds
+    net = net.to(dev).eval()
+    for q in net.parameters():
+        q.requires_grad_(False)
+    with torch.no_grad():
+        cw, rv = rend._rays_world(pixels, cam, wmat, smat)
+        far = rend._sphere_far(cw[:, 0], rv, cfg["rendering"]["radius"]).reshape(-1).contiguous()
+    ray0, dirs = cw.reshape(-1, 3).contiguous(), rv.reshape(-1, 3).contiguous()
+    frac = torch.linspace(0, 1, steps=512, device=dev)
+    fns["march_one_call"] = lambda: field.ray_march(net, ray0, dirs, far, frac, 0.0, 8, 0.5)
     ts = rounds_of(fns, warmup, reps, rounds)
-    return {k: summary(v) for k, v in ts.items()}
+    depth, first, _, counts = field.ray_march(net, ray0, dirs, far, frac, 0.0, 8, 0.5, want_bracket=True)
+    n = ray0.shape[0]
+    out = {k: summary(v) for k, v in ts.items()}
+    out["rays"] = n
+    out["rays_hit_share"] = float(counts[0]) / n
+    out["rays_in_round_share"] = [1.0] + [float(c) / n for c in counts[1:-1].tolist()]   # round k = steps 128 k .. 128 k + 127
+    out["tiles_evaluated_over_all_steps"] = (n + int(counts[1:-1].sum())) / (n * 4.0)
+    return out
 
 
 def main():
@@ -111,6 +141,7 @@ def main():
     ap.add_argument("--dims", type=int, nargs="*", default=list(DIMS))
     ap.add_argument("--frame", type=int, nargs=2, default=[270, 480], metavar=("H", "W"), help="geometry frame size; 0 0 skips it")
     ap.add_argument("--frame-reps", type=int, default=1)
+    ap.add_argument("--frame-dims", type=int, nargs="*", default=[256, 128, 64])
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("field_query_cost: needs a CUDA device (there is no CPU path and a CPU timing would say nothing about the GPU)")
@@ -144,8 +175,11 @@ def main():
             torch.cuda.empty_cache()
     H, W = args.frame
     if H > 0 and W > 0:
-        fr = geometry_frame(H, W, 1, args.frame_reps, args.rounds)
-        res["geometry_frame"] = {"H": H, "W": W, "hidden_dim": 256, **fr, "exact_over_tc": fr["exact"]["median_ms"] / fr["tc"]["median_ms"]}
+        res["geometry_frame"] = []
+        for D in args.frame_dims:
+            fr = geometry_frame(H, W, D, 1, args.frame_reps, args.rounds)
+            res["geometry_frame"].append({"H": H, "W": W, "hidden_dim": D, **fr, "exact_over_tc": fr["exact"]["median_ms"] / fr["tc"]["median_ms"],
+                                          "tc_torch_march_over_tc": fr["tc_torch_march"]["median_ms"] / fr["tc"]["median_ms"]})
     print(json.dumps(res))
 
 
