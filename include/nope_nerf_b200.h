@@ -32,15 +32,13 @@ extern "C" {
 #define NNB_SOFTPLUS 64u    /* model.occ_activation == 'softplus' (official_nerf.py:77-80)        */
 #define NNB_SHIFT_FIRST 128u /* training.shift_first    (training.py:241-245)                     */
 #define NNB_STASH 256u      /* keep activations in the workspace for nnb_render_bwd               */
-#define NNB_TCBWD 512u      /* operand-plane backward of the TC engine: not available in the sm_90a library (rc < 0) */
 #define NNB_RAW_DENSITY 2048u /* nnb_field_fwd/bwd only: out_rgba[3] = the density LOGIT (fc_density output, official_nerf.py:66-67
                                 * infer_occ) instead of alpha / sigma; used for OfficialStaticNerf.gradient() (normals)            */
-#define NNB_FWD_DROP_WLO 4096u /* forward precision experiment: rejected (rc -7) by this library */
-#define NNB_FWD_DROP_ALO 8192u /* forward precision experiment: rejected (rc -7) by this library */
-#define NNB_WG16 1024u      /* with NNB_TCBWD only (fp16 weight-gradient operand planes); without it the flag has no effect */
 #define NNB_HVP 16384u      /* with NNB_STASH on NNB_ENGINE_SIMT: the workspace also holds the tangent stash of nnb_field_hvp; sizes only */
 #define NNB_OCC_ONLY 32768u /* nnb_field_fwd on NNB_ENGINE_TC only: out_rgba = (0, 0, 0, a); the colour branch (fc_feature, rgb_layers.0,
                              * fc_rgb) is not evaluated.  a is bit-identical to the full query's (OfficialStaticNerf.forward(only_occupancy=True)) */
+/* A flag bit not defined above is rejected (rc -7) by nnb_render_fwd / bwd, nnb_field_fwd / bwd / hvp and nnb_debug_wgrad, and
+ * nnb_workspace_bytes(_dim) returns 0 for it.  Bits 512, 1024, 4096 and 8192 were defined before version 105 and are rejected too. */
 
 /* engines */
 #define NNB_ENGINE_SIMT 0 /* exact fp32 FMA path                                        */
@@ -97,17 +95,15 @@ typedef struct nnb_render_bwd_args {
   float* g_cam;     /* [16] ([0],[5] written) or NULL */
   float* g_depth;   /* [N] d/d prior depth (overwritten) or NULL */
   float* g_scale_shift; /* [2] d/d scale, d/d shift when depth_map is used, or NULL */
-  /* 0 = whole backward.  A caller may issue it in two calls (1, then 2) to fork independent work beside it; this library does
-   * everything in phase 1 (or 0) and nothing in phase 2. */
-  uint32_t phase;
-  /* state of the fp16 weight-gradient planes (NNB_WG16 with NNB_TCBWD); unused by this library, may be NULL */
-  float* wg_state;
-  uint32_t wg_seed;
 } nnb_render_bwd_args;
 
 const char* nnb_last_error(void);
 int nnb_version(void);   /* >= 101: nnb_chamfer with adjoints takes nnb_chamfer_workspace_bytes(P, Q) of keys; >= 102: nnb_field_hvp;
-                          * >= 103: nnb_field_fwd honours NNB_ENGINE_TC, NNB_OCC_ONLY; >= 104: nnb_ray_march */
+                          * >= 103: nnb_field_fwd honours NNB_ENGINE_TC, NNB_OCC_ONLY; >= 104: nnb_ray_march;
+                          * >= 105: nnb_render_bwd_args ends at g_scale_shift.  Its former trailing fields phase, wg_state and wg_seed are
+                          *   gone, so every nnb_render_bwd call runs the whole backward: a caller that still issues a phase-1 call and
+                          *   then a phase-2 call runs the backward twice.  NNB_TCBWD (512), NNB_WG16 (1024), NNB_FWD_DROP_WLO (4096)
+                          *   and NNB_FWD_DROP_ALO (8192) are removed and rejected as undefined bits. */
 /* Profiling hook used by bench.py: `events` is a HOST array of cudaEvent_t handles that stays alive until
  * nnb_profile_events(NULL,0).  Every nnb_render_fwd records 4 marks (start, weights imaged, field done,
  * composited) and every nnb_render_bwd 5 marks (start, compositing adjoint, data-gradient chain,
@@ -118,12 +114,11 @@ int nnb_profile_cursor(void);
 int nnb_debug_layout(int32_t N, int32_t S, uint32_t flags, int32_t engine, size_t* out14);
 /* test aid: the weight-gradient stage that nnb_render_bwd runs for a->engine, alone, on whatever the workspace's activation / output-
  * gradient stash holds (layout of nnb_debug_layout); g_weights [nnb_num_params(a->hidden_dim)] is ACCUMULATED (+=).  Reads a->N, S,
- * flags (NNB_STASH required; NNB_TCBWD, which no engine of this library runs, is rejected on both), engine, hidden_dim, workspace and
- * workspace_bytes only. */
+ * flags (NNB_STASH required), engine, hidden_dim, workspace and workspace_bytes only. */
 int nnb_debug_wgrad(const nnb_render_args* a, float* g_weights, void* stream);
-/* bytes of workspace needed by nnb_render_fwd (+bwd when NNB_STASH) at hidden_dim 256 */
+/* bytes of workspace needed by nnb_render_fwd (+bwd when NNB_STASH) at hidden_dim 256; 0 for an undefined flag bit */
 size_t nnb_workspace_bytes(int32_t N, int32_t S, uint32_t flags, int32_t engine);
-/* the same for the field of width hidden_dim (0 = 256); 0 for an unsupported width */
+/* the same for the field of width hidden_dim (0 = 256); 0 for an unsupported width or an undefined flag bit */
 size_t nnb_workspace_bytes_dim(int32_t N, int32_t S, uint32_t flags, int32_t engine, int32_t hidden_dim);
 /* floats of the flat MLP parameter vector of width hidden_dim (0 = 256; NNB_NUM_PARAMS at 256); 0 for an unsupported width */
 size_t nnb_num_params(int32_t hidden_dim);

@@ -11,8 +11,7 @@ LIB_PATH = os.environ.get("NNB_LIB_PATH") or os.path.join(HERE, "libnope_nerf_b2
 
 NUM_PARAMS = 595844              # hidden_dim 256; num_params(D) for the other widths
 HIDDEN_DIMS = (64, 128, 256)     # model.hidden_dim values with a kernel instantiation
-DIST_ALPHA, NDC, NORMALISE, USE_DIR, WHITE_BG, EVAL, SOFTPLUS, SHIFT_FIRST, STASH, TCBWD, WG16, RAW_DENSITY = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048
-FWD_DROP_WLO, FWD_DROP_ALO = 4096, 8192
+DIST_ALPHA, NDC, NORMALISE, USE_DIR, WHITE_BG, EVAL, SOFTPLUS, SHIFT_FIRST, STASH, RAW_DENSITY = 1, 2, 4, 8, 16, 32, 64, 128, 256, 2048
 HVP = 16384                      # with STASH: workspace of nnb_field_hvp (second-order field backward)
 OCC_ONLY = 32768                 # nnb_field_fwd on ENGINE_TC: density only, out = (0, 0, 0, a)
 ENGINE_SIMT, ENGINE_TC = 0, 1
@@ -39,8 +38,7 @@ class RayMarchArgs(C.Structure):   # nnb_ray_march_args
 
 class RenderBwdArgs(C.Structure):
     _fields_ = [("fwd", RenderArgs), ("g_rgb", _f), ("g_depth_pred", _f), ("g_depth_gt", _f),
-                ("g_weights", _f), ("g_c2w", _f), ("g_cam", _f), ("g_depth", _f), ("g_scale_shift", _f), ("phase", C.c_uint32),
-                ("wg_state", _f), ("wg_seed", C.c_uint32)]
+                ("g_weights", _f), ("g_c2w", _f), ("g_cam", _f), ("g_depth", _f), ("g_scale_shift", _f)]
 
 
 class RefStageArgs(C.Structure):

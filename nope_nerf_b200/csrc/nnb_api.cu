@@ -63,8 +63,8 @@ extern "C" {
 
 const char* nnb_last_error(void) { return g_err; }
 // 101: nnb_chamfer with adjoints needs nnb_chamfer_workspace_bytes(P, Q) of keys; 102: nnb_field_hvp; 103: nnb_field_fwd on NNB_ENGINE_TC;
-// 104: nnb_ray_march
-int nnb_version(void) { return 104; }
+// 104: nnb_ray_march; 105: one-call backward, undefined flag bits rejected (see the header)
+int nnb_version(void) { return 105; }
 int nnb_profile_events(void** events, int32_t count) {
   g_prof_events = reinterpret_cast<cudaEvent_t*>(events); g_prof_n = events ? count : 0; g_prof_i = 0;
   return 0;
@@ -83,6 +83,14 @@ int nnb_debug_layout(int32_t N, int32_t S, uint32_t flags, int32_t engine, size_
 // model.hidden_dim of a call: 0 means 256
 static int hidden_of(int32_t hidden_dim) { return hidden_dim == 0 ? 256 : hidden_dim; }
 
+// every rendering flag the header defines; any other bit (among them those of options removed in version 105) is an error
+static constexpr uint32_t KNOWN_FLAGS = NNB_DIST_ALPHA | NNB_NDC | NNB_NORMALISE | NNB_USE_DIR | NNB_WHITE_BG | NNB_EVAL | NNB_SOFTPLUS |
+                                        NNB_SHIFT_FIRST | NNB_STASH | NNB_RAW_DENSITY | NNB_HVP | NNB_OCC_ONLY;
+static int check_flags(uint32_t flags) {
+  if (flags & ~KNOWN_FLAGS) return fail(-7, "flags 0x%x: bits 0x%x are not defined by this library", flags, flags & ~KNOWN_FLAGS);
+  return 0;
+}
+
 size_t nnb_num_params(int32_t hidden_dim) {
   const int D = hidden_of(hidden_dim);
   return nnb::dim_supported(D) ? (size_t)nnb::num_params(D) : 0;
@@ -90,7 +98,7 @@ size_t nnb_num_params(int32_t hidden_dim) {
 
 size_t nnb_workspace_bytes_dim(int32_t N, int32_t S, uint32_t flags, int32_t engine, int32_t hidden_dim) {
   const int D = hidden_of(hidden_dim);
-  if (N <= 0 || S <= 0 || !nnb::dim_supported(D)) return 0;
+  if (N <= 0 || S <= 0 || !nnb::dim_supported(D) || (flags & ~KNOWN_FLAGS)) return 0;
   WsLayout L = make_layout(N, S, flags, engine, D);
   size_t tot = L.total;
 #ifdef NNB_WITH_TC
@@ -121,8 +129,9 @@ static int check_args(const nnb_render_args* a) {
   return check_engine_ws(a);
 }
 
-// engine, width, the engine's S range, and the workspace's size and alignment
+// flags, engine, width, the engine's S range, and the workspace's size and alignment
 static int check_engine_ws(const nnb_render_args* a) {
+  if (int rc = check_flags(a->flags)) return rc;
   if (a->engine != NNB_ENGINE_SIMT && a->engine != NNB_ENGINE_TC) return fail(-4, "unknown engine %d", a->engine);
   if (int rc = check_dim(a)) return rc;
 #ifndef NNB_WITH_TC
@@ -140,10 +149,6 @@ static int check_engine_ws(const nnb_render_args* a) {
 
 int nnb_render_fwd(const nnb_render_args* a, void* stream) {
   int rc = check_args(a); if (rc) return rc;
-#ifndef NNB_FWD_SPLIT_EXPERIMENT
-  if (a->flags & (NNB_FWD_DROP_WLO | NNB_FWD_DROP_ALO))
-    return fail(-7, "NNB_FWD_DROP_* (forward precision experiment) is not built into this library");
-#endif
   WsLayout L = make_layout(a->N, a->S, a->flags, a->engine, hidden_of(a->hidden_dim));
   cudaError_t e;
 #ifdef NNB_WITH_TC
@@ -158,13 +163,12 @@ int nnb_render_bwd(const nnb_render_bwd_args* b, void* stream) {
   int rc = check_args(&b->fwd); if (rc) return rc;
   if (!(b->fwd.flags & NNB_STASH)) return fail(-6, "nnb_render_bwd needs the forward call to have run with NNB_STASH");
   if (!b->g_rgb || !b->g_c2w) return fail(-3, "g_rgb and g_c2w must be non-null");
-  if (b->phase > 2) return fail(-2, "nnb_render_bwd: phase must be 0, 1 or 2");
   WsLayout L = make_layout(b->fwd.N, b->fwd.S, b->fwd.flags, b->fwd.engine, hidden_of(b->fwd.hidden_dim));
   cudaError_t e;
 #ifdef NNB_WITH_TC
   if (b->fwd.engine == NNB_ENGINE_TC) e = tc_render_bwd(*b, L, (cudaStream_t)stream); else
 #endif
-  e = (b->phase == 2) ? cudaSuccess : simt_render_bwd(*b, L, (cudaStream_t)stream);
+  e = simt_render_bwd(*b, L, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_bwd");
 }
 
@@ -173,7 +177,7 @@ int nnb_debug_wgrad(const nnb_render_args* a, float* g_weights, void* stream) {
   if (!a || !g_weights) return fail(-3, "nnb_debug_wgrad: need args and g_weights");
   if (a->N <= 0) return fail(-2, "N must be positive (got %d)", a->N);
   if (a->S < 2 || a->S > 1024) return fail(-2, "S must be in [2,1024] (got %d)", a->S);
-  if (!(a->flags & NNB_STASH) || (a->flags & NNB_TCBWD)) return fail(-6, "nnb_debug_wgrad needs the fp32 stash layout (NNB_STASH without NNB_TCBWD)");
+  if (!(a->flags & NNB_STASH)) return fail(-6, "nnb_debug_wgrad needs the stash (NNB_STASH)");
   if (int rc = check_engine_ws(a)) return rc;
   WsLayout L = make_layout(a->N, a->S, a->flags, a->engine, hidden_of(a->hidden_dim));
   cudaError_t e;
@@ -186,6 +190,7 @@ int nnb_debug_wgrad(const nnb_render_args* a, float* g_weights, void* stream) {
 
 static int check_field(const nnb_render_args* a) {
   if (!a || !a->pts || !a->weights || a->N <= 0) return fail(-3, "nnb_field_*: need pts, weights, N > 0");
+  if (int rc = check_flags(a->flags)) return rc;
   if (int rc = check_dim(a)) return rc;
   size_t need = make_layout(a->N, 1, a->flags, NNB_ENGINE_SIMT, hidden_of(a->hidden_dim)).total;
   if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
@@ -254,8 +259,8 @@ int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, f
 int nnb_field_hvp(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream) {
   int rc = check_field(a); if (rc) return rc;
   if (!u || (!g_pts && !g_weights)) return fail(-3, "nnb_field_hvp: need u and at least one of g_pts, g_weights");
-  if (!(a->flags & NNB_STASH) || !(a->flags & NNB_HVP) || (a->flags & NNB_TCBWD))
-    return fail(-6, "nnb_field_hvp: flags must contain NNB_STASH | NNB_HVP (without NNB_TCBWD), and the workspace be sized with them");
+  if (!(a->flags & NNB_STASH) || !(a->flags & NNB_HVP))
+    return fail(-6, "nnb_field_hvp: flags must contain NNB_STASH | NNB_HVP, and the workspace be sized with them");
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
   if ((reinterpret_cast<uintptr_t>(u) & 15) != 0 || (reinterpret_cast<uintptr_t>(g_pts) & 15) != 0)
     return fail(-3, "nnb_field_hvp: u and g_pts must be 16-byte aligned [N][4] arrays");

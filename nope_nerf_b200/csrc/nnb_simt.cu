@@ -289,9 +289,7 @@ __global__ void composite_fwd(nnb_render_args a, const SampleRec* recs) {
   }
 }
 
-// gmax (optional): running max |g| over all samples, as uint bits of a non-negative float
-// (feeds the power-of-two gradient scaling of an operand-plane backward)
-__global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, float4* gs, unsigned int* gmax) {
+__global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, float4* gs) {
   const nnb_render_args& a = b.fwd;
   const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (n >= a.N) return;
@@ -324,7 +322,7 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
   }
   // reverse sweep: each chunk's terms recomputed from the records with the same operations, then the in-chunk suffix scan with the
   // suffix of the later chunks carried in
-  float carry_s = 0.f, vmax = 0.f;
+  float carry_s = 0.f;
   for (int c = C - 1; c >= 0; --c) {
     const int i = c * 32 + lane; const bool valid = i < a.S;
     float alpha, om, incl_p, T;
@@ -344,16 +342,7 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
     float suffix = excl + carry_s;
     carry_s += __shfl_sync(0xffffffffu, incl, 0);
     float g_alpha = T * gw - suffix / om;
-    if (valid) {
-      float4 o = make_float4(w * gC0, w * gC1, w * gC2, g_alpha * df);
-      gs[(size_t)n * a.S + i] = o;
-      vmax = fmaxf(vmax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
-    }
-  }
-  if (gmax) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
-    if (lane == 0 && isfinite(vmax)) atomicMax(gmax, __float_as_uint(vmax));
+    if (valid) gs[(size_t)n * a.S + i] = make_float4(w * gC0, w * gC1, w * gC2, g_alpha * df);
   }
 }
 
@@ -1115,7 +1104,7 @@ cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L
   cudaError_t e0 = simt_init();
   if (e0 != cudaSuccess) return e0;
   nnb_prof_mark(st);
-  composite_bwd<<<(a.N + 7) / 8, 256, 0, st>>>(b, P.rec, P.gs, nullptr);
+  composite_bwd<<<(a.N + 7) / 8, 256, 0, st>>>(b, P.rec, P.gs);
   nnb_prof_mark(st);
   const int write_dy = b.g_weights ? 1 : 0;
   if (dgrad) { cudaError_t ed = dgrad(b, L, write_dy, st); if (ed != cudaSuccess) return ed; }

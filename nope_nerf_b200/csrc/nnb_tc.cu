@@ -1401,7 +1401,6 @@ bool tc_supports(int S) { return S >= 16 && S <= 1024; }
 
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st) {
   if (!tc_supports(a.S)) return cudaErrorNotSupported;
-  if (a.flags & NNB_TCBWD) return cudaErrorNotSupported;   // the operand-plane stash is not implemented for sm_90a
   return L.D == 128 ? tc_render_fwd_dim<128>(a, L, st) : (L.D == 64 ? tc_render_fwd_dim<64>(a, L, st) : tc_render_fwd_dim<256>(a, L, st));
 }
 
@@ -1418,10 +1417,9 @@ cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, flo
 }
 
 // Backward of the TC engine: compositing / ray adjoints of nnb_simt.cu around tc_dgrad and tc_wgrad, which read and write the SIMT
-// engine's fp32 stash layout.  The second phase of a split backward has nothing left to do.
+// engine's fp32 stash layout.
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st) {
-  if (b.fwd.flags & NNB_TCBWD) return cudaErrorNotSupported;
-  return b.phase == 2 ? cudaSuccess : simt_render_bwd_with(b, L, st, tc_dgrad_launch, tc_wgrad_all);
+  return simt_render_bwd_with(b, L, st, tc_dgrad_launch, tc_wgrad_all);
 }
 
 // the weight-gradient stage of tc_render_bwd alone, on whatever the stash holds (nnb_debug_wgrad)

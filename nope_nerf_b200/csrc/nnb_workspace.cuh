@@ -20,17 +20,8 @@ struct WsLayout {
   size_t th[8], tenc;
   // TC engine: ReLU gate bits (h > 0) of h0..h7 and the rgb hidden layer, written by tc_field_fwd, read by tc_dgrad (see gate_bits_off)
   size_t gates;
-  // operand-plane backward (NNB_TCBWD; rejected by the sm_90a library): activations / output-gradients as per-tile bf16 hi|lo
-  // operand planes ([tile][hi|lo][sample half][feature/8][64 samples][8 features]) + ReLU bitmasks
-  size_t n_tiles;
-  size_t xp[10];    // X planes: 0 = enc (64 feat), 1..8 = h0..h7, 9 = feat
-  size_t dyp[10];   // dY planes: 0..7 = dy0..dy7, 8 = dfeat, 9 = dyr (128 feat)
-  size_t mask;      // uint32 [9 layers][Mpad][8]: ReLU sign bits of h0..h7 and (slot 8, 4 words) of the rgb hidden layer
-  size_t gmax;      // uint32 bits of max |g| (gradient scaling)
-  size_t wgstate;   // NNB_WG16 scratch state (32 floats) for calls without a caller-owned wg_state
   size_t total;  // bytes
 };
-constexpr size_t PLANE_TILE_256 = 131072, PLANE_TILE_128 = 65536, PLANE_TILE_64 = 32768;
 
 // weight-gradient stage of a backward that consumes the fp32 stash: accumulates every MLP parameter gradient into gw
 typedef cudaError_t (*WgradFn)(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
@@ -99,30 +90,17 @@ inline WsLayout make_layout(int N, int S, uint32_t flags, int engine, int D = 25
   if (flags & NNB_STASH) {
     L.gs = take(L.Mpad * 16); L.gp = take(L.Mpad * 16); L.gv = take(L.Mpad * 16);
     L.rayred = take((size_t)N * 16 * 4); L.wpart = take(wpart_floats(L.M, D) * 4);
-    L.n_tiles = L.Mpad / 128;
-    if (engine == NNB_ENGINE_TC && (flags & NNB_TCBWD)) {
-      // small fp32 side stashes (heads) + operand planes
-      L.h[7] = take(L.Mpad * 256 * 4); L.hr = take(L.Mpad * 128 * 4); L.denc = take(L.Mpad * 32 * 4);
-      L.dyr = take(L.Mpad * 128 * 4); L.dyc = take(L.Mpad * 16);
-      L.xp[0] = take(L.n_tiles * PLANE_TILE_64);
-      for (int i = 1; i < 10; ++i) L.xp[i] = take(L.n_tiles * PLANE_TILE_256);
-      for (int i = 0; i < 9; ++i) L.dyp[i] = take(L.n_tiles * PLANE_TILE_256);
-      L.dyp[9] = take(L.n_tiles * PLANE_TILE_128);
-      L.mask = take(L.Mpad * 9 * 8 * 4);
-      L.gmax = take(256);
-      L.wgstate = take(256);
-    } else {  // fp32 [sample][feature] stash (SIMT backward; also consumed after a TC forward)
-      const size_t d = (size_t)D, dr = (size_t)(D / 2);
-      for (int l = 0; l < 8; ++l) L.h[l] = take(L.Mpad * d * 4);
-      L.feat = take(L.Mpad * d * 4); L.hr = take(L.Mpad * dr * 4);
-      L.enc = take(L.Mpad * 64 * 4); L.denc = take(L.Mpad * 32 * 4);
-      for (int l = 0; l < 8; ++l) L.dy[l] = take(L.Mpad * d * 4);
-      L.dfeat = take(L.Mpad * d * 4); L.dyr = take(L.Mpad * dr * 4); L.dyc = take(L.Mpad * 16);
-      if (engine == NNB_ENGINE_TC) L.gates = take(gate_bits_bytes(L.Mpad, D));
-      if (engine == NNB_ENGINE_SIMT && (flags & NNB_HVP)) {   // Mpad rows: the SIMT kernels process whole 64-row tiles
-        for (int l = 0; l < 8; ++l) L.th[l] = take(L.Mpad * d * 4);
-        L.tenc = take(L.Mpad * 64 * 4);
-      }
+    // fp32 [sample][feature] stash, written by the forward of either engine and read by the backward
+    const size_t d = (size_t)D, dr = (size_t)(D / 2);
+    for (int l = 0; l < 8; ++l) L.h[l] = take(L.Mpad * d * 4);
+    L.feat = take(L.Mpad * d * 4); L.hr = take(L.Mpad * dr * 4);
+    L.enc = take(L.Mpad * 64 * 4); L.denc = take(L.Mpad * 32 * 4);
+    for (int l = 0; l < 8; ++l) L.dy[l] = take(L.Mpad * d * 4);
+    L.dfeat = take(L.Mpad * d * 4); L.dyr = take(L.Mpad * dr * 4); L.dyc = take(L.Mpad * 16);
+    if (engine == NNB_ENGINE_TC) L.gates = take(gate_bits_bytes(L.Mpad, D));
+    if (engine == NNB_ENGINE_SIMT && (flags & NNB_HVP)) {   // Mpad rows: the SIMT kernels process whole 64-row tiles
+      for (int l = 0; l < 8; ++l) L.th[l] = take(L.Mpad * d * 4);
+      L.tenc = take(L.Mpad * 64 * 4);
     }
   }
   L.total = o;

@@ -334,19 +334,15 @@ class _GraphStep:
         ws = call.ws
         call.pooled = False                                 # memory referenced by a captured graph never returns to the pool
         bw = (self.g_rgb, self.g_dp, None if tr.detach_gt_depth else self.g_dg, gbuf[:net.num_params], g_c2w, g_cam, None, g_ss)
-        wgk = tr._wg_kwargs()
-        if not self.use_ref:
-            call.backward(*bw, **wgk)
-        else:
+        call.backward(*bw)
+        if self.use_ref:
             # The reference-image stage only needs the two poses / distortions / frames.  It runs on a side stream that starts after
-            # the whole render backward (this library does all of it in phase 1 and nothing in phase 2), so it sits on the step's
-            # critical path.  The stage sums in a fixed order (the chamfer's adjoint groups exactly, in integers) and adds its pose /
-            # distortion gradients once per element into the buffers the render backward also accumulates into; because the backward
-            # has finished by then, those adds always land in the same order and the step is reproducible bit for bit.
-            call.backward(*bw, phase=1, **wgk)
+            # the whole render backward, so it sits on the step's critical path.  The stage sums in a fixed order (the chamfer's
+            # adjoint groups exactly, in integers) and adds its pose / distortion gradients once per element into the buffers the
+            # render backward also accumulates into; because the backward has finished by then, those adds always land in the same
+            # order and the step is reproducible bit for bit.
             cur = torch.cuda.current_stream()
             self.side.wait_stream(cur)
-            call.backward(*bw, phase=2, **wgk)
             with torch.cuda.stream(self.side):
                 ops.pose_fwd_dev(pose.r.detach(), pose.t.detach(), init, self.idx_ref, self.c2w_ref)
                 ops.distortion_fwd_dev(dnet.global_scales.detach(), dnet.global_shifts.detach(), self.idx_ref, dnet.fix_scaleN, self.ss_ref)
@@ -563,7 +559,6 @@ class Trainer(object):
             raise ValueError("dp_mode='rays': training.n_training_points (%d) must be a multiple of the world size (%d): every rank "
                              "takes ray_idx[rank::world] and the loss normalisation assumes equal shards" % (self.n_training_points, self.world))
         self._gbuf = None
-        self._wg_state = None; self._wg_seeded = False
         self._peer = None
         # data-parallel exchange: ONE kernel over NVLink peer memory (all-reduce fused with the Adam updates, captured in the step
         # graph); peer_exchange=False / NNB_PEER_EXCHANGE=0 falls back to torch.distributed.all_reduce between two graphs
@@ -583,16 +578,6 @@ class Trainer(object):
         self.pixel_sampler = kwargs.get('pixel_sampler', 'auto')
 
     # ------------------------------------------------------------------------------------
-    def _wg_kwargs(self):
-        """persistent dY-scale state of the fp16 weight-gradient planes (NNB_WG16 'delayed scaling'): every step's data-gradient chain
-        records max |dY_l|, the next step scales its fp16 dY planes with it; the very first step measures them in an extra pass"""
-        if self._wg_state is None:
-            self._wg_state = torch.zeros(32, device=self.device)
-            self._wg_seeded = False
-        kw = dict(wg_state=self._wg_state, wg_seed=not self._wg_seeded)
-        self._wg_seeded = True
-        return kw
-
     def _smoothness_on(self):
         """the pose-smoothness terms have a non-zero weight somewhere on their annealing schedule"""
         return any(float(v) != 0.0 for v in list(self.weight_dist_1st_loss) + list(self.weight_dist_2nd_loss))
@@ -914,7 +899,7 @@ class Trainer(object):
                 g_c2w = torch.zeros(4, 4, device=device)
                 g_ss = torch.zeros(2, device=device)
                 g_cam = torch.zeros(4, 4, device=device) if fxfy is not None else None
-                call.backward(g_rgb, g_dp, None if self.detach_gt_depth else g_dg, gbuf[:net.num_params], g_c2w, g_cam, None, g_ss, **self._wg_kwargs())
+                call.backward(g_rgb, g_dp, None if self.detach_gt_depth else g_dg, gbuf[:net.num_params], g_c2w, g_cam, None, g_ss)
                 ops.pose_bwd_raw(pose.r.detach(), pose.t.detach(), init, img_idx, g_c2w,
                                  gv['r'] if pose.r.requires_grad else None, gv['t'] if pose.t.requires_grad else None)
                 # chain d/d(scale_eff, shift) into global_scales / global_shifts (clamp / fixed-last-view aware)

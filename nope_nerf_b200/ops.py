@@ -6,38 +6,6 @@ import torch
 from . import _lib as L
 
 _DEFAULT_ENGINE = [L.ENGINE_TC]
-# operand-plane backward of the tensor-core engine (NNB_TCBWD): not implemented for sm_90a (the library rejects the flag); a TC
-# forward stashes fp32 activations, which the TC backward's wgmma data- / weight-gradient kernels read
-_TC_BACKWARD = [False]
-# weight-gradient operand planes of the operand-plane backward: 'fp16' = one fp16 plane per operand, per-layer power-of-two dY scales
-# from the previous step (NNB_WG16: half the stash traffic, a third of the MMAs, MLP weight gradients to ~3e-4);
-# 'exact' = bf16 hi|lo planes, three MMAs per product (MLP weight gradients to fp32 round-off).  NNB_WGRAD overrides.
-import os as _os
-_WGRAD = [_os.environ.get("NNB_WGRAD", "fp16")]
-# forward-precision EXPERIMENT of the tensor-core engine (DESIGN.md section 4; never the default): 0 = three-term split, 1 = without
-# a_hi*b_lo (NNB_FWD_DROP_WLO), 2 = without a_lo*b_hi (NNB_FWD_DROP_ALO), 3 = a_hi*b_hi only
-_FWD_DROP = [int(_os.environ.get("NNB_FWD_DROP", "0"))]
-
-
-def set_forward_split_experiment(mode):
-    if mode not in (0, 1, 2, 3):
-        raise ValueError("forward split experiment mode must be 0..3")
-    _FWD_DROP[0] = mode
-
-
-def set_wgrad_precision(mode):
-    if mode not in ("fp16", "exact"):
-        raise ValueError("wgrad precision must be 'fp16' or 'exact'")
-    _WGRAD[0] = mode
-
-
-def wgrad_precision():
-    return _WGRAD[0]
-
-
-
-def set_tc_backward(on):
-    _TC_BACKWARD[0] = bool(on)
 
 
 def set_default_engine(name):
@@ -123,7 +91,7 @@ class RenderCall:
     """One forward launch + the state its backward needs (workspace with the stash)."""
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
-                 depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, wgrad=None, hidden_dim=256):
+                 depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256):
         for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels),
                        ("depth", depth), ("noise", noise)):
             _need_cuda(t_, n_)
@@ -141,11 +109,6 @@ class RenderCall:
         engine = pick_engine(engine, S)
         if stash:
             flags |= L.STASH
-            if engine == L.ENGINE_TC and _TC_BACKWARD[0]:
-                flags |= L.TCBWD
-                if (wgrad or _WGRAD[0]) == "fp16": flags |= L.WG16
-        if engine == L.ENGINE_TC and _FWD_DROP[0]:
-            flags |= (_FWD_DROP[0] & 1) * L.FWD_DROP_WLO | ((_FWD_DROP[0] >> 1) & 1) * L.FWD_DROP_ALO
         a.flags = flags; a.engine = engine; a.hidden_dim = int(hidden_dim)
         self.hidden_dim = int(hidden_dim)
         self.rgb = torch.empty(N, 3, device=dev); self.depth_pred = torch.empty(N, device=dev)
@@ -169,24 +132,18 @@ class RenderCall:
             if self.pooled: _pool.give(self.ws)
             self.ws = None
 
-    def backward(self, g_rgb, g_depth_pred, g_depth_gt, g_weights, g_c2w, g_cam=None, g_depth=None, g_scale_shift=None, phase=0,
-                 wg_state=None, wg_seed=False):
-        """all outputs are accumulated into (caller-zeroed) buffers; g_weights may be None (pose only).  phase 1 / 2: the two halves
-        of the backward (data gradients | weight gradients + ray adjoint), see include/nope_nerf_b200.h.  wg_state: the
-        caller's persistent 32-float dY-scale state of the fp16 weight-gradient planes (None: stateless, seeded per call)."""
+    def backward(self, g_rgb, g_depth_pred, g_depth_gt, g_weights, g_c2w, g_cam=None, g_depth=None, g_scale_shift=None):
+        """all outputs are accumulated into (caller-zeroed) buffers; g_weights may be None (pose only)"""
         if self.ws is None:
             raise RuntimeError("backward called without a stashed forward")
         b = L.RenderBwdArgs()
-        b.phase = int(phase)
         b.fwd = self.args
         keep = [_f32c(g_rgb), _f32c(g_depth_pred), _f32c(g_depth_gt)]
         b.g_rgb, b.g_depth_pred, b.g_depth_gt = L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2])
         b.g_weights = L.ptr(g_weights); b.g_c2w = L.ptr(g_c2w); b.g_cam = L.ptr(g_cam); b.g_depth = L.ptr(g_depth)
         b.g_scale_shift = L.ptr(g_scale_shift)
-        b.wg_state = L.ptr(wg_state); b.wg_seed = int(bool(wg_seed))
         L.check(L.lib.nnb_render_bwd(C.byref(b), _stream()), "nnb_render_bwd")
-        if phase != 1:
-            self.release()
+        self.release()
 
 
 class _RenderFn(torch.autograd.Function):

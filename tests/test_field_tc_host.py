@@ -120,8 +120,20 @@ def test_occ_only_does_not_change_the_workspace():
 
 
 def test_version_and_flag():
-    assert L.lib.nnb_version() >= 103
-    assert L.OCC_ONLY == 32768 and L.OCC_ONLY & (L.HVP | L.FWD_DROP_ALO | L.FWD_DROP_WLO | L.RAW_DENSITY | L.WG16 | L.TCBWD | L.STASH) == 0
+    assert L.lib.nnb_version() == 105
+    assert L.OCC_ONLY == 32768 and L.OCC_ONLY & (L.HVP | L.RAW_DENSITY | L.STASH) == 0
+
+
+REMOVED_FLAG_BITS = (512, 1024, 4096, 8192)   # flags defined before version 105
+
+
+def test_undefined_flag_bits_size_no_workspace():
+    for bit in REMOVED_FLAG_BITS + (1 << 16, 1 << 31):
+        for flags in (bit, bit | L.STASH, bit | L.STASH | L.SOFTPLUS):
+            for engine in (L.ENGINE_SIMT, L.ENGINE_TC):
+                for D in (0,) + L.HIDDEN_DIMS:
+                    assert L.lib.nnb_workspace_bytes_dim(64, 32, flags, engine, D) == 0, (flags, engine, D)
+                assert L.lib.nnb_workspace_bytes(64, 32, flags, engine) == 0, (flags, engine)
 
 
 def test_field_query_signature():

@@ -185,6 +185,60 @@ def test_error_paths():
     assert rc == 0 and bool(torch.isfinite(o).all()), (rc, err())
 
 
+def test_removed_flag_bits_are_rejected():
+    """the flag bits removed in version 105 (512, 1024, 4096, 8192) are rejected (rc -7) by every entry point that takes rendering
+    flags, on every engine it serves.  The buffers are real, zeroed and sized for the same call without the bit, which succeeds
+    first: a call that did not check the bit would run on valid memory."""
+    L, ops = _lib()
+    D, N, S, H, W = 64, 4, 32, 8, 8
+    z = lambda *shape, dtype=torch.float32: torch.zeros(*shape, dtype=dtype, device="cuda")
+    weights, g_weights = z(L.num_params(D)), z(L.num_params(D))
+    c2w, cam, g_c2w = torch.eye(4, device="cuda"), torch.diag(torch.tensor([1.0, 1.0, -1.0, 1.0])).cuda(), z(4, 4)
+    ray_idx, depth, g_rgb = z(N, dtype=torch.int64), z(N) + 1.0, z(N, 3)
+    rgb, depth_pred, depth_gt, mask = z(N, 3), z(N), z(N), z(N, dtype=torch.uint8)
+    pts, quad = z(N, 3), [z(N, 4) for _ in range(4)]   # quad: out_rgba / g_rgba / u, g_pts, g_dirs
+    need = max(L.lib.nnb_workspace_bytes_dim(n, s, f, e, D) for n, s in ((N, S), (N, 1)) for e in (L.ENGINE_SIMT, L.ENGINE_TC)
+               for f in (L.STASH, L.STASH | L.HVP))
+    ws = z(need, dtype=torch.uint8)
+    st = ops._stream()
+    err = lambda: L.lib.nnb_last_error().decode()
+
+    def render_args(flags, engine, fields=False):
+        a = L.RenderArgs()
+        a.weights, a.c2w, a.cam, a.ray_idx, a.depth = L.ptr(weights), L.ptr(c2w), L.ptr(cam), L.ptr(ray_idx), L.ptr(depth)
+        a.N, a.S, a.H, a.W, a.near_, a.far_, a.flags, a.engine, a.hidden_dim = N, 1 if fields else S, H, W, 0.1, 4.0, flags, engine, D
+        a.rgb, a.depth_pred, a.depth_gt, a.mask = L.ptr(rgb), L.ptr(depth_pred), L.ptr(depth_gt), L.ptr(mask)
+        a.pts = L.ptr(pts) if fields else None
+        a.workspace, a.workspace_bytes = L.ptr(ws), ws.numel()
+        return a
+
+    def render_bwd(flags, engine):
+        b = L.RenderBwdArgs()
+        b.fwd = render_args(flags, engine)
+        b.g_rgb, b.g_weights, b.g_c2w = L.ptr(g_rgb), L.ptr(g_weights), L.ptr(g_c2w)
+        return L.lib.nnb_render_bwd(C.byref(b), st)
+
+    out, u, g_pts, g_dirs = (L.ptr(t) for t in quad)
+    calls = []   # (name, valid flags, call(flags))
+    for e in (L.ENGINE_SIMT, L.ENGINE_TC):
+        calls += [("nnb_render_fwd/%d" % e, L.STASH, lambda f, e=e: L.lib.nnb_render_fwd(C.byref(render_args(f, e)), st)),
+                  ("nnb_render_bwd/%d" % e, L.STASH, lambda f, e=e: render_bwd(f, e)),
+                  ("nnb_debug_wgrad/%d" % e, L.STASH, lambda f, e=e: L.lib.nnb_debug_wgrad(C.byref(render_args(f, e)), L.ptr(g_weights), st)),
+                  ("nnb_field_fwd/%d" % e, L.SOFTPLUS, lambda f, e=e: L.lib.nnb_field_fwd(C.byref(render_args(f, e, True)), out, st))]
+    calls += [("nnb_field_bwd", L.STASH, lambda f: L.lib.nnb_field_bwd(C.byref(render_args(f, L.ENGINE_SIMT, True)), u, g_pts, g_dirs,
+                                                                      L.ptr(g_weights), st)),
+              ("nnb_field_hvp", L.STASH | L.HVP, lambda f: L.lib.nnb_field_hvp(C.byref(render_args(f, L.ENGINE_SIMT, True)), u, g_pts,
+                                                                             L.ptr(g_weights), st))]
+    for name, flags, call in calls:
+        rc = call(flags)
+        torch.cuda.synchronize()
+        assert rc == 0, (name, rc, err())
+        for bit in (512, 1024, 4096, 8192):
+            rc = call(flags | bit)
+            assert rc == -7 and "not defined" in err(), (name, bit, rc, err())
+    torch.cuda.synchronize()
+
+
 def _net(D=256, seed=3):
     import nope_nerf_b200.model as mdl
     cfg = FC.default_cfg(); cfg["model"]["hidden_dim"] = D

@@ -93,13 +93,14 @@ def oracle32(g):
     return T.run_render(g, np.float32)
 
 
+# "-exact": both engines compute MLP weight gradients to fp32 round-off and are held to the same gates
+ENGINE_IDS = ["simt-exact", "tc-exact"]
+
+
 @pytest.mark.parametrize("name", RENDER_CASES)
-@pytest.mark.parametrize("eng,wg", [("simt", "exact"), ("tc", "exact"), ("tc", "fp16")])
-def test_render_vs_reference_golden(name, eng, wg, monkeypatch):
-    """wg = the weight-gradient precision setting; with 'fp16' the MLP parameter digests keep the looser gate of fp16 operand planes
-    (2e-3 at these sample counts of 768 .. 6144); outputs and every pose / distortion / intrinsics gradient keep the gates below in
-    both modes.
-    Outputs: <= 1e-4 of the reference.  Gradients, two kinds of case:
+@pytest.mark.parametrize("eng", ["simt", "tc"], ids=ENGINE_IDS)
+def test_render_vs_reference_golden(name, eng):
+    """Outputs: <= 1e-4 of the reference.  Gradients, two kinds of case:
       * `*_damped` (oracle.init_params(hf_damp=True): no ReLU-gate switches between fp32 evaluation orders): every gradient
         <= 1e-4 of the fp64 truth (MLP parameter digests 5e-4) and <= max(1e-4, 3 x the reference's own distance from it);
       * default-initialised cases: gradients carry gate-switch noise (tests/test_oracle_golden.py::test_render_gate_matched_and_kxy):
@@ -108,8 +109,6 @@ def test_render_vs_reference_golden(name, eng, wg, monkeypatch):
     engine = dict(engines()).get(eng)
     if engine is None:
         pytest.skip("engine disabled")
-    from nope_nerf_b200 import ops as _ops
-    monkeypatch.setattr(_ops, "_WGRAD", [wg])
     g = load_golden(name)
     damped = bool(g.get("hf_damp", False))
     out, grads = run_case_cuda(g, engine)
@@ -130,7 +129,7 @@ def test_render_vs_reference_golden(name, eng, wg, monkeypatch):
     for k, (ours, ref, t64, t32) in terms.items():
         e["g_" + k] = relmax(ours, ref); e["g_%s_vs64" % k] = relmax(ours, t64); e["g_%s_vs32" % k] = relmax(ours, t32)
         e["env_" + k] = max(relmax(t64, ref), relmax(t32, t64)); e["ref64_" + k] = relmax(t64, ref)
-    _report("%s/%s%s" % (name, eng, "" if wg == "exact" else "-wg16"), **e)
+    _report("%s/%s" % (name, eng), **e)
     tol = 1e-4
     for k in ("rgb", "depth_pred", "depth_gt", "z", "c2w"):
         assert e[k] < tol, (k, e[k])
@@ -145,7 +144,7 @@ def test_render_vs_reference_golden(name, eng, wg, monkeypatch):
             assert e["g_" + k] < max(1e-4, 3 * e["ref64_" + k]), (k, e)
         else:
             assert e["g_" + k] < max(flip_floor, 3 * e["env_" + k]), (k, e)
-    assert e["g_params"] < max(2e-3 if wg == "fp16" else 5e-4, 3 * e["env_params"], flip_floor if not damped else 0.0), e
+    assert e["g_params"] < max(5e-4, 3 * e["env_params"], flip_floor if not damped else 0.0), e
 
 
 def test_pose_expmap_kernels():
@@ -206,17 +205,11 @@ def _build_trainer(g, engine_name, with_ref):
 
 @pytest.mark.parametrize("name,with_ref", [("train_render_only", False), ("train_full_losses", True), ("train_full_lastview", True),
                                            ("train_learn_focal", True)])
-@pytest.mark.parametrize("eng,wg", [("simt", "exact"), ("tc", "exact"), ("tc", "fp16")])
-def test_trainer_step_vs_reference_golden(name, with_ref, eng, wg, monkeypatch):
-    """Two consecutive reference Trainer.train_step calls.  wg = the weight-gradient precision setting ('exact' | 'fp16'); the
-    tensor-core backward computes both with bf16 hi|lo wgmma operands (three MMAs per product), and the gates below keep the looser
-    'fp16' bounds of fp16 operand planes: 2e-3 on the first step's MLP gradient digests; Adam's sign-like first update turns operand
-    rounding into lr-sized differences on weights whose gradient is near zero, so the SECOND step's gradients are gated at 5e-2 only;
-    pose / distortion gradients of the first step and every loss scalar keep the 'exact' gates."""
+@pytest.mark.parametrize("eng", ["simt", "tc"], ids=ENGINE_IDS)
+def test_trainer_step_vs_reference_golden(name, with_ref, eng, monkeypatch):
+    """Two consecutive reference Trainer.train_step calls."""
     if dict(engines()).get(eng) is None:
         pytest.skip("engine disabled")
-    from nope_nerf_b200 import ops as _ops
-    monkeypatch.setattr(_ops, "_WGRAD", [wg])
     g = load_golden(name)
     trainer, net, pose, dist = _build_trainer(g, eng, with_ref)
     kx, ky = float(g["kx"]), float(g["ky"])
@@ -254,14 +247,10 @@ def test_trainer_step_vs_reference_golden(name, with_ref, eng, wg, monkeypatch):
     if "focal0" in g:
         fo = trainer._test_focal
         worst["focal_end"] = relmax(np.array([fo.fx.item(), fo.fy.item()]) - g["focal0"], g["focal_end"] - g["focal0"])
-    _report("%s/%s%s" % (name, eng, "" if wg == "exact" else "-wg16"), **worst)
+    _report("%s/%s" % (name, eng), **worst)
     for k, v in worst.items():
         if k.startswith("loss"):
             assert v < 2e-4, (k, v)        # loss scalars (L1 sums of N*3 terms, fp32)
-        elif wg == "fp16" and k.startswith("g_") and not k.endswith("_0"):
-            assert v < 5e-2, (k, v)        # second step after an Adam update of fp16-rounded weight gradients (docstring)
-        elif wg == "fp16" and k == "g_params_0":
-            assert v < 2e-3, (k, v)
         elif k.startswith("g_params"):
             assert v < 5e-3, (k, v)        # digests of 24 tensors incl. near-zero ones; second step: parameters already differ by Adam noise
         elif k.startswith("g_"):
@@ -269,7 +258,7 @@ def test_trainer_step_vs_reference_golden(name, with_ref, eng, wg, monkeypatch):
         elif k in ("r_end", "t_end", "focal_end"):
             assert v < 5e-2, (k, v)        # Adam's first steps are ~ lr * sign(g): tiny gradients flip easily
         else:
-            assert v < (5e-3 if wg == "fp16" else 1e-3), (k, v)       # params_end digest (fp16: measured 1.3e-3)
+            assert v < 1e-3, (k, v)        # params_end digest
 
 
 @pytest.mark.parametrize("name", ["render_tanks_noise", "render_ndc_distalpha"])
@@ -668,12 +657,10 @@ def test_native_ref_stage_vs_oracle(name):
 
 
 @pytest.mark.parametrize("N,S", [(5, 32), (3, 64), (7, 32), (130, 32), (33, 64), (999, 128), (9, 256)])
-def test_ragged_last_tile_tc_vs_simt(N, S, monkeypatch):
+def test_ragged_last_tile_tc_vs_simt(N, S):
     """N*S not a multiple of the 128-sample tile: the tensor-core engine pads the last tile with clamped rows whose cotangents are
     zero; outputs and gradients must agree with the exact-fp32 engine (weights from init_params(hf_damp=True), so that the
     comparison of the two engines' GRADIENTS is not dominated by single ReLU-gate switches on a handful of rays)."""
-    from nope_nerf_b200 import ops as _ops_
-    monkeypatch.setattr(_ops_, "_WGRAD", ["exact"])       # tiling test: exact weight-gradient planes so that TC == SIMT to 5e-4
     from nope_nerf_b200 import ops, _lib as L
     if len(engines()) < 2:
         pytest.skip("needs both engines")

@@ -28,10 +28,10 @@ def _keep_default_engine(monkeypatch):
 
 @pytest.mark.parametrize("name", SG.RENDER_ALL)
 @pytest.mark.parametrize("eng", ["simt", "tc"])
-def test_render_vs_reference_golden(name, eng, monkeypatch):
+def test_render_vs_reference_golden(name, eng):
     """outputs <= 1e-4 of the reference; `_damped` cases: every gradient <= 1e-4 of the fp64 oracle and <= max(1e-4, 3 x the
     reference's own distance from it); default-initialised cases: <= max(1e-4, 3 x envelope)"""
-    GP.test_render_vs_reference_golden(name, eng, "exact", monkeypatch)
+    GP.test_render_vs_reference_golden(name, eng)
 
 
 def _trainer(g, eng, with_ref, use_cuda_graph):
@@ -184,10 +184,10 @@ def test_c2_size_tc_vs_simt(N, S):
 
 
 @pytest.mark.parametrize("N,S", [(333, 16), (301, 17), (97, 21), (130, 40), (77, 100)])
-def test_ragged_small_s_tc_vs_simt(N, S, monkeypatch):
+def test_ragged_small_s_tc_vs_simt(N, S):
     """the tensor-core engine against the exact-fp32 engine at small S, where one 64-row block overlaps up to 5 rays (S = 17, 21: the
     size of the per-ray bias buffer), with N*S not a multiple of the 128-sample tile (gates of test_gpu_parity's ragged-tile test)"""
-    GP.test_ragged_last_tile_tc_vs_simt(N, S, monkeypatch)
+    GP.test_ragged_last_tile_tc_vs_simt(N, S)
 
 
 def test_render_frame_s512_tc_vs_simt():

@@ -55,13 +55,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=2000); ap.add_argument("--seeds", type=int, default=3)
     ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "psnr_parity.json"))
-    ap.add_argument("--arms", default="eager,graph", help="comma list of: eager, graph, eager_simt (exact-fp32 engine), eager_exact (bf16 hi|lo "
-                    "weight-gradient planes), eager_torchadam (torch.optim.Adam.step instead of the fused one), graph_exact")
+    ap.add_argument("--arms", default="eager,graph", help="comma list of: eager, graph, eager_simt (exact-fp32 engine), eager_torchadam "
+                    "(torch.optim.Adam.step instead of the fused one)")
     a = ap.parse_args()
     ARMS = {"eager": dict(use_cuda_graph=False, pixel_sampler="randperm"), "graph": dict(),
             "eager_simt": dict(use_cuda_graph=False, pixel_sampler="randperm", _engine="simt"),
-            "eager_exact": dict(use_cuda_graph=False, pixel_sampler="randperm", _wgrad="exact"),
-            "graph_exact": dict(_wgrad="exact"),
             "eager_torchadam": dict(use_cuda_graph=False, pixel_sampler="randperm", fused_adam=False)}
     arms = [(n, dict(ARMS[n])) for n in a.arms.split(",")]
     assert RH.available(), "oracle/_ref missing (oracle/vendor_ref.py)"
@@ -126,7 +124,7 @@ def main():
         for arm, kw0 in arms:
             kw = dict(kw0)
             from nope_nerf_b200 import ops as _ops
-            _ops.set_default_engine(kw.pop("_engine", "tc")); _ops.set_wgrad_precision(kw.pop("_wgrad", "fp16"))
+            _ops.set_default_engine(kw.pop("_engine", "tc"))
             pcfg = json.loads(json.dumps(cfg)); pcfg["extract_images"] = {"resolution": (H, W)}
             net = mdl.OfficialStaticNerf(pcfg)
             net.load_state_dict({k: v.clone() for k, v in init["net"].items()})
