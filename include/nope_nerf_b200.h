@@ -73,7 +73,8 @@ typedef struct nnb_render_args {
   float* alpha;      /* [N,S] or NULL */
   void* workspace;
   size_t workspace_bytes;
-  /* explicit-point field queries (nnb_field_fwd/bwd only; NULL for rendering): OfficialStaticNerf.forward(p, ray_d) */
+  /* explicit-point field queries (nnb_field_fwd/bwd/hvp/vjp only; nnb_render_fwd / nnb_render_bwd never read them):
+   * OfficialStaticNerf.forward(p, ray_d) */
   const float* pts;  /* [N,3] */
   const float* dirs; /* [N,3] or NULL (-> ones, like use_ray_dir = False) */
   /* model.hidden_dim (official_nerf.py:11): 64, 128 or 256; 0 means 256.  `weights` / g_weights then hold nnb_num_params(hidden_dim)
@@ -128,7 +129,8 @@ int nnb_render_fwd(const nnb_render_args* a, void* stream);
  * out_rgba [N,4] = (r,g,b, alpha-or-sigma-or-logit).  nnb_field_bwd: g_rgba [N,4] -> g_pts [N,4], g_dirs [N,4] (xyz used),
  * g_weights (+=, may be NULL).
  * Engine of nnb_field_fwd: a->engine == NNB_ENGINE_TC runs the tensor-core kernel (inference only); every other value runs the
- * exact-fp32 engine, as in versions < 103, which ignored the field.  nnb_field_bwd and nnb_field_hvp always run exact fp32.
+ * exact-fp32 engine, as in versions < 103, which ignored the field.  nnb_field_bwd and nnb_field_hvp always run exact fp32; the data
+ * gradients alone run on tensor cores through nnb_field_vjp.
  *   NNB_ENGINE_TC: flags NNB_DIST_ALPHA / NNB_SOFTPLUS / NNB_RAW_DENSITY / NNB_OCC_ONLY.  NNB_STASH is rejected (rc -6): gradients
  *   need the exact-fp32 engine.  The workspace holds nnb_workspace_bytes_dim(N, 1, flags, NNB_ENGINE_TC, hidden_dim) bytes, 256-byte
  *   aligned; out_rgba is 16-byte aligned; c2w / cam / ray_idx are not read.  Rows of out_rgba past N are not written.
@@ -148,6 +150,33 @@ int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, f
  * nnb_workspace_bytes_dim(N, 1, flags, NNB_ENGINE_SIMT, hidden_dim); dirs and the activation flags do not enter (the logit is raw).
  * u and g_pts are 16-byte aligned.  Exact-fp32 engine; every sum runs in a fixed order, so the same inputs give the same bits. */
 int nnb_field_hvp(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream);
+/* Data gradients of OfficialStaticNerf.forward on explicit points, tensor-core engine: forward and data-gradient chain in one call (the
+ * surface normals of the geometry view: NNB_RAW_DENSITY | NNB_OCC_ONLY with g_rgba = (0, 0, 0, 1) gives g_pts = d logit / d p).
+ * Reads a->pts [N,3], a->dirs [N,3] or NULL (ones), N, weights, hidden_dim, flags (NNB_DIST_ALPHA | NNB_SOFTPLUS | NNB_RAW_DENSITY |
+ * NNB_OCC_ONLY), engine and the workspace;  g_rgba [N,4] is the cotangent on (r, g, b, a).
+ *   out_rgba [N,4] (optional, NULL = not wanted): bit-identical to nnb_field_fwd on NNB_ENGINE_TC with the same flags.
+ *   g_pts [N,4] (xyz; w is 0) = d<g_rgba, out>/d p;  g_dirs [N,4] (optional) = d<g_rgba, out>/d dirs (the ones when dirs is NULL).
+ *   Overwritten, rows < N only.  There are no weight gradients: they, and nnb_field_bwd / nnb_field_hvp, stay on the exact engine.
+ * NNB_OCC_ONLY: the colour branch is neither evaluated nor differentiated; g_rgba[:, :3] is not read and g_dirs must be NULL.
+ * Errors, with nothing launched: an engine other than NNB_ENGINE_TC (rc -4); an undefined flag bit (-7); NNB_STASH or NNB_HVP (-6);
+ * g_dirs with NNB_OCC_ONLY (-6); an unsupported width (-8); N < 0, a NULL pts / weights / g_rgba / g_pts, or one of g_rgba, out_rgba,
+ * g_pts, g_dirs not 16-byte aligned (-3); a workspace smaller than nnb_field_vjp_workspace_bytes(N, flags, hidden_dim) or not 256-byte
+ * aligned (-5).  N == 0 returns 0 and does nothing.
+ * Precision: the forward is nnb_field_fwd's split-fp16 product (three MMAs per layer, fp32 accumulation), the chain runs through the
+ * transposed weights as bf16 hi | lo products like the render backward (tc_dgrad), gated by the ReLU bits the forward writes; the
+ * encoding adjoints are fp32.  Measured against float64 evaluated with the same ReLU gates: g_pts within 2.5e-5 of its maximum, g_dirs
+ * within 1.1e-5, out_rgba within 3e-7 (the exact engine's gradients: within 1e-6).  Where a point's ReLU pre-activation lies within the
+ * forward's rounding of 0 (measured: within 8e-7 of the layer's largest), this engine may gate that unit differently from float64 or from
+ * the exact engine, and the gradient, which is discontinuous there, then differs by that unit's contribution.  The fp16 caveat of nnb_field_fwd
+ * holds for the forward: a field whose activations are very small (below about 2^-3 the low half is subnormal, below about 6e-8 an
+ * operand vanishes) is evaluated, and so gated, less accurately than on the exact engine.
+ * A point's outputs depend on that point alone (not on N, its tile or its row), like the forward's.
+ * Workspace, each section 256-byte aligned (Npad = N rounded up to 128, D = hidden_dim): per-point records (32 Npad bytes) | ReLU gate
+ * bits of h0..h7 (Npad D bytes) and, unless NNB_OCC_ONLY, of the rgb hidden layer (Npad D / 16 bytes) | the forward weight image (its
+ * occupancy-only prefix with NNB_OCC_ONLY) | the transposed weight image (its trunk part with NNB_OCC_ONLY).  The size query returns 0 for
+ * N <= 0, an undefined flag bit or an unsupported width. */
+size_t nnb_field_vjp_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim);
+int nnb_field_vjp(const nnb_render_args* a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, void* stream);
 int nnb_render_bwd(const nnb_render_bwd_args* a, void* stream);
 
 /* Fused ray marching of the geometry view: what Renderer.ray_marching + Renderer.secant (model/rendering.py:274-418) do for N rays, in

@@ -87,6 +87,9 @@ def _load():
     lib.nnb_ray_march_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     lib.nnb_field_bwd.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, C.c_void_p]
     lib.nnb_field_hvp.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, C.c_void_p]
+    lib.nnb_field_vjp.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, C.c_void_p]
+    lib.nnb_field_vjp_workspace_bytes.restype = C.c_size_t
+    lib.nnb_field_vjp_workspace_bytes.argtypes = [C.c_int32, C.c_uint32, C.c_int32]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]
     lib.nnb_pose_bwd.argtypes = [_f, _f, _f, C.c_int32, _f, _f, _f, C.c_void_p]
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,

@@ -20,6 +20,8 @@ cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, flo
 size_t tc_workspace_extra(int N, int S, uint32_t flags, int D);
 size_t tc_ray_march_workspace(int N, int n_steps, int D);
 cudaError_t tc_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st);
+size_t tc_field_vjp_workspace(int N, uint32_t flags, int D);
+cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
 cudaError_t launch_pose_fwd(const float*, const float*, const float*, int, const int*, float*, cudaStream_t);
@@ -150,11 +152,13 @@ static int check_engine_ws(const nnb_render_args* a) {
 int nnb_render_fwd(const nnb_render_args* a, void* stream) {
   int rc = check_args(a); if (rc) return rc;
   WsLayout L = make_layout(a->N, a->S, a->flags, a->engine, hidden_of(a->hidden_dim));
+  // pts / dirs belong to the nnb_field_* calls; the render kernels would take a non-NULL pts for N * S explicit points
+  nnb_render_args r = *a; r.pts = nullptr; r.dirs = nullptr;
   cudaError_t e;
 #ifdef NNB_WITH_TC
-  if (a->engine == NNB_ENGINE_TC) e = tc_render_fwd(*a, L, (cudaStream_t)stream); else
+  if (r.engine == NNB_ENGINE_TC) e = tc_render_fwd(r, L, (cudaStream_t)stream); else
 #endif
-  e = simt_render_fwd(*a, L, (cudaStream_t)stream);
+  e = simt_render_fwd(r, L, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_fwd");
 }
 
@@ -164,11 +168,12 @@ int nnb_render_bwd(const nnb_render_bwd_args* b, void* stream) {
   if (!(b->fwd.flags & NNB_STASH)) return fail(-6, "nnb_render_bwd needs the forward call to have run with NNB_STASH");
   if (!b->g_rgb || !b->g_c2w) return fail(-3, "g_rgb and g_c2w must be non-null");
   WsLayout L = make_layout(b->fwd.N, b->fwd.S, b->fwd.flags, b->fwd.engine, hidden_of(b->fwd.hidden_dim));
+  nnb_render_bwd_args r = *b; r.fwd.pts = nullptr; r.fwd.dirs = nullptr;   // as in nnb_render_fwd
   cudaError_t e;
 #ifdef NNB_WITH_TC
-  if (b->fwd.engine == NNB_ENGINE_TC) e = tc_render_bwd(*b, L, (cudaStream_t)stream); else
+  if (r.fwd.engine == NNB_ENGINE_TC) e = tc_render_bwd(r, L, (cudaStream_t)stream); else
 #endif
-  e = simt_render_bwd(*b, L, (cudaStream_t)stream);
+  e = simt_render_bwd(r, L, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_bwd");
 }
 
@@ -246,6 +251,40 @@ int nnb_ray_march(const nnb_ray_march_args* a, void* stream) {
   if ((reinterpret_cast<uintptr_t>(a->bracket) & 15) != 0) return fail(-3, "nnb_ray_march: bracket must be 16-byte aligned");
   cudaError_t e = tc_ray_march(*a, D, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_ray_march");
+#endif
+}
+size_t nnb_field_vjp_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && nnb::dim_supported(D) && !(flags & ~KNOWN_FLAGS)) return tc_field_vjp_workspace(N, flags, D);
+#endif
+  return 0;
+}
+static inline bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+int nnb_field_vjp(const nnb_render_args* a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, void* stream) {
+  if (!a) return fail(-3, "nnb_field_vjp: null args");
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_field_vjp: engine %d has no explicit-point data gradient here (NNB_ENGINE_TC only; the exact-fp32 engine has nnb_field_bwd)",
+                a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_flags(a->flags)) return rc;
+  if (a->flags & (NNB_STASH | NNB_HVP))
+    return fail(-6, "nnb_field_vjp: NNB_STASH and NNB_HVP are not accepted (nothing is stashed; weight gradients and nnb_field_hvp need the exact-fp32 engine)");
+  if (int rc = check_dim(a)) return rc;
+  if (a->N < 0) return fail(-3, "nnb_field_vjp: N must not be negative (got %d)", a->N);
+  if ((a->flags & NNB_OCC_ONLY) && g_dirs) return fail(-6, "nnb_field_vjp: g_dirs must be NULL with NNB_OCC_ONLY (the colour branch is not evaluated)");
+  if (a->N == 0) return 0;
+  if (!a->pts || !a->weights || !g_rgba || !g_pts) return fail(-3, "nnb_field_vjp: need pts, weights, g_rgba and g_pts");
+  if (misaligned16(g_rgba) || misaligned16(out_rgba) || misaligned16(g_pts) || misaligned16(g_dirs))
+    return fail(-3, "nnb_field_vjp: g_rgba, out_rgba, g_pts and g_dirs must be 16-byte aligned [N][4] arrays");
+  const size_t need = nnb_field_vjp_workspace_bytes(a->N, a->flags, a->hidden_dim);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  nnb_render_args b = *a; b.S = 1;
+  cudaError_t e = tc_field_vjp(b, g_rgba, out_rgba, g_pts, g_dirs, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_vjp");
 #endif
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {

@@ -85,6 +85,22 @@ template <int D> struct Tc {
   // ---- data-gradient chain (176 transposed stages at D = 256) ----
   static constexpr int N_STAGES_T = D / 32 + D / 32 + KS + 7 * KS + KS + KS;
   static constexpr size_t IMG_T_BYTES = (size_t)34 * D * D + (size_t)576 * D;
+  // The producer's and the consumers' bounds of the chain come from dg_steps: K-steps (= transposed stages) of chain GEMM j: 0 g_de,
+  // 1 g_feat, 2 g_h7 (W_feat), 3 + i (i = 0..6) g_h(6 - i) = dY_(7 - i) W_(7 - i), 10 the encoding slice of layer 4, 11 the encoding
+  // gradient of layer 0.  An occupancy-only chain (occ, nnb_field_vjp) starts at g_h7 = g_s w_sigma: GEMMs 0..2 (the colour prefix of the
+  // stage table) have no stages, and it walks the table from dg_first_stage(true) on.
+  static constexpr int N_DG_GEMM = 12;
+  static constexpr int dg_steps(int j, bool occ) { return j < 2 ? (occ ? 0 : D / 32) : (j == 2 && occ ? 0 : KS); }
+  static constexpr int dg_tile_stages(bool occ) {
+    int n = 0;
+    for (int j = 0; j < N_DG_GEMM; ++j) n += dg_steps(j, occ);
+    return n;
+  }
+  static constexpr int dg_first_stage(bool occ) { return dg_tile_stages(false) - dg_tile_stages(occ); }
+  static constexpr size_t IMG_T_PREFIX_BYTES = (size_t)(D / 32) * 32 * 64 + (size_t)(D / 32 + KS) * STAGE_BYTES;   // g_de, g_feat, W_feat
+  static_assert(dg_tile_stages(false) == N_STAGES_T && dg_first_stage(true) == D / 16 + KS, "chain stage count");
+  static_assert(dg_steps(3, false) == KS && dg_steps(9, false) == KS && dg_steps(3, true) == KS && dg_steps(9, true) == KS,
+                "the trunk layers of the chain share one K-step count");
   static constexpr int DG_AHI = 0, DG_ALO = D * 256, DG_W = 2 * D * 256, DG_GENC = DG_W + NST * STAGE_BYTES;
   static constexpr int DG_SMALL = DG_GENC + 2 * 64 * 64 * 4;     // W_rgb [3][D/2] | w_sigma [D]
   static constexpr int DG_GYC = DG_SMALL + (5 * D / 2) * 4;      // per row: d/d(rgb logits), d/d density logit
@@ -230,20 +246,24 @@ __device__ __forceinline__ void march_scan(const MarchPtrs& q, int ray, const fl
 
 // MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
 // out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is stashed and recs is not written.  M = a.N there, so point indices
-// are 32-bit.  FWD_MARCH / FWD_SECANT (tc_march / tc_secant): occupancy-only tiles of points made from q; n_tiles (and M, the hit count
-// of tc_secant) are read from *q.count when the kernel starts and fixed from then on.
+// are 32-bit.  FWD_VJP (tc_points_vjp_fwd, nnb_field_vjp): FWD_POINTS that also writes recs [Mpad] and the ReLU gate bits st.gates of
+// the chain that follows (h0..h7, and the rgb hidden layer unless NNB_OCC_ONLY); out may be NULL; no fp32 stash.  FWD_MARCH /
+// FWD_SECANT (tc_march / tc_secant): occupancy-only tiles of points made from q; n_tiles (and M, the hit count of tc_secant) are read
+// from *q.count when the kernel starts and fixed from then on.
 //   FWD_MARCH: tile = 128 consecutive steps of one ray; march_scan reduces them.
 //   FWD_SECANT: tile = 128 hit rays, evaluated q.n_secant times in a row at the secant iterate of each ray's bracket, which the thread
 //   that owns the row's logit then updates in q.brk1 (pass 0 reads q.brk0).  A row's prologue threads and that thread sit in the same
 //   warpgroup, whose barrier at the top of the tile loop orders the update before the next pass reads it.
-enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3 };
+enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4 };
 template <int D, int MODE>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
                                             int stash) {
   using T = Tc<D>;
-  constexpr bool PTS = MODE != FWD_RAYS, MARCH = MODE >= FWD_MARCH;
+  constexpr bool PTS = MODE != FWD_RAYS, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP;
+  constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
   if constexpr (PTS) stash = 0;
+  const bool gates = VJP || stash;   // the ReLU gate bits are stored
   if constexpr (MARCH) {
     if (q.count) {
       const int c = *q.count;
@@ -318,7 +338,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
   constexpr int RAYB_DE = T::RAYB_RAYS * DR;   // direction encodings after the per-ray biases
   uint32_t slot = 0, phase = 0;
   float acc[D / 2];
-  if constexpr (MODE == FWD_POINTS) {   // b_rgbh is a plain bias here; visible after the tile's first barrier
+  if constexpr (XPTS) {   // b_rgbh is a plain bias here; visible after the tile's first barrier
     if (tl < DR) rayb[tl] = __ldg(a.weights + nnb::B_RGBH(D) + tl);
   }
   const int n_gemm = T::n_gemm(occ);
@@ -462,7 +482,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             gw[j / 8] = push_gate(push_gate(gw[j / 8], v0), v1);
           }
         }
-        if (stash && g < 8) store_gates<D / 2>(st.gates + gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
+        if (gates && g < 8) store_gates<D / 2>(st.gates + gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
         if constexpr (PTS) {
           // Layer 4 was the last reader of E.  The direction operand of the rgb hidden layer takes its place: enc4(dirs[m]), 27 columns
           // padded to 32 (two K-steps), as fp16 hi | lo in E's layout.  A warp writes the 16 rows its own MMAs read, like the A operand
@@ -505,7 +525,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             gw[j / 8] = push_gate(push_gate(gw[j / 8], v0), v1);
           }
         }
-        if (stash) store_gates<D / 4>(st.gates + gate_bits_off(8, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
+        if (gates) store_gates<D / 4>(st.gates + gate_bits_off(8, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const float sl = quad_sum(s_logit[r]);
@@ -517,7 +537,12 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             SampleRec rec;
             rec.r = sigmoid_f(cr + s_bias[B_SIG0 + 1]); rec.g = sigmoid_f(cg + s_bias[B_SIG0 + 2]); rec.b = sigmoid_f(cb + s_bias[B_SIG0 + 3]);
             rec.a = density_act(s, a.flags, &sigma); rec.s = s;
-            if constexpr (PTS) {
+            if constexpr (VJP) {   // every row of the tile has its record; the point of a row past M is the last point
+              const uint32_t mp = computed_here(tile * (uint32_t)TILE + r0 + 8 * r);
+              rec.z = 0.f; rec.pad0 = 0.f; rec.pad1 = 0.f;
+              recs[mp] = rec;
+              if (out && mp < (uint32_t)M) out[mp] = make_float4(rec.r, rec.g, rec.b, rec.a);
+            } else if constexpr (PTS) {
               const uint32_t mp = computed_here(tile * (uint32_t)TILE + r0 + 8 * r);
               if (mp < (uint32_t)M) out[mp] = make_float4(rec.r, rec.g, rec.b, rec.a);
             } else {
@@ -540,6 +565,15 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         float sigma;
         if constexpr (MODE == FWD_POINTS) {
           if ((lane & 3) == 0 && mp < (uint32_t)M) out[mp] = make_float4(0.f, 0.f, 0.f, density_act(sl + s_bias[B_SIG0], a.flags, &sigma));
+        } else if constexpr (VJP) {
+          if ((lane & 3) == 0) {
+            SampleRec rec;
+            rec.s = sl + s_bias[B_SIG0];
+            rec.a = density_act(rec.s, a.flags, &sigma);
+            rec.r = 0.f; rec.g = 0.f; rec.b = 0.f; rec.z = 0.f; rec.pad0 = 0.f; rec.pad1 = 0.f;
+            recs[mp] = rec;
+            if (out && mp < (uint32_t)M) out[mp] = make_float4(0.f, 0.f, 0.f, rec.a);
+          }
         } else if constexpr (MODE == FWD_MARCH) {
           if ((lane & 3) == 0) s_val[r0 + 8 * r] = __fsub_rn(density_act(sl + s_bias[B_SIG0], a.flags, &sigma), q.tau);
         } else if constexpr (MODE == FWD_SECANT) {
@@ -931,10 +965,8 @@ cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw,
 // g_feat = g_yr W_rgbh[:, :256], g_h7 = g_feat W_feat + g_s w_sigma, then layers 7..1 (layer 4 first adds its encoding slice, N = 64)
 // and layer 0 (encoding, N = 64).
 template <int D>
-__global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __restrict__ img) {
-  const StageDescT sd = stage_t<D>(blockIdx.x);
-  unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] bf16
-  unsigned char* lo = hi + sd.nrows * 32;
+__device__ __forceinline__ void prep_stage_t(const float* __restrict__ w, const StageDescT& sd, unsigned char* __restrict__ hi) {
+  unsigned char* lo = hi + sd.nrows * 32;     // hi: [k-octet 0..1][nrows][8] bf16
   for (int idx = threadIdx.x; idx < sd.nrows * 2; idx += blockDim.x) {
     const int n = idx % sd.nrows, ko = idx / sd.nrows;
     float v[8];
@@ -945,6 +977,17 @@ __global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __
     }
     split_store8_bf16(v, hi + ko * sd.nrows * 16 + n * 16, lo + ko * sd.nrows * 16 + n * 16);
   }
+}
+template <int D>
+__global__ void tc_prep_weights_t(const float* __restrict__ w, unsigned char* __restrict__ img) {
+  const StageDescT sd = stage_t<D>(blockIdx.x);
+  prep_stage_t<D>(w, sd, img + sd.img_off);
+}
+// the stages s0, s0 + 1, ... of the table into an image that starts at stage s0 (the trunk part of an occupancy-only chain)
+template <int D>
+__global__ void tc_prep_weights_t_from(const float* __restrict__ w, unsigned char* __restrict__ img, int s0) {
+  const StageDescT sd = stage_t<D>(s0 + blockIdx.x);
+  prep_stage_t<D>(w, sd, img + (sd.img_off - stage_t<D>(s0).img_off));
 }
 
 struct DgPtrs {
@@ -985,13 +1028,25 @@ __device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint
   lo = *reinterpret_cast<uint32_t*>(&ll);
 }
 
-template <int D>
-__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, const unsigned char* __restrict__ wimg,
-                                                         const __grid_constant__ DgPtrs P, size_t M,
-                                                         int n_tiles, int write_dy) {
+// MODE DG_RAYS (tc_dgrad, the render backward): rows are the samples of a.N rays, the records / cotangents / gradients are the
+// workspace's [Mpad] arrays, and the dY stash is written when write_dy.  DG_POINTS / DG_POINTS_OCC (tc_points_vjp, nnb_field_vjp): rows
+// are the explicit points a.pts [M]; P.gs is the caller's g_rgba [M] (rows >= M read as zero), P.gp / P.gv are g_pts / g_dirs [M] (P.gv
+// may be NULL), only rows < M are stored and nothing is stashed.  DG_POINTS_OCC is the chain of an occupancy-only forward: it starts at
+// g_h7 = g_s w_sigma (the colour prefix of the stage table is neither loaded nor issued) and reads only g_rgba[m].w.
+enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2 };
+template <int D, int MODE>
+__device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
+                                              int n_tiles, int write_dy) {
   using T = Tc<D>;
+  constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC;
+  if constexpr (PTS) write_dy = 0;
   constexpr int DG_AHI = T::DG_AHI, DG_ALO = T::DG_ALO, DG_W = T::DG_W, DG_GENC = T::DG_GENC, DG_SMALL = T::DG_SMALL, DG_GYC = T::DG_GYC;
-  constexpr int DG_BAR = T::DG_BAR, STAGE_BYTES = T::STAGE_BYTES, N_STAGES_T = T::N_STAGES_T, DR = D / 2, KS = T::KS;
+  constexpr int DG_BAR = T::DG_BAR, STAGE_BYTES = T::STAGE_BYTES, DR = D / 2;
+  constexpr int S0 = T::dg_first_stage(OCC), S_END = S0 + T::dg_tile_stages(OCC);   // the stages of one tile
+  constexpr int IMG0 = OCC ? (int)T::IMG_T_PREFIX_BYTES : 0;   // wimg holds the stages from S0 on
+  // K-steps of the chain's GEMMs (constant expressions: Tc::dg_steps; every trunk layer has ST_TRUNK, static_assert in Tc)
+  constexpr int ST_DE = T::dg_steps(0, OCC), ST_FEAT = T::dg_steps(1, OCC), ST_H7 = T::dg_steps(2, OCC), ST_TRUNK = T::dg_steps(3, OCC);
+  constexpr int ST_ENC4 = T::dg_steps(10, OCC), ST_ENC0 = T::dg_steps(11, OCC);
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* s_small = reinterpret_cast<float*>(smem + DG_SMALL);
@@ -1009,11 +1064,11 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
     if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0;
       for (int t = 0; t < my_tiles; ++t)
-        for (int s = 0; s < N_STAGES_T; ++s) {
+        for (int s = S0; s < S_END; ++s) {
           const uint32_t bytes = (uint32_t)stage_t<D>(s).nrows * 64u;
           mbar_wait(bar0 + 8u * (NST + slot), phase ^ 1u);
           mbar_expect_tx(bar0 + 8u * slot, bytes);
-          bulk_g2s(smem_u32(smem + DG_W + slot * STAGE_BYTES), wimg + stage_t<D>(s).img_off, bytes, bar0 + 8u * slot);
+          bulk_g2s(smem_u32(smem + DG_W + slot * STAGE_BYTES), wimg + (stage_t<D>(s).img_off - IMG0), bytes, bar0 + 8u * slot);
           if (++slot == NST) { slot = 0; phase ^= 1u; }
         }
     }
@@ -1074,88 +1129,132 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
   for (int t = 0; t < my_tiles; ++t) {
     const int tile = blockIdx.x + t * gridDim.x;
     const size_t mt = (size_t)tile * TILE;
-    load_gates<D / 4>(P.gates + gate_bits_off(8, tile, threadIdx.x, Mpad, D), gm);
+    load_gates<OCC ? D / 2 : D / 4>(P.gates + gate_bits_off(OCC ? 7 : 8, tile, threadIdx.x, Mpad, D), gm);
     wg_sync();   // the previous tile's encoding adjoint is done with genc
     if (tl < 64) {   // head adjoints (one thread per row)
       const size_t m = mt + wg * 64 + tl;
-      const float4 g = (m < M) ? P.gs[m] : make_float4(0.f, 0.f, 0.f, 0.f);
-      const SampleRec rec = P.rec[m];
-      const float g0 = g.x * rec.r * (1.f - rec.r), g1 = g.y * rec.g * (1.f - rec.g), g2 = g.z * rec.b * (1.f - rec.b);
-      const float g3 = g.w * density_act_grad(rec.s, a.flags);
-      if (write_dy) P.dyc[m] = make_float4(g0, g1, g2, g3);
-      gyc[tl * 4] = g0; gyc[tl * 4 + 1] = g1; gyc[tl * 4 + 2] = g2; gyc[tl * 4 + 3] = g3;
+      if constexpr (OCC) {
+        const float gw = (m < M) ? reinterpret_cast<const float*>(P.gs + m)[3] : 0.f;
+        gyc[tl * 4 + 3] = gw * density_act_grad(P.rec[m].s, a.flags);
+      } else {
+        const float4 g = (m < M) ? P.gs[m] : make_float4(0.f, 0.f, 0.f, 0.f);
+        const SampleRec rec = P.rec[m];
+        const float g0 = g.x * rec.r * (1.f - rec.r), g1 = g.y * rec.g * (1.f - rec.g), g2 = g.z * rec.b * (1.f - rec.b);
+        const float g3 = g.w * density_act_grad(rec.s, a.flags);
+        if (write_dy) P.dyc[m] = make_float4(g0, g1, g2, g3);
+        gyc[tl * 4] = g0; gyc[tl * 4 + 1] = g1; gyc[tl * 4 + 2] = g2; gyc[tl * 4 + 3] = g3;
+      }
     }
     wg_sync();
-    {   // g_yr = (g_yc W_rgb) * (hr > 0), in the accumulator-fragment mapping of the gate bits -> A operand (K = D/2) + dY stash
+    if constexpr (OCC) {   // g_h7 = (g_s w_sigma) * (h7 > 0)
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = r0 + 8 * r;
-        const float* g4 = gyc + (row - wg * 64) * 4;
-        unsigned char* ahi = smem + DG_AHI + row * 16 + c0 * 2;
+      for (int i = 0; i < D / 2; ++i) acc[i] = 0.f;
+      epiD(mt, true, nullptr, true);
+    } else {
+      {   // g_yr = (g_yc W_rgb) * (hr > 0), in the accumulator-fragment mapping of the gate bits -> A operand (K = D/2) + dY stash
 #pragma unroll
-        for (int j = 0; j < DR / 8; ++j) {
-          const int col = j * 8 + c0;
-          const float x0 = g4[0] * s_small[col] + g4[1] * s_small[DR + col] + g4[2] * s_small[2 * DR + col];
-          const float x1 = g4[0] * s_small[col + 1] + g4[1] * s_small[DR + col + 1] + g4[2] * s_small[2 * DR + col + 1];
-          const uint32_t b = gm[j / 8] << (4 * (j & 7) + 2 * r);
-          const float v0 = (b & 0x80000000u) ? x0 : 0.f, v1 = (b & 0x40000000u) ? x1 : 0.f;
-          if (write_dy) *reinterpret_cast<float2*>(P.dyr + (mt + row) * DR + col) = make_float2(v0, v1);
-          uint32_t hw, lw;
-          split2_bf16(v0, v1, hw, lw);
-          *reinterpret_cast<uint32_t*>(ahi + j * 2048) = hw;
-          *reinterpret_cast<uint32_t*>(ahi + DG_ALO + j * 2048) = lw;
+        for (int r = 0; r < 2; ++r) {
+          const int row = r0 + 8 * r;
+          const float* g4 = gyc + (row - wg * 64) * 4;
+          unsigned char* ahi = smem + DG_AHI + row * 16 + c0 * 2;
+#pragma unroll
+          for (int j = 0; j < DR / 8; ++j) {
+            const int col = j * 8 + c0;
+            const float x0 = g4[0] * s_small[col] + g4[1] * s_small[DR + col] + g4[2] * s_small[2 * DR + col];
+            const float x1 = g4[0] * s_small[col + 1] + g4[1] * s_small[DR + col + 1] + g4[2] * s_small[2 * DR + col + 1];
+            const uint32_t b = gm[j / 8] << (4 * (j & 7) + 2 * r);
+            const float v0 = (b & 0x80000000u) ? x0 : 0.f, v1 = (b & 0x40000000u) ? x1 : 0.f;
+            if (write_dy) *reinterpret_cast<float2*>(P.dyr + (mt + row) * DR + col) = make_float2(v0, v1);
+            uint32_t hw, lw;
+            split2_bf16(v0, v1, hw, lw);
+            *reinterpret_cast<uint32_t*>(ahi + j * 2048) = hw;
+            *reinterpret_cast<uint32_t*>(ahi + DG_ALO + j * 2048) = lw;
+          }
         }
       }
-    }
-    fence_async_smem();
-    wg_sync();
-    // g_de (direction-encoding slice of rgb_layers.0) -> view-direction adjoint
-    dg_gemm<D, 32>(acc, a_hi, a_lo, D / 32, w_base, bar0, slot, phase, tl);
+      fence_async_smem();
+      wg_sync();
+      // g_de (direction-encoding slice of rgb_layers.0) -> view-direction adjoint
+      dg_gemm<D, 32>(acc, a_hi, a_lo, ST_DE, w_base, bar0, slot, phase, tl);
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
+      for (int j = 0; j < 4; ++j)
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        float* g = genc + (r0 + 8 * r - wg * 64) * 32 + j * 8 + c0;
-        g[0] = acc[4 * j + 2 * r]; g[1] = acc[4 * j + 2 * r + 1];
+        for (int r = 0; r < 2; ++r) {
+          float* g = genc + (r0 + 8 * r - wg * 64) * 32 + j * 8 + c0;
+          g[0] = acc[4 * j + 2 * r]; g[1] = acc[4 * j + 2 * r + 1];
+        }
+      wg_sync();
+      if (tl < 64) {
+        const size_t m = mt + wg * 64 + tl, mm = m < M ? m : M - 1;
+        Ray ray; float z, p[3], v[3], gvd[3];
+        if constexpr (PTS) {
+#pragma unroll
+          for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
+        } else {
+          row_geometry_tc(a, m, M, ray, z, p);
+          if (a.pts) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
+          } else {
+            view_dir(a, ray, v);
+          }
+        }
+        const float* ge = genc + tl * 32;
+        encode_bwd<4>(v, [&](int k) { return ge[k]; }, gvd);
+        if (!PTS || (P.gv && m < M)) P.gv[m] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
       }
-    wg_sync();
-    if (tl < 64) {
-      const size_t m = mt + wg * 64 + tl, mm = m < M ? m : M - 1;
-      Ray ray; float z, p[3], v[3], gvd[3];
-      row_geometry_tc(a, m, M, ray, z, p);
-      if (a.pts) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
-      } else {
-        view_dir(a, ray, v);
-      }
-      const float* ge = genc + tl * 32;
-      encode_bwd<4>(v, [&](int k) { return ge[k]; }, gvd);
-      P.gv[m] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
+      dg_gemm<D, D>(acc, a_hi, a_lo, ST_FEAT, w_base, bar0, slot, phase, tl);   // g_feat
+      epiD(mt, false, write_dy ? P.dfeat : nullptr, false);
+      load_gates<D / 2>(P.gates + gate_bits_off(7, tile, threadIdx.x, Mpad, D), gm);
+      dg_gemm<D, D>(acc, a_hi, a_lo, ST_H7, w_base, bar0, slot, phase, tl);   // g_h7 = g_feat W_feat + g_s w_sigma
+      epiD(mt, true, write_dy ? P.dy[7] : nullptr, true);
     }
-    dg_gemm<D, D>(acc, a_hi, a_lo, D / 32, w_base, bar0, slot, phase, tl);   // g_feat
-    epiD(mt, false, write_dy ? P.dfeat : nullptr, false);
-    load_gates<D / 2>(P.gates + gate_bits_off(7, tile, threadIdx.x, Mpad, D), gm);
-    dg_gemm<D, D>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);       // g_h7 = g_feat W_feat + g_s w_sigma
-    epiD(mt, true, write_dy ? P.dy[7] : nullptr, true);
     for (int l = 7; l >= 1; --l) {
       load_gates<D / 2>(P.gates + gate_bits_off(l - 1, tile, threadIdx.x, Mpad, D), gm);
-      if (l == 4) { dg_gemm<D, 64>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl); epi_enc(false); }
-      dg_gemm<D, D>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);     // g_h(l-1) = dY_l W_l
+      if (l == 4) { dg_gemm<D, 64>(acc, a_hi, a_lo, ST_ENC4, w_base, bar0, slot, phase, tl); epi_enc(false); }
+      dg_gemm<D, D>(acc, a_hi, a_lo, ST_TRUNK, w_base, bar0, slot, phase, tl);   // g_h(l-1) = dY_l W_l
       epiD(mt, true, write_dy ? P.dy[l - 1] : nullptr, false);
     }
-    dg_gemm<D, 64>(acc, a_hi, a_lo, KS, w_base, bar0, slot, phase, tl);      // encoding gradient of layer 0
+    dg_gemm<D, 64>(acc, a_hi, a_lo, ST_ENC0, w_base, bar0, slot, phase, tl);   // encoding gradient of layer 0
     epi_enc(true);
     wg_sync();
     if (tl < 64) {   // encoding adjoint -> d p
       const size_t m = mt + wg * 64 + tl;
       Ray ray; float z, p[3], gp[3];
-      row_geometry_tc(a, m, M, ray, z, p);
+      if constexpr (PTS) {
+        const size_t mm = m < M ? m : M - 1;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + 3 * mm + c);
+      } else {
+        row_geometry_tc(a, m, M, ray, z, p);
+      }
       const float* ge = genc + tl * 64;
       encode_bwd<10>(p, [&](int k) { return ge[k]; }, gp);
-      P.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
+      if (!PTS || m < M) P.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
     }
   }
+}
+
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                         const __grid_constant__ DgPtrs P, size_t M,
+                                                         int n_tiles, int write_dy) {
+  tc_dgrad_body<D, DG_RAYS>(a, wimg, P, M, n_tiles, write_dy);
+}
+
+// nnb_field_vjp: the forward of explicit points with records and gate bits (FWD_VJP), then the chain on them (DG_POINTS[_OCC])
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_vjp_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                  SampleRec* __restrict__ recs, float4* __restrict__ out,
+                                                                  unsigned char* __restrict__ gates, size_t M, int n_tiles) {
+  TcStash st{};
+  st.gates = gates;
+  tc_fwd_body<D, FWD_VJP>(a, wimg, recs, out, st, MarchPtrs{}, M, n_tiles, 0);
+}
+template <int D, int MODE>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_vjp(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                              const __grid_constant__ DgPtrs P, size_t M, int n_tiles) {
+  tc_dgrad_body<D, MODE>(a, wimg, P, M, n_tiles, 0);
 }
 
 template <int D>
@@ -1173,12 +1272,16 @@ cudaError_t upload_stage_table_t() {
   for (int i = 0; i < DR / 16; ++i) add(nnb::W_RGBH(D), D + 27, D, 27, 16 * i, DR, 32);
   for (int i = 0; i < DR / 16; ++i) add(nnb::W_RGBH(D), D + 27, 0, D, 16 * i, DR, D);
   for (int i = 0; i < KS; ++i) add(nnb::W_FEAT(D), D, 0, D, 16 * i, D, D);
+  // A producer that waits for a stage no consumer takes never returns: the chain's bounds (Tc::dg_steps) must be the table's, for the
+  // whole chain and for the occupancy-only chain, which starts here
+  if (s != T::dg_first_stage(true) || (size_t)off != T::IMG_T_PREFIX_BYTES) return cudaErrorInvalidValue;
   for (int l = 7; l >= 1; --l) {
     if (l == 4) for (int i = 0; i < KS; ++i) add(nnb::w_off(D, 4), D + 63, D, 63, 16 * i, D, 64);
     for (int i = 0; i < KS; ++i) add(nnb::w_off(D, l), nnb::w_ld(D, l), 0, D, 16 * i, D, D);
   }
   for (int i = 0; i < KS; ++i) add(nnb::w_off(D, 0), 63, 0, 63, 16 * i, D, 64);
-  if (s != T::N_STAGES_T || (size_t)off != T::IMG_T_BYTES) return cudaErrorInvalidValue;
+  if (s != T::dg_tile_stages(false) || s - T::dg_first_stage(true) != T::dg_tile_stages(true) || (size_t)off != T::IMG_T_BYTES)
+    return cudaErrorInvalidValue;
   cudaError_t e;
   if constexpr (D == 256) e = cudaMemcpyToSymbol(c_stages_t_256, h, sizeof(h));
   else if constexpr (D == 128) e = cudaMemcpyToSymbol(c_stages_t_128, h, sizeof(h));
@@ -1388,6 +1491,60 @@ cudaError_t tc_ray_march_dim(const nnb_ray_march_args& r, cudaStream_t st) {
   return cudaGetLastError();
 }
 
+// Workspace of nnb_field_vjp, every section 256-byte aligned: records [Npad] | gate bits (gate_bits_off; h0..h7 only when occ) | forward
+// weight image (the occupancy-only prefix when occ) | transposed weight image (its trunk part, from dg_first_stage(true) on, when occ)
+struct VjpWs { size_t rec, gates, img, img_t, total; };
+template <int D> VjpWs vjp_layout(int N, bool occ) {
+  using T = Tc<D>;
+  const size_t Npad = align_up((size_t)N, TILE);
+  VjpWs w{};
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  w.rec = take(Npad * sizeof(SampleRec));
+  w.gates = take(occ ? Npad * D : gate_bits_bytes(Npad, D));
+  w.img = take(occ ? (size_t)T::N_STAGES_OCC * T::STAGE_BYTES : T::IMG_PTS_BYTES);
+  w.img_t = take(occ ? T::IMG_T_BYTES - T::IMG_T_PREFIX_BYTES : T::IMG_T_BYTES);
+  w.total = off;
+  return w;
+}
+
+// nnb_field_vjp: both weight images, the forward with records and gate bits, the chain
+template <int D>
+cudaError_t tc_field_vjp_dim(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, cudaStream_t st) {
+  using T = Tc<D>;
+  const bool occ = (a.flags & NNB_OCC_ONLY) != 0;
+  cudaError_t e = upload_stage_table<D>();
+  if (e == cudaSuccess) e = upload_stage_table_t<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_points_vjp_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_vjp<D, DG_POINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_vjp<D, DG_POINTS_OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  const VjpWs w = vjp_layout<D>(a.N, occ);
+  char* base = static_cast<char*>(a.workspace);
+  SampleRec* recs = reinterpret_cast<SampleRec*>(base + w.rec);
+  unsigned char* gates = reinterpret_cast<unsigned char*>(base + w.gates);
+  unsigned char *img = reinterpret_cast<unsigned char*>(base + w.img), *img_t = reinterpret_cast<unsigned char*>(base + w.img_t);
+  tc_prep_weights<D><<<occ ? T::N_STAGES_OCC : T::N_STAGES_PTS, 256, 0, st>>>(a.weights, img);
+  tc_prep_weights_t_from<D><<<T::dg_tile_stages(occ), 256, 0, st>>>(a.weights, img_t, T::dg_first_stage(occ));
+  const int n_tiles = (a.N + TILE - 1) / TILE;
+  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  tc_points_vjp_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, reinterpret_cast<float4*>(out_rgba), gates, (size_t)a.N, n_tiles);
+  DgPtrs P{};
+  P.rec = recs; P.gates = gates;
+  P.gs = reinterpret_cast<const float4*>(g_rgba); P.gp = reinterpret_cast<float4*>(g_pts); P.gv = reinterpret_cast<float4*>(g_dirs);
+  if (occ) tc_points_vjp<D, DG_POINTS_OCC><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  else tc_points_vjp<D, DG_POINTS><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  return cudaGetLastError();
+}
+
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
 
 }  // namespace
@@ -1414,6 +1571,15 @@ cudaError_t tc_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st) {
 cudaError_t tc_field_fwd_points(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st) {
   return L.D == 128 ? tc_points_fwd_dim<128>(a, L, out_rgba, st)
        : L.D == 64  ? tc_points_fwd_dim<64>(a, L, out_rgba, st) : tc_points_fwd_dim<256>(a, L, out_rgba, st);
+}
+
+size_t tc_field_vjp_workspace(int N, uint32_t flags, int D) {
+  const bool occ = (flags & NNB_OCC_ONLY) != 0;
+  return D == 128 ? vjp_layout<128>(N, occ).total : (D == 64 ? vjp_layout<64>(N, occ).total : vjp_layout<256>(N, occ).total);
+}
+cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st) {
+  return D == 128 ? tc_field_vjp_dim<128>(a, g_rgba, out_rgba, g_pts, g_dirs, st)
+       : D == 64  ? tc_field_vjp_dim<64>(a, g_rgba, out_rgba, g_pts, g_dirs, st) : tc_field_vjp_dim<256>(a, g_rgba, out_rgba, g_pts, g_dirs, st);
 }
 
 // Backward of the TC engine: compositing / ray adjoints of nnb_simt.cu around tc_dgrad and tc_wgrad, which read and write the SIMT

@@ -98,13 +98,37 @@ class _GradFn(torch.autograd.Function):
         return (None, None, g_p[:, :3] if need_p else None) + tuple(gp)
 
 
-def field_normal(net, p):
+def field_normal(net, p, engine=None):
     """n = d(density logit)/d p, shape (M, 3), for p (M, 3).  Differentiable with respect to p and the MLP parameters (the second-order
-    backward is nnb_field_hvp); a third derivative raises.  M == 0 returns an empty tensor without a library call."""
+    backward is nnb_field_hvp); a third derivative raises.  M == 0 returns an empty tensor without a library call.
+    engine: None or 'simt' = the exact-fp32 engine.  'tc' (or ENGINE_TC) = the tensor-core data gradient (nnb_field_vjp) when the call
+    needs no autograd graph (the rule of field_query); a call that needs one runs on the exact engine, which has the second-order
+    backward.  The tensor-core normals agree with float64 to 1.4e-5 of their maximum (the exact engine's to 5e-7), where both use the same
+    ReLU gates; at a point whose pre-activation lies within rounding of 0 the engines may gate a unit differently, and the normal, which is
+    discontinuous there, then differs by that unit's contribution."""
     ops._need_cuda(p, "p")
     if p.shape[0] == 0:
         return p * 0.0          # shape (0, 3), connected to p when p requires grad, so a backward over it gives zeros
+    if _engine_id(engine) == L.ENGINE_TC and not needs_grad(net, p):
+        return _normal_tc(net, p)
     return _GradFn.apply(net, net.flat_weights(), p, *list(net.parameters()))
+
+
+def _normal_tc(net, p):
+    """nnb_field_vjp with the cotangent (0, 0, 0, 1) on the raw density logit, occupancy-only: d logit / d p (M, 3).  No autograd."""
+    M, dev = p.shape[0], p.device
+    flags = L.RAW_DENSITY | L.OCC_ONLY
+    a = L.RenderArgs()
+    flat = net.flat_weights()
+    p_c = ops._f32c(p.detach())
+    a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = None
+    a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_TC; a.hidden_dim = net.hidden_dim
+    g = torch.zeros(M, 4, device=dev); g[:, 3] = 1.0
+    g_p = torch.empty(M, 4, device=dev)
+    ws = torch.empty(L.lib.nnb_field_vjp_workspace_bytes(M, flags, net.hidden_dim), dtype=torch.uint8, device=dev)
+    a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+    L.check(L.lib.nnb_field_vjp(C.byref(a), L.ptr(g), None, L.ptr(g_p), None, ops._stream()), "nnb_field_vjp")
+    return g_p[:, :3]
 
 
 def _field_tc(net, flags, p, d):

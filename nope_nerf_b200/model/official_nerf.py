@@ -115,21 +115,23 @@ class OfficialStaticNerf(nn.Module):
         _, s = field_query(self, p, None, raw_density=True, occ_only=True, engine=engine)
         return None, s
 
-    def gradient(self, p, it):
+    def gradient(self, p, it, engine=None):
         """official_nerf.py:46-58: -d(density logit)/d p, shape (N, 1, 3) (surface normals of the geometry view).  The reference
         differentiates infer_occ with autograd (create_graph=True); here it is the data-gradient chain of the field kernel with cotangent
         1 on the logit.  With grad mode on and p requiring grad the result has a grad_fn: its backward is the second-order field kernel
         (nnb_field_hvp) and reaches p and the MLP parameters, so normal regularisers train the field.  The reference sets requires_grad
         on the caller's p itself; here the caller does (p.requires_grad_(True) for a regulariser on fixed points), and otherwise the
         normals come back detached, as plain values that callers may read directly (.numpy()).  Renderer.nope_nerf's normal term sets
-        requires_grad on its own surface points, as the reference does, so it reaches the MLP with a fixed pose, camera and depth too."""
+        requires_grad on its own surface points, as the reference does, so it reaches the MLP with a fixed pose, camera and depth too.
+        engine: None = the exact-fp32 engine; 'tc' = the tensor-core data gradient (nnb_field_vjp) for detached normals.  A call that
+        returns a grad_fn (grad mode on and p requiring grad) runs on the exact engine whatever engine it names (field.field_normal)."""
         from ..field import field_normal
         q = p.reshape(-1, 3)
         if torch.is_grad_enabled() and p.requires_grad:
             n = field_normal(self, q)
         else:
             with torch.no_grad():
-                n = field_normal(self, q)
+                n = field_normal(self, q, engine=engine)
         return -n.reshape(p.shape).unsqueeze(1)
 
     def forward(self, p, ray_d=None, only_occupancy=False, return_logits=False, return_addocc=False,

@@ -7,6 +7,13 @@ from .. import ops
 from .. import _lib as L
 from ..field import ray_march, needs_grad, _engine_id
 
+# Pixels per phong_renderer call of a whole-frame geometry view (Extract_Images.render_geometry, Trainer.render_visdata), on every
+# engine: the reference's 1024.  The field queries do not depend on the chunk (every point's result is its own on the tensor-core
+# engine), but the camera rays do: the batched matmul T @ ph of _rays_world rounds differently with the number of pixels in the call
+# (measured on an H100: about 1 % of a 60 x 80 frame's pixels change between one call and 1024-pixel chunks), so a larger chunk would
+# change the frame's bits.
+GEOMETRY_CHUNK = 1024
+
 
 class Renderer(nn.Module):
     def __init__(self, model, cfg, device=None, **kwargs):
@@ -20,8 +27,11 @@ class Renderer(nn.Module):
         self.engine = kwargs.get("engine", None)
         # engine of the geometry view's explicit-point queries (ray marching, secant steps, surface colour): None = exact fp32,
         # 'tc' = tensor cores (OfficialStaticNerf.forward(engine=)); ray marching and the secant steps are then one fused call
-        # (field.ray_march).  The normals stay on gradient(), which is exact fp32.
+        # (field.ray_march).
         self.field_engine = kwargs.get("field_engine", None)
+        # engine of the geometry view's normals (OfficialStaticNerf.gradient(engine=)): None = exact fp32, 'tc' = the tensor-core data
+        # gradient.  Separate from field_engine, so that a renderer built with field_engine='tc' keeps the bits it had.
+        self.normal_engine = kwargs.get("normal_engine", None)
 
     def to(self, device):
         model = super().to(device)
@@ -161,7 +171,7 @@ class Renderer(nn.Module):
             surface_view_vol = view_vol[network_object_mask]
         rgb_val = torch.zeros(batch_size * num_pixels, 3, device=dev)
         if surface_points.shape[0] > 0:
-            grad = self.model.gradient(surface_points, it)[:, 0, :].detach()
+            grad = self.model.gradient(surface_points, it, engine=self.normal_engine)[:, 0, :].detach()
             surface_normals = grad / grad.norm(2, 1, keepdim=True)
             diffuse = torch.mm(surface_normals, light).clamp_min(0).repeat(1, 3) * diffuse_per.unsqueeze(0)
             rgb_values[network_object_mask] = (ambiant.unsqueeze(0) + diffuse).clamp_max(1.0)

@@ -21,6 +21,7 @@ from .. import ops
 from .. import _lib as L
 from .losses import Loss
 from .common import arange_pixels
+from .rendering import GEOMETRY_CHUNK
 
 logger_py = logging.getLogger(__name__)
 
@@ -1025,7 +1026,8 @@ class Trainer(object):
         if self.vis_geo:       # training.py:146-161: the shaded geometry view is what render_visdata returns when it is on
             with torch.no_grad():
                 geo = torch.cat([self.model(px, None, camera_mat, world_mat, scale_mat, 'phong_renderer', add_noise=False, eval_mode=True,
-                                            it=it, depth_img=dpt, img_size=(h, w))['rgb'] for px in torch.split(pixels, 1024, dim=1)], dim=1)
+                                            it=it, depth_img=dpt, img_size=(h, w))['rgb']
+                                 for px in torch.split(pixels, GEOMETRY_CHUNK, dim=1)], dim=1)
             img_out = (geo.view(h, w, 3).cpu().numpy() * 255).astype(np.uint8)
             if out_render_path is not None:
                 from PIL import Image
