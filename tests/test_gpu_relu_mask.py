@@ -109,8 +109,9 @@ def _cuda(x):
     return torch.from_numpy(np.ascontiguousarray(x)).cuda()
 
 
-def _render(P, D, N, S, seed, engine=None):
-    """TC (or `engine`) render forward with NNB_STASH on seeded inputs; returns the call (its workspace holds the stash)"""
+def _render(P, D, N, S, seed, engine=None, flags=None):
+    """TC (or `engine`) render forward with NNB_STASH on seeded inputs; returns the call (its workspace holds the stash).  flags:
+    the rendering flags (default: those of the default config with the softplus occupancy activation)"""
     from nope_nerf_b200 import ops, _lib as L
     rng = np.random.default_rng(seed)
     H, W = 48, 64
@@ -119,7 +120,8 @@ def _render(P, D, N, S, seed, engine=None):
     c2w = torch.empty(4, 4, device="cuda"); ops.pose_fwd_raw(r, t, None, 1, c2w)
     cam = torch.diag(torch.tensor([1.2, -1.6, -1.0, 1.0])).cuda()
     ray_idx = rng.permutation(H * W)[:N]
-    return ops.RenderCall(_cuda(O.flatten_params(P)), c2w, cam, N=N, S=S, flags=ops.flags_from_cfg(cfg, "softplus"),
+    flags = ops.flags_from_cfg(cfg, "softplus") if flags is None else flags
+    return ops.RenderCall(_cuda(O.flatten_params(P)), c2w, cam, N=N, S=S, flags=flags,
                           engine=L.ENGINE_TC if engine is None else engine,
                           near=0.01, far=10.0, ray_idx=_cuda(ray_idx), depth_map=_cuda(rng.uniform(.6, 7.2, (24, 32)).astype(np.float32)),
                           scale=torch.tensor([1.05]).cuda(), shift=torch.tensor([0.02]).cuda(),
