@@ -392,8 +392,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         if ((kb >> 2) != part) continue;   // static register indices: ee[] stays in registers
         split_store8(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
         if (stash) {
-          *reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8) = make_float4(ee[kb * 8], ee[kb * 8 + 1], ee[kb * 8 + 2], ee[kb * 8 + 3]);
-          *reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8 + 4) = make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]);
+          __stcs(reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8), make_float4(ee[kb * 8], ee[kb * 8 + 1], ee[kb * 8 + 2], ee[kb * 8 + 3]));
+          __stcs(reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8 + 4), make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]));
         }
       }
       if constexpr (!PTS) if (part == 0) {   // direction-encoding term of rgb_layers.0 is constant per ray: folded into a per-ray bias below
@@ -405,7 +405,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         if (stash) {
 #pragma unroll
           for (int k4 = 0; k4 < 8; ++k4)
-            *reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4) = make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]);
+            __stcs(reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4), make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]));
         }
         if (rl == 0 || (off0 + rl) % a.S == 0) {   // the block's first row and every row that starts a ray publish its direction encoding
           const int r = (off0 + rl) / a.S;
@@ -1141,7 +1141,7 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
         const SampleRec rec = P.rec[m];
         const float g0 = g.x * rec.r * (1.f - rec.r), g1 = g.y * rec.g * (1.f - rec.g), g2 = g.z * rec.b * (1.f - rec.b);
         const float g3 = g.w * density_act_grad(rec.s, a.flags);
-        if (write_dy) P.dyc[m] = make_float4(g0, g1, g2, g3);
+        if (write_dy) __stcs(P.dyc + m, make_float4(g0, g1, g2, g3));
         gyc[tl * 4] = g0; gyc[tl * 4 + 1] = g1; gyc[tl * 4 + 2] = g2; gyc[tl * 4 + 3] = g3;
       }
     }
@@ -1164,7 +1164,7 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
             const float x1 = g4[0] * s_small[col + 1] + g4[1] * s_small[DR + col + 1] + g4[2] * s_small[2 * DR + col + 1];
             const uint32_t b = gm[j / 8] << (4 * (j & 7) + 2 * r);
             const float v0 = (b & 0x80000000u) ? x0 : 0.f, v1 = (b & 0x40000000u) ? x1 : 0.f;
-            if (write_dy) *reinterpret_cast<float2*>(P.dyr + (mt + row) * DR + col) = make_float2(v0, v1);
+            if (write_dy) __stcs(reinterpret_cast<float2*>(P.dyr + (mt + row) * DR + col), make_float2(v0, v1));
             uint32_t hw, lw;
             split2_bf16(v0, v1, hw, lw);
             *reinterpret_cast<uint32_t*>(ahi + j * 2048) = hw;
