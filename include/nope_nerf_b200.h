@@ -219,6 +219,54 @@ typedef struct nnb_ray_march_args {
 size_t nnb_ray_march_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
 int nnb_ray_march(const nnb_ray_march_args* a, void* stream);
 
+/* The geometry view of any set of N pixels in one stream-ordered call: what Renderer.phong_renderer (model/rendering.py:148-180) does,
+ * with every ray computed per pixel, on the tensor-core engine.  No version bump: the symbol marks the capability.
+ *   Rays: cw = T[:3,3] (T row-major [16], T = S^-1 W^-1 K^-1 as Renderer._rays_world forms it), pw_r = ((T[r,0] x + T[r,1] y) + T[r,2])
+ *     + T[r,3] for the pixel (x, y), d = pw - cw, |d| = sqrt((d0 d0 + d1 d1) + d2 d2), dir = d / |d|.
+ *   Far (Renderer._sphere_far): dot = (dir0 cw0 + dir1 cw1) + dir2 cw2, c = sqrt((cw0 cw0 + cw1 cw1) + cw2 cw2),
+ *     under = dot dot - (c c - radius radius), far = sqrt(under) - dot where under > 0, else 0; then clamped at 0.
+ *   March: nnb_ray_march on (ray0 = cw, dir, far) from near_ over frac, n_secant secant steps (its contract, above).
+ *   An object ray has a finite depth that is not 0.  Its surface point p = ray0 + dir depth (a product, then a sum, per component);
+ *     grad = -d logit / d p (OfficialStaticNerf.gradient: nnb_field_vjp with NNB_RAW_DENSITY | NNB_OCC_ONLY and the cotangent
+ *     (0, 0, 0, 1), negated); n = grad / sqrt((g0 g0 + g1 g1) + g2 g2); light = cw / |cw| (the same sum order);
+ *     rgb = min(0.3 + 0.7 max((n0 l0 + n1 l1) + n2 l2, 0), 1) in every channel; rgb_surf = the rgb of nnb_field_fwd (NNB_ENGINE_TC) at
+ *     (p, -dir).  The clamps are comparisons: a zero gradient gives NaN, which passes through them as through torch's clamp_min / clamp_max.
+ *   Any other pixel: rgb = (1, 1, 1), rgb_surf = (0, 0, 0) (and grad = 0).
+ * Every product, sum, quotient and square root above is rounded on its own (no FMA contraction), in the order written.
+ * Pixel independence: a pixel's outputs depend on its coordinates, T, the weights and the scalar arguments alone, not on N, its position in
+ * the list or the other pixels (every tensor-core query is independent of its row).  Splitting a frame into calls of any size gives the same
+ * bits.  Renderer.phong_renderer's rays come from a batched matmul whose rounding depends on the pixel count, so a frame from this call
+ * differs from that path's in the last bits of its rays.
+ * Stage bit-equality, from the call's own ray0 / ray_dir / far_: depth is nnb_ray_march's; grad is the negated g_pts of nnb_field_vjp at p;
+ * rgb_surf is nnb_field_fwd's (NNB_ENGINE_TC) at (p, -ray_dir).
+ * Errors, with nothing launched: engine != NNB_ENGINE_TC (rc -4); an undefined flag bit (-7); a defined flag other than NNB_DIST_ALPHA /
+ * NNB_SOFTPLUS (-6); an unsupported width (-8); N < 0, n_steps < 2 or n_secant < 0 (-2); a NULL weights / T / pixels / frac / rgb /
+ * rgb_surf, a float pointer not 4-byte aligned or grad not 16-byte aligned (-3); a workspace smaller than
+ * nnb_geometry_frame_workspace_bytes(N, n_steps, hidden_dim) or not 256-byte aligned (-5).  N == 0 returns 0 and launches nothing.
+ * Nothing synchronises or allocates: every launch after the first sizes itself from a counter in the workspace.
+ * Workspace, each section 256-byte aligned: hit count | ray0, dir (12 N bytes each), far, depth (4 N each) | compacted rows: surface
+ * points, view directions (12 N each), pixel indices (4 N), normal cotangents, normals, colours (16 N each) | nnb_ray_march's workspace
+ * for N rays | nnb_field_vjp's for N points with NNB_RAW_DENSITY | NNB_OCC_ONLY | the forward weight image of the points mode (all that
+ * nnb_field_fwd's tensor-core query uses of its workspace).  N rows everywhere: the worst case, every ray hits.  At N = 1080 x 1920,
+ * n_steps = 512, D = 256: 945 541 632 bytes (0.95 GB). */
+typedef struct nnb_geometry_args {
+  const float* weights;   /* [nnb_num_params(hidden_dim)] */
+  const float* T;         /* [16] row-major S^-1 W^-1 K^-1 */
+  const float* pixels;    /* [N,2] image-plane pixel coordinates (arange_pixels) */
+  const float* frac;      /* [n_steps] = torch.linspace(0, 1, n_steps), as for nnb_ray_march */
+  int32_t N, n_steps /* >= 2 */, n_secant /* >= 0 */, hidden_dim /* 64, 128, 256; 0 = 256 */;
+  float near_, tau, radius;
+  uint32_t flags;         /* NNB_DIST_ALPHA | NNB_SOFTPLUS (the occupancy of the march) */
+  int32_t engine;         /* NNB_ENGINE_TC */
+  float* rgb;             /* [N,3] shaded view */
+  float* rgb_surf;        /* [N,3] surface colour */
+  /* optional (NULL = not wanted): */
+  float* ray0; float* ray_dir; float* far_; float* depth; float* grad;   /* [N,3] [N,3] [N] [N] [N,4] (xyz; w = 0) */
+  void* workspace; size_t workspace_bytes;
+} nnb_geometry_args;
+size_t nnb_geometry_frame_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
+int nnb_geometry_frame(const nnb_geometry_args* a, void* stream);
+
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,
                  float* c2w /*[16]*/, void* stream);

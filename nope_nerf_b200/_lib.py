@@ -36,6 +36,14 @@ class RayMarchArgs(C.Structure):   # nnb_ray_march_args
                 ("depth", _f), ("first", _f), ("bracket", _f), ("workspace", _f), ("workspace_bytes", C.c_size_t)]
 
 
+class GeometryArgs(C.Structure):   # nnb_geometry_args
+    _fields_ = [("weights", _f), ("T", _f), ("pixels", _f), ("frac", _f),
+                ("N", C.c_int32), ("n_steps", C.c_int32), ("n_secant", C.c_int32), ("hidden_dim", C.c_int32),
+                ("near_", C.c_float), ("tau", C.c_float), ("radius", C.c_float), ("flags", C.c_uint32), ("engine", C.c_int32),
+                ("rgb", _f), ("rgb_surf", _f), ("ray0", _f), ("ray_dir", _f), ("far_", _f), ("depth", _f), ("grad", _f),
+                ("workspace", _f), ("workspace_bytes", C.c_size_t)]
+
+
 class RenderBwdArgs(C.Structure):
     _fields_ = [("fwd", RenderArgs), ("g_rgb", _f), ("g_depth_pred", _f), ("g_depth_gt", _f),
                 ("g_weights", _f), ("g_c2w", _f), ("g_cam", _f), ("g_depth", _f), ("g_scale_shift", _f)]
@@ -90,6 +98,9 @@ def _load():
     lib.nnb_field_vjp.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, C.c_void_p]
     lib.nnb_field_vjp_workspace_bytes.restype = C.c_size_t
     lib.nnb_field_vjp_workspace_bytes.argtypes = [C.c_int32, C.c_uint32, C.c_int32]
+    lib.nnb_geometry_frame.argtypes = [C.POINTER(GeometryArgs), C.c_void_p]
+    lib.nnb_geometry_frame_workspace_bytes.restype = C.c_size_t
+    lib.nnb_geometry_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]
     lib.nnb_pose_bwd.argtypes = [_f, _f, _f, C.c_int32, _f, _f, _f, C.c_void_p]
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,

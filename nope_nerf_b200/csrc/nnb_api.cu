@@ -3,6 +3,7 @@
 #include <cstdio>
 #include <cstdarg>
 #include <cstring>
+#include <initializer_list>
 #include "nnb_workspace.cuh"
 
 cudaError_t simt_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
@@ -22,6 +23,8 @@ size_t tc_ray_march_workspace(int N, int n_steps, int D);
 cudaError_t tc_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st);
 size_t tc_field_vjp_workspace(int N, uint32_t flags, int D);
 cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st);
+size_t tc_geometry_frame_workspace(int N, int n_steps, int D);
+cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
 cudaError_t launch_pose_fwd(const float*, const float*, const float*, int, const int*, float*, cudaStream_t);
@@ -285,6 +288,44 @@ int nnb_field_vjp(const nnb_render_args* a, const float* g_rgba, float* out_rgba
   nnb_render_args b = *a; b.S = 1;
   cudaError_t e = tc_field_vjp(b, g_rgba, out_rgba, g_pts, g_dirs, hidden_of(a->hidden_dim), (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_vjp");
+#endif
+}
+size_t nnb_geometry_frame_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && n_steps >= 2 && nnb::dim_supported(D)) return tc_geometry_frame_workspace(N, n_steps, D);
+#endif
+  return 0;
+}
+static inline bool misaligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
+int nnb_geometry_frame(const nnb_geometry_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_geometry_frame: engine %d has no geometry frame (NNB_ENGINE_TC only; Renderer.phong_renderer serves the exact engine)",
+                a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_flags(a->flags)) return rc;
+  if (a->flags & ~(NNB_DIST_ALPHA | NNB_SOFTPLUS))
+    return fail(-6, "nnb_geometry_frame: flags 0x%x: only NNB_DIST_ALPHA and NNB_SOFTPLUS are accepted", a->flags);
+  const int D = hidden_of(a->hidden_dim);
+  if (!nnb::dim_supported(D)) return fail(-8, "hidden_dim %d is not supported (supported: 64, 128, 256; 0 means 256)", a->hidden_dim);
+  if (a->N < 0) return fail(-2, "nnb_geometry_frame: N must not be negative (got %d)", a->N);
+  if (a->n_steps < 2 || a->n_secant < 0)
+    return fail(-2, "nnb_geometry_frame: need n_steps >= 2 and n_secant >= 0 (got %d, %d)", a->n_steps, a->n_secant);
+  if (a->N == 0) return 0;
+  if (!a->weights || !a->T || !a->pixels || !a->frac || !a->rgb || !a->rgb_surf)
+    return fail(-3, "nnb_geometry_frame: weights, T, pixels, frac, rgb and rgb_surf must be non-null");
+  for (const void* p : {(const void*)a->weights, (const void*)a->T, (const void*)a->pixels, (const void*)a->frac, (const void*)a->rgb,
+                        (const void*)a->rgb_surf, (const void*)a->ray0, (const void*)a->ray_dir, (const void*)a->far_, (const void*)a->depth})
+    if (misaligned4(p)) return fail(-3, "nnb_geometry_frame: float arrays must be 4-byte aligned");
+  if (misaligned16(a->grad)) return fail(-3, "nnb_geometry_frame: grad must be a 16-byte aligned [N][4] array");
+  const size_t need = tc_geometry_frame_workspace(a->N, a->n_steps, D);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  cudaError_t e = tc_geometry_frame(*a, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_geometry_frame");
 #endif
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {

@@ -23,6 +23,10 @@
 // (ray origin, direction, depth) in the prologue and a reduction instead of an output: the first sign change of a ray's 128-step block,
 // or the update of a hit ray's secant bracket (see MarchPtrs).
 //
+// nnb_geometry_frame (the geometry view of a frame in one call) runs that march on rays made per pixel (geo_rays), compacts the object
+// rays (geo_compact), runs the points kernels on them with the row count read on the device (the DEVN forms of the bodies), and shades
+// (geo_shade).
+//
 // The backward of this engine (tc_render_bwd) runs tc_dgrad (the same skeleton through the transposed weights, gated by the
 // forward's ReLU bits) and tc_wgrad (the MLP weight-gradient GEMMs on the fp32 stash), between the compositing and ray adjoints of
 // nnb_simt.cu.
@@ -254,21 +258,24 @@ __device__ __forceinline__ void march_scan(const MarchPtrs& q, int ray, const fl
 //   FWD_SECANT: tile = 128 hit rays, evaluated q.n_secant times in a row at the secant iterate of each ray's bracket, which the thread
 //   that owns the row's logit then updates in q.brk1 (pass 0 reads q.brk0).  A row's prologue threads and that thread sit in the same
 //   warpgroup, whose barrier at the top of the tile loop orders the update before the next pass reads it.
+// DEVN (FWD_POINTS / FWD_VJP of nnb_geometry_frame): M = *q.count points, read when the kernel starts like FWD_SECANT's count; the
+// launch is sized for the largest count and a CTA without a tile leaves at once.
 enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4 };
-template <int D, int MODE>
+template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
                                             int stash) {
   using T = Tc<D>;
   constexpr bool PTS = MODE != FWD_RAYS, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
+  static_assert(!DEVN || XPTS, "a device count of explicit points");
   if constexpr (PTS) stash = 0;
   const bool gates = VJP || stash;   // the ReLU gate bits are stored
-  if constexpr (MARCH) {
+  if constexpr (MARCH || DEVN) {
     if (q.count) {
       const int c = *q.count;
       M = (size_t)c;
-      n_tiles = MODE == FWD_SECANT ? (c + TILE - 1) / TILE : c;
+      n_tiles = MODE == FWD_MARCH ? c : (c + TILE - 1) / TILE;
     }
     if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
   }
@@ -607,6 +614,14 @@ template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_points_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                               float4* __restrict__ out, size_t M, int n_tiles) {
   tc_fwd_body<D, FWD_POINTS>(a, wimg, nullptr, out, TcStash{}, MarchPtrs{}, M, n_tiles, 0);
+}
+// the same on the *count points that nnb_geometry_frame's compaction wrote (a separate name in profiles)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_fwd_n(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                float4* __restrict__ out, const int* __restrict__ count) {
+  MarchPtrs q{};
+  q.count = count;
+  tc_fwd_body<D, FWD_POINTS, true>(a, wimg, nullptr, out, TcStash{}, q, 0, 0, 0);
 }
 
 // one round of nnb_ray_march: block q.block of every ray of q.list (n_rays rays when q.count is NULL)
@@ -1033,13 +1048,21 @@ __device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint
 // are the explicit points a.pts [M]; P.gs is the caller's g_rgba [M] (rows >= M read as zero), P.gp / P.gv are g_pts / g_dirs [M] (P.gv
 // may be NULL), only rows < M are stored and nothing is stashed.  DG_POINTS_OCC is the chain of an occupancy-only forward: it starts at
 // g_h7 = g_s w_sigma (the colour prefix of the stage table is neither loaded nor issued) and reads only g_rgba[m].w.
+// DEVN (points modes, nnb_geometry_frame): M = *count points, read when the kernel starts (see tc_fwd_body's DEVN).
 enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2 };
-template <int D, int MODE>
+template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
-                                              int n_tiles, int write_dy) {
+                                              int n_tiles, int write_dy, const int* count = nullptr) {
   using T = Tc<D>;
   constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC;
+  static_assert(!DEVN || PTS, "a device count of explicit points");
   if constexpr (PTS) write_dy = 0;
+  if constexpr (DEVN) {
+    const int c = *count;
+    M = (size_t)c;
+    n_tiles = (c + TILE - 1) / TILE;
+    if ((int)blockIdx.x >= n_tiles) return;   // before any barrier exists
+  }
   constexpr int DG_AHI = T::DG_AHI, DG_ALO = T::DG_ALO, DG_W = T::DG_W, DG_GENC = T::DG_GENC, DG_SMALL = T::DG_SMALL, DG_GYC = T::DG_GYC;
   constexpr int DG_BAR = T::DG_BAR, STAGE_BYTES = T::STAGE_BYTES, DR = D / 2;
   constexpr int S0 = T::dg_first_stage(OCC), S_END = S0 + T::dg_tile_stages(OCC);   // the stages of one tile
@@ -1256,6 +1279,22 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_points_vjp(nnb_render_args a,
                                                               const __grid_constant__ DgPtrs P, size_t M, int n_tiles) {
   tc_dgrad_body<D, MODE>(a, wimg, P, M, n_tiles, 0);
 }
+// the two kernels of nnb_field_vjp on the *count points of nnb_geometry_frame
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_vjp_fwd_n(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                    SampleRec* __restrict__ recs, float4* __restrict__ out,
+                                                                    unsigned char* __restrict__ gates, const int* __restrict__ count) {
+  TcStash st{};
+  st.gates = gates;
+  MarchPtrs q{};
+  q.count = count;
+  tc_fwd_body<D, FWD_VJP, true>(a, wimg, recs, out, st, q, 0, 0, 0);
+}
+template <int D, int MODE>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_vjp_n(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                const __grid_constant__ DgPtrs P, const int* __restrict__ count) {
+  tc_dgrad_body<D, MODE, true>(a, wimg, P, 0, 0, 0, count);
+}
 
 template <int D>
 cudaError_t upload_stage_table_t() {
@@ -1400,9 +1439,10 @@ cudaError_t tc_render_fwd_dim(const nnb_render_args& a, const WsLayout& L, cudaS
   return e;
 }
 
-// nnb_field_fwd on this engine: a.pts / a.dirs [L.M][3] -> out_rgba [L.M][4]
+// the points forward: weight image into img, then a.pts / a.dirs [M][3] -> out [M][4].  count (nnb_geometry_frame): M = *count <= a.N,
+// read on the device; the launch is sized for a.N.
 template <int D>
-cudaError_t tc_points_fwd_dim(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st) {
+cudaError_t tc_points_fwd_launch(const nnb_render_args& a, unsigned char* img, float* out_rgba, size_t M, const int* count, cudaStream_t st) {
   using T = Tc<D>;
   cudaError_t e = upload_stage_table<D>();
   if (e != cudaSuccess) return e;
@@ -1410,18 +1450,25 @@ cudaError_t tc_points_fwd_dim(const nnb_render_args& a, const WsLayout& L, float
   static int n_sm = 0;
   if (!attr) {
     e = cudaFuncSetAttribute(tc_points_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_fwd_n<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
     if (e != cudaSuccess) return e;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     attr = true;
   }
-  unsigned char* img = reinterpret_cast<unsigned char*>(static_cast<char*>(a.workspace) + L.total);
   const int n_st = (a.flags & NNB_OCC_ONLY) ? T::N_STAGES_OCC : T::N_STAGES_PTS;   // the stages the kernel walks
   tc_prep_weights<D><<<n_st, 256, 0, st>>>(a.weights, img);
-  const int n_tiles = (int)((L.M + TILE - 1) / TILE);
+  const int n_tiles = (int)((M + TILE - 1) / TILE);
   const int grid = n_tiles < n_sm ? n_tiles : n_sm;
-  tc_points_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, (const unsigned char*)img, reinterpret_cast<float4*>(out_rgba), L.M, n_tiles);
+  if (count) tc_points_fwd_n<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, (const unsigned char*)img, reinterpret_cast<float4*>(out_rgba), count);
+  else tc_points_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, (const unsigned char*)img, reinterpret_cast<float4*>(out_rgba), M, n_tiles);
   return cudaGetLastError();
+}
+
+// nnb_field_fwd on this engine: a.pts / a.dirs [L.M][3] -> out_rgba [L.M][4]
+template <int D>
+cudaError_t tc_points_fwd_dim(const nnb_render_args& a, const WsLayout& L, float* out_rgba, cudaStream_t st) {
+  return tc_points_fwd_launch<D>(a, reinterpret_cast<unsigned char*>(static_cast<char*>(a.workspace) + L.total), out_rgba, L.M, nullptr, st);
 }
 
 // Workspace of nnb_ray_march, every section 256-byte aligned: counters [rounds + 1] (0: hit rays; k >= 1: rays of round k) | status,
@@ -1508,11 +1555,14 @@ template <int D> VjpWs vjp_layout(int N, bool occ) {
   return w;
 }
 
-// nnb_field_vjp: both weight images, the forward with records and gate bits, the chain
+// nnb_field_vjp: both weight images, the forward with records and gate bits, the chain.  count (nnb_geometry_frame, occupancy-only):
+// the points are the first *count <= a.N rows, read on the device; the workspace and the launches are sized for a.N.
 template <int D>
-cudaError_t tc_field_vjp_dim(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, cudaStream_t st) {
+cudaError_t tc_field_vjp_dim(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, cudaStream_t st,
+                             const int* count = nullptr) {
   using T = Tc<D>;
   const bool occ = (a.flags & NNB_OCC_ONLY) != 0;
+  if (count && !occ) return cudaErrorInvalidValue;   // only the occupancy-only chain has a device-count instantiation
   cudaError_t e = upload_stage_table<D>();
   if (e == cudaSuccess) e = upload_stage_table_t<D>();
   if (e != cudaSuccess) return e;
@@ -1522,6 +1572,8 @@ cudaError_t tc_field_vjp_dim(const nnb_render_args& a, const float* g_rgba, floa
     e = cudaFuncSetAttribute(tc_points_vjp_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_vjp<D, DG_POINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_vjp<D, DG_POINTS_OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_vjp_fwd_n<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_vjp_n<D, DG_POINTS_OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
     if (e != cudaSuccess) return e;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -1536,12 +1588,158 @@ cudaError_t tc_field_vjp_dim(const nnb_render_args& a, const float* g_rgba, floa
   tc_prep_weights_t_from<D><<<T::dg_tile_stages(occ), 256, 0, st>>>(a.weights, img_t, T::dg_first_stage(occ));
   const int n_tiles = (a.N + TILE - 1) / TILE;
   const int grid = n_tiles < n_sm ? n_tiles : n_sm;
-  tc_points_vjp_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, reinterpret_cast<float4*>(out_rgba), gates, (size_t)a.N, n_tiles);
+  float4* out4 = reinterpret_cast<float4*>(out_rgba);
+  if (count) tc_points_vjp_fwd_n<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, out4, gates, count);
+  else tc_points_vjp_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, out4, gates, (size_t)a.N, n_tiles);
   DgPtrs P{};
   P.rec = recs; P.gates = gates;
   P.gs = reinterpret_cast<const float4*>(g_rgba); P.gp = reinterpret_cast<float4*>(g_pts); P.gv = reinterpret_cast<float4*>(g_dirs);
-  if (occ) tc_points_vjp<D, DG_POINTS_OCC><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  if (count) tc_points_vjp_n<D, DG_POINTS_OCC><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, count);
+  else if (occ) tc_points_vjp<D, DG_POINTS_OCC><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
   else tc_points_vjp<D, DG_POINTS><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  return cudaGetLastError();
+}
+
+// ---- nnb_geometry_frame: the geometry view (Renderer.phong_renderer) of N pixels on the device ----------------------------------
+// Every product, sum, quotient and square root below is rounded on its own (no FMA contraction), in the order the header states.
+__device__ __forceinline__ float dot3_rn(const float* u, const float* v) {   // (u0 v0 + u1 v1) + u2 v2
+  return __fadd_rn(__fadd_rn(__fmul_rn(u[0], v[0]), __fmul_rn(u[1], v[1])), __fmul_rn(u[2], v[2]));
+}
+// one thread per pixel: ray origin cw = T[:3, 3], unit direction of pw - cw with pw = T (x, y, 1, 1), far sphere intersection
+// (Renderer._rays_world, Renderer._sphere_far)
+__global__ void geo_rays(const float* __restrict__ T, const float* __restrict__ pix, int N, float radius, float* __restrict__ ray0,
+                         float* __restrict__ dir, float* __restrict__ far, float* __restrict__ o_ray0, float* __restrict__ o_dir,
+                         float* __restrict__ o_far) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  float t[12];
+#pragma unroll
+  for (int k = 0; k < 12; ++k) t[k] = __ldg(T + k);
+  const float x = __ldg(pix + 2 * (size_t)i), y = __ldg(pix + 2 * (size_t)i + 1);
+  const float c[3] = {t[3], t[7], t[11]};
+  float d[3], v[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const float pw = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t[4 * r], x), __fmul_rn(t[4 * r + 1], y)), t[4 * r + 2]), t[4 * r + 3]);
+    d[r] = __fsub_rn(pw, c[r]);
+  }
+  const float nd = __fsqrt_rn(dot3_rn(d, d));
+#pragma unroll
+  for (int r = 0; r < 3; ++r) v[r] = __fdiv_rn(d[r], nd);
+  const float dt = dot3_rn(v, c), nc = __fsqrt_rn(dot3_rn(c, c));
+  const float under = __fsub_rn(__fmul_rn(dt, dt), __fsub_rn(__fmul_rn(nc, nc), __fmul_rn(radius, radius)));
+  float f = under > 0.f ? __fsub_rn(__fsqrt_rn(under), dt) : 0.f;
+  f = f < 0.f ? 0.f : f;
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    ray0[3 * (size_t)i + r] = c[r]; dir[3 * (size_t)i + r] = v[r];
+    if (o_ray0) o_ray0[3 * (size_t)i + r] = c[r];
+    if (o_dir) o_dir[3 * (size_t)i + r] = v[r];
+  }
+  far[i] = f;
+  if (o_far) o_far[i] = f;
+}
+// one thread per pixel, after the march: an object ray (finite depth, not 0) appends its surface point p = ray0 + dir depth, view
+// direction -dir, pixel index and the cotangent (0, 0, 0, 1) of the normal to the compacted rows; any other pixel gets its final colours
+__global__ void geo_compact(int N, const float* __restrict__ ray0, const float* __restrict__ dir, const float* __restrict__ depth,
+                            int* __restrict__ count, float* __restrict__ pts, float* __restrict__ vdir, int* __restrict__ pix,
+                            float4* __restrict__ gs, float* __restrict__ rgb, float* __restrict__ rgb_surf, float* __restrict__ o_depth,
+                            float4* __restrict__ o_grad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const float dep = depth[i];
+  if (o_depth) o_depth[i] = dep;
+  if (isfinite(dep) && dep != 0.f) {
+    const int k = atomicAdd(count, 1);   // the row order does not matter: a point's outputs depend on that point alone
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float v = dir[3 * (size_t)i + c];
+      pts[3 * (size_t)k + c] = __fadd_rn(ray0[3 * (size_t)i + c], __fmul_rn(v, dep));
+      vdir[3 * (size_t)k + c] = -v;
+    }
+    pix[k] = i;
+    gs[k] = make_float4(0.f, 0.f, 0.f, 1.f);
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { rgb[3 * (size_t)i + c] = 1.f; rgb_surf[3 * (size_t)i + c] = 0.f; }
+    if (o_grad) o_grad[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+// one thread per compacted row k < *count: grad = -d logit / d p, n = grad / |grad|, rgb = min(0.3 + 0.7 max(n . light, 0), 1) with
+// light = cw / |cw|, rgb_surf = the colour query's rgb, scattered to the row's pixel.  The clamps are comparisons, so a NaN (a zero
+// gradient) passes through them as it does through torch's clamp_min / clamp_max.
+__global__ void geo_shade(const float* __restrict__ T, const int* __restrict__ count, const int* __restrict__ pix, const float4* __restrict__ gp,
+                          const float4* __restrict__ rgba, float* __restrict__ rgb, float* __restrict__ rgb_surf, float4* __restrict__ o_grad) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= *count) return;
+  const int i = pix[k];
+  const float4 g4 = gp[k], s4 = rgba[k];
+  const float g[3] = {-g4.x, -g4.y, -g4.z}, c[3] = {__ldg(T + 3), __ldg(T + 7), __ldg(T + 11)};
+  const float ng = __fsqrt_rn(dot3_rn(g, g)), nc = __fsqrt_rn(dot3_rn(c, c));
+  float n[3], l[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) { n[r] = __fdiv_rn(g[r], ng); l[r] = __fdiv_rn(c[r], nc); }
+  const float dt = dot3_rn(n, l);
+  float s = __fadd_rn(0.3f, __fmul_rn(dt < 0.f ? 0.f : dt, 0.7f));
+  s = s > 1.f ? 1.f : s;
+  const float surf[3] = {s4.x, s4.y, s4.z};
+#pragma unroll
+  for (int r = 0; r < 3; ++r) { rgb[3 * (size_t)i + r] = s; rgb_surf[3 * (size_t)i + r] = surf[r]; }
+  if (o_grad) o_grad[i] = make_float4(g[0], g[1], g[2], 0.f);
+}
+
+// Workspace of nnb_geometry_frame, every section 256-byte aligned: hit count | ray0, dir [N][3], far, depth [N] | compacted rows: surface
+// points, view directions [N][3], pixel indices [N], normal cotangents, d logit / d p, colour query outputs [N] float4 | nnb_ray_march's
+// workspace (N rays) | nnb_field_vjp's occupancy-only workspace (N points) | the points forward's weight image (the only part of
+// nnb_field_fwd's tensor-core workspace that the points forward uses)
+struct GeoWs { size_t count, ray0, dir, far, depth, pts, vdir, pix, gs, gp, rgba, march, vjp, img, total; };
+template <int D> GeoWs geo_layout(int N, int n_steps) {
+  GeoWs w{};
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  const size_t n = (size_t)N;
+  w.count = take(4);
+  w.ray0 = take(n * 12); w.dir = take(n * 12); w.far = take(n * 4); w.depth = take(n * 4);
+  w.pts = take(n * 12); w.vdir = take(n * 12); w.pix = take(n * 4); w.gs = take(n * 16); w.gp = take(n * 16); w.rgba = take(n * 16);
+  w.march = take(march_layout<D>(N, n_steps).total);
+  w.vjp = take(vjp_layout<D>(N, true).total);
+  w.img = take(Tc<D>::IMG_PTS_BYTES);
+  w.total = off;
+  return w;
+}
+
+// nnb_geometry_frame: rays, the fused march (tc_ray_march_dim), compaction, normals (tc_field_vjp_dim) and colour (tc_points_fwd_launch)
+// of the compacted rows with their device count, shading.  Nothing is read back.
+template <int D>
+cudaError_t tc_geometry_frame_dim(const nnb_geometry_args& g, cudaStream_t st) {
+  const GeoWs w = geo_layout<D>(g.N, g.n_steps);
+  char* base = static_cast<char*>(g.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  auto F4 = [&](size_t off) { return reinterpret_cast<float4*>(base + off); };
+  int* count = reinterpret_cast<int*>(base + w.count);
+  cudaError_t e = cudaMemsetAsync(count, 0, 4, st);
+  if (e != cudaSuccess) return e;
+  const int blocks = (g.N + 255) / 256;
+  geo_rays<<<blocks, 256, 0, st>>>(g.T, g.pixels, g.N, g.radius, F(w.ray0), F(w.dir), F(w.far), g.ray0, g.ray_dir, g.far_);
+  nnb_ray_march_args r{};
+  r.weights = g.weights; r.ray0 = F(w.ray0); r.ray_dir = F(w.dir); r.far_ = F(w.far); r.frac = g.frac;
+  r.N = g.N; r.n_steps = g.n_steps; r.n_secant = g.n_secant; r.hidden_dim = D; r.near_ = g.near_; r.tau = g.tau;
+  r.flags = g.flags; r.engine = NNB_ENGINE_TC; r.depth = F(w.depth);
+  r.workspace = base + w.march; r.workspace_bytes = w.vjp - w.march;
+  e = tc_ray_march_dim<D>(r, st);
+  if (e != cudaSuccess) return e;
+  int* pix = reinterpret_cast<int*>(base + w.pix);
+  geo_compact<<<blocks, 256, 0, st>>>(g.N, F(w.ray0), F(w.dir), F(w.depth), count, F(w.pts), F(w.vdir), pix, F4(w.gs), g.rgb, g.rgb_surf,
+                                      g.depth, reinterpret_cast<float4*>(g.grad));
+  nnb_render_args a{};
+  a.weights = g.weights; a.pts = F(w.pts); a.dirs = nullptr; a.N = g.N; a.S = 1; a.hidden_dim = D; a.engine = NNB_ENGINE_TC;
+  a.flags = NNB_RAW_DENSITY | NNB_OCC_ONLY; a.workspace = base + w.vjp; a.workspace_bytes = w.img - w.vjp;
+  e = tc_field_vjp_dim<D>(a, F(w.gs), nullptr, F(w.gp), nullptr, st, count);   // d logit / d p
+  if (e != cudaSuccess) return e;
+  a.dirs = F(w.vdir); a.flags = g.flags & (NNB_DIST_ALPHA | NNB_SOFTPLUS); a.workspace = base + w.img; a.workspace_bytes = w.total - w.img;
+  e = tc_points_fwd_launch<D>(a, reinterpret_cast<unsigned char*>(base + w.img), F(w.rgba), (size_t)g.N, count, st);   // surface colour
+  if (e != cudaSuccess) return e;
+  geo_shade<<<blocks, 256, 0, st>>>(g.T, count, pix, F4(w.gp), F4(w.rgba), g.rgb, g.rgb_surf, reinterpret_cast<float4*>(g.grad));
   return cudaGetLastError();
 }
 
@@ -1580,6 +1778,13 @@ size_t tc_field_vjp_workspace(int N, uint32_t flags, int D) {
 cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st) {
   return D == 128 ? tc_field_vjp_dim<128>(a, g_rgba, out_rgba, g_pts, g_dirs, st)
        : D == 64  ? tc_field_vjp_dim<64>(a, g_rgba, out_rgba, g_pts, g_dirs, st) : tc_field_vjp_dim<256>(a, g_rgba, out_rgba, g_pts, g_dirs, st);
+}
+
+size_t tc_geometry_frame_workspace(int N, int n_steps, int D) {
+  return D == 128 ? geo_layout<128>(N, n_steps).total : (D == 64 ? geo_layout<64>(N, n_steps).total : geo_layout<256>(N, n_steps).total);
+}
+cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st) {
+  return D == 128 ? tc_geometry_frame_dim<128>(g, st) : (D == 64 ? tc_geometry_frame_dim<64>(g, st) : tc_geometry_frame_dim<256>(g, st));
 }
 
 // Backward of the TC engine: compositing / ray adjoints of nnb_simt.cu around tc_dgrad and tc_wgrad, which read and write the SIMT

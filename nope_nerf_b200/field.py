@@ -180,6 +180,45 @@ def ray_march(net, ray0, dirs, far, frac, near, n_secant, tau, want_bracket=Fals
     return (depth, first, bracket, counts) if want_bracket else depth
 
 
+def geometry_frame(net, T, pixels, frac, radius, n_secant=8, tau=0.5, near=0.0, want_intermediates=False):
+    """nnb_geometry_frame: the geometry view (Renderer.phong_renderer) of N pixels in one call on the tensor-core engine, with each
+    pixel's camera ray computed on its own: ray setup, fused march (ray_march), normals (gradient(engine='tc')), shading and surface
+    colour (field_query(engine='tc')), with no host round trip.  T (4, 4) or (1, 4, 4) = S^-1 W^-1 K^-1; pixels (..., 2) image-plane
+    coordinates (N = their count); frac (n_steps,) = torch.linspace(0, 1, n_steps); radius, tau, near floats.  Returns rgb, rgb_surf
+    (N, 3): the shaded view (1 where no surface is hit) and the surface colour (0 there).  A pixel's outputs do not depend on the other
+    pixels of the call.  No autograd.
+    want_intermediates: also returns {'ray0', 'ray_dir' (N, 3), 'far', 'depth' (N,), 'grad' (N, 3)}: the call's rays, far sphere
+    depths, march depths and -d logit / d p on the object rays (0 elsewhere)."""
+    ops._need_cuda(pixels, "pixels")
+    ops._need_cuda(T, "T")
+    px = ops._f32c(pixels.detach().reshape(-1, 2))
+    N, dev = px.shape[0], px.device
+    rgb = torch.empty(N, 3, device=dev); surf = torch.empty(N, 3, device=dev)
+    inter = None
+    if want_intermediates:
+        inter = dict(ray0=torch.empty(N, 3, device=dev), ray_dir=torch.empty(N, 3, device=dev), far=torch.empty(N, device=dev),
+                     depth=torch.empty(N, device=dev), grad=torch.empty(N, 4, device=dev))
+    if N > 0:
+        a = L.GeometryArgs()
+        keep = [net.flat_weights(), ops._f32c(T.detach().reshape(16)), px, ops._f32c(frac.detach())]
+        a.weights, a.T, a.pixels, a.frac = [L.ptr(t) for t in keep]
+        a.N = N; a.n_steps = frac.shape[0]; a.n_secant = n_secant; a.hidden_dim = net.hidden_dim
+        a.near_ = near; a.tau = tau; a.radius = radius; a.flags = _field_flags(net); a.engine = L.ENGINE_TC
+        a.rgb = L.ptr(rgb); a.rgb_surf = L.ptr(surf)
+        if inter is not None:
+            a.ray0, a.ray_dir, a.far_, a.depth, a.grad = [L.ptr(inter[k]) for k in ("ray0", "ray_dir", "far", "depth", "grad")]
+        ws = ops._pool.take(L.lib.nnb_geometry_frame_workspace_bytes(N, a.n_steps, net.hidden_dim), dev)
+        a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+        try:
+            L.check(L.lib.nnb_geometry_frame(C.byref(a), ops._stream()), "nnb_geometry_frame")
+        finally:
+            ops._pool.give(ws)   # stream-ordered, as in ray_march
+    if inter is None:
+        return rgb, surf
+    inter["grad"] = inter["grad"][:, :3]
+    return rgb, surf, inter
+
+
 def needs_grad(net, *tensors):
     """whether a field call on these inputs has to be differentiable: grad mode is on and an input or a parameter of net requires grad"""
     return torch.is_grad_enabled() and (any(t is not None and t.requires_grad for t in tensors)

@@ -38,17 +38,18 @@ class Extract_Images(object):
 
     def render_geometry(self, c2w, camera_mat, scale_mat, h, w, it=0):
         """phong-shaded surface view (extracting_images.py:80-97): Renderer.forward(..., 'phong_renderer') over chunks of
-        rendering.GEOMETRY_CHUNK pixels of the frame, (h,w,3) uint8 -- the same call sequence as the geometry view of
-        Trainer.render_visdata"""
+        rendering.GEOMETRY_CHUNK pixels of the frame, or in one call with Renderer(geometry_frame=True), (h,w,3) uint8 -- the same
+        call sequence as the geometry view of Trainer.render_visdata"""
         from .rendering import GEOMETRY_CHUNK
         from .common import arange_pixels
         dev = self.device
         _, pixels = arange_pixels(resolution=(h, w), device=dev)
         world_mat = torch.linalg.inv(c2w.detach().reshape(4, 4).float()).unsqueeze(0)
         cam = camera_mat.detach().reshape(1, 4, 4).float()
+        chunk = pixels.shape[1] if getattr(self.renderer, 'geometry_frame', False) else GEOMETRY_CHUNK
         with torch.no_grad():
             rgb = torch.cat([self.renderer(px, None, cam, world_mat, scale_mat, 'phong_renderer', eval_=True, it=it, add_noise=False)['rgb']
-                             for px in torch.split(pixels, GEOMETRY_CHUNK, dim=1)], dim=1)
+                             for px in torch.split(pixels, chunk, dim=1)], dim=1)
         return (rgb.reshape(h, w, 3).cpu().numpy() * 255).astype(np.uint8)
 
     def generate_images(self, data, render_dir, c2ws, fxfy, it, output_geo):

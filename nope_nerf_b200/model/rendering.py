@@ -5,13 +5,14 @@ import torch
 import torch.nn as nn
 from .. import ops
 from .. import _lib as L
-from ..field import ray_march, needs_grad, _engine_id
+from ..field import ray_march, needs_grad, _engine_id, geometry_frame as field_geometry_frame
 
 # Pixels per phong_renderer call of a whole-frame geometry view (Extract_Images.render_geometry, Trainer.render_visdata), on every
 # engine: the reference's 1024.  The field queries do not depend on the chunk (every point's result is its own on the tensor-core
 # engine), but the camera rays do: the batched matmul T @ ph of _rays_world rounds differently with the number of pixels in the call
 # (measured on an H100: about 1 % of a 60 x 80 frame's pixels change between one call and 1024-pixel chunks), so a larger chunk would
-# change the frame's bits.
+# change the frame's bits.  Renderer(geometry_frame=True) computes the rays per pixel instead (phong_frame), and its callers pass the
+# whole frame in one call.
 GEOMETRY_CHUNK = 1024
 
 
@@ -32,6 +33,10 @@ class Renderer(nn.Module):
         # engine of the geometry view's normals (OfficialStaticNerf.gradient(engine=)): None = exact fp32, 'tc' = the tensor-core data
         # gradient.  Separate from field_engine, so that a renderer built with field_engine='tc' keeps the bits it had.
         self.normal_engine = kwargs.get("normal_engine", None)
+        # geometry_frame=True: forward(..., 'phong_renderer') runs phong_frame (one tensor-core call for any number of pixels, rays
+        # computed per pixel), and Extract_Images.render_geometry / Trainer.render_visdata pass the whole frame in one call.  Its
+        # frames differ from phong_renderer's in the last bits of the rays, so it is off by default.
+        self.geometry_frame = kwargs.get("geometry_frame", False)
 
     def to(self, device):
         model = super().to(device)
@@ -43,6 +48,8 @@ class Renderer(nn.Module):
         if rendering_technique == 'nope_nerf':
             return self.nope_nerf(pixels, depth, camera_mat, world_mat, scale_mat, it=it, add_noise=add_noise, eval_=eval_)
         if rendering_technique == 'phong_renderer':
+            if self.geometry_frame:
+                return self.phong_frame(pixels, camera_mat, world_mat, scale_mat, it)
             return self.phong_renderer(pixels, camera_mat, world_mat, scale_mat, it)
         raise ValueError(rendering_technique)
 
@@ -122,12 +129,17 @@ class Renderer(nn.Module):
     #      `visualize_every` iterations).  Host logic mirrors the reference; every field evaluation (occupancy along the rays, secant
     #      refinement, normals = gradient(), surface colour) is a call into the CUDA library (nnb_field_fwd / nnb_field_bwd). ----
     @staticmethod
+    def _ray_transform(camera_mat, world_mat, scale_mat, dev):
+        """T = S^-1 W^-1 K^-1: image plane (x, y, 1, 1) -> world (common.py:186-237, invert=True)"""
+        Ki = torch.inverse(camera_mat.to(dev)); Wi = torch.inverse(world_mat.to(dev)); Si = torch.inverse(scale_mat.to(dev))
+        return Si @ Wi @ Ki
+
+    @staticmethod
     def _rays_world(pixels, camera_mat, world_mat, scale_mat):
         """image_points_to_world / origin_to_world (common.py:186-237, invert=True): ray origins and unit directions"""
         b, n, _ = pixels.shape
         dev = pixels.device
-        Ki = torch.inverse(camera_mat.to(dev)); Wi = torch.inverse(world_mat.to(dev)); Si = torch.inverse(scale_mat.to(dev))
-        T = Si @ Wi @ Ki
+        T = Renderer._ray_transform(camera_mat, world_mat, scale_mat, dev)
         ph = torch.cat([pixels.permute(0, 2, 1), torch.ones(b, 2, n, device=dev)], dim=1)          # depth 1: (x, y, 1, 1)
         pw = (T @ ph)[:, :3].permute(0, 2, 1)
         o = torch.zeros(b, 4, n, device=dev); o[:, -1] = 1.
@@ -178,6 +190,24 @@ class Renderer(nn.Module):
             with torch.no_grad():
                 rgb_val[network_object_mask] = self.model(surface_points, surface_view_vol, engine=self.field_engine)
         return {'rgb': rgb_values.reshape(batch_size, -1, 3), 'normal': None, 'rgb_surf': rgb_val.reshape(batch_size, -1, 3)}
+
+    def phong_frame(self, pixels, camera_mat, world_mat, scale_mat, it):
+        """phong_renderer's view and output dict in one tensor-core call for any number of pixels (field.geometry_frame), always on the
+        tensor-core engine.  Each pixel's camera ray is computed on its own, so a pixel's result does not depend on how the frame is split
+        into calls; it differs from phong_renderer's, whose rays come from a batched matmul over the call's pixels, in the last bits of
+        the rays.  Draws the single torch.randint that ray_marching draws (n_steps = 512), so a call consumes the same random numbers."""
+        batch_size, num_pixels, _ = pixels.shape
+        if batch_size != 1:
+            raise NotImplementedError("batch_size must be 1 (configs/default.yaml:14)")
+        ops._need_cuda(pixels, "pixels")
+        dev = pixels.device
+        T = self._ray_transform(camera_mat, world_mat, scale_mat, dev)
+        n_steps = int(torch.randint(512, 513, (1,)).item())
+        frac = torch.linspace(0, 1, steps=n_steps, device=dev)
+        self.model.eval()
+        with torch.no_grad():
+            rgb, rgb_surf = field_geometry_frame(self.model, T, pixels, frac, float(self.cfg['radius']), n_secant=8, tau=0.5, near=0.0)
+        return {'rgb': rgb.reshape(batch_size, -1, 3), 'normal': None, 'rgb_surf': rgb_surf.reshape(batch_size, -1, 3)}
 
     def ray_marching(self, ray0, ray_direction, model, c=None, tau=0.5, n_steps=[128, 129], n_secant_steps=8, depth_range=[0., 2.4],
                      max_points=3500000, rad=1.0):

@@ -1024,10 +1024,12 @@ class Trainer(object):
             Image.fromarray(dn).save(os.path.join(out_render_path, '%04d_depth.png' % int(img_idx)))
             Image.fromarray(img_out).convert("RGB").save(os.path.join(out_render_path, '%04d_img.png' % int(img_idx)))
         if self.vis_geo:       # training.py:146-161: the shaded geometry view is what render_visdata returns when it is on
+            # Renderer(geometry_frame=True): the whole frame in one call (its rays do not depend on the chunk)
+            chunk = pixels.shape[1] if getattr(self.model.renderer, 'geometry_frame', False) else GEOMETRY_CHUNK
             with torch.no_grad():
                 geo = torch.cat([self.model(px, None, camera_mat, world_mat, scale_mat, 'phong_renderer', add_noise=False, eval_mode=True,
                                             it=it, depth_img=dpt, img_size=(h, w))['rgb']
-                                 for px in torch.split(pixels, GEOMETRY_CHUNK, dim=1)], dim=1)
+                                 for px in torch.split(pixels, chunk, dim=1)], dim=1)
             img_out = (geo.view(h, w, 3).cpu().numpy() * 255).astype(np.uint8)
             if out_render_path is not None:
                 from PIL import Image
