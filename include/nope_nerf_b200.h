@@ -267,6 +267,42 @@ typedef struct nnb_geometry_args {
 size_t nnb_geometry_frame_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
 int nnb_geometry_frame(const nnb_geometry_args* a, void* stream);
 
+/* The volumetric view of a whole frame (or any N rays) in one stream-ordered call on the tensor-core engine, with compositing fused into
+ * the field's forward: what nnb_render_fwd does without NNB_STASH, in a workspace that does not grow with S, and optionally with early ray
+ * termination.  No version bump: the symbol marks the capability.
+ *   Inputs and outputs are those of nnb_render_fwd (f->fwd): rgb, depth_pred, depth_gt and mask per ray, the flags NNB_DIST_ALPHA, NNB_NDC,
+ *   NNB_NORMALISE, NNB_USE_DIR, NNB_WHITE_BG, NNB_EVAL, NNB_SOFTPLUS and NNB_SHIFT_FIRST, ray_idx / pixels and depth / depth_map as there.
+ *   Chunk rule: the rays advance in rounds of 32 samples; round k evaluates samples 32 k .. 32 k + 31 of every ray still live and
+ *   composites them as composite_fwd's chunk k does.  A ray stops after the first chunk that leaves its transmittance (the product of
+ *   1 - alpha_j + 1e-6 over its samples so far) below t_min, or after its last chunk.  t_min = 0 never stops a ray.
+ *   n_eval [N] (optional): samples evaluated per ray (S when the ray was not stopped); t_final [N] (optional): its transmittance after
+ *   the last evaluated sample.
+ * Bit-equality: at t_min = 0 every output is bit-identical to nnb_render_fwd on NNB_ENGINE_TC with the same arguments (the tensor-core
+ *   field result of a sample does not depend on its tile or row, and the terms of a ray are summed in composite_fwd's order).  For any
+ *   t_min, a ray with n_eval == S has exactly the bits of the t_min = 0 call.  A ray's outputs depend on that ray alone, so they are the
+ *   same bits on every run and for any split of the rays into calls.
+ * Error bound for t_min > 0: with eps = 1e-6, T_{j+1} = T_j (1 - alpha_j + eps), so the weight a stopped ray drops, sum_{j >= n_eval}
+ *   alpha_j T_j, is at most t_final (1 + eps S (1 + eps)^S) < 1.002 t_final for S <= 1024.  rgb and the accumulated weight move by at
+ *   most that (plus rounding); with NNB_WHITE_BG rgb by at most twice that; depth_pred by at most that times far_ (1 with NNB_NDC),
+ *   divided by the ray's norm under NNB_EVAL | NNB_NORMALISE.
+ * Errors, with nothing launched (the codes of nnb_render_fwd / nnb_ray_march for the same faults): f == NULL (rc -1); an engine other than
+ *   NNB_ENGINE_TC (-4); an undefined flag bit (-7); NNB_STASH, NNB_HVP, NNB_OCC_ONLY or NNB_RAW_DENSITY (-6); an unsupported width (-8);
+ *   N <= 0 or S outside 2..1024 (-2); S in 2..15 (-4, the tensor-core engine's limit); a non-NULL noise, z_vals, alpha, pts or dirs (-6);
+ *   t_min negative or NaN (-2); a NULL weights / c2w / cam / output, no ray_idx or pixels, no depth or depth_map, or n_eval / t_final
+ *   not 4-byte aligned (-3); a workspace smaller than nnb_render_frame_workspace_bytes(N, S, hidden_dim) or not 256-byte aligned (-5).
+ * Workspace, each section 256-byte aligned: round counters (256 bytes) | carry, chunks per ray (4 N bytes each) | per-ray lane partials of
+ *   the weighted colour, depth and weight (640 N bytes) | two ray lists (4 N bytes each) | the forward weight image (2 359 296 bytes at
+ *   D = 256).  It does not depend on S: at N = 1080 x 1920, D = 256, 1 362 641 152 bytes (1.36 GB), where nnb_render_fwd needs 32 N S
+ *   bytes of sample records (8.5 GB at S = 128). */
+typedef struct nnb_frame_args {
+  nnb_render_args fwd;   /* the inputs and outputs of nnb_render_fwd; the workspace is sized by nnb_render_frame_workspace_bytes */
+  float t_min;           /* a ray stops after the first 32-sample chunk that leaves its transmittance below t_min; 0 = never */
+  int32_t* n_eval;       /* optional [N]: samples evaluated per ray (S when the ray was not stopped)                          */
+  float* t_final;        /* optional [N]: transmittance after the last evaluated sample                                        */
+} nnb_frame_args;
+size_t nnb_render_frame_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
+int nnb_render_frame(const nnb_frame_args* f, void* stream);
+
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,
                  float* c2w /*[16]*/, void* stream);

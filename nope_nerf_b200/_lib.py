@@ -44,6 +44,10 @@ class GeometryArgs(C.Structure):   # nnb_geometry_args
                 ("workspace", _f), ("workspace_bytes", C.c_size_t)]
 
 
+class FrameArgs(C.Structure):   # nnb_frame_args
+    _fields_ = [("fwd", RenderArgs), ("t_min", C.c_float), ("n_eval", _f), ("t_final", _f)]
+
+
 class RenderBwdArgs(C.Structure):
     _fields_ = [("fwd", RenderArgs), ("g_rgb", _f), ("g_depth_pred", _f), ("g_depth_gt", _f),
                 ("g_weights", _f), ("g_c2w", _f), ("g_cam", _f), ("g_depth", _f), ("g_scale_shift", _f)]
@@ -101,6 +105,9 @@ def _load():
     lib.nnb_geometry_frame.argtypes = [C.POINTER(GeometryArgs), C.c_void_p]
     lib.nnb_geometry_frame_workspace_bytes.restype = C.c_size_t
     lib.nnb_geometry_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    lib.nnb_render_frame.argtypes = [C.POINTER(FrameArgs), C.c_void_p]
+    lib.nnb_render_frame_workspace_bytes.restype = C.c_size_t
+    lib.nnb_render_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]
     lib.nnb_pose_bwd.argtypes = [_f, _f, _f, C.c_int32, _f, _f, _f, C.c_void_p]
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,

@@ -24,6 +24,8 @@ cudaError_t tc_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st);
 size_t tc_field_vjp_workspace(int N, uint32_t flags, int D);
 cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st);
 size_t tc_geometry_frame_workspace(int N, int n_steps, int D);
+size_t tc_render_frame_workspace(int N, int D);
+cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st);
 cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
@@ -326,6 +328,46 @@ int nnb_geometry_frame(const nnb_geometry_args* a, void* stream) {
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
   cudaError_t e = tc_geometry_frame(*a, D, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_geometry_frame");
+#endif
+}
+size_t nnb_render_frame_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && tc_supports(S) && nnb::dim_supported(D)) return tc_render_frame_workspace(N, D);
+#endif
+  return 0;
+}
+int nnb_render_frame(const nnb_frame_args* f, void* stream) {
+  if (!f) return fail(-1, "null args");
+  const nnb_render_args* a = &f->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_frame: engine %d has no frame renderer (NNB_ENGINE_TC only; nnb_render_fwd serves the exact engine)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_flags(a->flags)) return rc;
+  if (a->flags & (NNB_STASH | NNB_HVP | NNB_OCC_ONLY | NNB_RAW_DENSITY))
+    return fail(-6, "nnb_render_frame: NNB_STASH, NNB_HVP, NNB_OCC_ONLY and NNB_RAW_DENSITY are not accepted (flags 0x%x)", a->flags);
+  if (int rc = check_dim(a)) return rc;
+  if (a->N <= 0) return fail(-2, "N must be positive (got %d)", a->N);
+  if (a->S < 2 || a->S > 1024) return fail(-2, "S must be in [2,1024] (got %d)", a->S);
+  if (!tc_supports(a->S)) return fail(-4, "tensor-core engine needs S in [16,1024] (got %d); use nnb_render_fwd on NNB_ENGINE_SIMT", a->S);
+  if (a->noise || a->z_vals || a->alpha || a->pts || a->dirs)
+    return fail(-6, "nnb_render_frame: noise, z_vals, alpha, pts and dirs must be NULL (no jitter, no per-sample outputs)");
+  if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_frame: t_min must be >= 0 (got %g)", (double)f->t_min);
+  if (!a->weights || !a->c2w || !a->cam) return fail(-3, "weights / c2w / cam must be non-null");
+  if (!a->ray_idx && !a->pixels) return fail(-3, "need ray_idx or pixels");
+  if (!a->pixels && (a->H < 2 || a->W < 2)) return fail(-3, "H,W needed to derive pixels from ray_idx");
+  if (!a->depth && !(a->depth_map && a->ray_idx && a->h_d > 0 && a->w_d > 0 && a->H > 0 && a->W > 0))
+    return fail(-3, "need depth[N] or (depth_map,h_d,w_d,H,W,ray_idx)");
+  if (!a->rgb || !a->depth_pred || !a->depth_gt || !a->mask) return fail(-3, "output pointers must be non-null");
+  if (misaligned4(f->n_eval) || misaligned4(f->t_final)) return fail(-3, "nnb_render_frame: n_eval and t_final must be 4-byte aligned");
+  const int D = hidden_of(a->hidden_dim);
+  const size_t need = tc_render_frame_workspace(a->N, D);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  cudaError_t e = tc_render_frame(*a, f->t_min, f->n_eval, f->t_final, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame");
 #endif
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {

@@ -214,3 +214,42 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // per-sample record written by the MLP stage, read by compositing / backward
 struct __align__(16) SampleRec { float r, g, b, a; float s, z, pad0, pad1; };
+
+// ---- the arithmetic of composite_fwd (rendering.py:122-158) for the tensor-core frame renderer (tc_frame, frame_finish) ----
+// composite_alpha is composite_fwd's own (through sample_alpha).  composite_chunk and composite_tail are the statements of its loop body and
+// of its end, in the same order; composite_fwd keeps its own copy of them, because nvcc 12.9 allocates composite_fwd's registers
+// differently when it calls them, and its SASS is kept as it was.  tests/test_gpu_render_frame.py checks that the two give the same bits.
+// alpha of sample i from its MLP output a_i and depth z_i; z_next() is the depth of sample i + 1, read only with NNB_DIST_ALPHA and i < S - 1
+template <typename ZNext>
+__device__ __forceinline__ float composite_alpha(const nnb_render_args& a, int i, float a_i, float z_i, ZNext&& z_next) {
+  if (!(a.flags & NNB_DIST_ALPHA)) return a_i;
+  if (i == a.S - 1) return 1.f;  // alpha[:, -1] = 1 (rendering.py:128)
+  float delta = __fsub_rn(z_next(), z_i);
+  return 1.f - expf(-a_i * delta);
+}
+// one 32-sample chunk of a ray, one warp, lane = sample (valid: inside the ray; an invalid lane has alpha = r = g = b = z = 0): carry is
+// the transmittance before the chunk on entry and after it on return (the same in every lane); C0..C2, Dist and acc are this lane's
+// partial sums of the weighted colour, depth and weight
+__device__ __forceinline__ void composite_chunk(float alpha, bool valid, float r, float g, float b, float z, int lane, float& carry, float& C0,
+                                                float& C1, float& C2, float& Dist, float& acc) {
+  float om = valid ? __fadd_rn(__fsub_rn(1.f, alpha), NNB_EPS) : 1.f;
+  float incl = warp_incl_prod(om, lane);
+  float excl = __shfl_up_sync(0xffffffffu, incl, 1); if (lane == 0) excl = 1.f;
+  float T = carry * excl;
+  carry *= __shfl_sync(0xffffffffu, incl, 31);
+  float wgt = alpha * T;
+  C0 += wgt * r; C1 += wgt * g; C2 += wgt * b; Dist += wgt * z; acc += wgt;
+}
+// the ray's outputs from the lane partials: warp sums, white background, the EVAL | NORMALISE division, NDC depth_gt, mask
+__device__ __forceinline__ void composite_tail(const nnb_render_args& a, int n, const Ray& ray, float C0, float C1, float C2, float Dist, float acc,
+                                               int lane) {
+  C0 = warp_sum(C0); C1 = warp_sum(C1); C2 = warp_sum(C2); Dist = warp_sum(Dist); acc = warp_sum(acc);
+  if (lane == 0) {
+    if (a.flags & NNB_WHITE_BG) { float bg = 1.f - acc; C0 += bg; C1 += bg; C2 += bg; }
+    float g = ray.g;
+    if ((a.flags & NNB_EVAL) && (a.flags & NNB_NORMALISE)) { Dist = Dist / ray.nrm; g = g / ray.nrm; }
+    if (a.flags & NNB_NDC) g = 1.f - 1.f / g;
+    a.rgb[3 * n] = C0; a.rgb[3 * n + 1] = C1; a.rgb[3 * n + 2] = C2;
+    a.depth_pred[n] = Dist; a.depth_gt[n] = g; a.mask[n] = ray.mask ? 1 : 0;
+  }
+}

@@ -250,10 +250,7 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
 // compositing (rendering.py:122-158), one warp per ray; shared by both engines
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ float sample_alpha(const nnb_render_args& a, const SampleRec* rr, int i, const SampleRec& me) {
-  if (!(a.flags & NNB_DIST_ALPHA)) return me.a;
-  if (i == a.S - 1) return 1.f;  // alpha[:, -1] = 1 (rendering.py:128)
-  float delta = __fsub_rn(rr[i + 1].z, me.z);
-  return 1.f - expf(-me.a * delta);
+  return composite_alpha(a, i, me.a, me.z, [&] { return rr[i + 1].z; });
 }
 
 __global__ void composite_fwd(nnb_render_args a, const SampleRec* recs) {

@@ -248,6 +248,57 @@ __device__ __forceinline__ void march_scan(const MarchPtrs& q, int ray, const fl
   }
 }
 
+// nnb_render_frame (the volumetric view of a frame, tc_frame): rounds of 32-sample chunks.  Round k evaluates chunk k of every ray still
+// live; a tile is 4 ray-chunks x 32 rows, composited in the tile's back end (frame_step) into per-ray lane partials in the workspace
+// (FramePtrs); a ray whose transmittance fell below t_min, or that has no chunk left, leaves; frame_finish writes the outputs.
+struct FramePtrs {
+  int k;               // this round evaluates samples 32 k .. 32 k + 31 of its rays
+  float t_min;
+  const int* list;     // the rays of this round (NULL in round 0: every ray, ray-chunk = ray)
+  const int* count;    // device count of `list` (NULL: a.N)
+  int *next_list, *next_count;   // rays still live after this round
+  float* carry;        // [N] transmittance after the ray's last evaluated chunk
+  int* chunks;         // [N] chunks the ray evaluated (written when it leaves)
+  float* part;         // [N][5][32] lane partials C0, C1, C2, Dist, acc of composite_chunk
+};
+constexpr int FRAME_MAX_ROUNDS = 32;   // S <= 1024
+
+// workspace row of tile row `row` of a frame tile: sample i = 32 k + row % 32 of ray list[4 tile + row / 32].  Ray-chunks past the end of
+// the list repeat its last ray and rows past the ray's last sample evaluate that sample; frame_step ignores both.
+__device__ __forceinline__ size_t frame_sample(const nnb_render_args& a, const FramePtrs& f, int tile, int row, int n_live) {
+  const int slot = min(4 * tile + row / 32, n_live - 1);
+  const int n = f.list ? f.list[slot] : slot;
+  return (size_t)n * a.S + min(32 * f.k + row % 32, a.S - 1);
+}
+
+// Back end of a frame tile, one warp per ray-chunk: composite_fwd's chunk step on the chunk's (r, g, b, a) rows (s_rows, one float4 per
+// row), continued from the ray's carry and lane partials of the rounds before.  The ray leaves when its carry is below t_min or it has no
+// chunk left; otherwise it is appended to the next round's list.
+__device__ __forceinline__ void frame_step(const nnb_render_args& a, const FramePtrs& f, int slot, int n_live, const unsigned char* s_rows,
+                                           int lane) {
+  if (slot >= n_live) return;
+  const int n = f.list ? f.list[slot] : slot;
+  const int i = 32 * f.k + lane;
+  const bool valid = i < a.S;
+  float4 me = make_float4(0.f, 0.f, 0.f, 0.f);
+  float z = 0.f, alpha = 0.f;
+  if (valid) {
+    me = *reinterpret_cast<const float4*>(s_rows + lane * 16);
+    z = sample_z(a, n, i);
+    alpha = composite_alpha(a, i, me.w, z, [&] { return sample_z(a, n, i + 1); });
+  }
+  float* part = f.part + (size_t)n * 160 + lane;
+  float carry = 1.f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dist = 0.f, acc = 0.f;
+  if (f.k > 0) { carry = f.carry[n]; C0 = part[0]; C1 = part[32]; C2 = part[64]; Dist = part[96]; acc = part[128]; }
+  composite_chunk(alpha, valid, me.x, me.y, me.z, z, lane, carry, C0, C1, C2, Dist, acc);
+  part[0] = C0; part[32] = C1; part[64] = C2; part[96] = Dist; part[128] = acc;
+  if (lane == 0) {
+    f.carry[n] = carry;
+    if (carry < f.t_min || 32 * (f.k + 1) >= a.S) f.chunks[n] = f.k + 1;
+    else f.next_list[atomicAdd(f.next_count, 1)] = n;
+  }
+}
+
 // MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
 // out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is stashed and recs is not written.  M = a.N there, so point indices
 // are 32-bit.  FWD_VJP (tc_points_vjp_fwd, nnb_field_vjp): FWD_POINTS that also writes recs [Mpad] and the ReLU gate bits st.gates of
@@ -260,16 +311,26 @@ __device__ __forceinline__ void march_scan(const MarchPtrs& q, int ray, const fl
 //   warpgroup, whose barrier at the top of the tile loop orders the update before the next pass reads it.
 // DEVN (FWD_POINTS / FWD_VJP of nnb_geometry_frame): M = *q.count points, read when the kernel starts like FWD_SECANT's count; the
 // launch is sized for the largest count and a CTA without a tile leaves at once.
-enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4 };
+// FWD_FRAME (tc_frame): FWD_RAYS on the rows frame_sample gives (M = N S), with ray-chunks of 32 rows in place of whole rays in the per-ray
+// bias; nothing is stashed.  The colour head puts each row's (r, g, b, a) in this warpgroup's rows of the E operand (last read by layer
+// 4) and frame_step composites them.  n_tiles is read from *fr.count (ray-chunks, 4 per tile) when the kernel starts, as in FWD_MARCH.
+enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
-                                            int stash) {
+                                            int stash, const FramePtrs& fr = FramePtrs{}) {
   using T = Tc<D>;
-  constexpr bool PTS = MODE != FWD_RAYS, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP;
+  constexpr bool FRAME = MODE == FWD_FRAME;
+  constexpr bool PTS = MODE != FWD_RAYS && !FRAME, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
   static_assert(!DEVN || XPTS, "a device count of explicit points");
-  if constexpr (PTS) stash = 0;
+  if constexpr (PTS || FRAME) stash = 0;
+  int n_live = 0;   // FWD_FRAME: ray-chunks of this round
+  if constexpr (FRAME) {
+    n_live = fr.count ? *fr.count : a.N;
+    n_tiles = (n_live + 3) / 4;
+    if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
+  }
   const bool gates = VJP || stash;   // the ReLU gate bits are stored
   if constexpr (MARCH || DEVN) {
     if (q.count) {
@@ -356,12 +417,14 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
     // sample index of this warpgroup's first row inside its ray: row rl reads the bias of the block's ray (ray_off() + rl) / S.  Computed
     // where it is used, not held across the MMAs.
     auto ray_off = [&]() { return (int)((mt + (size_t)wg * 64) % (size_t)a.S); };
-    wg_sync();   // the previous tile's epilogue is done with the per-ray bias buffer
+    // rows per ray of the per-ray bias: a frame tile's ray-chunks take the place of rays
+    auto ray_len = [&]() { return FRAME ? 32 : a.S; };
+    wg_sync();   // the previous tile's epilogue (a frame tile: its frame_step) is done with the per-ray bias buffer and E
     {
-      const int off0 = PTS ? 0 : ray_off();
+      const int off0 = PTS || FRAME ? 0 : ray_off();
       // ---- prologue: thread (row rl, part) writes encoding columns [32 part, 32 part + 32) of its row ----
       const int rl = tl & 63, part = tl >> 6, row = wg * 64 + rl;
-      const size_t m = mt + row;
+      const size_t m = FRAME ? frame_sample(a, fr, tile, row, n_live) : mt + row;
       Ray ray; float z, p[3];
       if constexpr (MODE == FWD_MARCH) {
         const int ray = q.list ? q.list[tile] : tile;
@@ -414,8 +477,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
           for (int k4 = 0; k4 < 8; ++k4)
             __stcs(reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4), make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]));
         }
-        if (rl == 0 || (off0 + rl) % a.S == 0) {   // the block's first row and every row that starts a ray publish its direction encoding
-          const int r = (off0 + rl) / a.S;
+        if (rl == 0 || (off0 + rl) % ray_len() == 0) {   // the block's first row and every row that starts a ray publish its direction encoding
+          const int r = (off0 + rl) / ray_len();
 #pragma unroll
           for (int k = 0; k < 32; ++k) rayb[RAYB_DE + r * 32 + k] = de[k];
         }
@@ -423,7 +486,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
       fence_async_smem();
       wg_sync();
       const float* w = a.weights;
-      const int n_rays = PTS ? 0 : (off0 + 63) / a.S + 1;
+      const int n_rays = PTS ? 0 : (off0 + 63) / ray_len() + 1;
       for (int r = 0; r < n_rays; ++r) {   // thread tl = output column of the rgb hidden layer
         if (DR < 128 && tl >= DR) break;
         float b = __ldg(w + nnb::B_RGBH(D) + tl);
@@ -516,14 +579,14 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         // rgb hidden layer (D/2 columns) -> colour head + per-sample record
         float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
         uint32_t gw[D / 128 > 0 ? D / 128 : 1] = {};
-        const int off0 = PTS ? 0 : ray_off();
+        const int off0 = PTS || FRAME ? 0 : ray_off();
 #pragma unroll
         for (int j = 0; j < DR / 8; ++j) {
           const int col = j * 8 + c0;
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
             const int row = r0 + 8 * r;
-            const float* rb = PTS ? rayb : rayb + ((off0 + row - wg * 64) / a.S) * DR;   // points mode: b_rgbh
+            const float* rb = PTS ? rayb : rayb + ((off0 + row - wg * 64) / ray_len()) * DR;   // points mode: b_rgbh
             const float v0 = fmaxf(acc[4 * j + 2 * r] + rb[col], 0.f), v1 = fmaxf(acc[4 * j + 2 * r + 1] + rb[col + 1], 0.f);
 #pragma unroll
             for (int c = 0; c < 3; ++c)
@@ -552,6 +615,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             } else if constexpr (PTS) {
               const uint32_t mp = computed_here(tile * (uint32_t)TILE + r0 + 8 * r);
               if (mp < (uint32_t)M) out[mp] = make_float4(rec.r, rec.g, rec.b, rec.a);
+            } else if constexpr (FRAME) {   // E row r0 + 8 r, k-octet 0: this warpgroup's rows of E
+              *reinterpret_cast<float4*>(smem + SM_EHI + (r0 + 8 * r) * 16) = make_float4(rec.r, rec.g, rec.b, rec.a);
             } else {
               rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
               rec.pad0 = 0.f; rec.pad1 = 0.f;
@@ -600,6 +665,13 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         asm volatile("bar.sync 3, 256;" ::: "memory");
       }
     }
+    if constexpr (FRAME) {
+      // the warpgroup's 64 rows (its two ray-chunks) are in E before its first two warps composite them; the barrier at the top of
+      // the next tile orders their reads before the prologue writes E again
+      static_assert(TILE * 16 <= 2048, "a frame tile's (r, g, b, a) rows fit k-octet 0 of E");
+      wg_sync();
+      if ((warp & 3) < 2) frame_step(a, fr, 4 * tile + 2 * wg + (warp & 3), n_live, smem + SM_EHI + (wg * 64 + 32 * (warp & 3)) * 16, lane);
+    }
   }
 }
 
@@ -635,6 +707,26 @@ template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_secant(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                           const __grid_constant__ MarchPtrs q) {
   tc_fwd_body<D, FWD_SECANT>(a, wimg, nullptr, nullptr, TcStash{}, q, 0, 0, 0);
+}
+
+// one round of nnb_render_frame: chunk f.k of every ray of f.list (of every ray when f.list is NULL)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_frame(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                         const __grid_constant__ FramePtrs f) {
+  tc_fwd_body<D, FWD_FRAME>(a, wimg, nullptr, nullptr, TcStash{}, MarchPtrs{}, (size_t)a.N * a.S, 0, 0, f);
+}
+
+// one warp per ray after the last round: composite_fwd's tail on the ray's lane partials, n_eval and t_final
+__global__ void frame_finish(nnb_render_args a, const __grid_constant__ FramePtrs f, int* __restrict__ n_eval, float* __restrict__ t_final) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  Ray ray; setup_ray(a, n, ray);
+  const float* part = f.part + (size_t)n * 160 + lane;
+  composite_tail(a, n, ray, part[0], part[32], part[64], part[96], part[128], lane);
+  if (lane == 0) {
+    if (n_eval) n_eval[n] = min(32 * f.chunks[n], a.S);
+    if (t_final) t_final[n] = f.carry[n];
+  }
 }
 
 // depth (and the optional first / bracket) of every ray from the state the march and the secant passes left
@@ -1743,6 +1835,59 @@ cudaError_t tc_geometry_frame_dim(const nnb_geometry_args& g, cudaStream_t st) {
   return cudaGetLastError();
 }
 
+// Workspace of nnb_render_frame, every section 256-byte aligned: counters [FRAME_MAX_ROUNDS + 1] (k >= 1: rays of round k) | carry,
+// chunks [N] | lane partials [N][5][32] | the two ray lists that alternate between rounds [N] | the forward weight image
+struct FrameWs { size_t carry, chunks, part, list[2], img, total; };
+template <int D> FrameWs frame_layout(int N) {
+  FrameWs w{};
+  size_t off = align_up((size_t)(FRAME_MAX_ROUNDS + 1) * 4, 256);
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  const size_t n = (size_t)N;
+  w.carry = take(n * 4); w.chunks = take(n * 4); w.part = take(n * 640); w.list[0] = take(n * 4); w.list[1] = take(n * 4);
+  w.img = take(Tc<D>::IMG_BYTES);
+  w.total = off;
+  return w;
+}
+
+// nnb_render_frame: weight image once, one tc_frame launch per 32-sample chunk (round k takes its rays from the list round k - 1 appended
+// to), frame_finish.  Every launch after the first sizes itself from a device counter; nothing is read back.
+template <int D>
+cudaError_t tc_render_frame_dim(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, cudaStream_t st) {
+  using T = Tc<D>;
+  cudaError_t e = upload_stage_table<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  const FrameWs w = frame_layout<D>(a.N);
+  char* base = static_cast<char*>(a.workspace);
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  int* counters = I(0);
+  e = cudaMemsetAsync(counters, 0, (FRAME_MAX_ROUNDS + 1) * 4, st);
+  if (e != cudaSuccess) return e;
+  unsigned char* img = reinterpret_cast<unsigned char*>(base + w.img);
+  tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);
+  FramePtrs f{};
+  f.t_min = t_min;
+  f.carry = reinterpret_cast<float*>(base + w.carry); f.chunks = I(w.chunks); f.part = reinterpret_cast<float*>(base + w.part);
+  const int rounds = (a.S + 31) / 32, tiles = (a.N + 3) / 4;
+  const int grid = tiles < n_sm ? tiles : n_sm;
+  for (int k = 0; k < rounds; ++k) {
+    f.k = k;
+    f.list = k > 0 ? I(w.list[k & 1]) : nullptr; f.count = k > 0 ? counters + k : nullptr;
+    f.next_list = I(w.list[(k + 1) & 1]); f.next_count = counters + k + 1;   // not written by the last round
+    tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f);
+  }
+  frame_finish<<<(a.N + 7) / 8, 256, 0, st>>>(a, f, n_eval, t_final);
+  return cudaGetLastError();
+}
+
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
 
 }  // namespace
@@ -1778,6 +1923,14 @@ size_t tc_field_vjp_workspace(int N, uint32_t flags, int D) {
 cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st) {
   return D == 128 ? tc_field_vjp_dim<128>(a, g_rgba, out_rgba, g_pts, g_dirs, st)
        : D == 64  ? tc_field_vjp_dim<64>(a, g_rgba, out_rgba, g_pts, g_dirs, st) : tc_field_vjp_dim<256>(a, g_rgba, out_rgba, g_pts, g_dirs, st);
+}
+
+size_t tc_render_frame_workspace(int N, int D) {
+  return D == 128 ? frame_layout<128>(N).total : (D == 64 ? frame_layout<64>(N).total : frame_layout<256>(N).total);
+}
+cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st) {
+  return D == 128 ? tc_render_frame_dim<128>(a, t_min, n_eval, t_final, st)
+       : D == 64  ? tc_render_frame_dim<64>(a, t_min, n_eval, t_final, st) : tc_render_frame_dim<256>(a, t_min, n_eval, t_final, st);
 }
 
 size_t tc_geometry_frame_workspace(int N, int n_steps, int D) {

@@ -6,6 +6,7 @@ import os
 import numpy as np
 import torch
 from .. import ops
+from .. import _lib as L
 
 
 class Extract_Images(object):
@@ -20,7 +21,8 @@ class Extract_Images(object):
 
     def render_frame(self, c2w, camera_mat, h, w, rows=None):
         """rgb (rows,w,3) and z-depth (rows,w) of one view; eval mode, no jitter, prior depth = 1
-        (extracting_images.py:52-77).  rows=(r0,r1) renders a row block (multi-GPU sharding of one frame)."""
+        (extracting_images.py:52-77).  rows=(r0,r1) renders a row block (multi-GPU sharding of one frame).  With
+        Renderer(frame_t_min=t) on the tensor-core engine the frame is one ops.render_frame call (nnb_render_frame) instead."""
         rend = self.renderer
         net = rend.model
         r0, r1 = (0, h) if rows is None else rows
@@ -28,12 +30,17 @@ class Extract_Images(object):
         ray_idx = torch.arange(r0 * w, r1 * w, device=dev, dtype=torch.int64)
         n = ray_idx.numel()
         ndc = rend.cfg['sample_option'] == 'ndc'
-        call = ops.RenderCall(net.flat_weights(), c2w.detach().reshape(4, 4).contiguous().float(),
-                              camera_mat.detach().reshape(4, 4).contiguous().float(), N=n, S=int(rend.cfg['num_points']),
-                              flags=ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=True),
-                              engine=rend.engine if rend.engine is not None else ops.default_engine(),
-                              near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
-                              ray_idx=ray_idx, depth_map=torch.ones(1, 1, device=dev), H=h, W=w, stash=False, hidden_dim=net.hidden_dim)
+        S = int(rend.cfg['num_points'])
+        engine = rend.engine if rend.engine is not None else ops.default_engine()
+        args = (net.flat_weights(), c2w.detach().reshape(4, 4).contiguous().float(), camera_mat.detach().reshape(4, 4).contiguous().float())
+        kw = dict(N=n, S=S, flags=ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=True), engine=engine,
+                  near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
+                  ray_idx=ray_idx, depth_map=torch.ones(1, 1, device=dev), H=h, W=w, stash=False, hidden_dim=net.hidden_dim)
+        t_min = getattr(rend, 'frame_t_min', None)
+        if t_min is not None and ops.pick_engine(engine, S) == L.ENGINE_TC:   # Renderer(frame_t_min=t): the fused frame renderer
+            rgb, depth_pred = ops.render_frame(*args, t_min=t_min, **kw)[:2]
+            return rgb.view(r1 - r0, w, 3), depth_pred.view(r1 - r0, w)
+        call = ops.RenderCall(*args, **kw)
         return call.rgb.view(r1 - r0, w, 3), call.depth_pred.view(r1 - r0, w)
 
     def render_geometry(self, c2w, camera_mat, scale_mat, h, w, it=0):

@@ -37,6 +37,15 @@ class Renderer(nn.Module):
         # computed per pixel), and Extract_Images.render_geometry / Trainer.render_visdata pass the whole frame in one call.  Its
         # frames differ from phong_renderer's in the last bits of the rays, so it is off by default.
         self.geometry_frame = kwargs.get("geometry_frame", False)
+        # frame_t_min: None keeps Extract_Images.render_frame (and so generate_images / Eval_Images.eval_images) on nnb_render_fwd.  A
+        # float t >= 0 renders those frames with ops.render_frame (nnb_render_frame: compositing fused into the tensor-core forward, a
+        # workspace that does not grow with the sample count); t = 0 gives the same bits, t > 0 stops a ray once its transmittance is
+        # below t (bounded error, see the header).  Tensor-core engine only: with the SIMT engine (an explicit engine, or fewer than 16
+        # samples per ray) the frame takes the nnb_render_fwd path as before.  Trainer.render_visdata does not use it.
+        t_min = kwargs.get("frame_t_min", None)
+        if t_min is not None and not float(t_min) >= 0.0:
+            raise ValueError("frame_t_min must be None or a float >= 0 (got %r)" % (t_min,))
+        self.frame_t_min = None if t_min is None else float(t_min)
 
     def to(self, device):
         model = super().to(device)

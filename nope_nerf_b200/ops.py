@@ -146,6 +146,47 @@ class RenderCall:
         self.release()
 
 
+def render_frame(weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None, depth_map=None, scale=None,
+                 shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256, t_min=0.0, want_stats=False):
+    """nnb_render_frame: the forward of RenderCall (stash=False) on the tensor-core engine with compositing fused into the field's
+    forward, in a workspace that does not grow with S.  t_min = 0 gives RenderCall's bits; t_min > 0 stops a ray after the first
+    32-sample chunk that leaves its transmittance below t_min (the error bound is in include/nope_nerf_b200.h).
+    Returns (rgb, depth_pred, depth_gt, mask), and (n_eval, t_final) after them with want_stats.  noise, want_z_alpha and stash are
+    RenderCall's arguments and are rejected here, as is an engine other than the tensor-core engine (no fall-back)."""
+    if noise is not None or want_z_alpha or stash:
+        raise ValueError("render_frame: noise, want_z_alpha and stash are not supported (inference without jitter)")
+    for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels),
+                   ("depth", depth), ("depth_map", depth_map)):
+        _need_cuda(t_, n_)
+    dev = weights.device
+    f = L.FrameArgs()
+    a = f.fwd
+    a.weights = L.ptr(weights); a.c2w = L.ptr(c2w); a.cam = L.ptr(cam)
+    a.ray_idx = L.ptr(ray_idx); a.pixels = L.ptr(pixels); a.depth = L.ptr(depth); a.depth_map = L.ptr(depth_map)
+    a.scale = L.ptr(scale); a.shift = L.ptr(shift)
+    a.N, a.S, a.H, a.W = N, S, H, W
+    if depth_map is not None:
+        a.h_d, a.w_d = depth_map.shape[-2], depth_map.shape[-1]
+    a.near_, a.far_ = float(near), float(far)
+    a.flags = flags; a.engine = L.ENGINE_TC if engine is None else engine; a.hidden_dim = int(hidden_dim)
+    rgb = torch.empty(N, 3, device=dev); depth_pred = torch.empty(N, device=dev)
+    depth_gt = torch.empty(N, device=dev); mask = torch.empty(N, dtype=torch.uint8, device=dev)
+    a.rgb = L.ptr(rgb); a.depth_pred = L.ptr(depth_pred); a.depth_gt = L.ptr(depth_gt); a.mask = L.ptr(mask)
+    n_eval = torch.empty(N, dtype=torch.int32, device=dev) if want_stats else None
+    t_final = torch.empty(N, device=dev) if want_stats else None
+    f.t_min = float(t_min); f.n_eval = L.ptr(n_eval); f.t_final = L.ptr(t_final)
+    nbytes = L.lib.nnb_render_frame_workspace_bytes(N, S, int(hidden_dim))
+    ws = _pool.take(nbytes, dev) if nbytes else None
+    a.workspace = L.ptr(ws); a.workspace_bytes = 0 if ws is None else ws.numel()
+    try:
+        L.check(L.lib.nnb_render_frame(C.byref(f), _stream()), "nnb_render_frame")
+    finally:
+        if ws is not None:
+            _pool.give(ws)
+    outs = (rgb, depth_pred, depth_gt, mask)
+    return outs + (n_eval, t_final) if want_stats else outs
+
+
 class _RenderFn(torch.autograd.Function):
     """autograd glue for the drop-in Renderer / nope_nerf modules.
     differentiable inputs: c2w (4,4), cam (4,4), depth (N,) | (scale, shift) and the 24 MLP parameters.
