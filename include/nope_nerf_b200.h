@@ -177,6 +177,43 @@ int nnb_field_hvp(const nnb_render_args* a, const float* u, float* g_pts, float*
  * N <= 0, an undefined flag bit or an unsupported width. */
 size_t nnb_field_vjp_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim);
 int nnb_field_vjp(const nnb_render_args* a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, void* stream);
+/* The whole first-order backward of OfficialStaticNerf.forward on explicit points, tensor-core engine: what nnb_field_fwd (NNB_STASH) +
+ * nnb_field_bwd compute on the exact engine, in one call that recomputes everything from a->pts, a->dirs and a->weights (nothing is
+ * carried over from an earlier forward, as in nnb_field_hvp).  It runs the points forward with the fp32 training stash, the data-gradient
+ * chain of nnb_field_vjp with the dY stash, and the weight-gradient stage of the render backward (nnb_render_bwd on NNB_ENGINE_TC) on
+ * that stash.  No version bump: the symbol marks the capability.
+ * Reads a->pts [N,3], a->dirs [N,3] or NULL (ones), N, weights, hidden_dim, flags (NNB_DIST_ALPHA | NNB_SOFTPLUS | NNB_RAW_DENSITY |
+ * NNB_OCC_ONLY), engine and the workspace;  g_rgba [N,4] is the cotangent on (r, g, b, a).
+ *   out_rgba [N,4] (optional): bit-identical to nnb_field_fwd on NNB_ENGINE_TC with the same flags.
+ *   g_pts [N,4], g_dirs [N,4] (optional): bit-identical to nnb_field_vjp with the same cotangent (xyz; w is 0; overwritten, rows < N).
+ *   g_weights [nnb_num_params(hidden_dim)] (optional, 4-byte aligned) is ACCUMULATED (+=) with d<g_rgba, out>/d weights, like
+ *   nnb_field_bwd; plain adds, so no other work may write it during the call.  NULL makes the call nnb_field_vjp (the stash is still
+ *   written).
+ * NNB_OCC_ONLY (infer_occ under autograd): the colour branch is neither evaluated nor differentiated; g_rgba[:, :3] is not read, g_dirs
+ * must be NULL, and the slots of fc_feature, rgb_layers.0 and fc_rgb in g_weights are not touched.
+ * Errors, with nothing launched (those of nnb_field_vjp): an engine other than NNB_ENGINE_TC (rc -4); an undefined flag bit (-7);
+ * NNB_STASH or NNB_HVP, or g_dirs with NNB_OCC_ONLY (-6); an unsupported width (-8); N < 0, a NULL pts / weights / g_rgba / g_pts, one of
+ * g_rgba, out_rgba, g_pts, g_dirs not 16-byte aligned or g_weights not 4-byte aligned (-3); a workspace smaller than
+ * nnb_field_grad_workspace_bytes(N, flags, hidden_dim) or not 256-byte aligned (-5).  N == 0 returns 0 and does nothing.
+ * Precision: the forward and the chain are those of nnb_field_fwd / nnb_field_vjp; the weight gradients are the render backward's (bf16
+ * hi | lo products of the fp32 stash, fp32 accumulation; the heads in fp32).  Measured against float64 evaluated with the ReLU gates this
+ * call's forward wrote (NVIDIA H100 80GB HBM3, every flag and width): every dW / db within 9.4e-5 of its tensor's maximum, g_pts within
+ * 2.3e-5 and g_dirs within 1.4e-5 from 128 points on (a call of a few points has a g_pts maximum set by those points: 2.2e-4 at N = 1).  The
+ * gate caveat of nnb_field_vjp holds: where a pre-activation lies within the forward's rounding of 0 this engine may gate a unit differently
+ * from float64 or from the exact engine, and the gradients differ there by that unit's contribution.  The fp16 caveat of nnb_field_fwd
+ * holds for the forward: a field whose activations are very small (below about 2^-3 the low half of an fp16 operand is subnormal, below
+ * about 6e-8 an operand vanishes) is evaluated, and so gated and differentiated, less accurately than on the exact engine.
+ * Determinism: every sum runs in a fixed order, so the same inputs give the same bits on every run; a point's out_rgba, g_pts and g_dirs
+ * depend on that point alone.  The rows of the last tile past N have a zero cotangent and add exactly 0 to every dW / db, whatever the
+ * workspace held before the call.
+ * Workspace, each section 256-byte aligned (Npad = N rounded up to 128, D = hidden_dim): make_layout's layout for nnb_render_bwd at
+ * N x 1 samples with NNB_STASH on NNB_ENGINE_TC (records, the fp32 activation and dY stash of Npad rows, the weight-gradient partials,
+ * the ReLU gate bits) | the forward weight image (its occupancy-only prefix with NNB_OCC_ONLY) | the transposed weight image (its trunk
+ * part with NNB_OCC_ONLY).  20 272 bytes per point at D = 256 (10 408 at 128, 5 476 at 64) plus a constant: 2 700 501 248 bytes (2.7 GB)
+ * for 131 072 points at D = 256.  nnb_field_grad_workspace_bytes is the source of truth; it returns 0 for N <= 0, an undefined flag bit
+ * or an unsupported width. */
+size_t nnb_field_grad_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim);
+int nnb_field_grad(const nnb_render_args* a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream);
 int nnb_render_bwd(const nnb_render_bwd_args* a, void* stream);
 
 /* Fused ray marching of the geometry view: what Renderer.ray_marching + Renderer.secant (model/rendering.py:274-418) do for N rays, in

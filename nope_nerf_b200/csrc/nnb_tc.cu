@@ -314,17 +314,22 @@ __device__ __forceinline__ void frame_step(const nnb_render_args& a, const Frame
 // FWD_FRAME (tc_frame): FWD_RAYS on the rows frame_sample gives (M = N S), with ray-chunks of 32 rows in place of whole rays in the per-ray
 // bias; nothing is stashed.  The colour head puts each row's (r, g, b, a) in this warpgroup's rows of the E operand (last read by layer
 // 4) and frame_step composites them.  n_tiles is read from *fr.count (ray-chunks, 4 per tile) when the kernel starts, as in FWD_MARCH.
-enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5 };
+// FWD_GRAD (tc_points_grad_fwd, nnb_field_grad): FWD_VJP that also writes the fp32 training stash st of every row of every tile (rows
+// past M hold the last point's values): h0..h7, feat, hr and enc as FWD_RAYS does, and denc per point (the direction encoding of
+// a.dirs[m], or of the ones), which is a per-row operand of rgb_layers.0 here.  With NNB_OCC_ONLY the colour part (feat, hr, denc) is not
+// written.
+enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5, FWD_GRAD = 6 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
                                             int stash, const FramePtrs& fr = FramePtrs{}) {
   using T = Tc<D>;
-  constexpr bool FRAME = MODE == FWD_FRAME;
-  constexpr bool PTS = MODE != FWD_RAYS && !FRAME, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP;
+  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD;
+  constexpr bool PTS = MODE != FWD_RAYS && !FRAME, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP || GRAD;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
   static_assert(!DEVN || XPTS, "a device count of explicit points");
-  if constexpr (PTS || FRAME) stash = 0;
+  if constexpr ((PTS && !GRAD) || FRAME) stash = 0;
+  if constexpr (GRAD) stash = 1;
   int n_live = 0;   // FWD_FRAME: ray-chunks of this round
   if constexpr (FRAME) {
     n_live = fr.count ? *fr.count : a.N;
@@ -570,6 +575,11 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             for (int kb = 0; kb < 4; ++kb) {
               if ((kb >> 1) != part) continue;   // static register indices
               split_store8(de + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
+              if constexpr (GRAD) {   // the per-point direction encoding of the stash (the weight gradient of rgb_layers.0's last 27 columns)
+                float* dp = st.denc + (mt + row) * 32 + kb * 8;
+                __stcs(reinterpret_cast<float4*>(dp), make_float4(de[kb * 8], de[kb * 8 + 1], de[kb * 8 + 2], de[kb * 8 + 3]));
+                __stcs(reinterpret_cast<float4*>(dp + 4), make_float4(de[kb * 8 + 4], de[kb * 8 + 5], de[kb * 8 + 6], de[kb * 8 + 7]));
+              }
             }
           }
         }
@@ -1012,14 +1022,16 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
 // one plain-launched wgrad_reduce then adds the splits of all 14 jobs.  Each job has its own region of the partial buffer, so the
 // grids never write the same floats, and no two jobs write the same dW / db element (the encoding slice of layer 4 and the
 // direction slice of rgb_layers.0 are at column offset D, enc[1] has no bias), so one reduce gives the same bits as one per grid.
-cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) {
+// occ (nnb_field_grad with NNB_OCC_ONLY): the colour jobs (fc_feature, rgb_layers.0, fc_rgb) are left out, so grid 2 is not launched, the
+// head grid runs the density head alone, and the colour parameters' gradients are not touched.  The kernels are those of the full stage.
+cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw, bool occ, cudaStream_t st) {
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
   const int D = L.D, DR = D / 2;
   WgJobT big[8], enc[2];
   int nb = 0;
   for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(D, l), gw + nnb::b_off(D, l), D, D, D, D, nnb::w_ld(D, l), 0, 0};
-  big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT(D), gw + nnb::B_FEAT(D), D, D, D, D, D, 0, 0};
+  if (!occ) big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT(D), gw + nnb::B_FEAT(D), D, D, D, D, D, 0, 0};
   const WgJobT rgb{F(L.dyr), F(L.feat), gw + nnb::W_RGBH(D), gw + nnb::B_RGBH(D), DR, DR, D, D, D + 27, 0, 0};
   enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(D, 0), gw + nnb::b_off(D, 0), D, D, 64, 63, 63, 0, 0};
   enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(D, 4) + D, nullptr, D, D, 64, 63, D + 63, 0, 0};
@@ -1037,31 +1049,36 @@ cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw,
   // D = 256) fits as well only where wpart_floats is larger: at D = 256 when M > 36 864 (16 (np + 8192) at the C2 size), at D = 64
   // always, at D = 128 never.  Where it does not fit, the encoding jobs run after the chained reduce, with their own reduce, from
   // offset 0.
-  const size_t trunk_f = wg_part_floats(big, nb, ms_big), big_f = trunk_f + wg_part_floats(&rgb, 1, ms_big);
-  const size_t head_f = small_jobs_part_floats(sm, 3, L.M);
+  const int nsm = occ ? 1 : 3;   // sm[0] is the density head
+  const size_t trunk_f = wg_part_floats(big, nb, ms_big), big_f = trunk_f + (occ ? 0 : wg_part_floats(&rgb, 1, ms_big));
+  const size_t head_f = small_jobs_part_floats(sm, nsm, L.M);
   const bool enc_chained = big_f + head_f + wg_part_floats(enc, 2, ms_enc) <= wpart_floats(L.M, D);
   RedJob R[9 + 2 + 3];
   cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
                 : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
                            : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, 0, R, false, st);
   if (e != cudaSuccess) return e;
-  e = launch_wgrad<64, true>(&rgb, 1, L.M, D, ms_big, part, trunk_f, R + nb, true, st);
-  if (e != cudaSuccess) return e;
-  int nr = nb + 1;
+  int nr = nb;
+  if (!occ) {
+    e = launch_wgrad<64, true>(&rgb, 1, L.M, D, ms_big, part, trunk_f, R + nb, true, st);
+    if (e != cudaSuccess) return e;
+    nr += 1;
+  }
   if (enc_chained) {   // encoding before heads: its CTAs need a whole SM each, and the small head CTAs would fragment the free SMs
     e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, big_f + head_f, R + nr, true, st);
     if (e != cudaSuccess) return e;
     nr += 2;
   }
-  e = launch_head_wgrad(sm, 3, L.M, D, part, big_f, R + nr, st);
+  e = launch_head_wgrad(sm, nsm, L.M, D, part, big_f, R + nr, st);
   if (e != cudaSuccess) return e;
-  nr += 3;
+  nr += nsm;
   e = launch_wgrad_reduce(R, nr, part, st);
   if (e != cudaSuccess || enc_chained) return e;
   e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, 0, R, false, st);   // the chained reduce has read the whole buffer
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, 2, part, st);
 }
+cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) { return tc_wgrad_jobs(a, L, gw, false, st); }
 
 // ---- data-gradient chain (the forward's skeleton run backwards) ---------------------------------------------------------------------
 // Per 128-sample tile, two consumer warpgroups (64 rows each) and a producer warpgroup streaming TRANSPOSED weight stages: stage =
@@ -1141,14 +1158,18 @@ __device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint
 // may be NULL), only rows < M are stored and nothing is stashed.  DG_POINTS_OCC is the chain of an occupancy-only forward: it starts at
 // g_h7 = g_s w_sigma (the colour prefix of the stage table is neither loaded nor issued) and reads only g_rgba[m].w.
 // DEVN (points modes, nnb_geometry_frame): M = *count points, read when the kernel starts (see tc_fwd_body's DEVN).
-enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2 };
+// DG_POINTS_GRAD / DG_POINTS_GRAD_OCC (tc_points_grad, nnb_field_grad): DG_POINTS / DG_POINTS_OCC that also write the dY stash of every
+// row of every tile, as DG_RAYS does with write_dy (rows >= M have a zero cotangent, so their dY are zeros); the occupancy-only chain
+// writes dy0..dy7 and dyc = (0, 0, 0, d/d density logit).
+enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
                                               int n_tiles, int write_dy, const int* count = nullptr) {
   using T = Tc<D>;
-  constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC;
-  static_assert(!DEVN || PTS, "a device count of explicit points");
-  if constexpr (PTS) write_dy = 0;
+  constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC;
+  constexpr bool GRAD = MODE == DG_POINTS_GRAD || MODE == DG_POINTS_GRAD_OCC;
+  static_assert(!DEVN || (PTS && !GRAD), "a device count of explicit points");
+  if constexpr (PTS) write_dy = GRAD ? 1 : 0;
   if constexpr (DEVN) {
     const int c = *count;
     M = (size_t)c;
@@ -1174,11 +1195,17 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
     s_small[i] = (i < 3 * DR) ? __ldg(a.weights + nnb::W_RGB(D) + i) : __ldg(a.weights + nnb::W_SIG(D) + (i - 3 * DR));
   __syncthreads();
   const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  // GRAD: each warpgroup forms the tile count again after its setmaxnreg instead of holding it across (which spilled it at D = 256)
+  auto cta_tiles = [&]() {
+    if constexpr (GRAD) return ((int)computed_here((uint32_t)n_tiles) - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    else return my_tiles;
+  };
   if (warp >= 8) {   // weight producer (see tc_field_fwd)
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (warp == 8 && lane == 0) {
       uint32_t slot = 0, phase = 0;
-      for (int t = 0; t < my_tiles; ++t)
+      const int n_my = cta_tiles();
+      for (int t = 0; t < n_my; ++t)
         for (int s = S0; s < S_END; ++s) {
           const uint32_t bytes = (uint32_t)stage_t<D>(s).nrows * 64u;
           mbar_wait(bar0 + 8u * (NST + slot), phase ^ 1u);
@@ -1241,7 +1268,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
       }
   };
 
-  for (int t = 0; t < my_tiles; ++t) {
+  const int n_my = cta_tiles();
+  for (int t = 0; t < n_my; ++t) {
     const int tile = blockIdx.x + t * gridDim.x;
     const size_t mt = (size_t)tile * TILE;
     load_gates<OCC ? D / 2 : D / 4>(P.gates + gate_bits_off(OCC ? 7 : 8, tile, threadIdx.x, Mpad, D), gm);
@@ -1251,6 +1279,7 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
       if constexpr (OCC) {
         const float gw = (m < M) ? reinterpret_cast<const float*>(P.gs + m)[3] : 0.f;
         gyc[tl * 4 + 3] = gw * density_act_grad(P.rec[m].s, a.flags);
+        if constexpr (GRAD) __stcs(P.dyc + m, make_float4(0.f, 0.f, 0.f, gyc[tl * 4 + 3]));
       } else {
         const float4 g = (m < M) ? P.gs[m] : make_float4(0.f, 0.f, 0.f, 0.f);
         const SampleRec rec = P.rec[m];
@@ -1264,7 +1293,7 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
     if constexpr (OCC) {   // g_h7 = (g_s w_sigma) * (h7 > 0)
 #pragma unroll
       for (int i = 0; i < D / 2; ++i) acc[i] = 0.f;
-      epiD(mt, true, nullptr, true);
+      epiD(mt, true, GRAD ? P.dy[7] : nullptr, true);
     } else {
       {   // g_yr = (g_yc W_rgb) * (hr > 0), in the accumulator-fragment mapping of the gate bits -> A operand (K = D/2) + dY stash
 #pragma unroll
@@ -1386,6 +1415,19 @@ template <int D, int MODE>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_points_vjp_n(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                                 const __grid_constant__ DgPtrs P, const int* __restrict__ count) {
   tc_dgrad_body<D, MODE, true>(a, wimg, P, 0, 0, 0, count);
+}
+// nnb_field_grad: the forward of explicit points with records, gate bits and the fp32 training stash (FWD_GRAD), then the chain with
+// the dY stash (DG_POINTS_GRAD[_OCC]); tc_wgrad_jobs follows on that stash
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_grad_fwd(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                   SampleRec* __restrict__ recs, float4* __restrict__ out,
+                                                                   const __grid_constant__ TcStash st, size_t M, int n_tiles) {
+  tc_fwd_body<D, FWD_GRAD>(a, wimg, recs, out, st, MarchPtrs{}, M, n_tiles, 1);
+}
+template <int D, int MODE>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_grad(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                               const __grid_constant__ DgPtrs P, size_t M, int n_tiles) {
+  tc_dgrad_body<D, MODE>(a, wimg, P, M, n_tiles, 1);
 }
 
 template <int D>
@@ -1692,6 +1734,73 @@ cudaError_t tc_field_vjp_dim(const nnb_render_args& a, const float* g_rgba, floa
   return cudaGetLastError();
 }
 
+// Workspace of nnb_field_grad, every section 256-byte aligned: make_layout(N, 1, NNB_STASH, NNB_ENGINE_TC, D) (records, the fp32 stash
+// and its dY half, the weight-gradient partials, the gate bits) | the forward weight image (the occupancy-only prefix when occ) | the
+// transposed weight image (its trunk part when occ), as in vjp_layout
+struct GradWs { WsLayout L; size_t img, img_t, total; };
+template <int D> GradWs grad_layout(int N, bool occ) {
+  using T = Tc<D>;
+  GradWs w{};
+  w.L = make_layout(N, 1, NNB_STASH, NNB_ENGINE_TC, D);
+  size_t off = w.L.total;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  w.img = take(occ ? (size_t)T::N_STAGES_OCC * T::STAGE_BYTES : T::IMG_PTS_BYTES);
+  w.img_t = take(occ ? T::IMG_T_BYTES - T::IMG_T_PREFIX_BYTES : T::IMG_T_BYTES);
+  w.total = off;
+  return w;
+}
+
+// nnb_field_grad: both weight images, the forward with the training stash, the chain with the dY stash, then (g_weights) the weight-
+// gradient stage on Mpad rows; the rows past N have dY = 0, so they add exactly 0 to every dW / db
+template <int D>
+cudaError_t tc_field_grad_dim(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, float* g_weights,
+                              cudaStream_t st) {
+  using T = Tc<D>;
+  const bool occ = (a.flags & NNB_OCC_ONLY) != 0;
+  cudaError_t e = upload_stage_table<D>();
+  if (e == cudaSuccess) e = upload_stage_table_t<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_points_grad_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_grad<D, DG_POINTS_GRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_grad<D, DG_POINTS_GRAD_OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  const GradWs w = grad_layout<D>(a.N, occ);
+  const WsLayout& L = w.L;
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  SampleRec* recs = reinterpret_cast<SampleRec*>(base + L.rec);
+  unsigned char* gates = reinterpret_cast<unsigned char*>(base + L.gates);
+  unsigned char *img = reinterpret_cast<unsigned char*>(base + w.img), *img_t = reinterpret_cast<unsigned char*>(base + w.img_t);
+  TcStash ts{};
+  for (int l = 0; l < 8; ++l) ts.h[l] = F(L.h[l]);
+  ts.feat = F(L.feat); ts.hr = F(L.hr); ts.enc = F(L.enc); ts.denc = F(L.denc); ts.gates = gates;
+  tc_prep_weights<D><<<occ ? T::N_STAGES_OCC : T::N_STAGES_PTS, 256, 0, st>>>(a.weights, img);
+  tc_prep_weights_t_from<D><<<T::dg_tile_stages(occ), 256, 0, st>>>(a.weights, img_t, T::dg_first_stage(occ));
+  const int n_tiles = (a.N + TILE - 1) / TILE;
+  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  tc_points_grad_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, reinterpret_cast<float4*>(out_rgba), ts, (size_t)a.N, n_tiles);
+  DgPtrs P{};
+  P.rec = recs; P.gates = gates;
+  P.gs = reinterpret_cast<const float4*>(g_rgba); P.gp = reinterpret_cast<float4*>(g_pts); P.gv = reinterpret_cast<float4*>(g_dirs);
+  P.dyc = reinterpret_cast<float4*>(base + L.dyc);
+  for (int l = 0; l < 8; ++l) P.dy[l] = F(L.dy[l]);
+  P.dfeat = F(L.dfeat); P.dyr = F(L.dyr);
+  if (occ) tc_points_grad<D, DG_POINTS_GRAD_OCC><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  else tc_points_grad<D, DG_POINTS_GRAD><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  e = cudaGetLastError();
+  if (e != cudaSuccess || !g_weights) return e;
+  WsLayout Lw = L;
+  Lw.M = L.Mpad;   // whole tiles: the stash rows past N are written, with zero dY
+  return tc_wgrad_jobs(a, Lw, g_weights, occ, st);
+}
+
 // ---- nnb_geometry_frame: the geometry view (Renderer.phong_renderer) of N pixels on the device ----------------------------------
 // Every product, sum, quotient and square root below is rounded on its own (no FMA contraction), in the order the header states.
 __device__ __forceinline__ float dot3_rn(const float* u, const float* v) {   // (u0 v0 + u1 v1) + u2 v2
@@ -1923,6 +2032,17 @@ size_t tc_field_vjp_workspace(int N, uint32_t flags, int D) {
 cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, int D, cudaStream_t st) {
   return D == 128 ? tc_field_vjp_dim<128>(a, g_rgba, out_rgba, g_pts, g_dirs, st)
        : D == 64  ? tc_field_vjp_dim<64>(a, g_rgba, out_rgba, g_pts, g_dirs, st) : tc_field_vjp_dim<256>(a, g_rgba, out_rgba, g_pts, g_dirs, st);
+}
+
+size_t tc_field_grad_workspace(int N, uint32_t flags, int D) {
+  const bool occ = (flags & NNB_OCC_ONLY) != 0;
+  return D == 128 ? grad_layout<128>(N, occ).total : (D == 64 ? grad_layout<64>(N, occ).total : grad_layout<256>(N, occ).total);
+}
+cudaError_t tc_field_grad(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, float* g_weights, int D,
+                          cudaStream_t st) {
+  return D == 128 ? tc_field_grad_dim<128>(a, g_rgba, out_rgba, g_pts, g_dirs, g_weights, st)
+       : D == 64  ? tc_field_grad_dim<64>(a, g_rgba, out_rgba, g_pts, g_dirs, g_weights, st)
+                  : tc_field_grad_dim<256>(a, g_rgba, out_rgba, g_pts, g_dirs, g_weights, st);
 }
 
 size_t tc_render_frame_workspace(int N, int D) {

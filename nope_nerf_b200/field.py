@@ -1,6 +1,7 @@
 """OfficialStaticNerf.forward on explicit points (reference: model/official_nerf.py:69-96) through nnb_field_fwd/bwd: used by direct
 callers of the field module and the geometry view; the nope_nerf render path never materialises points.  The exact-fp32 engine
-serves every call; a call that needs no gradient can ask for the tensor-core engine (field_query(engine='tc'))."""
+serves every call; a call that needs no gradient can ask for the tensor-core engine (field_query(engine='tc')), and a call that needs one
+can stay there too (field_query_grad(engine='tc', grad_engine='tc'), whose backward is nnb_field_grad)."""
 import ctypes as C
 import torch
 from . import _lib as L
@@ -146,6 +147,47 @@ def _field_tc(net, flags, p, d):
     return out
 
 
+class _FieldTcFn(torch.autograd.Function):
+    """A field query on the tensor-core engine under autograd (field_query_grad(engine='tc', grad_engine='tc')).
+    forward: nnb_field_fwd on tensor cores, so the outputs are the inference query's bits.  backward: nnb_field_grad, which recomputes the
+    forward from the points, directions and weights (only they are kept) and returns the gradients to p, ray_d and every parameter, with
+    NNB_OCC_ONLY when the caller uses the occupancy alone.  Differentiable once, like nnb_field_bwd's _FieldFn."""
+
+    @staticmethod
+    def forward(ctx, flags, net, flat, p, d, *params):
+        p_c = ops._f32c(p.detach()); d_c = None if d is None else ops._f32c(d.detach())
+        out = _field_tc(net, flags, p_c, d_c)
+        ctx.flags = flags; ctx.net = net; ctx.flat = flat; ctx.nparams = len(params); ctx.slices = net.param_slices
+        ctx.save_for_backward(p_c, d_c)
+        return out[:, :3], out[:, 3]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_rgb, g_a):
+        p_c, d_c = ctx.saved_tensors
+        net, flat, flags = ctx.net, ctx.flat, ctx.flags
+        M, dev = p_c.shape[0], p_c.device
+        occ = bool(flags & L.OCC_ONLY)
+        need_d = ctx.needs_input_grad[4] and not occ   # the occupancy does not depend on the view direction
+        need_w = any(ctx.needs_input_grad[5:])
+        g = torch.zeros(M, 4, device=dev)
+        if g_rgb is not None and not occ: g[:, :3] = g_rgb
+        if g_a is not None: g[:, 3] = g_a
+        g_p = torch.empty(M, 4, device=dev)
+        g_d = torch.empty(M, 4, device=dev) if need_d else None
+        g_w = torch.zeros(flat.numel(), device=dev) if need_w else None
+        a = L.RenderArgs()
+        a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = L.ptr(d_c)
+        a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_TC; a.hidden_dim = net.hidden_dim
+        ws = torch.empty(L.lib.nnb_field_grad_workspace_bytes(M, flags, net.hidden_dim), dtype=torch.uint8, device=dev)
+        a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+        L.check(L.lib.nnb_field_grad(C.byref(a), L.ptr(g), None, L.ptr(g_p), L.ptr(g_d), L.ptr(g_w), ops._stream()), "nnb_field_grad")
+        gp = [None] * ctx.nparams
+        if g_w is not None:
+            gp = [g_w[o:o + n].view(s) for (o, n, s) in ctx.slices]
+        return (None, None, None, g_p[:, :3] if ctx.needs_input_grad[3] else None, g_d[:, :3] if need_d else None) + tuple(gp)
+
+
 MARCH_BLOCK = 128   # steps one round of nnb_ray_march advances every ray that is still searching
 
 
@@ -234,16 +276,36 @@ def _engine_id(engine):
         raise ValueError("engine must be None, 'simt', 'tc', ENGINE_SIMT or ENGINE_TC (got %r)" % (engine,))
 
 
+def _grad_engine_id(engine, grad_engine):
+    """the engine of a call that needs a gradient: None (the exact engine, the default) or ENGINE_TC, which needs engine='tc'"""
+    g = _engine_id(grad_engine)
+    if g is None or g == L.ENGINE_SIMT:
+        return None
+    if _engine_id(engine) != L.ENGINE_TC:
+        raise ValueError("grad_engine='tc' needs engine='tc' (got engine=%r): a query and its gradient on different engines would use "
+                         "different ReLU gates" % (engine,))
+    return g
+
+
 def field_query(net, p, ray_d, raw_density=False, occ_only=False, engine=None):
+    """field_query_grad with grad_engine=None: a call that needs a gradient runs on the exact engine (see there)"""
+    return field_query_grad(net, p, ray_d, raw_density, occ_only, engine)
+
+
+def field_query_grad(net, p, ray_d, raw_density=False, occ_only=False, engine=None, grad_engine=None):
     """returns (rgb (..,3), a (..,1)) with a = alpha (or sigma when rendering.dist_alpha), like return_addocc=True;
     raw_density: a = the density logit (OfficialStaticNerf.infer_occ, official_nerf.py:60-67).
     engine: None or 'simt' = the exact-fp32 engine.  'tc' (or ENGINE_TC) = the tensor-core engine when the call needs no gradient
     (grad mode off, or neither p, ray_d nor a parameter of net requires grad); a call that needs one runs on the exact engine, which
     has the backward.  The engines agree to about 1e-6 of the output's maximum, not bit for bit.
+    grad_engine: the engine of a call that needs a gradient.  None or 'simt' = the exact engine (the rule above).  'tc' (or ENGINE_TC)
+    needs engine='tc' (ValueError otherwise): the call then runs on tensor cores under autograd, its outputs the bits of the inference
+    query and its backward nnb_field_grad, once differentiable, with gradients to p, ray_d and every parameter of net.
     occ_only: the caller uses a only.  On the tensor-core engine the colour branch is then skipped and rgb is zeros (a is bit-identical
-    to the full query's); the exact engine evaluates everything regardless.
+    to the full query's), in the backward too; the exact engine evaluates everything regardless.
     No point (M == 0) returns empty tensors without a library call."""
     ops._need_cuda(p, "p")
+    g_engine = None if grad_engine is None else _grad_engine_id(engine, grad_engine)
     shp = p.shape[:-1]
     flags = (L.DIST_ALPHA if net.dist_alpha else 0) | (L.SOFTPLUS if net.occ_activation == 'softplus' else 0) | (L.RAW_DENSITY if raw_density else 0)
     d = None if ray_d is None else ray_d.reshape(-1, 3)
@@ -254,5 +316,9 @@ def field_query(net, p, ray_d, raw_density=False, occ_only=False, engine=None):
         if not needs_grad(net, p, d):
             out = _field_tc(net, flags | (L.OCC_ONLY if occ_only else 0), p.reshape(-1, 3), d)
             return out[:, :3].reshape(*shp, 3), out[:, 3].reshape(*shp, 1)
+        if g_engine == L.ENGINE_TC:
+            rgb, a = _FieldTcFn.apply(flags | (L.OCC_ONLY if occ_only else 0), net, net.flat_weights(), p.reshape(-1, 3), d,
+                                      *list(net.parameters()))
+            return rgb.reshape(*shp, 3), a.reshape(*shp, 1)
     rgb, a = _FieldFn.apply(flags, net, net.flat_weights(), p.reshape(-1, 3), d, *list(net.parameters()))
     return rgb.reshape(*shp, 3), a.reshape(*shp, 1)

@@ -108,11 +108,12 @@ class OfficialStaticNerf(nn.Module):
         return g
 
     # ---- reference API -------------------------------------------------------------------
-    def infer_occ(self, p, engine=None):
+    def infer_occ(self, p, engine=None, grad_engine=None):
         """official_nerf.py:60-67: (trunk features, density logit).  The trunk features never leave the kernel here; callers in the
-        reference (gradient(), forward()) only use the logit, so the first element is None.  engine: see forward()."""
-        from ..field import field_query
-        _, s = field_query(self, p, None, raw_density=True, occ_only=True, engine=engine)
+        reference (gradient(), forward()) only use the logit, so the first element is None.  engine, grad_engine: see forward(); with
+        engine='tc', grad_engine='tc' a logit under autograd differentiates the occupancy alone on tensor cores."""
+        from ..field import field_query_grad
+        _, s = field_query_grad(self, p, None, raw_density=True, occ_only=True, engine=engine, grad_engine=grad_engine)
         return None, s
 
     def gradient(self, p, it, engine=None):
@@ -135,13 +136,15 @@ class OfficialStaticNerf(nn.Module):
         return -n.reshape(p.shape).unsqueeze(1)
 
     def forward(self, p, ray_d=None, only_occupancy=False, return_logits=False, return_addocc=False,
-                noise=False, it=100000, engine=None, **kwargs):
+                noise=False, it=100000, engine=None, grad_engine=None, **kwargs):
         """Field query on explicit points (official_nerf.py:69-96); `noise`, `it`, `return_logits`
         are accepted and ignored exactly like the reference.
         engine: None = the exact-fp32 engine; 'tc' = the tensor-core engine for a call that needs no gradient (a call that does runs
-        on the exact engine), skipping the colour branch when only_occupancy (field.field_query)."""
-        from ..field import field_query
-        rgb, a = field_query(self, p, ray_d, occ_only=only_occupancy, engine=engine)
+        on the exact engine), skipping the colour branch when only_occupancy (field.field_query_grad).
+        grad_engine: None = a call that needs a gradient runs on the exact engine; 'tc' (with engine='tc' only, ValueError otherwise) =
+        it runs on tensor cores too, with the tensor-core backward nnb_field_grad (gradients to p, ray_d and every parameter)."""
+        from ..field import field_query_grad
+        rgb, a = field_query_grad(self, p, ray_d, occ_only=only_occupancy, engine=engine, grad_engine=grad_engine)
         if only_occupancy:
             return a
         if ray_d is not None:
