@@ -214,6 +214,39 @@ int nnb_field_vjp(const nnb_render_args* a, const float* g_rgba, float* out_rgba
  * or an unsupported width. */
 size_t nnb_field_grad_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim);
 int nnb_field_grad(const nnb_render_args* a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream);
+/* The second-order field backward of nnb_field_hvp on the tensor-core engine: for the raw density logit s and a cotangent u on the
+ * normals n = d s / d p, the gradients of s' = sum_m u[m] . n[m] to the points and the weights, recomputed from a->pts and a->weights in
+ * one call.  It runs the occupancy-only forward of nnb_field_vjp (records, ReLU gate bits), its data-gradient chain for a cotangent 1 on
+ * the logit with the dY stash and the point term, the tangent chain e' = J_enc(p) u, h'_l = [h_l > 0] (W_l x'_{l-1}) (no bias, gated with
+ * the forward's bits), and the weight-gradient stage of nnb_field_grad on (dY, tangent) without bias jobs.  nnb_field_hvp is unchanged
+ * and stays on the exact-fp32 engine.  No version bump: the symbol marks the capability.
+ * Reads a->pts [N,3], N, weights, hidden_dim, flags, engine and the workspace (a->dirs is not read: the logit does not depend on the view
+ * direction); the call always differentiates the raw logit of the occupancy-only query (NNB_RAW_DENSITY | NNB_OCC_ONLY are implied, and
+ * NNB_DIST_ALPHA / NNB_SOFTPLUS do not change it).  u [N,4]: the cotangent on n (xyz; w is not read).
+ *   g_pts [N,4] (optional): d s' / d p, only the encoding's diagonal second-derivative term (the ReLU masks are piecewise constant); xyz,
+ *   w is 0; overwritten, rows < N.
+ *   g_weights [nnb_num_params(hidden_dim)] (optional, 4-byte aligned) is ACCUMULATED (+=) with d s' / d weights, like nnb_field_hvp: only
+ *   the slots of the trunk weights (layers 0..7) and of fc_density.weight are written; every bias slot and every colour slot is left
+ *   untouched (s' has no bias term and no colour term).  Plain adds, so no other work may write it during the call.
+ * Errors, with nothing launched, in nnb_field_grad's order: a NULL a (-3); an engine other than NNB_ENGINE_TC (-4); an undefined flag
+ * bit (-7); NNB_STASH or NNB_HVP (-6); an unsupported width (-8); N < 0 (-3); then N == 0 returns 0 and does nothing; a NULL pts / weights
+ * / u, or both g_pts and g_weights NULL, u or g_pts not 16-byte aligned, or g_weights not 4-byte aligned (-3); a workspace smaller than
+ * nnb_field_hvp_tc_workspace_bytes(N, flags, hidden_dim) or not 256-byte aligned (-5).
+ * Precision: the forward and its gates are those of nnb_field_vjp (occupancy-only); the chain is nnb_field_vjp's (bf16 hi | lo operands);
+ * the tangent chain runs on bf16 hi | lo operands of the fp32 tangents and weights with fp32 accumulation (the fp16 hi | lo split of the
+ * forward is inaccurate below about 2^-3, and tangents span the range of gradients: e' reaches 2^9 |u|); the weight gradients are
+ * nnb_field_grad's.  Measured against float64 evaluated with the ReLU gates this call's forward wrote (NVIDIA H100 80GB HBM3, every
+ * width): every dW within 7.9e-5 of its tensor's maximum, g_pts within 1.7e-5 at every size (DESIGN.md §4).  The gate caveat of
+ * nnb_field_vjp holds: where a pre-activation lies within the forward's rounding of 0 this engine may gate a unit differently from float64
+ * or from the exact engine.
+ * Determinism: every sum runs in a fixed order, so the same inputs give the same bits on every run; a point's g_pts depends on that point
+ * alone.  The rows of the last tile past N have u = 0 and a zero cotangent, so they add exactly 0 to every dW whatever the workspace held.
+ * Workspace, each section 256-byte aligned (Npad = N rounded up to 128, D = hidden_dim): nnb_field_grad's occupancy-only layout (records,
+ * the fp32 stash, whose h0..h7 / enc rows hold the tangent h'0..h'7 / e' here, the dY stash, the weight-gradient partials, the gate bits,
+ * the occupancy-only forward image and the trunk part of the transposed image) | the bf16 image of the occupancy-only forward stages.
+ * nnb_field_hvp_tc_workspace_bytes is the source of truth; it returns 0 for N <= 0, an undefined flag bit or an unsupported width. */
+size_t nnb_field_hvp_tc_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim);
+int nnb_field_hvp_tc(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream);
 int nnb_render_bwd(const nnb_render_bwd_args* a, void* stream);
 
 /* Fused ray marching of the geometry view: what Renderer.ray_marching + Renderer.secant (model/rendering.py:274-418) do for N rays, in

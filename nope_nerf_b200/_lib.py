@@ -105,6 +105,9 @@ def _load():
     lib.nnb_field_grad.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, _f, _f, C.c_void_p]
     lib.nnb_field_grad_workspace_bytes.restype = C.c_size_t
     lib.nnb_field_grad_workspace_bytes.argtypes = [C.c_int32, C.c_uint32, C.c_int32]
+    lib.nnb_field_hvp_tc.argtypes = [C.POINTER(RenderArgs), _f, _f, _f, C.c_void_p]
+    lib.nnb_field_hvp_tc_workspace_bytes.restype = C.c_size_t
+    lib.nnb_field_hvp_tc_workspace_bytes.argtypes = [C.c_int32, C.c_uint32, C.c_int32]
     lib.nnb_geometry_frame.argtypes = [C.POINTER(GeometryArgs), C.c_void_p]
     lib.nnb_geometry_frame_workspace_bytes.restype = C.c_size_t
     lib.nnb_geometry_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]

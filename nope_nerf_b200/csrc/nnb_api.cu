@@ -26,6 +26,8 @@ cudaError_t tc_field_vjp(const nnb_render_args& a, const float* g_rgba, float* o
 size_t tc_field_grad_workspace(int N, uint32_t flags, int D);
 cudaError_t tc_field_grad(const nnb_render_args& a, const float* g_rgba, float* out_rgba, float* g_pts, float* g_dirs, float* g_weights, int D,
                           cudaStream_t st);
+size_t tc_field_hvp_workspace(int N, int D);
+cudaError_t tc_field_hvp(const nnb_render_args& a, const float* u, float* g_pts, float* g_weights, int D, cudaStream_t st);
 size_t tc_geometry_frame_workspace(int N, int n_steps, int D);
 size_t tc_render_frame_workspace(int N, int D);
 cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st);
@@ -328,6 +330,40 @@ int nnb_field_grad(const nnb_render_args* a, const float* g_rgba, float* out_rgb
   nnb_render_args b = *a; b.S = 1;
   cudaError_t e = tc_field_grad(b, g_rgba, out_rgba, g_pts, g_dirs, g_weights, hidden_of(a->hidden_dim), (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_grad");
+#endif
+}
+size_t nnb_field_hvp_tc_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && nnb::dim_supported(D) && !(flags & ~KNOWN_FLAGS)) return tc_field_hvp_workspace(N, D);
+#endif
+  return 0;
+}
+// the checks of nnb_field_grad in its order; u takes g_rgba's place and g_pts is optional when g_weights is given
+int nnb_field_hvp_tc(const nnb_render_args* a, const float* u, float* g_pts, float* g_weights, void* stream) {
+  if (!a) return fail(-3, "nnb_field_hvp_tc: null args");
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_field_hvp_tc: engine %d has no tensor-core second-order backward (NNB_ENGINE_TC only; the exact-fp32 engine has "
+                "nnb_field_hvp)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_flags(a->flags)) return rc;
+  if (a->flags & (NNB_STASH | NNB_HVP))
+    return fail(-6, "nnb_field_hvp_tc: NNB_STASH and NNB_HVP are not accepted (the call keeps its own stash; they size nnb_field_hvp's)");
+  if (int rc = check_dim(a)) return rc;
+  if (a->N < 0) return fail(-3, "nnb_field_hvp_tc: N must not be negative (got %d)", a->N);
+  if (a->N == 0) return 0;
+  if (!a->pts || !a->weights || !u || (!g_pts && !g_weights))
+    return fail(-3, "nnb_field_hvp_tc: need pts, weights, u and at least one of g_pts, g_weights");
+  if (misaligned16(u) || misaligned16(g_pts)) return fail(-3, "nnb_field_hvp_tc: u and g_pts must be 16-byte aligned [N][4] arrays");
+  if ((reinterpret_cast<uintptr_t>(g_weights) & 3) != 0) return fail(-3, "nnb_field_hvp_tc: g_weights must be 4-byte aligned");
+  const size_t need = nnb_field_hvp_tc_workspace_bytes(a->N, a->flags, a->hidden_dim);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  nnb_render_args b = *a; b.S = 1; b.dirs = nullptr; b.flags |= NNB_RAW_DENSITY | NNB_OCC_ONLY;
+  cudaError_t e = tc_field_hvp(b, u, g_pts, g_weights, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_hvp_tc");
 #endif
 }
 size_t nnb_geometry_frame_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim) {

@@ -132,10 +132,10 @@ template <int D> __device__ __forceinline__ const StageDescT& stage_t(int s) {
 using namespace tcu;
 
 // ---- weight imaging: fp32 (out,in) matrices -> per-stage shared-memory images (hi | lo) --------
-template <int D>
-__global__ void tc_prep_weights(const float* __restrict__ w, unsigned char* __restrict__ img) {
+template <int D, bool BF16>
+__device__ __forceinline__ void prep_stage(const float* __restrict__ w, unsigned char* __restrict__ img) {
   const StageDesc sd = stage<D>(blockIdx.x);
-  unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] fp16
+  unsigned char* hi = img + sd.img_off;       // [k-octet 0..1][nrows][8] fp16 (bf16)
   unsigned char* lo = hi + sd.nrows * 32;
   for (int idx = threadIdx.x; idx < sd.nrows * 2; idx += blockDim.x) {
     const int n = idx % sd.nrows, ko = idx / sd.nrows;
@@ -145,9 +145,15 @@ __global__ void tc_prep_weights(const float* __restrict__ w, unsigned char* __re
       const int k = sd.kcol0 + ko * 8 + j;
       v[j] = (k < sd.kvalid) ? __ldg(w + sd.w_off + (size_t)n * sd.ldw + k) : 0.f;
     }
-    split_store8(v, hi + ko * sd.nrows * 16 + n * 16, lo + ko * sd.nrows * 16 + n * 16);
+    if constexpr (BF16) split_store8_bf16(v, hi + ko * sd.nrows * 16 + n * 16, lo + ko * sd.nrows * 16 + n * 16);
+    else split_store8(v, hi + ko * sd.nrows * 16 + n * 16, lo + ko * sd.nrows * 16 + n * 16);
   }
 }
+template <int D>
+__global__ void tc_prep_weights(const float* __restrict__ w, unsigned char* __restrict__ img) { prep_stage<D, false>(w, img); }
+// the same stages as bf16 hi | lo (the tangent chain of nnb_field_hvp_tc, whose operands span the range of gradients)
+template <int D>
+__global__ void tc_prep_weights_bf16(const float* __restrict__ w, unsigned char* __restrict__ img) { prep_stage<D, true>(w, img); }
 
 // fp32 [sample][feature] stash, layout of nnb_simt.cu, and the ReLU gate bits of h0..h7 and hr (gate_bits_off).  This and DgPtrs are
 // __grid_constant__ kernel parameters: indexed by layer in parameter space, not copied to local memory (which would also leave the
@@ -172,6 +178,13 @@ template <int NB> __device__ __forceinline__ void load_gates(const unsigned char
 // shifts the gate bit of v (a ReLU output, so v >= 0 or -0) in at the bottom of w: w = (w << 1) | (v > 0).  0 - v is negative exactly
 // when v > 0 (0 - (-0) = +0), so the bit is its sign: one FADD and one funnel shift per bit.
 __device__ __forceinline__ uint32_t push_gate(uint32_t w, float v) { return __funnelshift_l(__float_as_uint(0.f - v), w, 1); }
+
+__device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 hh = __floats2bfloat162_rn(a, b);
+  hi = *reinterpret_cast<uint32_t*>(&hh);
+  __nv_bfloat162 ll = __floats2bfloat162_rn(a - __uint_as_float(hi << 16), b - __uint_as_float(hi & 0xffff0000u));
+  lo = *reinterpret_cast<uint32_t*>(&ll);
+}
 
 __device__ __forceinline__ void row_geometry_tc(const nnb_render_args& a, size_t m, size_t M, Ray& ray, float& z, float p[3]) {
   const size_t mm = m < M ? m : M - 1;
@@ -318,25 +331,31 @@ __device__ __forceinline__ void frame_step(const nnb_render_args& a, const Frame
 // past M hold the last point's values): h0..h7, feat, hr and enc as FWD_RAYS does, and denc per point (the direction encoding of
 // a.dirs[m], or of the ones), which is a per-row operand of rgb_layers.0 here.  With NNB_OCC_ONLY the colour part (feat, hr, denc) is not
 // written.
-enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5, FWD_GRAD = 6 };
+// FWD_TANGENT (tc_points_tangent, nnb_field_hvp_tc): the tangent chain of the density logit along u on the trunk of an occupancy-only
+// FWD_VJP forward: the prologue puts e' = J_enc(p) u in E (u = (*out)[m], read, never written; rows past M have u = 0), every layer is
+// the bias-free z'_l = W_l x'_{l-1} ([h'3 | e'] into layer 4), gated with the forward's bits st.gates (read as tc_dgrad reads them)
+// instead of a ReLU, and the tile ends after layer 7.  Operands are bf16 hi | lo (wimg is the bf16 image of the occupancy-only stages),
+// because tangents span the range of gradients.  e' and h'0..h'7 of every row of every tile go to st.enc / st.h with the stash's
+// streaming stores; nothing else is written.
+enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5, FWD_GRAD = 6, FWD_TANGENT = 7 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
                                             int stash, const FramePtrs& fr = FramePtrs{}) {
   using T = Tc<D>;
-  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD;
+  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD, TAN = MODE == FWD_TANGENT;
   constexpr bool PTS = MODE != FWD_RAYS && !FRAME, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP || GRAD;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
   static_assert(!DEVN || XPTS, "a device count of explicit points");
-  if constexpr ((PTS && !GRAD) || FRAME) stash = 0;
-  if constexpr (GRAD) stash = 1;
+  if constexpr ((PTS && !GRAD && !TAN) || FRAME) stash = 0;
+  if constexpr (GRAD || TAN) stash = 1;
   int n_live = 0;   // FWD_FRAME: ray-chunks of this round
   if constexpr (FRAME) {
     n_live = fr.count ? *fr.count : a.N;
     n_tiles = (n_live + 3) / 4;
     if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
   }
-  const bool gates = VJP || stash;   // the ReLU gate bits are stored
+  const bool gates = !TAN && (VJP || stash);   // the ReLU gate bits are stored
   if constexpr (MARCH || DEVN) {
     if (q.count) {
       const int c = *q.count;
@@ -345,7 +364,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
     }
     if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
   }
-  const bool occ = MARCH || (PTS && (a.flags & NNB_OCC_ONLY));
+  const bool occ = MARCH || TAN || (PTS && (a.flags & NNB_OCC_ONLY));
   constexpr int SM_AHI = T::SM_AHI, SM_ALO = T::SM_ALO, SM_EHI = T::SM_EHI, SM_ELO = T::SM_ELO, SM_W = T::SM_W, SM_BIAS = T::SM_BIAS;
   constexpr int SM_RAYB = T::SM_RAYB, SM_BAR = T::SM_BAR, BIAS_FLOATS = T::BIAS_FLOATS, RAYB_FLOATS = T::RAYB_FLOATS;
   constexpr int STAGE_BYTES = T::STAGE_BYTES, N_STAGES = T::N_STAGES, DR = D / 2;
@@ -453,19 +472,37 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         row_geometry_tc(a, m, M, ray, z, p);
       }
       float ee[64];
+      if constexpr (TAN) {   // e' = J_enc(p) u, rounded as simt_field_tangent rounds it
+        const uint32_t mp = tile * (uint32_t)TILE + row;
+        const float4 uv = mp < (uint32_t)M ? out[mp] : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float u[3] = {uv.x, uv.y, uv.z};
 #pragma unroll
-      for (int c = 0; c < 3; ++c) ee[c] = p[c];
+        for (int c = 0; c < 3; ++c) ee[c] = u[c];
 #pragma unroll
-      for (int l = 0; l < 10; ++l) {
-        const float f = (float)(1 << l);
+        for (int l = 0; l < 10; ++l) {
+          const float f = (float)(1 << l);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) { float sn, cs; sincosf(__fmul_rn(f, p[c]), &sn, &cs); ee[3 + 6 * l + c] = sn; ee[6 + 6 * l + c] = cs; }
+          for (int c = 0; c < 3; ++c) {
+            float sn, cs; sincosf(__fmul_rn(f, p[c]), &sn, &cs);
+            ee[3 + 6 * l + c] = __fmul_rn(__fmul_rn(f, cs), u[c]); ee[6 + 6 * l + c] = -__fmul_rn(__fmul_rn(f, sn), u[c]);
+          }
+        }
+      } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) ee[c] = p[c];
+#pragma unroll
+        for (int l = 0; l < 10; ++l) {
+          const float f = (float)(1 << l);
+#pragma unroll
+          for (int c = 0; c < 3; ++c) { float sn, cs; sincosf(__fmul_rn(f, p[c]), &sn, &cs); ee[3 + 6 * l + c] = sn; ee[6 + 6 * l + c] = cs; }
+        }
       }
       ee[63] = 0.f;
 #pragma unroll
       for (int kb = 0; kb < 8; ++kb) {
         if ((kb >> 2) != part) continue;   // static register indices: ee[] stays in registers
-        split_store8(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
+        if constexpr (TAN) split_store8_bf16(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
+        else split_store8(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
         if (stash) {
           __stcs(reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8), make_float4(ee[kb * 8], ee[kb * 8 + 1], ee[kb * 8 + 2], ee[kb * 8 + 3]));
           __stcs(reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8 + 4), make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]));
@@ -502,6 +539,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
     }
     float s_logit[2] = {0.f, 0.f};
     for (int g = 0; g < n_gemm; ++g) {
+      uint32_t gm[D / 64];   // FWD_TANGENT: the forward's gate bits of layer g, loaded before the MMAs so the load completes behind them
+      if constexpr (TAN) load_gates<D / 2>(st.gates + gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gm);
       // ---- MMAs: K-steps from the encoding operand E (layers 0 and 4) first, then from the previous layer's output; in points mode
       //      the rgb hidden layer ends with the two K-steps of the direction operand, which took E's place after layer 4 ----
       const int n_e = T::enc_steps(g), ns = T::gemm_steps(g, PTS);
@@ -515,7 +554,11 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         const uint64_t dbh = gdesc(wb, nrows * 16u, 128), dbl = gdesc(wb + nrows * 32u, nrows * 16u, 128);
         mbar_wait(FULL(slot), phase);
         wgmma_fence();
-        if (g < 9) {
+        if constexpr (TAN) {
+          wgmma_bf16<D>(acc, dal, dbh, s > 0 ? 1u : 0u);
+          wgmma_bf16<D>(acc, dah, dbl, 1u);
+          wgmma_bf16<D>(acc, dah, dbh, 1u);
+        } else if (g < 9) {
           wgmma_f16<D>(acc, dal, dbh, s > 0 ? 1u : 0u);
           wgmma_f16<D>(acc, dah, dbl, 1u);
           wgmma_f16<D>(acc, dah, dbh, 1u);
@@ -534,7 +577,26 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
       wgmma_wait<0>();
       if (tl == 0) mbar_arrive(EMPTY(slot == 0 ? NST - 1 : slot - 1));
       // ---- epilogue ----
-      if (g < 9) {
+      if constexpr (TAN) {   // h'_g = [h_g > 0] z'_g: no bias, the forward's gate -> tangent stash and the next A operand (bf16 hi | lo)
+#pragma unroll
+        for (int j = 0; j < D / 8; ++j) {
+          const int col = j * 8 + c0;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int row = r0 + 8 * r;
+            const uint32_t b = gm[j / 8] << (4 * (j & 7) + 2 * r);   // gate bits of columns c0 and c0 + 1 at bits 31 and 30
+            const float v0 = (b & 0x80000000u) ? acc[4 * j + 2 * r] : 0.f, v1 = (b & 0x40000000u) ? acc[4 * j + 2 * r + 1] : 0.f;
+            uint32_t hw, lw;
+            split2_bf16(v0, v1, hw, lw);
+            const int off = j * 2048 + row * 16 + c0 * 2;
+            *reinterpret_cast<uint32_t*>(smem + SM_AHI + off) = hw;
+            *reinterpret_cast<uint32_t*>(smem + SM_ALO + off) = lw;
+            __stcs(reinterpret_cast<float2*>(st.h[g] + (mt + row) * D + col), make_float2(v0, v1));
+          }
+        }
+        fence_async_smem();
+        wg_sync();
+      } else if (g < 9) {
         const float* bias = (g < 8) ? s_bias + g * D : s_bias + B_FEAT0;
         float* sp = stash ? (g < 8 ? st.h[g] : st.feat) : nullptr;
         uint32_t gw[D / 64] = {};   // ReLU gate bits of this thread's fragment, shifted in in the order b = 4j + 2r + e
@@ -1024,20 +1086,22 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
 // direction slice of rgb_layers.0 are at column offset D, enc[1] has no bias), so one reduce gives the same bits as one per grid.
 // occ (nnb_field_grad with NNB_OCC_ONLY): the colour jobs (fc_feature, rgb_layers.0, fc_rgb) are left out, so grid 2 is not launched, the
 // head grid runs the density head alone, and the colour parameters' gradients are not touched.  The kernels are those of the full stage.
-cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw, bool occ, cudaStream_t st) {
+// !bias (nnb_field_hvp_tc, whose tangent has no bias term): every job's db is NULL, so no bias slot of gw is touched.
+cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw, bool occ, bool bias, cudaStream_t st) {
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
   const int D = L.D, DR = D / 2;
   WgJobT big[8], enc[2];
   int nb = 0;
-  for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(D, l), gw + nnb::b_off(D, l), D, D, D, D, nnb::w_ld(D, l), 0, 0};
+  auto B = [&](size_t off) { return bias ? gw + off : nullptr; };
+  for (int l = 1; l < 8; ++l) big[nb++] = WgJobT{F(L.dy[l]), F(L.h[l - 1]), gw + nnb::w_off(D, l), B(nnb::b_off(D, l)), D, D, D, D, nnb::w_ld(D, l), 0, 0};
   if (!occ) big[nb++] = WgJobT{F(L.dfeat), F(L.h[7]), gw + nnb::W_FEAT(D), gw + nnb::B_FEAT(D), D, D, D, D, D, 0, 0};
   const WgJobT rgb{F(L.dyr), F(L.feat), gw + nnb::W_RGBH(D), gw + nnb::B_RGBH(D), DR, DR, D, D, D + 27, 0, 0};
-  enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(D, 0), gw + nnb::b_off(D, 0), D, D, 64, 63, 63, 0, 0};
+  enc[0] = WgJobT{F(L.dy[0]), F(L.enc), gw + nnb::w_off(D, 0), B(nnb::b_off(D, 0)), D, D, 64, 63, 63, 0, 0};
   enc[1] = WgJobT{F(L.dy[4]), F(L.enc), gw + nnb::w_off(D, 4) + D, nullptr, D, D, 64, 63, D + 63, 0, 0};
   const float* dyc = F(L.dyc);
   SmallJob sm[3] = {
-      {dyc + 3, F(L.h[7]), gw + nnb::W_SIG(D), gw + nnb::B_SIG(D), 4, 1, D, D, D},
+      {dyc + 3, F(L.h[7]), gw + nnb::W_SIG(D), B(nnb::B_SIG(D)), 4, 1, D, D, D},
       {F(L.dyr), F(L.denc), gw + nnb::W_RGBH(D) + D, nullptr, DR, DR, 32, 27, D + 27},
       {dyc, F(L.hr), gw + nnb::W_RGB(D), gw + nnb::B_RGB(D), 4, 3, DR, DR, DR}};
   float* part = F(L.wpart);
@@ -1078,7 +1142,7 @@ cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, 2, part, st);
 }
-cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) { return tc_wgrad_jobs(a, L, gw, false, st); }
+cudaError_t tc_wgrad_all(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st) { return tc_wgrad_jobs(a, L, gw, false, true, st); }
 
 // ---- data-gradient chain (the forward's skeleton run backwards) ---------------------------------------------------------------------
 // Per 128-sample tile, two consumer warpgroups (64 rows each) and a producer warpgroup streaming TRANSPOSED weight stages: stage =
@@ -1145,13 +1209,6 @@ __device__ __forceinline__ void dg_gemm(float* acc, uint32_t a_hi, uint32_t a_lo
   if (tl == 0) mbar_arrive(bar0 + 8u * (NST + (slot == 0 ? NST - 1 : slot - 1)));
 }
 
-__device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint32_t& lo) {
-  __nv_bfloat162 hh = __floats2bfloat162_rn(a, b);
-  hi = *reinterpret_cast<uint32_t*>(&hh);
-  __nv_bfloat162 ll = __floats2bfloat162_rn(a - __uint_as_float(hi << 16), b - __uint_as_float(hi & 0xffff0000u));
-  lo = *reinterpret_cast<uint32_t*>(&ll);
-}
-
 // MODE DG_RAYS (tc_dgrad, the render backward): rows are the samples of a.N rays, the records / cotangents / gradients are the
 // workspace's [Mpad] arrays, and the dY stash is written when write_dy.  DG_POINTS / DG_POINTS_OCC (tc_points_vjp, nnb_field_vjp): rows
 // are the explicit points a.pts [M]; P.gs is the caller's g_rgba [M] (rows >= M read as zero), P.gp / P.gv are g_pts / g_dirs [M] (P.gv
@@ -1161,13 +1218,18 @@ __device__ __forceinline__ void split2_bf16(float a, float b, uint32_t& hi, uint
 // DG_POINTS_GRAD / DG_POINTS_GRAD_OCC (tc_points_grad, nnb_field_grad): DG_POINTS / DG_POINTS_OCC that also write the dY stash of every
 // row of every tile, as DG_RAYS does with write_dy (rows >= M have a zero cotangent, so their dY are zeros); the occupancy-only chain
 // writes dy0..dy7 and dyc = (0, 0, 0, d/d density logit).
-enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4 };
+// DG_POINTS_HVP_OCC (tc_points_hvp, nnb_field_hvp_tc): DG_POINTS_GRAD_OCC with the cotangent 1 on the logit of every row < M (P.gs is
+// not read for it) and, in place of the first-order d p, the second-order point term of the tangent s' = u . d s / d p: from the
+// encoding adjoint delta_enc and p, -u_c sum_l f^2 (delta_sin sin(f p_c) + delta_cos cos(f p_c)), f = 2^l, with u = P.gs[m].  P.gp may be
+// NULL (no point term is stored).
+enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4, DG_POINTS_HVP_OCC = 5 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
                                               int n_tiles, int write_dy, const int* count = nullptr) {
   using T = Tc<D>;
-  constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC;
-  constexpr bool GRAD = MODE == DG_POINTS_GRAD || MODE == DG_POINTS_GRAD_OCC;
+  constexpr bool HVP = MODE == DG_POINTS_HVP_OCC;
+  constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC || HVP;
+  constexpr bool GRAD = MODE == DG_POINTS_GRAD || MODE == DG_POINTS_GRAD_OCC || HVP;
   static_assert(!DEVN || (PTS && !GRAD), "a device count of explicit points");
   if constexpr (PTS) write_dy = GRAD ? 1 : 0;
   if constexpr (DEVN) {
@@ -1277,7 +1339,9 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
     if (tl < 64) {   // head adjoints (one thread per row)
       const size_t m = mt + wg * 64 + tl;
       if constexpr (OCC) {
-        const float gw = (m < M) ? reinterpret_cast<const float*>(P.gs + m)[3] : 0.f;
+        float gw;
+        if constexpr (HVP) gw = (m < M) ? 1.f : 0.f;
+        else gw = (m < M) ? reinterpret_cast<const float*>(P.gs + m)[3] : 0.f;
         gyc[tl * 4 + 3] = gw * density_act_grad(P.rec[m].s, a.flags);
         if constexpr (GRAD) __stcs(P.dyc + m, make_float4(0.f, 0.f, 0.f, gyc[tl * 4 + 3]));
       } else {
@@ -1373,8 +1437,27 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
         row_geometry_tc(a, m, M, ray, z, p);
       }
       const float* ge = genc + tl * 64;
-      encode_bwd<10>(p, [&](int k) { return ge[k]; }, gp);
-      if (!PTS || m < M) P.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
+      if constexpr (HVP) {   // the point term of simt_field_tangent, in its order and rounding
+        if (P.gp && m < M) {
+          const float4 uv = P.gs[m];
+          const float u[3] = {uv.x, uv.y, uv.z};
+#pragma unroll
+          for (int c = 0; c < 3; ++c) {
+            float s2 = 0.f;
+#pragma unroll
+            for (int l = 0; l < 10; ++l) {
+              const float f = (float)(1 << l);
+              float sn, cs; sincosf(__fmul_rn(f, p[c]), &sn, &cs);
+              s2 = fmaf(__fmul_rn(f, f), fmaf(ge[3 + 6 * l + c], sn, __fmul_rn(ge[6 + 6 * l + c], cs)), s2);
+            }
+            gp[c] = -__fmul_rn(s2, u[c]);
+          }
+          P.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
+        }
+      } else {
+        encode_bwd<10>(p, [&](int k) { return ge[k]; }, gp);
+        if (!PTS || m < M) P.gp[m] = make_float4(gp[0], gp[1], gp[2], 0.f);
+      }
     }
   }
 }
@@ -1428,6 +1511,19 @@ template <int D, int MODE>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_points_grad(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                                const __grid_constant__ DgPtrs P, size_t M, int n_tiles) {
   tc_dgrad_body<D, MODE>(a, wimg, P, M, n_tiles, 1);
+}
+// nnb_field_hvp_tc, after the occupancy-only tc_points_vjp_fwd: the chain for a cotangent 1 on the logit with the dY stash and the point
+// term (DG_POINTS_HVP_OCC), and the tangent chain (FWD_TANGENT, u read through the output pointer) into the tangent stash st
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_hvp(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                              const __grid_constant__ DgPtrs P, size_t M, int n_tiles) {
+  tc_dgrad_body<D, DG_POINTS_HVP_OCC>(a, wimg, P, M, n_tiles, 1);
+}
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_points_tangent(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                  const float4* __restrict__ u, const __grid_constant__ TcStash st, size_t M,
+                                                                  int n_tiles) {
+  tc_fwd_body<D, FWD_TANGENT>(a, wimg, nullptr, const_cast<float4*>(u), st, MarchPtrs{}, M, n_tiles, 1);
 }
 
 template <int D>
@@ -1798,7 +1894,72 @@ cudaError_t tc_field_grad_dim(const nnb_render_args& a, const float* g_rgba, flo
   if (e != cudaSuccess || !g_weights) return e;
   WsLayout Lw = L;
   Lw.M = L.Mpad;   // whole tiles: the stash rows past N are written, with zero dY
-  return tc_wgrad_jobs(a, Lw, g_weights, occ, st);
+  return tc_wgrad_jobs(a, Lw, g_weights, occ, true, st);
+}
+
+// Workspace of nnb_field_hvp_tc, every section 256-byte aligned: grad_layout(N, occ = true) | the bf16 image of the occupancy-only
+// forward stages.  The tangent stash (e', h'0..h'7, Npad rows) takes the place of the fp32 activation stash (enc, h0..h7), which this
+// call does not write: the tangent chain gates with the forward's bits.
+struct HvpWs { GradWs g; size_t img16, total; };
+template <int D> HvpWs hvp_layout(int N) {
+  HvpWs w{};
+  w.g = grad_layout<D>(N, true);
+  w.img16 = w.g.total;
+  w.total = w.img16 + align_up((size_t)Tc<D>::N_STAGES_OCC * Tc<D>::STAGE_BYTES, 256);
+  return w;
+}
+
+// nnb_field_hvp_tc: the three weight images, the occupancy-only forward with records and gate bits (tc_points_vjp_fwd), the chain for a
+// cotangent 1 on the logit with the dY stash and the point term, then (g_weights) the tangent chain and the weight-gradient stage on
+// (dY, tangent) without bias jobs, on Mpad rows: the rows past N have dY = 0 and u = 0, so they add exactly 0
+template <int D>
+cudaError_t tc_field_hvp_dim(const nnb_render_args& a, const float* u, float* g_pts, float* g_weights, cudaStream_t st) {
+  using T = Tc<D>;
+  cudaError_t e = upload_stage_table<D>();
+  if (e == cudaSuccess) e = upload_stage_table_t<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_points_vjp_fwd<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_hvp<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_points_tangent<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  const HvpWs w = hvp_layout<D>(a.N);
+  const WsLayout& L = w.g.L;
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  SampleRec* recs = reinterpret_cast<SampleRec*>(base + L.rec);
+  unsigned char* gates = reinterpret_cast<unsigned char*>(base + L.gates);
+  unsigned char *img = reinterpret_cast<unsigned char*>(base + w.g.img), *img_t = reinterpret_cast<unsigned char*>(base + w.g.img_t);
+  unsigned char* img16 = reinterpret_cast<unsigned char*>(base + w.img16);
+  tc_prep_weights<D><<<T::N_STAGES_OCC, 256, 0, st>>>(a.weights, img);
+  tc_prep_weights_t_from<D><<<T::dg_tile_stages(true), 256, 0, st>>>(a.weights, img_t, T::dg_first_stage(true));
+  const int n_tiles = (a.N + TILE - 1) / TILE;
+  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  tc_points_vjp_fwd<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, nullptr, gates, (size_t)a.N, n_tiles);
+  DgPtrs P{};
+  P.rec = recs; P.gates = gates;
+  P.gs = reinterpret_cast<const float4*>(u); P.gp = reinterpret_cast<float4*>(g_pts);
+  P.dyc = reinterpret_cast<float4*>(base + L.dyc);
+  for (int l = 0; l < 8; ++l) P.dy[l] = F(L.dy[l]);
+  tc_points_hvp<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)a.N, n_tiles);
+  e = cudaGetLastError();
+  if (e != cudaSuccess || !g_weights) return e;
+  TcStash ts{};
+  for (int l = 0; l < 8; ++l) ts.h[l] = F(L.h[l]);
+  ts.enc = F(L.enc); ts.gates = gates;
+  tc_prep_weights_bf16<D><<<T::N_STAGES_OCC, 256, 0, st>>>(a.weights, img16);
+  tc_points_tangent<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img16, reinterpret_cast<const float4*>(u), ts, (size_t)a.N, n_tiles);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  WsLayout Lw = L;
+  Lw.M = L.Mpad;   // whole tiles: the stash rows past N are written, with zero dY and zero tangents
+  return tc_wgrad_jobs(a, Lw, g_weights, true, false, st);
 }
 
 // ---- nnb_geometry_frame: the geometry view (Renderer.phong_renderer) of N pixels on the device ----------------------------------
@@ -2043,6 +2204,14 @@ cudaError_t tc_field_grad(const nnb_render_args& a, const float* g_rgba, float* 
   return D == 128 ? tc_field_grad_dim<128>(a, g_rgba, out_rgba, g_pts, g_dirs, g_weights, st)
        : D == 64  ? tc_field_grad_dim<64>(a, g_rgba, out_rgba, g_pts, g_dirs, g_weights, st)
                   : tc_field_grad_dim<256>(a, g_rgba, out_rgba, g_pts, g_dirs, g_weights, st);
+}
+
+size_t tc_field_hvp_workspace(int N, int D) {
+  return D == 128 ? hvp_layout<128>(N).total : (D == 64 ? hvp_layout<64>(N).total : hvp_layout<256>(N).total);
+}
+cudaError_t tc_field_hvp(const nnb_render_args& a, const float* u, float* g_pts, float* g_weights, int D, cudaStream_t st) {
+  return D == 128 ? tc_field_hvp_dim<128>(a, u, g_pts, g_weights, st)
+       : D == 64  ? tc_field_hvp_dim<64>(a, u, g_pts, g_weights, st) : tc_field_hvp_dim<256>(a, u, g_pts, g_weights, st);
 }
 
 size_t tc_render_frame_workspace(int N, int D) {

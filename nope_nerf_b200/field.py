@@ -99,20 +99,66 @@ class _GradFn(torch.autograd.Function):
         return (None, None, g_p[:, :3] if need_p else None) + tuple(gp)
 
 
-def field_normal(net, p, engine=None):
+def field_normal(net, p, engine=None, grad_engine=None):
     """n = d(density logit)/d p, shape (M, 3), for p (M, 3).  Differentiable with respect to p and the MLP parameters (the second-order
     backward is nnb_field_hvp); a third derivative raises.  M == 0 returns an empty tensor without a library call.
     engine: None or 'simt' = the exact-fp32 engine.  'tc' (or ENGINE_TC) = the tensor-core data gradient (nnb_field_vjp) when the call
     needs no autograd graph (the rule of field_query); a call that needs one runs on the exact engine, which has the second-order
     backward.  The tensor-core normals agree with float64 to 1.4e-5 of their maximum (the exact engine's to 5e-7), where both use the same
     ReLU gates; at a point whose pre-activation lies within rounding of 0 the engines may gate a unit differently, and the normal, which is
-    discontinuous there, then differs by that unit's contribution."""
+    discontinuous there, then differs by that unit's contribution.
+    grad_engine: the engine of a call that needs the autograd graph (the rule of field_query_grad).  None or 'simt' = the exact engine (the
+    rule above).  'tc' (or ENGINE_TC) needs engine='tc' (ValueError otherwise): the normals are then the bits of the detached
+    tensor-core normals (nnb_field_vjp) and their backward is the tensor-core second-order backward nnb_field_hvp_tc, once differentiable,
+    with gradients to p and the MLP parameters."""
     ops._need_cuda(p, "p")
+    g_engine = None if grad_engine is None else _grad_engine_id(engine, grad_engine)
     if p.shape[0] == 0:
         return p * 0.0          # shape (0, 3), connected to p when p requires grad, so a backward over it gives zeros
-    if _engine_id(engine) == L.ENGINE_TC and not needs_grad(net, p):
-        return _normal_tc(net, p)
+    if _engine_id(engine) == L.ENGINE_TC:
+        if not needs_grad(net, p):
+            return _normal_tc(net, p)
+        if g_engine == L.ENGINE_TC:
+            return _GradTcFn.apply(net, net.flat_weights(), p, *list(net.parameters()))
     return _GradFn.apply(net, net.flat_weights(), p, *list(net.parameters()))
+
+
+class _GradTcFn(torch.autograd.Function):
+    """n = d s / d p of the density logit on the tensor-core engine under autograd (field_normal(engine='tc', grad_engine='tc')).
+    forward: nnb_field_vjp with cotangent 1 on the logit (_normal_tc), so n is the detached gradient(engine='tc') normals' bits.  backward:
+    nnb_field_hvp_tc, which recomputes everything from the points and weights, so only p is kept.  Differentiable once, like _GradFn."""
+
+    @staticmethod
+    def forward(ctx, net, flat, p, *params):
+        p_c = ops._f32c(p.detach())
+        n = _normal_tc(net, p_c)
+        ctx.net = net; ctx.flat = flat; ctx.nparams = len(params); ctx.slices = net.param_slices
+        ctx.save_for_backward(p_c)
+        return n
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, u):
+        p_c, = ctx.saved_tensors
+        net, flat = ctx.net, ctx.flat
+        need_p = ctx.needs_input_grad[2]
+        need_w = any(ctx.needs_input_grad[3:])
+        M, dev = p_c.shape[0], p_c.device
+        u4 = torch.zeros(M, 4, device=dev); u4[:, :3] = u
+        g_p = torch.empty(M, 4, device=dev) if need_p else None
+        g_w = torch.zeros(flat.numel(), device=dev) if need_w else None
+        if need_p or need_w:
+            flags = L.RAW_DENSITY | L.OCC_ONLY
+            a = L.RenderArgs()
+            a.weights = L.ptr(flat); a.pts = L.ptr(p_c); a.dirs = None
+            a.N = M; a.S = 1; a.flags = flags; a.engine = L.ENGINE_TC; a.hidden_dim = net.hidden_dim
+            ws = torch.empty(L.lib.nnb_field_hvp_tc_workspace_bytes(M, flags, net.hidden_dim), dtype=torch.uint8, device=dev)
+            a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
+            L.check(L.lib.nnb_field_hvp_tc(C.byref(a), L.ptr(u4), L.ptr(g_p), L.ptr(g_w), ops._stream()), "nnb_field_hvp_tc")
+        gp = [None] * ctx.nparams
+        if g_w is not None:
+            gp = [g_w[o:o + n].view(s) for (o, n, s) in ctx.slices]
+        return (None, None, g_p[:, :3] if need_p else None) + tuple(gp)
 
 
 def _normal_tc(net, p):

@@ -125,14 +125,22 @@ class OfficialStaticNerf(nn.Module):
         normals come back detached, as plain values that callers may read directly (.numpy()).  Renderer.nope_nerf's normal term sets
         requires_grad on its own surface points, as the reference does, so it reaches the MLP with a fixed pose, camera and depth too.
         engine: None = the exact-fp32 engine; 'tc' = the tensor-core data gradient (nnb_field_vjp) for detached normals.  A call that
-        returns a grad_fn (grad mode on and p requiring grad) runs on the exact engine whatever engine it names (field.field_normal)."""
+        returns a grad_fn (grad mode on and p requiring grad) runs on the exact engine whatever engine it names (field.field_normal).
+        gradient_grad(p, it, engine='tc', grad_engine='tc') keeps such a call on tensor cores."""
+        return self.gradient_grad(p, it, engine)
+
+    def gradient_grad(self, p, it, engine=None, grad_engine=None):
+        """gradient() with the engine of a call that returns a grad_fn.  grad_engine: None or 'simt' = the exact engine (gradient()'s
+        rule); 'tc' (with engine='tc' only, ValueError otherwise, whether or not the call needs the graph) = the normals keep the bits of
+        the detached tensor-core normals and their backward is the tensor-core second-order backward nnb_field_hvp_tc
+        (field.field_normal)."""
         from ..field import field_normal
         q = p.reshape(-1, 3)
         if torch.is_grad_enabled() and p.requires_grad:
-            n = field_normal(self, q)
+            n = field_normal(self, q) if grad_engine is None else field_normal(self, q, engine=engine, grad_engine=grad_engine)
         else:
             with torch.no_grad():
-                n = field_normal(self, q, engine=engine)
+                n = field_normal(self, q, engine=engine, grad_engine=grad_engine)
         return -n.reshape(p.shape).unsqueeze(1)
 
     def forward(self, p, ray_d=None, only_occupancy=False, return_logits=False, return_addocc=False,

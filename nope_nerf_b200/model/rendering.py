@@ -33,6 +33,13 @@ class Renderer(nn.Module):
         # engine of the geometry view's normals (OfficialStaticNerf.gradient(engine=)): None = exact fp32, 'tc' = the tensor-core data
         # gradient.  Separate from field_engine, so that a renderer built with field_engine='tc' keeps the bits it had.
         self.normal_engine = kwargs.get("normal_engine", None)
+        # engine of the differentiable normals of rendering.normal_loss (_normal_diff): None = the exact engine whatever normal_engine
+        # says; 'tc' (needs normal_engine='tc', ValueError otherwise) = the tensor-core normals with the tensor-core second-order backward
+        # (OfficialStaticNerf.gradient_grad(engine='tc', grad_engine='tc')).
+        self.normal_grad_engine = kwargs.get("normal_grad_engine", None)
+        if self.normal_grad_engine is not None:
+            from ..field import _grad_engine_id
+            _grad_engine_id(self.normal_engine, self.normal_grad_engine)
         # geometry_frame=True: forward(..., 'phong_renderer') runs phong_frame (one tensor-core call for any number of pixels, rays
         # computed per pixel), and Extract_Images.render_geometry / Trainer.render_visdata pass the whole frame in one call.  Its
         # frames differ from phong_renderer's in the last bits of the rays, so it is off by default.
@@ -130,7 +137,10 @@ class Renderer(nn.Module):
             # fixed pose, camera and depth: like the reference (official_nerf.py:48, p.requires_grad_(True) inside gradient()), the
             # points this renderer owns become a leaf that requires grad, so the normal term still reaches the MLP
             pp.requires_grad_(True)
-        g = self.model.gradient(pp, it)[:, 0, :]
+        if self.normal_grad_engine is None:
+            g = self.model.gradient(pp, it)[:, 0, :]
+        else:
+            g = self.model.gradient_grad(pp, it, engine=self.normal_engine, grad_engine=self.normal_grad_engine)[:, 0, :]
         normals = g / (g.norm(2, dim=1).unsqueeze(-1) + 10 ** (-5))
         return torch.norm(normals[:N] - normals[N:], dim=-1)
 
