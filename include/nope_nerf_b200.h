@@ -261,8 +261,8 @@ int nnb_render_bwd(const nnb_render_bwd_args* a, void* stream);
  *     +inf otherwise.
  *   first [N] (optional, NULL = not wanted): the index above; -1 where there is none or val_0 >= 0 (such a ray is not searched further).
  *   bracket [N,4] (optional, 16-byte aligned): the bracket before the secant steps on a hit, zeros elsewhere.
- * Engine: tensor cores only.  engine != NNB_ENGINE_TC is rejected (rc < 0); the exact-fp32 engine has no fused march.  Precision is
- * that of nnb_field_fwd on NNB_ENGINE_TC.
+ * Engine: tensor cores only.  engine != NNB_ENGINE_TC is rejected (rc < 0); the exact-fp32 engine's fused march is nnb_ray_march_engine
+ * (below).  Precision is that of nnb_field_fwd on NNB_ENGINE_TC.
  * Bit-equality contract: on this engine a point's occupancy does not depend on the tile or row that evaluates it, and every product, sum
  * and quotient above is rounded on its own in the order of the torch code.  depth, first and bracket are therefore bit-identical to
  * Renderer.ray_marching / secant run on nnb_field_fwd(NNB_ENGINE_TC | NNB_OCC_ONLY) with frac = torch.linspace(0, 1, n_steps) (passed in,
@@ -282,12 +282,24 @@ typedef struct nnb_ray_march_args {
   int32_t N, n_steps /* >= 2 */, n_secant /* >= 0 */, hidden_dim /* 64, 128, 256; 0 = 256 */;
   float near_, tau;
   uint32_t flags;        /* NNB_DIST_ALPHA | NNB_SOFTPLUS */
-  int32_t engine;        /* NNB_ENGINE_TC */
+  int32_t engine;        /* NNB_ENGINE_TC (nnb_ray_march_engine: or NNB_ENGINE_SIMT) */
   float* depth; int32_t* first; float* bracket;
   void* workspace; size_t workspace_bytes;
 } nnb_ray_march_args;
 size_t nnb_ray_march_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
 int nnb_ray_march(const nnb_ray_march_args* a, void* stream);
+/* nnb_ray_march on a->engine: NNB_ENGINE_TC (exactly nnb_ray_march) or NNB_ENGINE_SIMT, the exact-fp32 engine; any other engine is
+ * rejected (rc -4), and the other checks and codes are nnb_ray_march's.  nnb_ray_march keeps its contract (tensor cores only).  No version
+ * bump: the symbols mark the capability.
+ * On NNB_ENGINE_SIMT the contract above holds with the occupancy of nnb_field_fwd on NNB_ENGINE_SIMT (the exact engine's fp32 FMA field,
+ * the colour branch skipped).  A point's exact occupancy does not depend on its tile or row either, so depth, first and bracket are
+ * bit-identical to Renderer.ray_marching / secant on the default (exact) engine with frac = torch.linspace(0, 1, n_steps).  The same rounds
+ * of 128 steps, the same counters.  Its workspace is the layout above without a weight image, checked against
+ * nnb_ray_march_workspace_bytes_engine(N, n_steps, hidden_dim, NNB_ENGINE_SIMT).
+ * nnb_ray_march_workspace_bytes_engine: the workspace on `engine` (nnb_ray_march_workspace_bytes is this on NNB_ENGINE_TC); 0 on bad
+ * sizes, an unsupported width or an engine without the march. */
+int nnb_ray_march_engine(const nnb_ray_march_args* a, void* stream);
+size_t nnb_ray_march_workspace_bytes_engine(int32_t N, int32_t n_steps, int32_t hidden_dim, int32_t engine);
 
 /* The geometry view of any set of N pixels in one stream-ordered call: what Renderer.phong_renderer (model/rendering.py:148-180) does,
  * with every ray computed per pixel, on the tensor-core engine.  No version bump: the symbol marks the capability.
@@ -327,7 +339,7 @@ typedef struct nnb_geometry_args {
   int32_t N, n_steps /* >= 2 */, n_secant /* >= 0 */, hidden_dim /* 64, 128, 256; 0 = 256 */;
   float near_, tau, radius;
   uint32_t flags;         /* NNB_DIST_ALPHA | NNB_SOFTPLUS (the occupancy of the march) */
-  int32_t engine;         /* NNB_ENGINE_TC */
+  int32_t engine;         /* NNB_ENGINE_TC (nnb_geometry_frame_engine: or NNB_ENGINE_SIMT) */
   float* rgb;             /* [N,3] shaded view */
   float* rgb_surf;        /* [N,3] surface colour */
   /* optional (NULL = not wanted): */
@@ -336,6 +348,20 @@ typedef struct nnb_geometry_args {
 } nnb_geometry_args;
 size_t nnb_geometry_frame_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
 int nnb_geometry_frame(const nnb_geometry_args* a, void* stream);
+/* nnb_geometry_frame on a->engine: NNB_ENGINE_TC (exactly nnb_geometry_frame) or NNB_ENGINE_SIMT, the exact-fp32 engine; any other
+ * engine is rejected (rc -4), and the other checks and codes are nnb_geometry_frame's.  nnb_geometry_frame keeps its contract (tensor
+ * cores only).  No version bump: the symbols mark the capability.  nnb_geometry_frame_workspace_bytes_engine: the workspace on `engine`
+ * (nnb_geometry_frame_workspace_bytes is this on NNB_ENGINE_TC); 0 on bad sizes, an unsupported width or an engine without the frame.
+ * On NNB_ENGINE_SIMT the same contract and flags hold with every field query on the exact engine: the march is nnb_ray_march_engine on
+ * NNB_ENGINE_SIMT; grad is the negated g_pts of nnb_field_fwd + nnb_field_bwd on NNB_ENGINE_SIMT
+ * with NNB_RAW_DENSITY, no view directions and the cotangent (0, 0, 0, 1) (OfficialStaticNerf.gradient on the default engine); rgb_surf
+ * is the rgb of nnb_field_fwd on NNB_ENGINE_SIMT at (p, -dir).  The stage bit-equality and pixel independence above hold with those
+ * calls.  The normals and colours of the compacted rows run in passes of at most 32 768 rows, so the fp32 stash of the chain does not grow
+ * with N.  Workspace, each section 256-byte aligned: hit count | ray0, dir, far, depth | surface points, view directions, pixel indices,
+ * normal cotangents (16 N), normals (16 Npad, Npad = N rounded up to 64), colours (16 N) | the exact march's workspace | one pass's
+ * records and fp32 stash.  At N = 1080 x 1920, n_steps = 512, D = 256: 672 993 792 bytes (0.67 GB). */
+int nnb_geometry_frame_engine(const nnb_geometry_args* a, void* stream);
+size_t nnb_geometry_frame_workspace_bytes_engine(int32_t N, int32_t n_steps, int32_t hidden_dim, int32_t engine);
 
 /* The volumetric view of a whole frame (or any N rays) in one stream-ordered call on the tensor-core engine, with compositing fused into
  * the field's forward: what nnb_render_fwd does without NNB_STASH, in a workspace that does not grow with S, and optionally with early ray

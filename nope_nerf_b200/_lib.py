@@ -111,6 +111,12 @@ def _load():
     lib.nnb_geometry_frame.argtypes = [C.POINTER(GeometryArgs), C.c_void_p]
     lib.nnb_geometry_frame_workspace_bytes.restype = C.c_size_t
     lib.nnb_geometry_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    lib.nnb_ray_march_engine.argtypes = [C.POINTER(RayMarchArgs), C.c_void_p]
+    lib.nnb_geometry_frame_engine.argtypes = [C.POINTER(GeometryArgs), C.c_void_p]
+    lib.nnb_ray_march_workspace_bytes_engine.restype = C.c_size_t
+    lib.nnb_ray_march_workspace_bytes_engine.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+    lib.nnb_geometry_frame_workspace_bytes_engine.restype = C.c_size_t
+    lib.nnb_geometry_frame_workspace_bytes_engine.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
     lib.nnb_render_frame.argtypes = [C.POINTER(FrameArgs), C.c_void_p]
     lib.nnb_render_frame_workspace_bytes.restype = C.c_size_t
     lib.nnb_render_frame_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]

@@ -13,6 +13,10 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
                            cudaStream_t st);
 cudaError_t simt_field_hvp(const nnb_render_args& a, const WsLayout& L, const float* u, float* g_pts, float* g_weights, cudaStream_t st);
 cudaError_t simt_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float* gw, cudaStream_t st);
+size_t simt_ray_march_workspace(int N, int n_steps);
+cudaError_t simt_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st);
+size_t simt_geometry_frame_workspace(int N, int n_steps, int D);
+cudaError_t simt_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
@@ -235,19 +239,28 @@ int nnb_field_fwd(const nnb_render_args* a, float* out_rgba, void* stream) {
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_field_fwd");
 }
 size_t nnb_ray_march_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim) {
-#ifdef NNB_WITH_TC
+  return nnb_ray_march_workspace_bytes_engine(N, n_steps, hidden_dim, NNB_ENGINE_TC);
+}
+size_t nnb_ray_march_workspace_bytes_engine(int32_t N, int32_t n_steps, int32_t hidden_dim, int32_t engine) {
   const int D = hidden_of(hidden_dim);
-  if (N > 0 && n_steps >= 2 && nnb::dim_supported(D)) return tc_ray_march_workspace(N, n_steps, D);
+  if (N <= 0 || n_steps < 2 || !nnb::dim_supported(D)) return 0;
+  if (engine == NNB_ENGINE_SIMT) return simt_ray_march_workspace(N, n_steps);
+#ifdef NNB_WITH_TC
+  if (engine == NNB_ENGINE_TC) return tc_ray_march_workspace(N, n_steps, D);
 #endif
   return 0;
 }
-int nnb_ray_march(const nnb_ray_march_args* a, void* stream) {
-  if (!a) return fail(-1, "null args");
-  if (a->engine != NNB_ENGINE_TC)
-    return fail(-4, "nnb_ray_march: engine %d has no fused march (NNB_ENGINE_TC only; march on the exact-fp32 engine through nnb_field_fwd)", a->engine);
+// the engines of nnb_ray_march_engine / nnb_geometry_frame_engine: NNB_ENGINE_TC (when built with it) and NNB_ENGINE_SIMT
+static int check_march_engine(int32_t engine, const char* call) {
+  if (engine != NNB_ENGINE_TC && engine != NNB_ENGINE_SIMT)
+    return fail(-4, "%s: engine %d has no fused march (NNB_ENGINE_TC or NNB_ENGINE_SIMT)", call, engine);
 #ifndef NNB_WITH_TC
-  return fail(-4, "library built without the tensor-core engine");
-#else
+  if (engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
+#endif
+  return 0;
+}
+// the checks after the engine's and the call, on a->engine (validated by the caller)
+static int ray_march_on(const nnb_ray_march_args* a, void* stream) {
   const int D = hidden_of(a->hidden_dim);
   if (!nnb::dim_supported(D)) return fail(-8, "hidden_dim %d is not supported (supported: 64, 128, 256; 0 means 256)", a->hidden_dim);
   if (a->N < 0) return fail(-2, "nnb_ray_march: N must not be negative (got %d)", a->N);
@@ -255,13 +268,31 @@ int nnb_ray_march(const nnb_ray_march_args* a, void* stream) {
   if (a->N == 0) return 0;
   if (!a->weights || !a->ray0 || !a->ray_dir || !a->far_ || !a->frac || !a->depth)
     return fail(-3, "nnb_ray_march: weights, ray0, ray_dir, far_, frac and depth must be non-null");
-  const size_t need = tc_ray_march_workspace(a->N, a->n_steps, D);
+  const size_t need = nnb_ray_march_workspace_bytes_engine(a->N, a->n_steps, a->hidden_dim, a->engine);
   if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
   if ((reinterpret_cast<uintptr_t>(a->bracket) & 15) != 0) return fail(-3, "nnb_ray_march: bracket must be 16-byte aligned");
-  cudaError_t e = tc_ray_march(*a, D, (cudaStream_t)stream);
-  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_ray_march");
+  cudaError_t e;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) e = tc_ray_march(*a, D, (cudaStream_t)stream); else
 #endif
+  e = simt_ray_march(*a, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_ray_march");
+}
+int nnb_ray_march(const nnb_ray_march_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_ray_march: engine %d has no fused march here (NNB_ENGINE_TC only; nnb_ray_march_engine runs NNB_ENGINE_SIMT)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  return ray_march_on(a, stream);
+#endif
+}
+int nnb_ray_march_engine(const nnb_ray_march_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (int rc = check_march_engine(a->engine, "nnb_ray_march_engine")) return rc;
+  return ray_march_on(a, stream);
 }
 size_t nnb_field_vjp_workspace_bytes(int32_t N, uint32_t flags, int32_t hidden_dim) {
 #ifdef NNB_WITH_TC
@@ -367,21 +398,20 @@ int nnb_field_hvp_tc(const nnb_render_args* a, const float* u, float* g_pts, flo
 #endif
 }
 size_t nnb_geometry_frame_workspace_bytes(int32_t N, int32_t n_steps, int32_t hidden_dim) {
-#ifdef NNB_WITH_TC
+  return nnb_geometry_frame_workspace_bytes_engine(N, n_steps, hidden_dim, NNB_ENGINE_TC);
+}
+size_t nnb_geometry_frame_workspace_bytes_engine(int32_t N, int32_t n_steps, int32_t hidden_dim, int32_t engine) {
   const int D = hidden_of(hidden_dim);
-  if (N > 0 && n_steps >= 2 && nnb::dim_supported(D)) return tc_geometry_frame_workspace(N, n_steps, D);
+  if (N <= 0 || n_steps < 2 || !nnb::dim_supported(D)) return 0;
+  if (engine == NNB_ENGINE_SIMT) return simt_geometry_frame_workspace(N, n_steps, D);
+#ifdef NNB_WITH_TC
+  if (engine == NNB_ENGINE_TC) return tc_geometry_frame_workspace(N, n_steps, D);
 #endif
   return 0;
 }
 static inline bool misaligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
-int nnb_geometry_frame(const nnb_geometry_args* a, void* stream) {
-  if (!a) return fail(-1, "null args");
-  if (a->engine != NNB_ENGINE_TC)
-    return fail(-4, "nnb_geometry_frame: engine %d has no geometry frame (NNB_ENGINE_TC only; Renderer.phong_renderer serves the exact engine)",
-                a->engine);
-#ifndef NNB_WITH_TC
-  return fail(-4, "library built without the tensor-core engine");
-#else
+// the checks after the engine's and the call, on a->engine (validated by the caller)
+static int geometry_frame_on(const nnb_geometry_args* a, void* stream) {
   if (int rc = check_flags(a->flags)) return rc;
   if (a->flags & ~(NNB_DIST_ALPHA | NNB_SOFTPLUS))
     return fail(-6, "nnb_geometry_frame: flags 0x%x: only NNB_DIST_ALPHA and NNB_SOFTPLUS are accepted", a->flags);
@@ -397,12 +427,31 @@ int nnb_geometry_frame(const nnb_geometry_args* a, void* stream) {
                         (const void*)a->rgb_surf, (const void*)a->ray0, (const void*)a->ray_dir, (const void*)a->far_, (const void*)a->depth})
     if (misaligned4(p)) return fail(-3, "nnb_geometry_frame: float arrays must be 4-byte aligned");
   if (misaligned16(a->grad)) return fail(-3, "nnb_geometry_frame: grad must be a 16-byte aligned [N][4] array");
-  const size_t need = tc_geometry_frame_workspace(a->N, a->n_steps, D);
+  const size_t need = nnb_geometry_frame_workspace_bytes_engine(a->N, a->n_steps, a->hidden_dim, a->engine);
   if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
-  cudaError_t e = tc_geometry_frame(*a, D, (cudaStream_t)stream);
-  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_geometry_frame");
+  cudaError_t e;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) e = tc_geometry_frame(*a, D, (cudaStream_t)stream); else
 #endif
+  e = simt_geometry_frame(*a, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_geometry_frame");
+}
+int nnb_geometry_frame(const nnb_geometry_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_geometry_frame: engine %d has no geometry frame here (NNB_ENGINE_TC only; nnb_geometry_frame_engine runs NNB_ENGINE_SIMT)",
+                a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  return geometry_frame_on(a, stream);
+#endif
+}
+int nnb_geometry_frame_engine(const nnb_geometry_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (int rc = check_march_engine(a->engine, "nnb_geometry_frame_engine")) return rc;
+  return geometry_frame_on(a, stream);
 }
 size_t nnb_render_frame_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim) {
 #ifdef NNB_WITH_TC

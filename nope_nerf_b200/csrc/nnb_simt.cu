@@ -10,6 +10,7 @@
 //      head_wgrad       : the same arithmetic for the TC engine's narrow head jobs, streamed at memory speed
 //   B4 ray_bwd          : per-ray geometry adjoint -> d c2w, d K, d depth, d scale/shift
 #include "nnb_tc_common.cuh"   // mbarrier / bulk-copy wrappers (head_wgrad)
+#include "nnb_march.cuh"
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -146,18 +147,37 @@ __device__ __forceinline__ void row_geometry(const nnb_render_args& a, size_t m,
   sample_point(a, ray, z, p);
 }
 
-template <int D>
-__global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPtrs P, size_t M, int stash) {
+// MODE of simt_fwd_tile: SF_RAYS (simt_mlp_fwd: the render's samples, or explicit points a.pts) writes records and the stash.
+// SF_MARCH / SF_SECANT (simt_march / simt_secant, nnb_ray_march on this engine) are occupancy-only tiles whose points come from q: the
+// colour branch is skipped and the density head's occupancy - tau goes to the march's back end instead of a record.
+//   SF_MARCH: row r is step 128 q.block + 64 pass + r of ray `mray` (clamped to its last step); the value goes to s_val[64 pass + r].
+//   SF_SECANT: row r is the secant iterate of hit ray q.list[m0 + r] (rows past M: the point 0, ignored); pass = the secant pass.
+enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2 };
+
+// one 64-row tile of the exact forward: rows m0 = 64 tile .. m0 + 63 of M
+template <int D, int MODE>
+__device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int stash, unsigned tile, const MarchPtrs& q,
+                                              int mray, int pass, float* s_val) {
   constexpr int LDB = ldb<D>(), NJ = D / 64, NJR = D >= 128 ? D / 128 : 1;   // output column blocks of the trunk / rgb hidden layers
   extern __shared__ __align__(16) float smem[];
   float* buf0 = smem; float* buf1 = buf0 + TM * LDB; float* Ws = buf1 + TM * LDB;
   const int tid = threadIdx.x;
-  const size_t m0 = (size_t)blockIdx.x * TM;
+  const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
   {  // prologue: encode positions into columns D..D+63 of both buffers
     int row = tid & 63, part = tid >> 6;
     Ray ray; int n, i; float z, p[3];
-    row_geometry(a, m0 + row, M, ray, n, i, z, p);
+    if constexpr (MODE == SF_MARCH) {
+      march_point(q, mray, march_depth(q.near, __ldg(q.far + mray), __ldg(q.frac + min(q.block * MARCH_BLOCK + pass * TM + row, q.n_steps - 1))), p);
+    } else if constexpr (MODE == SF_SECANT) {
+      p[0] = p[1] = p[2] = 0.f;
+      if (m0 + row < M) {
+        const int r = q.list[m0 + row];
+        march_point(q, r, secant_depth((pass == 0 ? q.brk0 : q.brk1)[r]), p);
+      }
+    } else {
+      row_geometry(a, m0 + row, M, ray, n, i, z, p);
+    }
     float* e0 = buf0 + row * LDB + D; float* e1 = buf1 + row * LDB + D;
     if (part == 0) {
 #pragma unroll
@@ -174,7 +194,7 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
     }
   }
   __syncthreads();
-  if (stash) {
+  if (MODE == SF_RAYS && stash) {
     for (int idx = tid; idx < TM * 16; idx += 256) {
       int row = idx >> 4, c4 = idx & 15;
       *reinterpret_cast<float4*>(P.enc + (m0 + row) * 64 + c4 * 4) = *reinterpret_cast<const float4*>(buf0 + row * LDB + D + c4 * 4);
@@ -187,7 +207,7 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
     int kvalid = (l == 0) ? 63 : (l == 4 ? D + 63 : D);
     tile_gemm<NJ, false, 1, false>(in, LDB, K, w + nnb::w_off(D, l), nnb::w_ld(D, l), D, kvalid, w + nnb::b_off(D, l), oth, LDB, Ws);
     __syncthreads();
-    if (stash) tile_to_global(oth, LDB, P.h[l], m0, D);
+    if (MODE == SF_RAYS && stash) tile_to_global(oth, LDB, P.h[l], m0, D);
     float* t_ = cur; cur = oth; oth = t_;
   }
   // cur = h8.  density head: 4 threads per row
@@ -202,6 +222,15 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
     acc += __shfl_xor_sync(0xffffffffu, acc, 1);
     acc += __shfl_xor_sync(0xffffffffu, acc, 2);
     s_logit = acc + __ldg(w + nnb::B_SIG(D));
+  }
+  if constexpr (MODE != SF_RAYS) {   // occupancy only: the colour branch does not enter the march
+    if (hc == 0) {
+      float sigma;
+      auto f = [&] { return __fsub_rn(density_act(s_logit, a.flags, &sigma), q.tau); };
+      if (MODE == SF_MARCH) s_val[pass * TM + hrow] = f();
+      else if (m0 + hrow < M) secant_update(q, q.list[m0 + hrow], pass == 0, f);
+    }
+    return;
   }
   // feature layer (no activation) -> oth, then dir encoding into cols D..D+31
   tile_gemm<NJ, false, 0, false>(cur, LDB, D, w + nnb::W_FEAT(D), D, D, D, w + nnb::B_FEAT(D), oth, LDB, Ws);
@@ -244,6 +273,51 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPt
       rec[4] = s_logit; rec[5] = z; rec[6] = 0.f; rec[7] = 0.f;
     }
   }
+}
+
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_mlp_fwd(nnb_render_args a, SimtPtrs P, size_t M, int stash) {
+  simt_fwd_tile<D, SF_RAYS>(a, P, M, stash, blockIdx.x, MarchPtrs{}, 0, 0, nullptr);
+}
+
+// Device-count form of simt_mlp_fwd on explicit points (nnb_geometry_frame on this engine): the rows are points off .. off + n - 1 of the
+// compacted list, n = min(*count - off, cap), read when the kernel starts; a.pts / a.dirs and the outputs start at row off.  A CTA past
+// the n rows exits before any barrier.
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_mlp_fwd_n(nnb_render_args a, SimtPtrs P, const int* __restrict__ count, int off, int cap,
+                                                         int stash) {
+  const int n = min(*count - off, cap);
+  if ((int)blockIdx.x * TM >= n) return;
+  simt_fwd_tile<D, SF_RAYS>(a, P, (size_t)n, stash, blockIdx.x, MarchPtrs{}, 0, 0, nullptr);
+}
+
+// one round of nnb_ray_march on this engine: block q.block of every ray of q.list (n_rays rays when q.count is NULL), one ray per CTA
+// and iteration, its 128 steps as two 64-row tiles (the second only when the ray has steps there); march_scan reduces them
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_march(nnb_render_args a, const __grid_constant__ MarchPtrs q, int n_rays) {
+  __shared__ __align__(16) float s_val[MARCH_BLOCK];
+  const int n_tiles = q.count ? *q.count : n_rays;
+  for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const int ray = q.list ? q.list[t] : t;
+    for (int pass = 0; pass < 2 && q.block * MARCH_BLOCK + pass * TM < q.n_steps; ++pass) {
+      simt_fwd_tile<D, SF_MARCH>(a, SimtPtrs{}, 0, 0, 0u, q, ray, pass, s_val);
+      __syncthreads();
+    }
+    if (threadIdx.x < 32) march_scan(q, ray, s_val, threadIdx.x);
+    __syncthreads();
+  }
+}
+
+// the q.n_secant secant passes of nnb_ray_march over the *q.count hit rays of q.list, 64 rays per tile; a pass reads the brackets the
+// previous pass of the same CTA wrote
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_secant(nnb_render_args a, const __grid_constant__ MarchPtrs q) {
+  const size_t M = (size_t)*q.count;
+  for (unsigned tile = blockIdx.x; (size_t)tile * TM < M; tile += gridDim.x)
+    for (int pass = 0; pass < q.n_secant; ++pass) {
+      simt_fwd_tile<D, SF_SECANT>(a, SimtPtrs{}, M, 0, tile, q, 0, pass, nullptr);
+      __syncthreads();
+    }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -346,15 +420,16 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
 // ---------------------------------------------------------------------------------------
 // B2: data-gradient chain
 // ---------------------------------------------------------------------------------------
+// one 64-row tile of the chain: rows m0 = 64 tile .. m0 + 63 of M
 template <int D>
-__global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, SimtPtrs P, size_t M, int write_dy) {
+__device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int write_dy, unsigned tile) {
   constexpr int LDB = ldb<D>(), NJ = D / 64, DR = D / 2;
   extern __shared__ __align__(16) float smem[];
   float* bufA = smem; float* bufB = bufA + TM * LDB; float* Ws = bufB + TM * LDB;
   float* genc = Ws + 2 * KC * WS_LD;          // [64][64]
   float* gyc = genc + TM * 64;                // [64][4]
   const int tid = threadIdx.x;
-  const size_t m0 = (size_t)blockIdx.x * TM;
+  const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
   {  // 1. head adjoints
     int row = tid >> 2, c = tid & 3; size_t m = m0 + row;
@@ -428,6 +503,20 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, Simt
     encode_bwd<10>(p, [&](int k) { return ge[k]; }, gp);
     P.gp[m0 + tid] = make_float4(gp[0], gp[1], gp[2], 0.f);
   }
+}
+
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, SimtPtrs P, size_t M, int write_dy) {
+  simt_dgrad_tile<D>(a, P, M, write_dy, blockIdx.x);
+}
+
+// Device-count form of simt_mlp_dgrad (the normals of nnb_geometry_frame on this engine), rows as in simt_mlp_fwd_n: the chain on the
+// stash simt_mlp_fwd_n wrote, without the dY stash.  A CTA past the n rows exits before any barrier.
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_mlp_dgrad_n(nnb_render_args a, SimtPtrs P, const int* __restrict__ count, int off, int cap) {
+  const int n = min(*count - off, cap);
+  if ((int)blockIdx.x * TM >= n) return;
+  simt_dgrad_tile<D>(a, P, (size_t)n, 0, blockIdx.x);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -875,6 +964,11 @@ static cudaError_t simt_init_dim() {
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(simt_field_tangent<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
     if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(simt_mlp_fwd_n<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_mlp_dgrad_n<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_march<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_secant<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e != cudaSuccess) return e;
     attr = true;
   }
   return cudaSuccess;
@@ -977,6 +1071,117 @@ cudaError_t simt_field_bwd(const nnb_render_args& a, const WsLayout& L, const fl
   if (g_pts) { e = cudaMemcpyAsync(g_pts, P.gp, L.M * 16, cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) return e; }
   if (g_dirs) { e = cudaMemcpyAsync(g_dirs, P.gv, L.M * 16, cudaMemcpyDeviceToDevice, st); if (e != cudaSuccess) return e; }
   return cudaGetLastError();
+}
+
+// ---- nnb_ray_march and nnb_geometry_frame on this engine (NNB_ENGINE_SIMT) -----------------------------------------------------------
+// The march: run_ray_march (nnb_march.cuh) with simt_march rounds and simt_secant passes, persistent grids of every CTA the SMs hold.
+// A point's occupancy is the exact forward's (simt_mlp_fwd's arithmetic, which does not depend on the tile or row that evaluates it), so
+// depth, first and bracket are the bits of Renderer.ray_marching / secant over nnb_field_fwd on this engine.
+size_t simt_ray_march_workspace(int N, int n_steps) { return march_layout_bytes(N, n_steps, 0).total; }
+
+template <int D>
+static cudaError_t simt_ray_march_dim(const nnb_ray_march_args& r, cudaStream_t st) {
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  static int slots = 0;   // CTAs of simt_march resident on the device at once
+  if (!slots) {
+    int dev = 0, n_sm = 0, per_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, simt_march<D>, 256, fwd_smem<D>());
+    if (e != cudaSuccess) return e;
+    slots = n_sm * (per_sm > 0 ? per_sm : 1);
+  }
+  const MarchWs w = march_layout_bytes(r.N, r.n_steps, 0);
+  const int grid = r.N < slots ? r.N : slots, tiles = (r.N + TM - 1) / TM;
+  return run_ray_march(
+      r, w, D, st, [&](const nnb_render_args& a, const MarchPtrs& q) { simt_march<D><<<grid, 256, fwd_smem<D>(), st>>>(a, q, r.N); },
+      [&](const nnb_render_args& a, const MarchPtrs& q) { simt_secant<D><<<tiles < slots ? tiles : slots, 256, fwd_smem<D>(), st>>>(a, q); });
+}
+cudaError_t simt_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st) {
+  return D == 128 ? simt_ray_march_dim<128>(r, st) : (D == 64 ? simt_ray_march_dim<64>(r, st) : simt_ray_march_dim<256>(r, st));
+}
+
+// rgba[m] = the (r, g, b, a) of record m for the n = min(*count - off, cap) rows of simt_mlp_fwd_n
+__global__ void rec_to_rgba_n(const SampleRec* __restrict__ rec, float4* __restrict__ out, const int* __restrict__ count, int off, int cap) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m < min(*count - off, cap)) out[m] = make_float4(rec[m].r, rec[m].g, rec[m].b, rec[m].a);
+}
+
+// Workspace of nnb_geometry_frame on this engine, every section 256-byte aligned: hit count | ray0, dir [N][3], far, depth [N] | compacted
+// rows: surface points, view directions [N][3], pixel indices [N], normal cotangents [N], d logit / d p [Npad], colours [N] float4 | the
+// march's workspace (N rays) | the fp32 stash of one pass of at most GEO_PASS compacted rows: records, h0..h7, feat, hr, enc, denc, the
+// direction adjoint.  Npad = N rounded up to 64: the chain writes whole 64-row tiles of d logit / d p.
+constexpr int GEO_PASS = 32768;
+struct SimtGeoWs { size_t count, ray0, dir, far, depth, pts, vdir, pix, gs, gp, rgba, march, rec, h[8], feat, hr, enc, denc, gv, total; int cap; };
+static SimtGeoWs simt_geo_layout(int N, int n_steps, int D) {
+  SimtGeoWs w{};
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  const size_t n = (size_t)N, npad = align_up(n, TM);
+  w.cap = (int)(npad < (size_t)GEO_PASS ? npad : (size_t)GEO_PASS);
+  const size_t c = (size_t)w.cap, d = (size_t)D;
+  w.count = take(4);
+  w.ray0 = take(n * 12); w.dir = take(n * 12); w.far = take(n * 4); w.depth = take(n * 4);
+  w.pts = take(n * 12); w.vdir = take(n * 12); w.pix = take(n * 4); w.gs = take(n * 16); w.gp = take(npad * 16); w.rgba = take(n * 16);
+  w.march = take(march_layout_bytes(N, n_steps, 0).total);
+  w.rec = take(c * sizeof(SampleRec));
+  for (int l = 0; l < 8; ++l) w.h[l] = take(c * d * 4);
+  w.feat = take(c * d * 4); w.hr = take(c * d / 2 * 4); w.enc = take(c * 64 * 4); w.denc = take(c * 32 * 4); w.gv = take(c * 16);
+  w.total = off;
+  return w;
+}
+size_t simt_geometry_frame_workspace(int N, int n_steps, int D) { return simt_geo_layout(N, n_steps, D).total; }
+
+// nnb_geometry_frame on this engine: geo_rays, the exact march, geo_compact, then per pass of at most GEO_PASS compacted rows the normals
+// (simt_mlp_fwd_n with the stash and simt_mlp_dgrad_n: OfficialStaticNerf.gradient's nnb_field_fwd + nnb_field_bwd with NNB_RAW_DENSITY,
+// no view directions, cotangent (0, 0, 0, 1)) and the surface colour (simt_mlp_fwd_n at (p, -dir): OfficialStaticNerf.forward's
+// nnb_field_fwd), with the row count read on the device, and geo_shade.  Passes past the hit count exit at once.  Nothing is read back.
+template <int D>
+static cudaError_t simt_geometry_frame_dim(const nnb_geometry_args& g, cudaStream_t st) {
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  const SimtGeoWs w = simt_geo_layout(g.N, g.n_steps, D);
+  char* base = static_cast<char*>(g.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  auto F4 = [&](size_t off) { return reinterpret_cast<float4*>(base + off); };
+  int* count = reinterpret_cast<int*>(base + w.count);
+  e = cudaMemsetAsync(count, 0, 4, st);
+  if (e != cudaSuccess) return e;
+  const int blocks = (g.N + 255) / 256;
+  geo_rays<<<blocks, 256, 0, st>>>(g.T, g.pixels, g.N, g.radius, F(w.ray0), F(w.dir), F(w.far), g.ray0, g.ray_dir, g.far_);
+  nnb_ray_march_args r{};
+  r.weights = g.weights; r.ray0 = F(w.ray0); r.ray_dir = F(w.dir); r.far_ = F(w.far); r.frac = g.frac;
+  r.N = g.N; r.n_steps = g.n_steps; r.n_secant = g.n_secant; r.hidden_dim = D; r.near_ = g.near_; r.tau = g.tau;
+  r.flags = g.flags; r.engine = NNB_ENGINE_SIMT; r.depth = F(w.depth);
+  r.workspace = base + w.march; r.workspace_bytes = w.rec - w.march;
+  e = simt_ray_march_dim<D>(r, st);
+  if (e != cudaSuccess) return e;
+  int* pix = reinterpret_cast<int*>(base + w.pix);
+  geo_compact<<<blocks, 256, 0, st>>>(g.N, F(w.ray0), F(w.dir), F(w.depth), count, F(w.pts), F(w.vdir), pix, F4(w.gs), g.rgb, g.rgb_surf,
+                                      g.depth, reinterpret_cast<float4*>(g.grad));
+  SimtPtrs P{};
+  P.rec = reinterpret_cast<SampleRec*>(base + w.rec);
+  for (int l = 0; l < 8; ++l) P.h[l] = F(w.h[l]);
+  P.feat = F(w.feat); P.hr = F(w.hr); P.enc = F(w.enc); P.denc = F(w.denc); P.gv = F4(w.gv);
+  nnb_render_args a{};
+  a.weights = g.weights; a.N = g.N; a.S = 1; a.hidden_dim = D; a.engine = NNB_ENGINE_SIMT;
+  const uint32_t occ_flags = g.flags & (NNB_DIST_ALPHA | NNB_SOFTPLUS);
+  const int grid = w.cap / TM;
+  for (int off = 0; off < g.N; off += w.cap) {
+    a.pts = F(w.pts) + 3 * (size_t)off; a.dirs = nullptr; a.flags = occ_flags | NNB_RAW_DENSITY | NNB_STASH;
+    P.gs = F4(w.gs) + off; P.gp = F4(w.gp) + off;
+    simt_mlp_fwd_n<D><<<grid, 256, fwd_smem<D>(), st>>>(a, P, count, off, w.cap, 1);
+    simt_mlp_dgrad_n<D><<<grid, 256, bwd_smem<D>(), st>>>(a, P, count, off, w.cap);   // d logit / d p
+    a.dirs = F(w.vdir) + 3 * (size_t)off; a.flags = occ_flags;
+    simt_mlp_fwd_n<D><<<grid, 256, fwd_smem<D>(), st>>>(a, P, count, off, w.cap, 0);   // surface colour
+    rec_to_rgba_n<<<(w.cap + 255) / 256, 256, 0, st>>>(P.rec, F4(w.rgba) + off, count, off, w.cap);
+  }
+  geo_shade<<<blocks, 256, 0, st>>>(g.T, count, pix, F4(w.gp), F4(w.rgba), g.rgb, g.rgb_surf, reinterpret_cast<float4*>(g.grad));
+  return cudaGetLastError();
+}
+cudaError_t simt_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st) {
+  return D == 128 ? simt_geometry_frame_dim<128>(g, st) : (D == 64 ? simt_geometry_frame_dim<64>(g, st) : simt_geometry_frame_dim<256>(g, st));
 }
 
 // jobs -> simt_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent

@@ -237,13 +237,23 @@ class _FieldTcFn(torch.autograd.Function):
 MARCH_BLOCK = 128   # steps one round of nnb_ray_march advances every ray that is still searching
 
 
-def ray_march(net, ray0, dirs, far, frac, near, n_secant, tau, want_bracket=False):
-    """nnb_ray_march: Renderer.ray_marching + Renderer.secant for N rays in one call on the tensor-core engine, without points or
-    occupancies in global memory.  ray0, dirs (N, 3); far (N,) per-ray far depth; frac (n_steps,) = torch.linspace(0, 1, n_steps); near,
-    tau floats.  Returns depth (N,): the refined depth on a hit, 0 where the first sample is occupied, inf otherwise; bit-identical to
-    the torch march over field_query(engine='tc', occ_only=True).  No autograd.
+def _march_engine_id(engine):
+    """the engine of ray_march / geometry_frame: 'tc' (or ENGINE_TC) or 'simt' (or ENGINE_SIMT); anything else raises ValueError"""
+    e = _engine_id(engine)
+    if e is None:
+        raise ValueError("engine must be 'simt', 'tc', ENGINE_SIMT or ENGINE_TC (got None)")
+    return e
+
+
+def ray_march(net, ray0, dirs, far, frac, near, n_secant, tau, want_bracket=False, engine='tc'):
+    """nnb_ray_march_engine: Renderer.ray_marching + Renderer.secant for N rays in one call, without points or occupancies in global memory.
+    ray0, dirs (N, 3); far (N,) per-ray far depth; frac (n_steps,) = torch.linspace(0, 1, n_steps); near, tau floats.  Returns depth (N,):
+    the refined depth on a hit, 0 where the first sample is occupied, inf otherwise.  No autograd.
+    engine: 'tc' (or ENGINE_TC, the default) = the tensor-core engine, bit-identical to the torch march over field_query(engine='tc',
+    occ_only=True); 'simt' (or ENGINE_SIMT) = the exact-fp32 engine, bit-identical to the torch march over the default field_query.
     want_bracket: returns (depth, first (N,) int32, bracket (N, 4), counts) with first / bracket as nnb_ray_march documents them and
     counts (rounds + 1,) int32 = [rays that hit, rays that took part in round 1, 2, ...] (round 0 takes every ray)."""
+    eng = _march_engine_id(engine)
     ops._need_cuda(ray0, "ray0")
     N, n_steps, dev = ray0.shape[0], frac.shape[0], ray0.device
     depth = torch.empty(N, device=dev)
@@ -256,27 +266,30 @@ def ray_march(net, ray0, dirs, far, frac, near, n_secant, tau, want_bracket=Fals
     keep = [net.flat_weights()] + [ops._f32c(t.detach()) for t in (ray0, dirs, far, frac)]
     a.weights, a.ray0, a.ray_dir, a.far_, a.frac = [L.ptr(t) for t in keep]
     a.N = N; a.n_steps = n_steps; a.n_secant = n_secant; a.hidden_dim = net.hidden_dim
-    a.near_ = near; a.tau = tau; a.flags = _field_flags(net); a.engine = L.ENGINE_TC
+    a.near_ = near; a.tau = tau; a.flags = _field_flags(net); a.engine = eng
     a.depth = L.ptr(depth); a.first = L.ptr(first); a.bracket = L.ptr(bracket)
-    ws = ops._pool.take(L.lib.nnb_ray_march_workspace_bytes(N, n_steps, net.hidden_dim), dev)
+    ws = ops._pool.take(L.lib.nnb_ray_march_workspace_bytes_engine(N, n_steps, net.hidden_dim, eng), dev)
     a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
     try:
-        L.check(L.lib.nnb_ray_march(C.byref(a), ops._stream()), "nnb_ray_march")
+        L.check(L.lib.nnb_ray_march_engine(C.byref(a), ops._stream()), "nnb_ray_march_engine")
         counts = ws[:4 * (rounds + 1)].view(torch.int32).clone() if want_bracket else None
     finally:
         ops._pool.give(ws)   # stream-ordered: the next call on this stream that takes it runs after this one
     return (depth, first, bracket, counts) if want_bracket else depth
 
 
-def geometry_frame(net, T, pixels, frac, radius, n_secant=8, tau=0.5, near=0.0, want_intermediates=False):
-    """nnb_geometry_frame: the geometry view (Renderer.phong_renderer) of N pixels in one call on the tensor-core engine, with each
-    pixel's camera ray computed on its own: ray setup, fused march (ray_march), normals (gradient(engine='tc')), shading and surface
-    colour (field_query(engine='tc')), with no host round trip.  T (4, 4) or (1, 4, 4) = S^-1 W^-1 K^-1; pixels (..., 2) image-plane
+def geometry_frame(net, T, pixels, frac, radius, n_secant=8, tau=0.5, near=0.0, want_intermediates=False, engine='tc'):
+    """nnb_geometry_frame_engine: the geometry view (Renderer.phong_renderer) of N pixels in one call, with each pixel's camera ray computed on
+    its own: ray setup, fused march (ray_march), normals (gradient()), shading and surface colour (field_query()), with no host round
+    trip.  engine: 'tc' (or ENGINE_TC, the default) = every field query on the tensor-core engine (gradient(engine='tc'),
+    field_query(engine='tc')); 'simt' (or ENGINE_SIMT) = every field query on the exact-fp32 engine, the default engine of gradient() and
+    field_query().  T (4, 4) or (1, 4, 4) = S^-1 W^-1 K^-1; pixels (..., 2) image-plane
     coordinates (N = their count); frac (n_steps,) = torch.linspace(0, 1, n_steps); radius, tau, near floats.  Returns rgb, rgb_surf
     (N, 3): the shaded view (1 where no surface is hit) and the surface colour (0 there).  A pixel's outputs do not depend on the other
     pixels of the call.  No autograd.
     want_intermediates: also returns {'ray0', 'ray_dir' (N, 3), 'far', 'depth' (N,), 'grad' (N, 3)}: the call's rays, far sphere
     depths, march depths and -d logit / d p on the object rays (0 elsewhere)."""
+    eng = _march_engine_id(engine)
     ops._need_cuda(pixels, "pixels")
     ops._need_cuda(T, "T")
     px = ops._f32c(pixels.detach().reshape(-1, 2))
@@ -291,14 +304,14 @@ def geometry_frame(net, T, pixels, frac, radius, n_secant=8, tau=0.5, near=0.0, 
         keep = [net.flat_weights(), ops._f32c(T.detach().reshape(16)), px, ops._f32c(frac.detach())]
         a.weights, a.T, a.pixels, a.frac = [L.ptr(t) for t in keep]
         a.N = N; a.n_steps = frac.shape[0]; a.n_secant = n_secant; a.hidden_dim = net.hidden_dim
-        a.near_ = near; a.tau = tau; a.radius = radius; a.flags = _field_flags(net); a.engine = L.ENGINE_TC
+        a.near_ = near; a.tau = tau; a.radius = radius; a.flags = _field_flags(net); a.engine = eng
         a.rgb = L.ptr(rgb); a.rgb_surf = L.ptr(surf)
         if inter is not None:
             a.ray0, a.ray_dir, a.far_, a.depth, a.grad = [L.ptr(inter[k]) for k in ("ray0", "ray_dir", "far", "depth", "grad")]
-        ws = ops._pool.take(L.lib.nnb_geometry_frame_workspace_bytes(N, a.n_steps, net.hidden_dim), dev)
+        ws = ops._pool.take(L.lib.nnb_geometry_frame_workspace_bytes_engine(N, a.n_steps, net.hidden_dim, eng), dev)
         a.workspace = L.ptr(ws); a.workspace_bytes = ws.numel()
         try:
-            L.check(L.lib.nnb_geometry_frame(C.byref(a), ops._stream()), "nnb_geometry_frame")
+            L.check(L.lib.nnb_geometry_frame_engine(C.byref(a), ops._stream()), "nnb_geometry_frame_engine")
         finally:
             ops._pool.give(ws)   # stream-ordered, as in ray_march
     if inter is None:

@@ -44,6 +44,15 @@ class Renderer(nn.Module):
         # computed per pixel), and Extract_Images.render_geometry / Trainer.render_visdata pass the whole frame in one call.  Its
         # frames differ from phong_renderer's in the last bits of the rays, so it is off by default.
         self.geometry_frame = kwargs.get("geometry_frame", False)
+        # engine of that frame (field.geometry_frame(engine=)): None or 'tc' = the tensor-core frame; 'simt' = the exact-fp32 frame, whose
+        # march, normals and surface colour are the default engine's bits on the frame's own rays.
+        self.geometry_frame_engine = kwargs.get("geometry_frame_engine", None)
+        if self.geometry_frame_engine is not None:
+            from ..field import _march_engine_id
+            _march_engine_id(self.geometry_frame_engine)
+        # fused_march=True: ray_marching on the exact engine (field_engine None or 'simt', no gradient needed, CUDA tensors) is one fused
+        # call (field.ray_march(engine='simt')) instead of the torch march, with the same bits.  Off by default.
+        self.fused_march = bool(kwargs.get("fused_march", False))
         # frame_t_min: None keeps Extract_Images.render_frame (and so generate_images / Eval_Images.eval_images) on nnb_render_fwd.  A
         # float t >= 0 renders those frames with ops.render_frame (nnb_render_frame: compositing fused into the tensor-core forward, a
         # workspace that does not grow with the sample count); t = 0 gives the same bits, t > 0 stops a ray once its transmittance is
@@ -211,8 +220,8 @@ class Renderer(nn.Module):
         return {'rgb': rgb_values.reshape(batch_size, -1, 3), 'normal': None, 'rgb_surf': rgb_val.reshape(batch_size, -1, 3)}
 
     def phong_frame(self, pixels, camera_mat, world_mat, scale_mat, it):
-        """phong_renderer's view and output dict in one tensor-core call for any number of pixels (field.geometry_frame), always on the
-        tensor-core engine.  Each pixel's camera ray is computed on its own, so a pixel's result does not depend on how the frame is split
+        """phong_renderer's view and output dict in one call for any number of pixels (field.geometry_frame), on the tensor-core engine,
+        or on the exact engine with geometry_frame_engine='simt'.  Each pixel's camera ray is computed on its own, so a pixel's result does not depend on how the frame is split
         into calls; it differs from phong_renderer's, whose rays come from a batched matmul over the call's pixels, in the last bits of
         the rays.  Draws the single torch.randint that ray_marching draws (n_steps = 512), so a call consumes the same random numbers."""
         batch_size, num_pixels, _ = pixels.shape
@@ -224,15 +233,17 @@ class Renderer(nn.Module):
         n_steps = int(torch.randint(512, 513, (1,)).item())
         frac = torch.linspace(0, 1, steps=n_steps, device=dev)
         self.model.eval()
+        engine = 'tc' if self.geometry_frame_engine is None else self.geometry_frame_engine
         with torch.no_grad():
-            rgb, rgb_surf = field_geometry_frame(self.model, T, pixels, frac, float(self.cfg['radius']), n_secant=8, tau=0.5, near=0.0)
+            rgb, rgb_surf = field_geometry_frame(self.model, T, pixels, frac, float(self.cfg['radius']), n_secant=8, tau=0.5, near=0.0,
+                                                 engine=engine)
         return {'rgb': rgb.reshape(batch_size, -1, 3), 'normal': None, 'rgb_surf': rgb_surf.reshape(batch_size, -1, 3)}
 
     def ray_marching(self, ray0, ray_direction, model, c=None, tau=0.5, n_steps=[128, 129], n_secant_steps=8, depth_range=[0., 2.4],
                      max_points=3500000, rad=1.0):
         """rendering.py:274-384: first sign change of (occupancy - tau) along each ray, refined by the secant method.  With
         field_engine='tc' and no gradient needed (the rule of field.field_query) the march and the secant steps are one fused call into
-        the library; it returns the bits the torch march below returns on that engine."""
+        the library; it returns the bits the torch march below returns on that engine.  So does fused_march=True on the exact engine."""
         batch_size, n_pts, _ = ray0.shape
         dev = ray0.device
         tau = 0.5
@@ -242,6 +253,12 @@ class Renderer(nn.Module):
             frac = torch.linspace(0, 1, steps=n_steps, device=dev)
             return ray_march(model, ray0.reshape(-1, 3), ray_direction.reshape(-1, 3), d_intersect.reshape(-1), frac,
                              float(depth_range[0]), n_secant_steps, tau).view(batch_size, n_pts)
+        if (self.fused_march and _engine_id(self.field_engine) in (None, L.ENGINE_SIMT) and not needs_grad(model, ray0, ray_direction)
+                and ray0.is_cuda):
+            d_intersect = self._sphere_far(ray0[:, 0], ray_direction, rad)
+            frac = torch.linspace(0, 1, steps=n_steps, device=dev)
+            return ray_march(model, ray0.reshape(-1, 3), ray_direction.reshape(-1, 3), d_intersect.reshape(-1), frac,
+                             float(depth_range[0]), n_secant_steps, tau, engine='simt').view(batch_size, n_pts)
         return self._ray_marching_torch(ray0, ray_direction, model, n_steps, n_secant_steps, depth_range, max_points, rad,
                                         self.field_engine)
 
