@@ -399,6 +399,23 @@ typedef struct nnb_frame_args {
 size_t nnb_render_frame_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim);   /* 0 on bad sizes or an unsupported width */
 int nnb_render_frame(const nnb_frame_args* f, void* stream);
 
+/* nnb_render_frame on f->fwd.engine.  NNB_ENGINE_TC is exactly nnb_render_frame.  NNB_ENGINE_SIMT renders the frame on the exact-fp32
+ * engine with the same chunk rule, outputs, flags and early ray termination, at any S from 2 to 1024: a 64-row tile holds 64 / R
+ * ray-chunks of R = min(S, 32) rows, so a ray with fewer than 32 samples takes only its own rows.  No version bump: the symbols mark the
+ * capability.
+ * On NNB_ENGINE_SIMT:
+ *   Bit-equality: at t_min = 0 every output is bit-identical to nnb_render_fwd on NNB_ENGINE_SIMT without NNB_STASH (an exact-engine
+ *   sample result does not depend on its tile or row, and the lane terms of a ray are summed in composite_fwd's order).  For any t_min, a
+ *   ray with n_eval == S has exactly the bits of the t_min = 0 call, and a ray's outputs depend on that ray alone.
+ *   Error bound for t_min > 0: the bound stated above for the tensor-core frame, unchanged.  n_eval is a multiple of 32, or S.
+ * Errors: those of nnb_render_frame in the same order, except that an engine other than NNB_ENGINE_TC and NNB_ENGINE_SIMT is the -4, S in
+ *   2..15 is accepted on NNB_ENGINE_SIMT, and the workspace is sized by nnb_render_frame_workspace_bytes_engine.
+ * Workspace: nnb_render_frame_workspace_bytes_engine(N, S, hidden_dim, engine) is nnb_render_frame_workspace_bytes on NNB_ENGINE_TC; on
+ *   NNB_ENGINE_SIMT it is that layout without the weight image, 1 360 281 856 bytes at N = 1080 x 1920 for every width and every S, where
+ *   nnb_render_fwd needs 32 N S bytes of sample records.  0 on bad sizes, an unsupported width or another engine. */
+int nnb_render_frame_engine(const nnb_frame_args* f, void* stream);
+size_t nnb_render_frame_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine);
+
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,
                  float* c2w /*[16]*/, void* stream);

@@ -17,6 +17,8 @@ size_t simt_ray_march_workspace(int N, int n_steps);
 cudaError_t simt_ray_march(const nnb_ray_march_args& r, int D, cudaStream_t st);
 size_t simt_geometry_frame_workspace(int N, int n_steps, int D);
 cudaError_t simt_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
+size_t simt_render_frame_workspace(int N);
+cudaError_t simt_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st);
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
@@ -460,21 +462,25 @@ size_t nnb_render_frame_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim
 #endif
   return 0;
 }
-int nnb_render_frame(const nnb_frame_args* f, void* stream) {
-  if (!f) return fail(-1, "null args");
+size_t nnb_render_frame_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine) {
+  if (engine == NNB_ENGINE_TC) return nnb_render_frame_workspace_bytes(N, S, hidden_dim);
+  if (engine == NNB_ENGINE_SIMT && N > 0 && S >= 2 && S <= 1024 && nnb::dim_supported(hidden_of(hidden_dim)))
+    return simt_render_frame_workspace(N);
+  return 0;
+}
+// the checks after the engine's and the call, on f->fwd.engine (NNB_ENGINE_TC or NNB_ENGINE_SIMT, validated by the caller)
+static int render_frame_on(const nnb_frame_args* f, void* stream) {
   const nnb_render_args* a = &f->fwd;
-  if (a->engine != NNB_ENGINE_TC)
-    return fail(-4, "nnb_render_frame: engine %d has no frame renderer (NNB_ENGINE_TC only; nnb_render_fwd serves the exact engine)", a->engine);
-#ifndef NNB_WITH_TC
-  return fail(-4, "library built without the tensor-core engine");
-#else
   if (int rc = check_flags(a->flags)) return rc;
   if (a->flags & (NNB_STASH | NNB_HVP | NNB_OCC_ONLY | NNB_RAW_DENSITY))
     return fail(-6, "nnb_render_frame: NNB_STASH, NNB_HVP, NNB_OCC_ONLY and NNB_RAW_DENSITY are not accepted (flags 0x%x)", a->flags);
   if (int rc = check_dim(a)) return rc;
   if (a->N <= 0) return fail(-2, "N must be positive (got %d)", a->N);
   if (a->S < 2 || a->S > 1024) return fail(-2, "S must be in [2,1024] (got %d)", a->S);
-  if (!tc_supports(a->S)) return fail(-4, "tensor-core engine needs S in [16,1024] (got %d); use nnb_render_fwd on NNB_ENGINE_SIMT", a->S);
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC && !tc_supports(a->S))
+    return fail(-4, "tensor-core engine needs S in [16,1024] (got %d); use nnb_render_fwd on NNB_ENGINE_SIMT", a->S);
+#endif
   if (a->noise || a->z_vals || a->alpha || a->pts || a->dirs)
     return fail(-6, "nnb_render_frame: noise, z_vals, alpha, pts and dirs must be NULL (no jitter, no per-sample outputs)");
   if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_frame: t_min must be >= 0 (got %g)", (double)f->t_min);
@@ -486,12 +492,37 @@ int nnb_render_frame(const nnb_frame_args* f, void* stream) {
   if (!a->rgb || !a->depth_pred || !a->depth_gt || !a->mask) return fail(-3, "output pointers must be non-null");
   if (misaligned4(f->n_eval) || misaligned4(f->t_final)) return fail(-3, "nnb_render_frame: n_eval and t_final must be 4-byte aligned");
   const int D = hidden_of(a->hidden_dim);
-  const size_t need = tc_render_frame_workspace(a->N, D);
+  const size_t need = nnb_render_frame_workspace_bytes_engine(a->N, a->S, a->hidden_dim, a->engine);
   if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
-  cudaError_t e = tc_render_frame(*a, f->t_min, f->n_eval, f->t_final, D, (cudaStream_t)stream);
-  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame");
+  cudaError_t e;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) e = tc_render_frame(*a, f->t_min, f->n_eval, f->t_final, D, (cudaStream_t)stream); else
 #endif
+  e = simt_render_frame(*a, f->t_min, f->n_eval, f->t_final, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame");
+}
+int nnb_render_frame(const nnb_frame_args* f, void* stream) {
+  if (!f) return fail(-1, "null args");
+  const nnb_render_args* a = &f->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_frame: engine %d has no frame renderer here (NNB_ENGINE_TC only; nnb_render_frame_engine runs NNB_ENGINE_SIMT)",
+                a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  return render_frame_on(f, stream);
+#endif
+}
+int nnb_render_frame_engine(const nnb_frame_args* f, void* stream) {
+  if (!f) return fail(-1, "null args");
+  const int32_t engine = f->fwd.engine;
+  if (engine != NNB_ENGINE_TC && engine != NNB_ENGINE_SIMT)
+    return fail(-4, "nnb_render_frame_engine: engine %d has no frame renderer (NNB_ENGINE_TC or NNB_ENGINE_SIMT)", engine);
+#ifndef NNB_WITH_TC
+  if (engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
+#endif
+  return render_frame_on(f, stream);
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {
   int rc = check_field(a); if (rc) return rc;

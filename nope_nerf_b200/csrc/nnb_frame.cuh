@@ -1,0 +1,106 @@
+// nnb_render_frame (the volumetric view of a frame with compositing fused into the field's forward), the parts both engines share: the
+// per-ray state of the rounds (FramePtrs), the back end of a ray-chunk (frame_step), the end of the call (frame_finish), the workspace
+// layout without the engine's own part (frame_layout_bytes) and the rounds themselves (run_render_frame).  nnb_tc.cu (tc_frame) and
+// nnb_simt.cu (simt_frame) supply the field evaluations.
+//
+// Round k evaluates samples 32 k .. 32 k + 31 of every ray still live and composites them into per-ray lane partials in the workspace; a
+// ray whose transmittance fell below t_min, or that has no chunk left, leaves; frame_finish writes the outputs.
+#pragma once
+#include "nnb_workspace.cuh"
+
+namespace {
+
+struct FramePtrs {
+  int k;               // this round evaluates samples 32 k .. 32 k + 31 of its rays
+  float t_min;
+  const int* list;     // the rays of this round (NULL in round 0: every ray, ray-chunk = ray)
+  const int* count;    // device count of `list` (NULL: a.N)
+  int *next_list, *next_count;   // rays still live after this round
+  float* carry;        // [N] transmittance after the ray's last evaluated chunk
+  int* chunks;         // [N] chunks the ray evaluated (written when it leaves)
+  float* part;         // [N][5][32] lane partials C0, C1, C2, Dist, acc of composite_chunk
+};
+constexpr int FRAME_MAX_ROUNDS = 32;   // S <= 1024
+
+// Back end of a frame tile, one warp per ray-chunk: composite_fwd's chunk step on the chunk's (r, g, b, a) rows (s_rows, one float4 per
+// row; lane i reads row i, lanes past the ray's last sample are invalid), continued from the ray's carry and lane partials of the rounds
+// before.  The ray leaves when its carry is below t_min or it has no chunk left; otherwise it is appended to the next round's list.
+__device__ __forceinline__ void frame_step(const nnb_render_args& a, const FramePtrs& f, int slot, int n_live, const unsigned char* s_rows,
+                                           int lane) {
+  if (slot >= n_live) return;
+  const int n = f.list ? f.list[slot] : slot;
+  const int i = 32 * f.k + lane;
+  const bool valid = i < a.S;
+  float4 me = make_float4(0.f, 0.f, 0.f, 0.f);
+  float z = 0.f, alpha = 0.f;
+  if (valid) {
+    me = *reinterpret_cast<const float4*>(s_rows + lane * 16);
+    z = sample_z(a, n, i);
+    alpha = composite_alpha(a, i, me.w, z, [&] { return sample_z(a, n, i + 1); });
+  }
+  float* part = f.part + (size_t)n * 160 + lane;
+  float carry = 1.f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dist = 0.f, acc = 0.f;
+  if (f.k > 0) { carry = f.carry[n]; C0 = part[0]; C1 = part[32]; C2 = part[64]; Dist = part[96]; acc = part[128]; }
+  composite_chunk(alpha, valid, me.x, me.y, me.z, z, lane, carry, C0, C1, C2, Dist, acc);
+  part[0] = C0; part[32] = C1; part[64] = C2; part[96] = Dist; part[128] = acc;
+  if (lane == 0) {
+    f.carry[n] = carry;
+    if (carry < f.t_min || 32 * (f.k + 1) >= a.S) f.chunks[n] = f.k + 1;
+    else f.next_list[atomicAdd(f.next_count, 1)] = n;
+  }
+}
+
+// one warp per ray after the last round: composite_fwd's tail on the ray's lane partials, n_eval and t_final
+__global__ void frame_finish(nnb_render_args a, const __grid_constant__ FramePtrs f, int* __restrict__ n_eval, float* __restrict__ t_final) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  Ray ray; setup_ray(a, n, ray);
+  const float* part = f.part + (size_t)n * 160 + lane;
+  composite_tail(a, n, ray, part[0], part[32], part[64], part[96], part[128], lane);
+  if (lane == 0) {
+    if (n_eval) n_eval[n] = min(32 * f.chunks[n], a.S);
+    if (t_final) t_final[n] = f.carry[n];
+  }
+}
+
+// Workspace of nnb_render_frame, every section 256-byte aligned: counters [FRAME_MAX_ROUNDS + 1] (k >= 1: rays of round k) | carry,
+// chunks [N] | lane partials [N][5][32] | the two ray lists that alternate between rounds [N] | the engine's own part (img_bytes: the
+// tensor-core engine's forward weight image; none on the exact engine).  S does not enter.
+struct FrameWs { size_t carry, chunks, part, list[2], img, total; };
+inline FrameWs frame_layout_bytes(int N, size_t img_bytes) {
+  FrameWs w{};
+  size_t off = align_up((size_t)(FRAME_MAX_ROUNDS + 1) * 4, 256);
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  const size_t n = (size_t)N;
+  w.carry = take(n * 4); w.chunks = take(n * 4); w.part = take(n * 640); w.list[0] = take(n * 4); w.list[1] = take(n * 4);
+  w.img = img_bytes ? take(img_bytes) : off;
+  w.total = off;
+  return w;
+}
+
+// The rounds of nnb_render_frame on either engine: round(f) launches one round (chunk f.k of the rays of f.list, of every ray when it is
+// NULL; round k takes its rays from the list round k - 1 appended to), then frame_finish.  Every launch after the first sizes itself from
+// a device counter; nothing is read back.
+template <class Round>
+cudaError_t run_render_frame(const nnb_render_args& a, const FrameWs& w, float t_min, int* n_eval, float* t_final, cudaStream_t st,
+                             Round round) {
+  char* base = static_cast<char*>(a.workspace);
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  int* counters = I(0);
+  cudaError_t e = cudaMemsetAsync(counters, 0, (FRAME_MAX_ROUNDS + 1) * 4, st);
+  if (e != cudaSuccess) return e;
+  FramePtrs f{};
+  f.t_min = t_min;
+  f.carry = reinterpret_cast<float*>(base + w.carry); f.chunks = I(w.chunks); f.part = reinterpret_cast<float*>(base + w.part);
+  const int rounds = (a.S + 31) / 32;
+  for (int k = 0; k < rounds; ++k) {
+    f.k = k;
+    f.list = k > 0 ? I(w.list[k & 1]) : nullptr; f.count = k > 0 ? counters + k : nullptr;
+    f.next_list = I(w.list[(k + 1) & 1]); f.next_count = counters + k + 1;   // not written by the last round
+    round(f);
+  }
+  frame_finish<<<(a.N + 7) / 8, 256, 0, st>>>(a, f, n_eval, t_final);
+  return cudaGetLastError();
+}
+
+}  // namespace

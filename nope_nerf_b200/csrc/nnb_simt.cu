@@ -11,6 +11,7 @@
 //   B4 ray_bwd          : per-ray geometry adjoint -> d c2w, d K, d depth, d scale/shift
 #include "nnb_tc_common.cuh"   // mbarrier / bulk-copy wrappers (head_wgrad)
 #include "nnb_march.cuh"
+#include "nnb_frame.cuh"
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -152,18 +153,32 @@ __device__ __forceinline__ void row_geometry(const nnb_render_args& a, size_t m,
 // colour branch is skipped and the density head's occupancy - tau goes to the march's back end instead of a record.
 //   SF_MARCH: row r is step 128 q.block + 64 pass + r of ray `mray` (clamped to its last step); the value goes to s_val[64 pass + r].
 //   SF_SECANT: row r is the secant iterate of hit ray q.list[m0 + r] (rows past M: the point 0, ignored); pass = the secant pass.
-enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2 };
+// SF_FRAME (simt_frame, nnb_render_frame on this engine): SF_RAYS on the rows frame_row gives (M = N S), with nothing stashed and no
+// record.  The colour head puts each row's (r, g, b, a) in a row area at the start of oth, and the CTA's warps take the tile's
+// ray-chunks in turn through frame_step (nnb_frame.cuh).  fr / n_live: the round and its ray-chunk count.
+enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2, SF_FRAME = 3 };
+
+// Row `row` of frame tile `tile`: a ray-chunk is R = min(S, 32) rows and a tile holds 64 / R of them, so row r is sample 32 fr.k + r % R
+// of the ray in slot (64 / R) tile + r / R of the round.  Slots past the round's last repeat it, rows past a ray's last sample evaluate
+// that sample, and the rows past the tile's last whole ray-chunk (64 % R of them) evaluate some sample; frame_step reads none of them.
+__device__ __forceinline__ size_t frame_row(const nnb_render_args& a, const FramePtrs& fr, unsigned tile, int row, int n_live) {
+  const int R = min(a.S, 32);
+  const int slot = min((TM / R) * (int)tile + row / R, n_live - 1);
+  const int n = fr.list ? fr.list[slot] : slot;
+  return (size_t)n * a.S + min(32 * fr.k + row % R, a.S - 1);
+}
 
 // one 64-row tile of the exact forward: rows m0 = 64 tile .. m0 + 63 of M
 template <int D, int MODE>
 __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int stash, unsigned tile, const MarchPtrs& q,
-                                              int mray, int pass, float* s_val) {
+                                              int mray, int pass, float* s_val, const FramePtrs& fr = FramePtrs{}, int n_live = 0) {
   constexpr int LDB = ldb<D>(), NJ = D / 64, NJR = D >= 128 ? D / 128 : 1;   // output column blocks of the trunk / rgb hidden layers
   extern __shared__ __align__(16) float smem[];
   float* buf0 = smem; float* buf1 = buf0 + TM * LDB; float* Ws = buf1 + TM * LDB;
   const int tid = threadIdx.x;
   const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
+  auto row_m = [&](int row) { return MODE == SF_FRAME ? frame_row(a, fr, tile, row, n_live) : m0 + row; };
   {  // prologue: encode positions into columns D..D+63 of both buffers
     int row = tid & 63, part = tid >> 6;
     Ray ray; int n, i; float z, p[3];
@@ -176,7 +191,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
         march_point(q, r, secant_depth((pass == 0 ? q.brk0 : q.brk1)[r]), p);
       }
     } else {
-      row_geometry(a, m0 + row, M, ray, n, i, z, p);
+      row_geometry(a, row_m(row), M, ray, n, i, z, p);
     }
     float* e0 = buf0 + row * LDB + D; float* e1 = buf1 + row * LDB + D;
     if (part == 0) {
@@ -223,7 +238,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
     acc += __shfl_xor_sync(0xffffffffu, acc, 2);
     s_logit = acc + __ldg(w + nnb::B_SIG(D));
   }
-  if constexpr (MODE != SF_RAYS) {   // occupancy only: the colour branch does not enter the march
+  if constexpr (MODE == SF_MARCH || MODE == SF_SECANT) {   // occupancy only: the colour branch does not enter the march
     if (hc == 0) {
       float sigma;
       auto f = [&] { return __fsub_rn(density_act(s_logit, a.flags, &sigma), q.tau); };
@@ -236,8 +251,8 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
   tile_gemm<NJ, false, 0, false>(cur, LDB, D, w + nnb::W_FEAT(D), D, D, D, w + nnb::B_FEAT(D), oth, LDB, Ws);
   if (tid < TM) {
     Ray ray; int n, i; float z, p[3], v[3];
-    row_geometry(a, m0 + tid, M, ray, n, i, z, p);
-    row_view_dir(a, m0 + tid, M, ray, v);
+    row_geometry(a, row_m(tid), M, ray, n, i, z, p);
+    row_view_dir(a, row_m(tid), M, ray, v);
     float* de = oth + tid * LDB + D;
     encode<4>(v, [&](int k, float val) { de[k] = val; });
 #pragma unroll
@@ -264,14 +279,25 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
       for (int k = 0; k < D / 2; ++k) acc = fmaf(hr_[k], __ldg(wc + k), acc);
       val = sigmoid_f(acc + __ldg(w + nnb::B_RGB(D) + hc));
     }
-    float* rec = reinterpret_cast<float*>(P.rec + m0 + hrow);
-    if (hc < 3) rec[hc] = val;
-    else {
-      Ray ray; int n, i; float z, p[3], sigma;
-      row_geometry(a, m0 + hrow, M, ray, n, i, z, p);
-      rec[3] = density_act(s_logit, a.flags, &sigma);
-      rec[4] = s_logit; rec[5] = z; rec[6] = 0.f; rec[7] = 0.f;
+    if constexpr (MODE == SF_FRAME) {   // row area: (r, g, b, a) of row hrow; oth was last read by the rgb hidden layer
+      float sigma;
+      oth[hrow * 4 + hc] = hc < 3 ? val : density_act(s_logit, a.flags, &sigma);
+    } else {
+      float* rec = reinterpret_cast<float*>(P.rec + m0 + hrow);
+      if (hc < 3) rec[hc] = val;
+      else {
+        Ray ray; int n, i; float z, p[3], sigma;
+        row_geometry(a, m0 + hrow, M, ray, n, i, z, p);
+        rec[3] = density_act(s_logit, a.flags, &sigma);
+        rec[4] = s_logit; rec[5] = z; rec[6] = 0.f; rec[7] = 0.f;
+      }
     }
+  }
+  if constexpr (MODE == SF_FRAME) {
+    __syncthreads();   // every row is in the row area
+    const int R = min(a.S, 32), per = TM / R;
+    for (int c = tid >> 5; c < per; c += 8)
+      frame_step(a, fr, per * (int)tile + c, n_live, reinterpret_cast<const unsigned char*>(oth + c * R * 4), tid & 31);
   }
 }
 
@@ -318,6 +344,18 @@ __global__ void __launch_bounds__(256, 1) simt_secant(nnb_render_args a, const _
       simt_fwd_tile<D, SF_SECANT>(a, SimtPtrs{}, M, 0, tile, q, 0, pass, nullptr);
       __syncthreads();
     }
+}
+
+// one round of nnb_render_frame on this engine: chunk f.k of every ray of f.list (of every ray when f.list is NULL), 64 / min(S, 32)
+// ray-chunks per 64-row tile; the ray-chunk count is read when the kernel starts
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_frame(nnb_render_args a, const __grid_constant__ FramePtrs f) {
+  const int n_live = f.count ? *f.count : a.N, per = TM / min(a.S, 32);
+  const unsigned n_tiles = (unsigned)((n_live + per - 1) / per);
+  for (unsigned tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    simt_fwd_tile<D, SF_FRAME>(a, SimtPtrs{}, (size_t)a.N * a.S, 0, tile, MarchPtrs{}, 0, 0, nullptr, f, n_live);
+    __syncthreads();   // the back end is done with the row area before the next tile's prologue writes the buffers
+  }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -968,6 +1006,7 @@ static cudaError_t simt_init_dim() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_mlp_dgrad_n<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_march<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_secant<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -1182,6 +1221,33 @@ static cudaError_t simt_geometry_frame_dim(const nnb_geometry_args& g, cudaStrea
 }
 cudaError_t simt_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st) {
   return D == 128 ? simt_geometry_frame_dim<128>(g, st) : (D == 64 ? simt_geometry_frame_dim<64>(g, st) : simt_geometry_frame_dim<256>(g, st));
+}
+
+// ---- nnb_render_frame on this engine: run_render_frame (nnb_frame.cuh) with one simt_frame round per 32-sample chunk, a persistent grid
+// of every CTA the SMs hold.  A sample's (r, g, b, a) is simt_mlp_fwd's (the exact forward does not depend on the tile or row that
+// evaluates it) and frame_step sums the lane terms in composite_fwd's order, so at t_min = 0 the outputs are nnb_render_fwd's bits.
+size_t simt_render_frame_workspace(int N) { return frame_layout_bytes(N, 0).total; }
+
+template <int D>
+static cudaError_t simt_render_frame_dim(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, cudaStream_t st) {
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  static int slots = 0;   // CTAs of simt_frame resident on the device at once
+  if (!slots) {
+    int dev = 0, n_sm = 0, per_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, simt_frame<D>, 256, fwd_smem<D>());
+    if (e != cudaSuccess) return e;
+    slots = n_sm * (per_sm > 0 ? per_sm : 1);
+  }
+  const int per = TM / (a.S < 32 ? a.S : 32), tiles = (a.N + per - 1) / per, grid = tiles < slots ? tiles : slots;
+  return run_render_frame(a, frame_layout_bytes(a.N, 0), t_min, n_eval, t_final, st,
+                          [&](const FramePtrs& f) { simt_frame<D><<<grid, 256, fwd_smem<D>(), st>>>(a, f); });
+}
+cudaError_t simt_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st) {
+  return D == 128 ? simt_render_frame_dim<128>(a, t_min, n_eval, t_final, st)
+       : D == 64  ? simt_render_frame_dim<64>(a, t_min, n_eval, t_final, st) : simt_render_frame_dim<256>(a, t_min, n_eval, t_final, st);
 }
 
 // jobs -> simt_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent

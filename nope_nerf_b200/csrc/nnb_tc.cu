@@ -36,6 +36,7 @@
 // LBO = rows * 16 B between the two k-halves of one MMA.
 #include "nnb_tc_common.cuh"
 #include "nnb_march.cuh"
+#include "nnb_frame.cuh"
 #include <cuda.h>            // CUtensorMap (types only: the driver entry point is obtained at run time)
 #include <cudaTypedefs.h>    // PFN_cuTensorMapEncodeTiled
 
@@ -207,55 +208,13 @@ __device__ __forceinline__ float quad_sum(float v) {
 // (origin, direction, depth) and a back end that reduces the tile's occupancies instead of writing them (nnb_march.cuh) ----
 static_assert(TILE == MARCH_BLOCK, "a march tile is one block of a ray's steps");
 
-// nnb_render_frame (the volumetric view of a frame, tc_frame): rounds of 32-sample chunks.  Round k evaluates chunk k of every ray still
-// live; a tile is 4 ray-chunks x 32 rows, composited in the tile's back end (frame_step) into per-ray lane partials in the workspace
-// (FramePtrs); a ray whose transmittance fell below t_min, or that has no chunk left, leaves; frame_finish writes the outputs.
-struct FramePtrs {
-  int k;               // this round evaluates samples 32 k .. 32 k + 31 of its rays
-  float t_min;
-  const int* list;     // the rays of this round (NULL in round 0: every ray, ray-chunk = ray)
-  const int* count;    // device count of `list` (NULL: a.N)
-  int *next_list, *next_count;   // rays still live after this round
-  float* carry;        // [N] transmittance after the ray's last evaluated chunk
-  int* chunks;         // [N] chunks the ray evaluated (written when it leaves)
-  float* part;         // [N][5][32] lane partials C0, C1, C2, Dist, acc of composite_chunk
-};
-constexpr int FRAME_MAX_ROUNDS = 32;   // S <= 1024
-
+// nnb_render_frame (tc_frame): a tile is 4 ray-chunks x 32 rows, composited by frame_step (nnb_frame.cuh) in the tile's back end.
 // workspace row of tile row `row` of a frame tile: sample i = 32 k + row % 32 of ray list[4 tile + row / 32].  Ray-chunks past the end of
 // the list repeat its last ray and rows past the ray's last sample evaluate that sample; frame_step ignores both.
 __device__ __forceinline__ size_t frame_sample(const nnb_render_args& a, const FramePtrs& f, int tile, int row, int n_live) {
   const int slot = min(4 * tile + row / 32, n_live - 1);
   const int n = f.list ? f.list[slot] : slot;
   return (size_t)n * a.S + min(32 * f.k + row % 32, a.S - 1);
-}
-
-// Back end of a frame tile, one warp per ray-chunk: composite_fwd's chunk step on the chunk's (r, g, b, a) rows (s_rows, one float4 per
-// row), continued from the ray's carry and lane partials of the rounds before.  The ray leaves when its carry is below t_min or it has no
-// chunk left; otherwise it is appended to the next round's list.
-__device__ __forceinline__ void frame_step(const nnb_render_args& a, const FramePtrs& f, int slot, int n_live, const unsigned char* s_rows,
-                                           int lane) {
-  if (slot >= n_live) return;
-  const int n = f.list ? f.list[slot] : slot;
-  const int i = 32 * f.k + lane;
-  const bool valid = i < a.S;
-  float4 me = make_float4(0.f, 0.f, 0.f, 0.f);
-  float z = 0.f, alpha = 0.f;
-  if (valid) {
-    me = *reinterpret_cast<const float4*>(s_rows + lane * 16);
-    z = sample_z(a, n, i);
-    alpha = composite_alpha(a, i, me.w, z, [&] { return sample_z(a, n, i + 1); });
-  }
-  float* part = f.part + (size_t)n * 160 + lane;
-  float carry = 1.f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dist = 0.f, acc = 0.f;
-  if (f.k > 0) { carry = f.carry[n]; C0 = part[0]; C1 = part[32]; C2 = part[64]; Dist = part[96]; acc = part[128]; }
-  composite_chunk(alpha, valid, me.x, me.y, me.z, z, lane, carry, C0, C1, C2, Dist, acc);
-  part[0] = C0; part[32] = C1; part[64] = C2; part[96] = Dist; part[128] = acc;
-  if (lane == 0) {
-    f.carry[n] = carry;
-    if (carry < f.t_min || 32 * (f.k + 1) >= a.S) f.chunks[n] = f.k + 1;
-    else f.next_list[atomicAdd(f.next_count, 1)] = n;
-  }
 }
 
 // MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
@@ -730,19 +689,6 @@ template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_frame(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                          const __grid_constant__ FramePtrs f) {
   tc_fwd_body<D, FWD_FRAME>(a, wimg, nullptr, nullptr, TcStash{}, MarchPtrs{}, (size_t)a.N * a.S, 0, 0, f);
-}
-
-// one warp per ray after the last round: composite_fwd's tail on the ray's lane partials, n_eval and t_final
-__global__ void frame_finish(nnb_render_args a, const __grid_constant__ FramePtrs f, int* __restrict__ n_eval, float* __restrict__ t_final) {
-  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (n >= a.N) return;
-  Ray ray; setup_ray(a, n, ray);
-  const float* part = f.part + (size_t)n * 160 + lane;
-  composite_tail(a, n, ray, part[0], part[32], part[64], part[96], part[128], lane);
-  if (lane == 0) {
-    if (n_eval) n_eval[n] = min(32 * f.chunks[n], a.S);
-    if (t_final) t_final[n] = f.carry[n];
-  }
 }
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
@@ -1913,22 +1859,7 @@ cudaError_t tc_geometry_frame_dim(const nnb_geometry_args& g, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-// Workspace of nnb_render_frame, every section 256-byte aligned: counters [FRAME_MAX_ROUNDS + 1] (k >= 1: rays of round k) | carry,
-// chunks [N] | lane partials [N][5][32] | the two ray lists that alternate between rounds [N] | the forward weight image
-struct FrameWs { size_t carry, chunks, part, list[2], img, total; };
-template <int D> FrameWs frame_layout(int N) {
-  FrameWs w{};
-  size_t off = align_up((size_t)(FRAME_MAX_ROUNDS + 1) * 4, 256);
-  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
-  const size_t n = (size_t)N;
-  w.carry = take(n * 4); w.chunks = take(n * 4); w.part = take(n * 640); w.list[0] = take(n * 4); w.list[1] = take(n * 4);
-  w.img = take(Tc<D>::IMG_BYTES);
-  w.total = off;
-  return w;
-}
-
-// nnb_render_frame: weight image once, one tc_frame launch per 32-sample chunk (round k takes its rays from the list round k - 1 appended
-// to), frame_finish.  Every launch after the first sizes itself from a device counter; nothing is read back.
+// nnb_render_frame: weight image once, then run_render_frame (nnb_frame.cuh) with one tc_frame launch per 32-sample chunk
 template <int D>
 cudaError_t tc_render_frame_dim(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, cudaStream_t st) {
   using T = Tc<D>;
@@ -1943,27 +1874,12 @@ cudaError_t tc_render_frame_dim(const nnb_render_args& a, float t_min, int* n_ev
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     attr = true;
   }
-  const FrameWs w = frame_layout<D>(a.N);
-  char* base = static_cast<char*>(a.workspace);
-  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
-  int* counters = I(0);
-  e = cudaMemsetAsync(counters, 0, (FRAME_MAX_ROUNDS + 1) * 4, st);
-  if (e != cudaSuccess) return e;
-  unsigned char* img = reinterpret_cast<unsigned char*>(base + w.img);
+  const FrameWs w = frame_layout_bytes(a.N, T::IMG_BYTES);
+  unsigned char* img = static_cast<unsigned char*>(a.workspace) + w.img;
   tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);
-  FramePtrs f{};
-  f.t_min = t_min;
-  f.carry = reinterpret_cast<float*>(base + w.carry); f.chunks = I(w.chunks); f.part = reinterpret_cast<float*>(base + w.part);
-  const int rounds = (a.S + 31) / 32, tiles = (a.N + 3) / 4;
-  const int grid = tiles < n_sm ? tiles : n_sm;
-  for (int k = 0; k < rounds; ++k) {
-    f.k = k;
-    f.list = k > 0 ? I(w.list[k & 1]) : nullptr; f.count = k > 0 ? counters + k : nullptr;
-    f.next_list = I(w.list[(k + 1) & 1]); f.next_count = counters + k + 1;   // not written by the last round
-    tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f);
-  }
-  frame_finish<<<(a.N + 7) / 8, 256, 0, st>>>(a, f, n_eval, t_final);
-  return cudaGetLastError();
+  const int tiles = (a.N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm;
+  return run_render_frame(a, w, t_min, n_eval, t_final, st,
+                          [&](const FramePtrs& f) { tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f); });
 }
 
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
@@ -2023,7 +1939,7 @@ cudaError_t tc_field_hvp(const nnb_render_args& a, const float* u, float* g_pts,
 }
 
 size_t tc_render_frame_workspace(int N, int D) {
-  return D == 128 ? frame_layout<128>(N).total : (D == 64 ? frame_layout<64>(N).total : frame_layout<256>(N).total);
+  return frame_layout_bytes(N, D == 128 ? Tc<128>::IMG_BYTES : (D == 64 ? Tc<64>::IMG_BYTES : Tc<256>::IMG_BYTES)).total;
 }
 cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st) {
   return D == 128 ? tc_render_frame_dim<128>(a, t_min, n_eval, t_final, st)

@@ -22,7 +22,8 @@ class Extract_Images(object):
     def render_frame(self, c2w, camera_mat, h, w, rows=None):
         """rgb (rows,w,3) and z-depth (rows,w) of one view; eval mode, no jitter, prior depth = 1
         (extracting_images.py:52-77).  rows=(r0,r1) renders a row block (multi-GPU sharding of one frame).  With
-        Renderer(frame_t_min=t) on the tensor-core engine the frame is one ops.render_frame call (nnb_render_frame) instead."""
+        Renderer(frame_t_min=t) on the tensor-core engine the frame is one ops.render_frame call (nnb_render_frame) instead, and with
+        Renderer(frame_t_min=t, frame_engine='simt') one ops.render_frame_engine call on the exact-fp32 engine at any engine and S."""
         rend = self.renderer
         net = rend.model
         r0, r1 = (0, h) if rows is None else rows
@@ -37,6 +38,9 @@ class Extract_Images(object):
                   near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
                   ray_idx=ray_idx, depth_map=torch.ones(1, 1, device=dev), H=h, W=w, stash=False, hidden_dim=net.hidden_dim)
         t_min = getattr(rend, 'frame_t_min', None)
+        if t_min is not None and getattr(rend, 'frame_engine', None) == 'simt':   # Renderer(frame_engine='simt'): the exact frame
+            rgb, depth_pred = ops.render_frame_engine(*args, t_min=t_min, **dict(kw, engine=L.ENGINE_SIMT))[:2]
+            return rgb.view(r1 - r0, w, 3), depth_pred.view(r1 - r0, w)
         if t_min is not None and ops.pick_engine(engine, S) == L.ENGINE_TC:   # Renderer(frame_t_min=t): the fused frame renderer
             rgb, depth_pred = ops.render_frame(*args, t_min=t_min, **kw)[:2]
             return rgb.view(r1 - r0, w, 3), depth_pred.view(r1 - r0, w)

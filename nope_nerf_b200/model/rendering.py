@@ -57,11 +57,21 @@ class Renderer(nn.Module):
         # float t >= 0 renders those frames with ops.render_frame (nnb_render_frame: compositing fused into the tensor-core forward, a
         # workspace that does not grow with the sample count); t = 0 gives the same bits, t > 0 stops a ray once its transmittance is
         # below t (bounded error, see the header).  Tensor-core engine only: with the SIMT engine (an explicit engine, or fewer than 16
-        # samples per ray) the frame takes the nnb_render_fwd path as before.  Trainer.render_visdata does not use it.
+        # samples per ray) the frame takes the nnb_render_fwd path as before, unless frame_engine='simt' (below) is given too.
+        # Trainer.render_visdata does not use it.
         t_min = kwargs.get("frame_t_min", None)
         if t_min is not None and not float(t_min) >= 0.0:
             raise ValueError("frame_t_min must be None or a float >= 0 (got %r)" % (t_min,))
         self.frame_t_min = None if t_min is None else float(t_min)
+        # frame_engine: None keeps the routing above.  'simt' renders those frames with ops.render_frame_engine on the exact-fp32 engine
+        # (nnb_render_frame_engine: the same fused frame, at any sample count from 2 to 1024; t = 0 gives nnb_render_fwd's exact-engine
+        # bits) whatever `engine` says; it needs frame_t_min, without which it would do nothing.  'tc' is the default routing.
+        frame_engine = kwargs.get("frame_engine", None)
+        if frame_engine not in (None, 'tc', 'simt'):
+            raise ValueError("frame_engine must be None, 'tc' or 'simt' (got %r)" % (frame_engine,))
+        if frame_engine == 'simt' and self.frame_t_min is None:
+            raise ValueError("frame_engine='simt' needs frame_t_min (a float >= 0)")
+        self.frame_engine = frame_engine
 
     def to(self, device):
         model = super().to(device)

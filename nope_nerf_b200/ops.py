@@ -153,6 +153,29 @@ def render_frame(weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=N
     32-sample chunk that leaves its transmittance below t_min (the error bound is in include/nope_nerf_b200.h).
     Returns (rgb, depth_pred, depth_gt, mask), and (n_eval, t_final) after them with want_stats.  noise, want_z_alpha and stash are
     RenderCall's arguments and are rejected here, as is an engine other than the tensor-core engine (no fall-back)."""
+    return _render_frame(L.lib.nnb_render_frame, "nnb_render_frame", L.lib.nnb_render_frame_workspace_bytes(N, S, int(hidden_dim)),
+                         L.ENGINE_TC if engine is None else engine, weights, c2w, cam, N=N, S=S, flags=flags, near=near, far=far,
+                         ray_idx=ray_idx, pixels=pixels, depth=depth, depth_map=depth_map, scale=scale, shift=shift, noise=noise, H=H, W=W,
+                         want_z_alpha=want_z_alpha, stash=stash, hidden_dim=hidden_dim, t_min=t_min, want_stats=want_stats)
+
+
+def render_frame_engine(weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None, depth_map=None,
+                        scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256, t_min=0.0,
+                        want_stats=False):
+    """nnb_render_frame_engine: render_frame on either engine.  engine=None resolves through pick_engine (so S < 16 runs on the exact
+    engine); ENGINE_TC gives render_frame's bits; ENGINE_SIMT renders on the exact-fp32 engine at any S from 2 to 1024, and at t_min = 0
+    gives the bits of RenderCall(engine=ENGINE_SIMT, stash=False)."""
+    engine = pick_engine(engine, S)
+    return _render_frame(L.lib.nnb_render_frame_engine, "nnb_render_frame_engine",
+                         L.lib.nnb_render_frame_workspace_bytes_engine(N, S, int(hidden_dim), engine), engine, weights, c2w, cam, N=N, S=S,
+                         flags=flags, near=near, far=far, ray_idx=ray_idx, pixels=pixels, depth=depth, depth_map=depth_map, scale=scale,
+                         shift=shift, noise=noise, H=H, W=W, want_z_alpha=want_z_alpha, stash=stash, hidden_dim=hidden_dim, t_min=t_min,
+                         want_stats=want_stats)
+
+
+def _render_frame(fn, name, nbytes, engine, weights, c2w, cam, *, N, S, flags, near, far, ray_idx, pixels, depth, depth_map, scale, shift,
+                  noise, H, W, want_z_alpha, stash, hidden_dim, t_min, want_stats):
+    """the body of render_frame / render_frame_engine: fn is the C entry point, nbytes its workspace size (0: the call rejects it)"""
     if noise is not None or want_z_alpha or stash:
         raise ValueError("render_frame: noise, want_z_alpha and stash are not supported (inference without jitter)")
     for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels),
@@ -168,18 +191,17 @@ def render_frame(weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=N
     if depth_map is not None:
         a.h_d, a.w_d = depth_map.shape[-2], depth_map.shape[-1]
     a.near_, a.far_ = float(near), float(far)
-    a.flags = flags; a.engine = L.ENGINE_TC if engine is None else engine; a.hidden_dim = int(hidden_dim)
+    a.flags = flags; a.engine = engine; a.hidden_dim = int(hidden_dim)
     rgb = torch.empty(N, 3, device=dev); depth_pred = torch.empty(N, device=dev)
     depth_gt = torch.empty(N, device=dev); mask = torch.empty(N, dtype=torch.uint8, device=dev)
     a.rgb = L.ptr(rgb); a.depth_pred = L.ptr(depth_pred); a.depth_gt = L.ptr(depth_gt); a.mask = L.ptr(mask)
     n_eval = torch.empty(N, dtype=torch.int32, device=dev) if want_stats else None
     t_final = torch.empty(N, device=dev) if want_stats else None
     f.t_min = float(t_min); f.n_eval = L.ptr(n_eval); f.t_final = L.ptr(t_final)
-    nbytes = L.lib.nnb_render_frame_workspace_bytes(N, S, int(hidden_dim))
     ws = _pool.take(nbytes, dev) if nbytes else None
     a.workspace = L.ptr(ws); a.workspace_bytes = 0 if ws is None else ws.numel()
     try:
-        L.check(L.lib.nnb_render_frame(C.byref(f), _stream()), "nnb_render_frame")
+        L.check(fn(C.byref(f), _stream()), name)
     finally:
         if ws is not None:
             _pool.give(ws)
