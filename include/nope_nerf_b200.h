@@ -416,6 +416,31 @@ int nnb_render_frame(const nnb_frame_args* f, void* stream);
 int nnb_render_frame_engine(const nnb_frame_args* f, void* stream);
 size_t nnb_render_frame_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine);
 
+/* The differentiable frame on the tensor-core engine: what nnb_render_fwd (NNB_STASH) + nnb_render_bwd compute, at t_min = 0 and without
+ * jitter, in a workspace whose only part that grows with S is one float per ray and 32-sample chunk.  No version bump: the symbols mark
+ * the capability.
+ *   b->fwd: the inputs of nnb_render_frame with its flags (NNB_STASH is rejected: nothing is kept between calls), engine NNB_ENGINE_TC,
+ *   the workspace sized by nnb_render_frame_bwd_workspace_bytes.  The call runs the forward again and writes rgb, depth_pred, depth_gt and
+ *   mask: bit-identical to nnb_render_fwd on NNB_ENGINE_TC with the same arguments.  The gradient fields of b are those of
+ *   nnb_render_bwd, with its rules: g_weights (NULL: no MLP gradient), g_c2w, g_cam, g_scale_shift ACCUMULATED, g_depth overwritten.
+ * Method: the forward stores each ray's transmittance after every chunk but the last.  Then, for each chunk from the last to the first,
+ *   the chunk of every ray is evaluated again with a training stash of 32 N rows, its compositing adjoint runs with the suffix of the
+ *   later chunks carried in, then the data-gradient chain and the weight-gradient stage of nnb_render_bwd, whose reduce adds the
+ *   chunk's dW / db into g_weights.  The chunks' point and direction adjoints are summed per ray, chunk by chunk, and the pose adjoint
+ *   follows as in nnb_render_bwd.
+ * Reproducible: every sum runs in a fixed order (no float atomics but the one add per element of g_c2w, g_cam and g_scale_shift), so the
+ *   same inputs give the same bits on every run, whatever the workspace held.  Against nnb_render_fwd + nnb_render_bwd the gradients
+ *   differ in the order of their sums only (the weight gradients are summed chunk by chunk, the ray sums from the last chunk).
+ * Errors, with nothing launched: b == NULL (rc -1); an engine other than NNB_ENGINE_TC (-4); then nnb_render_frame's checks and codes
+ *   without t_min, n_eval and t_final; a NULL g_rgb or g_c2w (-3); a workspace smaller than nnb_render_frame_bwd_workspace_bytes(N, S,
+ *   hidden_dim) or not 256-byte aligned (-5).
+ * Workspace, each section 256-byte aligned: nnb_render_frame's workspace | the transmittance checkpoints (4 N (ceil(S / 32) - 1) bytes) |
+ *   suffix carries (4 N) | per-ray lane partials of the pose adjoint (1152 N) | nnb_workspace_bytes_dim(N, 32, NNB_STASH, NNB_ENGINE_TC,
+ *   hidden_dim) without its weight images (the chunk stash of 32 N rows) | the transposed weight image.  About 650 KB per ray at D = 256.
+ *   nnb_render_frame_bwd_workspace_bytes: 0 on bad sizes (N <= 0, S outside 16..1024) or an unsupported width. */
+size_t nnb_render_frame_bwd_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim);
+int nnb_render_frame_bwd(const nnb_render_bwd_args* b, void* stream);
+
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,
                  float* c2w /*[16]*/, void* stream);

@@ -37,6 +37,8 @@ cudaError_t tc_field_hvp(const nnb_render_args& a, const float* u, float* g_pts,
 size_t tc_geometry_frame_workspace(int N, int n_steps, int D);
 size_t tc_render_frame_workspace(int N, int D);
 cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st);
+size_t tc_render_frame_bwd_workspace(int N, int S, int D);
+cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
@@ -468,9 +470,8 @@ size_t nnb_render_frame_workspace_bytes_engine(int32_t N, int32_t S, int32_t hid
     return simt_render_frame_workspace(N);
   return 0;
 }
-// the checks after the engine's and the call, on f->fwd.engine (NNB_ENGINE_TC or NNB_ENGINE_SIMT, validated by the caller)
-static int render_frame_on(const nnb_frame_args* f, void* stream) {
-  const nnb_render_args* a = &f->fwd;
+// the checks of the frame's render arguments after the engine's, in nnb_render_frame's order up to the output pointers
+static int check_frame(const nnb_render_args* a) {
   if (int rc = check_flags(a->flags)) return rc;
   if (a->flags & (NNB_STASH | NNB_HVP | NNB_OCC_ONLY | NNB_RAW_DENSITY))
     return fail(-6, "nnb_render_frame: NNB_STASH, NNB_HVP, NNB_OCC_ONLY and NNB_RAW_DENSITY are not accepted (flags 0x%x)", a->flags);
@@ -483,13 +484,24 @@ static int render_frame_on(const nnb_frame_args* f, void* stream) {
 #endif
   if (a->noise || a->z_vals || a->alpha || a->pts || a->dirs)
     return fail(-6, "nnb_render_frame: noise, z_vals, alpha, pts and dirs must be NULL (no jitter, no per-sample outputs)");
-  if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_frame: t_min must be >= 0 (got %g)", (double)f->t_min);
+  return 0;
+}
+// the render arguments' checks after the t_min check
+static int check_frame_io(const nnb_render_args* a) {
   if (!a->weights || !a->c2w || !a->cam) return fail(-3, "weights / c2w / cam must be non-null");
   if (!a->ray_idx && !a->pixels) return fail(-3, "need ray_idx or pixels");
   if (!a->pixels && (a->H < 2 || a->W < 2)) return fail(-3, "H,W needed to derive pixels from ray_idx");
   if (!a->depth && !(a->depth_map && a->ray_idx && a->h_d > 0 && a->w_d > 0 && a->H > 0 && a->W > 0))
     return fail(-3, "need depth[N] or (depth_map,h_d,w_d,H,W,ray_idx)");
   if (!a->rgb || !a->depth_pred || !a->depth_gt || !a->mask) return fail(-3, "output pointers must be non-null");
+  return 0;
+}
+// the checks after the engine's and the call, on f->fwd.engine (NNB_ENGINE_TC or NNB_ENGINE_SIMT, validated by the caller)
+static int render_frame_on(const nnb_frame_args* f, void* stream) {
+  const nnb_render_args* a = &f->fwd;
+  if (int rc = check_frame(a)) return rc;
+  if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_frame: t_min must be >= 0 (got %g)", (double)f->t_min);
+  if (int rc = check_frame_io(a)) return rc;
   if (misaligned4(f->n_eval) || misaligned4(f->t_final)) return fail(-3, "nnb_render_frame: n_eval and t_final must be 4-byte aligned");
   const int D = hidden_of(a->hidden_dim);
   const size_t need = nnb_render_frame_workspace_bytes_engine(a->N, a->S, a->hidden_dim, a->engine);
@@ -523,6 +535,32 @@ int nnb_render_frame_engine(const nnb_frame_args* f, void* stream) {
   if (engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
 #endif
   return render_frame_on(f, stream);
+}
+size_t nnb_render_frame_bwd_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && tc_supports(S) && nnb::dim_supported(D)) return tc_render_frame_bwd_workspace(N, S, D);
+#endif
+  return 0;
+}
+int nnb_render_frame_bwd(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_frame_bwd: engine %d has no differentiable frame (NNB_ENGINE_TC only)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_frame(a)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_frame_bwd: g_rgb and g_c2w must be non-null");
+  const int D = hidden_of(a->hidden_dim);
+  const size_t need = nnb_render_frame_bwd_workspace_bytes(a->N, a->S, a->hidden_dim);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  const cudaError_t e = tc_render_frame_bwd(*b, D, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_bwd");
+#endif
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {
   int rc = check_field(a); if (rc) return rc;

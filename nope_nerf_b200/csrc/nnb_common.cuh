@@ -253,3 +253,113 @@ __device__ __forceinline__ void composite_tail(const nnb_render_args& a, int n, 
     a.depth_pred[n] = Dist; a.depth_gt[n] = g; a.mask[n] = ray.mask ? 1 : 0;
   }
 }
+
+// ---- the per-ray geometry adjoint (SURVEY.md A.6) of ray_bwd, from the ray's sums over its samples of the point adjoint (so), the
+// depth-weighted point adjoint (sd) and the view-direction adjoint (sv): red[0..8] d R, [9..11] d t, [12,13] d kx, ky, [14,15] d scale, shift
+// -> rayred[n][16], and b.g_depth[n]: the statements of ray_bwd's lane-0 block, for the differentiable frame (frame_ray_finish,
+// nnb_frame.cuh).  ray_bwd keeps its own copy: nvcc 12.9 schedules ray_bwd differently when it calls this, and its SASS is kept as it was.
+__device__ __forceinline__ void ray_adjoint(const nnb_render_bwd_args& b, int n, const Ray& r, const float so[3], const float sd[3],
+                                            const float sv[3], float* rayred) {
+  const nnb_render_args& a = b.fwd;
+  float red[16];
+#pragma unroll
+  for (int k = 0; k < 16; ++k) red[k] = 0.f;
+  const bool normalise = a.flags & NNB_NORMALISE, ev = (a.flags & NNB_EVAL) && normalise;
+  float g_nrm = 0.f;
+  float gDo = b.g_depth_pred ? __ldg(b.g_depth_pred + n) : 0.f;
+  float g_g = b.g_depth_gt ? __ldg(b.g_depth_gt + n) : 0.f;
+  float gcur = ev ? r.g / r.nrm : r.g;
+  if (a.flags & NNB_NDC) g_g = g_g / (gcur * gcur);
+  if (ev) {
+    float Dist = a.depth_pred[n] * r.nrm;  // stored output is Dist / nrm
+    g_nrm -= gDo * Dist / (r.nrm * r.nrm);
+    g_nrm -= g_g * r.g / (r.nrm * r.nrm);
+    g_g = g_g / r.nrm;
+  }
+  float g_gdepth;
+  if (normalise) { g_gdepth = g_g * r.nrm; g_nrm += g_g * fabsf(r.depth); } else g_gdepth = g_g;
+  float g_depth = g_gdepth * (r.depth > 0.f ? 1.f : (r.depth < 0.f ? -1.f : 0.f));
+  float g_o[3], g_d[3], g_kx = 0.f, g_ky = 0.f;
+  if (a.flags & NNB_NDC) {
+    const float* d = r.d; const float* o2 = r.o2;
+    float ox = o2[0] / o2[2], oy = o2[1] / o2[2];
+    float gO[3] = {so[0], so[1], so[2]}, gDn[3] = {sd[0], sd[1], sd[2]};
+    float g_Oz = gO[2] - gDn[2];
+    float g_ox = -r.kx * gO[0] + r.kx * gDn[0];
+    float g_oy = -r.ky * gO[1] + r.ky * gDn[1];
+    g_d[0] = -r.kx * gDn[0] / d[2];
+    g_d[1] = -r.ky * gDn[1] / d[2];
+    g_d[2] = (r.kx * gDn[0] * d[0] + r.ky * gDn[1] * d[1]) / (d[2] * d[2]);
+    g_kx = -ox * gO[0] - (d[0] / d[2] - ox) * gDn[0];
+    g_ky = -oy * gO[1] - (d[1] / d[2] - oy) * gDn[1];
+    float g_o2[3];
+    g_o2[0] = g_ox / o2[2]; g_o2[1] = g_oy / o2[2];
+    g_o2[2] = -(g_ox * ox + g_oy * oy) / o2[2] - 2.f * g_Oz / (o2[2] * o2[2]);
+    float g_tau = g_o2[0] * d[0] + g_o2[1] * d[1] + g_o2[2] * d[2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { g_o[c] = g_o2[c]; g_d[c] += g_o2[c] * r.tau; }
+    g_o[2] += -g_tau / d[2];
+    g_d[2] += g_tau * (1.f + r.t[2]) / (d[2] * d[2]);
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { g_o[c] = so[c]; g_d[c] = sd[c]; }
+  }
+  if (a.flags & NNB_USE_DIR) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g_d[c] -= sv[c];
+  }
+  float g_dt[3];
+  if (normalise) {
+    float dot = r.d[0] * g_d[0] + r.d[1] * g_d[1] + r.d[2] * g_d[2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g_dt[c] = (g_d[c] - r.d[c] * dot) / r.nrm;
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g_dt[c] = g_d[c];
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) g_dt[c] += (g_nrm / r.nrm) * r.dt[c];
+  // g_R[a][b] = g_dt[a] * dc[b]; g_t = g_o
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+#pragma unroll
+    for (int j = 0; j < 3; ++j) red[3 * i + j] = g_dt[i] * r.dc[j];
+    red[9 + i] = g_o[i];
+  }
+  float g_dc0 = g_dt[0] * r.R[0] + g_dt[1] * r.R[3] + g_dt[2] * r.R[6];
+  float g_dc1 = g_dt[0] * r.R[1] + g_dt[1] * r.R[4] + g_dt[2] * r.R[7];
+  g_kx += g_dc0 * (-r.x / (r.kx * r.kx));
+  g_ky += g_dc1 * (-r.y / (r.ky * r.ky));
+  red[12] = g_kx; red[13] = g_ky;
+  if (b.g_depth) b.g_depth[n] = g_depth;
+  if (!a.depth) {  // depth = raw*scale + shift  |  (raw + shift)*scale
+    float sc = ld_scalar(a.scale, 1.f), sf = ld_scalar(a.shift, 0.f);
+    if (a.flags & NNB_SHIFT_FIRST) { red[14] = g_depth * (r.depth_raw + sf); red[15] = g_depth * sc; }
+    else { red[14] = g_depth * r.depth_raw; red[15] = g_depth; }
+  }
+#pragma unroll
+  for (int k = 0; k < 16; ++k) rayred[(size_t)n * 16 + k] = red[k];
+}
+
+// ---- the compositing adjoint of one 32-sample chunk of a ray (the differentiable frame, nnb_render_frame_bwd): the statements of
+// composite_bwd's reverse sweep for chunk c, in the same order, from the transmittance `carry` into the chunk instead of composite_bwd's
+// forward sweep (the frame's forward stores it with the bits that sweep has).  composite_bwd keeps its own copy so that its SASS is kept as
+// it was.  carry_s is the suffix sum of w gw over the later chunks on entry, and includes this chunk on return; it is carried from chunk to
+// chunk and never formed as total - prefix (DESIGN.md §4).  df = d alpha / d a.  Returns (w gC0, w gC1, w gC2, d L / d a) of the lane's
+// sample, zeros for an invalid lane.
+__device__ __forceinline__ float4 composite_chunk_bwd(float alpha, bool valid, float r, float g, float b, float z, float df, int lane, float carry,
+                                                      float gC0, float gC1, float gC2, float gD, float gsum, float& carry_s) {
+  const float om = valid ? __fadd_rn(__fsub_rn(1.f, alpha), NNB_EPS) : 1.f;
+  const float incl_p = warp_incl_prod(om, lane);
+  float excl_p = __shfl_up_sync(0xffffffffu, incl_p, 1); if (lane == 0) excl_p = 1.f;
+  const float T = carry * excl_p;
+  const float w = alpha * T;
+  const float gw = fmaf(gD, z, fmaf(gC2, b, fmaf(gC1, g, gC0 * r))) - gsum;
+  const float wg = valid ? w * gw : 0.f;
+  const float incl = warp_incl_sum_rev(wg, lane);
+  float excl = __shfl_down_sync(0xffffffffu, incl, 1); if (lane == 31) excl = 0.f;
+  const float suffix = excl + carry_s;
+  carry_s += __shfl_sync(0xffffffffu, incl, 0);
+  const float g_alpha = T * gw - suffix / om;
+  return valid ? make_float4(w * gC0, w * gC1, w * gC2, g_alpha * df) : make_float4(0.f, 0.f, 0.f, 0.f);
+}

@@ -103,4 +103,100 @@ cudaError_t run_render_frame(const nnb_render_args& a, const FrameWs& w, float t
   return cudaGetLastError();
 }
 
+
+// ---- nnb_render_frame_bwd (the differentiable frame, t_min = 0, tensor-core engine): the forward above with checkpoints, then reverse
+// rounds k = C - 1 .. 0 (C = ceil(S / 32)).  Round k evaluates chunk k of every ray again with a chunk-sized training stash (ray n's chunk
+// is rows 32 n .. 32 n + 31 of it), runs frame_chunk_adjoint, the data-gradient chain and the weight-gradient stage on it, and adds the
+// chunk's point and direction adjoints to the ray's lane partials (frame_ray_acc).  frame_ray_finish then forms each ray's pose adjoint
+// from them as ray_bwd does.  Every sum runs in a fixed order: chunk by chunk from the last, in the lanes of composite_bwd / ray_bwd.
+struct FrameBwdPtrs {
+  int k, rounds;          // this round's chunk; C
+  const float* ckpt;      // [C - 1][N]: transmittance into chunk k + 1 (after chunk k) of every ray, written by the forward
+  float* suffix;          // [N] carry_s of composite_chunk_bwd between rounds
+  const SampleRec* rec;   // [32 N] records of the chunk (the chunk stash)
+  float4* gs;             // [32 N] d / d (rgb, a) of the chunk's samples
+  const float4 *gp, *gv;  // [32 N] d / d p and d / d viewdir of the chunk's samples
+  float* raypart;         // [N][9][32] lane partials of ray_bwd's so, sd, sv
+};
+
+// one warp per ray, lane = sample 32 k + lane: composite_bwd's adjoint of chunk k, the suffix of the later chunks carried in f.suffix
+__global__ void frame_chunk_adjoint(nnb_render_bwd_args b, const __grid_constant__ FrameBwdPtrs f) {
+  const nnb_render_args& a = b.fwd;
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  Ray ray; setup_ray(a, n, ray);
+  float gD = b.g_depth_pred ? __ldg(b.g_depth_pred + n) : 0.f;
+  if ((a.flags & NNB_EVAL) && (a.flags & NNB_NORMALISE)) gD = gD / ray.nrm;
+  const float gC0 = __ldg(b.g_rgb + 3 * n), gC1 = __ldg(b.g_rgb + 3 * n + 1), gC2 = __ldg(b.g_rgb + 3 * n + 2);
+  const float gsum = (a.flags & NNB_WHITE_BG) ? (gC0 + gC1 + gC2) : 0.f;
+  const int i = 32 * f.k + lane;
+  const bool valid = i < a.S;
+  const size_t m = (size_t)n * 32 + lane;
+  const SampleRec me = valid ? f.rec[m] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
+  float alpha = 0.f, df = 1.f;   // df = d alpha / d a
+  if (valid) {
+    alpha = composite_alpha(a, i, me.a, me.z, [&] { return sample_z(a, n, i + 1); });
+    if (a.flags & NNB_DIST_ALPHA) {
+      if (i >= a.S - 1) df = 0.f;
+      else { const float delta = __fsub_rn(sample_z(a, n, i + 1), me.z); df = delta * expf(-me.a * delta); }
+    }
+  }
+  const float carry = f.k > 0 ? f.ckpt[(size_t)(f.k - 1) * a.N + n] : 1.f;
+  float carry_s = f.k == f.rounds - 1 ? 0.f : f.suffix[n];
+  f.gs[m] = composite_chunk_bwd(alpha, valid, me.r, me.g, me.b, me.z, df, lane, carry, gC0, gC1, gC2, gD, gsum, carry_s);
+  if (lane == 0) f.suffix[n] = carry_s;
+}
+
+// one warp per ray: the chunk's terms of ray_bwd's lane sums (lane = sample 32 k + lane), added to the ray's lane partials (written by the
+// first round, k = C - 1)
+__global__ void frame_ray_acc(nnb_render_args a, const __grid_constant__ FrameBwdPtrs f) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  float* part = f.raypart + (size_t)n * 288 + lane;
+  float v[9];
+#pragma unroll
+  for (int c = 0; c < 9; ++c) v[c] = f.k == f.rounds - 1 ? 0.f : part[32 * c];
+  if (32 * f.k + lane < a.S) {
+    const size_t m = (size_t)n * 32 + lane;
+    const float4 g = f.gp[m], dv = f.gv[m];
+    const float z = f.rec[m].z;
+    v[0] += g.x; v[1] += g.y; v[2] += g.z;
+    v[3] += z * g.x; v[4] += z * g.y; v[5] += z * g.z;
+    v[6] += dv.x; v[7] += dv.y; v[8] += dv.z;
+  }
+#pragma unroll
+  for (int c = 0; c < 9; ++c) part[32 * c] = v[c];
+}
+
+// one warp per ray after the last round: ray_bwd's warp sums of the lane partials and its per-ray adjoint -> rayred [N][16] (ray_reduce
+// follows)
+__global__ void frame_ray_finish(nnb_render_bwd_args b, const float* __restrict__ raypart, float* __restrict__ rayred) {
+  const nnb_render_args& a = b.fwd;
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  Ray r; setup_ray(a, n, r);
+  const float* part = raypart + (size_t)n * 288 + lane;
+  float so[3], sd[3], sv[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) { so[c] = warp_sum(part[32 * c]); sd[c] = warp_sum(part[32 * (3 + c)]); sv[c] = warp_sum(part[32 * (6 + c)]); }
+  if (lane == 0) ray_adjoint(b, n, r, so, sd, sv, rayred);
+}
+
+// Workspace of nnb_render_frame_bwd, every section 256-byte aligned: frame_layout_bytes(N, img_bytes) (the forward, with the engine's forward
+// weight image) | checkpoints [C - 1][N] | suffix carries [N] | ray lane partials [N][9][32] | the chunk stash (chunk_bytes: the records,
+// training stash, gate bits, per-ray reduction and weight-gradient partials of 32 N samples) | the engine's transposed weight image.  Only
+// the checkpoints grow with S: 4 bytes per ray and chunk.
+struct FrameBwdWs { FrameWs f; size_t ckpt, suffix, raypart, chunk, img_t, total; };
+inline FrameBwdWs frame_bwd_layout_bytes(int N, int S, size_t img_bytes, size_t chunk_bytes, size_t img_t_bytes) {
+  FrameBwdWs w{};
+  w.f = frame_layout_bytes(N, img_bytes);
+  size_t off = w.f.total;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  const size_t n = (size_t)N;
+  w.ckpt = take((size_t)((S + 31) / 32 - 1) * n * 4); w.suffix = take(n * 4); w.raypart = take(n * 288 * 4);
+  w.chunk = take(chunk_bytes); w.img_t = take(img_t_bytes);
+  w.total = off;
+  return w;
+}
+
 }  // namespace

@@ -1353,6 +1353,12 @@ cudaError_t simt_wgrad_stage(const nnb_render_args& a, const WsLayout& L, float*
   return simt_wgrad_all(make_ptrs(L, a.workspace), L, gw, st);
 }
 
+// ray_reduce of rayred [N][16] into b's pose, camera and scale / shift gradients (nnb_render_frame_bwd)
+cudaError_t launch_ray_reduce(const nnb_render_bwd_args& b, const float* rayred, cudaStream_t st) {
+  ray_reduce<<<1, 512, 0, st>>>(b, rayred);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_wgrad_reduce(const RedJob* jobs, int njobs, const float* part, cudaStream_t st) {
   RedJobs J{};
   J.njobs = njobs < 16 ? njobs : 16;

@@ -42,6 +42,7 @@
 
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st);
 cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
+cudaError_t launch_ray_reduce(const nnb_render_bwd_args& b, const float* rayred, cudaStream_t st);
 cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st);
 
 void nnb_prof_mark(cudaStream_t st);
@@ -216,6 +217,18 @@ __device__ __forceinline__ size_t frame_sample(const nnb_render_args& a, const F
   const int n = f.list ? f.list[slot] : slot;
   return (size_t)n * a.S + min(32 * f.k + row % 32, a.S - 1);
 }
+// nnb_render_frame_bwd (tc_frame_stash, tc_dgrad_frame): (ray, sample) of row m of chunk k's stash (row 32 n + j: sample 32 k + j of ray n;
+// rows past the last ray take its last ray, rows past the ray's last sample that sample; their cotangent is zero).  32-bit: m < 32 N + 128.
+__device__ __forceinline__ int2 chunk_sample(const nnb_render_args& a, int k, size_t m) {
+  return make_int2(min((int)(m >> 5), a.N - 1), min(32 * k + (int)(m & 31), a.S - 1));
+}
+// row_geometry_tc of that sample
+__device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, size_t m, Ray& ray, float& z, float p[3]) {
+  const int2 ni = chunk_sample(a, k, m);
+  setup_ray(a, ni.x, ray);
+  z = sample_z(a, ni.x, ni.y);
+  sample_point(a, ray, z, p);
+}
 
 // MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
 // out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is stashed and recs is not written.  M = a.N there, so point indices
@@ -232,6 +245,9 @@ __device__ __forceinline__ size_t frame_sample(const nnb_render_args& a, const F
 // FWD_FRAME (tc_frame): FWD_RAYS on the rows frame_sample gives (M = N S), with ray-chunks of 32 rows in place of whole rays in the per-ray
 // bias; nothing is stashed.  The colour head puts each row's (r, g, b, a) in this warpgroup's rows of the E operand (last read by layer
 // 4) and frame_step composites them.  n_tiles is read from *fr.count (ray-chunks, 4 per tile) when the kernel starts, as in FWD_MARCH.
+// FWD_CHUNK (tc_frame_stash, nnb_render_frame_bwd): FWD_RAYS with the training stash on the rows of chunk fr.k of every ray (M = 32 N,
+// row m is sample chunk_sample(a, fr.k, m) of its ray), with ray-chunks of 32 rows in place of whole rays in the per-ray bias as in FWD_FRAME; records,
+// stash and gate bits are indexed by the row.
 // FWD_GRAD (tc_points_grad_fwd, nnb_field_grad): FWD_VJP that also writes the fp32 training stash st of every row of every tile (rows
 // past M hold the last point's values): h0..h7, feat, hr and enc as FWD_RAYS does, and denc per point (the direction encoding of
 // a.dirs[m], or of the ones), which is a per-row operand of rgb_layers.0 here.  With NNB_OCC_ONLY the colour part (feat, hr, denc) is not
@@ -242,18 +258,19 @@ __device__ __forceinline__ size_t frame_sample(const nnb_render_args& a, const F
 // instead of a ReLU, and the tile ends after layer 7.  Operands are bf16 hi | lo (wimg is the bf16 image of the occupancy-only stages),
 // because tangents span the range of gradients.  e' and h'0..h'7 of every row of every tile go to st.enc / st.h with the stash's
 // streaming stores; nothing else is written.
-enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5, FWD_GRAD = 6, FWD_TANGENT = 7 };
+enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5, FWD_GRAD = 6, FWD_TANGENT = 7,
+             FWD_CHUNK = 8 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
                                             int stash, const FramePtrs& fr = FramePtrs{}) {
   using T = Tc<D>;
-  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD, TAN = MODE == FWD_TANGENT;
-  constexpr bool PTS = MODE != FWD_RAYS && !FRAME, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP || GRAD;
+  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD, TAN = MODE == FWD_TANGENT, CHUNK = MODE == FWD_CHUNK;
+  constexpr bool PTS = MODE != FWD_RAYS && !FRAME && !CHUNK, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP || GRAD;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
   static_assert(!DEVN || XPTS, "a device count of explicit points");
   if constexpr ((PTS && !GRAD && !TAN) || FRAME) stash = 0;
-  if constexpr (GRAD || TAN) stash = 1;
+  if constexpr (GRAD || TAN || CHUNK) stash = 1;
   int n_live = 0;   // FWD_FRAME: ray-chunks of this round
   if constexpr (FRAME) {
     n_live = fr.count ? *fr.count : a.N;
@@ -347,10 +364,10 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
     // where it is used, not held across the MMAs.
     auto ray_off = [&]() { return (int)((mt + (size_t)wg * 64) % (size_t)a.S); };
     // rows per ray of the per-ray bias: a frame tile's ray-chunks take the place of rays
-    auto ray_len = [&]() { return FRAME ? 32 : a.S; };
+    auto ray_len = [&]() { return FRAME || CHUNK ? 32 : a.S; };
     wg_sync();   // the previous tile's epilogue (a frame tile: its frame_step) is done with the per-ray bias buffer and E
     {
-      const int off0 = PTS || FRAME ? 0 : ray_off();
+      const int off0 = PTS || FRAME || CHUNK ? 0 : ray_off();
       // ---- prologue: thread (row rl, part) writes encoding columns [32 part, 32 part + 32) of its row ----
       const int rl = tl & 63, part = tl >> 6, row = wg * 64 + rl;
       const size_t m = FRAME ? frame_sample(a, fr, tile, row, n_live) : mt + row;
@@ -372,7 +389,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
 #pragma unroll
         for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + (size_t)mm * 3 + c);
       } else {
-        row_geometry_tc(a, m, M, ray, z, p);
+        if constexpr (CHUNK) chunk_geometry(a, fr.k, m, ray, z, p);
+        else row_geometry_tc(a, m, M, ray, z, p);
       }
       float ee[64];
       if constexpr (TAN) {   // e' = J_enc(p) u, rounded as simt_field_tangent rounds it
@@ -554,7 +572,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         // rgb hidden layer (D/2 columns) -> colour head + per-sample record
         float c_acc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
         uint32_t gw[D / 128 > 0 ? D / 128 : 1] = {};
-        const int off0 = PTS || FRAME ? 0 : ray_off();
+        const int off0 = PTS || FRAME || CHUNK ? 0 : ray_off();
 #pragma unroll
         for (int j = 0; j < DR / 8; ++j) {
           const int col = j * 8 + c0;
@@ -592,6 +610,11 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
               if (mp < (uint32_t)M) out[mp] = make_float4(rec.r, rec.g, rec.b, rec.a);
             } else if constexpr (FRAME) {   // E row r0 + 8 r, k-octet 0: this warpgroup's rows of E
               *reinterpret_cast<float4*>(smem + SM_EHI + (r0 + 8 * r) * 16) = make_float4(rec.r, rec.g, rec.b, rec.a);
+            } else if constexpr (CHUNK) {
+              const int2 ni = chunk_sample(a, fr.k, m);
+              rec.z = sample_z(a, ni.x, ni.y);
+              rec.pad0 = 0.f; rec.pad1 = 0.f;
+              recs[m] = rec;
             } else {
               rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
               rec.pad0 = 0.f; rec.pad1 = 0.f;
@@ -689,6 +712,13 @@ template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_frame(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                          const __grid_constant__ FramePtrs f) {
   tc_fwd_body<D, FWD_FRAME>(a, wimg, nullptr, nullptr, TcStash{}, MarchPtrs{}, (size_t)a.N * a.S, 0, 0, f);
+}
+// one reverse round of nnb_render_frame_bwd: chunk f.k of every ray with records, the training stash and gate bits (n_tiles = ceil(N / 4))
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_frame_stash(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                               SampleRec* __restrict__ recs, const __grid_constant__ TcStash st,
+                                                               const __grid_constant__ FramePtrs f, int n_tiles) {
+  tc_fwd_body<D, FWD_CHUNK>(a, wimg, recs, nullptr, st, MarchPtrs{}, (size_t)a.N * 32, n_tiles, 1, f);
 }
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
@@ -1101,13 +1131,15 @@ __device__ __forceinline__ void dg_gemm(float* acc, uint32_t a_hi, uint32_t a_lo
 // not read for it) and, in place of the first-order d p, the second-order point term of the tangent s' = u . d s / d p: from the
 // encoding adjoint delta_enc and p, -u_c sum_l f^2 (delta_sin sin(f p_c) + delta_cos cos(f p_c)), f = 2^l, with u = P.gs[m].  P.gp may be
 // NULL (no point term is stored).
-enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4, DG_POINTS_HVP_OCC = 5 };
+// DG_FRAME (tc_dgrad_frame, nnb_render_frame_bwd): DG_RAYS on the rows of chunk `chunk` of every ray (M = 32 N, row m is sample
+// chunk_sample(a, chunk, m)), the workspace arrays indexed by the row as tc_frame_stash wrote them.
+enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4, DG_POINTS_HVP_OCC = 5, DG_FRAME = 6 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
-                                              int n_tiles, int write_dy, const int* count = nullptr) {
+                                              int n_tiles, int write_dy, const int* count = nullptr, int chunk = 0) {
   using T = Tc<D>;
-  constexpr bool HVP = MODE == DG_POINTS_HVP_OCC;
-  constexpr bool PTS = MODE != DG_RAYS, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC || HVP;
+  constexpr bool HVP = MODE == DG_POINTS_HVP_OCC, CHUNK = MODE == DG_FRAME;
+  constexpr bool PTS = MODE != DG_RAYS && !CHUNK, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC || HVP;
   constexpr bool GRAD = MODE == DG_POINTS_GRAD || MODE == DG_POINTS_GRAD_OCC || HVP;
   static_assert(!DEVN || (PTS && !GRAD), "a device count of explicit points");
   if constexpr (PTS) write_dy = GRAD ? 1 : 0;
@@ -1278,7 +1310,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
 #pragma unroll
           for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
         } else {
-          row_geometry_tc(a, m, M, ray, z, p);
+          if constexpr (CHUNK) chunk_geometry(a, chunk, m, ray, z, p);
+          else row_geometry_tc(a, m, M, ray, z, p);
           if (a.pts) {
 #pragma unroll
             for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
@@ -1312,6 +1345,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
         const size_t mm = m < M ? m : M - 1;
 #pragma unroll
         for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + 3 * mm + c);
+      } else if constexpr (CHUNK) {
+        chunk_geometry(a, chunk, m, ray, z, p);
       } else {
         row_geometry_tc(a, m, M, ray, z, p);
       }
@@ -1346,6 +1381,12 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad(nnb_render_args a, cons
                                                          const __grid_constant__ DgPtrs P, size_t M,
                                                          int n_tiles, int write_dy) {
   tc_dgrad_body<D, DG_RAYS>(a, wimg, P, M, n_tiles, write_dy);
+}
+// the chain of one reverse round of nnb_render_frame_bwd on chunk k's stash (M = 32 N)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad_frame(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                               const __grid_constant__ DgPtrs P, size_t M, int n_tiles, int write_dy, int k) {
+  tc_dgrad_body<D, DG_FRAME>(a, wimg, P, M, n_tiles, write_dy, nullptr, k);
 }
 
 // nnb_field_vjp: the forward of explicit points with records and gate bits (FWD_VJP), then the chain on them (DG_POINTS[_OCC])
@@ -1882,6 +1923,88 @@ cudaError_t tc_render_frame_dim(const nnb_render_args& a, float t_min, int* n_ev
                           [&](const FramePtrs& f) { tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f); });
 }
 
+// Workspace of nnb_render_frame_bwd: frame_bwd_layout_bytes (nnb_frame.cuh) with this engine's forward weight image, the chunk stash
+// make_layout(N, 32, NNB_STASH, NNB_ENGINE_TC, D) (32 N rows) and the transposed weight image
+template <int D> FrameBwdWs frame_bwd_layout(int N, int S) {
+  return frame_bwd_layout_bytes(N, S, Tc<D>::IMG_BYTES, make_layout(N, 32, NNB_STASH, NNB_ENGINE_TC, D).total, Tc<D>::IMG_T_BYTES);
+}
+
+// nnb_render_frame_bwd: both weight images; the forward (run_render_frame at t_min = 0, so every ray runs every round) with the carry
+// after each chunk copied to the checkpoints; then the reverse rounds k = C - 1 .. 0, each on the chunk stash: tc_frame_stash,
+// frame_chunk_adjoint, tc_dgrad_frame, (g_weights) the weight-gradient stage, whose reduce adds the round's dW into g_weights, and
+// frame_ray_acc; then frame_ray_finish and ray_reduce.  The rounds run one after another on the stream.
+template <int D>
+cudaError_t tc_render_frame_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+  using T = Tc<D>;
+  const nnb_render_args& a = b.fwd;
+  cudaError_t e = upload_stage_table<D>();
+  if (e == cudaSuccess) e = upload_stage_table_t<D>();
+  if (e != cudaSuccess) return e;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    e = cudaFuncSetAttribute(tc_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_frame_stash<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_dgrad_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (e != cudaSuccess) return e;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  const int N = a.N, C = (a.S + 31) / 32;
+  const FrameBwdWs w = frame_bwd_layout<D>(N, a.S);
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  unsigned char *img = reinterpret_cast<unsigned char*>(base + w.f.img), *img_t = reinterpret_cast<unsigned char*>(base + w.img_t);
+  tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);
+  tc_prep_weights_t<D><<<T::N_STAGES_T, 256, 0, st>>>(a.weights, img_t);
+  const int tiles = (N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm;   // 4 ray-chunks of 32 rows per tile, forward and reverse
+  float* ckpt = F(w.ckpt);
+  cudaError_t ec = cudaSuccess;
+  e = run_render_frame(a, w.f, 0.f, nullptr, nullptr, st, [&](const FramePtrs& f) {
+    tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f);
+    if (f.k + 1 < C && ec == cudaSuccess) ec = cudaMemcpyAsync(ckpt + (size_t)f.k * N, f.carry, (size_t)N * 4, cudaMemcpyDeviceToDevice, st);
+  });
+  if (e == cudaSuccess) e = ec;
+  if (e != cudaSuccess) return e;
+  // the chunk stash: make_layout's offsets from its own base
+  nnb_render_args ac = a;
+  ac.workspace = base + w.chunk; ac.workspace_bytes = w.img_t - w.chunk;
+  const WsLayout L = make_layout(N, 32, NNB_STASH, NNB_ENGINE_TC, D);
+  char* cb = base + w.chunk;
+  auto CF = [&](size_t off) { return reinterpret_cast<float*>(cb + off); };
+  SampleRec* recs = reinterpret_cast<SampleRec*>(cb + L.rec);
+  TcStash ts{};
+  for (int l = 0; l < 8; ++l) ts.h[l] = CF(L.h[l]);
+  ts.feat = CF(L.feat); ts.hr = CF(L.hr); ts.enc = CF(L.enc); ts.denc = CF(L.denc); ts.gates = reinterpret_cast<unsigned char*>(cb + L.gates);
+  DgPtrs P{};
+  P.rec = recs; P.gates = ts.gates;
+  P.gs = reinterpret_cast<const float4*>(cb + L.gs); P.gp = reinterpret_cast<float4*>(cb + L.gp); P.gv = reinterpret_cast<float4*>(cb + L.gv);
+  P.dyc = reinterpret_cast<float4*>(cb + L.dyc);
+  for (int l = 0; l < 8; ++l) P.dy[l] = CF(L.dy[l]);
+  P.dfeat = CF(L.dfeat); P.dyr = CF(L.dyr);
+  FrameBwdPtrs fb{};
+  fb.rounds = C; fb.ckpt = ckpt; fb.suffix = F(w.suffix); fb.rec = recs;
+  fb.gs = reinterpret_cast<float4*>(cb + L.gs); fb.gp = P.gp; fb.gv = P.gv; fb.raypart = F(w.raypart);
+  const int write_dy = b.g_weights ? 1 : 0, warps = (N + 7) / 8;
+  for (int k = C - 1; k >= 0; --k) {
+    FramePtrs f{};
+    f.k = k;
+    fb.k = k;
+    tc_frame_stash<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, ts, f, tiles);
+    frame_chunk_adjoint<<<warps, 256, 0, st>>>(b, fb);
+    tc_dgrad_frame<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)N * 32, tiles, write_dy, k);
+    e = cudaGetLastError();
+    if (e == cudaSuccess && b.g_weights) e = tc_wgrad_jobs(ac, L, b.g_weights, false, true, st);
+    if (e != cudaSuccess) return e;
+    frame_ray_acc<<<warps, 256, 0, st>>>(a, fb);
+  }
+  float* rayred = CF(L.rayred);
+  frame_ray_finish<<<warps, 256, 0, st>>>(b, F(w.raypart), rayred);
+  e = cudaGetLastError();
+  return e != cudaSuccess ? e : launch_ray_reduce(b, rayred, st);
+}
+
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
 
 }  // namespace
@@ -1944,6 +2067,13 @@ size_t tc_render_frame_workspace(int N, int D) {
 cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st) {
   return D == 128 ? tc_render_frame_dim<128>(a, t_min, n_eval, t_final, st)
        : D == 64  ? tc_render_frame_dim<64>(a, t_min, n_eval, t_final, st) : tc_render_frame_dim<256>(a, t_min, n_eval, t_final, st);
+}
+
+size_t tc_render_frame_bwd_workspace(int N, int S, int D) {
+  return D == 128 ? frame_bwd_layout<128>(N, S).total : (D == 64 ? frame_bwd_layout<64>(N, S).total : frame_bwd_layout<256>(N, S).total);
+}
+cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  return D == 128 ? tc_render_frame_bwd_dim<128>(b, st) : (D == 64 ? tc_render_frame_bwd_dim<64>(b, st) : tc_render_frame_bwd_dim<256>(b, st));
 }
 
 size_t tc_geometry_frame_workspace(int N, int n_steps, int D) {

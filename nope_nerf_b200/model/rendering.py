@@ -72,6 +72,11 @@ class Renderer(nn.Module):
         if frame_engine == 'simt' and self.frame_t_min is None:
             raise ValueError("frame_engine='simt' needs frame_t_min (a float >= 0)")
         self.frame_engine = frame_engine
+        # frame_grad=True: training renders of nope_nerf (eval_=False) run on ops.render_frame_grad (nnb_render_frame_bwd: the same bits,
+        # gradients from a backward whose memory does not grow with the sample count) instead of render_autograd.  Tensor-core engine
+        # only, without jitter: such a render with add_noise on uniform sampling, or on the SIMT engine, is a ValueError.  Its output
+        # dict has z_vals and alpha None (the frame keeps no per-sample values).  Off by default.
+        self.frame_grad = bool(kwargs.get("frame_grad", False))
 
     def to(self, device):
         model = super().to(device)
@@ -123,7 +128,14 @@ class Renderer(nn.Module):
                                                       want_z_alpha=True, param_slices=getattr(self.model, 'param_slices', None)))
         flat = self.model.flat_weights()
         d = depth.reshape(n_points)
-        rgb, dp, dg, mask, z, alpha = ops.render_autograd(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))
+        if self.frame_grad and not eval_:
+            if noise is not None:
+                raise ValueError("Renderer(frame_grad=True) renders without jitter: call with add_noise=False or use ndc sampling")
+            meta.update(want_z_alpha=False, noise=None)
+            rgb, dp, dg, mask = ops.render_frame_grad(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))
+            z = alpha = None
+        else:
+            rgb, dp, dg, mask, z, alpha = ops.render_autograd(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))
         m = mask.bool()
         diff_norm = None
         if self.cfg.get('normal_loss', False) and not eval_:

@@ -209,6 +209,100 @@ def _render_frame(fn, name, nbytes, engine, weights, c2w, cam, *, N, S, flags, n
     return outs + (n_eval, t_final) if want_stats else outs
 
 
+def render_frame_bwd(weights, c2w, cam, g_rgb, g_depth_pred, g_depth_gt, g_weights, g_c2w, g_cam=None, g_depth=None, g_scale_shift=None, *, N,
+                     S, flags, near, far, ray_idx=None, pixels=None, depth=None, depth_map=None, scale=None, shift=None, H=0, W=0,
+                     hidden_dim=256):
+    """nnb_render_frame_bwd: the gradients of render_frame's outputs (t_min = 0, tensor-core engine) in a workspace whose only part that
+    grows with S is one float per ray and 32-sample chunk.  The g_* outputs follow RenderCall.backward (accumulated; g_depth overwritten;
+    g_weights may be None).  Returns (rgb, depth_pred, depth_gt, mask) of the call's own forward, the bits of render_frame."""
+    for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels), ("depth", depth),
+                   ("depth_map", depth_map)):
+        _need_cuda(t_, n_)
+    dev = weights.device
+    b = L.RenderBwdArgs()
+    a = b.fwd
+    a.weights = L.ptr(weights); a.c2w = L.ptr(c2w); a.cam = L.ptr(cam)
+    a.ray_idx = L.ptr(ray_idx); a.pixels = L.ptr(pixels); a.depth = L.ptr(depth); a.depth_map = L.ptr(depth_map)
+    a.scale = L.ptr(scale); a.shift = L.ptr(shift)
+    a.N, a.S, a.H, a.W = N, S, H, W
+    if depth_map is not None:
+        a.h_d, a.w_d = depth_map.shape[-2], depth_map.shape[-1]
+    a.near_, a.far_ = float(near), float(far)
+    a.flags = flags; a.engine = L.ENGINE_TC; a.hidden_dim = int(hidden_dim)
+    rgb = torch.empty(N, 3, device=dev); depth_pred = torch.empty(N, device=dev)
+    depth_gt = torch.empty(N, device=dev); mask = torch.empty(N, dtype=torch.uint8, device=dev)
+    a.rgb = L.ptr(rgb); a.depth_pred = L.ptr(depth_pred); a.depth_gt = L.ptr(depth_gt); a.mask = L.ptr(mask)
+    keep = [_f32c(g_rgb), _f32c(g_depth_pred), _f32c(g_depth_gt)]
+    b.g_rgb, b.g_depth_pred, b.g_depth_gt = L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2])
+    b.g_weights = L.ptr(g_weights); b.g_c2w = L.ptr(g_c2w); b.g_cam = L.ptr(g_cam); b.g_depth = L.ptr(g_depth)
+    b.g_scale_shift = L.ptr(g_scale_shift)
+    nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, int(hidden_dim))
+    ws = _pool.take(nbytes, dev) if nbytes else None
+    a.workspace = L.ptr(ws); a.workspace_bytes = 0 if ws is None else ws.numel()
+    try:
+        L.check(L.lib.nnb_render_frame_bwd(C.byref(b), _stream()), "nnb_render_frame_bwd")
+    finally:
+        if ws is not None:
+            _pool.give(ws)
+    return rgb, depth_pred, depth_gt, mask
+
+
+class _FrameGradFn(torch.autograd.Function):
+    """render_frame_grad's autograd glue: the forward is render_frame_engine on the tensor-core engine at t_min = 0 (RenderCall's bits
+    without a stash), the backward nnb_render_frame_bwd, which evaluates the field again chunk by chunk.  Differentiable inputs as in
+    _RenderFn."""
+
+    @staticmethod
+    def forward(ctx, meta, flat, c2w, cam, depth, scale, shift, *params):
+        meta = dict(meta)
+        ctx.param_slices = meta.pop("param_slices", None)
+        det = lambda t: None if t is None else _f32c(t.detach())
+        kw = dict(meta, depth=det(depth), scale=det(scale), shift=det(shift))
+        ctx.kw = kw; ctx.inputs = (flat, det(c2w), det(cam))
+        ctx.nparams = len(params)
+        ctx.has = (depth is not None, scale is not None, shift is not None)
+        ctx.params_need = any(p.requires_grad for p in params)
+        rgb, dp, dg, mask = render_frame_engine(flat, ctx.inputs[1], ctx.inputs[2], t_min=0.0, **kw)
+        ctx.mark_non_differentiable(mask)
+        return rgb, dp, dg, mask
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_dp, g_dg, _g_mask):
+        kw = ctx.kw
+        flat, c2w, cam = ctx.inputs
+        dev = flat.device
+        N = kw["N"]
+        if g_rgb is None: g_rgb = torch.zeros(N, 3, device=dev)
+        g_c2w = torch.zeros(4, 4, device=dev); g_cam = torch.zeros(4, 4, device=dev)
+        g_w = torch.zeros(L.num_params(kw.get("hidden_dim", 256)), device=dev) if ctx.params_need else None
+        has_depth, has_scale, has_shift = ctx.has
+        g_depth = torch.empty(N, device=dev) if has_depth else None
+        g_ss = torch.zeros(2, device=dev) if (has_scale or has_shift) else None
+        render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c2w, g_cam, g_depth, g_ss,
+                         **{k: v for k, v in kw.items() if k not in ("engine",)})
+        gp = [None] * ctx.nparams
+        if g_w is not None:
+            slices = ctx.param_slices
+            if slices is None:
+                from .model.official_nerf import PARAM_SLICES as slices
+            gp = [g_w[o:o + n].view(shape) for (o, n, shape) in slices]
+        return (None, None, g_c2w, g_cam, g_depth, g_ss[0] if has_scale else None, g_ss[1] if has_shift else None) + tuple(gp)
+
+
+def render_frame_grad(meta, flat, c2w, cam, depth, scale, shift, params):
+    """render_autograd on the differentiable frame: (rgb, depth_pred, depth_gt, mask) of render_frame_engine (tensor-core engine,
+    t_min = 0; the bits of RenderCall), with gradients to the MLP parameters, c2w, cam, depth and scale / shift from
+    nnb_render_frame_bwd, whose memory does not grow with S but by one float per ray and 32-sample chunk.  meta as render_autograd's
+    without noise, want_z_alpha and stash (no jitter, no per-sample outputs); its engine must resolve to the tensor-core engine."""
+    meta = dict(meta)
+    if meta.pop("noise", None) is not None or meta.pop("want_z_alpha", False) or meta.pop("stash", False):
+        raise ValueError("render_frame_grad: noise, want_z_alpha and stash are not supported (no jitter, no per-sample outputs)")
+    if pick_engine(meta.get("engine"), meta["S"]) != L.ENGINE_TC:
+        raise ValueError("render_frame_grad runs on the tensor-core engine only (16 <= S <= 1024)")
+    meta["engine"] = L.ENGINE_TC   # render_frame_engine's forward and nnb_render_frame_bwd run this engine only
+    return _FrameGradFn.apply(meta, flat, c2w, cam, depth, scale, shift, *params)
+
+
 class _RenderFn(torch.autograd.Function):
     """autograd glue for the drop-in Renderer / nope_nerf modules.
     differentiable inputs: c2w (4,4), cam (4,4), depth (N,) | (scale, shift) and the 24 MLP parameters.
