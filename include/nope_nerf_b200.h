@@ -441,6 +441,29 @@ size_t nnb_render_frame_workspace_bytes_engine(int32_t N, int32_t S, int32_t hid
 size_t nnb_render_frame_bwd_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim);
 int nnb_render_frame_bwd(const nnb_render_bwd_args* b, void* stream);
 
+/* nnb_render_frame_bwd as a forward / backward pair for training, with jitter: the forward's outputs feed the loss, and the backward starts
+ * from the checkpoints the forward left, so the field is evaluated twice per step, not three times.  Both calls use one workspace sized
+ * by nnb_render_frame_bwd_workspace_bytes(N, S, hidden_dim), in its layout.  No version bump: the symbols mark the capability.
+ * nnb_render_frame_train_fwd(a): a as b->fwd of nnb_render_frame_bwd, and noise is accepted ([N][S] jitter in [0, 1), read as
+ *   nnb_render_fwd reads it; ignored under NNB_NDC).  Writes rgb, depth_pred, depth_gt and mask, bit-identical to nnb_render_fwd on
+ *   NNB_ENGINE_TC with the same arguments (noise included), and leaves the forward weight image and the per-chunk transmittance
+ *   checkpoints in the workspace.
+ * nnb_render_frame_train_bwd(b): b->fwd must be the train_fwd call's arguments, the same pointers with unchanged contents (weights, c2w,
+ *   cam, ray_idx, depth_map / depth, scale, shift, noise), and its workspace as that call left it, on the same stream.  Runs the reverse
+ *   half of nnb_render_frame_bwd only (the transposed weight image, the reverse rounds, the per-ray pose adjoint and its reduction); the
+ *   forward outputs are not written.  The gradient fields and their accumulate / overwrite rules are nnb_render_frame_bwd's.  Its results
+ *   are defined only after a train_fwd into that workspace.  Of what train_fwd wrote it reads the forward weight image and the
+ *   checkpoints, which are data, never an index or a counter: a missing forward gives wrong numbers, not an access outside the workspace.
+ *   Without noise, train_fwd + train_bwd give nnb_render_frame_bwd's outputs and gradients bit for bit.
+ * Neither call synchronises, reads anything back to the host or allocates, so both can be captured in a CUDA graph once an eager call of
+ * the same width has run the library's one-time set-up.
+ * Errors, with nothing launched: a == NULL / b == NULL (rc -1); then nnb_render_frame_bwd's checks and codes in its order, except that
+ *   noise is accepted (z_vals, alpha, pts and dirs stay -6, as do NNB_STASH, NNB_HVP, NNB_OCC_ONLY and NNB_RAW_DENSITY); the NULL g_rgb
+ *   or g_c2w check (-3) applies to train_bwd only.  nnb_render_frame_bwd, nnb_render_frame and nnb_render_frame_engine keep rejecting
+ *   noise (-6). */
+int nnb_render_frame_train_fwd(const nnb_render_args* a, void* stream);
+int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream);
+
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,
                  float* c2w /*[16]*/, void* stream);

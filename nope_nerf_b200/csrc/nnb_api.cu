@@ -39,6 +39,8 @@ size_t tc_render_frame_workspace(int N, int D);
 cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st);
 size_t tc_render_frame_bwd_workspace(int N, int S, int D);
 cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
+cudaError_t tc_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStream_t st);
+cudaError_t tc_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
@@ -470,8 +472,9 @@ size_t nnb_render_frame_workspace_bytes_engine(int32_t N, int32_t S, int32_t hid
     return simt_render_frame_workspace(N);
   return 0;
 }
-// the checks of the frame's render arguments after the engine's, in nnb_render_frame's order up to the output pointers
-static int check_frame(const nnb_render_args* a) {
+// the checks of the frame's render arguments after the engine's, in nnb_render_frame's order up to the output pointers; `noise` is
+// accepted with allow_noise only (nnb_render_frame_train_fwd / _bwd)
+static int check_frame(const nnb_render_args* a, bool allow_noise = false) {
   if (int rc = check_flags(a->flags)) return rc;
   if (a->flags & (NNB_STASH | NNB_HVP | NNB_OCC_ONLY | NNB_RAW_DENSITY))
     return fail(-6, "nnb_render_frame: NNB_STASH, NNB_HVP, NNB_OCC_ONLY and NNB_RAW_DENSITY are not accepted (flags 0x%x)", a->flags);
@@ -482,8 +485,9 @@ static int check_frame(const nnb_render_args* a) {
   if (a->engine == NNB_ENGINE_TC && !tc_supports(a->S))
     return fail(-4, "tensor-core engine needs S in [16,1024] (got %d); use nnb_render_fwd on NNB_ENGINE_SIMT", a->S);
 #endif
-  if (a->noise || a->z_vals || a->alpha || a->pts || a->dirs)
-    return fail(-6, "nnb_render_frame: noise, z_vals, alpha, pts and dirs must be NULL (no jitter, no per-sample outputs)");
+  if ((a->noise && !allow_noise) || a->z_vals || a->alpha || a->pts || a->dirs)
+    return fail(-6, allow_noise ? "nnb_render_frame_train: z_vals, alpha, pts and dirs must be NULL (no per-sample outputs)"
+                                : "nnb_render_frame: noise, z_vals, alpha, pts and dirs must be NULL (no jitter, no per-sample outputs)");
   return 0;
 }
 // the render arguments' checks after the t_min check
@@ -560,6 +564,46 @@ int nnb_render_frame_bwd(const nnb_render_bwd_args* b, void* stream) {
   if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
   const cudaError_t e = tc_render_frame_bwd(*b, D, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_bwd");
+#endif
+}
+// the checks of nnb_render_frame_train_fwd / _bwd on b->fwd up to the workspace's, nnb_render_frame_bwd's with noise accepted
+static int check_frame_train(const nnb_render_args* a, const char* name) {
+  if (a->engine != NNB_ENGINE_TC) return fail(-4, "%s: engine %d has no differentiable frame (NNB_ENGINE_TC only)", name, a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_frame(a, true)) return rc;
+  return check_frame_io(a);
+#endif
+}
+static int check_frame_train_ws(const nnb_render_args* a) {
+  const size_t need = nnb_render_frame_bwd_workspace_bytes(a->N, a->S, a->hidden_dim);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  return 0;
+}
+int nnb_render_frame_train_fwd(const nnb_render_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (int rc = check_frame_train(a, "nnb_render_frame_train_fwd")) return rc;
+  if (int rc = check_frame_train_ws(a)) return rc;
+#ifdef NNB_WITH_TC
+  const cudaError_t e = tc_render_frame_train_fwd(*a, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_fwd");
+#else
+  return fail(-4, "library built without the tensor-core engine");
+#endif
+}
+int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (int rc = check_frame_train(a, "nnb_render_frame_train_bwd")) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_frame_train_bwd: g_rgb and g_c2w must be non-null");
+  if (int rc = check_frame_train_ws(a)) return rc;
+#ifdef NNB_WITH_TC
+  const cudaError_t e = tc_render_frame_train_bwd(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_bwd");
+#else
+  return fail(-4, "library built without the tensor-core engine");
 #endif
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {

@@ -1929,44 +1929,71 @@ template <int D> FrameBwdWs frame_bwd_layout(int N, int S) {
   return frame_bwd_layout_bytes(N, S, Tc<D>::IMG_BYTES, make_layout(N, 32, NNB_STASH, NNB_ENGINE_TC, D).total, Tc<D>::IMG_T_BYTES);
 }
 
-// nnb_render_frame_bwd: both weight images; the forward (run_render_frame at t_min = 0, so every ray runs every round) with the carry
-// after each chunk copied to the checkpoints; then the reverse rounds k = C - 1 .. 0, each on the chunk stash: tc_frame_stash,
-// frame_chunk_adjoint, tc_dgrad_frame, (g_weights) the weight-gradient stage, whose reduce adds the round's dW into g_weights, and
-// frame_ray_acc; then frame_ray_finish and ray_reduce.  The rounds run one after another on the stream.
+// the lazy set-up of nnb_render_frame_bwd and of its two halves (both stage tables, the kernels' shared-memory limits); returns the
+// SM count, 0 on an error (in *e)
 template <int D>
-cudaError_t tc_render_frame_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+int frame_bwd_setup(cudaError_t* e) {
   using T = Tc<D>;
-  const nnb_render_args& a = b.fwd;
-  cudaError_t e = upload_stage_table<D>();
-  if (e == cudaSuccess) e = upload_stage_table_t<D>();
-  if (e != cudaSuccess) return e;
+  *e = upload_stage_table<D>();
+  if (*e == cudaSuccess) *e = upload_stage_table_t<D>();
+  if (*e != cudaSuccess) return 0;
   static bool attr = false;
   static int n_sm = 0;
   if (!attr) {
-    e = cudaFuncSetAttribute(tc_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_frame_stash<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_dgrad_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
-    if (e != cudaSuccess) return e;
+    *e = cudaFuncSetAttribute(tc_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_frame_stash<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_dgrad_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (*e != cudaSuccess) return 0;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     attr = true;
   }
+  return n_sm;
+}
+
+// The forward half of nnb_render_frame_bwd (nnb_render_frame_train_fwd): the forward weight image, then the forward (run_render_frame at
+// t_min = 0, so every ray runs every round) with the carry after each chunk copied to the checkpoints.  It leaves the weight image and
+// the checkpoints in the workspace for the reverse half.
+template <int D>
+cudaError_t tc_frame_train_fwd_dim(const nnb_render_args& a, cudaStream_t st) {
+  using T = Tc<D>;
+  cudaError_t e;
+  const int n_sm = frame_bwd_setup<D>(&e);
+  if (e != cudaSuccess) return e;
   const int N = a.N, C = (a.S + 31) / 32;
   const FrameBwdWs w = frame_bwd_layout<D>(N, a.S);
   char* base = static_cast<char*>(a.workspace);
-  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
-  unsigned char *img = reinterpret_cast<unsigned char*>(base + w.f.img), *img_t = reinterpret_cast<unsigned char*>(base + w.img_t);
+  unsigned char* img = reinterpret_cast<unsigned char*>(base + w.f.img);
   tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);
-  tc_prep_weights_t<D><<<T::N_STAGES_T, 256, 0, st>>>(a.weights, img_t);
-  const int tiles = (N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm;   // 4 ray-chunks of 32 rows per tile, forward and reverse
-  float* ckpt = F(w.ckpt);
+  const int tiles = (N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm;   // 4 ray-chunks of 32 rows per tile
+  float* ckpt = reinterpret_cast<float*>(base + w.ckpt);
   cudaError_t ec = cudaSuccess;
   e = run_render_frame(a, w.f, 0.f, nullptr, nullptr, st, [&](const FramePtrs& f) {
     tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f);
     if (f.k + 1 < C && ec == cudaSuccess) ec = cudaMemcpyAsync(ckpt + (size_t)f.k * N, f.carry, (size_t)N * 4, cudaMemcpyDeviceToDevice, st);
   });
-  if (e == cudaSuccess) e = ec;
+  return e == cudaSuccess ? ec : e;
+}
+
+// The reverse half of nnb_render_frame_bwd (nnb_render_frame_train_bwd): the transposed weight image, then the reverse rounds
+// k = C - 1 .. 0, each on the chunk stash: tc_frame_stash, frame_chunk_adjoint, tc_dgrad_frame, (g_weights) the weight-gradient stage,
+// whose reduce adds the round's dW into g_weights, and frame_ray_acc; then frame_ray_finish and ray_reduce.  The rounds run one after
+// another on the stream.  Of what the forward half wrote it reads the forward weight image and the checkpoints only (data, no index or
+// counter), so a workspace the forward half did not fill gives wrong numbers, never an access outside the workspace.
+template <int D>
+cudaError_t tc_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+  using T = Tc<D>;
+  const nnb_render_args& a = b.fwd;
+  cudaError_t e;
+  const int n_sm = frame_bwd_setup<D>(&e);
   if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32;
+  const FrameBwdWs w = frame_bwd_layout<D>(N, a.S);
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  unsigned char *img = reinterpret_cast<unsigned char*>(base + w.f.img), *img_t = reinterpret_cast<unsigned char*>(base + w.img_t);
+  tc_prep_weights_t<D><<<T::N_STAGES_T, 256, 0, st>>>(a.weights, img_t);
+  const int tiles = (N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm;   // 4 ray-chunks of 32 rows per tile
   // the chunk stash: make_layout's offsets from its own base
   nnb_render_args ac = a;
   ac.workspace = base + w.chunk; ac.workspace_bytes = w.img_t - w.chunk;
@@ -1984,7 +2011,7 @@ cudaError_t tc_render_frame_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t s
   for (int l = 0; l < 8; ++l) P.dy[l] = CF(L.dy[l]);
   P.dfeat = CF(L.dfeat); P.dyr = CF(L.dyr);
   FrameBwdPtrs fb{};
-  fb.rounds = C; fb.ckpt = ckpt; fb.suffix = F(w.suffix); fb.rec = recs;
+  fb.rounds = C; fb.ckpt = F(w.ckpt); fb.suffix = F(w.suffix); fb.rec = recs;
   fb.gs = reinterpret_cast<float4*>(cb + L.gs); fb.gp = P.gp; fb.gv = P.gv; fb.raypart = F(w.raypart);
   const int write_dy = b.g_weights ? 1 : 0, warps = (N + 7) / 8;
   for (int k = C - 1; k >= 0; --k) {
@@ -2072,8 +2099,16 @@ cudaError_t tc_render_frame(const nnb_render_args& a, float t_min, int* n_eval, 
 size_t tc_render_frame_bwd_workspace(int N, int S, int D) {
   return D == 128 ? frame_bwd_layout<128>(N, S).total : (D == 64 ? frame_bwd_layout<64>(N, S).total : frame_bwd_layout<256>(N, S).total);
 }
+cudaError_t tc_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStream_t st) {
+  return D == 128 ? tc_frame_train_fwd_dim<128>(a, st) : (D == 64 ? tc_frame_train_fwd_dim<64>(a, st) : tc_frame_train_fwd_dim<256>(a, st));
+}
+cudaError_t tc_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  return D == 128 ? tc_frame_train_bwd_dim<128>(b, st) : (D == 64 ? tc_frame_train_bwd_dim<64>(b, st) : tc_frame_train_bwd_dim<256>(b, st));
+}
+// nnb_render_frame_bwd: the two halves in sequence
 cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
-  return D == 128 ? tc_render_frame_bwd_dim<128>(b, st) : (D == 64 ? tc_render_frame_bwd_dim<64>(b, st) : tc_render_frame_bwd_dim<256>(b, st));
+  const cudaError_t e = tc_render_frame_train_fwd(b.fwd, D, st);
+  return e != cudaSuccess ? e : tc_render_frame_train_bwd(b, D, st);
 }
 
 size_t tc_geometry_frame_workspace(int N, int n_steps, int D) {

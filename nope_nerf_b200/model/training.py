@@ -320,11 +320,12 @@ class _GraphStep:
         n_local = ray_idx.shape[0]
         flags = ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=False, shift_first=tr.shift_first)
         ndc = rend.cfg['sample_option'] == 'ndc'
-        call = ops.RenderCall(net.flat_weights(), self.c2w, self.cam, N=n_local, S=S, flags=flags,
-                              engine=rend.engine if rend.engine is not None else ops.default_engine(),
-                              near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
-                              ray_idx=ray_idx, depth_map=self.dpt, scale=self.ss[0:1], shift=self.ss[1:2], noise=noise, H=h, W=w, stash=True,
-                              hidden_dim=net.hidden_dim)
+        render_call = ops.FrameRenderCall if tr.frame_grad else ops.RenderCall
+        call = render_call(net.flat_weights(), self.c2w, self.cam, N=n_local, S=S, flags=flags,
+                           engine=rend.engine if rend.engine is not None else ops.default_engine(),
+                           near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
+                           ray_idx=ray_idx, depth_map=self.dpt, scale=self.ss[0:1], shift=self.ss[1:2], noise=noise, H=h, W=w, stash=True,
+                           hidden_dim=net.hidden_dim)
         if rend.cfg.get('normal_loss', False) and not tr.use_cuda_graph:
             tr._normal_draw(call.mask)
         ops.loss_rgb_depth_indirect(call.rgb, call.depth_pred, call.depth_gt, call.mask, 0.0, 0.0, self.rgb_l2, self.imgpp,
@@ -514,6 +515,13 @@ class _GraphStep:
 
 
 class Trainer(object):
+    """Keyword options (besides the reference's arguments) include frame_grad (default False): with True, every training render that has
+    a backward, in the captured graph step and in the general path, runs the differentiable frame's training pair ops.FrameRenderCall.
+    Its workspace grows with rendering.num_points by one float per ray and 32-sample chunk instead of the per-sample stash, and it takes
+    the jitter of sample_option 'uniform'.  The renderer's engine and rendering.num_points must resolve to the tensor-core engine
+    (ValueError otherwise).  Renders without a backward are unchanged.  This is a Trainer keyword, not a reading of
+    Renderer(frame_grad=...): that flag governs Renderer.nope_nerf, which the Trainer does not call."""
+
     def __init__(self, model, optimizer, cfg, device=None, optimizer_pose=None, pose_param_net=None,
                  optimizer_focal=None, focal_net=None, optimizer_distortion=None, distortion_net=None, **kwargs):
         self.model = model
@@ -577,6 +585,13 @@ class Trainer(object):
         # 'randperm' = the reference's torch.randperm(H*W)[:N] (identical RNG stream in eager mode); 'hash' = nnb_sample_pixels;
         # 'auto' = randperm when running eagerly, hash inside the CUDA graph (whose RNG stream differs from eager anyway)
         self.pixel_sampler = kwargs.get('pixel_sampler', 'auto')
+        self.frame_grad = bool(kwargs.get('frame_grad', False))
+        if self.frame_grad:
+            rend = model.renderer
+            engine = rend.engine if rend.engine is not None else ops.default_engine()
+            if ops.pick_engine(engine, int(rend.cfg['num_points'])) != L.ENGINE_TC:
+                raise ValueError("Trainer(frame_grad=True) needs the tensor-core engine: the renderer's engine and rendering.num_points "
+                                 "(16..1024) must resolve to it")
 
     # ------------------------------------------------------------------------------------
     def _smoothness_on(self):
@@ -874,11 +889,12 @@ class Trainer(object):
             ops.pose_fwd_raw(pose.r.detach(), pose.t.detach(), init, img_idx, c2w)
             flags = ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=eval_mode, shift_first=self.shift_first)
             ndc = rend.cfg['sample_option'] == 'ndc'
-            call = ops.RenderCall(net.flat_weights(), c2w, cam_dev, N=n_local, S=S, flags=flags,
-                                  engine=rend.engine if rend.engine is not None else ops.default_engine(),
-                                  near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
-                                  ray_idx=ray_idx, depth_map=depth_input.detach().reshape(h_depth, w_depth).contiguous(),
-                                  scale=scale_dev, shift=shift_dev, noise=noise, H=h, W=w, stash=backward, hidden_dim=net.hidden_dim)
+            render_call = ops.FrameRenderCall if self.frame_grad and backward else ops.RenderCall
+            call = render_call(net.flat_weights(), c2w, cam_dev, N=n_local, S=S, flags=flags,
+                               engine=rend.engine if rend.engine is not None else ops.default_engine(),
+                               near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
+                               ray_idx=ray_idx, depth_map=depth_input.detach().reshape(h_depth, w_depth).contiguous(),
+                               scale=scale_dev, shift=shift_dev, noise=noise, H=h, W=w, stash=backward, hidden_dim=net.hidden_dim)
             if rend.cfg.get('normal_loss', False) and not eval_mode:
                 self._normal_draw(call.mask)
             inv = self.depth_loss_type == 'invariant' and weights['depth_weight'] != 0.0

@@ -89,9 +89,17 @@ _pool = _WorkspacePool()
 
 class RenderCall:
     """One forward launch + the state its backward needs (workspace with the stash)."""
+    frame = False   # FrameRenderCall: the differentiable frame's training pair
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
                  depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256):
+        frame = self.frame
+        if frame:
+            if want_z_alpha:
+                raise ValueError("FrameRenderCall: want_z_alpha is not supported (no per-sample outputs)")
+            if pick_engine(engine, S) != L.ENGINE_TC:
+                raise ValueError("FrameRenderCall runs on the tensor-core engine only (16 <= S <= 1024)")
+            stash = True
         for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels),
                        ("depth", depth), ("noise", noise)):
             _need_cuda(t_, n_)
@@ -107,7 +115,7 @@ class RenderCall:
             a.h_d, a.w_d = depth_map.shape[-2], depth_map.shape[-1]
         a.near_, a.far_ = float(near), float(far)
         engine = pick_engine(engine, S)
-        if stash:
+        if stash and not frame:
             flags |= L.STASH
         a.flags = flags; a.engine = engine; a.hidden_dim = int(hidden_dim)
         self.hidden_dim = int(hidden_dim)
@@ -117,13 +125,19 @@ class RenderCall:
         self.alpha = torch.empty(N, S, device=dev) if want_z_alpha else None
         a.rgb = L.ptr(self.rgb); a.depth_pred = L.ptr(self.depth_pred); a.depth_gt = L.ptr(self.depth_gt)
         a.mask = L.ptr(self.mask); a.z_vals = L.ptr(self.z_vals); a.alpha = L.ptr(self.alpha)
-        nbytes = L.lib.nnb_workspace_bytes_dim(N, S, flags, engine, int(hidden_dim))
+        if frame:
+            nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, int(hidden_dim))
+        else:
+            nbytes = L.lib.nnb_workspace_bytes_dim(N, S, flags, engine, int(hidden_dim))
         if nbytes == 0:
             raise ValueError("nope_nerf_b200: hidden_dim %s is not supported (supported: %s)" % (hidden_dim, L.HIDDEN_DIMS))
         self.ws = _pool.take(nbytes, dev)
         a.workspace = L.ptr(self.ws); a.workspace_bytes = self.ws.numel()
         self.args = a; self.N = N; self.S = S; self.stash = stash; self.pooled = True
-        L.check(L.lib.nnb_render_fwd(C.byref(a), _stream()), "nnb_render_fwd")
+        if frame:
+            L.check(L.lib.nnb_render_frame_train_fwd(C.byref(a), _stream()), "nnb_render_frame_train_fwd")
+        else:
+            L.check(L.lib.nnb_render_fwd(C.byref(a), _stream()), "nnb_render_fwd")
         if not stash:
             self.release()
 
@@ -142,8 +156,21 @@ class RenderCall:
         b.g_rgb, b.g_depth_pred, b.g_depth_gt = L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2])
         b.g_weights = L.ptr(g_weights); b.g_c2w = L.ptr(g_c2w); b.g_cam = L.ptr(g_cam); b.g_depth = L.ptr(g_depth)
         b.g_scale_shift = L.ptr(g_scale_shift)
-        L.check(L.lib.nnb_render_bwd(C.byref(b), _stream()), "nnb_render_bwd")
+        if self.frame:
+            L.check(L.lib.nnb_render_frame_train_bwd(C.byref(b), _stream()), "nnb_render_frame_train_bwd")
+        else:
+            L.check(L.lib.nnb_render_bwd(C.byref(b), _stream()), "nnb_render_bwd")
         self.release()
+
+
+class FrameRenderCall(RenderCall):
+    """RenderCall on the differentiable frame's training pair (tensor-core engine), with RenderCall's arguments, outputs, pooling and
+    backward() rules.  The forward is nnb_render_frame_train_fwd, which gives the bits of RenderCall's forward, jitter included, and
+    backward() is nnb_render_frame_train_bwd, in one workspace of nnb_render_frame_bwd_workspace_bytes: its only part that grows with S is
+    one float per ray and 32-sample chunk, where RenderCall(stash=True) keeps every sample.  The workspace is always kept for backward(),
+    so `stash` is implied and ignored.  want_z_alpha, and an engine that pick_engine does not resolve to the tensor-core engine
+    (ENGINE_SIMT, or S < 16), are a ValueError, raised before any other check."""
+    frame = True
 
 
 def render_frame(weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None, depth_map=None, scale=None,

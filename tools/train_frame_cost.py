@@ -1,0 +1,135 @@
+"""Cost of Trainer(frame_grad=True): the captured training step with the differentiable frame's training pair (FrameRenderCall:
+nnb_render_frame_train_fwd + nnb_render_frame_train_bwd) against the default step (nnb_render_fwd with NNB_STASH + nnb_render_bwd).
+Shapes: the C2 step (1024 rays x 128 samples, bench.py's render-only configuration and frames) and N = 4096, S = 512, D = 256.
+  * Trainer graph steps: one Trainer per path, steps alternated between the two over --rounds rounds of --steps steps each, median ms per
+    step; the peak torch.cuda.max_memory_allocated over each Trainer's build and warm-up, above what was allocated before it.
+  * The ops-level pair: FrameRenderCall + backward against render_frame_engine + nnb_render_frame_bwd (ops.render_frame_bwd), which
+    evaluates the field once more, same inputs, alternated, median.
+The card's name and power limit are read in the same run (nvidia-smi query, read-only).  Without a CUDA device the tool fails."""
+import argparse, gc, json, os, sys
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from field_query_cost import card  # noqa: E402
+
+SHAPES = ((1024, 128), (4096, 512))
+
+
+def build(N, S, frame_grad, dev):
+    import bench
+    import nope_nerf_b200.model as mdl
+    cfg = bench.make_cfg(N)
+    cfg["rendering"]["num_points"] = S
+    np.random.seed(42); torch.manual_seed(42)
+    net = mdl.OfficialStaticNerf(cfg)
+    model = mdl.get_model(mdl.Renderer(net, cfg["rendering"], device=dev), cfg, device=dev)
+    pose = mdl.LearnPose(bench.V, True, True, cfg).to(dev); dnet = mdl.Learn_Distortion(bench.V, True, True, cfg).to(dev)
+    with torch.no_grad():
+        pose.r.normal_(0, 0.05); pose.t.normal_(0, 0.05)
+    return mdl.Trainer(model, torch.optim.Adam(model.parameters(), lr=1e-3), cfg["training"], device=dev,
+                       optimizer_pose=torch.optim.Adam(pose.parameters(), lr=5e-4), pose_param_net=pose,
+                       optimizer_distortion=torch.optim.Adam(dnet.parameters(), lr=5e-4), distortion_net=dnet, frame_grad=frame_grad)
+
+
+def timed(fn, n):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(n):
+        fn(i)
+    e1.record(); e1.synchronize()
+    return e0.elapsed_time(e1) / n
+
+
+def trainer_steps(N, S, frames, rounds, steps, dev):
+    trainers, peak = {}, {}
+    for key, fg in (("stash", False), ("frame", True)):
+        torch.cuda.synchronize()
+        base = torch.cuda.memory_allocated(); torch.cuda.reset_peak_memory_stats()
+        tr = build(N, S, fg, dev)
+        for i in range(3):                                   # eager warm-up, capture, first replay
+            tr.train_step(frames[i % len(frames)], it=i, epoch=0, scheduling_start=10000, render_path=None)
+        torch.cuda.synchronize()
+        peak[key] = torch.cuda.max_memory_allocated() - base
+        trainers[key] = tr
+    assert all(len([v for v in tr._gsteps.values() if v]) == 1 for tr in trainers.values()), "the graph step did not run"
+    times = {"stash": [], "frame": []}
+    for r in range(rounds):
+        for key in (("stash", "frame") if r % 2 == 0 else ("frame", "stash")):
+            tr = trainers[key]
+            times[key].append(timed(lambda i: tr.train_step(frames[i % len(frames)], it=i, epoch=0, scheduling_start=10000, render_path=None),
+                                    steps))
+    del trainers
+    gc.collect(); torch.cuda.empty_cache()
+    return {k: float(np.median(v)) for k, v in times.items()}, peak
+
+
+def ops_pair(N, S, D, rounds):
+    from nope_nerf_b200 import ops, _lib as L
+    from oracle import nerf_oracle as O
+    rng = np.random.default_rng(0)
+    cu = lambda x: torch.from_numpy(np.ascontiguousarray(x)).cuda()
+    flat = cu(O.flatten_params(O.init_params(seed=7, D=D, hf_damp=True)))
+    c2w = cu(O.make_c2w(np.array([0.02, -0.03, 0.01], np.float32), np.array([0.05, 0.0, -0.04], np.float32)))
+    cam = torch.diag(torch.tensor([1.2, -1.6, -1.0, 1.0])).cuda()
+    H, W = 270, 480
+    kw = dict(N=N, S=S, flags=ops.flags_from_cfg(dict(O.DEFAULT_CFG), "softplus"), near=0.01, far=10.0,
+              ray_idx=cu(rng.permutation(H * W)[:N].astype(np.int64)), depth_map=cu(rng.uniform(0.6, 7.2, (48, 64)).astype(np.float32)),
+              scale=torch.tensor([1.05]).cuda(), shift=torch.tensor([0.02]).cuda(), H=H, W=W, hidden_dim=D)
+    g_rgb, g_dp, g_dg = cu(rng.normal(0, 1, (N, 3)).astype(np.float32)), torch.zeros(N, device="cuda"), torch.zeros(N, device="cuda")
+    g_w = torch.zeros(L.num_params(D), device="cuda"); g_c = torch.zeros(4, 4, device="cuda")
+
+    def pair(_):
+        call = ops.FrameRenderCall(flat, c2w, cam, engine=None, **kw)
+        call.backward(g_rgb, g_dp, g_dg, g_w, g_c)
+
+    def one_call(_):
+        ops.render_frame_engine(flat, c2w, cam, engine=L.ENGINE_TC, **kw)
+        ops.render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c, **kw)
+
+    for fn in (pair, one_call):
+        fn(0); fn(0)
+    torch.cuda.synchronize()
+    times = {"pair": [], "fwd_plus_frame_bwd": []}
+    for r in range(rounds):
+        for key, fn in (("pair", pair), ("fwd_plus_frame_bwd", one_call)) if r % 2 == 0 else (("fwd_plus_frame_bwd", one_call), ("pair", pair)):
+            times[key].append(timed(fn, 1))
+    ops._pool.free.clear(); torch.cuda.empty_cache()
+    return {k: float(np.median(v)) for k, v in times.items()}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=7)
+    ap.add_argument("--steps", type=int, default=20, help="graph steps per timed round")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("train_frame_cost: needs a CUDA device (there is no CPU path and a CPU timing would say nothing about the GPU)")
+    import bench
+    from nope_nerf_b200 import ops, _lib as L
+    ops.set_default_engine("tc")
+    dev = torch.device("cuda", 0); torch.cuda.set_device(0)
+    name, limit = card()
+    D = 256
+    _, frames = bench.synth_frames(bench.H, bench.W, bench.HD, bench.WD, 4, bench.V, dev, with_ref=False)
+    res = {"gpu": name, "power_limit": limit, "hidden_dim": D, "rounds": args.rounds, "steps": args.steps, "shapes": []}
+    for N, S in SHAPES:
+        step, peak = trainer_steps(N, S, frames, args.rounds, args.steps, dev)
+        pair = ops_pair(N, S, D, args.rounds)
+        row = {"N": N, "S": S, "step_stash_ms": step["stash"], "step_frame_ms": step["frame"], "step_ratio": step["frame"] / step["stash"],
+               "peak_stash_bytes": int(peak["stash"]), "peak_frame_bytes": int(peak["frame"]),
+               "ops_pair_ms": pair["pair"], "ops_fwd_plus_frame_bwd_ms": pair["fwd_plus_frame_bwd"],
+               "ops_ratio": pair["pair"] / pair["fwd_plus_frame_bwd"]}
+        res["shapes"].append(row)
+        print("N=%d S=%d D=%d  graph step: stash %.2f ms, frame_grad %.2f ms (x%.2f); peak %.2f GB -> %.2f GB | ops: train pair %.2f ms, "
+              "render_frame_engine + nnb_render_frame_bwd %.2f ms (x%.2f)"
+              % (N, S, D, step["stash"], step["frame"], row["step_ratio"], peak["stash"] / 1e9, peak["frame"] / 1e9, pair["pair"],
+                 pair["fwd_plus_frame_bwd"], row["ops_ratio"]), file=sys.stderr, flush=True)
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
