@@ -464,6 +464,34 @@ int nnb_render_frame_bwd(const nnb_render_bwd_args* b, void* stream);
 int nnb_render_frame_train_fwd(const nnb_render_args* a, void* stream);
 int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream);
 
+/* nnb_render_frame_bwd, nnb_render_frame_train_fwd and nnb_render_frame_train_bwd on fwd.engine.  NNB_ENGINE_TC is exactly the call
+ * without the suffix (its checks, codes, bits and workspace).  NNB_ENGINE_SIMT runs the same method on the exact-fp32 engine at any S from
+ * 2 to 1024, with a chunk stash that packs R = min(S, 32) rows per ray (row R n + j is sample 32 k + j of ray n), so a round at S < 32
+ * evaluates N S rows.  The four calls without the suffix keep their contracts.  No version bump: the symbols mark the capability.
+ * On NNB_ENGINE_SIMT:
+ *   Forward bits: the outputs of nnb_render_frame_bwd_engine and nnb_render_frame_train_fwd_engine are bit-identical to nnb_render_fwd on
+ *   NNB_ENGINE_SIMT with the same arguments (noise included, for the train pair).
+ *   Gradients at S <= 32 (one chunk): the chunk stash holds nnb_render_fwd's rows in its order and the weight-gradient stage splits them
+ *   as nnb_render_bwd does, so the gradients are those of nnb_render_fwd (NNB_STASH) + nnb_render_bwd on NNB_ENGINE_SIMT, bit for bit.
+ *   At S > 32 they differ from them in the order of their sums only (weight gradients chunk by chunk, the ray sums from the last chunk);
+ *   every dW / db, g_c2w and the other pose outputs stay within 1e-4 of the largest magnitude of their tensor.
+ *   Without noise, train_fwd_engine + train_bwd_engine give nnb_render_frame_bwd_engine's outputs and gradients bit for bit.  Every sum
+ *   runs in a fixed order, so the same inputs give the same bits whatever the workspace held.  Neither call of the pair synchronises,
+ *   reads back or allocates.  Of what train_fwd_engine wrote, train_bwd_engine reads the checkpoints only.
+ * Errors, with nothing launched: NULL args (rc -1); an engine other than NNB_ENGINE_TC and NNB_ENGINE_SIMT (-4); then the checks and codes
+ *   of the call without the suffix in its order, except that S in 2..15 is accepted on NNB_ENGINE_SIMT and the workspace is sized by
+ *   nnb_render_frame_bwd_workspace_bytes_engine.  noise is accepted by the train pair only (-6 on nnb_render_frame_bwd_engine).
+ * Workspace: nnb_render_frame_bwd_workspace_bytes_engine(N, S, hidden_dim, engine) is nnb_render_frame_bwd_workspace_bytes on
+ *   NNB_ENGINE_TC.  On NNB_ENGINE_SIMT it is that layout without weight images and with the chunk stash nnb_workspace_bytes_dim(N, R,
+ *   NNB_STASH, NNB_ENGINE_SIMT, hidden_dim): 2.66 GB at N = 4096, D = 256 for every S >= 32, where nnb_render_fwd's stash needs about
+ *   19.9 KB per sample (83.7 GB at S = 1024).  At S <= 32 the chunk stash is the stash path's, so the workspace is about 1.8 KB per ray
+ *   larger than nnb_workspace_bytes_dim(N, S, NNB_STASH, NNB_ENGINE_SIMT, hidden_dim).  0 on bad sizes (N <= 0, S outside 2..1024 on
+ *   NNB_ENGINE_SIMT), an unsupported width or another engine. */
+size_t nnb_render_frame_bwd_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine);
+int nnb_render_frame_bwd_engine(const nnb_render_bwd_args* b, void* stream);
+int nnb_render_frame_train_fwd_engine(const nnb_render_args* a, void* stream);
+int nnb_render_frame_train_bwd_engine(const nnb_render_bwd_args* b, void* stream);
+
 /* LearnPose.forward (model/poses.py:23-31): c2w = [Exp(r[id]) t[id]; 0 1] @ init_c2w[id] */
 int nnb_pose_fwd(const float* r, const float* t, const float* init_c2w /*[V,16] or NULL*/, int32_t cam_id,
                  float* c2w /*[16]*/, void* stream);

@@ -128,6 +128,11 @@ def _load():
     lib.nnb_render_frame_bwd_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     lib.nnb_render_frame_train_fwd.argtypes = [C.POINTER(RenderArgs), C.c_void_p]
     lib.nnb_render_frame_train_bwd.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
+    lib.nnb_render_frame_bwd_workspace_bytes_engine.restype = C.c_size_t
+    lib.nnb_render_frame_bwd_workspace_bytes_engine.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+    lib.nnb_render_frame_bwd_engine.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
+    lib.nnb_render_frame_train_fwd_engine.argtypes = [C.POINTER(RenderArgs), C.c_void_p]
+    lib.nnb_render_frame_train_bwd_engine.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]
     lib.nnb_pose_bwd.argtypes = [_f, _f, _f, C.c_int32, _f, _f, _f, C.c_void_p]
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,
@@ -168,7 +173,8 @@ lib = _load()
 EXPORTS = ["nnb_last_error", "nnb_version", "nnb_profile_events", "nnb_profile_cursor", "nnb_workspace_bytes", "nnb_render_fwd", "nnb_render_bwd", "nnb_pose_fwd",
            "nnb_pose_bwd", "nnb_loss_rgb_depth", "nnb_chamfer", "nnb_chamfer_workspace_bytes", "nnb_adam_step", "nnb_render_frame_engine",
            "nnb_render_frame_workspace_bytes_engine", "nnb_render_frame_bwd", "nnb_render_frame_bwd_workspace_bytes",
-           "nnb_render_frame_train_fwd", "nnb_render_frame_train_bwd"]
+           "nnb_render_frame_train_fwd", "nnb_render_frame_train_bwd", "nnb_render_frame_bwd_workspace_bytes_engine",
+           "nnb_render_frame_bwd_engine", "nnb_render_frame_train_fwd_engine", "nnb_render_frame_train_bwd_engine"]
 
 
 def check(rc, what):

@@ -19,6 +19,10 @@ size_t simt_geometry_frame_workspace(int N, int n_steps, int D);
 cudaError_t simt_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 size_t simt_render_frame_workspace(int N);
 cudaError_t simt_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st);
+size_t simt_render_frame_bwd_workspace(int N, int S, int D);
+cudaError_t simt_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
+cudaError_t simt_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStream_t st);
+cudaError_t simt_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
@@ -605,6 +609,69 @@ int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream) {
 #else
   return fail(-4, "library built without the tensor-core engine");
 #endif
+}
+size_t nnb_render_frame_bwd_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine) {
+  if (engine == NNB_ENGINE_TC) return nnb_render_frame_bwd_workspace_bytes(N, S, hidden_dim);
+  const int D = hidden_of(hidden_dim);
+  if (engine == NNB_ENGINE_SIMT && N > 0 && S >= 2 && S <= 1024 && nnb::dim_supported(D)) return simt_render_frame_bwd_workspace(N, S, D);
+  return 0;
+}
+// the engine check of the _engine forms of the differentiable frame: NNB_ENGINE_TC (when built with it) or NNB_ENGINE_SIMT
+static int check_frame_bwd_engine(int32_t engine, const char* name) {
+  if (engine != NNB_ENGINE_TC && engine != NNB_ENGINE_SIMT)
+    return fail(-4, "%s: engine %d has no differentiable frame (NNB_ENGINE_TC or NNB_ENGINE_SIMT)", name, engine);
+#ifndef NNB_WITH_TC
+  if (engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
+#endif
+  return 0;
+}
+static int check_frame_bwd_ws_engine(const nnb_render_args* a) {
+  const size_t need = nnb_render_frame_bwd_workspace_bytes_engine(a->N, a->S, a->hidden_dim, a->engine);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  return 0;
+}
+// The _engine forms: NNB_ENGINE_TC is the call without the suffix (its checks, bits and workspace); NNB_ENGINE_SIMT runs the exact engine
+// at any S from 2 to 1024 (check_frame accepts S < 16 there) with the same checks in the same order.
+int nnb_render_frame_bwd_engine(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (int rc = check_frame_bwd_engine(a->engine, "nnb_render_frame_bwd_engine")) return rc;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) return nnb_render_frame_bwd(b, stream);
+#endif
+  if (int rc = check_frame(a)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_frame_bwd: g_rgb and g_c2w must be non-null");
+  if (int rc = check_frame_bwd_ws_engine(a)) return rc;
+  const cudaError_t e = simt_render_frame_bwd(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_bwd_engine");
+}
+int nnb_render_frame_train_fwd_engine(const nnb_render_args* a, void* stream) {
+  if (!a) return fail(-1, "null args");
+  if (int rc = check_frame_bwd_engine(a->engine, "nnb_render_frame_train_fwd_engine")) return rc;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) return nnb_render_frame_train_fwd(a, stream);
+#endif
+  if (int rc = check_frame(a, true)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (int rc = check_frame_bwd_ws_engine(a)) return rc;
+  const cudaError_t e = simt_render_frame_train_fwd(*a, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_fwd_engine");
+}
+int nnb_render_frame_train_bwd_engine(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (int rc = check_frame_bwd_engine(a->engine, "nnb_render_frame_train_bwd_engine")) return rc;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) return nnb_render_frame_train_bwd(b, stream);
+#endif
+  if (int rc = check_frame(a, true)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_frame_train_bwd: g_rgb and g_c2w must be non-null");
+  if (int rc = check_frame_bwd_ws_engine(a)) return rc;
+  const cudaError_t e = simt_render_frame_train_bwd(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_bwd_engine");
 }
 int nnb_field_bwd(const nnb_render_args* a, const float* g_rgba, float* g_pts, float* g_dirs, float* g_weights, void* stream) {
   int rc = check_field(a); if (rc) return rc;

@@ -347,6 +347,10 @@ __device__ __forceinline__ void ray_adjoint(const nnb_render_bwd_args& b, int n,
 // it was.  carry_s is the suffix sum of w gw over the later chunks on entry, and includes this chunk on return; it is carried from chunk to
 // chunk and never formed as total - prefix (DESIGN.md §4).  df = d alpha / d a.  Returns (w gC0, w gC1, w gC2, d L / d a) of the lane's
 // sample, zeros for an invalid lane.
+// FUSED: d L / d alpha = T gw - suffix / om as one fma, which is what nvcc 12.9 makes of composite_bwd's statement; the exact engine's frame
+// (FUSED = true) spells it so that at S <= 32 its gradients are nnb_render_bwd's bits.  FUSED = false is the statement as written, which
+// this copy compiles to a product and a subtraction: the tensor-core frame's form, kept as it was.
+template <bool FUSED = false>
 __device__ __forceinline__ float4 composite_chunk_bwd(float alpha, bool valid, float r, float g, float b, float z, float df, int lane, float carry,
                                                       float gC0, float gC1, float gC2, float gD, float gsum, float& carry_s) {
   const float om = valid ? __fadd_rn(__fsub_rn(1.f, alpha), NNB_EPS) : 1.f;
@@ -360,6 +364,6 @@ __device__ __forceinline__ float4 composite_chunk_bwd(float alpha, bool valid, f
   float excl = __shfl_down_sync(0xffffffffu, incl, 1); if (lane == 31) excl = 0.f;
   const float suffix = excl + carry_s;
   carry_s += __shfl_sync(0xffffffffu, incl, 0);
-  const float g_alpha = T * gw - suffix / om;
+  const float g_alpha = FUSED ? fmaf(T, gw, -(suffix / om)) : T * gw - suffix / om;
   return valid ? make_float4(w * gC0, w * gC1, w * gC2, g_alpha * df) : make_float4(0.f, 0.f, 0.f, 0.f);
 }

@@ -104,22 +104,30 @@ cudaError_t run_render_frame(const nnb_render_args& a, const FrameWs& w, float t
 }
 
 
-// ---- nnb_render_frame_bwd (the differentiable frame, t_min = 0, tensor-core engine): the forward above with checkpoints, then reverse
-// rounds k = C - 1 .. 0 (C = ceil(S / 32)).  Round k evaluates chunk k of every ray again with a chunk-sized training stash (ray n's chunk
-// is rows 32 n .. 32 n + 31 of it), runs frame_chunk_adjoint, the data-gradient chain and the weight-gradient stage on it, and adds the
-// chunk's point and direction adjoints to the ray's lane partials (frame_ray_acc).  frame_ray_finish then forms each ray's pose adjoint
-// from them as ray_bwd does.  Every sum runs in a fixed order: chunk by chunk from the last, in the lanes of composite_bwd / ray_bwd.
+// ---- nnb_render_frame_bwd (the differentiable frame, t_min = 0, either engine): the forward above with checkpoints, then reverse
+// rounds k = C - 1 .. 0 (C = ceil(S / 32)).  Round k evaluates chunk k of every ray again with a chunk-sized training stash, runs
+// frame_chunk_adjoint, the data-gradient chain and the weight-gradient stage on it, and adds the chunk's point and direction adjoints to
+// the ray's lane partials (frame_ray_acc).  frame_ray_finish then forms each ray's pose adjoint from them as ray_bwd does.  Every sum runs
+// in a fixed order: chunk by chunk from the last, in the lanes of composite_bwd / ray_bwd.
+// Rows of the chunk stash: ray n owns R consecutive rows, row R n + j is sample 32 k + j.  The tensor-core engine pads every ray to R = 32
+// rows (PACKED = false); the exact engine packs them, R = min(S, 32) (PACKED = true), so that at S < 32 a round evaluates N S rows.
 struct FrameBwdPtrs {
   int k, rounds;          // this round's chunk; C
   const float* ckpt;      // [C - 1][N]: transmittance into chunk k + 1 (after chunk k) of every ray, written by the forward
   float* suffix;          // [N] carry_s of composite_chunk_bwd between rounds
-  const SampleRec* rec;   // [32 N] records of the chunk (the chunk stash)
-  float4* gs;             // [32 N] d / d (rgb, a) of the chunk's samples
-  const float4 *gp, *gv;  // [32 N] d / d p and d / d viewdir of the chunk's samples
+  const SampleRec* rec;   // [R N] records of the chunk (the chunk stash)
+  float4* gs;             // [R N] d / d (rgb, a) of the chunk's samples
+  const float4 *gp, *gv;  // [R N] d / d p and d / d viewdir of the chunk's samples
   float* raypart;         // [N][9][32] lane partials of ray_bwd's so, sd, sv
 };
 
-// one warp per ray, lane = sample 32 k + lane: composite_bwd's adjoint of chunk k, the suffix of the later chunks carried in f.suffix
+// rows per ray of the chunk stash (see above)
+template <bool PACKED> __device__ __forceinline__ int chunk_rows(const nnb_render_args& a) { return PACKED ? min(a.S, 32) : 32; }
+
+// one warp per ray, lane = sample 32 k + lane: composite_bwd's adjoint of chunk k, the suffix of the later chunks carried in f.suffix.
+// A packed ray has no row for a lane past its last sample (lane >= R only when S < 32): that lane writes nothing.  The exact engine's
+// instantiation (PACKED) takes composite_bwd's fused form of d L / d alpha (composite_chunk_bwd<true>).
+template <bool PACKED>
 __global__ void frame_chunk_adjoint(nnb_render_bwd_args b, const __grid_constant__ FrameBwdPtrs f) {
   const nnb_render_args& a = b.fwd;
   const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -131,7 +139,8 @@ __global__ void frame_chunk_adjoint(nnb_render_bwd_args b, const __grid_constant
   const float gsum = (a.flags & NNB_WHITE_BG) ? (gC0 + gC1 + gC2) : 0.f;
   const int i = 32 * f.k + lane;
   const bool valid = i < a.S;
-  const size_t m = (size_t)n * 32 + lane;
+  const int R = chunk_rows<PACKED>(a);
+  const size_t m = (size_t)n * R + lane;
   const SampleRec me = valid ? f.rec[m] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
   float alpha = 0.f, df = 1.f;   // df = d alpha / d a
   if (valid) {
@@ -143,12 +152,14 @@ __global__ void frame_chunk_adjoint(nnb_render_bwd_args b, const __grid_constant
   }
   const float carry = f.k > 0 ? f.ckpt[(size_t)(f.k - 1) * a.N + n] : 1.f;
   float carry_s = f.k == f.rounds - 1 ? 0.f : f.suffix[n];
-  f.gs[m] = composite_chunk_bwd(alpha, valid, me.r, me.g, me.b, me.z, df, lane, carry, gC0, gC1, gC2, gD, gsum, carry_s);
+  const float4 g = composite_chunk_bwd<PACKED>(alpha, valid, me.r, me.g, me.b, me.z, df, lane, carry, gC0, gC1, gC2, gD, gsum, carry_s);
+  if (!PACKED || lane < R) f.gs[m] = g;
   if (lane == 0) f.suffix[n] = carry_s;
 }
 
 // one warp per ray: the chunk's terms of ray_bwd's lane sums (lane = sample 32 k + lane), added to the ray's lane partials (written by the
 // first round, k = C - 1)
+template <bool PACKED>
 __global__ void frame_ray_acc(nnb_render_args a, const __grid_constant__ FrameBwdPtrs f) {
   const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (n >= a.N) return;
@@ -156,8 +167,8 @@ __global__ void frame_ray_acc(nnb_render_args a, const __grid_constant__ FrameBw
   float v[9];
 #pragma unroll
   for (int c = 0; c < 9; ++c) v[c] = f.k == f.rounds - 1 ? 0.f : part[32 * c];
-  if (32 * f.k + lane < a.S) {
-    const size_t m = (size_t)n * 32 + lane;
+  if (32 * f.k + lane < a.S) {   // a packed ray's rows: lane < R
+    const size_t m = (size_t)n * chunk_rows<PACKED>(a) + lane;
     const float4 g = f.gp[m], dv = f.gv[m];
     const float z = f.rec[m].z;
     v[0] += g.x; v[1] += g.y; v[2] += g.z;
@@ -184,7 +195,7 @@ __global__ void frame_ray_finish(nnb_render_bwd_args b, const float* __restrict_
 
 // Workspace of nnb_render_frame_bwd, every section 256-byte aligned: frame_layout_bytes(N, img_bytes) (the forward, with the engine's forward
 // weight image) | checkpoints [C - 1][N] | suffix carries [N] | ray lane partials [N][9][32] | the chunk stash (chunk_bytes: the records,
-// training stash, gate bits, per-ray reduction and weight-gradient partials of 32 N samples) | the engine's transposed weight image.  Only
+// training stash, gate bits, per-ray reduction and weight-gradient partials of R N samples) | the engine's transposed weight image.  Only
 // the checkpoints grow with S: 4 bytes per ray and chunk.
 struct FrameBwdWs { FrameWs f; size_t ckpt, suffix, raypart, chunk, img_t, total; };
 inline FrameBwdWs frame_bwd_layout_bytes(int N, int S, size_t img_bytes, size_t chunk_bytes, size_t img_t_bytes) {

@@ -156,7 +156,9 @@ __device__ __forceinline__ void row_geometry(const nnb_render_args& a, size_t m,
 // SF_FRAME (simt_frame, nnb_render_frame on this engine): SF_RAYS on the rows frame_row gives (M = N S), with nothing stashed and no
 // record.  The colour head puts each row's (r, g, b, a) in a row area at the start of oth, and the CTA's warps take the tile's
 // ray-chunks in turn through frame_step (nnb_frame.cuh).  fr / n_live: the round and its ray-chunk count.
-enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2, SF_FRAME = 3 };
+// SF_CHUNK (simt_frame_stash, nnb_render_frame_bwd on this engine): SF_RAYS with the stash and records on the rows of chunk fr.k of every
+// ray (chunk_row); geometry, view direction and the record's z come from the row's sample, stores go to the row.
+enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2, SF_FRAME = 3, SF_CHUNK = 4 };
 
 // Row `row` of frame tile `tile`: a ray-chunk is R = min(S, 32) rows and a tile holds 64 / R of them, so row r is sample 32 fr.k + r % R
 // of the ray in slot (64 / R) tile + r / R of the round.  Slots past the round's last repeat it, rows past a ray's last sample evaluate
@@ -166,6 +168,16 @@ __device__ __forceinline__ size_t frame_row(const nnb_render_args& a, const Fram
   const int slot = min((TM / R) * (int)tile + row / R, n_live - 1);
   const int n = fr.list ? fr.list[slot] : slot;
   return (size_t)n * a.S + min(32 * fr.k + row % R, a.S - 1);
+}
+
+// Row m of chunk k's stash (nnb_render_frame_bwd on this engine, nnb_frame.cuh): ray n owns R = min(S, 32) consecutive rows, row R n + j
+// is sample 32 k + j of ray n, clamped to the ray's last sample; rows past the last ray (the Mpad tail) repeat row R N - 1, and no later
+// stage reads them.  Returns the sample's row n S + i in nnb_render_fwd's order, which is m itself at S <= 32.
+__device__ __forceinline__ size_t chunk_row(const nnb_render_args& a, int k, size_t m) {
+  const int R = min(a.S, 32);
+  const size_t last = (size_t)a.N * R - 1;
+  if (m > last) m = last;
+  return (m / R) * a.S + min(32 * k + (int)(m % R), a.S - 1);
 }
 
 // one 64-row tile of the exact forward: rows m0 = 64 tile .. m0 + 63 of M
@@ -178,7 +190,9 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
   const int tid = threadIdx.x;
   const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
-  auto row_m = [&](int row) { return MODE == SF_FRAME ? frame_row(a, fr, tile, row, n_live) : m0 + row; };
+  auto row_m = [&](int row) {
+    return MODE == SF_FRAME ? frame_row(a, fr, tile, row, n_live) : MODE == SF_CHUNK ? chunk_row(a, fr.k, m0 + row) : m0 + row;
+  };
   {  // prologue: encode positions into columns D..D+63 of both buffers
     int row = tid & 63, part = tid >> 6;
     Ray ray; int n, i; float z, p[3];
@@ -209,7 +223,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
     }
   }
   __syncthreads();
-  if (MODE == SF_RAYS && stash) {
+  if ((MODE == SF_RAYS || MODE == SF_CHUNK) && stash) {
     for (int idx = tid; idx < TM * 16; idx += 256) {
       int row = idx >> 4, c4 = idx & 15;
       *reinterpret_cast<float4*>(P.enc + (m0 + row) * 64 + c4 * 4) = *reinterpret_cast<const float4*>(buf0 + row * LDB + D + c4 * 4);
@@ -222,7 +236,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
     int kvalid = (l == 0) ? 63 : (l == 4 ? D + 63 : D);
     tile_gemm<NJ, false, 1, false>(in, LDB, K, w + nnb::w_off(D, l), nnb::w_ld(D, l), D, kvalid, w + nnb::b_off(D, l), oth, LDB, Ws);
     __syncthreads();
-    if (MODE == SF_RAYS && stash) tile_to_global(oth, LDB, P.h[l], m0, D);
+    if ((MODE == SF_RAYS || MODE == SF_CHUNK) && stash) tile_to_global(oth, LDB, P.h[l], m0, D);
     float* t_ = cur; cur = oth; oth = t_;
   }
   // cur = h8.  density head: 4 threads per row
@@ -287,7 +301,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
       if (hc < 3) rec[hc] = val;
       else {
         Ray ray; int n, i; float z, p[3], sigma;
-        row_geometry(a, m0 + hrow, M, ray, n, i, z, p);
+        row_geometry(a, row_m(hrow), M, ray, n, i, z, p);
         rec[3] = density_act(s_logit, a.flags, &sigma);
         rec[4] = s_logit; rec[5] = z; rec[6] = 0.f; rec[7] = 0.f;
       }
@@ -356,6 +370,13 @@ __global__ void __launch_bounds__(256, 1) simt_frame(nnb_render_args a, const __
     simt_fwd_tile<D, SF_FRAME>(a, SimtPtrs{}, (size_t)a.N * a.S, 0, tile, MarchPtrs{}, 0, 0, nullptr, f, n_live);
     __syncthreads();   // the back end is done with the row area before the next tile's prologue writes the buffers
   }
+}
+
+// one reverse round of nnb_render_frame_bwd on this engine: chunk f.k of every ray, records and the training stash of its R N rows
+// (chunk_row), one 64-row tile per CTA
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_frame_stash(nnb_render_args a, SimtPtrs P, const __grid_constant__ FramePtrs f) {
+  simt_fwd_tile<D, SF_CHUNK>(a, P, (size_t)a.N * a.S, 1, blockIdx.x, MarchPtrs{}, 0, 0, nullptr, f);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -458,9 +479,15 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
 // ---------------------------------------------------------------------------------------
 // B2: data-gradient chain
 // ---------------------------------------------------------------------------------------
+// MODE of simt_dgrad_tile: DG_ROWS (simt_mlp_dgrad): row m is sample m.  DG_CHUNK (simt_dgrad_chunk, nnb_render_frame_bwd on this engine):
+// the rows of chunk `chunk`'s stash as simt_frame_stash wrote them: row_geometry and row_view_dir take the row's sample chunk_row(a,
+// chunk, m), everything else the row.
+enum : int { DG_ROWS = 0, DG_CHUNK = 1 };
+
 // one 64-row tile of the chain: rows m0 = 64 tile .. m0 + 63 of M
-template <int D>
-__device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int write_dy, unsigned tile) {
+template <int D, int MODE = DG_ROWS>
+__device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int write_dy, unsigned tile,
+                                                int chunk = 0) {
   constexpr int LDB = ldb<D>(), NJ = D / 64, DR = D / 2;
   extern __shared__ __align__(16) float smem[];
   float* bufA = smem; float* bufB = bufA + TM * LDB; float* Ws = bufB + TM * LDB;
@@ -469,6 +496,9 @@ __device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const 
   const int tid = threadIdx.x;
   const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
+  // the row's sample for the geometry (DG_CHUNK: M counts the chunk's rows, the samples are the N S of the render)
+  auto row_s = [&](int row) { return MODE == DG_CHUNK ? chunk_row(a, chunk, m0 + row) : m0 + row; };
+  const size_t MS = MODE == DG_CHUNK ? (size_t)a.N * a.S : M;
   {  // 1. head adjoints
     int row = tid >> 2, c = tid & 3; size_t m = m0 + row;
     float4 g = (m < M) ? P.gs[m] : make_float4(0, 0, 0, 0);
@@ -497,8 +527,8 @@ __device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const 
   if (write_dy) tile_to_global(bufB, LDB, P.dfeat, m0, D);
   if (tid < TM) {
     Ray ray; int n, i; float z, p[3], v[3], gvd[3];
-    row_geometry(a, m0 + tid, M, ray, n, i, z, p);
-    row_view_dir(a, m0 + tid, M, ray, v);
+    row_geometry(a, row_s(tid), MS, ray, n, i, z, p);
+    row_view_dir(a, row_s(tid), MS, ray, v);
     const float* ge = bufB + tid * LDB + D;
     encode_bwd<4>(v, [&](int k) { return ge[k]; }, gvd);
     P.gv[m0 + tid] = make_float4(gvd[0], gvd[1], gvd[2], 0.f);
@@ -536,7 +566,7 @@ __device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const 
   // 6. encoding adjoint
   if (tid < TM) {
     Ray ray; int n, i; float z, p[3], gp[3];
-    row_geometry(a, m0 + tid, M, ray, n, i, z, p);
+    row_geometry(a, row_s(tid), MS, ray, n, i, z, p);
     const float* ge = genc + tid * 64;
     encode_bwd<10>(p, [&](int k) { return ge[k]; }, gp);
     P.gp[m0 + tid] = make_float4(gp[0], gp[1], gp[2], 0.f);
@@ -546,6 +576,12 @@ __device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const 
 template <int D>
 __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, SimtPtrs P, size_t M, int write_dy) {
   simt_dgrad_tile<D>(a, P, M, write_dy, blockIdx.x);
+}
+
+// the chain of one reverse round of nnb_render_frame_bwd on this engine, on chunk k's stash (M = R N rows, R = min(S, 32))
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_dgrad_chunk(nnb_render_args a, SimtPtrs P, size_t M, int write_dy, int k) {
+  simt_dgrad_tile<D, DG_CHUNK>(a, P, M, write_dy, blockIdx.x, k);
 }
 
 // Device-count form of simt_mlp_dgrad (the normals of nnb_geometry_frame on this engine), rows as in simt_mlp_fwd_n: the chain on the
@@ -1007,6 +1043,8 @@ static cudaError_t simt_init_dim() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_march<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_secant<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_frame_stash<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_dgrad_chunk<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -1228,26 +1266,110 @@ cudaError_t simt_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t 
 // evaluates it) and frame_step sums the lane terms in composite_fwd's order, so at t_min = 0 the outputs are nnb_render_fwd's bits.
 size_t simt_render_frame_workspace(int N) { return frame_layout_bytes(N, 0).total; }
 
+// the persistent grid of simt_frame for a: every CTA the SMs hold, at most one per tile (0 on an error, in *e)
 template <int D>
-static cudaError_t simt_render_frame_dim(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, cudaStream_t st) {
-  cudaError_t e = simt_init();
-  if (e != cudaSuccess) return e;
+static int simt_frame_grid(const nnb_render_args& a, cudaError_t* e) {
+  *e = simt_init();
+  if (*e != cudaSuccess) return 0;
   static int slots = 0;   // CTAs of simt_frame resident on the device at once
   if (!slots) {
     int dev = 0, n_sm = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, simt_frame<D>, 256, fwd_smem<D>());
-    if (e != cudaSuccess) return e;
+    *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, simt_frame<D>, 256, fwd_smem<D>());
+    if (*e != cudaSuccess) return 0;
     slots = n_sm * (per_sm > 0 ? per_sm : 1);
   }
-  const int per = TM / (a.S < 32 ? a.S : 32), tiles = (a.N + per - 1) / per, grid = tiles < slots ? tiles : slots;
+  const int per = TM / (a.S < 32 ? a.S : 32), tiles = (a.N + per - 1) / per;
+  return tiles < slots ? tiles : slots;
+}
+
+template <int D>
+static cudaError_t simt_render_frame_dim(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, cudaStream_t st) {
+  cudaError_t e;
+  const int grid = simt_frame_grid<D>(a, &e);
+  if (e != cudaSuccess) return e;
   return run_render_frame(a, frame_layout_bytes(a.N, 0), t_min, n_eval, t_final, st,
                           [&](const FramePtrs& f) { simt_frame<D><<<grid, 256, fwd_smem<D>(), st>>>(a, f); });
 }
 cudaError_t simt_render_frame(const nnb_render_args& a, float t_min, int* n_eval, float* t_final, int D, cudaStream_t st) {
   return D == 128 ? simt_render_frame_dim<128>(a, t_min, n_eval, t_final, st)
        : D == 64  ? simt_render_frame_dim<64>(a, t_min, n_eval, t_final, st) : simt_render_frame_dim<256>(a, t_min, n_eval, t_final, st);
+}
+
+// ---- nnb_render_frame_bwd on this engine (nnb_render_frame_bwd_engine, nnb_render_frame_train_fwd_engine / _bwd_engine): the rounds of
+// nnb_frame.cuh with the exact kernels.  The chunk stash packs R = min(S, 32) rows per ray (frame_chunk_adjoint<true>), so at S <= 32 it
+// holds nnb_render_fwd's rows in nnb_render_fwd's order, and its weight-gradient stage has the stash path's M and split count.  Workspace:
+// frame_bwd_layout_bytes without weight images, the chunk stash make_layout(N, R, NNB_STASH, NNB_ENGINE_SIMT, D).
+static FrameBwdWs simt_frame_bwd_layout(int N, int S, int D) {
+  return frame_bwd_layout_bytes(N, S, 0, make_layout(N, S < 32 ? S : 32, NNB_STASH, NNB_ENGINE_SIMT, D).total, 0);
+}
+size_t simt_render_frame_bwd_workspace(int N, int S, int D) { return simt_frame_bwd_layout(N, S, D).total; }
+
+// The forward half: run_render_frame with simt_frame at t_min = 0 (every ray runs every round), the carry after each chunk but the last
+// copied to the checkpoints.  It leaves the checkpoints in the workspace for the reverse half.
+template <int D>
+static cudaError_t simt_frame_train_fwd_dim(const nnb_render_args& a, cudaStream_t st) {
+  cudaError_t e;
+  const int grid = simt_frame_grid<D>(a, &e);
+  if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32;
+  const FrameBwdWs w = simt_frame_bwd_layout(N, a.S, D);
+  float* ckpt = reinterpret_cast<float*>(static_cast<char*>(a.workspace) + w.ckpt);
+  cudaError_t ec = cudaSuccess;
+  e = run_render_frame(a, w.f, 0.f, nullptr, nullptr, st, [&](const FramePtrs& f) {
+    simt_frame<D><<<grid, 256, fwd_smem<D>(), st>>>(a, f);
+    if (f.k + 1 < C && ec == cudaSuccess) ec = cudaMemcpyAsync(ckpt + (size_t)f.k * N, f.carry, (size_t)N * 4, cudaMemcpyDeviceToDevice, st);
+  });
+  return e == cudaSuccess ? ec : e;
+}
+
+// The reverse half: rounds k = C - 1 .. 0, each on the chunk stash: simt_frame_stash, frame_chunk_adjoint, simt_dgrad_chunk, (g_weights)
+// simt_wgrad_all, whose reduce adds the round's dW into g_weights, and frame_ray_acc; then frame_ray_finish and ray_reduce.  Of what the
+// forward half wrote it reads the checkpoints only (data, no index or counter), so a workspace the forward half did not fill gives wrong
+// numbers, never an access outside the workspace.
+template <int D>
+static cudaError_t simt_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+  const nnb_render_args& a = b.fwd;
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32, R = a.S < 32 ? a.S : 32;
+  const FrameBwdWs w = simt_frame_bwd_layout(N, a.S, D);
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  const WsLayout L = make_layout(N, R, NNB_STASH, NNB_ENGINE_SIMT, D);   // offsets from the chunk stash's own base
+  const SimtPtrs P = make_ptrs(L, base + w.chunk);
+  FrameBwdPtrs fb{};
+  fb.rounds = C; fb.ckpt = F(w.ckpt); fb.suffix = F(w.suffix); fb.rec = P.rec;
+  fb.gs = P.gs; fb.gp = P.gp; fb.gv = P.gv; fb.raypart = F(w.raypart);
+  const int write_dy = b.g_weights ? 1 : 0, warps = (N + 7) / 8, tiles = (int)((L.M + TM - 1) / TM);
+  for (int k = C - 1; k >= 0; --k) {
+    FramePtrs f{};
+    f.k = k;
+    fb.k = k;
+    simt_frame_stash<D><<<tiles, 256, fwd_smem<D>(), st>>>(a, P, f);
+    frame_chunk_adjoint<true><<<warps, 256, 0, st>>>(b, fb);
+    simt_dgrad_chunk<D><<<tiles, 256, bwd_smem<D>(), st>>>(a, P, L.M, write_dy, k);
+    e = cudaGetLastError();
+    if (e == cudaSuccess && b.g_weights) e = simt_wgrad_all(P, L, b.g_weights, st);
+    if (e != cudaSuccess) return e;
+    frame_ray_acc<true><<<warps, 256, 0, st>>>(a, fb);
+  }
+  frame_ray_finish<<<warps, 256, 0, st>>>(b, F(w.raypart), P.rayred);
+  ray_reduce<<<1, 512, 0, st>>>(b, P.rayred);
+  return cudaGetLastError();
+}
+
+cudaError_t simt_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStream_t st) {
+  return D == 128 ? simt_frame_train_fwd_dim<128>(a, st) : (D == 64 ? simt_frame_train_fwd_dim<64>(a, st) : simt_frame_train_fwd_dim<256>(a, st));
+}
+cudaError_t simt_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  return D == 128 ? simt_frame_train_bwd_dim<128>(b, st) : (D == 64 ? simt_frame_train_bwd_dim<64>(b, st) : simt_frame_train_bwd_dim<256>(b, st));
+}
+// nnb_render_frame_bwd_engine on this engine: the two halves in sequence
+cudaError_t simt_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  const cudaError_t e = simt_render_frame_train_fwd(b.fwd, D, st);
+  return e != cudaSuccess ? e : simt_render_frame_train_bwd(b, D, st);
 }
 
 // jobs -> simt_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent

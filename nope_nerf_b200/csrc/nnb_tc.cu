@@ -2019,12 +2019,12 @@ cudaError_t tc_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st
     f.k = k;
     fb.k = k;
     tc_frame_stash<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, ts, f, tiles);
-    frame_chunk_adjoint<<<warps, 256, 0, st>>>(b, fb);
+    frame_chunk_adjoint<false><<<warps, 256, 0, st>>>(b, fb);
     tc_dgrad_frame<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)N * 32, tiles, write_dy, k);
     e = cudaGetLastError();
     if (e == cudaSuccess && b.g_weights) e = tc_wgrad_jobs(ac, L, b.g_weights, false, true, st);
     if (e != cudaSuccess) return e;
-    frame_ray_acc<<<warps, 256, 0, st>>>(a, fb);
+    frame_ray_acc<false><<<warps, 256, 0, st>>>(a, fb);
   }
   float* rayred = CF(L.rayred);
   frame_ray_finish<<<warps, 256, 0, st>>>(b, F(w.raypart), rayred);

@@ -16,6 +16,15 @@ from ..field import ray_march, needs_grad, _engine_id, geometry_frame as field_g
 GEOMETRY_CHUNK = 1024
 
 
+def _frame_grad_engine(value, frame_grad, owner):
+    """the frame_grad_engine keyword of Renderer / Trainer: None, 'tc' or 'simt', and only together with frame_grad=True"""
+    if value not in (None, 'tc', 'simt'):
+        raise ValueError("%s: frame_grad_engine must be None, 'tc' or 'simt' (got %r)" % (owner, value))
+    if value is not None and not frame_grad:
+        raise ValueError("%s: frame_grad_engine needs frame_grad=True" % owner)
+    return value
+
+
 class Renderer(nn.Module):
     def __init__(self, model, cfg, device=None, **kwargs):
         super().__init__()
@@ -77,6 +86,9 @@ class Renderer(nn.Module):
         # only, without jitter: such a render with add_noise on uniform sampling, or on the SIMT engine, is a ValueError.  Its output
         # dict has z_vals and alpha None (the frame keeps no per-sample values).  Off by default.
         self.frame_grad = bool(kwargs.get("frame_grad", False))
+        # frame_grad_engine: None or 'tc' keeps those renders on the tensor-core engine; 'simt' runs them on the exact-fp32 engine
+        # (nnb_render_frame_bwd_engine, any sample count from 2 to 1024, whatever `engine` says), still without jitter.  Needs frame_grad.
+        self.frame_grad_engine = _frame_grad_engine(kwargs.get("frame_grad_engine", None), self.frame_grad, "Renderer")
 
     def to(self, device):
         model = super().to(device)
@@ -132,7 +144,8 @@ class Renderer(nn.Module):
             if noise is not None:
                 raise ValueError("Renderer(frame_grad=True) renders without jitter: call with add_noise=False or use ndc sampling")
             meta.update(want_z_alpha=False, noise=None)
-            rgb, dp, dg, mask = ops.render_frame_grad(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))
+            rgb, dp, dg, mask = ops.render_frame_grad(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()),
+                                                      frame_engine=L.ENGINE_SIMT if self.frame_grad_engine == 'simt' else None)
             z = alpha = None
         else:
             rgb, dp, dg, mask, z, alpha = ops.render_autograd(meta, flat, c2w, cam, d, None, None, list(self.model.parameters()))

@@ -21,7 +21,7 @@ from .. import ops
 from .. import _lib as L
 from .losses import Loss
 from .common import arange_pixels
-from .rendering import GEOMETRY_CHUNK
+from .rendering import GEOMETRY_CHUNK, _frame_grad_engine
 
 logger_py = logging.getLogger(__name__)
 
@@ -320,7 +320,7 @@ class _GraphStep:
         n_local = ray_idx.shape[0]
         flags = ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=False, shift_first=tr.shift_first)
         ndc = rend.cfg['sample_option'] == 'ndc'
-        render_call = ops.FrameRenderCall if tr.frame_grad else ops.RenderCall
+        render_call = tr._train_render_call(True)
         call = render_call(net.flat_weights(), self.c2w, self.cam, N=n_local, S=S, flags=flags,
                            engine=rend.engine if rend.engine is not None else ops.default_engine(),
                            near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],
@@ -520,7 +520,10 @@ class Trainer(object):
     Its workspace grows with rendering.num_points by one float per ray and 32-sample chunk instead of the per-sample stash, and it takes
     the jitter of sample_option 'uniform'.  The renderer's engine and rendering.num_points must resolve to the tensor-core engine
     (ValueError otherwise).  Renders without a backward are unchanged.  This is a Trainer keyword, not a reading of
-    Renderer(frame_grad=...): that flag governs Renderer.nope_nerf, which the Trainer does not call."""
+    Renderer(frame_grad=...): that flag governs Renderer.nope_nerf, which the Trainer does not call.
+    frame_grad_engine (default None, needs frame_grad=True): 'simt' runs those renders on the exact-fp32 engine's pair,
+    ops.ExactFrameRenderCall, at any rendering.num_points from 2 to 1024 whatever the renderer's engine; None or 'tc' is the tensor-core
+    pair above."""
 
     def __init__(self, model, optimizer, cfg, device=None, optimizer_pose=None, pose_param_net=None,
                  optimizer_focal=None, focal_net=None, optimizer_distortion=None, distortion_net=None, **kwargs):
@@ -586,7 +589,11 @@ class Trainer(object):
         # 'auto' = randperm when running eagerly, hash inside the CUDA graph (whose RNG stream differs from eager anyway)
         self.pixel_sampler = kwargs.get('pixel_sampler', 'auto')
         self.frame_grad = bool(kwargs.get('frame_grad', False))
-        if self.frame_grad:
+        self.frame_grad_engine = _frame_grad_engine(kwargs.get('frame_grad_engine', None), self.frame_grad, "Trainer")
+        if self.frame_grad_engine == 'simt':
+            if not 2 <= int(model.renderer.cfg['num_points']) <= 1024:
+                raise ValueError("Trainer(frame_grad_engine='simt') needs rendering.num_points in 2..1024")
+        elif self.frame_grad:
             rend = model.renderer
             engine = rend.engine if rend.engine is not None else ops.default_engine()
             if ops.pick_engine(engine, int(rend.cfg['num_points'])) != L.ENGINE_TC:
@@ -594,6 +601,12 @@ class Trainer(object):
                                  "(16..1024) must resolve to it")
 
     # ------------------------------------------------------------------------------------
+    def _train_render_call(self, backward):
+        """the RenderCall class of a training render: the differentiable frame's pair (frame_grad) when it has a backward"""
+        if not (self.frame_grad and backward):
+            return ops.RenderCall
+        return ops.ExactFrameRenderCall if self.frame_grad_engine == 'simt' else ops.FrameRenderCall
+
     def _smoothness_on(self):
         """the pose-smoothness terms have a non-zero weight somewhere on their annealing schedule"""
         return any(float(v) != 0.0 for v in list(self.weight_dist_1st_loss) + list(self.weight_dist_2nd_loss))
@@ -889,7 +902,7 @@ class Trainer(object):
             ops.pose_fwd_raw(pose.r.detach(), pose.t.detach(), init, img_idx, c2w)
             flags = ops.flags_from_cfg(rend.cfg, net.occ_activation, eval_=eval_mode, shift_first=self.shift_first)
             ndc = rend.cfg['sample_option'] == 'ndc'
-            render_call = ops.FrameRenderCall if self.frame_grad and backward else ops.RenderCall
+            render_call = self._train_render_call(backward)
             call = render_call(net.flat_weights(), c2w, cam_dev, N=n_local, S=S, flags=flags,
                                engine=rend.engine if rend.engine is not None else ops.default_engine(),
                                near=0.0 if ndc else rend.depth_range[0], far=1.0 if ndc else rend.depth_range[1],

@@ -89,15 +89,20 @@ _pool = _WorkspacePool()
 
 class RenderCall:
     """One forward launch + the state its backward needs (workspace with the stash)."""
-    frame = False   # FrameRenderCall: the differentiable frame's training pair
+    frame = False         # FrameRenderCall: the differentiable frame's training pair
+    exact_frame = False   # ExactFrameRenderCall: that pair on the exact-fp32 engine
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
                  depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256):
-        frame = self.frame
+        frame, exact = self.frame, self.exact_frame
         if frame:
             if want_z_alpha:
                 raise ValueError("FrameRenderCall: want_z_alpha is not supported (no per-sample outputs)")
-            if pick_engine(engine, S) != L.ENGINE_TC:
+            if exact:
+                if not 2 <= S <= 1024:
+                    raise ValueError("ExactFrameRenderCall needs 2 <= S <= 1024 (got %d)" % S)
+                engine = L.ENGINE_SIMT
+            elif pick_engine(engine, S) != L.ENGINE_TC:
                 raise ValueError("FrameRenderCall runs on the tensor-core engine only (16 <= S <= 1024)")
             stash = True
         for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels),
@@ -125,7 +130,9 @@ class RenderCall:
         self.alpha = torch.empty(N, S, device=dev) if want_z_alpha else None
         a.rgb = L.ptr(self.rgb); a.depth_pred = L.ptr(self.depth_pred); a.depth_gt = L.ptr(self.depth_gt)
         a.mask = L.ptr(self.mask); a.z_vals = L.ptr(self.z_vals); a.alpha = L.ptr(self.alpha)
-        if frame:
+        if exact:
+            nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes_engine(N, S, int(hidden_dim), engine)
+        elif frame:
             nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, int(hidden_dim))
         else:
             nbytes = L.lib.nnb_workspace_bytes_dim(N, S, flags, engine, int(hidden_dim))
@@ -134,7 +141,9 @@ class RenderCall:
         self.ws = _pool.take(nbytes, dev)
         a.workspace = L.ptr(self.ws); a.workspace_bytes = self.ws.numel()
         self.args = a; self.N = N; self.S = S; self.stash = stash; self.pooled = True
-        if frame:
+        if exact:
+            L.check(L.lib.nnb_render_frame_train_fwd_engine(C.byref(a), _stream()), "nnb_render_frame_train_fwd_engine")
+        elif frame:
             L.check(L.lib.nnb_render_frame_train_fwd(C.byref(a), _stream()), "nnb_render_frame_train_fwd")
         else:
             L.check(L.lib.nnb_render_fwd(C.byref(a), _stream()), "nnb_render_fwd")
@@ -156,7 +165,9 @@ class RenderCall:
         b.g_rgb, b.g_depth_pred, b.g_depth_gt = L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2])
         b.g_weights = L.ptr(g_weights); b.g_c2w = L.ptr(g_c2w); b.g_cam = L.ptr(g_cam); b.g_depth = L.ptr(g_depth)
         b.g_scale_shift = L.ptr(g_scale_shift)
-        if self.frame:
+        if self.exact_frame:
+            L.check(L.lib.nnb_render_frame_train_bwd_engine(C.byref(b), _stream()), "nnb_render_frame_train_bwd_engine")
+        elif self.frame:
             L.check(L.lib.nnb_render_frame_train_bwd(C.byref(b), _stream()), "nnb_render_frame_train_bwd")
         else:
             L.check(L.lib.nnb_render_bwd(C.byref(b), _stream()), "nnb_render_bwd")
@@ -171,6 +182,14 @@ class FrameRenderCall(RenderCall):
     so `stash` is implied and ignored.  want_z_alpha, and an engine that pick_engine does not resolve to the tensor-core engine
     (ENGINE_SIMT, or S < 16), are a ValueError, raised before any other check."""
     frame = True
+
+
+class ExactFrameRenderCall(FrameRenderCall):
+    """FrameRenderCall on the exact-fp32 engine (nnb_render_frame_train_fwd_engine / _bwd_engine on ENGINE_SIMT) at any S from 2 to
+    1024, whatever `engine` says.  Its forward gives the bits of RenderCall(engine=ENGINE_SIMT), jitter included; its workspace packs
+    min(S, 32) stash rows per ray, so it stays near 650 KB per ray at D = 256 for every S where the exact stash path keeps about 20 KB per
+    sample.  At S <= 32 the gradients are the exact stash path's bits.  want_z_alpha, or S outside 2..1024, is a ValueError."""
+    exact_frame = True
 
 
 def render_frame(weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None, depth_map=None, scale=None,
@@ -238,10 +257,11 @@ def _render_frame(fn, name, nbytes, engine, weights, c2w, cam, *, N, S, flags, n
 
 def render_frame_bwd(weights, c2w, cam, g_rgb, g_depth_pred, g_depth_gt, g_weights, g_c2w, g_cam=None, g_depth=None, g_scale_shift=None, *, N,
                      S, flags, near, far, ray_idx=None, pixels=None, depth=None, depth_map=None, scale=None, shift=None, H=0, W=0,
-                     hidden_dim=256):
-    """nnb_render_frame_bwd: the gradients of render_frame's outputs (t_min = 0, tensor-core engine) in a workspace whose only part that
-    grows with S is one float per ray and 32-sample chunk.  The g_* outputs follow RenderCall.backward (accumulated; g_depth overwritten;
-    g_weights may be None).  Returns (rgb, depth_pred, depth_gt, mask) of the call's own forward, the bits of render_frame."""
+                     hidden_dim=256, engine=L.ENGINE_TC):
+    """nnb_render_frame_bwd_engine: the gradients of render_frame_engine's outputs (t_min = 0) in a workspace whose only part that grows
+    with S is one float per ray and 32-sample chunk.  engine: ENGINE_TC (nnb_render_frame_bwd's bits, 16 <= S <= 1024) or ENGINE_SIMT (the
+    exact engine, 2 <= S <= 1024).  The g_* outputs follow RenderCall.backward (accumulated; g_depth overwritten; g_weights may be None).
+    Returns (rgb, depth_pred, depth_gt, mask) of the call's own forward, the bits of render_frame_engine on that engine."""
     for n_, t_ in (("weights", weights), ("c2w", c2w), ("camera_mat", cam), ("ray_idx", ray_idx), ("pixels", pixels), ("depth", depth),
                    ("depth_map", depth_map)):
         _need_cuda(t_, n_)
@@ -255,7 +275,7 @@ def render_frame_bwd(weights, c2w, cam, g_rgb, g_depth_pred, g_depth_gt, g_weigh
     if depth_map is not None:
         a.h_d, a.w_d = depth_map.shape[-2], depth_map.shape[-1]
     a.near_, a.far_ = float(near), float(far)
-    a.flags = flags; a.engine = L.ENGINE_TC; a.hidden_dim = int(hidden_dim)
+    a.flags = flags; a.engine = int(engine); a.hidden_dim = int(hidden_dim)
     rgb = torch.empty(N, 3, device=dev); depth_pred = torch.empty(N, device=dev)
     depth_gt = torch.empty(N, device=dev); mask = torch.empty(N, dtype=torch.uint8, device=dev)
     a.rgb = L.ptr(rgb); a.depth_pred = L.ptr(depth_pred); a.depth_gt = L.ptr(depth_gt); a.mask = L.ptr(mask)
@@ -263,11 +283,11 @@ def render_frame_bwd(weights, c2w, cam, g_rgb, g_depth_pred, g_depth_gt, g_weigh
     b.g_rgb, b.g_depth_pred, b.g_depth_gt = L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2])
     b.g_weights = L.ptr(g_weights); b.g_c2w = L.ptr(g_c2w); b.g_cam = L.ptr(g_cam); b.g_depth = L.ptr(g_depth)
     b.g_scale_shift = L.ptr(g_scale_shift)
-    nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, int(hidden_dim))
+    nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes_engine(N, S, int(hidden_dim), int(engine))
     ws = _pool.take(nbytes, dev) if nbytes else None
     a.workspace = L.ptr(ws); a.workspace_bytes = 0 if ws is None else ws.numel()
     try:
-        L.check(L.lib.nnb_render_frame_bwd(C.byref(b), _stream()), "nnb_render_frame_bwd")
+        L.check(L.lib.nnb_render_frame_bwd_engine(C.byref(b), _stream()), "nnb_render_frame_bwd_engine")
     finally:
         if ws is not None:
             _pool.give(ws)
@@ -275,8 +295,8 @@ def render_frame_bwd(weights, c2w, cam, g_rgb, g_depth_pred, g_depth_gt, g_weigh
 
 
 class _FrameGradFn(torch.autograd.Function):
-    """render_frame_grad's autograd glue: the forward is render_frame_engine on the tensor-core engine at t_min = 0 (RenderCall's bits
-    without a stash), the backward nnb_render_frame_bwd, which evaluates the field again chunk by chunk.  Differentiable inputs as in
+    """render_frame_grad's autograd glue: the forward is render_frame_engine on meta's engine at t_min = 0 (RenderCall's bits without a
+    stash), the backward render_frame_bwd on that engine, which evaluates the field again chunk by chunk.  Differentiable inputs as in
     _RenderFn."""
 
     @staticmethod
@@ -305,8 +325,7 @@ class _FrameGradFn(torch.autograd.Function):
         has_depth, has_scale, has_shift = ctx.has
         g_depth = torch.empty(N, device=dev) if has_depth else None
         g_ss = torch.zeros(2, device=dev) if (has_scale or has_shift) else None
-        render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c2w, g_cam, g_depth, g_ss,
-                         **{k: v for k, v in kw.items() if k not in ("engine",)})
+        render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c2w, g_cam, g_depth, g_ss, **kw)
         gp = [None] * ctx.nparams
         if g_w is not None:
             slices = ctx.param_slices
@@ -316,17 +335,25 @@ class _FrameGradFn(torch.autograd.Function):
         return (None, None, g_c2w, g_cam, g_depth, g_ss[0] if has_scale else None, g_ss[1] if has_shift else None) + tuple(gp)
 
 
-def render_frame_grad(meta, flat, c2w, cam, depth, scale, shift, params):
-    """render_autograd on the differentiable frame: (rgb, depth_pred, depth_gt, mask) of render_frame_engine (tensor-core engine,
-    t_min = 0; the bits of RenderCall), with gradients to the MLP parameters, c2w, cam, depth and scale / shift from
-    nnb_render_frame_bwd, whose memory does not grow with S but by one float per ray and 32-sample chunk.  meta as render_autograd's
-    without noise, want_z_alpha and stash (no jitter, no per-sample outputs); its engine must resolve to the tensor-core engine."""
+def render_frame_grad(meta, flat, c2w, cam, depth, scale, shift, params, frame_engine=None):
+    """render_autograd on the differentiable frame: (rgb, depth_pred, depth_gt, mask) of render_frame_engine (t_min = 0; the bits of
+    RenderCall), with gradients to the MLP parameters, c2w, cam, depth and scale / shift from nnb_render_frame_bwd_engine, whose memory
+    does not grow with S but by one float per ray and 32-sample chunk.  meta as render_autograd's without noise, want_z_alpha and stash
+    (no jitter, no per-sample outputs).  frame_engine None (or ENGINE_TC): the tensor-core engine, to which meta's engine must resolve;
+    ENGINE_SIMT: the exact-fp32 engine at any S from 2 to 1024, whatever meta's engine says."""
     meta = dict(meta)
     if meta.pop("noise", None) is not None or meta.pop("want_z_alpha", False) or meta.pop("stash", False):
         raise ValueError("render_frame_grad: noise, want_z_alpha and stash are not supported (no jitter, no per-sample outputs)")
-    if pick_engine(meta.get("engine"), meta["S"]) != L.ENGINE_TC:
-        raise ValueError("render_frame_grad runs on the tensor-core engine only (16 <= S <= 1024)")
-    meta["engine"] = L.ENGINE_TC   # render_frame_engine's forward and nnb_render_frame_bwd run this engine only
+    if frame_engine == L.ENGINE_SIMT:
+        if not 2 <= meta["S"] <= 1024:
+            raise ValueError("render_frame_grad on the exact engine needs 2 <= S <= 1024 (got %d)" % meta["S"])
+        meta["engine"] = L.ENGINE_SIMT
+    elif frame_engine is None or frame_engine == L.ENGINE_TC:
+        if pick_engine(meta.get("engine"), meta["S"]) != L.ENGINE_TC:
+            raise ValueError("render_frame_grad runs on the tensor-core engine only (16 <= S <= 1024)")
+        meta["engine"] = L.ENGINE_TC   # render_frame_engine's forward and nnb_render_frame_bwd run this engine only
+    else:
+        raise ValueError("render_frame_grad: frame_engine must be None, ENGINE_TC or ENGINE_SIMT (got %r)" % (frame_engine,))
     return _FrameGradFn.apply(meta, flat, c2w, cam, depth, scale, shift, *params)
 
 

@@ -2,7 +2,9 @@
 evaluating its chunk again with a chunk-sized stash) against nnb_render_fwd (NNB_STASH) + nnb_render_bwd, gradients to the MLP and the
 pose.  Shapes: the C2 training step (1024 rays x 128 samples) and N = 4096, S = 512, D = 256; each timed call is a whole forward +
 backward, alternated between the two paths over --rounds rounds, median reported.  Workspace bytes of both paths are printed beside
-them.  The card's name and power limit are read in the same run (nvidia-smi query, read-only).  Without a CUDA device the tool fails."""
+them.  --engine simt times the exact-fp32 engine's forms instead (nnb_render_frame_bwd_engine against nnb_render_fwd + nnb_render_bwd on
+NNB_ENGINE_SIMT) and adds one call of the frame backward alone at N = 4096, S = 1024, where the exact stash path cannot be sized.  The
+card's name and power limit are read in the same run (nvidia-smi query, read-only).  Without a CUDA device the tool fails."""
 import argparse, json, os, sys
 import numpy as np
 import torch
@@ -14,12 +16,14 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from field_query_cost import card  # noqa: E402
 
 SHAPES = ((1024, 128), (4096, 512))
+FRAME_ONLY = {"simt": ((4096, 1024),), "tc": ()}   # shapes timed on the frame path alone
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=7)
     ap.add_argument("--dim", type=int, default=256)
+    ap.add_argument("--engine", choices=("tc", "simt"), default="tc")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("frame_grad_cost: needs a CUDA device (there is no CPU path and a CPU timing would say nothing about the GPU)")
@@ -28,7 +32,11 @@ def main():
     name, limit = card()
     D = args.dim
     res = {"gpu": name, "power_limit": limit, "hidden_dim": D, "rounds": args.rounds, "shapes": []}
-    for N, S in SHAPES:
+    eng = L.ENGINE_SIMT if args.engine == "simt" else L.ENGINE_TC
+    if args.engine == "simt":
+        res["engine"] = "simt"
+    for N, S in SHAPES + FRAME_ONLY[args.engine]:
+        frame_only = (N, S) in FRAME_ONLY[args.engine]
         rng = np.random.default_rng(0)
         cu = lambda x: torch.from_numpy(np.ascontiguousarray(x)).cuda()
         flat = cu(O.flatten_params(O.init_params(seed=7, D=D, hf_damp=True)))
@@ -42,25 +50,34 @@ def main():
         g_w = torch.zeros(L.num_params(D), device="cuda"); g_c = torch.zeros(4, 4, device="cuda")
 
         def stash():
-            call = ops.RenderCall(flat, c2w, cam, stash=True, engine=L.ENGINE_TC, **kw)
+            call = ops.RenderCall(flat, c2w, cam, stash=True, engine=eng, **kw)
             call.backward(g_rgb, g_dp, g_dg, g_w, g_c)
 
         def frame():
-            ops.render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c, **kw)
+            ops.render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c, engine=eng, **kw)
 
-        times = {"stash": [], "frame": []}
-        for fn in (stash, frame):   # warm-up: module load, workspace allocation
+        paths = (("frame", frame),) if frame_only else (("stash", stash), ("frame", frame))
+        times = {k: [] for k, _ in paths}
+        for _, fn in paths:   # warm-up: module load, workspace allocation
             fn(); fn()
         torch.cuda.synchronize()
         for r in range(args.rounds):
-            for key, fn in (("stash", stash), ("frame", frame)) if r % 2 == 0 else (("frame", frame), ("stash", stash)):
+            for key, fn in paths if r % 2 == 0 else paths[::-1]:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record(); fn(); e1.record(); e1.synchronize()
                 times[key].append(e0.elapsed_time(e1))
         med = {k: float(np.median(v)) for k, v in times.items()}
+        stash_ws = int(L.lib.nnb_workspace_bytes_dim(N, S, L.STASH, eng, D))
+        frame_ws = int(L.lib.nnb_render_frame_bwd_workspace_bytes_engine(N, S, D, eng))
+        if frame_only:
+            row = {"N": N, "S": S, "frame_bwd_ms": med["frame"], "stash_ws_bytes": stash_ws, "frame_bwd_ws_bytes": frame_ws}
+            res["shapes"].append(row)
+            print("N=%d S=%d D=%d  frame_bwd %.2f ms  workspace %.2f GB (the stash path would need %.2f GB)"
+                  % (N, S, D, med["frame"], frame_ws / 1e9, stash_ws / 1e9), file=sys.stderr, flush=True)
+            ops._pool.free.clear(); torch.cuda.empty_cache()
+            continue
         row = {"N": N, "S": S, "stash_fwd_bwd_ms": med["stash"], "frame_bwd_ms": med["frame"], "ratio": med["frame"] / med["stash"],
-               "stash_ws_bytes": int(L.lib.nnb_workspace_bytes_dim(N, S, L.STASH, L.ENGINE_TC, D)),
-               "frame_bwd_ws_bytes": int(L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, D))}
+               "stash_ws_bytes": stash_ws, "frame_bwd_ws_bytes": frame_ws}
         res["shapes"].append(row)
         print("N=%d S=%d D=%d  render_fwd+bwd %.2f ms  frame_bwd %.2f ms (x%.2f)  workspace %.2f GB -> %.2f GB"
               % (N, S, D, med["stash"], med["frame"], row["ratio"], row["stash_ws_bytes"] / 1e9, row["frame_bwd_ws_bytes"] / 1e9),

@@ -5,6 +5,8 @@ Shapes: the C2 step (1024 rays x 128 samples, bench.py's render-only configurati
     step; the peak torch.cuda.max_memory_allocated over each Trainer's build and warm-up, above what was allocated before it.
   * The ops-level pair: FrameRenderCall + backward against render_frame_engine + nnb_render_frame_bwd (ops.render_frame_bwd), which
     evaluates the field once more, same inputs, alternated, median.
+--engine simt compares Trainer(frame_grad=True, frame_grad_engine='simt') (ExactFrameRenderCall) with the default step on the exact-fp32
+engine, at the C2 step and at S = 8, below the tensor-core range, and the ops-level pair on that engine.
 The card's name and power limit are read in the same run (nvidia-smi query, read-only).  Without a CUDA device the tool fails."""
 import argparse, gc, json, os, sys
 import numpy as np
@@ -16,10 +18,11 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from field_query_cost import card  # noqa: E402
 
-SHAPES = ((1024, 128), (4096, 512))
+SHAPES = {"tc": ((1024, 128), (4096, 512)), "simt": ((1024, 128), (1024, 8))}
+FRAME_KW = {"tc": dict(frame_grad=True), "simt": dict(frame_grad=True, frame_grad_engine="simt")}
 
 
-def build(N, S, frame_grad, dev):
+def build(N, S, frame_grad, dev, engine="tc"):
     import bench
     import nope_nerf_b200.model as mdl
     cfg = bench.make_cfg(N)
@@ -32,7 +35,8 @@ def build(N, S, frame_grad, dev):
         pose.r.normal_(0, 0.05); pose.t.normal_(0, 0.05)
     return mdl.Trainer(model, torch.optim.Adam(model.parameters(), lr=1e-3), cfg["training"], device=dev,
                        optimizer_pose=torch.optim.Adam(pose.parameters(), lr=5e-4), pose_param_net=pose,
-                       optimizer_distortion=torch.optim.Adam(dnet.parameters(), lr=5e-4), distortion_net=dnet, frame_grad=frame_grad)
+                       optimizer_distortion=torch.optim.Adam(dnet.parameters(), lr=5e-4), distortion_net=dnet,
+                       **(FRAME_KW[engine] if frame_grad else {}))
 
 
 def timed(fn, n):
@@ -44,12 +48,12 @@ def timed(fn, n):
     return e0.elapsed_time(e1) / n
 
 
-def trainer_steps(N, S, frames, rounds, steps, dev):
+def trainer_steps(N, S, frames, rounds, steps, dev, engine="tc"):
     trainers, peak = {}, {}
     for key, fg in (("stash", False), ("frame", True)):
         torch.cuda.synchronize()
         base = torch.cuda.memory_allocated(); torch.cuda.reset_peak_memory_stats()
-        tr = build(N, S, fg, dev)
+        tr = build(N, S, fg, dev, engine)
         for i in range(3):                                   # eager warm-up, capture, first replay
             tr.train_step(frames[i % len(frames)], it=i, epoch=0, scheduling_start=10000, render_path=None)
         torch.cuda.synchronize()
@@ -67,7 +71,7 @@ def trainer_steps(N, S, frames, rounds, steps, dev):
     return {k: float(np.median(v)) for k, v in times.items()}, peak
 
 
-def ops_pair(N, S, D, rounds):
+def ops_pair(N, S, D, rounds, engine="tc"):
     from nope_nerf_b200 import ops, _lib as L
     from oracle import nerf_oracle as O
     rng = np.random.default_rng(0)
@@ -82,13 +86,16 @@ def ops_pair(N, S, D, rounds):
     g_rgb, g_dp, g_dg = cu(rng.normal(0, 1, (N, 3)).astype(np.float32)), torch.zeros(N, device="cuda"), torch.zeros(N, device="cuda")
     g_w = torch.zeros(L.num_params(D), device="cuda"); g_c = torch.zeros(4, 4, device="cuda")
 
+    exact = engine == "simt"
+    eng = L.ENGINE_SIMT if exact else L.ENGINE_TC
+
     def pair(_):
-        call = ops.FrameRenderCall(flat, c2w, cam, engine=None, **kw)
+        call = (ops.ExactFrameRenderCall if exact else ops.FrameRenderCall)(flat, c2w, cam, engine=None, **kw)
         call.backward(g_rgb, g_dp, g_dg, g_w, g_c)
 
     def one_call(_):
-        ops.render_frame_engine(flat, c2w, cam, engine=L.ENGINE_TC, **kw)
-        ops.render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c, **kw)
+        ops.render_frame_engine(flat, c2w, cam, engine=eng, **kw)
+        ops.render_frame_bwd(flat, c2w, cam, g_rgb, g_dp, g_dg, g_w, g_c, engine=eng, **kw)
 
     for fn in (pair, one_call):
         fn(0); fn(0)
@@ -105,20 +112,23 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=7)
     ap.add_argument("--steps", type=int, default=20, help="graph steps per timed round")
+    ap.add_argument("--engine", choices=("tc", "simt"), default="tc")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("train_frame_cost: needs a CUDA device (there is no CPU path and a CPU timing would say nothing about the GPU)")
     import bench
     from nope_nerf_b200 import ops, _lib as L
-    ops.set_default_engine("tc")
+    ops.set_default_engine(args.engine)   # the engine of the default step
     dev = torch.device("cuda", 0); torch.cuda.set_device(0)
     name, limit = card()
     D = 256
     _, frames = bench.synth_frames(bench.H, bench.W, bench.HD, bench.WD, 4, bench.V, dev, with_ref=False)
     res = {"gpu": name, "power_limit": limit, "hidden_dim": D, "rounds": args.rounds, "steps": args.steps, "shapes": []}
-    for N, S in SHAPES:
-        step, peak = trainer_steps(N, S, frames, args.rounds, args.steps, dev)
-        pair = ops_pair(N, S, D, args.rounds)
+    if args.engine == "simt":
+        res["engine"] = "simt"
+    for N, S in SHAPES[args.engine]:
+        step, peak = trainer_steps(N, S, frames, args.rounds, args.steps, dev, args.engine)
+        pair = ops_pair(N, S, D, args.rounds, args.engine)
         row = {"N": N, "S": S, "step_stash_ms": step["stash"], "step_frame_ms": step["frame"], "step_ratio": step["frame"] / step["stash"],
                "peak_stash_bytes": int(peak["stash"]), "peak_frame_bytes": int(peak["frame"]),
                "ops_pair_ms": pair["pair"], "ops_fwd_plus_frame_bwd_ms": pair["fwd_plus_frame_bwd"],
