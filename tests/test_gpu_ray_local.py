@@ -253,6 +253,8 @@ def transmittance(A, alpha, bug=None):
         carry = r(carry * incl[:, c, 31])
     if bug == "carry":
         carries = [carries[max(c - 1, 0)] for c in range(len(carries))]
+    elif bug == "carry_one":
+        carries = [torch.ones_like(carry)] * len(carries)
     T = torch.stack([r(carries[c][:, None] * excl[:, c]) for c in range(a.shape[1])], 1)
     return om, T
 
@@ -292,8 +294,9 @@ def composite_fwd_ref(A, rec, ray, flags, bug=None):
     return alpha, torch.stack(C, 1), Dist, g
 
 
-def composite_bwd_ref(A, rec, ray, seeds, flags, bug=None):
-    """composite_bwd: gs [N, S, 4]"""
+def composite_bwd_ref(A, rec, ray, seeds, flags, bug=None, want_suffix=False):
+    """composite_bwd: gs [N, S, 4] (and with want_suffix the suffix carry after the first chunk, sum of w gw over the ray); bugs of the
+    frame's reverse rounds: suffix_reset (the carry zeroed at every chunk), drop_late (chunks after the first dropped)"""
     r = A.r
     N, S = rec["a"].shape
     gC, gD = seeds["g_rgb"], seeds["g_dp"]
@@ -318,17 +321,23 @@ def composite_bwd_ref(A, rec, ray, seeds, flags, bug=None):
     if bug == "total_minus_prefix":   # fp32 total minus the inclusive prefix (the emulation's dtype carries the rounding)
         flat = wg.reshape(N, -1)
         suffix = (flat.sum(1, keepdim=True) - torch.cumsum(flat, 1)).view(wg.shape)
+        carry_s = flat.sum(1)
     else:
         incl = incl_sum_rev(A, wg)
         excl = torch.cat([incl[..., 1:], torch.zeros_like(incl[..., :1])], -1)
         carry_s, suf = torch.zeros_like(gD), [None] * wg.shape[1]
         for c in range(wg.shape[1] - 1, -1, -1):
+            if bug in ("suffix_reset", "drop_late"):
+                carry_s = torch.zeros_like(gD)
             suf[c] = r(excl[:, c] + carry_s[:, None])
             carry_s = r(carry_s + incl[:, c, 0])
         suffix = torch.stack(suf, 1)
     g_alpha = r(r(T * gw) - r(suffix / om))
     gs = torch.stack([r(w * e(gC[:, k])) for k in range(3)] + [r(g_alpha * df)], -1)
-    return gs.reshape(N, -1, 4)[:, :S]
+    if bug == "drop_late":
+        gs = torch.cat([gs[:, :1], torch.zeros_like(gs[:, 1:])], 1)
+    gs = gs.reshape(N, -1, 4)[:, :S]
+    return (gs, carry_s) if want_suffix else gs
 
 
 def encode_bwd_ref(A, x, ge, levels, bug=None):
@@ -346,10 +355,15 @@ def encode_bwd_ref(A, x, ge, levels, bug=None):
 
 def ray_bwd_ref(A, ray, gp, gv, z, depth_pred, seeds, flags, explicit_depth, bug=None):
     """ray_bwd: rows [N]; gp / gv [N, S, 3], z [N, S] -> (rayred [N, 16], g_depth [N])"""
-    r = A.r
     so = [lane_sum(A, gp[..., c]) for c in range(3)]
-    sd = [lane_sum(A, r(z * gp[..., c])) for c in range(3)]
+    sd = [lane_sum(A, A.r(z * gp[..., c])) for c in range(3)]
     sv = [lane_sum(A, gv[..., c]) for c in range(3)]
+    return ray_adjoint_ref(A, ray, so, sd, sv, depth_pred, seeds, flags, explicit_depth, bug)
+
+
+def ray_adjoint_ref(A, ray, so, sd, sv, depth_pred, seeds, flags, explicit_depth, bug=None):
+    """ray_bwd's lane-0 block from its ray sums so = sum gp, sd = sum z gp, sv = sum gv (3 lists of [N]) -> (rayred [N, 16], g_depth)"""
+    r = A.r
     norm = bool(flags & L.NORMALISE)
     ev = bool(flags & L.EVAL) and norm
     nrm, d, dt, dc, R = ray["nrm"], ray["d"], ray["dt"], ray["dc"], ray["R"]
