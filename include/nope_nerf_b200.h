@@ -464,6 +464,31 @@ int nnb_render_frame_bwd(const nnb_render_bwd_args* b, void* stream);
 int nnb_render_frame_train_fwd(const nnb_render_args* a, void* stream);
 int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream);
 
+/* The training pair with early ray termination, on the tensor-core engine.  No version bump: the symbols mark the capability.
+ * nnb_render_frame_train_fwd_tmin(f): f->fwd as nnb_render_frame_train_fwd's argument (noise accepted), plus f->t_min and the optional
+ *   f->n_eval / f->t_final of nnb_render_frame.  Ray n evaluates chunks 0 .. c_n - 1 under nnb_render_frame's stop rule (it stops after
+ *   the first chunk that leaves its transmittance below t_min, or after the last chunk).  Without noise, rgb, depth_pred, depth_gt, mask,
+ *   n_eval and t_final are bit-identical to nnb_render_frame at the same t_min; with noise, a ray with n_eval == S has the bits of
+ *   nnb_render_frame_train_fwd, and a stopped ray keeps nnb_render_frame's bound on the weight it dropped (below 1.002 t_final).  At
+ *   t_min = 0 every output is nnb_render_frame_train_fwd's.  Leaves the weight image, the checkpoints and the chunk counts c_n in the
+ *   workspace.
+ * nnb_render_frame_train_bwd_tmin(b): after that call, with nnb_render_frame_train_bwd's rules for b and the workspace.  The gradients are
+ *   the exact gradients of the truncated outputs with every c_n held constant (the stop decision is piecewise constant): reverse round k
+ *   visits only the rays with c_n > k, and a ray's suffix carry into composite_chunk_bwd is 0 at its own last chunk.  Before round k the
+ *   list {n : c_n > k} is built in increasing n by a block scan into the forward's first ray list and round counter (free once the
+ *   forward has ended), and the data-gradient and weight-gradient kernels take their row count, 32 per listed ray, from the device.  So
+ *   both calls can be captured in a CUDA graph and replayed when the stop pattern changes.  At t_min = 0 every list is 0 .. N - 1, and
+ *   the outputs and gradients are nnb_render_frame_train_bwd's bit for bit, after either forward.
+ *   Every c_n read is clamped to 1..C (C = ceil(S / 32)) and every device count to 0..N: a backward without its forward gives wrong
+ *   numbers, never an access outside the workspace.  Every sum runs in a fixed order, so the same inputs give the same bits whatever the
+ *   workspace held.  Neither call synchronises, reads back or allocates.
+ * Workspace: nnb_render_frame_bwd_workspace_bytes(N, S, hidden_dim), in its layout; nothing is added.
+ * Errors, with nothing launched: NULL args (rc -1); an engine other than NNB_ENGINE_TC (-4, also when nnb_render_frame_bwd_engine would
+ *   take it); then nnb_render_frame_train_fwd / _bwd's checks and codes in their order, with, on the forward, a negative or NaN t_min (-2)
+ *   after the flag and size checks and misaligned n_eval / t_final (-3) after the output pointers, as in nnb_render_frame. */
+int nnb_render_frame_train_fwd_tmin(const nnb_frame_args* f, void* stream);
+int nnb_render_frame_train_bwd_tmin(const nnb_render_bwd_args* b, void* stream);
+
 /* nnb_render_frame_bwd, nnb_render_frame_train_fwd and nnb_render_frame_train_bwd on fwd.engine.  NNB_ENGINE_TC is exactly the call
  * without the suffix (its checks, codes, bits and workspace).  NNB_ENGINE_SIMT runs the same method on the exact-fp32 engine at any S from
  * 2 to 1024, with a chunk stash that packs R = min(S, 32) rows per ray (row R n + j is sample 32 k + j of ray n), so a round at S < 32

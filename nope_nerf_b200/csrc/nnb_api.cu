@@ -45,6 +45,8 @@ size_t tc_render_frame_bwd_workspace(int N, int S, int D);
 cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t tc_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStream_t st);
 cudaError_t tc_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
+cudaError_t tc_render_frame_train_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st);
+cudaError_t tc_render_frame_train_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
@@ -608,6 +610,42 @@ int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream) {
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_bwd");
 #else
   return fail(-4, "library built without the tensor-core engine");
+#endif
+}
+int nnb_render_frame_train_fwd_tmin(const nnb_frame_args* f, void* stream) {
+  if (!f) return fail(-1, "null args");
+  const nnb_render_args* a = &f->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_frame_train_fwd_tmin: engine %d has no differentiable frame with early termination (NNB_ENGINE_TC only)",
+                a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_frame(a, true)) return rc;
+  if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_frame_train_fwd_tmin: t_min must be >= 0 (got %g)", (double)f->t_min);
+  if (int rc = check_frame_io(a)) return rc;
+  if (misaligned4(f->n_eval) || misaligned4(f->t_final))
+    return fail(-3, "nnb_render_frame_train_fwd_tmin: n_eval and t_final must be 4-byte aligned");
+  if (int rc = check_frame_train_ws(a)) return rc;
+  const cudaError_t e = tc_render_frame_train_fwd_tmin(*f, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_fwd_tmin");
+#endif
+}
+int nnb_render_frame_train_bwd_tmin(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_frame_train_bwd_tmin: engine %d has no differentiable frame with early termination (NNB_ENGINE_TC only)",
+                a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_frame(a, true)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_frame_train_bwd_tmin: g_rgb and g_c2w must be non-null");
+  if (int rc = check_frame_train_ws(a)) return rc;
+  const cudaError_t e = tc_render_frame_train_bwd_tmin(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_bwd_tmin");
 #endif
 }
 size_t nnb_render_frame_bwd_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine) {

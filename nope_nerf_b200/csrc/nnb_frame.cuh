@@ -179,6 +179,96 @@ __global__ void frame_ray_acc(nnb_render_args a, const __grid_constant__ FrameBw
   for (int c = 0; c < 9; ++c) part[32 * c] = v[c];
 }
 
+// Early ray termination in the reverse rounds (nnb_render_frame_train_bwd_tmin): ray n evaluated chunks 0 .. c_n - 1 in the forward
+// (c_n = FramePtrs::chunks[n], clamped to 1..C), so reverse round k visits only the rays with c_n > k.  frame_live_list writes them to
+// `list` in increasing n, with their count in *count; the round's stash row 32 slot + j is sample 32 k + j of ray list[slot], and the
+// per-ray kernels run one warp per slot.  A ray starts its suffix carry and lane partials in its own last round, k = c_n - 1.
+struct FrameLive { const int* chunks; const int* list; const int* count; };
+__device__ __forceinline__ int frame_ray_chunks(const int* chunks, int n, int C) { return min(max(chunks[n], 1), C); }
+__device__ __forceinline__ int frame_live_count(const int* count, int N) { return min(max(*count, 0), N); }
+
+// one CTA of 1024 threads: list = {n : c_n > k} in increasing n, *count = its size.  1024 rays at a time, each placed by a block scan of
+// the live flags (no atomics: the order of the list is the order of the weight-gradient sums, so it must not depend on scheduling).
+__global__ void __launch_bounds__(1024) frame_live_list(const int* __restrict__ chunks, int N, int k, int C, int* __restrict__ list,
+                                                        int* __restrict__ count) {
+  __shared__ int s_warp[32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  int base = 0;
+  for (int n0 = 0; n0 < N; n0 += 1024) {
+    const int n = n0 + t;
+    const int live = n < N && frame_ray_chunks(chunks, n, C) > k ? 1 : 0;
+    int x = live;   // inclusive scan over the warp, then over the warps' totals
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      int v = s_warp[lane];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += y; }
+      s_warp[lane] = v;
+    }
+    __syncthreads();
+    const int before = base + (warp > 0 ? s_warp[warp - 1] : 0) + x - live;
+    if (live) list[before] = n;
+    base += s_warp[31];
+    __syncthreads();   // s_warp is rewritten by the next 1024 rays
+  }
+  if (t == 0) *count = base;
+}
+
+// frame_chunk_adjoint<false> on round k's live list: one warp per slot, ray n = list[slot], rows 32 slot .. 32 slot + 31; the ray's suffix
+// starts at 0 in its own last round, k = c_n - 1.  A copy of that kernel's body: shared, nvcc 12.9 changed the existing kernels' SASS.
+__global__ void frame_chunk_adjoint_live(nnb_render_bwd_args b, const __grid_constant__ FrameBwdPtrs f, const __grid_constant__ FrameLive l) {
+  const nnb_render_args& a = b.fwd;
+  const int lane = threadIdx.x & 31, slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (slot >= frame_live_count(l.count, a.N)) return;
+  const int n = l.list[slot];
+  Ray ray; setup_ray(a, n, ray);
+  float gD = b.g_depth_pred ? __ldg(b.g_depth_pred + n) : 0.f;
+  if ((a.flags & NNB_EVAL) && (a.flags & NNB_NORMALISE)) gD = gD / ray.nrm;
+  const float gC0 = __ldg(b.g_rgb + 3 * n), gC1 = __ldg(b.g_rgb + 3 * n + 1), gC2 = __ldg(b.g_rgb + 3 * n + 2);
+  const float gsum = (a.flags & NNB_WHITE_BG) ? (gC0 + gC1 + gC2) : 0.f;
+  const int i = 32 * f.k + lane;
+  const bool valid = i < a.S;
+  const size_t m = (size_t)slot * 32 + lane;
+  const SampleRec me = valid ? f.rec[m] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
+  float alpha = 0.f, df = 1.f;   // df = d alpha / d a
+  if (valid) {
+    alpha = composite_alpha(a, i, me.a, me.z, [&] { return sample_z(a, n, i + 1); });
+    if (a.flags & NNB_DIST_ALPHA) {
+      if (i >= a.S - 1) df = 0.f;
+      else { const float delta = __fsub_rn(sample_z(a, n, i + 1), me.z); df = delta * expf(-me.a * delta); }
+    }
+  }
+  const float carry = f.k > 0 ? f.ckpt[(size_t)(f.k - 1) * a.N + n] : 1.f;
+  float carry_s = f.k == frame_ray_chunks(l.chunks, n, f.rounds) - 1 ? 0.f : f.suffix[n];
+  f.gs[m] = composite_chunk_bwd<false>(alpha, valid, me.r, me.g, me.b, me.z, df, lane, carry, gC0, gC1, gC2, gD, gsum, carry_s);
+  if (lane == 0) f.suffix[n] = carry_s;
+}
+
+// frame_ray_acc<false> on round k's live list (a copy, as above): the ray's lane partials are written by its own last round, k = c_n - 1
+__global__ void frame_ray_acc_live(nnb_render_args a, const __grid_constant__ FrameBwdPtrs f, const __grid_constant__ FrameLive l) {
+  const int lane = threadIdx.x & 31, slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (slot >= frame_live_count(l.count, a.N)) return;
+  const int n = l.list[slot];
+  const bool first = f.k == frame_ray_chunks(l.chunks, n, f.rounds) - 1;
+  float* part = f.raypart + (size_t)n * 288 + lane;
+  float v[9];
+#pragma unroll
+  for (int c = 0; c < 9; ++c) v[c] = first ? 0.f : part[32 * c];
+  if (32 * f.k + lane < a.S) {
+    const size_t m = (size_t)slot * 32 + lane;
+    const float4 g = f.gp[m], dv = f.gv[m];
+    const float z = f.rec[m].z;
+    v[0] += g.x; v[1] += g.y; v[2] += g.z;
+    v[3] += z * g.x; v[4] += z * g.y; v[5] += z * g.z;
+    v[6] += dv.x; v[7] += dv.y; v[8] += dv.z;
+  }
+#pragma unroll
+  for (int c = 0; c < 9; ++c) part[32 * c] = v[c];
+}
+
 // one warp per ray after the last round: ray_bwd's warp sums of the lane partials and its per-ray adjoint -> rayred [N][16] (ray_reduce
 // follows)
 __global__ void frame_ray_finish(nnb_render_bwd_args b, const float* __restrict__ raypart, float* __restrict__ rayred) {

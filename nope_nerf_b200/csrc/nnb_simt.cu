@@ -851,7 +851,7 @@ __device__ __forceinline__ void head_wgrad_split(const HJob& J, size_t mb, size_
 }
 
 // grid (msplit, jobs): split blockIdx.x of job blockIdx.y; chained launch as simt_wgrad
-__global__ void __launch_bounds__(256) head_wgrad(const __grid_constant__ HJobs jobs, size_t M, int msplit, float* part) {
+__device__ __forceinline__ void head_wgrad_body(const HJobs& jobs, size_t M, int msplit, float* part) {
   extern __shared__ __align__(128) unsigned char hsmem[];
   const HJob& J = jobs.j[blockIdx.y];
   size_t chunk = (M + msplit - 1) / msplit; chunk = (chunk + 15) / 16 * 16;
@@ -865,6 +865,16 @@ __global__ void __launch_bounds__(256) head_wgrad(const __grid_constant__ HJobs 
     default: head_wgrad_split<16>(J, mb, me, pp, hsmem); break;
   }
   if (blockIdx.x == gridDim.x - 1 && blockIdx.y == gridDim.y - 1) pdl_wait();   // chained launch: see tc_wgrad_all
+}
+__global__ void __launch_bounds__(256) head_wgrad(const __grid_constant__ HJobs jobs, size_t M, int msplit, float* part) {
+  head_wgrad_body(jobs, M, msplit, part);
+}
+// head_wgrad on the first min(32 *mcount, M) rows (the live rays of a reverse round of nnb_render_frame_train_bwd_tmin), read on the
+// device, at the launch's split count: the splits past those rows store zeros, and at *mcount = M / 32 the splits are head_wgrad's
+__global__ void __launch_bounds__(256) head_wgrad_live(const __grid_constant__ HJobs jobs, size_t M, int msplit, float* part,
+                                                       const int* __restrict__ mcount) {
+  const size_t m = (size_t)max(*mcount, 0) * 32;
+  head_wgrad_body(jobs, m < M ? m : M, msplit, part);
 }
 
 // dW[n][k] += sum over splits (fixed order); one thread per element of all jobs
@@ -1404,11 +1414,13 @@ cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, c
 }
 
 // the head jobs of tc_wgrad_all -> head_wgrad at jobs_wgrad_msplit(M) splits, launched chained into part[off ..] (njobs <= 4); the
-// caller reduces them through R
-cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st) {
+// caller reduces them through R.  mcount (not NULL): head_wgrad_live on min(32 *mcount, M) rows
+cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st,
+                              const int* mcount) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(head_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, HW_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(head_wgrad_live, cudaFuncAttributeMaxDynamicSharedMemorySize, HW_SMEM);
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -1438,7 +1450,8 @@ cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, 
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(msplit, njobs); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = HW_SMEM; cfg.stream = st;
   cfg.attrs = &at; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, head_wgrad, J, M, msplit, part);
+  cudaError_t e = mcount ? cudaLaunchKernelEx(&cfg, head_wgrad_live, J, M, msplit, part, mcount)
+                         : cudaLaunchKernelEx(&cfg, head_wgrad, J, M, msplit, part);
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 

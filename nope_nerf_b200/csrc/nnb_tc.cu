@@ -43,7 +43,8 @@
 cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs, cudaStream_t st);
 cudaError_t simt_render_bwd_with(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st, DgradFn dgrad, WgradFn wgrad);
 cudaError_t launch_ray_reduce(const nnb_render_bwd_args& b, const float* rayred, cudaStream_t st);
-cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st);
+cudaError_t launch_head_wgrad(const SmallJob* jobs, int njobs, size_t M, int D, float* part, size_t off, RedJob* R, cudaStream_t st,
+                              const int* mcount = nullptr);
 
 void nnb_prof_mark(cudaStream_t st);
 
@@ -222,12 +223,19 @@ __device__ __forceinline__ size_t frame_sample(const nnb_render_args& a, const F
 __device__ __forceinline__ int2 chunk_sample(const nnb_render_args& a, int k, size_t m) {
   return make_int2(min((int)(m >> 5), a.N - 1), min(32 * k + (int)(m & 31), a.S - 1));
 }
-// row_geometry_tc of that sample
-__device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, size_t m, Ray& ray, float& z, float p[3]) {
-  const int2 ni = chunk_sample(a, k, m);
+// nnb_render_frame_train_bwd_tmin (the live-list forms, DEVN): row m of round k's stash is sample 32 k + m % 32 of ray list[m / 32], over
+// the n_live rays of the list (rows past the last slot take its ray, rows past the ray's last sample that sample; their cotangent is zero)
+__device__ __forceinline__ int2 live_sample(const nnb_render_args& a, int k, const int* list, int n_live, size_t m) {
+  return make_int2(list[min((int)(m >> 5), n_live - 1)], min(32 * k + (int)(m & 31), a.S - 1));
+}
+// row_geometry_tc of a sample (ray, index)
+__device__ __forceinline__ void sample_geometry(const nnb_render_args& a, int2 ni, Ray& ray, float& z, float p[3]) {
   setup_ray(a, ni.x, ray);
   z = sample_z(a, ni.x, ni.y);
   sample_point(a, ray, z, p);
+}
+__device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, size_t m, Ray& ray, float& z, float p[3]) {
+  sample_geometry(a, chunk_sample(a, k, m), ray, z, p);
 }
 
 // MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
@@ -247,7 +255,9 @@ __device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, 
 // 4) and frame_step composites them.  n_tiles is read from *fr.count (ray-chunks, 4 per tile) when the kernel starts, as in FWD_MARCH.
 // FWD_CHUNK (tc_frame_stash, nnb_render_frame_bwd): FWD_RAYS with the training stash on the rows of chunk fr.k of every ray (M = 32 N,
 // row m is sample chunk_sample(a, fr.k, m) of its ray), with ray-chunks of 32 rows in place of whole rays in the per-ray bias as in FWD_FRAME; records,
-// stash and gate bits are indexed by the row.
+// stash and gate bits are indexed by the row.  With DEVN (tc_frame_stash_live): the rows of the rays of round fr.k's live list fr.list
+// (live_sample), M = 32 n_live and n_tiles = ceil(n_live / 4) with n_live = *fr.count clamped to 0..N, read when the kernel starts; the
+// launch is sized for N and a CTA without a tile leaves at once.
 // FWD_GRAD (tc_points_grad_fwd, nnb_field_grad): FWD_VJP that also writes the fp32 training stash st of every row of every tile (rows
 // past M hold the last point's values): h0..h7, feat, hr and enc as FWD_RAYS does, and denc per point (the direction encoding of
 // a.dirs[m], or of the ones), which is a per-row operand of rgb_layers.0 here.  With NNB_OCC_ONLY the colour part (feat, hr, denc) is not
@@ -268,17 +278,22 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
   constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD, TAN = MODE == FWD_TANGENT, CHUNK = MODE == FWD_CHUNK;
   constexpr bool PTS = MODE != FWD_RAYS && !FRAME && !CHUNK, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP || GRAD;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
-  static_assert(!DEVN || XPTS, "a device count of explicit points");
+  static_assert(!DEVN || XPTS || CHUNK, "a device count of explicit points or of a frame round's rays");
   if constexpr ((PTS && !GRAD && !TAN) || FRAME) stash = 0;
   if constexpr (GRAD || TAN || CHUNK) stash = 1;
-  int n_live = 0;   // FWD_FRAME: ray-chunks of this round
+  int n_live = 0;   // FWD_FRAME, FWD_CHUNK with DEVN: ray-chunks of this round
   if constexpr (FRAME) {
     n_live = fr.count ? *fr.count : a.N;
     n_tiles = (n_live + 3) / 4;
     if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
   }
+  if constexpr (CHUNK && DEVN) {
+    n_live = frame_live_count(fr.count, a.N);
+    n_tiles = (n_live + 3) / 4;
+    if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
+  }
   const bool gates = !TAN && (VJP || stash);   // the ReLU gate bits are stored
-  if constexpr (MARCH || DEVN) {
+  if constexpr (MARCH || (DEVN && !CHUNK)) {
     if (q.count) {
       const int c = *q.count;
       M = (size_t)c;
@@ -389,7 +404,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
 #pragma unroll
         for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + (size_t)mm * 3 + c);
       } else {
-        if constexpr (CHUNK) chunk_geometry(a, fr.k, m, ray, z, p);
+        if constexpr (CHUNK && DEVN) sample_geometry(a, live_sample(a, fr.k, fr.list, n_live, m), ray, z, p);
+        else if constexpr (CHUNK) chunk_geometry(a, fr.k, m, ray, z, p);
         else row_geometry_tc(a, m, M, ray, z, p);
       }
       float ee[64];
@@ -611,7 +627,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             } else if constexpr (FRAME) {   // E row r0 + 8 r, k-octet 0: this warpgroup's rows of E
               *reinterpret_cast<float4*>(smem + SM_EHI + (r0 + 8 * r) * 16) = make_float4(rec.r, rec.g, rec.b, rec.a);
             } else if constexpr (CHUNK) {
-              const int2 ni = chunk_sample(a, fr.k, m);
+              const int2 ni = DEVN ? live_sample(a, fr.k, fr.list, n_live, m) : chunk_sample(a, fr.k, m);
               rec.z = sample_z(a, ni.x, ni.y);
               rec.pad0 = 0.f; rec.pad1 = 0.f;
               recs[m] = rec;
@@ -720,6 +736,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_frame_stash(nnb_render_args a
                                                                const __grid_constant__ FramePtrs f, int n_tiles) {
   tc_fwd_body<D, FWD_CHUNK>(a, wimg, recs, nullptr, st, MarchPtrs{}, (size_t)a.N * 32, n_tiles, 1, f);
 }
+// tc_frame_stash on the rays of round f.k's live list f.list (*f.count of them; the launch is sized for N)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_frame_stash_live(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                    SampleRec* __restrict__ recs, const __grid_constant__ TcStash st,
+                                                                    const __grid_constant__ FramePtrs f) {
+  tc_fwd_body<D, FWD_CHUNK, true>(a, wimg, recs, nullptr, st, MarchPtrs{}, (size_t)a.N * 32, 0, 1, f);
+}
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
 // CTA = one 128-row slice of dW (all KN columns) over a contiguous share of the samples, warp-specialized in 32-sample chunks:
@@ -758,9 +781,13 @@ __device__ __forceinline__ void tma_g2s_2d(uint32_t dst, const CUtensorMap* map,
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar) : "memory");
 }
 
-// KN = 256 | 128 | 64: columns of dW (features of X) held by one CTA.  XMAP: X column block k0 .. k0 + KN - 1 through xmap (box KN x CH)
-template <int KN, bool XMAP>
-__device__ __forceinline__ void wgrad_body(const WgJobsT& J, const CUtensorMap* xmap, size_t M, float* __restrict__ part) {
+// KN = 256 | 128 | 64: columns of dW (features of X) held by one CTA.  XMAP: X column block k0 .. k0 + KN - 1 through xmap (box KN x CH).
+// DEVM (tc_wgrad_live, tc_wgrad_piece_live: a reverse round of nnb_render_frame_train_bwd_tmin): M = min(32 *mcount, M), the rows of the
+// round's live rays, read when the kernel starts, and per_cta formed from it as launch_wgrad forms it, with the launch's split count: at
+// *mcount = N the splits are those of tc_wgrad on 32 N rows; splits past M store zeros.
+template <int KN, bool XMAP, bool DEVM = false>
+__device__ __forceinline__ void wgrad_body(const WgJobsT& J, const CUtensorMap* xmap, size_t M, float* __restrict__ part,
+                                           const int* mcount = nullptr) {
   using W = Wg<KN>;
   constexpr int CH = W::CH, NSTG = W::NSTG, NOP = W::NOP, A_BYTES = W::A_BYTES, B_BYTES = W::B_BYTES;
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -768,8 +795,16 @@ __device__ __forceinline__ void wgrad_body(const WgJobsT& J, const CUtensorMap* 
   while (ji + 1 < J.njobs && (int)blockIdx.x >= J.j[ji + 1].cta0) ++ji;
   const WgJobT& jb = J.j[ji];
   const int local = blockIdx.x - jb.cta0, n0 = (local / J.msplit) * 128;
-  const size_t s_begin = (size_t)(local % J.msplit) * J.per_cta;
-  const size_t s_end = (s_begin + J.per_cta < M) ? s_begin + J.per_cta : M;   // an empty split stores zeros
+  size_t s_begin, s_end;
+  if constexpr (DEVM) {
+    const size_t m = (size_t)max(*mcount, 0) * 32, Md = m < M ? m : M;
+    const size_t per_cta = ((Md + J.msplit - 1) / J.msplit + WG_BLOCK - 1) / WG_BLOCK * WG_BLOCK;
+    s_begin = (size_t)(local % J.msplit) * per_cta;
+    s_end = (s_begin + per_cta < Md) ? s_begin + per_cta : Md;   // an empty split stores zeros
+  } else {
+    s_begin = (size_t)(local % J.msplit) * J.per_cta;
+    s_end = (s_begin + J.per_cta < M) ? s_begin + J.per_cta : M;   // an empty split stores zeros
+  }
   const int nch = s_begin < s_end ? (int)((s_end - s_begin + WG_BLOCK - 1) / WG_BLOCK) * (WG_BLOCK / CH) : 0;
   float* pp = part + jb.part_off + (size_t)(local % J.msplit) * ((size_t)jb.Nn * jb.Kk + 2 * jb.Nn);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -902,6 +937,17 @@ __global__ void __launch_bounds__(384, 1) tc_wgrad_piece(const __grid_constant__
                                                          size_t M, float* __restrict__ part) {
   wgrad_body<KN, true>(J, &xmap, M, part);
 }
+// the same two kernels with the row count read on the device (wgrad_body's DEVM)
+template <int KN>
+__global__ void __launch_bounds__(384, 1) tc_wgrad_live(const __grid_constant__ WgJobsT J, size_t M, float* __restrict__ part,
+                                                        const int* __restrict__ mcount) {
+  wgrad_body<KN, false, true>(J, nullptr, M, part, mcount);
+}
+template <int KN>
+__global__ void __launch_bounds__(384, 1) tc_wgrad_piece_live(const __grid_constant__ WgJobsT J, const __grid_constant__ CUtensorMap xmap,
+                                                              size_t M, float* __restrict__ part, const int* __restrict__ mcount) {
+  wgrad_body<KN, true, true>(J, &xmap, M, part, mcount);
+}
 
 // floats of the partial buffer that tc_wgrad uses for these jobs at msplit sample splits (two bias slots per row)
 size_t wg_part_floats(const WgJobT* jobs, int njobs, int msplit) {
@@ -932,15 +978,20 @@ cudaError_t encode_x_map(CUtensorMap* map, const float* X, int ldx, size_t rows,
 
 // jobs -> tc_wgrad<KN> into part[off ..], or with PIECES one job as ceil(Kk / KN) column pieces of tc_wgrad_piece<KN>; R[i] receives
 // job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent launch behind the previous grid on the stream (see
-// tc_wgrad_all)
+// tc_wgrad_all).  mcount (not NULL): the _live kernels, whose rows are min(32 *mcount, M); the splits and the partial buffer stay M's.
 template <int KN, bool PIECES = false>
 cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msplit, float* part, size_t off, RedJob* R, bool chained,
-                         cudaStream_t st) {
+                         cudaStream_t st, const int* mcount = nullptr) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e;
-    if constexpr (PIECES) e = cudaFuncSetAttribute(tc_wgrad_piece<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
-    else e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+    if constexpr (PIECES) {
+      e = cudaFuncSetAttribute(tc_wgrad_piece<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_wgrad_piece_live<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+    } else {
+      e = cudaFuncSetAttribute(tc_wgrad<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_wgrad_live<KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Wg<KN>::SMEM);
+    }
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -973,9 +1024,10 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
   if constexpr (PIECES) {
     CUtensorMap xmap;
     e = encode_x_map(&xmap, jobs[0].X, jobs[0].ldx, M, KN, Wg<KN>::CH);
-    if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, tc_wgrad_piece<KN>, J, xmap, M, part);
+    if (e == cudaSuccess) e = mcount ? cudaLaunchKernelEx(&cfg, tc_wgrad_piece_live<KN>, J, xmap, M, part, mcount)
+                                     : cudaLaunchKernelEx(&cfg, tc_wgrad_piece<KN>, J, xmap, M, part);
   } else {
-    e = cudaLaunchKernelEx(&cfg, tc_wgrad<KN>, J, M, part);
+    e = mcount ? cudaLaunchKernelEx(&cfg, tc_wgrad_live<KN>, J, M, part, mcount) : cudaLaunchKernelEx(&cfg, tc_wgrad<KN>, J, M, part);
   }
   return e != cudaSuccess ? e : cudaGetLastError();
 }
@@ -996,7 +1048,10 @@ cudaError_t launch_wgrad(const WgJobT* jobs, int njobs, size_t M, int D, int msp
 // occ (nnb_field_grad with NNB_OCC_ONLY): the colour jobs (fc_feature, rgb_layers.0, fc_rgb) are left out, so grid 2 is not launched, the
 // head grid runs the density head alone, and the colour parameters' gradients are not touched.  The kernels are those of the full stage.
 // !bias (nnb_field_hvp_tc, whose tangent has no bias term): every job's db is NULL, so no bias slot of gw is touched.
-cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw, bool occ, bool bias, cudaStream_t st) {
+// mcount (nnb_render_frame_train_bwd_tmin's reverse rounds): every grid runs on the first min(32 *mcount, L.M) rows, read on the device,
+// with the split counts and partial regions of L.M (the _live kernels); at *mcount = L.M / 32 the results are those of mcount = NULL.
+cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw, bool occ, bool bias, cudaStream_t st,
+                          const int* mcount = nullptr) {
   char* base = static_cast<char*>(a.workspace);
   auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
   const int D = L.D, DR = D / 2;
@@ -1027,27 +1082,27 @@ cudaError_t tc_wgrad_jobs(const nnb_render_args& a, const WsLayout& L, float* gw
   const size_t head_f = small_jobs_part_floats(sm, nsm, L.M);
   const bool enc_chained = big_f + head_f + wg_part_floats(enc, 2, ms_enc) <= wpart_floats(L.M, D);
   RedJob R[9 + 2 + 3];
-  cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
-                : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, 0, R, false, st)
-                           : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, 0, R, false, st);
+  cudaError_t e = D == 256 ? launch_wgrad<256>(big, nb, L.M, D, ms_big, part, 0, R, false, st, mcount)
+                : D == 128 ? launch_wgrad<128>(big, nb, L.M, D, ms_big, part, 0, R, false, st, mcount)
+                           : launch_wgrad<64>(big, nb, L.M, D, ms_big, part, 0, R, false, st, mcount);
   if (e != cudaSuccess) return e;
   int nr = nb;
   if (!occ) {
-    e = launch_wgrad<64, true>(&rgb, 1, L.M, D, ms_big, part, trunk_f, R + nb, true, st);
+    e = launch_wgrad<64, true>(&rgb, 1, L.M, D, ms_big, part, trunk_f, R + nb, true, st, mcount);
     if (e != cudaSuccess) return e;
     nr += 1;
   }
   if (enc_chained) {   // encoding before heads: its CTAs need a whole SM each, and the small head CTAs would fragment the free SMs
-    e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, big_f + head_f, R + nr, true, st);
+    e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, big_f + head_f, R + nr, true, st, mcount);
     if (e != cudaSuccess) return e;
     nr += 2;
   }
-  e = launch_head_wgrad(sm, nsm, L.M, D, part, big_f, R + nr, st);
+  e = launch_head_wgrad(sm, nsm, L.M, D, part, big_f, R + nr, st, mcount);
   if (e != cudaSuccess) return e;
   nr += nsm;
   e = launch_wgrad_reduce(R, nr, part, st);
   if (e != cudaSuccess || enc_chained) return e;
-  e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, 0, R, false, st);   // the chained reduce has read the whole buffer
+  e = launch_wgrad<64>(enc, 2, L.M, D, ms_enc, part, 0, R, false, st, mcount);   // the chained reduce has read the whole buffer
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, 2, part, st);
 }
@@ -1132,19 +1187,23 @@ __device__ __forceinline__ void dg_gemm(float* acc, uint32_t a_hi, uint32_t a_lo
 // encoding adjoint delta_enc and p, -u_c sum_l f^2 (delta_sin sin(f p_c) + delta_cos cos(f p_c)), f = 2^l, with u = P.gs[m].  P.gp may be
 // NULL (no point term is stored).
 // DG_FRAME (tc_dgrad_frame, nnb_render_frame_bwd): DG_RAYS on the rows of chunk `chunk` of every ray (M = 32 N, row m is sample
-// chunk_sample(a, chunk, m)), the workspace arrays indexed by the row as tc_frame_stash wrote them.
+// chunk_sample(a, chunk, m)), the workspace arrays indexed by the row as tc_frame_stash wrote them.  With DEVN (tc_dgrad_frame_live): the
+// rows of the live list `list` as tc_frame_stash_live wrote them, M = 32 *count (count clamped to 0..N) read when the kernel starts.
 enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4, DG_POINTS_HVP_OCC = 5, DG_FRAME = 6 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
-                                              int n_tiles, int write_dy, const int* count = nullptr, int chunk = 0) {
+                                              int n_tiles, int write_dy, const int* count = nullptr, int chunk = 0,
+                                              const int* list = nullptr) {
   using T = Tc<D>;
   constexpr bool HVP = MODE == DG_POINTS_HVP_OCC, CHUNK = MODE == DG_FRAME;
   constexpr bool PTS = MODE != DG_RAYS && !CHUNK, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC || HVP;
   constexpr bool GRAD = MODE == DG_POINTS_GRAD || MODE == DG_POINTS_GRAD_OCC || HVP;
-  static_assert(!DEVN || (PTS && !GRAD), "a device count of explicit points");
+  static_assert(!DEVN || (PTS && !GRAD) || CHUNK, "a device count of explicit points or of a frame round's rays");
   if constexpr (PTS) write_dy = GRAD ? 1 : 0;
   if constexpr (DEVN) {
-    const int c = *count;
+    int c;   // rows
+    if constexpr (CHUNK) c = 32 * frame_live_count(count, a.N);
+    else c = *count;
     M = (size_t)c;
     n_tiles = (c + TILE - 1) / TILE;
     if ((int)blockIdx.x >= n_tiles) return;   // before any barrier exists
@@ -1310,7 +1369,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
 #pragma unroll
           for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
         } else {
-          if constexpr (CHUNK) chunk_geometry(a, chunk, m, ray, z, p);
+          if constexpr (CHUNK && DEVN) sample_geometry(a, live_sample(a, chunk, list, (int)(M >> 5), m), ray, z, p);
+          else if constexpr (CHUNK) chunk_geometry(a, chunk, m, ray, z, p);
           else row_geometry_tc(a, m, M, ray, z, p);
           if (a.pts) {
 #pragma unroll
@@ -1345,6 +1405,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
         const size_t mm = m < M ? m : M - 1;
 #pragma unroll
         for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + 3 * mm + c);
+      } else if constexpr (CHUNK && DEVN) {
+        sample_geometry(a, live_sample(a, chunk, list, (int)(M >> 5), m), ray, z, p);
       } else if constexpr (CHUNK) {
         chunk_geometry(a, chunk, m, ray, z, p);
       } else {
@@ -1387,6 +1449,13 @@ template <int D>
 __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad_frame(nnb_render_args a, const unsigned char* __restrict__ wimg,
                                                                const __grid_constant__ DgPtrs P, size_t M, int n_tiles, int write_dy, int k) {
   tc_dgrad_body<D, DG_FRAME>(a, wimg, P, M, n_tiles, write_dy, nullptr, k);
+}
+// tc_dgrad_frame on the rays of round k's live list (*count of them; the launch is sized for N)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad_frame_live(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                                    const __grid_constant__ DgPtrs P, int write_dy, int k,
+                                                                    const int* __restrict__ count, const int* __restrict__ list) {
+  tc_dgrad_body<D, DG_FRAME, true>(a, wimg, P, 0, 0, write_dy, count, k, list);
 }
 
 // nnb_field_vjp: the forward of explicit points with records and gate bits (FWD_VJP), then the chain on them (DG_POINTS[_OCC])
@@ -1943,6 +2012,8 @@ int frame_bwd_setup(cudaError_t* e) {
     *e = cudaFuncSetAttribute(tc_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
     if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_frame_stash<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
     if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_dgrad_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_frame_stash_live<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_dgrad_frame_live<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
     if (*e != cudaSuccess) return 0;
     int dev = 0; cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -1953,9 +2024,12 @@ int frame_bwd_setup(cudaError_t* e) {
 
 // The forward half of nnb_render_frame_bwd (nnb_render_frame_train_fwd): the forward weight image, then the forward (run_render_frame at
 // t_min = 0, so every ray runs every round) with the carry after each chunk copied to the checkpoints.  It leaves the weight image and
-// the checkpoints in the workspace for the reverse half.
+// the checkpoints in the workspace for the reverse half.  nnb_render_frame_train_fwd_tmin: the same at t_min, which also leaves the
+// per-ray chunk counts (FramePtrs::chunks) for the reverse rounds; a ray that stopped keeps its carry, so every checkpoint from its last
+// chunk on holds its final transmittance.
 template <int D>
-cudaError_t tc_frame_train_fwd_dim(const nnb_render_args& a, cudaStream_t st) {
+cudaError_t tc_frame_train_fwd_dim(const nnb_render_args& a, cudaStream_t st, float t_min = 0.f, int* n_eval = nullptr,
+                                   float* t_final = nullptr) {
   using T = Tc<D>;
   cudaError_t e;
   const int n_sm = frame_bwd_setup<D>(&e);
@@ -1968,7 +2042,7 @@ cudaError_t tc_frame_train_fwd_dim(const nnb_render_args& a, cudaStream_t st) {
   const int tiles = (N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm;   // 4 ray-chunks of 32 rows per tile
   float* ckpt = reinterpret_cast<float*>(base + w.ckpt);
   cudaError_t ec = cudaSuccess;
-  e = run_render_frame(a, w.f, 0.f, nullptr, nullptr, st, [&](const FramePtrs& f) {
+  e = run_render_frame(a, w.f, t_min, n_eval, t_final, st, [&](const FramePtrs& f) {
     tc_frame<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, f);
     if (f.k + 1 < C && ec == cudaSuccess) ec = cudaMemcpyAsync(ckpt + (size_t)f.k * N, f.carry, (size_t)N * 4, cudaMemcpyDeviceToDevice, st);
   });
@@ -1980,8 +2054,12 @@ cudaError_t tc_frame_train_fwd_dim(const nnb_render_args& a, cudaStream_t st) {
 // whose reduce adds the round's dW into g_weights, and frame_ray_acc; then frame_ray_finish and ray_reduce.  The rounds run one after
 // another on the stream.  Of what the forward half wrote it reads the forward weight image and the checkpoints only (data, no index or
 // counter), so a workspace the forward half did not fill gives wrong numbers, never an access outside the workspace.
+// live (nnb_render_frame_train_bwd_tmin): round k runs on the rays that evaluated chunk k (frame_live_list from the forward's chunk counts,
+// into the forward's first ray list and round counter, which are free once the forward has ended): the _live kernels, and the
+// weight-gradient stage on the list's rows.  Every count and counter read is clamped (1..C, 0..N), so a backward without its forward still
+// stays inside the workspace.
 template <int D>
-cudaError_t tc_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+cudaError_t tc_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st, bool live = false) {
   using T = Tc<D>;
   const nnb_render_args& a = b.fwd;
   cudaError_t e;
@@ -2014,17 +2092,29 @@ cudaError_t tc_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st
   fb.rounds = C; fb.ckpt = F(w.ckpt); fb.suffix = F(w.suffix); fb.rec = recs;
   fb.gs = reinterpret_cast<float4*>(cb + L.gs); fb.gp = P.gp; fb.gv = P.gv; fb.raypart = F(w.raypart);
   const int write_dy = b.g_weights ? 1 : 0, warps = (N + 7) / 8;
+  int* list = reinterpret_cast<int*>(base + w.f.list[0]);
+  int* count = reinterpret_cast<int*>(base);   // round counter 0 of the forward
+  const FrameLive fl{reinterpret_cast<const int*>(base + w.f.chunks), list, count};
   for (int k = C - 1; k >= 0; --k) {
     FramePtrs f{};
     f.k = k;
     fb.k = k;
-    tc_frame_stash<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, ts, f, tiles);
-    frame_chunk_adjoint<false><<<warps, 256, 0, st>>>(b, fb);
-    tc_dgrad_frame<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)N * 32, tiles, write_dy, k);
+    if (live) {
+      f.list = list; f.count = count;
+      frame_live_list<<<1, 1024, 0, st>>>(fl.chunks, N, k, C, list, count);
+      tc_frame_stash_live<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, ts, f);
+      frame_chunk_adjoint_live<<<warps, 256, 0, st>>>(b, fb, fl);
+      tc_dgrad_frame_live<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, write_dy, k, count, list);
+    } else {
+      tc_frame_stash<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, ts, f, tiles);
+      frame_chunk_adjoint<false><<<warps, 256, 0, st>>>(b, fb);
+      tc_dgrad_frame<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, (size_t)N * 32, tiles, write_dy, k);
+    }
     e = cudaGetLastError();
-    if (e == cudaSuccess && b.g_weights) e = tc_wgrad_jobs(ac, L, b.g_weights, false, true, st);
+    if (e == cudaSuccess && b.g_weights) e = tc_wgrad_jobs(ac, L, b.g_weights, false, true, st, live ? count : nullptr);
     if (e != cudaSuccess) return e;
-    frame_ray_acc<false><<<warps, 256, 0, st>>>(a, fb);
+    if (live) frame_ray_acc_live<<<warps, 256, 0, st>>>(a, fb, fl);
+    else frame_ray_acc<false><<<warps, 256, 0, st>>>(a, fb);
   }
   float* rayred = CF(L.rayred);
   frame_ray_finish<<<warps, 256, 0, st>>>(b, F(w.raypart), rayred);
@@ -2104,6 +2194,16 @@ cudaError_t tc_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStrea
 }
 cudaError_t tc_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
   return D == 128 ? tc_frame_train_bwd_dim<128>(b, st) : (D == 64 ? tc_frame_train_bwd_dim<64>(b, st) : tc_frame_train_bwd_dim<256>(b, st));
+}
+cudaError_t tc_render_frame_train_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st) {
+  const nnb_render_args& a = f.fwd;
+  return D == 128 ? tc_frame_train_fwd_dim<128>(a, st, f.t_min, f.n_eval, f.t_final)
+       : D == 64  ? tc_frame_train_fwd_dim<64>(a, st, f.t_min, f.n_eval, f.t_final)
+                  : tc_frame_train_fwd_dim<256>(a, st, f.t_min, f.n_eval, f.t_final);
+}
+cudaError_t tc_render_frame_train_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  return D == 128 ? tc_frame_train_bwd_dim<128>(b, st, true)
+       : (D == 64 ? tc_frame_train_bwd_dim<64>(b, st, true) : tc_frame_train_bwd_dim<256>(b, st, true));
 }
 // nnb_render_frame_bwd: the two halves in sequence
 cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {

@@ -523,7 +523,11 @@ class Trainer(object):
     Renderer(frame_grad=...): that flag governs Renderer.nope_nerf, which the Trainer does not call.
     frame_grad_engine (default None, needs frame_grad=True): 'simt' runs those renders on the exact-fp32 engine's pair,
     ops.ExactFrameRenderCall, at any rendering.num_points from 2 to 1024 whatever the renderer's engine; None or 'tc' is the tensor-core
-    pair above."""
+    pair above.
+    frame_grad_t_min (default None, needs frame_grad=True on the tensor-core pair): train with early ray termination,
+    ops.frame_render_call(t): a ray stops after the first 32-sample chunk that leaves its transmittance below t, and the backward
+    differentiates that truncated render, visiting only the rays that evaluated each chunk.  0.0 gives the frame_grad=True step's bits.
+    With frame_grad=False, frame_grad_engine='simt', or a negative or NaN value, it is a ValueError."""
 
     def __init__(self, model, optimizer, cfg, device=None, optimizer_pose=None, pose_param_net=None,
                  optimizer_focal=None, focal_net=None, optimizer_distortion=None, distortion_net=None, **kwargs):
@@ -599,13 +603,22 @@ class Trainer(object):
             if ops.pick_engine(engine, int(rend.cfg['num_points'])) != L.ENGINE_TC:
                 raise ValueError("Trainer(frame_grad=True) needs the tensor-core engine: the renderer's engine and rendering.num_points "
                                  "(16..1024) must resolve to it")
+        self.frame_grad_t_min = kwargs.get('frame_grad_t_min', None)
+        if self.frame_grad_t_min is not None:
+            if not self.frame_grad:
+                raise ValueError("Trainer: frame_grad_t_min needs frame_grad=True")
+            if self.frame_grad_engine == 'simt':
+                raise ValueError("Trainer: frame_grad_t_min runs on the tensor-core pair only (not with frame_grad_engine='simt')")
+            ops.frame_render_call(self.frame_grad_t_min)   # ValueError for a negative or NaN value
 
     # ------------------------------------------------------------------------------------
     def _train_render_call(self, backward):
         """the RenderCall class of a training render: the differentiable frame's pair (frame_grad) when it has a backward"""
         if not (self.frame_grad and backward):
             return ops.RenderCall
-        return ops.ExactFrameRenderCall if self.frame_grad_engine == 'simt' else ops.FrameRenderCall
+        if self.frame_grad_engine == 'simt':
+            return ops.ExactFrameRenderCall
+        return ops.FrameRenderCall if self.frame_grad_t_min is None else ops.frame_render_call(self.frame_grad_t_min)
 
     def _smoothness_on(self):
         """the pose-smoothness terms have a non-zero weight somewhere on their annealing schedule"""

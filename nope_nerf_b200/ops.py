@@ -91,6 +91,7 @@ class RenderCall:
     """One forward launch + the state its backward needs (workspace with the stash)."""
     frame = False         # FrameRenderCall: the differentiable frame's training pair
     exact_frame = False   # ExactFrameRenderCall: that pair on the exact-fp32 engine
+    t_min = None          # frame_render_call(t_min): that pair with early ray termination (the _tmin calls); None: without
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
                  depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256):
@@ -143,6 +144,12 @@ class RenderCall:
         self.args = a; self.N = N; self.S = S; self.stash = stash; self.pooled = True
         if exact:
             L.check(L.lib.nnb_render_frame_train_fwd_engine(C.byref(a), _stream()), "nnb_render_frame_train_fwd_engine")
+        elif frame and self.t_min is not None:
+            f = L.FrameArgs()
+            f.fwd = a
+            self.n_eval = torch.empty(N, dtype=torch.int32, device=dev)
+            f.t_min = self.t_min; f.n_eval = L.ptr(self.n_eval); f.t_final = None
+            L.check(L.lib.nnb_render_frame_train_fwd_tmin(C.byref(f), _stream()), "nnb_render_frame_train_fwd_tmin")
         elif frame:
             L.check(L.lib.nnb_render_frame_train_fwd(C.byref(a), _stream()), "nnb_render_frame_train_fwd")
         else:
@@ -167,6 +174,8 @@ class RenderCall:
         b.g_scale_shift = L.ptr(g_scale_shift)
         if self.exact_frame:
             L.check(L.lib.nnb_render_frame_train_bwd_engine(C.byref(b), _stream()), "nnb_render_frame_train_bwd_engine")
+        elif self.frame and self.t_min is not None:
+            L.check(L.lib.nnb_render_frame_train_bwd_tmin(C.byref(b), _stream()), "nnb_render_frame_train_bwd_tmin")
         elif self.frame:
             L.check(L.lib.nnb_render_frame_train_bwd(C.byref(b), _stream()), "nnb_render_frame_train_bwd")
         else:
@@ -182,6 +191,26 @@ class FrameRenderCall(RenderCall):
     so `stash` is implied and ignored.  want_z_alpha, and an engine that pick_engine does not resolve to the tensor-core engine
     (ENGINE_SIMT, or S < 16), are a ValueError, raised before any other check."""
     frame = True
+
+
+_frame_tmin_calls = {}
+
+
+def frame_render_call(t_min):
+    """the FrameRenderCall class that trains with early ray termination at t_min (one class per value, cached): its forward is
+    nnb_render_frame_train_fwd_tmin, which stops each ray as render_frame(t_min=...) does and exposes the samples each ray evaluated as
+    the int32 [N] tensor `n_eval`, and backward() is nnb_render_frame_train_bwd_tmin, whose reverse rounds visit only the rays that
+    evaluated each chunk.  The gradients are those of the truncated render.  t_min = 0 gives FrameRenderCall's bits.  A negative or NaN
+    t_min is a ValueError."""
+    t = float(t_min)
+    if not t >= 0.0:
+        raise ValueError("frame_render_call: t_min must be >= 0 (got %r)" % (t_min,))
+    t = float(C.c_float(t).value)   # the value the library receives
+    cls = _frame_tmin_calls.get(t)
+    if cls is None:
+        cls = type("FrameRenderCall_tmin", (FrameRenderCall,), {"t_min": t, "__doc__": frame_render_call.__doc__})
+        _frame_tmin_calls[t] = cls
+    return cls
 
 
 class ExactFrameRenderCall(FrameRenderCall):
