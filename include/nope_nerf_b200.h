@@ -489,6 +489,36 @@ int nnb_render_frame_train_bwd(const nnb_render_bwd_args* b, void* stream);
 int nnb_render_frame_train_fwd_tmin(const nnb_frame_args* f, void* stream);
 int nnb_render_frame_train_bwd_tmin(const nnb_render_bwd_args* b, void* stream);
 
+/* Training with early ray termination on the per-sample stash, on the tensor-core engine: each sample is evaluated once, and the backward
+ * runs one weight-gradient stage over the rows the forward evaluated.  It trades the memory of nnb_render_frame_train_fwd_tmin's pair
+ * (the stash path's worst case here) for time.  No version bump: the symbols mark the capability.
+ * nnb_render_fwd_tmin(f): f->fwd as nnb_render_frame_train_fwd_tmin's (nnb_render_fwd's training arguments without NNB_STASH, which is
+ *   implied; noise accepted), f->t_min, and the optional f->n_eval / f->t_final.  Ray n evaluates chunks 0 .. c_n - 1 under
+ *   nnb_render_frame's stop rule; round k evaluates chunk k of the rays {n : c_n > k}, listed in increasing n by a block scan, with the
+ *   training stash, and composites them with nnb_render_frame's statements.  rgb, depth_pred, depth_gt, mask and n_eval are
+ *   nnb_render_frame_train_fwd_tmin's bits at the same t_min, noise or not (t_final is formed by the same statements); at t_min = 0 the
+ *   outputs are nnb_render_fwd's (NNB_STASH).
+ *   Every round's rows go into one packed stash: round k's start at R_k, the rows of the rounds before padded to the 128-row tile, formed
+ *   on the device from the rounds' counts.  The workspace keeps the stash, the chunk counts, the lists and the checkpoints.
+ * nnb_render_bwd_tmin(b): after that call, with nnb_render_bwd's cotangents and outputs (g_weights may be NULL: pose, camera, depth and
+ *   scale-shift gradients only).  The gradients are the exact gradients of the truncated render with every c_n held constant, the
+ *   definition of nnb_render_frame_train_bwd_tmin: the compositing adjoint of ray n runs from its chunk c_n - 1, with a zero suffix there,
+ *   to chunk 0; the data-gradient chain runs on the packed rows and the weight-gradient stage once over them, with the row count read on
+ *   the device.  The pose, camera, depth and scale-shift gradients are nnb_render_frame_train_bwd_tmin's bits; the MLP gradients differ
+ *   from it in the order of their sums.  Every c_n read is clamped to 1..C (C = ceil(S / 32)) and every device count to 0..N: a backward
+ *   without its forward gives wrong numbers, never an access outside the workspace.  Every sum runs in a fixed order, padding rows get a
+ *   zero cotangent, and no count is read back, so the same inputs give the same bits whatever the workspace held, and both calls can be
+ *   captured in a CUDA graph and replayed when the stop pattern changes.  Neither call synchronises or allocates.
+ * nnb_render_tmin_workspace_bytes(N, S, hidden_dim): the workspace of both calls, for every ray running every chunk: the training stash of
+ *   C 128 ceil(N / 4) rows (at least nnb_workspace_bytes_dim(N, S, NNB_STASH, NNB_ENGINE_TC, hidden_dim)) and the per-ray state.  0 for
+ *   N <= 0, S outside 16..1024 or an unsupported width.
+ * Errors, with nothing launched: NULL args (rc -1); an engine other than NNB_ENGINE_TC (-4); then the checks and codes of
+ *   nnb_render_frame_train_fwd_tmin / _bwd_tmin in their order (sizes -2, with S below 16 -4 as on that pair; a negative or NaN t_min -2;
+ *   misaligned n_eval / t_final -3; non-NULL z_vals, alpha, pts or dirs -6; NNB_STASH -6), with this workspace's size (-5). */
+size_t nnb_render_tmin_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim);
+int nnb_render_fwd_tmin(const nnb_frame_args* f, void* stream);
+int nnb_render_bwd_tmin(const nnb_render_bwd_args* b, void* stream);
+
 /* nnb_render_frame_bwd, nnb_render_frame_train_fwd and nnb_render_frame_train_bwd on fwd.engine.  NNB_ENGINE_TC is exactly the call
  * without the suffix (its checks, codes, bits and workspace).  NNB_ENGINE_SIMT runs the same method on the exact-fp32 engine at any S from
  * 2 to 1024, with a chunk stash that packs R = min(S, 32) rows per ray (row R n + j is sample 32 k + j of ray n), so a round at S < 32

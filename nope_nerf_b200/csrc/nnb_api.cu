@@ -47,6 +47,9 @@ cudaError_t tc_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStrea
 cudaError_t tc_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t tc_render_frame_train_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st);
 cudaError_t tc_render_frame_train_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st);
+size_t tc_render_tmin_workspace(int N, int S, int D);
+cudaError_t tc_render_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st);
+cudaError_t tc_render_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t tc_geometry_frame(const nnb_geometry_args& g, int D, cudaStream_t st);
 bool tc_supports(int S);
 #endif
@@ -646,6 +649,52 @@ int nnb_render_frame_train_bwd_tmin(const nnb_render_bwd_args* b, void* stream) 
   if (int rc = check_frame_train_ws(a)) return rc;
   const cudaError_t e = tc_render_frame_train_bwd_tmin(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_frame_train_bwd_tmin");
+#endif
+}
+size_t nnb_render_tmin_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim) {
+#ifdef NNB_WITH_TC
+  const int D = hidden_of(hidden_dim);
+  if (N > 0 && tc_supports(S) && nnb::dim_supported(D)) return tc_render_tmin_workspace(N, S, D);
+#endif
+  return 0;
+}
+static int check_tmin_ws(const nnb_render_args* a) {
+  const size_t need = nnb_render_tmin_workspace_bytes(a->N, a->S, a->hidden_dim);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  return 0;
+}
+int nnb_render_fwd_tmin(const nnb_frame_args* f, void* stream) {
+  if (!f) return fail(-1, "null args");
+  const nnb_render_args* a = &f->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_fwd_tmin: engine %d has no stash render with early termination (NNB_ENGINE_TC only)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_frame(a, true)) return rc;
+  if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_fwd_tmin: t_min must be >= 0 (got %g)", (double)f->t_min);
+  if (int rc = check_frame_io(a)) return rc;
+  if (misaligned4(f->n_eval) || misaligned4(f->t_final)) return fail(-3, "nnb_render_fwd_tmin: n_eval and t_final must be 4-byte aligned");
+  if (int rc = check_tmin_ws(a)) return rc;
+  const cudaError_t e = tc_render_fwd_tmin(*f, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_fwd_tmin");
+#endif
+}
+int nnb_render_bwd_tmin(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (a->engine != NNB_ENGINE_TC)
+    return fail(-4, "nnb_render_bwd_tmin: engine %d has no stash render with early termination (NNB_ENGINE_TC only)", a->engine);
+#ifndef NNB_WITH_TC
+  return fail(-4, "library built without the tensor-core engine");
+#else
+  if (int rc = check_frame(a, true)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_bwd_tmin: g_rgb and g_c2w must be non-null");
+  if (int rc = check_tmin_ws(a)) return rc;
+  const cudaError_t e = tc_render_bwd_tmin(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_bwd_tmin");
 #endif
 }
 size_t nnb_render_frame_bwd_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine) {

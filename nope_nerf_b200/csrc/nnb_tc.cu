@@ -238,6 +238,138 @@ __device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, 
   sample_geometry(a, chunk_sample(a, k, m), ray, z, p);
 }
 
+// ---- nnb_render_fwd_tmin / nnb_render_bwd_tmin (early ray termination on the per-sample stash, tensor-core engine) ----------------
+// Round k evaluates chunk k of the rays {n : c_n > k}, listed in increasing n by frame_live_list into lists[k] ([C][N]) with their count
+// in counts[k]; the forward writes c_n (FramePtrs::chunks) as C while a ray is live and k + 1 when it stops in round k, so the lists of
+// the rounds after round 0 (whose list is every ray whatever chunks holds) come from the chunk counts the rounds before wrote.  Every
+// round's training stash goes into one packed stash: round k's rows start at R_k = sum over j < k of 128 ceil(count_j / 4) (each round
+// padded to the 128-row tile, the unit of the gate bits), and row R_k + 32 slot + j is sample 32 k + j of ray lists[k][slot].  counts[C]
+// holds R_C / 32, the stash's row count for the weight-gradient stage.  Every count is clamped to 0..N where it is read, so every row
+// index stays below the packed stash's C 128 ceil(N / 4) rows.
+__device__ __forceinline__ size_t stash_round_base(const int* counts, int k, int N) {
+  size_t r = 0;
+  for (int j = 0; j < k; ++j) r += (size_t)128 * ((frame_live_count(counts + j, N) + 3) / 4);
+  return r;
+}
+// (ray, sample) of packed row m: the round whose rows hold m (the last round past them), the slot's ray (padding slots take the list's
+// last ray, rows past the ray's last sample that sample: their cotangent is zero)
+__device__ __forceinline__ int2 stash_row_sample(const nnb_render_args& a, const int* lists, const int* counts, int C, size_t m) {
+  size_t r = 0;
+  int k = 0;
+  for (; k < C - 1; ++k) {
+    const size_t rows = (size_t)128 * ((frame_live_count(counts + k, a.N) + 3) / 4);
+    if (m < r + rows) break;
+    r += rows;
+  }
+  const int slot = min((int)((m - r) >> 5), max(frame_live_count(counts + k, a.N) - 1, 0));
+  return make_int2(min(max(lists[(size_t)k * a.N + slot], 0), a.N - 1), min(32 * k + (int)(m & 31), a.S - 1));
+}
+// slot of ray n in a round's list (increasing n): the first slot whose ray is not below n, clamped to the list
+__device__ __forceinline__ int stash_slot(const int* list, int count, int n) {
+  int lo = 0, hi = count;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (list[mid] < n) lo = mid + 1; else hi = mid;
+  }
+  return min(lo, max(count - 1, 0));
+}
+
+// Back end of forward round f.k (f.list = lists[k], f.count = counts + k): one warp per slot, frame_step's arithmetic on the (r, g, b, a)
+// of the round's packed records, from the ray's carry and lane partials of the rounds before.  Lane 0 stores the carry, its checkpoint
+// ckpt[k][n] (transmittance into chunk k + 1) and c_n: k + 1 when the ray stops (frame_step's rule), C while it stays live.
+__global__ void stash_frame_step(nnb_render_args a, const __grid_constant__ FramePtrs f, const SampleRec* __restrict__ rec,
+                                 float* __restrict__ ckpt, int C) {
+  const int lane = threadIdx.x & 31, slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (slot >= frame_live_count(f.count, a.N)) return;
+  const int n = f.list[slot];
+  const int i = 32 * f.k + lane;
+  const bool valid = i < a.S;
+  float4 me = make_float4(0.f, 0.f, 0.f, 0.f);
+  float z = 0.f, alpha = 0.f;
+  if (valid) {
+    const SampleRec r = rec[stash_round_base(f.count - f.k, f.k, a.N) + (size_t)slot * 32 + lane];
+    me = make_float4(r.r, r.g, r.b, r.a);
+    z = sample_z(a, n, i);
+    alpha = composite_alpha(a, i, me.w, z, [&] { return sample_z(a, n, i + 1); });
+  }
+  float* part = f.part + (size_t)n * 160 + lane;
+  float carry = 1.f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dist = 0.f, acc = 0.f;
+  if (f.k > 0) { carry = f.carry[n]; C0 = part[0]; C1 = part[32]; C2 = part[64]; Dist = part[96]; acc = part[128]; }
+  composite_chunk(alpha, valid, me.x, me.y, me.z, z, lane, carry, C0, C1, C2, Dist, acc);
+  part[0] = C0; part[32] = C1; part[64] = C2; part[96] = Dist; part[128] = acc;
+  if (lane == 0) {
+    f.carry[n] = carry;
+    if (f.k + 1 < C) ckpt[(size_t)f.k * a.N + n] = carry;
+    f.chunks[n] = carry < f.t_min || 32 * (f.k + 1) >= a.S ? f.k + 1 : C;
+  }
+}
+
+// Compositing adjoint of the packed stash, one warp per ray: frame_chunk_adjoint_live's statements for chunks c_n - 1 .. 0, the suffix
+// carry starting at 0 in the ray's last chunk and held in a register between chunks.  Warps N .. N + 3 C - 1 zero the cotangents of
+// round (w - N) / 3's padding slots count .. 4 ceil(count / 4) - 1, so those rows give zero dY.  Thread 0 stores counts[C] = R_C / 32.
+__global__ void stash_chunk_adjoint(nnb_render_bwd_args b, const __grid_constant__ FrameBwdPtrs f, const int* __restrict__ chunks,
+                                    const int* __restrict__ lists, int* __restrict__ counts) {
+  const nnb_render_args& a = b.fwd;
+  const int C = f.rounds;
+  const int lane = threadIdx.x & 31, w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w == 0 && lane == 0) counts[C] = (int)(stash_round_base(counts, C, a.N) / 32);
+  if (w >= a.N) {
+    const int k = (w - a.N) / 3;
+    if (k >= C) return;
+    const int cnt = frame_live_count(counts + k, a.N), slot = cnt + (w - a.N) % 3;
+    if (slot < (cnt + 3) / 4 * 4) f.gs[stash_round_base(counts, k, a.N) + (size_t)slot * 32 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  const int n = w;
+  Ray ray; setup_ray(a, n, ray);
+  float gD = b.g_depth_pred ? __ldg(b.g_depth_pred + n) : 0.f;
+  if ((a.flags & NNB_EVAL) && (a.flags & NNB_NORMALISE)) gD = gD / ray.nrm;
+  const float gC0 = __ldg(b.g_rgb + 3 * n), gC1 = __ldg(b.g_rgb + 3 * n + 1), gC2 = __ldg(b.g_rgb + 3 * n + 2);
+  const float gsum = (a.flags & NNB_WHITE_BG) ? (gC0 + gC1 + gC2) : 0.f;
+  float carry_s = 0.f;
+  for (int k = frame_ray_chunks(chunks, n, C) - 1; k >= 0; --k) {
+    const int slot = stash_slot(lists + (size_t)k * a.N, frame_live_count(counts + k, a.N), n);
+    const size_t m = stash_round_base(counts, k, a.N) + (size_t)slot * 32 + lane;
+    const int i = 32 * k + lane;
+    const bool valid = i < a.S;
+    const SampleRec me = valid ? f.rec[m] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
+    float alpha = 0.f, df = 1.f;   // df = d alpha / d a
+    if (valid) {
+      alpha = composite_alpha(a, i, me.a, me.z, [&] { return sample_z(a, n, i + 1); });
+      if (a.flags & NNB_DIST_ALPHA) {
+        if (i >= a.S - 1) df = 0.f;
+        else { const float delta = __fsub_rn(sample_z(a, n, i + 1), me.z); df = delta * expf(-me.a * delta); }
+      }
+    }
+    const float carry = k > 0 ? f.ckpt[(size_t)(k - 1) * a.N + n] : 1.f;
+    f.gs[m] = composite_chunk_bwd<false>(alpha, valid, me.r, me.g, me.b, me.z, df, lane, carry, gC0, gC1, gC2, gD, gsum, carry_s);
+  }
+}
+
+// frame_ray_acc_live's sums on the packed stash, one warp per ray: the terms of chunks c_n - 1 .. 0 added in that order to lane partials
+// that start at 0, stored once for frame_ray_finish
+__global__ void stash_ray_acc(nnb_render_args a, const __grid_constant__ FrameBwdPtrs f, const int* __restrict__ chunks,
+                              const int* __restrict__ lists, const int* __restrict__ counts) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  float v[9];
+#pragma unroll
+  for (int c = 0; c < 9; ++c) v[c] = 0.f;
+  for (int k = frame_ray_chunks(chunks, n, f.rounds) - 1; k >= 0; --k) {
+    if (32 * k + lane >= a.S) continue;
+    const int slot = stash_slot(lists + (size_t)k * a.N, frame_live_count(counts + k, a.N), n);
+    const size_t m = stash_round_base(counts, k, a.N) + (size_t)slot * 32 + lane;
+    const float4 g = f.gp[m], dv = f.gv[m];
+    const float z = f.rec[m].z;
+    v[0] += g.x; v[1] += g.y; v[2] += g.z;
+    v[3] += z * g.x; v[4] += z * g.y; v[5] += z * g.z;
+    v[6] += dv.x; v[7] += dv.y; v[8] += dv.z;
+  }
+  float* part = f.raypart + (size_t)n * 288 + lane;
+#pragma unroll
+  for (int c = 0; c < 9; ++c) part[32 * c] = v[c];
+}
+
 // MODE FWD_RAYS (tc_field_fwd): recs [Mpad], out unused.  FWD_POINTS: explicit points (tc_points_fwd): a.pts / a.dirs [M][3] ->
 // out [M] = (r, g, b, a), or (0, 0, 0, a) with NNB_OCC_ONLY; nothing is stashed and recs is not written.  M = a.N there, so point indices
 // are 32-bit.  FWD_VJP (tc_points_vjp_fwd, nnb_field_vjp): FWD_POINTS that also writes recs [Mpad] and the ReLU gate bits st.gates of
@@ -262,6 +394,9 @@ __device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, 
 // past M hold the last point's values): h0..h7, feat, hr and enc as FWD_RAYS does, and denc per point (the direction encoding of
 // a.dirs[m], or of the ones), which is a per-row operand of rgb_layers.0 here.  With NNB_OCC_ONLY the colour part (feat, hr, denc) is not
 // written.
+// FWD_PACK (tc_stash_pack, nnb_render_fwd_tmin): FWD_CHUNK with DEVN on round fr.k's list (fr.list, fr.count = counts + k), into the
+// packed stash of nnb_frame.cuh: its rows go to packed rows R_k + m (R_k from counts[0 .. k - 1], read when the kernel starts), its gate
+// bits to tiles R_k / 128 + tile of a stash of M rows.
 // FWD_TANGENT (tc_points_tangent, nnb_field_hvp_tc): the tangent chain of the density logit along u on the trunk of an occupancy-only
 // FWD_VJP forward: the prologue puts e' = J_enc(p) u in E (u = (*out)[m], read, never written; rows past M have u = 0), every layer is
 // the bias-free z'_l = W_l x'_{l-1} ([h'3 | e'] into layer 4), gated with the forward's bits st.gates (read as tc_dgrad reads them)
@@ -269,13 +404,15 @@ __device__ __forceinline__ void chunk_geometry(const nnb_render_args& a, int k, 
 // because tangents span the range of gradients.  e' and h'0..h'7 of every row of every tile go to st.enc / st.h with the stash's
 // streaming stores; nothing else is written.
 enum : int { FWD_RAYS = 0, FWD_POINTS = 1, FWD_MARCH = 2, FWD_SECANT = 3, FWD_VJP = 4, FWD_FRAME = 5, FWD_GRAD = 6, FWD_TANGENT = 7,
-             FWD_CHUNK = 8 };
+             FWD_CHUNK = 8, FWD_PACK = 9 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, SampleRec* __restrict__ recs,
                                             float4* __restrict__ out, const TcStash& st, const MarchPtrs& q, size_t M, int n_tiles,
                                             int stash, const FramePtrs& fr = FramePtrs{}) {
   using T = Tc<D>;
-  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD, TAN = MODE == FWD_TANGENT, CHUNK = MODE == FWD_CHUNK;
+  constexpr bool PACK = MODE == FWD_PACK;
+  constexpr bool FRAME = MODE == FWD_FRAME, GRAD = MODE == FWD_GRAD, TAN = MODE == FWD_TANGENT, CHUNK = MODE == FWD_CHUNK || PACK;
+  static_assert(!PACK || DEVN, "the packed stash takes its rows from the round's list");
   constexpr bool PTS = MODE != FWD_RAYS && !FRAME && !CHUNK, MARCH = MODE == FWD_MARCH || MODE == FWD_SECANT, VJP = MODE == FWD_VJP || GRAD;
   constexpr bool XPTS = MODE == FWD_POINTS || VJP;   // points read from a.pts
   static_assert(!DEVN || XPTS || CHUNK, "a device count of explicit points or of a frame round's rays");
@@ -292,6 +429,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
     n_tiles = (n_live + 3) / 4;
     if ((int)blockIdx.x >= n_tiles) return;   // a CTA without a tile leaves before any barrier exists
   }
+  const size_t mo = PACK ? stash_round_base(fr.count - fr.k, fr.k, a.N) : 0;   // FWD_PACK: packed row of the round's row 0
   const bool gates = !TAN && (VJP || stash);   // the ReLU gate bits are stored
   if constexpr (MARCH || (DEVN && !CHUNK)) {
     if (q.count) {
@@ -441,8 +579,8 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         if constexpr (TAN) split_store8_bf16(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
         else split_store8(ee + kb * 8, smem + SM_EHI + kb * 2048 + row * 16, smem + SM_ELO + kb * 2048 + row * 16);
         if (stash) {
-          __stcs(reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8), make_float4(ee[kb * 8], ee[kb * 8 + 1], ee[kb * 8 + 2], ee[kb * 8 + 3]));
-          __stcs(reinterpret_cast<float4*>(st.enc + m * 64 + kb * 8 + 4), make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]));
+          __stcs(reinterpret_cast<float4*>(st.enc + (mo + m) * 64 + kb * 8), make_float4(ee[kb * 8], ee[kb * 8 + 1], ee[kb * 8 + 2], ee[kb * 8 + 3]));
+          __stcs(reinterpret_cast<float4*>(st.enc + (mo + m) * 64 + kb * 8 + 4), make_float4(ee[kb * 8 + 4], ee[kb * 8 + 5], ee[kb * 8 + 6], ee[kb * 8 + 7]));
         }
       }
       if constexpr (!PTS) if (part == 0) {   // direction-encoding term of rgb_layers.0 is constant per ray: folded into a per-ray bias below
@@ -454,7 +592,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
         if (stash) {
 #pragma unroll
           for (int k4 = 0; k4 < 8; ++k4)
-            __stcs(reinterpret_cast<float4*>(st.denc + m * 32 + k4 * 4), make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]));
+            __stcs(reinterpret_cast<float4*>(st.denc + (mo + m) * 32 + k4 * 4), make_float4(de[4 * k4], de[4 * k4 + 1], de[4 * k4 + 2], de[4 * k4 + 3]));
         }
         if (rl == 0 || (off0 + rl) % ray_len() == 0) {   // the block's first row and every row that starts a ray publish its direction encoding
           const int r = (off0 + rl) / ray_len();
@@ -552,11 +690,12 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
             *reinterpret_cast<uint32_t*>(smem + SM_AHI + off) = hw;
             *reinterpret_cast<uint32_t*>(smem + SM_ALO + off) = lw;
             if (g == 7) s_logit[r] = fmaf(v1, s_bias[W_SIG0 + col + 1], fmaf(v0, s_bias[W_SIG0 + col], s_logit[r]));
-            if (sp) __stcs(reinterpret_cast<float2*>(sp + (mt + row) * D + col), make_float2(v0, v1));
+            if (sp) __stcs(reinterpret_cast<float2*>(sp + (mo + mt + row) * D + col), make_float2(v0, v1));
             gw[j / 8] = push_gate(push_gate(gw[j / 8], v0), v1);
           }
         }
-        if (gates && g < 8) store_gates<D / 2>(st.gates + gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
+        if (gates && g < 8) store_gates<D / 2>(st.gates + (PACK ? gate_bits_off(g, mo / TILE + tile, threadIdx.x, M, D)
+                                                               : gate_bits_off(g, tile, threadIdx.x, (size_t)n_tiles * TILE, D)), gw);
         if constexpr (PTS) {
           // Layer 4 was the last reader of E.  The direction operand of the rgb hidden layer takes its place: enc4(dirs[m]), 27 columns
           // padded to 32 (two K-steps), as fp16 hi | lo in E's layout.  A warp writes the 16 rows its own MMAs read, like the A operand
@@ -600,11 +739,12 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
 #pragma unroll
             for (int c = 0; c < 3; ++c)
               c_acc[r][c] = fmaf(v1, s_bias[W_RGB0 + c * DR + col + 1], fmaf(v0, s_bias[W_RGB0 + c * DR + col], c_acc[r][c]));
-            if (stash) __stcs(reinterpret_cast<float2*>(st.hr + (mt + row) * DR + col), make_float2(v0, v1));
+            if (stash) __stcs(reinterpret_cast<float2*>(st.hr + (mo + mt + row) * DR + col), make_float2(v0, v1));
             gw[j / 8] = push_gate(push_gate(gw[j / 8], v0), v1);
           }
         }
-        if (gates) store_gates<D / 4>(st.gates + gate_bits_off(8, tile, threadIdx.x, (size_t)n_tiles * TILE, D), gw);
+        if (gates) store_gates<D / 4>(st.gates + (PACK ? gate_bits_off(8, mo / TILE + tile, threadIdx.x, M, D)
+                                                               : gate_bits_off(8, tile, threadIdx.x, (size_t)n_tiles * TILE, D)), gw);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const float sl = quad_sum(s_logit[r]);
@@ -630,7 +770,7 @@ __device__ __forceinline__ void tc_fwd_body(const nnb_render_args& a, const unsi
               const int2 ni = DEVN ? live_sample(a, fr.k, fr.list, n_live, m) : chunk_sample(a, fr.k, m);
               rec.z = sample_z(a, ni.x, ni.y);
               rec.pad0 = 0.f; rec.pad1 = 0.f;
-              recs[m] = rec;
+              recs[mo + m] = rec;
             } else {
               rec.z = sample_z(a, (int)(mm / a.S), (int)(mm % a.S));
               rec.pad0 = 0.f; rec.pad1 = 0.f;
@@ -742,6 +882,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_frame_stash_live(nnb_render_a
                                                                     SampleRec* __restrict__ recs, const __grid_constant__ TcStash st,
                                                                     const __grid_constant__ FramePtrs f) {
   tc_fwd_body<D, FWD_CHUNK, true>(a, wimg, recs, nullptr, st, MarchPtrs{}, (size_t)a.N * 32, 0, 1, f);
+}
+// one forward round of nnb_render_fwd_tmin: tc_frame_stash_live into the packed stash of M rows (FWD_PACK)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_stash_pack(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                              SampleRec* __restrict__ recs, const __grid_constant__ TcStash st,
+                                                              const __grid_constant__ FramePtrs f, size_t M) {
+  tc_fwd_body<D, FWD_PACK, true>(a, wimg, recs, nullptr, st, MarchPtrs{}, M, 0, 1, f);
 }
 
 // ---- weight gradients: dW[n][k] += sum_m dY[m][n] X[m][k] (and db[n] += sum_m dY[m][n]) over the fp32 stash ----------------------
@@ -1189,20 +1336,28 @@ __device__ __forceinline__ void dg_gemm(float* acc, uint32_t a_hi, uint32_t a_lo
 // DG_FRAME (tc_dgrad_frame, nnb_render_frame_bwd): DG_RAYS on the rows of chunk `chunk` of every ray (M = 32 N, row m is sample
 // chunk_sample(a, chunk, m)), the workspace arrays indexed by the row as tc_frame_stash wrote them.  With DEVN (tc_dgrad_frame_live): the
 // rows of the live list `list` as tc_frame_stash_live wrote them, M = 32 *count (count clamped to 0..N) read when the kernel starts.
-enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4, DG_POINTS_HVP_OCC = 5, DG_FRAME = 6 };
+// DG_PACK (tc_dgrad_pack, nnb_render_bwd_tmin, DEVN): DG_RAYS on the packed stash of nnb_frame.cuh (M rows; its gate bits are laid out for
+// M), on its first 32 count[C] rows (C = `chunk`, count = the rounds' counts, list = their lists), read when the kernel starts; row m is
+// sample stash_row_sample(m).
+enum : int { DG_RAYS = 0, DG_POINTS = 1, DG_POINTS_OCC = 2, DG_POINTS_GRAD = 3, DG_POINTS_GRAD_OCC = 4, DG_POINTS_HVP_OCC = 5, DG_FRAME = 6,
+             DG_PACK = 7 };
 template <int D, int MODE, bool DEVN = false>
 __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const unsigned char* __restrict__ wimg, const DgPtrs& P, size_t M,
                                               int n_tiles, int write_dy, const int* count = nullptr, int chunk = 0,
                                               const int* list = nullptr) {
   using T = Tc<D>;
-  constexpr bool HVP = MODE == DG_POINTS_HVP_OCC, CHUNK = MODE == DG_FRAME;
+  constexpr bool PACK = MODE == DG_PACK;
+  constexpr bool HVP = MODE == DG_POINTS_HVP_OCC, CHUNK = MODE == DG_FRAME || PACK;
+  static_assert(!PACK || DEVN, "the packed stash's row count is read on the device");
+  const size_t m_cap = M;   // DG_PACK: rows of the packed stash
   constexpr bool PTS = MODE != DG_RAYS && !CHUNK, OCC = MODE == DG_POINTS_OCC || MODE == DG_POINTS_GRAD_OCC || HVP;
   constexpr bool GRAD = MODE == DG_POINTS_GRAD || MODE == DG_POINTS_GRAD_OCC || HVP;
   static_assert(!DEVN || (PTS && !GRAD) || CHUNK, "a device count of explicit points or of a frame round's rays");
   if constexpr (PTS) write_dy = GRAD ? 1 : 0;
   if constexpr (DEVN) {
     int c;   // rows
-    if constexpr (CHUNK) c = 32 * frame_live_count(count, a.N);
+    if constexpr (PACK) c = 32 * min(max(count[chunk], 0), (int)(m_cap / 32));
+    else if constexpr (CHUNK) c = 32 * frame_live_count(count, a.N);
     else c = *count;
     M = (size_t)c;
     n_tiles = (c + TILE - 1) / TILE;
@@ -1262,7 +1417,7 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
   // ReLU gate bits of the layer below the next epilogue (the rgb hidden layer's for the head prologue), loaded before the GEMM that
   // precedes that epilogue so the load completes behind its MMAs
   uint32_t gm[D / 64];
-  const size_t Mpad = (size_t)n_tiles * TILE;
+  const size_t Mpad = PACK ? m_cap : (size_t)n_tiles * TILE;
   // epilogue of a D-wide layer: x (+ g_s w_sigma) -> ReLU gate gm (when `gated`) -> dY stash -> next A operand (in place)
   auto epiD = [&](size_t mt, bool gated, float* dst, bool add_sigma) {
 #pragma unroll
@@ -1369,7 +1524,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
 #pragma unroll
           for (int c = 0; c < 3; ++c) v[c] = a.dirs ? __ldg(a.dirs + 3 * mm + c) : 1.f;
         } else {
-          if constexpr (CHUNK && DEVN) sample_geometry(a, live_sample(a, chunk, list, (int)(M >> 5), m), ray, z, p);
+          if constexpr (PACK) sample_geometry(a, stash_row_sample(a, list, count, chunk, m), ray, z, p);
+          else if constexpr (CHUNK && DEVN) sample_geometry(a, live_sample(a, chunk, list, (int)(M >> 5), m), ray, z, p);
           else if constexpr (CHUNK) chunk_geometry(a, chunk, m, ray, z, p);
           else row_geometry_tc(a, m, M, ray, z, p);
           if (a.pts) {
@@ -1405,6 +1561,8 @@ __device__ __forceinline__ void tc_dgrad_body(const nnb_render_args& a, const un
         const size_t mm = m < M ? m : M - 1;
 #pragma unroll
         for (int c = 0; c < 3; ++c) p[c] = __ldg(a.pts + 3 * mm + c);
+      } else if constexpr (PACK) {
+        sample_geometry(a, stash_row_sample(a, list, count, chunk, m), ray, z, p);
       } else if constexpr (CHUNK && DEVN) {
         sample_geometry(a, live_sample(a, chunk, list, (int)(M >> 5), m), ray, z, p);
       } else if constexpr (CHUNK) {
@@ -1456,6 +1614,13 @@ __global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad_frame_live(nnb_render_a
                                                                     const __grid_constant__ DgPtrs P, int write_dy, int k,
                                                                     const int* __restrict__ count, const int* __restrict__ list) {
   tc_dgrad_body<D, DG_FRAME, true>(a, wimg, P, 0, 0, write_dy, count, k, list);
+}
+// the chain of nnb_render_bwd_tmin on the packed stash of M rows, over its first 32 counts[C] rows (DG_PACK; the launch is sized for M)
+template <int D>
+__global__ void __launch_bounds__(N_THREADS, 1) tc_dgrad_pack(nnb_render_args a, const unsigned char* __restrict__ wimg,
+                                                              const __grid_constant__ DgPtrs P, size_t M, int write_dy, int C,
+                                                              const int* __restrict__ counts, const int* __restrict__ lists) {
+  tc_dgrad_body<D, DG_PACK, true>(a, wimg, P, M, 0, write_dy, counts, C, lists);
 }
 
 // nnb_field_vjp: the forward of explicit points with records and gate bits (FWD_VJP), then the chain on them (DG_POINTS[_OCC])
@@ -2122,6 +2287,131 @@ cudaError_t tc_frame_train_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st
   return e != cudaSuccess ? e : launch_ray_reduce(b, rayred, st);
 }
 
+// Workspace of nnb_render_fwd_tmin / nnb_render_bwd_tmin, every section 256-byte aligned: the packed stash make_layout(4 ceil(N / 4), 32 C,
+// NNB_STASH, NNB_ENGINE_TC, D) at offset 0 (C 128 ceil(N / 4) rows: every ray in every round, each round padded to the tile) | carry,
+// chunk counts [N] | lane partials [N][5][32] | checkpoints [C - 1][N] | lists [C][N] | counts [C + 1] | ray lane partials [N][9][32] |
+// the forward and the transposed weight images.
+struct StashTminWs { WsLayout L; size_t carry, chunks, part, ckpt, lists, counts, raypart, img, img_t, total; };
+template <int D> StashTminWs stash_tmin_layout(int N, int S) {
+  StashTminWs w{};
+  const int C = (S + 31) / 32;
+  const size_t n = (size_t)N;
+  w.L = make_layout((N + 3) / 4 * 4, 32 * C, NNB_STASH, NNB_ENGINE_TC, D);
+  size_t off = w.L.total;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  w.carry = take(n * 4); w.chunks = take(n * 4); w.part = take(n * 640); w.ckpt = take((size_t)(C - 1) * n * 4);
+  w.lists = take((size_t)C * n * 4); w.counts = take((size_t)(C + 1) * 4); w.raypart = take(n * 288 * 4);
+  w.img = take(Tc<D>::IMG_BYTES); w.img_t = take(Tc<D>::IMG_T_BYTES);
+  w.total = off;
+  return w;
+}
+template <int D>
+int stash_tmin_setup(cudaError_t* e) {
+  using T = Tc<D>;
+  *e = upload_stage_table<D>();
+  if (*e == cudaSuccess) *e = upload_stage_table_t<D>();
+  if (*e != cudaSuccess) return 0;
+  static bool attr = false;
+  static int n_sm = 0;
+  if (!attr) {
+    *e = cudaFuncSetAttribute(tc_stash_pack<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SM_TOTAL);
+    if (*e == cudaSuccess) *e = cudaFuncSetAttribute(tc_dgrad_pack<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::DG_TOTAL);
+    if (*e != cudaSuccess) return 0;
+    int dev = 0; cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    attr = true;
+  }
+  return n_sm;
+}
+// the training stash pointers of a layout at `base`
+inline TcStash stash_ptrs(char* base, const WsLayout& L) {
+  TcStash ts{};
+  for (int l = 0; l < 8; ++l) ts.h[l] = reinterpret_cast<float*>(base + L.h[l]);
+  ts.feat = reinterpret_cast<float*>(base + L.feat); ts.hr = reinterpret_cast<float*>(base + L.hr);
+  ts.enc = reinterpret_cast<float*>(base + L.enc); ts.denc = reinterpret_cast<float*>(base + L.denc);
+  ts.gates = reinterpret_cast<unsigned char*>(base + L.gates);
+  return ts;
+}
+
+// nnb_render_fwd_tmin: the forward weight image, then rounds k = 0 .. C - 1: frame_live_list (round k's list from the chunk counts),
+// tc_stash_pack (chunk k of the listed rays with the training stash, into the packed stash) and stash_frame_step (frame_step's compositing
+// and stop rule on the round's records); then frame_finish.  Every launch sizes itself from device counts; nothing is read back.
+template <int D>
+cudaError_t tc_render_tmin_fwd_dim(const nnb_frame_args& fa, cudaStream_t st) {
+  using T = Tc<D>;
+  const nnb_render_args& a = fa.fwd;
+  cudaError_t e;
+  const int n_sm = stash_tmin_setup<D>(&e);
+  if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32;
+  const StashTminWs w = stash_tmin_layout<D>(N, a.S);
+  char* base = static_cast<char*>(a.workspace);
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  unsigned char* img = reinterpret_cast<unsigned char*>(base + w.img);
+  tc_prep_weights<D><<<T::N_STAGES, 256, 0, st>>>(a.weights, img);
+  SampleRec* recs = reinterpret_cast<SampleRec*>(base + w.L.rec);
+  const TcStash ts = stash_ptrs(base, w.L);
+  const int tiles = (N + 3) / 4, grid = tiles < n_sm ? tiles : n_sm, warps = (N + 7) / 8;
+  int *lists = I(w.lists), *counts = I(w.counts);
+  FramePtrs f{};
+  f.t_min = fa.t_min;
+  f.carry = reinterpret_cast<float*>(base + w.carry); f.chunks = I(w.chunks); f.part = reinterpret_cast<float*>(base + w.part);
+  float* ckpt = reinterpret_cast<float*>(base + w.ckpt);
+  for (int k = 0; k < C; ++k) {
+    f.k = k; f.list = lists + (size_t)k * N; f.count = counts + k;
+    frame_live_list<<<1, 1024, 0, st>>>(f.chunks, N, k, C, lists + (size_t)k * N, counts + k);
+    tc_stash_pack<D><<<grid, N_THREADS, T::SM_TOTAL, st>>>(a, img, recs, ts, f, w.L.M);
+    stash_frame_step<<<warps, 256, 0, st>>>(a, f, recs, ckpt, C);
+  }
+  frame_finish<<<warps, 256, 0, st>>>(a, f, fa.n_eval, fa.t_final);
+  return cudaGetLastError();
+}
+
+// nnb_render_bwd_tmin: the transposed weight image; the C lists again from the chunk counts (frame_live_list); stash_chunk_adjoint (every
+// ray's compositing adjoint, padding cotangents, the row count); the data-gradient chain on the packed rows (tc_dgrad_pack); with
+// g_weights, one weight-gradient stage on those rows; stash_ray_acc, frame_ray_finish and ray_reduce.  Of what the forward wrote it reads
+// the chunk counts (clamped to 1..C), the checkpoints and the stash, so a backward without its forward gives wrong numbers, never an
+// access outside the workspace.
+template <int D>
+cudaError_t tc_render_tmin_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+  using T = Tc<D>;
+  const nnb_render_args& a = b.fwd;
+  cudaError_t e;
+  const int n_sm = stash_tmin_setup<D>(&e);
+  if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32;
+  const StashTminWs w = stash_tmin_layout<D>(N, a.S);
+  const WsLayout& L = w.L;
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  unsigned char* img_t = reinterpret_cast<unsigned char*>(base + w.img_t);
+  tc_prep_weights_t<D><<<T::N_STAGES_T, 256, 0, st>>>(a.weights, img_t);
+  const int *chunks = I(w.chunks);
+  int *lists = I(w.lists), *counts = I(w.counts);
+  for (int k = 0; k < C; ++k) frame_live_list<<<1, 1024, 0, st>>>(chunks, N, k, C, lists + (size_t)k * N, counts + k);
+  DgPtrs P{};
+  P.rec = reinterpret_cast<const SampleRec*>(base + L.rec); P.gates = reinterpret_cast<const unsigned char*>(base + L.gates);
+  P.gs = reinterpret_cast<const float4*>(base + L.gs); P.gp = reinterpret_cast<float4*>(base + L.gp); P.gv = reinterpret_cast<float4*>(base + L.gv);
+  P.dyc = reinterpret_cast<float4*>(base + L.dyc);
+  for (int l = 0; l < 8; ++l) P.dy[l] = F(L.dy[l]);
+  P.dfeat = F(L.dfeat); P.dyr = F(L.dyr);
+  FrameBwdPtrs fb{};
+  fb.rounds = C; fb.ckpt = F(w.ckpt); fb.rec = P.rec;
+  fb.gs = reinterpret_cast<float4*>(base + L.gs); fb.gp = P.gp; fb.gv = P.gv; fb.raypart = F(w.raypart);
+  const int warps = (N + 7) / 8, tiles = (int)(L.M / TILE), grid = tiles < n_sm ? tiles : n_sm;
+  stash_chunk_adjoint<<<(N + 3 * C + 7) / 8, 256, 0, st>>>(b, fb, chunks, lists, counts);
+  tc_dgrad_pack<D><<<grid, N_THREADS, T::DG_TOTAL, st>>>(a, img_t, P, L.M, b.g_weights ? 1 : 0, C, counts, lists);
+  e = cudaGetLastError();
+  if (e == cudaSuccess && b.g_weights) e = tc_wgrad_jobs(a, L, b.g_weights, false, true, st, counts + C);
+  if (e != cudaSuccess) return e;
+  stash_ray_acc<<<warps, 256, 0, st>>>(a, fb, chunks, lists, counts);
+  float* rayred = F(L.rayred);
+  frame_ray_finish<<<warps, 256, 0, st>>>(b, F(w.raypart), rayred);
+  e = cudaGetLastError();
+  return e != cudaSuccess ? e : launch_ray_reduce(b, rayred, st);
+}
+
 template <int D> size_t tc_extra_dim() { return align_up(Tc<D>::IMG_BYTES, 256) + align_up(Tc<D>::IMG_T_BYTES, 256); }
 
 }  // namespace
@@ -2204,6 +2494,15 @@ cudaError_t tc_render_frame_train_fwd_tmin(const nnb_frame_args& f, int D, cudaS
 cudaError_t tc_render_frame_train_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
   return D == 128 ? tc_frame_train_bwd_dim<128>(b, st, true)
        : (D == 64 ? tc_frame_train_bwd_dim<64>(b, st, true) : tc_frame_train_bwd_dim<256>(b, st, true));
+}
+size_t tc_render_tmin_workspace(int N, int S, int D) {
+  return D == 128 ? stash_tmin_layout<128>(N, S).total : (D == 64 ? stash_tmin_layout<64>(N, S).total : stash_tmin_layout<256>(N, S).total);
+}
+cudaError_t tc_render_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st) {
+  return D == 128 ? tc_render_tmin_fwd_dim<128>(f, st) : (D == 64 ? tc_render_tmin_fwd_dim<64>(f, st) : tc_render_tmin_fwd_dim<256>(f, st));
+}
+cudaError_t tc_render_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  return D == 128 ? tc_render_tmin_bwd_dim<128>(b, st) : (D == 64 ? tc_render_tmin_bwd_dim<64>(b, st) : tc_render_tmin_bwd_dim<256>(b, st));
 }
 // nnb_render_frame_bwd: the two halves in sequence
 cudaError_t tc_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st) {

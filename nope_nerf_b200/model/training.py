@@ -527,7 +527,12 @@ class Trainer(object):
     frame_grad_t_min (default None, needs frame_grad=True on the tensor-core pair): train with early ray termination,
     ops.frame_render_call(t): a ray stops after the first 32-sample chunk that leaves its transmittance below t, and the backward
     differentiates that truncated render, visiting only the rays that evaluated each chunk.  0.0 gives the frame_grad=True step's bits.
-    With frame_grad=False, frame_grad_engine='simt', or a negative or NaN value, it is a ValueError."""
+    With frame_grad=False, frame_grad_engine='simt', or a negative or NaN value, it is a ValueError.
+    train_t_min (default None): train with early ray termination on the per-sample stash, ops.stash_render_call(t), for every training
+    render that has a backward: each sample is evaluated once and the backward runs one weight-gradient stage on the samples evaluated,
+    in the stash path's worst-case memory (frame_grad_t_min is the choice when memory is the limit).  0.0 gives the default step's
+    forward.  With frame_grad=True, a renderer that does not resolve to the tensor-core engine, or a negative or NaN value, it is a
+    ValueError."""
 
     def __init__(self, model, optimizer, cfg, device=None, optimizer_pose=None, pose_param_net=None,
                  optimizer_focal=None, focal_net=None, optimizer_distortion=None, distortion_net=None, **kwargs):
@@ -610,10 +615,23 @@ class Trainer(object):
             if self.frame_grad_engine == 'simt':
                 raise ValueError("Trainer: frame_grad_t_min runs on the tensor-core pair only (not with frame_grad_engine='simt')")
             ops.frame_render_call(self.frame_grad_t_min)   # ValueError for a negative or NaN value
+        self.train_t_min = kwargs.get('train_t_min', None)
+        if self.train_t_min is not None:
+            if self.frame_grad:
+                raise ValueError("Trainer: train_t_min is not taken with frame_grad=True (use frame_grad_t_min)")
+            rend = model.renderer
+            engine = rend.engine if rend.engine is not None else ops.default_engine()
+            if ops.pick_engine(engine, int(rend.cfg['num_points'])) != L.ENGINE_TC:
+                raise ValueError("Trainer(train_t_min=...) needs the tensor-core engine: the renderer's engine and rendering.num_points "
+                                 "(16..1024) must resolve to it")
+            ops.stash_render_call(self.train_t_min)   # ValueError for a negative or NaN value
 
     # ------------------------------------------------------------------------------------
     def _train_render_call(self, backward):
-        """the RenderCall class of a training render: the differentiable frame's pair (frame_grad) when it has a backward"""
+        """the RenderCall class of a training render: the differentiable frame's pair (frame_grad), or the stash pair with early ray
+        termination (train_t_min), when it has a backward"""
+        if backward and self.train_t_min is not None:
+            return ops.stash_render_call(self.train_t_min)
         if not (self.frame_grad and backward):
             return ops.RenderCall
         if self.frame_grad_engine == 'simt':

@@ -92,11 +92,18 @@ class RenderCall:
     frame = False         # FrameRenderCall: the differentiable frame's training pair
     exact_frame = False   # ExactFrameRenderCall: that pair on the exact-fp32 engine
     t_min = None          # frame_render_call(t_min): that pair with early ray termination (the _tmin calls); None: without
+    stash_tmin = False    # stash_render_call(t_min): the per-sample stash pair with early ray termination (nnb_render_fwd_tmin / _bwd_tmin)
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
                  depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256):
         frame, exact = self.frame, self.exact_frame
-        if frame:
+        if self.stash_tmin:
+            if want_z_alpha:
+                raise ValueError("stash_render_call: want_z_alpha is not supported (no per-sample outputs)")
+            if pick_engine(engine, S) != L.ENGINE_TC:
+                raise ValueError("stash_render_call runs on the tensor-core engine only (16 <= S <= 1024)")
+            stash = True
+        elif frame:
             if want_z_alpha:
                 raise ValueError("FrameRenderCall: want_z_alpha is not supported (no per-sample outputs)")
             if exact:
@@ -121,7 +128,7 @@ class RenderCall:
             a.h_d, a.w_d = depth_map.shape[-2], depth_map.shape[-1]
         a.near_, a.far_ = float(near), float(far)
         engine = pick_engine(engine, S)
-        if stash and not frame:
+        if stash and not frame and not self.stash_tmin:
             flags |= L.STASH
         a.flags = flags; a.engine = engine; a.hidden_dim = int(hidden_dim)
         self.hidden_dim = int(hidden_dim)
@@ -135,6 +142,8 @@ class RenderCall:
             nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes_engine(N, S, int(hidden_dim), engine)
         elif frame:
             nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, int(hidden_dim))
+        elif self.stash_tmin:
+            nbytes = L.lib.nnb_render_tmin_workspace_bytes(N, S, int(hidden_dim))
         else:
             nbytes = L.lib.nnb_workspace_bytes_dim(N, S, flags, engine, int(hidden_dim))
         if nbytes == 0:
@@ -144,12 +153,13 @@ class RenderCall:
         self.args = a; self.N = N; self.S = S; self.stash = stash; self.pooled = True
         if exact:
             L.check(L.lib.nnb_render_frame_train_fwd_engine(C.byref(a), _stream()), "nnb_render_frame_train_fwd_engine")
-        elif frame and self.t_min is not None:
+        elif self.t_min is not None:
             f = L.FrameArgs()
             f.fwd = a
             self.n_eval = torch.empty(N, dtype=torch.int32, device=dev)
             f.t_min = self.t_min; f.n_eval = L.ptr(self.n_eval); f.t_final = None
-            L.check(L.lib.nnb_render_frame_train_fwd_tmin(C.byref(f), _stream()), "nnb_render_frame_train_fwd_tmin")
+            name = "nnb_render_fwd_tmin" if self.stash_tmin else "nnb_render_frame_train_fwd_tmin"
+            L.check(getattr(L.lib, name)(C.byref(f), _stream()), name)
         elif frame:
             L.check(L.lib.nnb_render_frame_train_fwd(C.byref(a), _stream()), "nnb_render_frame_train_fwd")
         else:
@@ -174,6 +184,8 @@ class RenderCall:
         b.g_scale_shift = L.ptr(g_scale_shift)
         if self.exact_frame:
             L.check(L.lib.nnb_render_frame_train_bwd_engine(C.byref(b), _stream()), "nnb_render_frame_train_bwd_engine")
+        elif self.stash_tmin:
+            L.check(L.lib.nnb_render_bwd_tmin(C.byref(b), _stream()), "nnb_render_bwd_tmin")
         elif self.frame and self.t_min is not None:
             L.check(L.lib.nnb_render_frame_train_bwd_tmin(C.byref(b), _stream()), "nnb_render_frame_train_bwd_tmin")
         elif self.frame:
@@ -210,6 +222,29 @@ def frame_render_call(t_min):
     if cls is None:
         cls = type("FrameRenderCall_tmin", (FrameRenderCall,), {"t_min": t, "__doc__": frame_render_call.__doc__})
         _frame_tmin_calls[t] = cls
+    return cls
+
+
+_stash_tmin_calls = {}
+
+
+def stash_render_call(t_min):
+    """the RenderCall class that trains with early ray termination on the per-sample stash at t_min (one class per value, cached), with
+    RenderCall's arguments, outputs, pooling and backward() rules.  Its forward is nnb_render_fwd_tmin, which stops each ray as
+    render_frame(t_min=...) does, evaluates each sample once with the training stash, and exposes the samples each ray evaluated as the
+    int32 [N] tensor `n_eval`; backward() is nnb_render_bwd_tmin, which runs the data-gradient chain and one weight-gradient stage on the
+    rows the forward evaluated.  Outputs and n_eval are frame_render_call(t_min)'s bits, the gradients those of the truncated render;
+    t_min = 0 gives RenderCall(stash=True)'s outputs.  Its workspace is the stash path's worst case (every ray runs every chunk), so
+    `stash` is implied and ignored.  A negative or NaN t_min is a ValueError; so are want_z_alpha and an engine that pick_engine does not
+    resolve to the tensor-core engine, raised before any other check."""
+    t = float(t_min)
+    if not t >= 0.0:
+        raise ValueError("stash_render_call: t_min must be >= 0 (got %r)" % (t_min,))
+    t = float(C.c_float(t).value)   # the value the library receives
+    cls = _stash_tmin_calls.get(t)
+    if cls is None:
+        cls = type("StashRenderCall_tmin", (RenderCall,), {"t_min": t, "stash_tmin": True, "__doc__": stash_render_call.__doc__})
+        _stash_tmin_calls[t] = cls
     return cls
 
 
