@@ -519,6 +519,28 @@ size_t nnb_render_tmin_workspace_bytes(int32_t N, int32_t S, int32_t hidden_dim)
 int nnb_render_fwd_tmin(const nnb_frame_args* f, void* stream);
 int nnb_render_bwd_tmin(const nnb_render_bwd_args* b, void* stream);
 
+/* nnb_render_fwd_tmin, nnb_render_bwd_tmin and nnb_render_tmin_workspace_bytes on fwd.engine (on `engine` for the size).  NNB_ENGINE_TC
+ * is exactly the call without the suffix (its checks, codes, bits and workspace).  NNB_ENGINE_SIMT runs the same method on the exact-fp32
+ * engine at any S from 2 to 1024, with every flag, density head, width, NDC / uniform setting, eval mode and jitter the tensor-core pair
+ * accepts.  Its packed stash holds R = min(S, 32) rows per listed ray and round, each round padded to the 64-row tile: round k's rows start
+ * at base_k, formed on the device from the rounds' counts, and row base_k + R slot + j is sample 32 k + j of the round's ray `slot`.  At
+ * S <= 32 (one round) the rows are nnb_render_fwd's, in its order: outputs and gradients are nnb_render_fwd / nnb_render_bwd's (NNB_STASH,
+ * NNB_ENGINE_SIMT) bits, and n_eval is S.  At t_min = 0 the outputs are nnb_render_fwd's at every S, and the pose, camera and scale-shift
+ * gradients are nnb_render_frame_train_bwd_engine's on NNB_ENGINE_SIMT.  The compositing adjoint takes composite_bwd's fused d L / d alpha.
+ * The data-gradient chain and one weight-gradient stage run on the packed rows, with the row count and the stage's split count read on the
+ * device (at S <= 32: nnb_render_bwd's M and splits).  No count is read back, no float atomic is used, every chunk count read is clamped to
+ * 1..C and every device count to 0..N, as on the tensor-core pair.
+ * Workspace: nnb_render_tmin_workspace_bytes_engine(N, S, hidden_dim, NNB_ENGINE_SIMT): the packed stash for every ray running every chunk
+ * (at least nnb_workspace_bytes_dim(N, S, NNB_STASH, NNB_ENGINE_SIMT, hidden_dim)), then carry, chunk counts, lane partials, checkpoints,
+ * lists, counts and ray lane partials; no weight images.  0 for N <= 0, S outside 2..1024 (16..1024 on NNB_ENGINE_TC), an unsupported
+ * width or an unknown engine.
+ * Errors, with nothing launched: NULL args (-1); an engine other than NNB_ENGINE_TC and NNB_ENGINE_SIMT (-4); then the checks and codes of
+ * nnb_render_fwd_tmin / _bwd_tmin in their order (flags, width, sizes -2, per-sample outputs -6, t_min -2, pointers -3, workspace -5).
+ * g_weights may be NULL (pose only). */
+size_t nnb_render_tmin_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine);
+int nnb_render_fwd_tmin_engine(const nnb_frame_args* f, void* stream);
+int nnb_render_bwd_tmin_engine(const nnb_render_bwd_args* b, void* stream);
+
 /* nnb_render_frame_bwd, nnb_render_frame_train_fwd and nnb_render_frame_train_bwd on fwd.engine.  NNB_ENGINE_TC is exactly the call
  * without the suffix (its checks, codes, bits and workspace).  NNB_ENGINE_SIMT runs the same method on the exact-fp32 engine at any S from
  * 2 to 1024, with a chunk stash that packs R = min(S, 32) rows per ray (row R n + j is sample 32 k + j of ray n), so a round at S < 32

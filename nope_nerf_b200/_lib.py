@@ -139,6 +139,10 @@ def _load():
     lib.nnb_render_tmin_workspace_bytes.restype = C.c_size_t
     lib.nnb_render_fwd_tmin.argtypes = [C.POINTER(FrameArgs), C.c_void_p]
     lib.nnb_render_bwd_tmin.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
+    lib.nnb_render_tmin_workspace_bytes_engine.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+    lib.nnb_render_tmin_workspace_bytes_engine.restype = C.c_size_t
+    lib.nnb_render_fwd_tmin_engine.argtypes = [C.POINTER(FrameArgs), C.c_void_p]
+    lib.nnb_render_bwd_tmin_engine.argtypes = [C.POINTER(RenderBwdArgs), C.c_void_p]
     lib.nnb_pose_fwd.argtypes = [_f, _f, _f, C.c_int32, _f, C.c_void_p]
     lib.nnb_pose_bwd.argtypes = [_f, _f, _f, C.c_int32, _f, _f, _f, C.c_void_p]
     lib.nnb_loss_rgb_depth.argtypes = [_f, _f, _f, _f, C.c_int32, _f, _f, _f, C.c_int32, C.c_float, C.c_float, C.c_int32,
@@ -182,7 +186,7 @@ EXPORTS = ["nnb_last_error", "nnb_version", "nnb_profile_events", "nnb_profile_c
            "nnb_render_frame_train_fwd", "nnb_render_frame_train_bwd", "nnb_render_frame_bwd_workspace_bytes_engine",
            "nnb_render_frame_bwd_engine", "nnb_render_frame_train_fwd_engine", "nnb_render_frame_train_bwd_engine",
            "nnb_render_frame_train_fwd_tmin", "nnb_render_frame_train_bwd_tmin", "nnb_render_tmin_workspace_bytes", "nnb_render_fwd_tmin",
-           "nnb_render_bwd_tmin"]
+           "nnb_render_bwd_tmin", "nnb_render_tmin_workspace_bytes_engine", "nnb_render_fwd_tmin_engine", "nnb_render_bwd_tmin_engine"]
 
 
 def check(rc, what):

@@ -23,6 +23,9 @@ size_t simt_render_frame_bwd_workspace(int N, int S, int D);
 cudaError_t simt_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 cudaError_t simt_render_frame_train_fwd(const nnb_render_args& a, int D, cudaStream_t st);
 cudaError_t simt_render_frame_train_bwd(const nnb_render_bwd_args& b, int D, cudaStream_t st);
+size_t simt_render_tmin_workspace(int N, int S, int D);
+cudaError_t simt_render_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st);
+cudaError_t simt_render_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st);
 #ifdef NNB_WITH_TC
 cudaError_t tc_render_fwd(const nnb_render_args& a, const WsLayout& L, cudaStream_t st);
 cudaError_t tc_render_bwd(const nnb_render_bwd_args& b, const WsLayout& L, cudaStream_t st);
@@ -696,6 +699,58 @@ int nnb_render_bwd_tmin(const nnb_render_bwd_args* b, void* stream) {
   const cudaError_t e = tc_render_bwd_tmin(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_bwd_tmin");
 #endif
+}
+// The _engine forms of the stash pair with early termination: NNB_ENGINE_TC is the call without the suffix (its checks, codes, bits and
+// workspace); NNB_ENGINE_SIMT runs the exact engine at any S from 2 to 1024 with the same checks in the same order.
+size_t nnb_render_tmin_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine) {
+  if (engine == NNB_ENGINE_TC) return nnb_render_tmin_workspace_bytes(N, S, hidden_dim);
+  const int D = hidden_of(hidden_dim);
+  if (engine == NNB_ENGINE_SIMT && N > 0 && S >= 2 && S <= 1024 && nnb::dim_supported(D)) return simt_render_tmin_workspace(N, S, D);
+  return 0;
+}
+static int check_tmin_engine(int32_t engine, const char* name) {
+  if (engine != NNB_ENGINE_TC && engine != NNB_ENGINE_SIMT)
+    return fail(-4, "%s: engine %d has no stash render with early termination (NNB_ENGINE_TC or NNB_ENGINE_SIMT)", name, engine);
+#ifndef NNB_WITH_TC
+  if (engine == NNB_ENGINE_TC) return fail(-4, "library built without the tensor-core engine");
+#endif
+  return 0;
+}
+static int check_tmin_ws_engine(const nnb_render_args* a) {
+  const size_t need = nnb_render_tmin_workspace_bytes_engine(a->N, a->S, a->hidden_dim, a->engine);
+  if (!a->workspace || a->workspace_bytes < need) return fail(-5, "workspace too small: have %zu need %zu", a->workspace_bytes, need);
+  if ((reinterpret_cast<uintptr_t>(a->workspace) & 255) != 0) return fail(-5, "workspace must be 256-byte aligned");
+  return 0;
+}
+int nnb_render_fwd_tmin_engine(const nnb_frame_args* f, void* stream) {
+  if (!f) return fail(-1, "null args");
+  const nnb_render_args* a = &f->fwd;
+  if (int rc = check_tmin_engine(a->engine, "nnb_render_fwd_tmin_engine")) return rc;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) return nnb_render_fwd_tmin(f, stream);
+#endif
+  if (int rc = check_frame(a, true)) return rc;
+  if (!(f->t_min >= 0.f)) return fail(-2, "nnb_render_fwd_tmin_engine: t_min must be >= 0 (got %g)", (double)f->t_min);
+  if (int rc = check_frame_io(a)) return rc;
+  if (misaligned4(f->n_eval) || misaligned4(f->t_final))
+    return fail(-3, "nnb_render_fwd_tmin_engine: n_eval and t_final must be 4-byte aligned");
+  if (int rc = check_tmin_ws_engine(a)) return rc;
+  const cudaError_t e = simt_render_fwd_tmin(*f, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_fwd_tmin_engine");
+}
+int nnb_render_bwd_tmin_engine(const nnb_render_bwd_args* b, void* stream) {
+  if (!b) return fail(-1, "null args");
+  const nnb_render_args* a = &b->fwd;
+  if (int rc = check_tmin_engine(a->engine, "nnb_render_bwd_tmin_engine")) return rc;
+#ifdef NNB_WITH_TC
+  if (a->engine == NNB_ENGINE_TC) return nnb_render_bwd_tmin(b, stream);
+#endif
+  if (int rc = check_frame(a, true)) return rc;
+  if (int rc = check_frame_io(a)) return rc;
+  if (!b->g_rgb || !b->g_c2w) return fail(-3, "nnb_render_bwd_tmin_engine: g_rgb and g_c2w must be non-null");
+  if (int rc = check_tmin_ws_engine(a)) return rc;
+  const cudaError_t e = simt_render_bwd_tmin(*b, hidden_of(a->hidden_dim), (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : cuda_fail(e, "nnb_render_bwd_tmin_engine");
 }
 size_t nnb_render_frame_bwd_workspace_bytes_engine(int32_t N, int32_t S, int32_t hidden_dim, int32_t engine) {
   if (engine == NNB_ENGINE_TC) return nnb_render_frame_bwd_workspace_bytes(N, S, hidden_dim);

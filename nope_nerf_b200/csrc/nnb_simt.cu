@@ -158,7 +158,9 @@ __device__ __forceinline__ void row_geometry(const nnb_render_args& a, size_t m,
 // ray-chunks in turn through frame_step (nnb_frame.cuh).  fr / n_live: the round and its ray-chunk count.
 // SF_CHUNK (simt_frame_stash, nnb_render_frame_bwd on this engine): SF_RAYS with the stash and records on the rows of chunk fr.k of every
 // ray (chunk_row); geometry, view direction and the record's z come from the row's sample, stores go to the row.
-enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2, SF_FRAME = 3, SF_CHUNK = 4 };
+// SF_PACK (simt_stash_pack, nnb_render_fwd_tmin_engine on this engine): SF_CHUNK on the rows of round fr.k's list (pack_row), n_live of
+// them; the caller offsets P to the round's first row of the packed stash.
+enum : int { SF_RAYS = 0, SF_MARCH = 1, SF_SECANT = 2, SF_FRAME = 3, SF_CHUNK = 4, SF_PACK = 5 };
 
 // Row `row` of frame tile `tile`: a ray-chunk is R = min(S, 32) rows and a tile holds 64 / R of them, so row r is sample 32 fr.k + r % R
 // of the ray in slot (64 / R) tile + r / R of the round.  Slots past the round's last repeat it, rows past a ray's last sample evaluate
@@ -180,6 +182,38 @@ __device__ __forceinline__ size_t chunk_row(const nnb_render_args& a, int k, siz
   return (m / R) * a.S + min(32 * k + (int)(m % R), a.S - 1);
 }
 
+// ---- the packed stash of nnb_render_fwd_tmin_engine / nnb_render_bwd_tmin_engine on this engine ------------------------------------
+// Round k evaluates chunk k of the rays lists[k] ([C][N], increasing n, frame_live_list) with counts[k] of them.  Its rows start at
+// base_k = sum over j < k of 64 ceil(R count_j / 64) (R = min(S, 32); each round padded to the 64-row tile), and row base_k + R slot + j is
+// sample 32 k + j of ray lists[k][slot].  At S <= 32 there is one round and row n S + j is nnb_render_fwd's row.  Counts are clamped to
+// 0..N where they are read, so every row stays below the stash's C 64 ceil(R N / 64) rows.
+__device__ __forceinline__ size_t pack_round_base(const int* counts, int k, int N, int R) {
+  size_t r = 0;
+  for (int j = 0; j < k; ++j) r += (size_t)TM * ((R * frame_live_count(counts + j, N) + TM - 1) / TM);
+  return r;
+}
+// sample row n S + i (nnb_render_fwd's order) of row m of round fr.k (n_live >= 1 rays): slots past the list's last repeat it
+__device__ __forceinline__ size_t pack_row(const nnb_render_args& a, const FramePtrs& fr, size_t m, int n_live) {
+  const int R = min(a.S, 32);
+  const int slot = min((int)(m / R), n_live - 1);
+  return (size_t)fr.list[slot] * a.S + min(32 * fr.k + (int)(m % R), a.S - 1);
+}
+// sample row of packed row m: the round whose rows hold m (the last round past them), the slot's ray (padding rows take the list's last
+// ray; their cotangent is zero)
+__device__ __forceinline__ size_t pack_row_sample(const nnb_render_args& a, const int* lists, const int* counts, int C, size_t m) {
+  const int R = min(a.S, 32);
+  size_t r = 0;
+  int k = 0;
+  for (; k < C - 1; ++k) {
+    const size_t rows = (size_t)TM * ((R * frame_live_count(counts + k, a.N) + TM - 1) / TM);
+    if (m < r + rows) break;
+    r += rows;
+  }
+  const int slot = min((int)((m - r) / R), max(frame_live_count(counts + k, a.N) - 1, 0));
+  const int n = min(max(lists[(size_t)k * a.N + slot], 0), a.N - 1);
+  return (size_t)n * a.S + min(32 * k + (int)((m - r) % R), a.S - 1);
+}
+
 // one 64-row tile of the exact forward: rows m0 = 64 tile .. m0 + 63 of M
 template <int D, int MODE>
 __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int stash, unsigned tile, const MarchPtrs& q,
@@ -191,7 +225,8 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
   const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
   auto row_m = [&](int row) {
-    return MODE == SF_FRAME ? frame_row(a, fr, tile, row, n_live) : MODE == SF_CHUNK ? chunk_row(a, fr.k, m0 + row) : m0 + row;
+    return MODE == SF_FRAME ? frame_row(a, fr, tile, row, n_live) : MODE == SF_CHUNK ? chunk_row(a, fr.k, m0 + row)
+         : MODE == SF_PACK ? pack_row(a, fr, m0 + row, n_live) : m0 + row;
   };
   {  // prologue: encode positions into columns D..D+63 of both buffers
     int row = tid & 63, part = tid >> 6;
@@ -223,7 +258,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
     }
   }
   __syncthreads();
-  if ((MODE == SF_RAYS || MODE == SF_CHUNK) && stash) {
+  if ((MODE == SF_RAYS || MODE == SF_CHUNK || MODE == SF_PACK) && stash) {
     for (int idx = tid; idx < TM * 16; idx += 256) {
       int row = idx >> 4, c4 = idx & 15;
       *reinterpret_cast<float4*>(P.enc + (m0 + row) * 64 + c4 * 4) = *reinterpret_cast<const float4*>(buf0 + row * LDB + D + c4 * 4);
@@ -236,7 +271,7 @@ __device__ __forceinline__ void simt_fwd_tile(const nnb_render_args& a, const Si
     int kvalid = (l == 0) ? 63 : (l == 4 ? D + 63 : D);
     tile_gemm<NJ, false, 1, false>(in, LDB, K, w + nnb::w_off(D, l), nnb::w_ld(D, l), D, kvalid, w + nnb::b_off(D, l), oth, LDB, Ws);
     __syncthreads();
-    if ((MODE == SF_RAYS || MODE == SF_CHUNK) && stash) tile_to_global(oth, LDB, P.h[l], m0, D);
+    if ((MODE == SF_RAYS || MODE == SF_CHUNK || MODE == SF_PACK) && stash) tile_to_global(oth, LDB, P.h[l], m0, D);
     float* t_ = cur; cur = oth; oth = t_;
   }
   // cur = h8.  density head: 4 threads per row
@@ -379,6 +414,19 @@ __global__ void __launch_bounds__(256, 1) simt_frame_stash(nnb_render_args a, Si
   simt_fwd_tile<D, SF_CHUNK>(a, P, (size_t)a.N * a.S, 1, blockIdx.x, MarchPtrs{}, 0, 0, nullptr, f);
 }
 
+// one forward round of nnb_render_fwd_tmin_engine on this engine: chunk f.k of the f.count rays of f.list, records and the training stash
+// of its R count rows (SF_PACK) into the packed stash from row base_k on, one 64-row tile per CTA.  The count is read when the kernel
+// starts; a CTA past the round's rows exits before any barrier.
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_stash_pack(nnb_render_args a, SimtPtrs P, const __grid_constant__ FramePtrs f) {
+  const int R = min(a.S, 32), n_live = frame_live_count(f.count, a.N);
+  if ((int)blockIdx.x * TM >= R * n_live) return;
+  const size_t mo = pack_round_base(f.count - f.k, f.k, a.N, R);
+  P.rec += mo; P.feat += mo * D; P.hr += mo * (D / 2); P.enc += mo * 64; P.denc += mo * 32;
+  for (int l = 0; l < 8; ++l) P.h[l] += mo * D;
+  simt_fwd_tile<D, SF_PACK>(a, P, (size_t)a.N * a.S, 1, blockIdx.x, MarchPtrs{}, 0, 0, nullptr, f, n_live);
+}
+
 // ---------------------------------------------------------------------------------------
 // compositing (rendering.py:122-158), one warp per ray; shared by both engines
 // ---------------------------------------------------------------------------------------
@@ -476,18 +524,133 @@ __global__ void composite_bwd(nnb_render_bwd_args b, const SampleRec* recs, floa
   }
 }
 
+// The per-ray kernels of nnb_render_fwd_tmin_engine / nnb_render_bwd_tmin_engine on the packed stash.  They are the statements of the
+// tensor-core pair's stash_frame_step, stash_chunk_adjoint and stash_ray_acc (nnb_tc.cu) on this engine's rows (R = min(S, 32) rows per
+// slot, rounds padded to 64 rows), copied rather than shared so that those kernels keep their SASS; the adjoint takes composite_bwd's fused
+// d L / d alpha (composite_chunk_bwd<true>), as the exact frame pair does, so that at S <= 32 the gradients are nnb_render_bwd's bits.
+
+// back end of forward round f.k: one warp per slot, frame_step's arithmetic on the round's records, from the ray's carry and lane partials
+// of the rounds before.  Lane 0 stores the carry, its checkpoint ckpt[k][n] and c_n: k + 1 when the ray stops, C while it stays live.
+__global__ void simt_pack_step(nnb_render_args a, const __grid_constant__ FramePtrs f, const SampleRec* __restrict__ rec,
+                               float* __restrict__ ckpt, int C) {
+  const int lane = threadIdx.x & 31, slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (slot >= frame_live_count(f.count, a.N)) return;
+  const int n = f.list[slot], R = min(a.S, 32);
+  const int i = 32 * f.k + lane;
+  const bool valid = i < a.S;   // implies lane < R
+  float4 me = make_float4(0.f, 0.f, 0.f, 0.f);
+  float z = 0.f, alpha = 0.f;
+  if (valid) {
+    const SampleRec r = rec[pack_round_base(f.count - f.k, f.k, a.N, R) + (size_t)slot * R + lane];
+    me = make_float4(r.r, r.g, r.b, r.a);
+    z = sample_z(a, n, i);
+    alpha = composite_alpha(a, i, me.w, z, [&] { return sample_z(a, n, i + 1); });
+  }
+  float* part = f.part + (size_t)n * 160 + lane;
+  float carry = 1.f, C0 = 0.f, C1 = 0.f, C2 = 0.f, Dist = 0.f, acc = 0.f;
+  if (f.k > 0) { carry = f.carry[n]; C0 = part[0]; C1 = part[32]; C2 = part[64]; Dist = part[96]; acc = part[128]; }
+  composite_chunk(alpha, valid, me.x, me.y, me.z, z, lane, carry, C0, C1, C2, Dist, acc);
+  part[0] = C0; part[32] = C1; part[64] = C2; part[96] = Dist; part[128] = acc;
+  if (lane == 0) {
+    f.carry[n] = carry;
+    if (f.k + 1 < C) ckpt[(size_t)f.k * a.N + n] = carry;
+    f.chunks[n] = carry < f.t_min || 32 * (f.k + 1) >= a.S ? f.k + 1 : C;
+  }
+}
+
+// slot of ray n in a round's list (increasing n): the first slot whose ray is not below n, clamped to the list
+__device__ __forceinline__ int pack_slot(const int* list, int count, int n) {
+  int lo = 0, hi = count;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (list[mid] < n) lo = mid + 1; else hi = mid;
+  }
+  return min(lo, max(count - 1, 0));
+}
+
+// Compositing adjoint of the packed stash, one warp per ray: chunks c_n - 1 .. 0, the suffix carry starting at 0 in the ray's last chunk.
+// Lanes past a ray's R rows (S < 32 only) have no row and write nothing.  Warps N .. N + 2 C - 1 zero the cotangents of round
+// (w - N) / 2's padding rows base_k + R count_k .. base_k+1 - 1 (fewer than 64).  Thread 0 stores counts[C] = base_C-1 + R count_C-1, the
+// rows of the weight-gradient stage (N S at S <= 32).
+__global__ void simt_pack_adjoint(nnb_render_bwd_args b, const __grid_constant__ FrameBwdPtrs f, const int* __restrict__ chunks,
+                                  const int* __restrict__ lists, int* __restrict__ counts) {
+  const nnb_render_args& a = b.fwd;
+  const int C = f.rounds, R = min(a.S, 32);
+  const int lane = threadIdx.x & 31, w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w == 0 && lane == 0)
+    counts[C] = (int)(pack_round_base(counts, C - 1, a.N, R) + (size_t)R * frame_live_count(counts + C - 1, a.N));
+  if (w >= a.N) {
+    const int k = (w - a.N) / 2;
+    if (k >= C) return;
+    const int rows = R * frame_live_count(counts + k, a.N), r = rows + 32 * ((w - a.N) % 2) + lane;
+    if (r < (rows + TM - 1) / TM * TM) f.gs[pack_round_base(counts, k, a.N, R) + r] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  const int n = w;
+  Ray ray; setup_ray(a, n, ray);
+  float gD = b.g_depth_pred ? __ldg(b.g_depth_pred + n) : 0.f;
+  if ((a.flags & NNB_EVAL) && (a.flags & NNB_NORMALISE)) gD = gD / ray.nrm;
+  const float gC0 = __ldg(b.g_rgb + 3 * n), gC1 = __ldg(b.g_rgb + 3 * n + 1), gC2 = __ldg(b.g_rgb + 3 * n + 2);
+  const float gsum = (a.flags & NNB_WHITE_BG) ? (gC0 + gC1 + gC2) : 0.f;
+  float carry_s = 0.f;
+  for (int k = frame_ray_chunks(chunks, n, C) - 1; k >= 0; --k) {
+    const int slot = pack_slot(lists + (size_t)k * a.N, frame_live_count(counts + k, a.N), n);
+    const size_t m = pack_round_base(counts, k, a.N, R) + (size_t)slot * R + lane;
+    const int i = 32 * k + lane;
+    const bool valid = i < a.S;
+    const SampleRec me = valid ? f.rec[m] : SampleRec{0, 0, 0, 0, 0, 0, 0, 0};
+    float alpha = 0.f, df = 1.f;   // df = d alpha / d a
+    if (valid) {
+      alpha = composite_alpha(a, i, me.a, me.z, [&] { return sample_z(a, n, i + 1); });
+      if (a.flags & NNB_DIST_ALPHA) {
+        if (i >= a.S - 1) df = 0.f;
+        else { const float delta = __fsub_rn(sample_z(a, n, i + 1), me.z); df = delta * expf(-me.a * delta); }
+      }
+    }
+    const float carry = k > 0 ? f.ckpt[(size_t)(k - 1) * a.N + n] : 1.f;
+    const float4 g = composite_chunk_bwd<true>(alpha, valid, me.r, me.g, me.b, me.z, df, lane, carry, gC0, gC1, gC2, gD, gsum, carry_s);
+    if (lane < R) f.gs[m] = g;
+  }
+}
+
+// ray_bwd's lane sums on the packed stash, one warp per ray: the terms of chunks c_n - 1 .. 0 added in that order (frame_ray_acc<true>'s)
+// to lane partials that start at 0, stored once for frame_ray_finish
+__global__ void simt_pack_ray_acc(nnb_render_args a, const __grid_constant__ FrameBwdPtrs f, const int* __restrict__ chunks,
+                                  const int* __restrict__ lists, const int* __restrict__ counts) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= a.N) return;
+  const int R = min(a.S, 32);
+  float v[9];
+#pragma unroll
+  for (int c = 0; c < 9; ++c) v[c] = 0.f;
+  for (int k = frame_ray_chunks(chunks, n, f.rounds) - 1; k >= 0; --k) {
+    if (32 * k + lane >= a.S) continue;   // implies lane < R
+    const int slot = pack_slot(lists + (size_t)k * a.N, frame_live_count(counts + k, a.N), n);
+    const size_t m = pack_round_base(counts, k, a.N, R) + (size_t)slot * R + lane;
+    const float4 g = f.gp[m], dv = f.gv[m];
+    const float z = f.rec[m].z;
+    v[0] += g.x; v[1] += g.y; v[2] += g.z;
+    v[3] += z * g.x; v[4] += z * g.y; v[5] += z * g.z;
+    v[6] += dv.x; v[7] += dv.y; v[8] += dv.z;
+  }
+  float* part = f.raypart + (size_t)n * 288 + lane;
+#pragma unroll
+  for (int c = 0; c < 9; ++c) part[32 * c] = v[c];
+}
+
 // ---------------------------------------------------------------------------------------
 // B2: data-gradient chain
 // ---------------------------------------------------------------------------------------
 // MODE of simt_dgrad_tile: DG_ROWS (simt_mlp_dgrad): row m is sample m.  DG_CHUNK (simt_dgrad_chunk, nnb_render_frame_bwd on this engine):
 // the rows of chunk `chunk`'s stash as simt_frame_stash wrote them: row_geometry and row_view_dir take the row's sample chunk_row(a,
-// chunk, m), everything else the row.
-enum : int { DG_ROWS = 0, DG_CHUNK = 1 };
+// chunk, m), everything else the row.  DG_PACK (simt_dgrad_pack, nnb_render_bwd_tmin_engine on this engine): the rows of the packed stash,
+// whose samples are pack_row_sample(a, lists, counts, chunk, m) (chunk = C).
+enum : int { DG_ROWS = 0, DG_CHUNK = 1, DG_PACK = 2 };
 
 // one 64-row tile of the chain: rows m0 = 64 tile .. m0 + 63 of M
 template <int D, int MODE = DG_ROWS>
 __device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const SimtPtrs& P, size_t M, int write_dy, unsigned tile,
-                                                int chunk = 0) {
+                                                int chunk = 0, const int* lists = nullptr, const int* counts = nullptr) {
   constexpr int LDB = ldb<D>(), NJ = D / 64, DR = D / 2;
   extern __shared__ __align__(16) float smem[];
   float* bufA = smem; float* bufB = bufA + TM * LDB; float* Ws = bufB + TM * LDB;
@@ -497,8 +660,11 @@ __device__ __forceinline__ void simt_dgrad_tile(const nnb_render_args& a, const 
   const size_t m0 = (size_t)tile * TM;
   const float* w = a.weights;
   // the row's sample for the geometry (DG_CHUNK: M counts the chunk's rows, the samples are the N S of the render)
-  auto row_s = [&](int row) { return MODE == DG_CHUNK ? chunk_row(a, chunk, m0 + row) : m0 + row; };
-  const size_t MS = MODE == DG_CHUNK ? (size_t)a.N * a.S : M;
+  auto row_s = [&](int row) {
+    return MODE == DG_CHUNK ? chunk_row(a, chunk, m0 + row)
+         : MODE == DG_PACK ? pack_row_sample(a, lists, counts, chunk, m0 + row) : m0 + row;
+  };
+  const size_t MS = MODE == DG_CHUNK || MODE == DG_PACK ? (size_t)a.N * a.S : M;
   {  // 1. head adjoints
     int row = tid >> 2, c = tid & 3; size_t m = m0 + row;
     float4 g = (m < M) ? P.gs[m] : make_float4(0, 0, 0, 0);
@@ -582,6 +748,16 @@ __global__ void __launch_bounds__(256, 1) simt_mlp_dgrad(nnb_render_args a, Simt
 template <int D>
 __global__ void __launch_bounds__(256, 1) simt_dgrad_chunk(nnb_render_args a, SimtPtrs P, size_t M, int write_dy, int k) {
   simt_dgrad_tile<D, DG_CHUNK>(a, P, M, write_dy, blockIdx.x, k);
+}
+
+// the chain of nnb_render_bwd_tmin_engine on this engine on the packed stash of cap rows, over its first counts[C] rows (clamped to
+// 0..cap), read when the kernel starts; a CTA past them exits before any barrier
+template <int D>
+__global__ void __launch_bounds__(256, 1) simt_dgrad_pack(nnb_render_args a, SimtPtrs P, size_t cap, int write_dy, int C,
+                                                          const int* __restrict__ counts, const int* __restrict__ lists) {
+  const size_t M = min((size_t)max(counts[C], 0), cap);
+  if ((size_t)blockIdx.x * TM >= M) return;
+  simt_dgrad_tile<D, DG_PACK>(a, P, M, write_dy, blockIdx.x, C, lists, counts);
 }
 
 // Device-count form of simt_mlp_dgrad (the normals of nnb_geometry_frame on this engine), rows as in simt_mlp_fwd_n: the chain on the
@@ -716,7 +892,7 @@ struct WJob {
 struct WJobs { WJob j[16]; int njobs; };
 
 // split blockIdx.y of job j writes its partial dW / db to part (layout of RedJob; wgrad_reduce sums the splits in order)
-__global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int msplit, float* part) {
+__device__ __forceinline__ void simt_wgrad_body(const WJobs& jobs, size_t M, int msplit, float* part) {
   __shared__ __align__(16) float Ys[16][64];
   __shared__ __align__(16) float Xs[16][64];
   int ji = 0;
@@ -763,6 +939,14 @@ __global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int mspl
     if (tk == 0 && ki == 0) pp[(size_t)J.Nn * J.Kk + n] = bs[r];
   }
   if (blockIdx.x == gridDim.x - 1 && blockIdx.y == gridDim.y - 1) pdl_wait();   // chained launch: see tc_wgrad_all
+}
+__global__ void __launch_bounds__(256) simt_wgrad(WJobs jobs, size_t M, int msplit, float* part) { simt_wgrad_body(jobs, M, msplit, part); }
+// simt_wgrad on the first *mrows rows (clamped to 0..cap), read on the device, at simt_wgrad_msplit of that count (at most the launch's
+// gridDim.y splits): the splits past it store zeros, so at *mrows = M the partials are simt_wgrad's at M
+__global__ void __launch_bounds__(256) simt_wgrad_live(WJobs jobs, size_t cap, float* part, const int* __restrict__ mrows) {
+  const size_t M = min((size_t)max(*mrows, 0), cap);
+  const int msplit = min(max((int)((M + 4095) / 4096), 1), min((int)gridDim.y, 16));
+  simt_wgrad_body(jobs, M, msplit, part);
 }
 
 // The head jobs of the TC engine's weight-gradient stage (fc_density, fc_rgb: 1 and 3 rows of dW; the direction slice of
@@ -1055,6 +1239,8 @@ static cudaError_t simt_init_dim() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_frame<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_frame_stash<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
     if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_dgrad_chunk<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_stash_pack<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(simt_dgrad_pack<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem<D>());
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -1106,8 +1292,8 @@ cudaError_t simt_field_fwd(const nnb_render_args& a, const WsLayout& L, float* o
   return cudaGetLastError();
 }
 
-cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cudaStream_t st);
-cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st);
+cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cudaStream_t st, const int* mrows = nullptr);
+cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st, const int* mrows = nullptr);
 
 // nnb_field_hvp: forward with stash, data-gradient chain for a cotangent 1 on the logit (dy stash), tangent chain + point term, then
 // the weight-gradient jobs d s' / d W_l = sum_m dy_l[m] (x) x'_{l-1}[m] and d s' / d w_sigma = sum_m h'7[m] (no bias jobs).
@@ -1382,9 +1568,98 @@ cudaError_t simt_render_frame_bwd(const nnb_render_bwd_args& b, int D, cudaStrea
   return e != cudaSuccess ? e : simt_render_frame_train_bwd(b, D, st);
 }
 
+// ---- nnb_render_fwd_tmin_engine / nnb_render_bwd_tmin_engine on this engine: the tensor-core pair's rounds (tc_render_tmin_fwd_dim /
+// _bwd_dim) with the exact kernels, on the packed stash of pack_round_base.  Workspace, every section 256-byte aligned: the packed stash
+// make_layout(C 64 ceil(R N / 64), 1, NNB_STASH, NNB_ENGINE_SIMT, D) at offset 0 (every ray in every round) | carry, chunk counts [N] |
+// lane partials [N][5][32] | checkpoints [C - 1][N] | lists [C][N] | counts [C + 1] | ray lane partials [N][9][32].  No weight images:
+// the exact kernels read the fp32 weights.
+struct PackWs { WsLayout L; size_t carry, chunks, part, ckpt, lists, counts, raypart, total; };
+static PackWs simt_pack_layout(int N, int S, int D) {
+  PackWs w{};
+  const int C = (S + 31) / 32, R = S < 32 ? S : 32;
+  const size_t n = (size_t)N;
+  w.L = make_layout((int)((size_t)C * TM * (((size_t)R * n + TM - 1) / TM)), 1, NNB_STASH, NNB_ENGINE_SIMT, D);
+  size_t off = w.L.total;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align_up(bytes, 256); return o; };
+  w.carry = take(n * 4); w.chunks = take(n * 4); w.part = take(n * 640); w.ckpt = take((size_t)(C - 1) * n * 4);
+  w.lists = take((size_t)C * n * 4); w.counts = take((size_t)(C + 1) * 4); w.raypart = take(n * 288 * 4);
+  w.total = off;
+  return w;
+}
+size_t simt_render_tmin_workspace(int N, int S, int D) { return simt_pack_layout(N, S, D).total; }
+
+// the forward: rounds k = 0 .. C - 1 of frame_live_list (round k's list from the chunk counts), simt_stash_pack (chunk k of the listed rays
+// with the training stash) and simt_pack_step (frame_step's compositing and stop rule); then frame_finish.  Every launch after the first
+// sizes itself from device counts; nothing is read back.
+template <int D>
+static cudaError_t simt_tmin_fwd_dim(const nnb_frame_args& fa, cudaStream_t st) {
+  const nnb_render_args& a = fa.fwd;
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32, R = a.S < 32 ? a.S : 32;
+  const PackWs w = simt_pack_layout(N, a.S, D);
+  char* base = static_cast<char*>(a.workspace);
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  const SimtPtrs P = make_ptrs(w.L, base);
+  int *lists = I(w.lists), *counts = I(w.counts);
+  FramePtrs f{};
+  f.t_min = fa.t_min;
+  f.carry = reinterpret_cast<float*>(base + w.carry); f.chunks = I(w.chunks); f.part = reinterpret_cast<float*>(base + w.part);
+  float* ckpt = reinterpret_cast<float*>(base + w.ckpt);
+  const int tiles = (R * N + TM - 1) / TM, warps = (N + 7) / 8;
+  for (int k = 0; k < C; ++k) {
+    f.k = k; f.list = lists + (size_t)k * N; f.count = counts + k;
+    frame_live_list<<<1, 1024, 0, st>>>(f.chunks, N, k, C, lists + (size_t)k * N, counts + k);
+    simt_stash_pack<D><<<tiles, 256, fwd_smem<D>(), st>>>(a, P, f);
+    simt_pack_step<<<warps, 256, 0, st>>>(a, f, P.rec, ckpt, C);
+  }
+  frame_finish<<<warps, 256, 0, st>>>(a, f, fa.n_eval, fa.t_final);
+  return cudaGetLastError();
+}
+
+// the backward: the C lists again from the chunk counts (clamped to 1..C); simt_pack_adjoint (every ray's compositing adjoint, padding
+// cotangents, the row count); simt_dgrad_pack on those rows; with g_weights, one weight-gradient stage on them (simt_wgrad_live, the
+// jobs of simt_wgrad_all); simt_pack_ray_acc, frame_ray_finish and ray_reduce.  Of what the forward wrote it reads the chunk counts, the
+// checkpoints and the stash, so a backward without its forward gives wrong numbers, never an access outside the workspace.
+template <int D>
+static cudaError_t simt_tmin_bwd_dim(const nnb_render_bwd_args& b, cudaStream_t st) {
+  const nnb_render_args& a = b.fwd;
+  cudaError_t e = simt_init();
+  if (e != cudaSuccess) return e;
+  const int N = a.N, C = (a.S + 31) / 32;
+  const PackWs w = simt_pack_layout(N, a.S, D);
+  const WsLayout& L = w.L;
+  char* base = static_cast<char*>(a.workspace);
+  auto F = [&](size_t off) { return reinterpret_cast<float*>(base + off); };
+  auto I = [&](size_t off) { return reinterpret_cast<int*>(base + off); };
+  const SimtPtrs P = make_ptrs(L, base);
+  const int* chunks = I(w.chunks);
+  int *lists = I(w.lists), *counts = I(w.counts);
+  for (int k = 0; k < C; ++k) frame_live_list<<<1, 1024, 0, st>>>(chunks, N, k, C, lists + (size_t)k * N, counts + k);
+  FrameBwdPtrs fb{};
+  fb.rounds = C; fb.ckpt = F(w.ckpt); fb.rec = P.rec; fb.gs = P.gs; fb.gp = P.gp; fb.gv = P.gv; fb.raypart = F(w.raypart);
+  const int warps = (N + 7) / 8;
+  simt_pack_adjoint<<<(N + 2 * C + 7) / 8, 256, 0, st>>>(b, fb, chunks, lists, counts);
+  simt_dgrad_pack<D><<<(unsigned)(L.M / TM), 256, bwd_smem<D>(), st>>>(a, P, L.M, b.g_weights ? 1 : 0, C, counts, lists);
+  e = cudaGetLastError();
+  if (e == cudaSuccess && b.g_weights) e = simt_wgrad_all(P, L, b.g_weights, st, counts + C);
+  if (e != cudaSuccess) return e;
+  simt_pack_ray_acc<<<warps, 256, 0, st>>>(a, fb, chunks, lists, counts);
+  frame_ray_finish<<<warps, 256, 0, st>>>(b, F(w.raypart), P.rayred);
+  ray_reduce<<<1, 512, 0, st>>>(b, P.rayred);
+  return cudaGetLastError();
+}
+cudaError_t simt_render_fwd_tmin(const nnb_frame_args& f, int D, cudaStream_t st) {
+  return D == 128 ? simt_tmin_fwd_dim<128>(f, st) : (D == 64 ? simt_tmin_fwd_dim<64>(f, st) : simt_tmin_fwd_dim<256>(f, st));
+}
+cudaError_t simt_render_bwd_tmin(const nnb_render_bwd_args& b, int D, cudaStream_t st) {
+  return D == 128 ? simt_tmin_bwd_dim<128>(b, st) : (D == 64 ? simt_tmin_bwd_dim<64>(b, st) : simt_tmin_bwd_dim<256>(b, st));
+}
+
 // jobs -> simt_wgrad into part[off ..]; R[i] receives job i's reduction (launch_wgrad_reduce).  chained: programmatic dependent
-// launch behind the previous grid on the stream (see tc_wgrad_all)
-cudaError_t launch_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, size_t off, RedJob* R, bool chained, cudaStream_t st) {
+// launch behind the previous grid on the stream (see tc_wgrad_all).  mrows (not NULL): simt_wgrad_live on the first *mrows of M rows
+cudaError_t launch_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, size_t off, RedJob* R, bool chained, cudaStream_t st,
+                              const int* mrows = nullptr) {
   int tiles = 0;
   for (int i = 0; i < J.njobs; ++i) {
     WJob& j = J.j[i];
@@ -1401,14 +1676,15 @@ cudaError_t launch_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(tiles, msplit); cfg.blockDim = dim3(256); cfg.stream = st;
   cfg.attrs = &at; cfg.numAttrs = chained ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, simt_wgrad, J, M, msplit, part);
+  cudaError_t e = mrows ? cudaLaunchKernelEx(&cfg, simt_wgrad_live, J, M, part, mrows)
+                        : cudaLaunchKernelEx(&cfg, simt_wgrad, J, M, msplit, part);
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 // jobs -> simt_wgrad into the partial buffer, then wgrad_reduce into dW / db
-cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st) {
+cudaError_t run_simt_wgrad(WJobs& J, size_t M, int D, int msplit, float* part, cudaStream_t st, const int* mrows) {
   RedJob R[16];
-  cudaError_t e = launch_simt_wgrad(J, M, D, msplit, part, 0, R, false, st);
+  cudaError_t e = launch_simt_wgrad(J, M, D, msplit, part, 0, R, false, st, mrows);
   if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(R, J.njobs, part, st);
 }
@@ -1460,7 +1736,8 @@ cudaError_t launch_composite_fwd(const nnb_render_args& a, const SampleRec* recs
   return cudaGetLastError();
 }
 
-cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cudaStream_t st) {
+// mrows (not NULL): every job on the first *mrows of L.M rows, read on the device (simt_wgrad_live)
+cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cudaStream_t st, const int* mrows) {
   {
     WJobs J{}; int nj = 0;
     auto add = [&](const float* dY, int ldy, int Nn, const float* X, int ldx, int Kk, float* dW, int ldw, float* db) {
@@ -1479,7 +1756,7 @@ cudaError_t simt_wgrad_all(const SimtPtrs& P, const WsLayout& L, float* gw, cuda
     add(P.dyr, DR, DR, P.denc, 32, 27, gw + nnb::W_RGBH(D) + D, D + 27, nullptr);
     add(reinterpret_cast<const float*>(P.dyc), 4, 3, P.hr, DR, DR, gw + nnb::W_RGB(D), DR, gw + nnb::B_RGB(D));
     J.njobs = nj;
-    return run_simt_wgrad(J, L.M, D, simt_wgrad_msplit(L.M), P.wpart, st);
+    return run_simt_wgrad(J, L.M, D, simt_wgrad_msplit(L.M), P.wpart, st, mrows);
   }
 }
 

@@ -532,7 +532,11 @@ class Trainer(object):
     render that has a backward: each sample is evaluated once and the backward runs one weight-gradient stage on the samples evaluated,
     in the stash path's worst-case memory (frame_grad_t_min is the choice when memory is the limit).  0.0 gives the default step's
     forward.  With frame_grad=True, a renderer that does not resolve to the tensor-core engine, or a negative or NaN value, it is a
-    ValueError."""
+    ValueError.
+    train_t_min_engine (default None, needs train_t_min): 'simt' runs those renders on the exact-fp32 engine's pair,
+    ops.exact_stash_render_call(t), at any rendering.num_points from 2 to 1024 whatever the renderer's engine, so that a truncated run can
+    be told apart from the tensor cores' rounding; None or 'tc' is the tensor-core pair above.  Any other value, the keyword without
+    train_t_min, or with frame_grad=True, is a ValueError."""
 
     def __init__(self, model, optimizer, cfg, device=None, optimizer_pose=None, pose_param_net=None,
                  optimizer_focal=None, focal_net=None, optimizer_distortion=None, distortion_net=None, **kwargs):
@@ -616,7 +620,18 @@ class Trainer(object):
                 raise ValueError("Trainer: frame_grad_t_min runs on the tensor-core pair only (not with frame_grad_engine='simt')")
             ops.frame_render_call(self.frame_grad_t_min)   # ValueError for a negative or NaN value
         self.train_t_min = kwargs.get('train_t_min', None)
-        if self.train_t_min is not None:
+        self.train_t_min_engine = kwargs.get('train_t_min_engine', None)
+        if self.train_t_min_engine not in (None, 'tc', 'simt'):
+            raise ValueError("Trainer: train_t_min_engine must be None, 'tc' or 'simt' (got %r)" % (self.train_t_min_engine,))
+        if self.train_t_min_engine is not None and self.train_t_min is None:
+            raise ValueError("Trainer: train_t_min_engine needs train_t_min")
+        if self.train_t_min_engine is not None and self.frame_grad:
+            raise ValueError("Trainer: train_t_min_engine is not taken with frame_grad=True")
+        if self.train_t_min is not None and self.train_t_min_engine == 'simt':
+            if not 2 <= int(model.renderer.cfg['num_points']) <= 1024:
+                raise ValueError("Trainer(train_t_min_engine='simt') needs rendering.num_points in 2..1024")
+            ops.exact_stash_render_call(self.train_t_min)   # ValueError for a negative or NaN value
+        elif self.train_t_min is not None:
             if self.frame_grad:
                 raise ValueError("Trainer: train_t_min is not taken with frame_grad=True (use frame_grad_t_min)")
             rend = model.renderer
@@ -629,8 +644,10 @@ class Trainer(object):
     # ------------------------------------------------------------------------------------
     def _train_render_call(self, backward):
         """the RenderCall class of a training render: the differentiable frame's pair (frame_grad), or the stash pair with early ray
-        termination (train_t_min), when it has a backward"""
+        termination (train_t_min, on the engine train_t_min_engine names), when it has a backward"""
         if backward and self.train_t_min is not None:
+            if self.train_t_min_engine == 'simt':
+                return ops.exact_stash_render_call(self.train_t_min)
             return ops.stash_render_call(self.train_t_min)
         if not (self.frame_grad and backward):
             return ops.RenderCall

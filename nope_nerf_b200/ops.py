@@ -93,6 +93,7 @@ class RenderCall:
     exact_frame = False   # ExactFrameRenderCall: that pair on the exact-fp32 engine
     t_min = None          # frame_render_call(t_min): that pair with early ray termination (the _tmin calls); None: without
     stash_tmin = False    # stash_render_call(t_min): the per-sample stash pair with early ray termination (nnb_render_fwd_tmin / _bwd_tmin)
+    exact_stash = False   # exact_stash_render_call(t_min): that pair on the exact-fp32 engine (the _tmin_engine calls on ENGINE_SIMT)
 
     def __init__(self, weights, c2w, cam, *, N, S, flags, engine, near, far, ray_idx=None, pixels=None, depth=None,
                  depth_map=None, scale=None, shift=None, noise=None, H=0, W=0, want_z_alpha=False, stash=False, hidden_dim=256):
@@ -100,7 +101,11 @@ class RenderCall:
         if self.stash_tmin:
             if want_z_alpha:
                 raise ValueError("stash_render_call: want_z_alpha is not supported (no per-sample outputs)")
-            if pick_engine(engine, S) != L.ENGINE_TC:
+            if self.exact_stash:
+                if not 2 <= S <= 1024:
+                    raise ValueError("exact_stash_render_call needs 2 <= S <= 1024 (got %d)" % S)
+                engine = L.ENGINE_SIMT
+            elif pick_engine(engine, S) != L.ENGINE_TC:
                 raise ValueError("stash_render_call runs on the tensor-core engine only (16 <= S <= 1024)")
             stash = True
         elif frame:
@@ -142,6 +147,8 @@ class RenderCall:
             nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes_engine(N, S, int(hidden_dim), engine)
         elif frame:
             nbytes = L.lib.nnb_render_frame_bwd_workspace_bytes(N, S, int(hidden_dim))
+        elif self.exact_stash:
+            nbytes = L.lib.nnb_render_tmin_workspace_bytes_engine(N, S, int(hidden_dim), engine)
         elif self.stash_tmin:
             nbytes = L.lib.nnb_render_tmin_workspace_bytes(N, S, int(hidden_dim))
         else:
@@ -158,7 +165,8 @@ class RenderCall:
             f.fwd = a
             self.n_eval = torch.empty(N, dtype=torch.int32, device=dev)
             f.t_min = self.t_min; f.n_eval = L.ptr(self.n_eval); f.t_final = None
-            name = "nnb_render_fwd_tmin" if self.stash_tmin else "nnb_render_frame_train_fwd_tmin"
+            name = ("nnb_render_fwd_tmin_engine" if self.exact_stash else "nnb_render_fwd_tmin") if self.stash_tmin \
+                else "nnb_render_frame_train_fwd_tmin"
             L.check(getattr(L.lib, name)(C.byref(f), _stream()), name)
         elif frame:
             L.check(L.lib.nnb_render_frame_train_fwd(C.byref(a), _stream()), "nnb_render_frame_train_fwd")
@@ -184,6 +192,8 @@ class RenderCall:
         b.g_scale_shift = L.ptr(g_scale_shift)
         if self.exact_frame:
             L.check(L.lib.nnb_render_frame_train_bwd_engine(C.byref(b), _stream()), "nnb_render_frame_train_bwd_engine")
+        elif self.exact_stash:
+            L.check(L.lib.nnb_render_bwd_tmin_engine(C.byref(b), _stream()), "nnb_render_bwd_tmin_engine")
         elif self.stash_tmin:
             L.check(L.lib.nnb_render_bwd_tmin(C.byref(b), _stream()), "nnb_render_bwd_tmin")
         elif self.frame and self.t_min is not None:
@@ -245,6 +255,28 @@ def stash_render_call(t_min):
     if cls is None:
         cls = type("StashRenderCall_tmin", (RenderCall,), {"t_min": t, "stash_tmin": True, "__doc__": stash_render_call.__doc__})
         _stash_tmin_calls[t] = cls
+    return cls
+
+
+_exact_stash_tmin_calls = {}
+
+
+def exact_stash_render_call(t_min):
+    """stash_render_call(t_min) on the exact-fp32 engine (nnb_render_fwd_tmin_engine / _bwd_tmin_engine on ENGINE_SIMT) at any S from 2 to
+    1024, whatever `engine` says (one class per value, cached), with RenderCall's arguments, outputs, pooling and backward() rules and
+    `n_eval`.  At S <= 32 (one round) its outputs and gradients are RenderCall(engine=ENGINE_SIMT, stash=True)'s bits and n_eval is S; at
+    t_min = 0 its outputs are RenderCall(engine=ENGINE_SIMT)'s and its pose, camera and scale-shift gradients ExactFrameRenderCall's at
+    every S; without jitter its outputs and n_eval are render_frame_engine(engine=ENGINE_SIMT, t_min=t_min)'s.  A negative or NaN t_min,
+    want_z_alpha, and S outside 2..1024 are a ValueError."""
+    t = float(t_min)
+    if not t >= 0.0:
+        raise ValueError("exact_stash_render_call: t_min must be >= 0 (got %r)" % (t_min,))
+    t = float(C.c_float(t).value)   # the value the library receives
+    cls = _exact_stash_tmin_calls.get(t)
+    if cls is None:
+        cls = type("ExactStashRenderCall_tmin", (RenderCall,), {"t_min": t, "stash_tmin": True, "exact_stash": True,
+                                                               "__doc__": exact_stash_render_call.__doc__})
+        _exact_stash_tmin_calls[t] = cls
     return cls
 
 

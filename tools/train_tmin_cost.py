@@ -8,7 +8,10 @@ One Trainer per configuration; graph steps alternated between them over --rounds
 4096 x 512, where two trainers' stashes do not fit in the card together, each configuration's rounds run alone in turn); the mean
 n_eval of the training render over --steps untimed steps after the timed rounds; the peak torch.cuda.max_memory_allocated over each
 Trainer's build and warm-up, above what was allocated before it.  The card's name and power limit are read in the same run
-(nvidia-smi query, read-only).  Writes one JSON line to stdout.  Without a CUDA device the tool fails."""
+(nvidia-smi query, read-only).  Writes one JSON line to stdout.  Without a CUDA device the tool fails.
+--engine simt measures the exact-fp32 engine instead (every render of the step on it, ops.set_default_engine('simt')): the default exact
+step against Trainer(train_t_min=t, train_t_min_engine='simt') (ops.exact_stash_render_call) and the same at t = 0, at the C2 step for
+D = 256 and 64 and at 1024 rays x 8 samples (D = 256), on the same two fields."""
 import argparse, gc, json, os, sys
 import numpy as np
 import torch
@@ -21,9 +24,13 @@ from field_query_cost import card  # noqa: E402
 from train_frame_cost import timed  # noqa: E402
 
 SIZES = ((1024, 128, 256), (4096, 512, 256), (1024, 128, 128), (1024, 128, 64))
+SIMT_SIZES = ((1024, 128, 256), (1024, 128, 64), (1024, 8, 256))
 
 
-def configs(t):
+def configs(t, engine="tc"):
+    if engine == "simt":
+        return {"default": {}, "stash_tmin": dict(train_t_min=t, train_t_min_engine="simt"),
+                "stash_t0": dict(train_t_min=0.0, train_t_min_engine="simt")}
     return {"default": {}, "frame_tmin": dict(frame_grad=True, frame_grad_t_min=t), "stash_tmin": dict(train_t_min=t),
             "stash_t0": dict(train_t_min=0.0)}
 
@@ -48,10 +55,10 @@ def build(N, S, D, field, dev, kw):
                        optimizer_distortion=torch.optim.Adam(dnet.parameters(), lr=5e-4), distortion_net=dnet, **kw)
 
 
-def run(N, S, D, field, frames, t, rounds, steps, dev, keys):
+def run(N, S, D, field, frames, t, rounds, steps, dev, keys, engine="tc"):
     trainers, peak, calls = {}, {}, {}
     step = lambda tr, i: tr.train_step(frames[i % len(frames)], it=i, epoch=0, scheduling_start=10000, render_path=None)
-    for key, kw in configs(t).items():
+    for key, kw in configs(t, engine).items():
         if key not in keys:
             continue
         torch.cuda.synchronize()
@@ -97,21 +104,27 @@ def main():
     ap.add_argument("--steps", type=int, default=20, help="graph steps per timed round")
     ap.add_argument("--t-min", type=float, default=1e-4)
     ap.add_argument("--sizes", default="all", help="'all' or 'c2' (the C2 step at D = 256 only)")
+    ap.add_argument("--engine", default="tc", choices=("tc", "simt"))
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("train_tmin_cost.py needs a CUDA device")
     import bench
+    from nope_nerf_b200 import ops
+    if args.engine == "simt":
+        ops.set_default_engine("simt")
     dev = torch.device("cuda")
     name, limit = card()
     _, frames = bench.synth_frames(bench.H, bench.W, bench.HD, bench.WD, 4, bench.V, dev, with_ref=False)
-    out = dict(card=name, power_limit=limit, t_min=args.t_min, rounds=args.rounds, steps=args.steps, results=[])
-    for N, S, D in (SIZES if args.sizes == "all" else SIZES[:1]):
+    out = dict(card=name, power_limit=limit, engine=args.engine, t_min=args.t_min, rounds=args.rounds, steps=args.steps, results=[])
+    sizes = SIMT_SIZES if args.engine == "simt" else SIZES
+    for N, S, D in (sizes if args.sizes == "all" else sizes[:1]):
         for field in ("bench", "surface"):
             # the stash of two 4096 x 512 trainers does not fit in 80 GB together: there each configuration runs alone, not alternated
-            groups = [list(configs(0.0))] if N * S <= 1024 * 128 else [[k] for k in configs(0.0)]
+            groups = [list(configs(0.0, args.engine))] if N * S <= 1024 * 128 else [[k] for k in configs(0.0, args.engine)]
             ms, peak, n_eval = {}, {}, {}
             for keys in groups:
-                for d, r in zip((ms, peak, n_eval), run(N, S, D, field, frames, args.t_min, args.rounds, args.steps, dev, keys)):
+                res = run(N, S, D, field, frames, args.t_min, args.rounds, args.steps, dev, keys, args.engine)
+                for d, r in zip((ms, peak, n_eval), res):
                     d.update(r)
                 release()
             row = dict(N=N, S=S, D=D, field=field, ms=ms, peak_mb={k: v / 2 ** 20 for k, v in peak.items()}, mean_n_eval=n_eval)
